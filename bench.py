@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- X-UNet DDPM training throughput (BASELINE.json metric: train images/sec) on N B200s.
+"""bench.py -- X-UNet DDPM training throughput (BASELINE.json metric: train images/sec) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload small64|small128|full128|full64]
-                    [--batch B] [--dtype bf16|fp32] [--no-full128] [--sampler-steps 256]
+                    [--batch B] [--dtype bf16|fp32] [--no-full128] [--sampler-steps 256] [--dump-outputs DIR]
 
 One "step" = one optimisation step (pinned H2D staging -> forward -> backward -> [bucketed NCCL all-reduce, overlapped
 with the backward] -> Adam) on a synthetic SRN-shaped batch of B (source,target) pairs PER GPU (weak scaling).
@@ -17,10 +17,14 @@ Printed JSON (rank 0, one line):
   cpu_baseline : the CPU oracle (restatement of the JAX reference; JAX is not installable here) on the host cores: thread
              sweep, best thread count, train step (config B) and the single eps-forward of BASELINE configs[0]
   full128  : BASELINE configs[2]/[3] in the SAME line at every N: full 3DiM X-UNet (439 M parameters) at 128x128, per-GPU
-             batch 4: ms/step, images/s, step TFLOP/s and fraction of the sustained tensor peak, and at N>1 the measured
+             batch 4, max(3, min(--steps, --full-steps)) timed steps: ms/step, images/s, step TFLOP/s and fraction of the sustained tensor peak, and at N>1 the measured
              all-reduce time of the 1.755 GB gradient bucket and how much of it the backward hides; at N=1 also the
              256-step CFG sampler of the full model at 128x128 (views/s at 1 view and at 4 views in flight)
 --impl reference times the CPU oracle alone with the same metric/unit/config (rank 0 only).
+--dump-outputs DIR writes what the last timed device-resident step computed (loss, updated parameters, gradients; float32
+.npy, a fixed seeded sample of at most 4 M elements per array) so that two builds can be compared output for output: the
+inputs, the initial parameters and the dropout seeds are the same in every run with the same arguments, and the step's
+reductions do not depend on execution order, so the outputs are the same bits as well.
 """
 from __future__ import annotations
 
@@ -64,7 +68,8 @@ def load_peaks():
         p = json.load(open(path))
         return dict(hbm=p['hbm_gbs'], tf_burst=p['bf16_tflops'], tf_sustained=p.get('bf16_tflops_sustained', p['bf16_tflops']),
                     source='measured')
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source='fallback')
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- a ceiling, not a measured rate
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, source='H100 SXM data sheet')
 
 
 class ClockSampler:
@@ -315,13 +320,13 @@ def time_kernel(fn, iters=30, warm=5):
 
 def dominant_kernel_roofline(P, model, B, S, peaks):
     """Times the step's heaviest kernels ALONE (CUDA events on the launching stream, >=3 warm-ups) through the operator-level
-    C-ABI at the exact shapes and with the exact implementations (tcgen05) the step uses, and returns the roofline of the
+    C-ABI at the exact shapes and with the exact implementations (wgmma) the step uses, and returns the roofline of the
     one with the largest share of the step.  Algorithmic FLOPs per launch are SURVEY 8(d)'s (2*MAC; backward := 2 x forward)."""
     import torch
     from novel_view_synthesis_3d_b200 import _lib
     lib = _lib.load()
     os.environ['XUNET_OP_CACHE_SHADOW'] = '1'     # time the conv kernel alone (the step converts weights once per forward)
-    os.environ.pop('XUNET_OP_ATTN_FOLD', None)    # attention backward as the engine runs it: prep + fused dK/dV/dQ + store (hd <= 32)
+    os.environ.pop('XUNET_OP_ATTN_FOLD', None)    # attention backward as the engine runs it: prep + dK/dV/dQ + store
     cfg = model.config
     tc = cfg.dtype == 'bf16'
     dt = _lib.DTYPE_BF16 if tc else _lib.DTYPE_F32
@@ -340,10 +345,10 @@ def dominant_kernel_roofline(P, model, B, S, peaks):
         flops = 2.0 * N * H * H * 9 * Ci * Co
         fn = lambda: lib.xunet_op_conv(dt, impl, x.data_ptr(), w.data_ptr(), b.data_ptr(), None, y.data_ptr(), N, H, H, Ci, Co, 3, 1, 1, 1.0, st)
         assert fn() == 0, lib.xunet_last_error()
-        out.append(dict(kernel=f'conv3x3 fwd {Ci}->{Co} @{H} ({"tcgen05" if tc else "simt"})', seconds=time_kernel(fn), flops=flops, count=count))
+        out.append(dict(kernel=f'conv3x3 fwd {Ci}->{Co} @{H} ({"wgmma" if tc else "simt"})', seconds=time_kernel(fn), flops=flops, count=count))
         fw = lambda: lib.xunet_op_conv_wgrad(dt, impl, x.data_ptr(), y.data_ptr(), dw.data_ptr(), b.data_ptr(), N, H, H, Ci, Co, 3, 1, 1, 1.0, st)
         assert fw() == 0, lib.xunet_last_error()
-        out.append(dict(kernel=f'conv3x3 wgrad {Ci}->{Co} @{H} ({"tcgen05" if tc else "simt"})', seconds=time_kernel(fw), flops=flops, count=count))
+        out.append(dict(kernel=f'conv3x3 wgrad {Ci}->{Co} @{H} ({"wgmma" if tc else "simt"})', seconds=time_kernel(fw), flops=flops, count=count))
 
     def attn_case(Lq, C, heads, count):
         qkv = torch.randn(N, Lq, 3 * C, device=dev).to(tdt)
@@ -360,7 +365,7 @@ def dominant_kernel_roofline(P, model, B, S, peaks):
                                                 dscr.data_ptr(), dqkv.data_ptr(), N, Lq, C, heads, 0, st)
         assert fb() == 0, lib.xunet_last_error()
         # algorithmic backward work = 5 GEMMs (S, dP, dV, dK, dQ) = 2.5x the forward's two
-        bname = 'attention bwd (prep + fused dK/dV/dQ + store)' if C // heads <= 32 else 'attention bwd (dQ + dK/dV)'
+        bname = 'attention bwd (prep + dK/dV/dQ + store)'
         out.append(dict(kernel=f'{bname} L={Lq} hd={C // heads}', seconds=time_kernel(fb), flops=2.5 * flops, count=count))
 
     feat = [cfg.ch * m for m in cfg.ch_mult]
@@ -372,12 +377,8 @@ def dominant_kernel_roofline(P, model, B, S, peaks):
     top = max(out, key=lambda r: r['seconds'] * r['count'])
     peak = peaks['tf_burst']
     achieved = top['flops'] / top['seconds'] / 1e12
-    traffic = None
-    tpath = os.path.join(ROOT, 'profiles', 'roofline_traffic.json')   # dram bytes/launch from the committed ncu --set full capture
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath)).get(top['kernel'])
     return {'bound': 'tensor', 'kernel': top['kernel'], 'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s',
-            'frac': achieved / peak, 'traffic': traffic, 'peak_source': peaks['source'] + ' (burst, kernel timed alone)',
+            'frac': achieved / peak, 'peak_source': peaks['source'] + ' (burst, kernel timed alone)',
             'per_launch_us': top['seconds'] * 1e6, 'algorithmic_flops_per_launch': top['flops'],
             'candidates': [{'kernel': r['kernel'], 'us': r['seconds'] * 1e6, 'tflops': r['flops'] / r['seconds'] / 1e12,
                             'launches_per_step': r['count']} for r in out]}
@@ -421,12 +422,35 @@ class TrainBench:
 
     def dev_step(self, i, step=None):
         b, nz = self.devb[i % self.n_host]
-        (step or self.step)(b, nz, cond_mask=self.dmasks[i % self.n_host])
+        return (step or self.step)(b, nz, cond_mask=self.dmasks[i % self.n_host])
 
     def run_device(self, warmup, K, step=None):
+        """K timed steps after `warmup` untimed ones; self.last_loss = the loss tensor of the last timed step"""
         for i in range(warmup):
             self.dev_step(i, step)
-        return self.timed(lambda i: self.dev_step(i, step), K)
+        last = {}
+
+        def one(i):
+            last['loss'] = self.dev_step(i, step)
+
+        t = self.timed(one, K)
+        self.last_loss = last.get('loss')
+        return t
+
+    def outputs(self, max_elems=1 << 22):
+        """What a caller of the step holds after the last run_device step: its loss, the updated parameters and the gradients
+        (float32 numpy; arrays above max_elems as a fixed seeded sample of max_elems elements)"""
+        torch = self.torch
+
+        def sample(t):
+            t = t.detach().reshape(-1).float()
+            if t.numel() > max_elems:
+                g = torch.Generator().manual_seed(0)
+                idx = torch.randint(0, t.numel(), (max_elems,), generator=g).sort().values
+                t = t[idx.to(t.device)]
+            return t.cpu().numpy()
+        return {'loss': self.last_loss.detach().float().cpu().numpy(), 'params': sample(self.state.params.flat),
+                'grads': sample(self.eng.grads)}
 
     def run_e2e(self, K):
         """host numpy inputs through the public API; the loss of every step is read back device->host inside the timed
@@ -540,9 +564,14 @@ def main():
     ap.add_argument('--sampler-steps', type=int, default=256, help='extra: DDPM sampler views/s at N=1 (0 = skip)')
     ap.add_argument('--no-full128', action='store_true', help='skip the full-3DiM 128x128 sub-record')
     ap.add_argument('--full-batch', type=int, default=0, help='per-GPU batch of the full128 sub-record (default 4)')
-    ap.add_argument('--full-steps', type=int, default=8, help='timed steps of the full128 sub-record (<= --steps)')
+    ap.add_argument('--full-steps', type=int, default=8,
+                    help='the full128 sub-record times max(3, min(--steps, --full-steps)) steps after 3 warm-up steps')
     ap.add_argument('--ref-budget-s', type=float, default=200.0, help='wall-clock budget of --impl reference')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step as DIR/<name>.npy (loss, params, grads)')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     preset, S, B0, fwd_flops = WORKLOADS[args.workload]
     B = args.batch or B0
     if args.impl == 'reference':
@@ -569,6 +598,10 @@ def main():
     # ---- value: inputs resident in HBM; e2e: host numpy inputs through the public API, loss read back every step -------
     t_dev = tb.run_device(args.warmup, args.steps)
     progress(f'{args.workload}: {t_dev / args.steps * 1e3:.3f} ms/step device-resident; timing end-to-end')
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in tb.outputs().items():
+            np.save(os.path.join(args.dump_outputs, f'{name}.npy'), arr)
     t_e2e, h2d, losses = tb.run_e2e(args.steps)
     clk = clocks.stop() if rank == 0 else None
     progress(f'{args.workload}: e2e {t_e2e / args.steps * 1e3:.3f} ms/step; kernel counts + roofline candidates')
@@ -608,7 +641,7 @@ def main():
             'config': {'workload': args.workload, 'model': preset, 'side': S, 'per_gpu_batch': B, 'global_batch': B * world,
                        'parallelism': f'dp{world}', 'optimizer': 'adam lr1e-4', 'loss': 'frobenius (train.py:67)',
                        'cuda_graph': not args.no_graph, 'step_mode': mode,
-                       'l2': 'no explicit flush: one step touches ~%.1f GB of activations+grads (>> 126 MB L2) and rotates over %d '
+                       'l2': 'no explicit flush: one step touches ~%.1f GB of activations+grads (>> 50 MB L2) and rotates over %d '
                              'different input batches' % (ws_gb, 4)},
             'e2e': {'value': imgs / t_e2e, 'unit': UNIT, 'h2d_bytes_per_step': int(h2d), 'd2h_bytes_per_step': 4,
                     'ms_per_step': t_e2e / args.steps * 1e3},

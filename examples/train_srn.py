@@ -1,4 +1,4 @@
-"""train.py look-alike on the B200 path (reference: train.py:78-176).  Differences from the reference script: imports,
+"""train.py look-alike on the CUDA path (reference: train.py:78-176).  Differences from the reference script: imports,
 a sharded batch under torchrun, device-side forward diffusion, and a Flax-format checkpoint every `save_every` steps.
 
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 1000

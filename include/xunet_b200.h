@@ -1,4 +1,4 @@
-/* xunet_b200.h -- C-ABI of libxunet_b200.so: the B200 (sm_100a) X-UNet hot path.
+/* xunet_b200.h -- C-ABI of libxunet_b200.so: the H100 (sm_90a) X-UNet hot path.
  *
  * The reference (shiveshkhaitan/novel_view_synthesis_3d) has no FFI/plugin layer: its boundary is the
  * Flax functional API used by train.py / sampling.py.  Each entry point below names the reference

@@ -1,5 +1,5 @@
 """novel_view_synthesis_3d_b200 -- the X-UNet pose-conditional denoiser hot path of
-shiveshkhaitan/novel_view_synthesis_3d, rebuilt B200-native (hand-written sm_100a CUDA behind a C-ABI)."""
+shiveshkhaitan/novel_view_synthesis_3d, rebuilt H100-native (hand-written sm_90a CUDA behind a C-ABI)."""
 from .xunet import XUNet, XUNetConfig, SMALL, FULL_3DIM, ParamTree, Engine
 from .train import (TrainState, Adam, AdamState, create_train_state, create_sample_data, apply_model, update_model,
                     TrainStep)

@@ -1,19 +1,39 @@
-// attn_tc.cu -- tcgen05/TMEM/TMA flash attention over frames (bf16 operands, fp32 softmax state and accumulators).
+// attn_tc.cu -- wgmma / TMA flash attention over frames for sm_90a (bf16 operands, fp32 softmax state and accumulators).
 //
 // Replaces nn.dot_product_attention (model/xunet.py:103: two einsums + a materialised (B,h,L,L) fp32 score tensor) and
 // the AttnBlock residual (model/xunet.py:127) for BOTH attention flavours: kv_frame = frame ^ cross (model/xunet.py:114-121).
 //
-// One CTA = one (frame n, head h, 128-query tile).  Per 128-key block j:
-//   MMA warp    : S_j[128q,128k] = Q K_j^T            (tcgen05.mma, A,B K-major from TMA-swizzled smem, D in TMEM)
-//   softmax warps (one thread per query row = one TMEM lane): tcgen05.ld S_j, running max / sum in registers,
-//                 P_j = exp2(...) -> bf16 -> shared memory in the K-major 128B-swizzled UMMA layout
-//   MMA warp    : Oblk[128q,hd] = P_j V_j             (A = P_j from smem, B = V_j MN-major straight from the TMA box)
-//   softmax warps: tcgen05.ld Oblk, O = O * corr + Oblk in registers (no TMEM-side rescale needed)
+// Forward: one CTA = one (frame n, head h, 64-query tile) = one consumer warpgroup + one TMA producer warp.  Per 64-key block j:
+//   S_j[64q,64k] = Q K_j^T            (wgmma, Q and K_j K-major from TMA-swizzled smem, fp32 accumulators in registers)
+//   online softmax on the accumulator fragment (a row lives in the 4 lanes of a quad), P_j -> bf16 A-operand registers
+//   O = O * corr + P_j V_j            (wgmma with A from registers, B = V_j MN-major straight from the TMA box)
 // Epilogue: out = (O / l + residual) / sqrt(2), lse = m + log(l) for the backward.
+// Backward (FlashAttention-2 order): one CTA = one (query frame n, head h, 64-key tile); it streams the 64-query blocks of the
+// frame and accumulates dK, dV in registers; the dQ contributions of its keys are summed in an fp64 buffer (xu_det_scratch),
+// so the result does not depend on the order in which the key tiles finish.  attn_bwd_prep_kernel forms D = rowsum(dO * O),
+// attn_bwd_dq_store_kernel rounds dQ to bf16 and re-zeroes the fp64 buffer.
 #include "kernels.h"
 #include "tc_common.cuh"
 
 namespace {
+
+constexpr int kBlk = 64;          // queries per forward CTA, keys per backward CTA, keys / queries per streamed block
+constexpr int kAttnThreads = 160; // one consumer warpgroup + one producer warp
+
+__host__ __device__ constexpr int attn_cw(int hd) { return hd < 64 ? hd : 64; }     // channel chunk = one swizzle span
+__host__ __device__ constexpr int attn_stages(int hd) { return hd <= 32 ? 4 : 2; }
+
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+// accumulator fragment of a 64 x 64 tile (32 floats) -> the four 16-column A-operand slices of the next wgmma
+__device__ __forceinline__ void frag_to_a(const float (&x)[32], uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) a[kk][q] = pack_bf16(x[8 * kk + 2 * q], x[8 * kk + 2 * q + 1]);
+}
 
 struct AttnTcParams {
   const bf16* res;
@@ -21,957 +41,326 @@ struct AttnTcParams {
   float* lse;
   int L, C, heads, cross;
   float scale_log2;   // log2(e) / sqrt(hd)
-  float* cstats;      // optional: per-(sample, channel) [sum, sumsq] of the stored output (N/2, C, 2) -- the next GroupNorm's statistics
+  double* cstats;     // optional: per-(sample, channel) [sum, sumsq] of the stored output (N/2, C, 2) -- the next GroupNorm's statistics,
+                      // accumulated in fp64 (xu_det_scratch) and folded into the caller's fp32 buffer after the kernel
 };
 
-constexpr int kQT = 128;   // queries per CTA (UMMA M)
-constexpr int kKB = 64;    // keys per block (UMMA N of the score GEMM, K of the PV GEMM)
-
-// Software pipeline (per 64-key block j):   MMA lane: S_{j+1} = Q K_{j+1}^T is issued while the softmax warps still work
-// on S_j (two S buffers in TMEM); PV_j is issued as soon as P_j is in shared memory (two P buffers).  Softmax threads read
-// the PV_{j-1} result one block late, so the tensor-core round trip is hidden behind the exponentials of block j.
-// key/value ring depth: a 64-key block of head_dim <= 32 is 2-4 KB and is consumed faster than a TMA load returns -> 6 stages there
-__host__ __device__ constexpr int fwd_kv_stages(int hd) { return hd <= 32 ? 6 : 3; }
 template <int HD>
-__global__ void __launch_bounds__(192) attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ128,
-                                                          const __grid_constant__ CUtensorMap tmKV64, const AttnTcParams p) {
-  constexpr int CW = HD < 64 ? HD : 64;       // channel-chunk width = one swizzle span
+__global__ void __launch_bounds__(kAttnThreads) attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnTcParams p) {
+  constexpr int CW = attn_cw(HD);
   constexpr int NCH = HD / CW;
-  constexpr int TILE = 128 * CW * 2;          // Q sub-tile  [128 rows][CW]
-  constexpr int TILE_B = kKB * CW * 2;        // K / V sub-tile [64 rows][CW]
-  constexpr int KV_STAGES = fwd_kv_stages(HD);
-  constexpr int P_BYTES = 128 * kKB * 2;      // one P buffer: [128 q][64 keys] bf16, 128B-swizzled
-  // two S buffers (S_{j+1} overlaps softmax_j inside the CTA) + O = 256 TMEM columns -> 2 CTAs per SM.  (Measured alternative:
-  // one S buffer in 128 columns with 3 CTAs/SM was 8 % slower at head_dim 16.)
-  constexpr int S_BUFS = 2;
-  constexpr uint32_t TMEM_COLS = 256;
-  constexpr int O_COL = S_BUFS * kKB;
+  constexpr int TILE = kBlk * CW * 2;         // [64 rows][CW] bf16
+  constexpr int ST = attn_stages(HD);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smQ = base;                                   // NCH * TILE
-  uint8_t* smK = smQ + NCH * TILE;                       // KV_STAGES * NCH * TILE_B
-  uint8_t* smV = smK + KV_STAGES * NCH * TILE_B;
-  uint8_t* smP = smV + KV_STAGES * NCH * TILE_B;         // 2 * P_BYTES
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smP + 2 * P_BYTES);
-  uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;                          // [KV_STAGES]
-  uint64_t* kv_empty = kv_full + KV_STAGES;              // [KV_STAGES]
-  uint64_t* s_full = kv_empty + KV_STAGES;               // [2]
-  uint64_t* p_full = s_full + 2;                         // [2]
-  uint64_t* o_full = p_full + 2;
-  uint64_t* o_free = o_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_free + 1);
+  uint8_t* smQ = base;
+  uint8_t* smK = smQ + NCH * TILE;            // ST x NCH tiles
+  uint8_t* smV = smK + ST * NCH * TILE;
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(smV + ST * NCH * TILE);
+  uint64_t* kv_full = q_full + 1;
+  uint64_t* kv_empty = kv_full + ST;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * kQT, h = blockIdx.y, n = blockIdx.z;
+  const int q0 = blockIdx.x * kBlk, h = blockIdx.y, n = blockIdx.z;
   const int nkv = p.cross ? (n ^ 1) : n;
-  const int nkb = p.L / kKB;
-
+  const int nkb = p.L / kBlk;
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < KV_STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&s_full[s], 1); mbar_init(&p_full[s], 128); }
-    mbar_init(o_full, 1);
-    mbar_init(o_free, 128);
+    for (int s = 0; s < ST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQ128) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmKV64) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQKV) : "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  xu_grid_dep_sync();     // PDL: everything above (barriers, TMEM) overlaps the previous kernel's tail
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_O = tmem_base + O_COL;
+  xu_grid_dep_sync();
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
-      // ===== TMA producer: Q once, then K_j / V_j blocks through a 3-deep ring =====
       mbar_expect_tx(q_full, NCH * TILE);
-      for (int c = 0; c < NCH; ++c) tma_load_3d(smQ + c * TILE, &tmQ128, q_full, h * HD + c * CW, q0, n);
+      for (int c = 0; c < NCH; ++c) tma_load_3d(smQ + c * TILE, &tmQKV, q_full, h * HD + c * CW, q0, n);
       for (int j = 0; j < nkb; ++j) {
-        const int s = j % KV_STAGES;
-        mbar_wait(&kv_empty[s], ((j / KV_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&kv_full[s], 2 * NCH * TILE_B);
+        const int s = j % ST;
+        mbar_wait(&kv_empty[s], ((j / ST) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[s], 2 * NCH * TILE);
         for (int c = 0; c < NCH; ++c) {
-          tma_load_3d(smK + (s * NCH + c) * TILE_B, &tmKV64, &kv_full[s], p.C + h * HD + c * CW, j * kKB, nkv);
-          tma_load_3d(smV + (s * NCH + c) * TILE_B, &tmKV64, &kv_full[s], 2 * p.C + h * HD + c * CW, j * kKB, nkv);
+          tma_load_3d(smK + (s * NCH + c) * TILE, &tmQKV, &kv_full[s], p.C + h * HD + c * CW, j * kBlk, nkv);
+          tma_load_3d(smV + (s * NCH + c) * TILE, &tmQKV, &kv_full[s], 2 * p.C + h * HD + c * CW, j * kBlk, nkv);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc_s = make_idesc_bf16(kKB, 0, 0);     // S = Q K^T : both operands K-major (hd contiguous)
-      const uint32_t idesc_o = make_idesc_bf16(HD, 0, 1);      // O = P V   : B = V is MN-major (hd contiguous)
-      auto issue_s = [&](int j) {
-        const int s = j % KV_STAGES;
-        mbar_wait(&kv_full[s], (j / KV_STAGES) & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int c = 0; c < NCH; ++c)
-#pragma unroll
-          for (int k = 0; k < CW / 16; ++k)
-            umma_bf16(tmem_base + (j % S_BUFS) * kKB, make_kmajor_desc<CW>(smem_u32(smQ + c * TILE) + k * 32),
-                      make_kmajor_desc<CW>(smem_u32(smK + (s * NCH + c) * TILE_B) + k * 32), idesc_s, (c > 0 || k > 0) ? 1u : 0u);
-        umma_commit(&s_full[j & 1]);
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      for (int j = 0; j < nkb; ++j) {
-        const int s = j % KV_STAGES;
-        // two buffers: S buffer (j+1)&1 was last read for block j-1, whose p_full this thread has already waited on
-        if (S_BUFS == 2 && j + 1 < nkb) issue_s(j + 1);
-        mbar_wait(&p_full[j & 1], (j >> 1) & 1);
-        if (S_BUFS == 1 && j + 1 < nkb) issue_s(j + 1);   // single buffer: free once softmax_j has read it
-        if (j > 0) mbar_wait(o_free, (j - 1) & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < kKB / 16; ++kk) {
-          const uint64_t dp = make_kmajor_desc<64>(smem_u32(smP + (j & 1) * P_BYTES) + kk * 32);
-          const uint64_t dv = make_mnmajor_desc<CW>(smem_u32(smV + s * NCH * TILE_B) + kk * 16 * (CW * 2), TILE_B);
-          umma_bf16(tmem_O, dp, dv, idesc_o, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(o_full);
-        umma_commit(&kv_empty[s]);
-      }
-    }
-  } else {
-    // ===== softmax + accumulate: thread <-> query row <-> TMEM lane =====
-    const int lane_base = (warp & 3) * 32;
-    const int r = lane_base + lane;
-    const uint32_t lane_addr = (uint32_t)lane_base << 16;
-    float m = -INFINITY, l = 0.f, corr_prev = 0.f;
-    float acc[HD];
-#pragma unroll
-    for (int i = 0; i < HD; ++i) acc[i] = 0.f;
-    const uint32_t prow_off = (r >> 3) * 1024 + (r & 7) * 128;
-    auto absorb_o = [&](int jj, float corr) {   // acc = acc * corr + O_blk(jj)
-      mbar_wait(o_full, jj & 1);
-      tcgen05_fence_after();
-#pragma unroll
-      for (int c0 = 0; c0 < HD; c0 += 16) {
-        uint32_t v[16];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(tmem_O + lane_addr + c0));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[c0 + i] = fmaf(acc[c0 + i], corr, __uint_as_float(v[i]));
-      }
-      tcgen05_fence_before();
-      mbar_arrive(o_free);
-    };
-    for (int j = 0; j < nkb; ++j) {
-      mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-      tcgen05_fence_after();
-      uint32_t v[2][32];
-      tmem_ld32_nowait(tmem_base + (j % S_BUFS) * kKB + lane_addr, v[0]);
-      tmem_ld32_nowait(tmem_base + (j % S_BUFS) * kKB + lane_addr + 32, v[1]);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      // four independent max chains (and four row-sum accumulators below): with two softmax warps per scheduler a
-      // 32-deep dependent chain is exposed latency
-      float mq[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 32; i += 4)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) mq[c] = fmaxf(mq[c], fmaxf(__uint_as_float(v[0][i + c]), __uint_as_float(v[1][i + c])));
-      const float mraw = fmaxf(fmaxf(mq[0], mq[1]), fmaxf(mq[2], mq[3]));
-      const float mx = fmaxf(m, mraw * p.scale_log2);      // scale > 0: max commutes with the scaling
-      const float corr = ex2_approx(m - mx);               // m = -inf on the first block -> 0
-      float rsq[4] = {0.f, 0.f, 0.f, 0.f};
-      uint8_t* prow = smP + (j & 1) * P_BYTES + prow_off;  // free: PV_{j-2} completed (absorbed in iteration j-1)
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 pk;
-          uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float p0 = ex2_approx(fmaf(__uint_as_float(v[hh][g * 8 + 2 * q]), p.scale_log2, -mx));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(v[hh][g * 8 + 2 * q + 1]), p.scale_log2, -mx));
-            rsq[q] += p0 + p1;
-            __nv_bfloat162 b2 = __floats2bfloat162_rn(p0, p1);
-            pw[q] = *reinterpret_cast<uint32_t*>(&b2);
-          }
-          const int chunk = hh * 4 + g;
-          sts128(prow + ((chunk ^ (r & 7)) << 4), pk);
-        }
-      l = l * corr + ((rsq[0] + rsq[1]) + (rsq[2] + rsq[3]));
-      m = mx;
-      fence_async_smem();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tcgen05_fence_before();
-      mbar_arrive(&p_full[j & 1]);
-      if (j > 0) absorb_o(j - 1, corr_prev);   // one block late: PV_{j-1} ran while this thread did the exponentials above
-      corr_prev = corr;
-    }
-    absorb_o(nkb - 1, corr_prev);
-    // epilogue: (O / l + residual) / sqrt2
-    const float inv = 1.f / l;
-    const long long o = ((long long)n * p.L + q0 + r) * p.C + h * HD;
-    float* cs_row = p.cstats ? p.cstats + ((long long)(n >> 1) * p.C + h * HD) * 2 : nullptr;   // both frames of a sample pool
-    float sx[32];
-#pragma unroll
-    for (int c0 = 0; c0 < HD; c0 += 8) {
-      uint4 rv = *reinterpret_cast<const uint4*>(p.res + o + c0);
-      const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rv);
-      uint4 ov;
-      __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&ov);
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        o2[q] = __floats2bfloat162_rn((acc[c0 + 2 * q] * inv + __low2float(r2[q])) * XU_RSQRT2,
-                                      (acc[c0 + 2 * q + 1] * inv + __high2float(r2[q])) * XU_RSQRT2);
-      *reinterpret_cast<uint4*>(p.out + o + c0) = ov;
-      if (cs_row != nullptr) {     // statistics of the rounded, stored values (CTA-uniform branch)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float a = __low2float(o2[q]), b = __high2float(o2[q]);
-          sx[(c0 & 8) + 2 * q] = a;            sx[(c0 & 8) + 2 * q + 1] = b;
-          sx[16 + (c0 & 8) + 2 * q] = a * a;   sx[16 + (c0 & 8) + 2 * q + 1] = b * b;
-        }
-        if (c0 & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 - 8) * 2);
-      }
-    }
-    // natural-log LSE of the scaled scores (what the backward kernels expect): m is in log2 units
-    p.lse[((long long)n * p.heads + h) * p.L + q0 + r] = m * 0.69314718055994530942f + __logf(l);
+    return;
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  // ===== consumer warpgroup: thread rows 16 warp + g and + 8 (g = lane / 4), columns 8 i + 2 t (+1) =====
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};     // m in log2 units; l = this thread's partial row sums
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nkb; ++j) {
+    const int s = j % ST;
+    mbar_wait(&kv_full[s], (j / ST) & 1);
+    float sc[32];
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int kk = 0; kk < CW / 16; ++kk)
+        Wgmma<64>::template ss<0, 0>(sc, make_kmajor_desc<CW>(smem_u32(smQ + c * TILE) + kk * 32),
+                                     make_kmajor_desc<CW>(smem_u32(smK + (s * NCH + c) * TILE) + kk * 32), (c > 0 || kk > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    float corr[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hh], sc[4 * i + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mn = fmaxf(m[hh], mx * p.scale_log2);      // scale > 0: max commutes with the scaling
+      corr[hh] = ex2_approx(m[hh] - mn);                      // m = -inf on the first block -> 0
+      m[hh] = mn;
+      float rs = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float pv = ex2_approx(fmaf(sc[4 * i + 2 * hh + e], p.scale_log2, -mn));
+          sc[4 * i + 2 * hh + e] = pv;
+          rs += pv;
+        }
+      l[hh] = l[hh] * corr[hh] + rs;
+    }
+#pragma unroll
+    for (int i = 0; i < HD / 8; ++i) {
+      o[4 * i] *= corr[0]; o[4 * i + 1] *= corr[0];
+      o[4 * i + 2] *= corr[1]; o[4 * i + 3] *= corr[1];
+    }
+    uint32_t pa[4][4];
+    frag_to_a(sc, pa);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      Wgmma<HD>::template rs<1>(o, pa[kk], make_mnmajor_desc<CW>(smem_u32(smV + s * NCH * TILE) + kk * 16 * (CW * 2), TILE), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
+  }
+  // epilogue: (O / l + residual) / sqrt2
+  float inv[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    inv[hh] = 1.f / l[hh];
+  }
+  const int g = lane >> 2, t = lane & 3;
+  const long long row0 = (long long)n * p.L + q0 + 16 * warp + g;
+  double* cs_row = p.cstats ? p.cstats + ((long long)(n >> 1) * p.C + h * HD) * 2 : nullptr;   // both frames of a sample pool
+#pragma unroll
+  for (int i = 0; i < HD / 8; ++i) {
+    const int col = 8 * i + 2 * t;
+    float sum0 = 0.f, sum1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const long long off = (row0 + 8 * hh) * p.C + h * HD + col;
+      const __nv_bfloat162 r2 = *reinterpret_cast<const __nv_bfloat162*>(p.res + off);
+      const __nv_bfloat162 o2 = __floats2bfloat162_rn((o[4 * i + 2 * hh] * inv[hh] + __low2float(r2)) * XU_RSQRT2,
+                                                      (o[4 * i + 2 * hh + 1] * inv[hh] + __high2float(r2)) * XU_RSQRT2);
+      *reinterpret_cast<__nv_bfloat162*>(p.out + off) = o2;
+      const float a = __low2float(o2), b = __high2float(o2);   // statistics of the rounded, stored values
+      sum0 += a; sum1 += b; sq0 += a * a; sq1 += b * b;
+    }
+    if (cs_row != nullptr) {     // CTA-uniform branch: reduce over the 8 row groups of the warp, one red per channel and warp
+#pragma unroll
+      for (int sh = 4; sh < 32; sh <<= 1) {
+        sum0 += __shfl_xor_sync(0xffffffffu, sum0, sh); sum1 += __shfl_xor_sync(0xffffffffu, sum1, sh);
+        sq0 += __shfl_xor_sync(0xffffffffu, sq0, sh); sq1 += __shfl_xor_sync(0xffffffffu, sq1, sh);
+      }
+      if (g == 0) {
+        xu_det_add(cs_row + col * 2, sum0); xu_det_add(cs_row + col * 2 + 1, sq0);
+        xu_det_add(cs_row + col * 2 + 2, sum1); xu_det_add(cs_row + col * 2 + 3, sq1);
+      }
+    }
+  }
+  // natural-log LSE of the scaled scores (what the backward expects): m is in log2 units
+  if (t == 0) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+      p.lse[((long long)n * p.heads + h) * p.L + q0 + 16 * warp + g + 8 * hh] = m[hh] * 0.69314718055994530942f + __logf(l[hh]);
   }
 }
 
 // ================================================================================================================
 // backward.  dO = dout / sqrt2 (the AttnBlock residual scale), D = rowsum(dO * O), P = exp(S*scale - lse),
-// dS = P * (dP - D) * scale.  Two kernels (no atomics): dQ per query tile, dK/dV per key tile.
+// dS = P * (dP - D) * scale.
 // ================================================================================================================
 struct AttnBwdParams {
   const bf16* res; const bf16* out; const bf16* dout;
-  const float* lse; float* Dbuf; float* dq32; bf16* dqkv;
+  const float* lse; float* Dbuf; double* dq64; bf16* dqkv;
   int L, C, heads, cross;
   float scale, scale_log2;
-  int fold;      // fused backward: D and the dQ rounding inside the kernel (scratch must be zero on entry, is zero on exit)
 };
 
-constexpr int kBB = 64;    // streamed block (keys in the dQ kernel, queries in the dK/dV kernel): keeps TMEM <= 256 columns
-
-__device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ---- dQ: CTA = (frame n, head h, 128-query tile); streams 64-key blocks of the kv frame -------------------------
 template <int HD>
-__global__ void __launch_bounds__(320) attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ128,   // qkv, box 128 rows
-                                                             const __grid_constant__ CUtensorMap tmQ64,    // qkv, box 64 rows
-                                                             const __grid_constant__ CUtensorMap tmG128,   // dout, box 128 rows
-                                                             const AttnBwdParams p) {
-  constexpr int CW = HD < 64 ? HD : 64;
+__global__ void __launch_bounds__(kAttnThreads) attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQKV,
+                                                                   const __grid_constant__ CUtensorMap tmG, const AttnBwdParams p) {
+  constexpr int CW = attn_cw(HD);
   constexpr int NCH = HD / CW;
-  constexpr int TILE = 128 * CW * 2;
-  constexpr int TILE_B = kBB * CW * 2;
-  constexpr int STAGES = 2;
-  constexpr uint32_t TMEM_COLS = (2 * kBB + HD) <= 256 ? 256 : 512;
+  constexpr int TILE = kBlk * CW * 2;
+  constexpr int ST = attn_stages(HD);
+  constexpr int DQN = HD <= 64 ? HD : 64;     // dQ is formed DQN columns at a time (register budget at head_dim 128)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smQ = base;
-  uint8_t* smG = smQ + NCH * TILE;
-  uint8_t* smK = smG + NCH * TILE;                    // STAGES * NCH * TILE_B
-  uint8_t* smV = smK + STAGES * NCH * TILE_B;
-  uint8_t* smS = smV + STAGES * NCH * TILE_B;         // dS [128 q][64 keys], SW128: 16384 B
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smS + 16384);
-  uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;
-  uint64_t* kv_empty = kv_full + STAGES;
-  uint64_t* sp_full = kv_empty + STAGES;
-  uint64_t* ds_full = sp_full + 1;
-  uint64_t* dq_full = ds_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dq_full + 1);
+  uint8_t* smK = base;                        // resident key / value tiles of this CTA
+  uint8_t* smV = smK + NCH * TILE;
+  uint8_t* smDS = smV + NCH * TILE;           // dS^T [64 keys][64 queries] bf16, 128B-swizzled (MN-major A operand of dQ)
+  uint8_t* smQ = smDS + kBlk * kBlk * 2;      // ST x NCH tiles
+  uint8_t* smG = smQ + ST * NCH * TILE;       // ST x NCH tiles of dout
+  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smG + ST * NCH * TILE);
+  uint64_t* full = kv_full + 1;
+  uint64_t* empty = full + ST;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * kQT, h = blockIdx.y, n = blockIdx.z;
+  const int k0 = blockIdx.x * kBlk, h = blockIdx.y, n = blockIdx.z;     // n = query frame
   const int nkv = p.cross ? (n ^ 1) : n;
-  const int nb = p.L / kBB;
-  if (threadIdx.x == 0) {
-    mbar_init(q_full, 1);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    mbar_init(sp_full, 1);
-    mbar_init(ds_full, 256);
-    mbar_init(dq_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  xu_grid_dep_sync();     // PDL: everything above (barriers, TMEM) overlaps the previous kernel's tail
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_dP = tmem_base + kBB, tmem_dQ = tmem_base + 2 * kBB;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(q_full, 2 * NCH * TILE);
-      for (int c = 0; c < NCH; ++c) {
-        tma_load_3d(smQ + c * TILE, &tmQ128, q_full, h * HD + c * CW, q0, n);
-        tma_load_3d(smG + c * TILE, &tmG128, q_full, h * HD + c * CW, q0, n);
-      }
-      for (int j = 0; j < nb; ++j) {
-        const int s = j % STAGES;
-        mbar_wait(&kv_empty[s], ((j / STAGES) & 1) ^ 1);
-        mbar_expect_tx(&kv_full[s], 2 * NCH * TILE_B);
-        for (int c = 0; c < NCH; ++c) {
-          tma_load_3d(smK + (s * NCH + c) * TILE_B, &tmQ64, &kv_full[s], p.C + h * HD + c * CW, j * kBB, nkv);
-          tma_load_3d(smV + (s * NCH + c) * TILE_B, &tmQ64, &kv_full[s], 2 * p.C + h * HD + c * CW, j * kBB, nkv);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(kBB, 0, 0);
-      const uint32_t idesc_q = make_idesc_bf16(HD, 0, 1);     // dQ = dS K : B = K block MN-major
-      mbar_wait(q_full, 0);
-      for (int j = 0; j < nb; ++j) {
-        const int s = j % STAGES;
-        mbar_wait(&kv_full[s], (j / STAGES) & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int c = 0; c < NCH; ++c)
-#pragma unroll
-          for (int k = 0; k < CW / 16; ++k) {
-            const uint32_t acc = (c > 0 || k > 0) ? 1u : 0u;
-            umma_bf16(tmem_S, make_kmajor_desc<CW>(smem_u32(smQ + c * TILE) + k * 32),
-                      make_kmajor_desc<CW>(smem_u32(smK + (s * NCH + c) * TILE_B) + k * 32), idesc_s, acc);
-            umma_bf16(tmem_dP, make_kmajor_desc<CW>(smem_u32(smG + c * TILE) + k * 32),
-                      make_kmajor_desc<CW>(smem_u32(smV + (s * NCH + c) * TILE_B) + k * 32), idesc_s, acc);
-          }
-        umma_commit(sp_full);
-        mbar_wait(ds_full, j & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < kBB / 16; ++kk)
-          umma_bf16(tmem_dQ, make_kmajor_desc<64>(smem_u32(smS) + kk * 32),
-                    make_mnmajor_desc<CW>(smem_u32(smK + s * NCH * TILE_B) + kk * 16 * (CW * 2), TILE_B), idesc_q,
-                    (j > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&kv_empty[s]);
-      }
-      umma_commit(dq_full);
-    }
-  } else {
-    // warps 2..9: two warps per TMEM lane quadrant (warp % 4); the pair splits the 64 key columns of every block
-    const int lane_base = (warp & 3) * 32;
-    const int wg = (warp - 2) >> 2;                   // 0: columns [0,32)   1: columns [32,64)
-    const int r = lane_base + lane;
-    const uint32_t lane_addr = (uint32_t)lane_base << 16;
-    const long long row = (long long)n * p.L + q0 + r;
-    // D = rowsum(dO * O) with dO = dout/sqrt2, O = out*sqrt2 - res
-    float D = 0.f;
-    {
-      const long long o = row * p.C + h * HD;
-#pragma unroll
-      for (int c0 = 0; c0 < HD; c0 += 8) {
-        uint4 gv = *reinterpret_cast<const uint4*>(p.dout + o + c0);
-        uint4 ov = *reinterpret_cast<const uint4*>(p.out + o + c0);
-        uint4 rv = *reinterpret_cast<const uint4*>(p.res + o + c0);
-        const __nv_bfloat162* g2 = reinterpret_cast<const __nv_bfloat162*>(&gv);
-        const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&ov);
-        const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          D = fmaf(__low2float(g2[q]) * XU_RSQRT2, __low2float(o2[q]) * XU_SQRT2 - __low2float(r2[q]), D);
-          D = fmaf(__high2float(g2[q]) * XU_RSQRT2, __high2float(o2[q]) * XU_SQRT2 - __high2float(r2[q]), D);
-        }
-      }
-    }
-    const long long li = ((long long)n * p.heads + h) * p.L + q0 + r;
-    if (wg == 0) p.Dbuf[li] = D;
-    const float lse2 = p.lse[li] * 1.4426950408889634f;
-    uint8_t* srow = smS + (r >> 3) * 1024 + (r & 7) * 128;
-    const int c0 = wg * 32;
-    for (int j = 0; j < nb; ++j) {
-      mbar_wait(sp_full, j & 1);
-      tcgen05_fence_after();
-      {
-        uint32_t sv[32], dv[32];
-        tmem_ld32_nowait(tmem_S + lane_addr + c0, sv);
-        tmem_ld32_nowait(tmem_dP + lane_addr + c0, dv);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 pk;
-          uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int i0 = g * 8 + 2 * q;
-            const float p0 = ex2_approx(fmaf(__uint_as_float(sv[i0]), p.scale_log2, -lse2));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(sv[i0 + 1]), p.scale_log2, -lse2));
-            const float d0 = p0 * (__uint_as_float(dv[i0]) * XU_RSQRT2 - D) * p.scale;
-            const float d1 = p1 * (__uint_as_float(dv[i0 + 1]) * XU_RSQRT2 - D) * p.scale;
-            __nv_bfloat162 b2 = __floats2bfloat162_rn(d0, d1);
-            pw[q] = *reinterpret_cast<uint32_t*>(&b2);
-          }
-          const int chunk = (c0 >> 3) + g;
-          sts128(srow + ((chunk ^ (r & 7)) << 4), pk);
-        }
-      }
-      fence_async_smem();
-      tcgen05_fence_before();
-      mbar_arrive(ds_full);
-    }
-    mbar_wait(dq_full, 0);
-    tcgen05_fence_after();
-    bf16* dq = p.dqkv + row * (3LL * p.C) + h * HD;
-#pragma unroll
-    for (int cc = 0; cc < HD; cc += 16) {
-      if (((cc >> 4) & 1) != wg && HD > 16) continue;       // the warp pair alternates 16-column chunks
-      if (HD == 16 && wg != 0) continue;
-      uint32_t v[16];
-      tmem_ld16(tmem_dQ + lane_addr + cc, v);
-      uint4 o[2];
-      __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(o);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) o2[q] = __floats2bfloat162_rn(__uint_as_float(v[2 * q]), __uint_as_float(v[2 * q + 1]));
-      *reinterpret_cast<uint4*>(dq + cc) = o[0];
-      *reinterpret_cast<uint4*>(dq + cc + 8) = o[1];
-    }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ---- dK/dV: CTA = (kv frame m, head h, 128-key tile); streams 64-query blocks of the query frame -----------------
-template <int HD>
-__global__ void __launch_bounds__(320) attn_bwd_dkv_tc_kernel(const __grid_constant__ CUtensorMap tmQ128,
-                                                              const __grid_constant__ CUtensorMap tmQ64,
-                                                              const __grid_constant__ CUtensorMap tmG64,   // dout, box 64 rows
-                                                              const AttnBwdParams p) {
-  constexpr int CW = HD < 64 ? HD : 64;
-  constexpr int NCH = HD / CW;
-  constexpr int TILE = 128 * CW * 2;
-  constexpr int TILE_B = kBB * CW * 2;
-  constexpr int STAGES = 2;
-  constexpr uint32_t TMEM_COLS = (2 * kBB + 2 * HD) <= 256 ? 256 : 512;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smK = base;
-  uint8_t* smV = smK + NCH * TILE;
-  uint8_t* smQ = smV + NCH * TILE;                    // STAGES * NCH * TILE_B
-  uint8_t* smG = smQ + STAGES * NCH * TILE_B;
-  uint8_t* smPT = smG + STAGES * NCH * TILE_B;        // P^T  [128 keys][64 q]  16384 B
-  uint8_t* smST = smPT + 16384;                       // dS^T [128 keys][64 q]  16384 B
-  float* smL = reinterpret_cast<float*>(smST + 16384);  // STAGES * 64 lse
-  float* smD = smL + STAGES * kBB;                      // STAGES * 64 D
-  float* smW = smD + STAGES * kBB;                      // 8 warps x 64: per-warp pre-scaled constants (see the fused kernel)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smW + 8 * 64);
-  uint64_t* kv_full = bars;
-  uint64_t* q_full = bars + 1;
-  uint64_t* q_empty = q_full + STAGES;
-  uint64_t* sp_full = q_empty + STAGES;
-  uint64_t* pt_full = sp_full + 1;
-  uint64_t* dkv_full = pt_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dkv_full + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int k0 = blockIdx.x * 128, h = blockIdx.y, mfr = blockIdx.z;
-  const int nq = p.cross ? (mfr ^ 1) : mfr;
-  const int nb = p.L / kBB;
+  const int nqb = p.L / kBlk;
   if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&q_full[s], 1); mbar_init(&q_empty[s], 1); }
-    mbar_init(sp_full, 1);
-    mbar_init(pt_full, 256);
-    mbar_init(dkv_full, 1);
+    for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQKV) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  xu_grid_dep_sync();     // PDL: everything above (barriers, TMEM) overlaps the previous kernel's tail
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_dP = tmem_base + kBB, tmem_dK = tmem_base + 2 * kBB, tmem_dV = tmem_dK + HD;
-  const long long lrow = ((long long)nq * p.heads + h) * p.L;
+  xu_grid_dep_sync();
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       mbar_expect_tx(kv_full, 2 * NCH * TILE);
       for (int c = 0; c < NCH; ++c) {
-        tma_load_3d(smK + c * TILE, &tmQ128, kv_full, p.C + h * HD + c * CW, k0, mfr);
-        tma_load_3d(smV + c * TILE, &tmQ128, kv_full, 2 * p.C + h * HD + c * CW, k0, mfr);
+        tma_load_3d(smK + c * TILE, &tmQKV, kv_full, p.C + h * HD + c * CW, k0, nkv);
+        tma_load_3d(smV + c * TILE, &tmQKV, kv_full, 2 * p.C + h * HD + c * CW, k0, nkv);
       }
-      for (int i = 0; i < nb; ++i) {
-        const int s = i % STAGES;
-        mbar_wait(&q_empty[s], ((i / STAGES) & 1) ^ 1);
-        mbar_expect_tx(&q_full[s], 2 * NCH * TILE_B + 2 * kBB * 4);
+      for (int j = 0; j < nqb; ++j) {
+        const int s = j % ST;
+        mbar_wait(&empty[s], ((j / ST) & 1) ^ 1);
+        mbar_expect_tx(&full[s], 2 * NCH * TILE);
         for (int c = 0; c < NCH; ++c) {
-          tma_load_3d(smQ + (s * NCH + c) * TILE_B, &tmQ64, &q_full[s], h * HD + c * CW, i * kBB, nq);
-          tma_load_3d(smG + (s * NCH + c) * TILE_B, &tmG64, &q_full[s], h * HD + c * CW, i * kBB, nq);
-        }
-        bulk_load_1d(smL + s * kBB, p.lse + lrow + i * kBB, kBB * 4, &q_full[s]);
-        bulk_load_1d(smD + s * kBB, p.Dbuf + lrow + i * kBB, kBB * 4, &q_full[s]);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(kBB, 0, 0);
-      const uint32_t idesc_o = make_idesc_bf16(HD, 0, 1);
-      mbar_wait(kv_full, 0);
-      for (int i = 0; i < nb; ++i) {
-        const int s = i % STAGES;
-        mbar_wait(&q_full[s], (i / STAGES) & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int c = 0; c < NCH; ++c)
-#pragma unroll
-          for (int k = 0; k < CW / 16; ++k) {
-            const uint32_t acc = (c > 0 || k > 0) ? 1u : 0u;
-            umma_bf16(tmem_S, make_kmajor_desc<CW>(smem_u32(smK + c * TILE) + k * 32),
-                      make_kmajor_desc<CW>(smem_u32(smQ + (s * NCH + c) * TILE_B) + k * 32), idesc_s, acc);
-            umma_bf16(tmem_dP, make_kmajor_desc<CW>(smem_u32(smV + c * TILE) + k * 32),
-                      make_kmajor_desc<CW>(smem_u32(smG + (s * NCH + c) * TILE_B) + k * 32), idesc_s, acc);
-          }
-        umma_commit(sp_full);
-        mbar_wait(pt_full, i & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < kBB / 16; ++kk) {
-          const uint32_t acc = (i > 0 || kk > 0) ? 1u : 0u;
-          umma_bf16(tmem_dV, make_kmajor_desc<64>(smem_u32(smPT) + kk * 32),
-                    make_mnmajor_desc<CW>(smem_u32(smG + s * NCH * TILE_B) + kk * 16 * (CW * 2), TILE_B), idesc_o, acc);
-          umma_bf16(tmem_dK, make_kmajor_desc<64>(smem_u32(smST) + kk * 32),
-                    make_mnmajor_desc<CW>(smem_u32(smQ + s * NCH * TILE_B) + kk * 16 * (CW * 2), TILE_B), idesc_o, acc);
-        }
-        umma_commit(&q_empty[s]);
-      }
-      umma_commit(dkv_full);
-    }
-  } else {
-    // warps 2..9: two warps per TMEM lane quadrant; the pair splits the 64 query columns of every block
-    const int lane_base = (warp & 3) * 32;
-    const int wg = (warp - 2) >> 2;
-    const int r = lane_base + lane;
-    const uint32_t lane_addr = (uint32_t)lane_base << 16;
-    uint8_t* prow = smPT + (r >> 3) * 1024 + (r & 7) * 128;
-    uint8_t* srow = smST + (r >> 3) * 1024 + (r & 7) * 128;
-    const int c0 = wg * 32;
-    // per-query constants, negated and pre-scaled, in a per-warp copy: see the fused kernel below
-    float* wrow = smW + (warp - 2) * 64;
-    const uint32_t wrow_a = smem_u32(wrow);
-    const float c1 = XU_RSQRT2 * p.scale;
-    for (int i = 0; i < nb; ++i) {
-      const int s = i % STAGES;
-      mbar_wait(&q_full[s], (i / STAGES) & 1);     // lse / D of this query block have landed
-      mbar_wait(sp_full, i & 1);
-      tcgen05_fence_after();
-      {
-        uint32_t sv[32], dv[32];
-        tmem_ld32_nowait(tmem_S + lane_addr + c0, sv);
-        tmem_ld32_nowait(tmem_dP + lane_addr + c0, dv);
-        __syncwarp();
-        sts_f32(wrow + lane, lds_f32(smL + s * kBB + c0 + lane) * -1.4426950408889634f);
-        sts_f32(wrow + 32 + lane, lds_f32(smD + s * kBB + c0 + lane) * -p.scale);
-        __syncwarp();
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 pk, sk;
-          uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
-          uint32_t* sw = reinterpret_cast<uint32_t*>(&sk);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int i0 = g * 8 + 2 * q;
-            float2 nl, nd;                                                         // -lse * log2(e), -D * scale of the two queries
-            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(nl.x), "=f"(nl.y) : "r"(wrow_a + (uint32_t)(i0 * 4)));
-            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(nd.x), "=f"(nd.y) : "r"(wrow_a + (uint32_t)(128 + i0 * 4)));
-            const float p0 = ex2_approx(fmaf(__uint_as_float(sv[i0]), p.scale_log2, nl.x));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(sv[i0 + 1]), p.scale_log2, nl.y));
-            const float d0 = p0 * fmaf(__uint_as_float(dv[i0]), c1, nd.x);
-            const float d1 = p1 * fmaf(__uint_as_float(dv[i0 + 1]), c1, nd.y);
-            __nv_bfloat162 a2 = __floats2bfloat162_rn(p0, p1);
-            __nv_bfloat162 b2 = __floats2bfloat162_rn(d0, d1);
-            pw[q] = *reinterpret_cast<uint32_t*>(&a2);
-            sw[q] = *reinterpret_cast<uint32_t*>(&b2);
-          }
-          const int chunk = (c0 >> 3) + g;
-          sts128(prow + ((chunk ^ (r & 7)) << 4), pk);
-          sts128(srow + ((chunk ^ (r & 7)) << 4), sk);
+          tma_load_3d(smQ + (s * NCH + c) * TILE, &tmQKV, &full[s], h * HD + c * CW, j * kBlk, n);
+          tma_load_3d(smG + (s * NCH + c) * TILE, &tmG, &full[s], h * HD + c * CW, j * kBlk, n);
         }
       }
-      fence_async_smem();
-      tcgen05_fence_before();
-      mbar_arrive(pt_full);
     }
-    mbar_wait(dkv_full, 0);
-    tcgen05_fence_after();
-    // the warp pair splits the epilogue: wg 0 writes dK, wg 1 writes dV (= P^T dout / sqrt2)
-    bf16* dst = p.dqkv + ((long long)mfr * p.L + k0 + r) * (3LL * p.C) + p.C + h * HD + (wg ? p.C : 0);
-    const uint32_t tsrc = wg ? tmem_dV : tmem_dK;
-    const float sc = wg ? XU_RSQRT2 : 1.f;
-#pragma unroll
-    for (int cc = 0; cc < HD; cc += 16) {
-      uint32_t a[16];
-      tmem_ld16(tsrc + lane_addr + cc, a);
-      uint4 oa[2];
-      __nv_bfloat162* a2 = reinterpret_cast<__nv_bfloat162*>(oa);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) a2[q] = __floats2bfloat162_rn(__uint_as_float(a[2 * q]) * sc, __uint_as_float(a[2 * q + 1]) * sc);
-      *reinterpret_cast<uint4*>(dst + cc) = oa[0];
-      *reinterpret_cast<uint4*>(dst + cc + 8) = oa[1];
-    }
+    return;
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  const int g = lane >> 2, t = lane & 3;
+  float dv[HD / 2], dk[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  const float* lse_row = p.lse + ((long long)n * p.heads + h) * p.L;
+  const float* D_row = p.Dbuf + ((long long)n * p.heads + h) * p.L;
+  mbar_wait(kv_full, 0);
+  for (int j = 0; j < nqb; ++j) {
+    const int s = j % ST;
+    // per-query operands of the 16 columns this thread holds (L1 / L2 hits: 64 floats per block)
+    float lq[16], dq_[16];
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int q = j * kBlk + 8 * i + 2 * t + e;
+        lq[2 * i + e] = __ldg(lse_row + q) * 1.4426950408889634f;
+        dq_[2 * i + e] = __ldg(D_row + q);
+      }
+    mbar_wait(&full[s], (j / ST) & 1);
+    const uint32_t q_addr = smem_u32(smQ + s * NCH * TILE), g_addr = smem_u32(smG + s * NCH * TILE);
+    float st[32], dpt[32];
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int kk = 0; kk < CW / 16; ++kk) {
+        // S^T = K Q^T  and  dP^T = V dout^T  (every operand K-major: head_dim contiguous)
+        Wgmma<64>::template ss<0, 0>(st, make_kmajor_desc<CW>(smem_u32(smK + c * TILE) + kk * 32),
+                                     make_kmajor_desc<CW>(q_addr + c * TILE + kk * 32), (c > 0 || kk > 0) ? 1u : 0u);
+        Wgmma<64>::template ss<0, 0>(dpt, make_kmajor_desc<CW>(smem_u32(smV + c * TILE) + kk * 32),
+                                     make_kmajor_desc<CW>(g_addr + c * TILE + kk * 32), (c > 0 || kk > 0) ? 1u : 0u);
+      }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * i + 2 * hh + e;
+          const float pv = ex2_approx(fmaf(st[x], p.scale_log2, -lq[2 * i + e]));
+          st[x] = pv;
+          dpt[x] = pv * (dpt[x] * XU_RSQRT2 - dq_[2 * i + e]) * p.scale;
+        }
+    uint32_t pa[4][4], da[4][4];
+    frag_to_a(st, pa);
+    frag_to_a(dpt, da);
+    // dS^T -> shared memory (row = key, 128-byte rows of 64 queries, 16-byte chunks XOR-swizzled by row)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int R = 16 * warp + g + 8 * hh;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const uint32_t v = pack_bf16(dpt[4 * i + 2 * hh], dpt[4 * i + 2 * hh + 1]);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(smDS + R * 128 + ((i ^ (R & 7)) << 4) + 4 * t)), "r"(v) : "memory");
+      }
+    }
+    fence_async_smem();
+    named_bar_sync(1, 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      // dV += P^T dout,  dK += dS^T Q   (B = the query-block tiles, MN-major: head_dim contiguous)
+      Wgmma<HD>::template rs<1>(dv, pa[kk], make_mnmajor_desc<CW>(g_addr + kk * 16 * (CW * 2), TILE), 1u);
+      Wgmma<HD>::template rs<1>(dk, da[kk], make_mnmajor_desc<CW>(q_addr + kk * 16 * (CW * 2), TILE), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    // dQ[64 q][HD] += dS K: A = dS^T in shared memory read MN-major (M = queries), B = the resident key tile (MN-major)
+    const long long qrow0 = (long long)n * p.L + j * kBlk + 16 * warp + g;
+#pragma unroll
+    for (int c2 = 0; c2 < HD / DQN; ++c2) {
+      float dq[DQN / 2];
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        Wgmma<DQN>::template ss<1, 1>(dq, make_mnmajor_desc<64>(smem_u32(smDS) + kk * 16 * 128, 8192),
+                                      make_mnmajor_desc<CW>(smem_u32(smK + c2 * TILE) + kk * 16 * (CW * 2), TILE), kk > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < DQN / 8; ++i)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          double* d = p.dq64 + (qrow0 + 8 * hh) * p.C + h * HD + c2 * DQN + 8 * i + 2 * t;
+          xu_det_add(d, dq[4 * i + 2 * hh]);
+          xu_det_add(d + 1, dq[4 * i + 2 * hh + 1]);
+        }
+    }
+    if (lane == 0) mbar_arrive(&empty[s]);
+    named_bar_sync(1, 128);      // every warp's dQ MMAs have read smDS before the next block overwrites it
   }
+  // dK, dV of this CTA's 64 keys (dV picks up the 1/sqrt2 of dO here)
+  const long long krow0 = (long long)nkv * p.L + k0 + 16 * warp + g;
+#pragma unroll
+  for (int i = 0; i < HD / 8; ++i)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      bf16* d = p.dqkv + (krow0 + 8 * hh) * (3LL * p.C) + h * HD + 8 * i + 2 * t;
+      *reinterpret_cast<__nv_bfloat162*>(d + p.C) = __floats2bfloat162_rn(dk[4 * i + 2 * hh], dk[4 * i + 2 * hh + 1]);
+      *reinterpret_cast<__nv_bfloat162*>(d + 2 * p.C) =
+          __floats2bfloat162_rn(dv[4 * i + 2 * hh] * XU_RSQRT2, dv[4 * i + 2 * hh + 1] * XU_RSQRT2);
+    }
 }
 
-// ring depth of the fused kernel: as deep as two resident CTAs per SM allow (227 KB): 4 stages at head_dim 16 (92 KB per CTA), 3 at 32 (106 KB)
-__host__ __device__ constexpr int fused_stages(int hd) { return hd <= 16 ? 4 : 3; }
-// ---- fused backward for head_dim <= 32: the dK/dV kernel above + dQ in the same pass ------------------------------
-// At head_dim 16/32 the backward is bound by the per-score work (exp, dS, bf16 packing), not by the MMAs, so computing the
-// scores twice (once per kernel) costs 2x.  Here P^T and dS^T are formed once per (128-key, 64-query) tile; besides
-// dV += P^T dO and dK += dS^T Q, a third MMA takes the two adjacent shared-memory tiles [P^T ; dS^T] as ONE MN-major A
-// operand (M = 2 x 64 queries, K = 128 keys) against the resident K tile: TMEM lanes 64..127 of the result are
-// dS K = this key tile's contribution to dQ of the 64 queries (lanes 0..63 = P K, ignored).  It is read back one
-// iteration later, after the arrival that releases the next MMAs (two TMEM dQ buffers), and reduced into an fp32 dQ buffer with red.global.add.v4;
-// attn_bwd_prep_kernel zeroes that buffer and computes D, attn_bwd_dq_store_kernel rounds it to bf16.
-// FOLD (p.fold): the two helper kernels are gone -- D = rowsum(dO * O) of each 64-query block is formed in shared memory from
-// the dout / out / res tiles the producer streams anyway (every key-tile CTA recomputes it: 64 x head_dim MACs per block), and
-// the LAST key-tile CTA of a (query frame, head) -- an atomic ticket after a device-scope fence -- rounds the finished fp32
-// dQ rows to bf16 and re-zeroes them (and the ticket), so the scratch buffer is zero again when the call returns.
-template <int HD>
-__global__ void __launch_bounds__(320, 2) attn_bwd_fused_tc_kernel(const __grid_constant__ CUtensorMap tmQ128,
-                                                              const __grid_constant__ CUtensorMap tmQ64,
-                                                              const __grid_constant__ CUtensorMap tmG64,   // dout, box 64 rows
-                                                              const __grid_constant__ CUtensorMap tmO64,   // out,  box 64 rows (fold)
-                                                              const __grid_constant__ CUtensorMap tmR64,   // res,  box 64 rows (fold)
-                                                              const AttnBwdParams p) {
-  constexpr int CW = HD < 64 ? HD : 64;
-  constexpr int NCH = HD / CW;
-  constexpr int TILE = 128 * CW * 2;
-  constexpr int TILE_B = kBB * CW * 2;
-  // query-block ring: the tiles are tiny (64 x head_dim) and a block is consumed faster than a TMA load returns, so with two stages
-  // every block paid the full load latency (2.1 us per block measured); four stages let the producer run three blocks ahead
-  constexpr int STAGES = fused_stages(HD);
-  constexpr uint32_t TMEM_COLS = 256;
-  static_assert(2 * kBB + 4 * HD <= 256, "fused backward: head_dim <= 32");      // S, dP, dK, dV, 2 x dQ
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smK = base;
-  uint8_t* smV = smK + NCH * TILE;
-  uint8_t* smQ = smV + NCH * TILE;                    // STAGES * NCH * TILE_B
-  uint8_t* smG = smQ + STAGES * NCH * TILE_B;
-  uint8_t* smPT = smG + STAGES * NCH * TILE_B;        // 2 x { P^T [128 keys][64 q] 16384 B ; dS^T [128 keys][64 q] 16384 B }: buffer b at + b * 32768
-  float* smL = reinterpret_cast<float*>(smPT + 2 * 32768);  // STAGES * 64 lse
-  float* smD = smL + STAGES * kBB;                      // STAGES * 64 D
-  float* smW = smD + STAGES * kBB;                      // 8 warps x 64: each softmax warp's own pre-scaled (-lse*log2e | -D*scale) of its 32 queries
-  uint8_t* smO = reinterpret_cast<uint8_t*>(smW + 8 * 64);           // fold: out tiles, STAGES * NCH * TILE_B
-  uint8_t* smR = smO + (p.fold ? STAGES * NCH * TILE_B : 0);         // fold: res tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smR + (p.fold ? STAGES * NCH * TILE_B : 0));
-  uint64_t* kv_full = bars;
-  uint64_t* q_full = bars + 1;
-  uint64_t* q_empty = q_full + STAGES;
-  uint64_t* sp_full = q_empty + STAGES;
-  uint64_t* pt_full = sp_full + 1;
-  uint64_t* dkv_full = pt_full + 1;
-  uint64_t* s_free = dkv_full + 1;     // the softmax warps have read S_i / dP_i out of TMEM
-  uint64_t* pt_empty = s_free + 1;     // [2]: the MMAs that read [P^T ; dS^T] buffer b (and wrote the dQ partial) have completed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pt_empty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int k0 = blockIdx.x * 128, h = blockIdx.y, mfr = blockIdx.z;
-  const int nq = p.cross ? (mfr ^ 1) : mfr;
-  const int nb = p.L / kBB;
-  if (threadIdx.x == 0) {
-    mbar_init(kv_full, 1);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&q_full[s], 1); mbar_init(&q_empty[s], 1); }
-    mbar_init(sp_full, 1);
-    mbar_init(pt_full, 256);
-    mbar_init(dkv_full, 1);
-    mbar_init(s_free, 256);
-    mbar_init(&pt_empty[0], 1); mbar_init(&pt_empty[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  xu_grid_dep_sync();     // PDL: everything above (barriers, TMEM) overlaps the previous kernel's tail
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_dP = tmem_base + kBB, tmem_dK = tmem_base + 2 * kBB, tmem_dV = tmem_dK + HD, tmem_dQ = tmem_dV + HD;
-  const long long lrow = ((long long)nq * p.heads + h) * p.L;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(kv_full, 2 * NCH * TILE);
-      for (int c = 0; c < NCH; ++c) {
-        tma_load_3d(smK + c * TILE, &tmQ128, kv_full, p.C + h * HD + c * CW, k0, mfr);
-        tma_load_3d(smV + c * TILE, &tmQ128, kv_full, 2 * p.C + h * HD + c * CW, k0, mfr);
-      }
-      for (int i = 0; i < nb; ++i) {
-        const int s = i % STAGES;
-        mbar_wait(&q_empty[s], ((i / STAGES) & 1) ^ 1);
-        mbar_expect_tx(&q_full[s], p.fold ? 4 * NCH * TILE_B + kBB * 4 : 2 * NCH * TILE_B + 2 * kBB * 4);
-        for (int c = 0; c < NCH; ++c) {
-          tma_load_3d(smQ + (s * NCH + c) * TILE_B, &tmQ64, &q_full[s], h * HD + c * CW, i * kBB, nq);
-          tma_load_3d(smG + (s * NCH + c) * TILE_B, &tmG64, &q_full[s], h * HD + c * CW, i * kBB, nq);
-          if (p.fold) {
-            tma_load_3d(smO + (s * NCH + c) * TILE_B, &tmO64, &q_full[s], h * HD + c * CW, i * kBB, nq);
-            tma_load_3d(smR + (s * NCH + c) * TILE_B, &tmR64, &q_full[s], h * HD + c * CW, i * kBB, nq);
-          }
-        }
-        bulk_load_1d(smL + s * kBB, p.lse + lrow + i * kBB, kBB * 4, &q_full[s]);
-        if (!p.fold) bulk_load_1d(smD + s * kBB, p.Dbuf + lrow + i * kBB, kBB * 4, &q_full[s]);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(kBB, 0, 0);
-      const uint32_t idesc_o = make_idesc_bf16(HD, 0, 1);
-      const uint32_t idesc_dq = make_idesc_bf16(HD, 1, 1);    // A = [P^T ; dS^T] MN-major (queries), B = K tile MN-major (channels)
-      mbar_wait(kv_full, 0);
-      // Software pipeline: S_{i+1} / dP_{i+1} are issued as soon as the softmax warps have READ S_i / dP_i out of TMEM (s_free), i.e.
-      // while they still compute P / dS of block i; the dV / dK / dQ MMAs of block i follow when [P^T ; dS^T] (buffer i & 1) is in shared
-      // memory.  The softmax warps therefore go from block to block without waiting for a tensor-core round trip (round 1 / early
-      // round 2: strictly serial S -> softmax -> dV/dK/dQ -> next S, 2.4 us per block of which the arithmetic was a small part).
-      auto issue_scores = [&](int blk) {
-        const int s = blk % STAGES;
-        mbar_wait(&q_full[s], (blk / STAGES) & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int c = 0; c < NCH; ++c)
-#pragma unroll
-          for (int k = 0; k < CW / 16; ++k) {
-            const uint32_t acc = (c > 0 || k > 0) ? 1u : 0u;
-            umma_bf16(tmem_S, make_kmajor_desc<CW>(smem_u32(smK + c * TILE) + k * 32),
-                      make_kmajor_desc<CW>(smem_u32(smQ + (s * NCH + c) * TILE_B) + k * 32), idesc_s, acc);
-            umma_bf16(tmem_dP, make_kmajor_desc<CW>(smem_u32(smV + c * TILE) + k * 32),
-                      make_kmajor_desc<CW>(smem_u32(smG + (s * NCH + c) * TILE_B) + k * 32), idesc_s, acc);
-          }
-        umma_commit(sp_full);
-      };
-      issue_scores(0);
-      for (int i = 0; i < nb; ++i) {
-        const int s = i % STAGES;
-        if (i + 1 < nb) {
-          mbar_wait(s_free, i & 1);              // S_i / dP_i are in the softmax warps' registers
-          issue_scores(i + 1);
-        }
-        mbar_wait(pt_full, i & 1);
-        tcgen05_fence_after();
-        const uint32_t pt = smem_u32(smPT) + (uint32_t)((i & 1) * 32768), st = pt + 16384u;
-#pragma unroll
-        for (int kk = 0; kk < kBB / 16; ++kk) {
-          const uint32_t acc = (i > 0 || kk > 0) ? 1u : 0u;
-          umma_bf16(tmem_dV, make_kmajor_desc<64>(pt + kk * 32),
-                    make_mnmajor_desc<CW>(smem_u32(smG + s * NCH * TILE_B) + kk * 16 * (CW * 2), TILE_B), idesc_o, acc);
-          umma_bf16(tmem_dK, make_kmajor_desc<64>(st + kk * 32),
-                    make_mnmajor_desc<CW>(smem_u32(smQ + s * NCH * TILE_B) + kk * 16 * (CW * 2), TILE_B), idesc_o, acc);
-        }
-#pragma unroll
-        for (int kk = 0; kk < 128 / 16; ++kk)
-          umma_bf16(tmem_dQ + (uint32_t)((i & 1) * HD), make_mnmajor_desc<64>(pt + kk * 16 * 128, 16384),
-                    make_mnmajor_desc<CW>(smem_u32(smK) + kk * 16 * (CW * 2), TILE), idesc_dq, kk > 0 ? 1u : 0u);
-        umma_commit(&q_empty[s]);
-        umma_commit(&pt_empty[i & 1]);
-      }
-      umma_commit(dkv_full);
-    }
-  } else {
-    // warps 2..9: two warps per TMEM lane quadrant; the pair splits the 64 query columns of every block
-    const int lane_base = (warp & 3) * 32;
-    const int wg = (warp - 2) >> 2;
-    const int r = lane_base + lane;
-    const uint32_t lane_addr = (uint32_t)lane_base << 16;
-    uint8_t* prow0 = smPT + (r >> 3) * 1024 + (r & 7) * 128;
-    const int c0 = wg * 32;
-    // lanes 64..127 of tmem_dQ = dS K for query (r - 64) of the block; the warp pair splits the HD columns
-    auto flush_dq = [&](int blk) {
-      constexpr int HC = HD / 2;
-      float* dst = p.dq32 + ((long long)nq * p.L + blk * kBB + (r - 64)) * p.C + h * HD + wg * HC;
-      uint32_t v[HC];
-      const uint32_t src = tmem_dQ + (uint32_t)((blk & 1) * HD) + lane_addr + wg * HC;   // dQ partials are double-buffered
-      if constexpr (HC == 8) tmem_ld8(src, v);
-      else tmem_ld16(src, v);
-#pragma unroll
-      for (int j = 0; j < HC; j += 4)
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(__uint_as_float(v[j])),
-                     "f"(__uint_as_float(v[j + 1])), "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
-                     : "memory");
-    };
-    // The per-query constants of a block (lse, D: one value per query = per COLUMN of the transposed score tile) enter the per-score
-    // work negated and pre-scaled (-lse*log2(e), -D*scale), so that a score costs FFMA, EX2, FFMA, FMUL + packing.  Each warp keeps
-    // its own copy of the 32 queries it handles (lane l scales query c0 + l): no block-wide barrier, explicit ld.shared broadcasts.
-    float* wrow = smW + (warp - 2) * 64;
-    const uint32_t wrow_a = smem_u32(wrow);
-    const float c1 = XU_RSQRT2 * p.scale;
-    for (int i = 0; i < nb; ++i) {
-      const int s = i % STAGES;
-      mbar_wait(&q_full[s], (i / STAGES) & 1);     // lse / D of this query block have landed
-      if (p.fold) {
-        // D[q] = sum_c (dout/sqrt2) * (out*sqrt2 - res) of query q of this block, from the three [64][HD] tiles: the same
-        // swizzle permutes the 16-byte chunks of a row identically in all three, and a dot product does not care about the order
-        if (wg == 0 && r < kBB) {
-          float D = 0.f;
-#pragma unroll
-          for (int c = 0; c < NCH; ++c)
-#pragma unroll
-            for (int j = 0; j < CW / 8; ++j) {
-              const uint32_t off = (uint32_t)((s * NCH + c) * TILE_B + r * (CW * 2) + j * 16);
-              const uint4 gv = *reinterpret_cast<const uint4*>(smG + off);
-              const uint4 ov = *reinterpret_cast<const uint4*>(smO + off);
-              const uint4 rv = *reinterpret_cast<const uint4*>(smR + off);
-              const __nv_bfloat162* g2 = reinterpret_cast<const __nv_bfloat162*>(&gv);
-              const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&ov);
-              const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                D = fmaf(__low2float(g2[q]) * XU_RSQRT2, __low2float(o2[q]) * XU_SQRT2 - __low2float(r2[q]), D);
-                D = fmaf(__high2float(g2[q]) * XU_RSQRT2, __high2float(o2[q]) * XU_SQRT2 - __high2float(r2[q]), D);
-              }
-            }
-          smD[s * kBB + r] = D;
-        }
-        named_bar_sync(2, 256);
-      }
-      mbar_wait(sp_full, i & 1);
-      tcgen05_fence_after();
-      uint8_t* prow = prow0 + (i & 1) * 32768;         // [P^T ; dS^T] buffer of this block
-      uint8_t* srow = prow + 16384;
-      {
-        uint32_t sv[32], dv[32];
-        tmem_ld32_nowait(tmem_S + lane_addr + c0, sv);
-        tmem_ld32_nowait(tmem_dP + lane_addr + c0, dv);
-        // while the TMEM loads fly: this warp's pre-scaled constants of block i (the previous block's reads are behind a __syncwarp)
-        __syncwarp();
-        sts_f32(wrow + lane, lds_f32(smL + s * kBB + c0 + lane) * -1.4426950408889634f);
-        sts_f32(wrow + 32 + lane, lds_f32(smD + s * kBB + c0 + lane) * -p.scale);
-        __syncwarp();
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        tcgen05_fence_before();
-        mbar_arrive(s_free);                       // the MMA lane may overwrite S / dP with block i+1
-        mbar_wait(&pt_empty[i & 1], ((i >> 1) & 1) ^ 1);   // the MMAs of block i-2 have finished reading this [P^T ; dS^T] buffer
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 pk, sk;
-          uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
-          uint32_t* sw = reinterpret_cast<uint32_t*>(&sk);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int i0 = g * 8 + 2 * q;
-            float2 nl, nd;                                                         // -lse * log2(e), -D * scale of the two queries
-            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(nl.x), "=f"(nl.y) : "r"(wrow_a + (uint32_t)(i0 * 4)));
-            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(nd.x), "=f"(nd.y) : "r"(wrow_a + (uint32_t)(128 + i0 * 4)));
-            const float p0 = ex2_approx(fmaf(__uint_as_float(sv[i0]), p.scale_log2, nl.x));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(sv[i0 + 1]), p.scale_log2, nl.y));
-            const float d0 = p0 * fmaf(__uint_as_float(dv[i0]), c1, nd.x);
-            const float d1 = p1 * fmaf(__uint_as_float(dv[i0 + 1]), c1, nd.y);
-            __nv_bfloat162 a2 = __floats2bfloat162_rn(p0, p1);
-            __nv_bfloat162 b2 = __floats2bfloat162_rn(d0, d1);
-            pw[q] = *reinterpret_cast<uint32_t*>(&a2);
-            sw[q] = *reinterpret_cast<uint32_t*>(&b2);
-          }
-          const int chunk = (c0 >> 3) + g;
-          sts128(prow + ((chunk ^ (r & 7)) << 4), pk);
-          sts128(srow + ((chunk ^ (r & 7)) << 4), sk);
-        }
-      }
-      fence_async_smem();
-      tcgen05_fence_before();
-      mbar_arrive(pt_full);
-      // off the critical path: block i-1's dQ part sits in the OTHER dQ buffer (complete once pt_empty of that block has fired); the
-      // issuer reuses that buffer only for block i+1, i.e. after this thread's next arrival
-      if (i > 0 && r >= 64) {
-        mbar_wait(&pt_empty[(i - 1) & 1], ((i - 1) >> 1) & 1);
-        tcgen05_fence_after();
-        flush_dq(i - 1);
-      }
-    }
-    mbar_wait(dkv_full, 0);
-    tcgen05_fence_after();
-    if (r >= 64) flush_dq(nb - 1);
-    // the warp pair splits the epilogue: wg 0 writes dK, wg 1 writes dV (= P^T dout / sqrt2)
-    bf16* dst = p.dqkv + ((long long)mfr * p.L + k0 + r) * (3LL * p.C) + p.C + h * HD + (wg ? p.C : 0);
-    const uint32_t tsrc = wg ? tmem_dV : tmem_dK;
-    const float sc = wg ? XU_RSQRT2 : 1.f;
-#pragma unroll
-    for (int cc = 0; cc < HD; cc += 16) {
-      uint32_t a[16];
-      tmem_ld16(tsrc + lane_addr + cc, a);
-      uint4 oa[2];
-      __nv_bfloat162* a2 = reinterpret_cast<__nv_bfloat162*>(oa);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) a2[q] = __floats2bfloat162_rn(__uint_as_float(a[2 * q]) * sc, __uint_as_float(a[2 * q + 1]) * sc);
-      *reinterpret_cast<uint4*>(dst + cc) = oa[0];
-      *reinterpret_cast<uint4*>(dst + cc + 8) = oa[1];
-    }
-    if (p.fold) {
-      // ---- last key-tile CTA of this (query frame, head): dQ fp32 -> bf16, then leave the scratch zeroed ----
-      __threadfence();                                   // this thread's red.global.adds are performed device-wide
-      named_bar_sync(2, 256);
-      int* flag = reinterpret_cast<int*>(smD);           // D values are dead by now
-      if (threadIdx.x == 64) {
-        int* ticket = reinterpret_cast<int*>(p.Dbuf) + nq * p.heads + h;
-        const int old = atomicAdd(ticket, 1);
-        const int last = old == (int)gridDim.x - 1;
-        if (last) *ticket = 0;                           // nobody else touches it any more in this launch
-        *flag = last;
-      }
-      named_bar_sync(2, 256);
-      if (*flag) {
-        __threadfence();
-        const int t = threadIdx.x - 64;                  // 0..255
-        constexpr int V4 = HD / 4;                       // float4 per query row of this head
-        for (int idx = t; idx < p.L * V4; idx += 256) {
-          const int q = idx / V4, v = idx - q * V4;
-          float4* src = reinterpret_cast<float4*>(p.dq32 + ((long long)nq * p.L + q) * p.C + h * HD) + v;
-          const float4 x = __ldcg(src);
-          __stcg(src, make_float4(0.f, 0.f, 0.f, 0.f));
-          __nv_bfloat162 a = __floats2bfloat162_rn(x.x, x.y), b = __floats2bfloat162_rn(x.z, x.w);
-          uint2 o;
-          o.x = *reinterpret_cast<uint32_t*>(&a);
-          o.y = *reinterpret_cast<uint32_t*>(&b);
-          *reinterpret_cast<uint2*>(p.dqkv + ((long long)nq * p.L + q) * (3LL * p.C) + h * HD + v * 4) = o;
-        }
-      }
-    }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// D = rowsum(dO * O) per (row, head) and dq32 = 0, for the fused backward (one thread per row and head)
+// D = rowsum(dO * O) per (row, head) (one thread per row and head)
 template <int HD>
 __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnBwdParams p, long long total) {
   xu_grid_dep_sync();
@@ -997,109 +386,87 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnBwdParams 
   }
   const long long n = row / p.L, l = row % p.L;
   p.Dbuf[(n * p.heads + h) * p.L + l] = D;
-#pragma unroll
-  for (int c0 = 0; c0 < HD; c0 += 4) *reinterpret_cast<float4*>(p.dq32 + o + c0) = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-// dq32 -> the q third of dqkv (bf16), 4 channels per thread
-__global__ void __launch_bounds__(256) attn_bwd_dq_store_kernel(const float* __restrict__ dq32, bf16* __restrict__ dqkv, long long total4,
-                                                                int C) {
+// dq64 -> the q third of dqkv (bf16), 4 channels per thread, re-zeroing dq64.  zero: also clear the n_d D values, so that a
+// caller that keeps its scratch buffer all-zero between calls gets it back that way.
+__global__ void __launch_bounds__(256) attn_bwd_dq_store_kernel(double* __restrict__ dq64, bf16* __restrict__ dqkv, long long total4,
+                                                                int C, float* __restrict__ dbuf, long long n_d, int zero) {
   xu_grid_dep_sync();
   const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
   if (idx >= total4) return;
   const int c4 = (int)(idx % (C / 4));
   const long long row = idx / (C / 4);
-  const float4 v = *reinterpret_cast<const float4*>(dq32 + row * C + c4 * 4);
-  __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+  double2* src = reinterpret_cast<double2*>(dq64 + row * C + c4 * 4);
+  const double2 v01 = src[0], v23 = src[1];
+  src[0] = make_double2(0.0, 0.0);
+  src[1] = make_double2(0.0, 0.0);
+  __nv_bfloat162 a = __floats2bfloat162_rn((float)v01.x, (float)v01.y), b = __floats2bfloat162_rn((float)v23.x, (float)v23.y);
   uint2 t;
   t.x = *reinterpret_cast<uint32_t*>(&a);
   t.y = *reinterpret_cast<uint32_t*>(&b);
   *reinterpret_cast<uint2*>(dqkv + row * (3LL * C) + c4 * 4) = t;
+  if (zero && idx < n_d) dbuf[idx] = 0.f;
 }
 
 template <int HD>
 void launch_bwd(const AttnArgs& a, cudaStream_t s) {
-  constexpr int CW = HD < 64 ? HD : 64;
+  constexpr int CW = attn_cw(HD);
   constexpr int NCH = HD / CW;
-  constexpr int TILE = 128 * CW * 2;
-  constexpr int TILE_B = kBB * CW * 2;
-  CUtensorMap q128, q64, g128, g64, o64, r64;
+  constexpr int TILE = kBlk * CW * 2;
+  CUtensorMap tq, tg;
   uint64_t qd[3] = {(uint64_t)(3 * a.C), (uint64_t)a.L, (uint64_t)a.N};
   uint64_t qs[2] = {(uint64_t)3 * a.C * 2, (uint64_t)a.L * 3 * a.C * 2};
   uint64_t gd[3] = {(uint64_t)a.C, (uint64_t)a.L, (uint64_t)a.N};
   uint64_t gs[2] = {(uint64_t)a.C * 2, (uint64_t)a.L * a.C * 2};
-  uint32_t b128[3] = {(uint32_t)CW, 128u, 1u}, b64[3] = {(uint32_t)CW, (uint32_t)kBB, 1u};
-  if (!xu_encode_bf16_map(&q128, a.qkv, 3, qd, qs, b128, CW) || !xu_encode_bf16_map(&q64, a.qkv, 3, qd, qs, b64, CW) ||
-      !xu_encode_bf16_map(&g128, a.dout, 3, gd, gs, b128, CW) || !xu_encode_bf16_map(&g64, a.dout, 3, gd, gs, b64, CW) ||
-      !xu_encode_bf16_map(&o64, a.out, 3, gd, gs, b64, CW) || !xu_encode_bf16_map(&r64, a.res, 3, gd, gs, b64, CW))
-    return;
+  uint32_t box[3] = {(uint32_t)CW, (uint32_t)kBlk, 1u};
+  if (!xu_encode_bf16_map(&tq, a.qkv, 3, qd, qs, box, CW) || !xu_encode_bf16_map(&tg, a.dout, 3, gd, gs, box, CW)) return;
   AttnBwdParams p;
   p.res = (const bf16*)a.res; p.out = (const bf16*)a.out; p.dout = (const bf16*)a.dout;
   p.lse = a.lse; p.Dbuf = a.dscratch; p.dqkv = (bf16*)a.dqkv;
-  p.dq32 = a.dscratch + (long long)a.N * a.heads * a.L;      // [N*L][C] fp32, used by the fused (head_dim <= 32) path
+  const long long rows = (long long)a.N * a.L;
+  p.dq64 = xu_det_scratch(s, rows * a.C);                     // [N*L][C] fp64
+  if (p.dq64 == nullptr) return;
   p.L = a.L; p.C = a.C; p.heads = a.heads; p.cross = a.cross;
   p.scale = 1.f / sqrtf((float)HD);
   p.scale_log2 = 1.4426950408889634f * p.scale;
-  p.fold = 0;
-  const size_t smem_dq = (size_t)2 * NCH * TILE + 4 * NCH * TILE_B + 16384 + 1024 + 128;
-  const size_t smem_dkv = (size_t)2 * NCH * TILE + 4 * NCH * TILE_B + 2 * 16384 + 4 * kBB * 4 + 8 * 64 * 4 + 1024 + 128;
-  // fused kernel: K, V tiles + fused_stages(HD) x (q, dout tiles) + two [P^T ; dS^T] pairs + fused_stages(HD) x (lse, D) + barriers
-  const size_t smem_fused = (size_t)2 * NCH * TILE + 2 * fused_stages(HD) * NCH * TILE_B + 4 * 16384 + 2 * fused_stages(HD) * kBB * 4 + 8 * 64 * 4 + 1024 + 256;
+  const size_t smem = (size_t)2 * NCH * TILE + kBlk * kBlk * 2 + (size_t)2 * attn_stages(HD) * NCH * TILE + 1024 + 256;
   static bool configured = false;
   if (!configured) {
-    cudaFuncSetAttribute(attn_bwd_dq_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024));
-    cudaFuncSetAttribute(attn_bwd_dkv_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024));
+    cudaFuncSetAttribute(attn_bwd_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     configured = true;
   }
-  dim3 grid(a.L / 128, a.heads, a.N);
-  if constexpr (HD <= 32) {
-    static const bool split = getenv("XUNET_ATTN_BWD_SPLIT") != nullptr;     // A/B switch: the two-kernel path
-    if (!split) {
-      static bool configured_f = false;
-      if (!configured_f) {
-        cudaFuncSetAttribute(attn_bwd_fused_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024));
-        configured_f = true;
-      }
-      const long long rows = (long long)a.N * a.L;
-      if (a.scratch_zeroed) {      // the caller guarantees a zeroed scratch buffer (and gets it back zeroed): no helper kernels
-        p.fold = 1;
-        xu_launch(attn_bwd_fused_tc_kernel<HD>, grid, 320, smem_fused + 2 * fused_stages(HD) * NCH * TILE_B, s, q128, q64, g64, o64, r64, p);
-        return;
-      }
-      xu_launch(attn_bwd_prep_kernel<HD>, cdiv(rows * a.heads, 256), 256, 0, s, p, rows * a.heads);
-      xu_launch(attn_bwd_fused_tc_kernel<HD>, grid, 320, smem_fused, s, q128, q64, g64, o64, r64, p);
-      xu_launch(attn_bwd_dq_store_kernel, cdiv(rows * a.C / 4, 256), 256, 0, s, (const float*)p.dq32, p.dqkv, rows * a.C / 4, a.C);
-      return;
-    }
-  }
-  xu_launch(attn_bwd_dq_tc_kernel<HD>, grid, 320, smem_dq, s, q128, q64, g128, p);
-  xu_launch(attn_bwd_dkv_tc_kernel<HD>, grid, 320, smem_dkv, s, q128, q64, g64, p);
+  xu_launch(attn_bwd_prep_kernel<HD>, cdiv(rows * a.heads, 256), 256, 0, s, p, rows * a.heads);
+  xu_launch(attn_bwd_tc_kernel<HD>, dim3(a.L / kBlk, a.heads, a.N), kAttnThreads, smem, s, tq, tg, p);
+  xu_launch(attn_bwd_dq_store_kernel, cdiv(rows * a.C / 4, 256), 256, 0, s, p.dq64, p.dqkv, rows * a.C / 4, a.C, p.Dbuf,
+            rows * a.heads, a.scratch_zeroed);
 }
 
 template <int HD>
 void launch_fwd(const AttnArgs& a, cudaStream_t s) {
-  constexpr int CW = HD < 64 ? HD : 64;
+  constexpr int CW = attn_cw(HD);
   constexpr int NCH = HD / CW;
-  constexpr int TILE = 128 * CW * 2;
-  constexpr int TILE_B = kKB * CW * 2;
-  CUtensorMap tq, tkv;
+  constexpr int TILE = kBlk * CW * 2;
+  CUtensorMap tq;
   uint64_t dims[3] = {(uint64_t)(3 * a.C), (uint64_t)a.L, (uint64_t)a.N};
   uint64_t strides[2] = {(uint64_t)3 * a.C * 2, (uint64_t)a.L * 3 * a.C * 2};
-  uint32_t box_q[3] = {(uint32_t)CW, 128u, 1u}, box_kv[3] = {(uint32_t)CW, (uint32_t)kKB, 1u};
-  if (!xu_encode_bf16_map(&tq, a.qkv, 3, dims, strides, box_q, CW) || !xu_encode_bf16_map(&tkv, a.qkv, 3, dims, strides, box_kv, CW)) return;
+  uint32_t box[3] = {(uint32_t)CW, (uint32_t)kBlk, 1u};
+  if (!xu_encode_bf16_map(&tq, a.qkv, 3, dims, strides, box, CW)) return;
   AttnTcParams p;
   p.res = (const bf16*)a.res; p.out = (bf16*)a.out; p.lse = a.lse;
   p.L = a.L; p.C = a.C; p.heads = a.heads; p.cross = a.cross;
   p.scale_log2 = 1.4426950408889634f / sqrtf((float)HD);
-  p.cstats = a.cstats;
-  const size_t smem = (size_t)NCH * TILE + 2 * fwd_kv_stages(HD) * NCH * TILE_B + 2 * 128 * kKB * 2 + 1024 + 256;
+  const long long ncs = a.cstats ? (long long)(a.N / 2) * a.C * 2 : 0;
+  p.cstats = nullptr;
+  if (ncs > 0 && (p.cstats = xu_det_scratch(s, ncs)) == nullptr) return;
+  const size_t smem = (size_t)NCH * TILE + (size_t)2 * attn_stages(HD) * NCH * TILE + 1024 + 256;
   static bool configured = false;
   if (!configured) {
-    cudaFuncSetAttribute(attn_fwd_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024));
+    cudaFuncSetAttribute(attn_fwd_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     configured = true;
   }
-  dim3 grid(a.L / kQT, a.heads, a.N);
-  xu_launch(attn_fwd_tc_kernel<HD>, grid, 192, smem, s, tq, tkv, p);
+  xu_launch(attn_fwd_tc_kernel<HD>, dim3(a.L / kBlk, a.heads, a.N), kAttnThreads, smem, s, tq, p);
+  if (p.cstats != nullptr) xu_det_fold(a.cstats, p.cstats, ncs, s);
 }
 
 }  // namespace

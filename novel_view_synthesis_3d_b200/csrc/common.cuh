@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the X-UNet sm_100a kernels.
+// common.cuh -- shared device helpers for the X-UNet sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -136,13 +136,13 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-// SM count of the current device (148 on B200), queried once; grids of persistent / wave-sized kernels derive from it
+// SM count of the current device (132 on an H100 SXM), queried once; grids of persistent / wave-sized kernels derive from it
 static inline int xu_num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0, v = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) n = v;
-    else n = 148;
+    else n = 132;
     // data parallel: NCCL's reduction CTAs need SMs of their own while the persistent one-CTA-per-SM kernels run; with
     // XUNET_SM_RESERVE=k the persistent / wave-sized grids leave k SMs free (a persistent grid that does not fit runs a second wave)
     const char* e = getenv("XUNET_SM_RESERVE");

@@ -1,19 +1,19 @@
-// conv_tc.cu -- tcgen05 / TMEM / TMA implicit-GEMM convolution for sm_100a (bf16 operands, fp32 accumulate in TMEM).
+// conv_tc.cu -- wgmma / TMA implicit-GEMM convolution for sm_90a (bf16 operands, fp32 accumulate in registers).
 //
 // Replaces the cuDNN/cuBLAS calls behind flax nn.Conv(3x3, SAME, stride 1) / nn.Dense / nn.DenseGeneral on the
 // reference's hot path (model/xunet.py:59,81,85-89,91,100-102) -- forward AND data-gradient.
 //
-//   D[128 pixels, BN] (TMEM, fp32)  =  sum over (tap, channel-chunk)  A[128 pixels, BK] (smem)  x  B[BN, BK] (smem)
+//   D[128 pixels, BN] (registers, fp32)  =  sum over (tap, channel-chunk)  A[128 pixels, BK] (smem)  x  B[BN, BK] (smem)
 //
 // * A is never materialised as im2col: an M-tile is a TN x TH x TW brick of output pixels of the NHWC tensor and each
 //   (tap, chunk) stage is ONE 4-D TMA box load at coordinates (c0, x0+dx-1, y0+dy-1, n0); out-of-bounds rows/cols are
 //   zero-filled by the TMA unit, which IS the SAME padding.  The box lands in shared memory in exactly the K-major
-//   128B/64B/32B-swizzled layout the UMMA smem descriptor expects.
+//   128B/64B/32B-swizzled layout the GMMA smem descriptor expects.
 // * B comes from a bf16 "shadow" of the fp32 master weights, K-major: forward [Co][tap][Ci] (transposed by
 //   weight_prep_kernel), data-gradient the plain cast [tap][Ci][Co] (there K = Co is already contiguous).
-// * Warp-specialised: warp 0 = TMA producer (one elected lane), warp 1 = TMEM allocator + MMA issuer (one lane issues
-//   tcgen05.mma, tcgen05.commit releases smem stages / signals the epilogue through mbarriers), warps 2-5 = epilogue
-//   (tcgen05.ld 32 lanes x 32 columns -> +bias (+residual) * alpha -> bf16 -> 16-byte global stores).
+// * Warp-specialised: warp 8 = TMA producer (one elected lane), warps 0-7 = two consumer warpgroups that issue
+//   wgmma.mma_async (64 rows each), release ring stages through mbarriers and run the epilogue
+//   (+bias (+residual) * alpha -> bf16 -> 16-byte global stores or a TMA store).
 #include "conv_tc.h"
 #include "tc_common.cuh"
 
@@ -34,12 +34,10 @@ struct TcParams {
   const bf16* res;
   const float* bias;
   int BN, stages;
-  int n_tiles, m_tiles, total_tiles, nacc;
+  int n_tiles, m_tiles, total_tiles;
   int halo;      // 3x3 stride-1: one (TH+2) x TW halo box per (channel chunk, dx) serves the three dy taps
-  int m2;        // halo only: a work unit is TWO vertically adjacent 8 x 16 tiles (16 x 16 pixels, an 18-row box) accumulated into two
-                 // TMEM buffers by the same pipeline steps, so one fetch of the weight tile feeds 256 output pixels
   int n_fast;    // tile order: 1 = the n-tiles of one m-tile are adjacent (A tile re-read from L2, not HBM); 0 = m fastest
-  float* cstats; // EPI 1: per-(sample, channel) [sum, sumsq] of the stored output, (N/2, Co, 2) fp32, accumulated
+  double* cstats; // fp64 accumulators (xu_det_scratch). EPI 1: per-(sample, channel) [sum, sumsq] of the stored output, (N/2, Co, 2) fp32, accumulated
                  // EPI 2: per-(sample, channel) [sum dyh*xhat, sum dyh] of the GroupNorm backward (same layout)
   const bf16* gx;      // EPI 2: input x of the GroupNorm whose OUTPUT gradient this data-gradient produces, (N,H,W,Co)
   const float4* gnp;   // EPI 2: per-(sample, channel) {rstd, -mean*rstd, gamma, beta} written by the forward gn_apply
@@ -51,13 +49,15 @@ struct TcParams {
   // output through shared memory + TMA store: the epilogue writes the rounded tile into a swizzled [128 pixels][cws channels]
   // staging buffer (conflict-free 16-byte st.shared) and one thread issues cp.async.bulk.tensor stores of whole boxes
   int tma_store, cws;
-  int ew;        // epilogue warps (4 or 8), see the kernel
   int prefetch;  // pipeline steps by which an L2 prefetch of the activation box runs ahead of its TMA load (0: none)
 };
 
 // Persistent: each CTA walks tiles  blockIdx.x, blockIdx.x + gridDim.x, ...  (tile = m_tile * n_tiles + n_tile) with the
-// smem ring running continuously across tiles and TWO accumulator buffers in TMEM, so the epilogue of tile i (TMEM -> regs
-// -> global) overlaps the TMA/MMA main loop of tile i+1.
+// smem ring running continuously across tiles.  Warps 0-7 are two consumer warpgroups: warpgroup wg issues the wgmma for
+// rows 64 wg .. 64 wg + 63 of the 128-pixel tile (fp32 accumulators in registers) and then runs the epilogue of those rows;
+// warp 8 is the TMA producer (one elected lane), which runs ahead into the next tile while the consumers drain theirs.
+// The epilogue moves 64 accumulator columns at a time through a shared-memory transpose ([64 rows][64 columns] fp32 per
+// warpgroup) so that a thread owns ONE pixel row and 32 consecutive channels: 16-byte bf16 stores and per-pixel statistics.
 // EPI 1 (forward): the epilogue also emits the GroupNorm input statistics of the tensor it writes (per sample and channel: sum
 // and sum of squares of the bf16-rounded outputs), so the consumer norm needs no statistics pass over HBM.
 // EPI 2 (data gradient of the conv that consumes a GroupNorm[+swish] output): the epilogue turns dy into the gradient w.r.t.
@@ -66,59 +66,44 @@ struct TcParams {
 // x and dy from HBM again (gn_bwd_reduce_kernel disappears for these norms).
 // EPI 3: the same for the FiLM norm of a ResnetBlock (model/xunet.py:82-84): dy -> dropout mask -> du = . * swish'(u) with
 // u = yhat*(1+scale)+shift, stores dyh = du*(1+scale) and the FiLM gradient [du*yhat | du], emits the same channel sums.
-// EW = epilogue warps: 4 (one per TMEM lane quadrant; small tiles, several CTAs per SM) or 8 (two per quadrant taking alternate
-// 32-column chunks; the one-CTA-per-SM big tiles).  With one warp per scheduler the ~770 dependent instructions of a 32-column chunk
-// (statistics included) issue at ~6 cycles each -- ncu: 26 us per 128 x 256 tile, longer than the 18 us main loop at K = 2304
-// (profiles/r02_conv_epilogue_ncu.md) -- so the big-tile variant doubles the warps (and gets the full register file: no spills).
-// The 4-warp variant is compiled for two CTAs per SM (<= 168 registers: no spills either); with three per SM (96 registers, 36-148
-// bytes of spills in the epilogue) the small-model step was 1.4 % slower (3.653 vs 3.600 ms, same call).
-template <int BK, int EPI, int EW>
-__global__ void __launch_bounds__(64 + 32 * EW, EW == 8 ? 1 : 2) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                      const __grid_constant__ CUtensorMap tmB,
-                                                      const __grid_constant__ CUtensorMap tmY, const TcParams p) {
+constexpr int kConvThreads = 288;      // two consumer warpgroups + one producer warp
+constexpr int kXP = 68;                // fp32 pitch of the transpose buffer (16-byte row reads without bank conflicts)
+// Two CTAs per SM (96 registers per thread) only for narrow tiles with the plain / statistics epilogues; the fused GroupNorm-
+// backward epilogues (EPI 2/3) need more registers and run one CTA per SM.
+__host__ __device__ constexpr int conv_ctas_per_sm(int epi, int bn) { return (bn <= 64 && epi < 2) ? 2 : 1; }
+template <int BK, int EPI, int BN>
+__global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                               const __grid_constant__ CUtensorMap tmB,
+                                                                               const __grid_constant__ CUtensorMap tmY, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  const int B_TILE = p.BN * BK * 2;
+  constexpr int B_TILE = BN * BK * 2;
   // halo mode: the A stage holds (TH+2) x TW pixels -- the dy = 0,1,2 operands are the 128-pixel windows starting
   // dy*TW rows in (dy*TW*BK*2 bytes: a whole number of swizzle atoms since TW % 8 == 0) -- and the B stage the 3 dy taps
-  const int A_BYTES = p.halo ? (p.TH * (1 + p.m2) + 2) * p.TW * BK * 2 : 128 * BK * 2;
+  const int A_BYTES = p.halo ? (p.TH + 2) * p.TW * BK * 2 : 128 * BK * 2;
   const int B_BYTES = p.halo ? 3 * B_TILE : B_TILE;
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* smA = base;
   uint8_t* smB = base + (size_t)p.stages * A_BYTES;
   uint8_t* smY = smB + (size_t)p.stages * B_BYTES;                       // 2 x [128][cws] bf16 staging (tma_store only)
   const int Y_BYTES = p.tma_store ? 128 * p.cws * 2 : 0;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smY + 2 * (size_t)Y_BYTES);
+  float* smT = reinterpret_cast<float*>(smY + 2 * (size_t)Y_BYTES);      // 2 x [64][kXP] fp32 transpose buffers
+  uint64_t* full = reinterpret_cast<uint64_t*>(smT + 2 * 64 * kXP);
   uint64_t* empty = full + p.stages;
-  uint64_t* tmem_full = empty + p.stages;     // [4]
-  uint64_t* tmem_empty = tmem_full + 4;       // [4]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_k = p.halo ? 3 * p.KC : p.T * p.KC;
-  const int nacc = p.nacc;                    // 1, 2 or 4 accumulator buffers of BN columns
-  const int UH = p.TH * (1 + p.m2);           // rows of output pixels per work unit
-  uint32_t ncols = 32;
-  while ((int)ncols < nacc * p.BN) ncols <<= 1;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 4; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 32 * EW); }
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // one arrival per consumer warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     if (p.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmY) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  xu_grid_dep_sync();     // PDL: everything above (barriers, TMEM) overlaps the previous kernel's tail
-  const uint32_t tmem_base = *tmem_slot;
+  xu_grid_dep_sync();     // PDL: everything above (barriers) overlaps the previous kernel's tail
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       // ===== TMA producer =====
       // activation coordinates of pipeline step `it` of tile `tile` (shared by the load and by the L2 prefetch cursor)
@@ -127,7 +112,7 @@ __global__ void __launch_bounds__(64 + 32 * EW, EW == 8 ? 1 : 2) conv_tc_kernel(
         int t = p.n_fast ? tile / p.n_tiles : tile - n_tile * p.m_tiles;
         const int tx = t % p.tiles_x; t /= p.tiles_x;
         const int ty = t % p.tiles_y; t /= p.tiles_y;
-        const int x0 = tx * p.TW, y0 = ty * UH;
+        const int x0 = tx * p.TW, y0 = ty * p.TH;
         cn = t * p.TN;
         const int tt = it / p.KC, c = it - tt * p.KC;
         if (p.halo) {
@@ -151,7 +136,7 @@ __global__ void __launch_bounds__(64 + 32 * EW, EW == 8 ? 1 : 2) conv_tc_kernel(
         int t = p.n_fast ? tile / p.n_tiles : tile - n_tile * p.m_tiles;
         const int tx = t % p.tiles_x; t /= p.tiles_x;
         const int ty = t % p.tiles_y; t /= p.tiles_y;
-        const int x0 = tx * p.TW, y0 = ty * UH, n0 = t * p.TN;
+        const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
         for (int it = 0; it < total_k; ++it, ++itg) {
           const int s = itg % p.stages;
           const uint32_t ph = (itg / p.stages) & 1;
@@ -177,8 +162,8 @@ __global__ void __launch_bounds__(64 + 32 * EW, EW == 8 ? 1 : 2) conv_tc_kernel(
             for (int j = 0; j < 3; ++j) {            // window j starts at input row y0 - 1 + j  <->  dy = j (dgrad: 2 - j)
               const int tap = (p.flip ? 2 - j : j) * 3 + tt;
               uint8_t* dst = smB + (size_t)s * B_BYTES + j * B_TILE;
-              if (p.b_mode == 0) tma_load_3d(dst, &tmB, &full[s], c * BK, tap, n_tile * p.BN);
-              else tma_load_3d(dst, &tmB, &full[s], c * BK, n_tile * p.BN, tap);
+              if (p.b_mode == 0) tma_load_3d(dst, &tmB, &full[s], c * BK, tap, n_tile * BN);
+              else tma_load_3d(dst, &tmB, &full[s], c * BK, n_tile * BN, tap);
             }
             continue;
           }
@@ -190,264 +175,261 @@ __global__ void __launch_bounds__(64 + 32 * EW, EW == 8 ? 1 : 2) conv_tc_kernel(
           }
           mbar_expect_tx(&full[s], A_BYTES + B_BYTES);
           tma_load_4d(smA + (size_t)s * A_BYTES, &tmA, &full[s], tt * p.a_seg_stride + c * BK, x0 * p.stride + ox, y0 * p.stride + oy, n0);
-          if (p.b_mode == 0) tma_load_3d(smB + (size_t)s * B_BYTES, &tmB, &full[s], c * BK, tt, n_tile * p.BN);
-          else tma_load_3d(smB + (size_t)s * B_BYTES, &tmB, &full[s], c * BK, n_tile * p.BN, tt);
+          if (p.b_mode == 0) tma_load_3d(smB + (size_t)s * B_BYTES, &tmB, &full[s], c * BK, tt, n_tile * BN);
+          else tma_load_3d(smB + (size_t)s * B_BYTES, &tmB, &full[s], c * BK, n_tile * BN, tt);
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      // instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-      // A,B K-major (bits 15,16 = 0), N>>3 [17,23), M>>4 [24,29)
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.BN >> 3) << 17) | ((128u >> 4) << 24);
-      int itg = 0, lt = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++lt) {
-        // accumulator buffer(s) of this unit: one, or (m2) one per 8-row half
-        const int lt0 = lt * (1 + p.m2);
-        const int buf = lt0 % nacc, buf1 = (lt0 + 1) % nacc;
-        mbar_wait(&tmem_empty[buf], (((lt0 / nacc) & 1) ^ 1));      // epilogue drained this accumulator
-        if (p.m2) mbar_wait(&tmem_empty[buf1], ((((lt0 + 1) / nacc) & 1) ^ 1));
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf * p.BN);
-        const uint32_t tmem_d1 = tmem_base + (uint32_t)(buf1 * p.BN);
-        for (int it = 0; it < total_k; ++it, ++itg) {
-          const int s = itg % p.stages;
-          const uint32_t ph = (itg / p.stages) & 1;
-          mbar_wait(&full[s], ph);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_u32(smA + (size_t)s * A_BYTES);
-          const uint32_t b_addr = smem_u32(smB + (size_t)s * B_BYTES);
-          if (p.halo) {
-            const uint32_t win = (uint32_t)(p.TW * BK * 2);
-#pragma unroll
-            for (int j = 0; j < 3; ++j)
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t db = make_kmajor_desc<BK>(b_addr + j * B_TILE + k * 32);
-                umma_bf16(tmem_d, make_kmajor_desc<BK>(a_addr + j * win + k * 32), db, idesc, (it > 0 || j > 0 || k > 0) ? 1u : 0u);
-                if (p.m2) umma_bf16(tmem_d1, make_kmajor_desc<BK>(a_addr + (p.TH + j) * win + k * 32), db, idesc, (it > 0 || j > 0 || k > 0) ? 1u : 0u);
-              }
-            umma_commit(&empty[s]);
-            continue;
-          }
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = make_kmajor_desc<BK>(a_addr + k * 32);
-            const uint64_t db = make_kmajor_desc<BK>(b_addr + k * 32);
-            umma_bf16(tmem_d, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty[s]);   // frees the smem stage once the MMAs above have consumed it
-        }
-        umma_commit(&tmem_full[buf]);   // accumulator(s) complete
-        if (p.m2) umma_commit(&tmem_full[buf1]);
       }
     }
   } else {
-    // ===== epilogue: warps 2.. own TMEM lanes 32*(warp%4) .. +31; with EW = 8 the two warps of a quadrant alternate chunks =====
-    const int ehalf = (warp - 2) >> 2;                   // 0, or 1 for the second warp of the quadrant
+    const int wg = warp >> 2;                            // consumer warpgroup: rows 64 wg .. 64 wg + 63 of the tile
+    const int wq = warp & 3;
+    const uint32_t a_row_off = (uint32_t)(wg * 64 * BK * 2);
+    // epilogue mapping: warp wq of the warpgroup owns pixel rows lane_base .. +31 and the 32-column half `ehalf` of every
+    // 64-column group
+    const int ehalf = wq >> 1;
     const bool bias_vec = (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0;   // leaf offsets are 16-byte aligned in the flat buffer; scalar loads otherwise
-    const int lane_base = (warp & 3) * 32;
+    const int lane_base = wg * 64 + (wq & 1) * 32;
     const int r = lane_base + lane;                      // row of the 128-pixel tile
     const int tw = r % p.TW;
     const int th = (r / p.TW) % p.TH;
     const int tn = r / (p.TW * p.TH);
-    const bool y_issuer = threadIdx.x == 64;              // first epilogue thread issues / retires the TMA stores
-    const int sub_per_box = p.cws >> 5;                   // 32-column chunks per staging box (1 or 2)
+    float* tbuf = smT + wg * 64 * kXP;
+    const int fr = wq * 16 + (lane >> 2), fc = (lane & 3) * 2;   // accumulator fragment: rows fr, fr + 8; columns 8 i + fc, + 1
+    const bool y_issuer = threadIdx.x == 0;               // first consumer thread issues / retires the TMA stores
     const int yswz = p.cws == 64 ? (r & 7) : ((r >> 1) & 3);
     int ybox = 0;                                         // running count of staging boxes (selects the buffer)
-    int lt = 0;
-    // (m2: the 8-row halves of a work unit are drained in the order the MMA lane fills their accumulators)
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x)
-    for (int half = 0; half <= p.m2; ++half, ++lt) {
-      const int buf = lt % nacc;
+    int itg = 0;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      // ===== main loop: wgmma over the ring =====
+      int prev_s = 0;
+      for (int it = 0; it < total_k; ++it, ++itg) {
+        const int s = itg % p.stages;
+        mbar_wait(&full[s], (itg / p.stages) & 1);
+        wgmma_fence();
+        const uint32_t a_addr = smem_u32(smA + (size_t)s * A_BYTES) + a_row_off;
+        const uint32_t b_addr = smem_u32(smB + (size_t)s * B_BYTES);
+        if (p.halo) {
+          const uint32_t win = (uint32_t)(p.TW * BK * 2);
+#pragma unroll
+          for (int j = 0; j < 3; ++j)
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+              Wgmma<BN>::template ss<0, 0>(acc, make_kmajor_desc<BK>(a_addr + j * win + k * 32),
+                                           make_kmajor_desc<BK>(b_addr + j * B_TILE + k * 32), (it > 0 || j > 0 || k > 0) ? 1u : 0u);
+        } else {
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k)
+            Wgmma<BN>::template ss<0, 0>(acc, make_kmajor_desc<BK>(a_addr + k * 32), make_kmajor_desc<BK>(b_addr + k * 32),
+                                         (it > 0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                 // the previous step's MMAs are done: release its stage
+        if (it > 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(&empty[prev_s]);
+
+      // ===== epilogue =====
       const int n_tile = p.n_fast ? tile % p.n_tiles : tile / p.m_tiles;
       int t = p.n_fast ? tile / p.n_tiles : tile - n_tile * p.m_tiles;
       const int tx = t % p.tiles_x; t /= p.tiles_x;
       const int ty = t % p.tiles_y; t /= p.tiles_y;
-      const int x0 = tx * p.TW, y0 = ty * UH + half * p.TH, n0 = t * p.TN;
-      mbar_wait(&tmem_full[buf], (lt / nacc) & 1);
-      tcgen05_fence_after();
+      const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
       const long long pix = ((long long)(n0 + tn) * p.H + (y0 + th)) * p.W + (x0 + tw);
-      bf16* yrow = p.y + pix * p.Co + (long long)n_tile * p.BN;
-      const bf16* rrow = p.res ? p.res + pix * p.Co + (long long)n_tile * p.BN : nullptr;
-      const float* brow = p.bias ? p.bias + (long long)n_tile * p.BN : nullptr;
-      const uint32_t tsrc = tmem_base + ((uint32_t)lane_base << 16) + (uint32_t)(buf * p.BN);
+      bf16* yrow = p.y + pix * p.Co + (long long)n_tile * BN;
+      const bf16* rrow = p.res ? p.res + pix * p.Co + (long long)n_tile * BN : nullptr;
+      const float* brow = p.bias ? p.bias + (long long)n_tile * BN : nullptr;
       // STATS: the 32 pixels of this warp belong to one sample (host-checked): b = image of the warp's first row / 2
-      float* cs_row = nullptr;
-      const long long srow = (long long)((n0 + lane_base / (p.TW * p.TH)) >> 1) * p.Co + (long long)n_tile * p.BN;
+      double* cs_row = nullptr;
+      const long long srow = (long long)((n0 + lane_base / (p.TW * p.TH)) >> 1) * p.Co + (long long)n_tile * BN;
       if constexpr (EPI != 0) cs_row = p.cstats + srow * 2;
       const bf16* gxrow = nullptr;
       const float4* gprow = nullptr;
-      if constexpr (EPI >= 2) { gxrow = p.gx + pix * p.Co + (long long)n_tile * p.BN; gprow = p.gnp + srow; }
+      if constexpr (EPI >= 2) { gxrow = p.gx + pix * p.Co + (long long)n_tile * BN; gprow = p.gnp + srow; }
       const bf16* gerow = nullptr;
       bf16* gderow = nullptr;
       unsigned long long dseed = 0ULL;
       if constexpr (EPI == 3) {
-        gerow = p.ge + pix * (2LL * p.Co) + (long long)n_tile * p.BN;
-        gderow = p.gde + pix * (2LL * p.Co) + (long long)n_tile * p.BN;
+        gerow = p.ge + pix * (2LL * p.Co) + (long long)n_tile * BN;
+        gderow = p.gde + pix * (2LL * p.Co) + (long long)n_tile * BN;
         if (p.drop_on) dseed = *p.seed_dev;
       }
-      for (int c0 = ehalf * 32; c0 < p.BN; c0 += 8 * EW) {
+#pragma unroll
+      for (int cc = 0; cc < BN; cc += 64) {
+        // accumulator columns cc .. cc + 63 of this warpgroup's 64 rows -> transpose buffer
+#pragma unroll
+        for (int i = 0; i < BN / 2; i += 4) {
+          const int col = 8 * (i / 4);
+          if (col >= cc && col < cc + 64) {
+            *reinterpret_cast<float2*>(tbuf + fr * kXP + col - cc + fc) = make_float2(acc[i], acc[i + 1]);
+            *reinterpret_cast<float2*>(tbuf + (fr + 8) * kXP + col - cc + fc) = make_float2(acc[i + 2], acc[i + 3]);
+          }
+        }
+        named_bar_sync(2 + wg, 128);
+        const int c0 = cc + ehalf * 32;
+        const bool active = c0 < BN;
         // the residual / accumulate operands of the whole 32-column chunk are requested before anything waits on them:
         // each is a 16-byte access of a (pixel-pitch strided) row, i.e. a DRAM-latency load per thread when issued one by one
         uint4 rv[4], ov[4];
-        if (EPI < 2 && rrow) {
+        if (active && EPI < 2 && rrow) {
 #pragma unroll
           for (int q = 0; q < 4; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(rrow + c0 + 8 * q));
         }
-        if (p.accumulate && !p.tma_store) {
+        if (active && p.accumulate && !p.tma_store) {
 #pragma unroll
           for (int q = 0; q < 4; ++q) ov[q] = *reinterpret_cast<const uint4*>(yrow + c0 + 8 * q);
         }
         if constexpr (EPI >= 2) {      // the GroupNorm input of this pixel (rv is free: a data gradient has no residual operand)
+          if (active) {
 #pragma unroll
-          for (int q = 0; q < 4; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(gxrow + c0 + 8 * q));
+            for (int q = 0; q < 4; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(gxrow + c0 + 8 * q));
+          }
         }
         uint4 scv[4], shv[4];
         if constexpr (EPI == 3) {
+          if (active) {
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            scv[q] = __ldg(reinterpret_cast<const uint4*>(gerow + c0 + 8 * q));
-            shv[q] = __ldg(reinterpret_cast<const uint4*>(gerow + p.Co + c0 + 8 * q));
+            for (int q = 0; q < 4; ++q) {
+              scv[q] = __ldg(reinterpret_cast<const uint4*>(gerow + c0 + 8 * q));
+              shv[q] = __ldg(reinterpret_cast<const uint4*>(gerow + p.Co + c0 + 8 * q));
+            }
           }
         }
-        uint32_t v[32];
-        tmem_ld32(tsrc + (uint32_t)c0, v);
-        const int ysub = (c0 >> 5) % sub_per_box;
+        float v[32];
+        if (active) {
+          const float* trow = tbuf + (r - wg * 64) * kXP + ehalf * 32;
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const float4 t4 = *reinterpret_cast<const float4*>(trow + 4 * q);
+            v[4 * q] = t4.x; v[4 * q + 1] = t4.y; v[4 * q + 2] = t4.z; v[4 * q + 3] = t4.w;
+          }
+        }
+        const int ysub = p.cws == 64 ? ehalf : 0;
         uint8_t* yst = smY + (size_t)(ybox & 1) * Y_BYTES + (size_t)r * (p.cws * 2);
-        // EW = 8 (64-column boxes only): the two warp groups fill the two halves of the same box in lockstep
-        if (p.tma_store && (EW == 8 || ysub == 0)) {
+        if (p.tma_store) {
           // the store that read this staging buffer two boxes ago must have finished reading before it is overwritten
           if (y_issuer) bulk_wait_group_read<1>();
-          named_bar_sync(1, 32 * EW);
+          named_bar_sync(1, 256);
         }
-        float sx[32];     // STATS only (dead otherwise)
+        if (active) {
+          float sx[32];     // STATS only (dead otherwise)
 #pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          float f[8];
-          if constexpr (EW == 8) {
-            // two broadcast 16-byte loads per 8 columns instead of eight 4-byte ones (the big-tile variant has the registers)
-            float4 bq0 = make_float4(0.f, 0.f, 0.f, 0.f), bq1 = bq0;
-            if (brow && bias_vec) { bq0 = __ldg(reinterpret_cast<const float4*>(brow + c0 + j)); bq1 = __ldg(reinterpret_cast<const float4*>(brow + c0 + j) + 1); }
-            else if (brow) { bq0 = make_float4(brow[c0 + j], brow[c0 + j + 1], brow[c0 + j + 2], brow[c0 + j + 3]); bq1 = make_float4(brow[c0 + j + 4], brow[c0 + j + 5], brow[c0 + j + 6], brow[c0 + j + 7]); }
-            const float bq[8] = {bq0.x, bq0.y, bq0.z, bq0.w, bq1.x, bq1.y, bq1.z, bq1.w};
+          for (int j = 0; j < 32; j += 8) {
+            float f[8];
+            {
+              float4 bq0 = make_float4(0.f, 0.f, 0.f, 0.f), bq1 = bq0;
+              if (brow && bias_vec) { bq0 = __ldg(reinterpret_cast<const float4*>(brow + c0 + j)); bq1 = __ldg(reinterpret_cast<const float4*>(brow + c0 + j) + 1); }
+              else if (brow) { bq0 = make_float4(brow[c0 + j], brow[c0 + j + 1], brow[c0 + j + 2], brow[c0 + j + 3]); bq1 = make_float4(brow[c0 + j + 4], brow[c0 + j + 5], brow[c0 + j + 6], brow[c0 + j + 7]); }
+              const float bq[8] = {bq0.x, bq0.y, bq0.z, bq0.w, bq1.x, bq1.y, bq1.z, bq1.w};
 #pragma unroll
-            for (int q = 0; q < 8; ++q) f[q] = __uint_as_float(v[j + q]) + bq[q];
-          } else {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) f[q] = __uint_as_float(v[j + q]) + (brow ? brow[c0 + j + q] : 0.f);
-          }
-          if (EPI < 2 && rrow) {
-            const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) { f[2 * q] += __low2float(r2[q]); f[2 * q + 1] += __high2float(r2[q]); }
-          }
-#pragma unroll
-          for (int q = 0; q < 8; ++q) f[q] *= p.alpha;
-          float xh[8];
-          if constexpr (EPI == 2) {
-            const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 pp = __ldg(gprow + c0 + j + q);
-              const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
-              xh[q] = fmaf(xv, pp.x, pp.y);
-              if (p.gn_swish) f[q] *= swish_gradf_(fmaf(xh[q], pp.z, pp.w));
+              for (int q = 0; q < 8; ++q) f[q] = v[j + q] + bq[q];
             }
-          }
-          if constexpr (EPI == 3) {
-            const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
-            const __nv_bfloat162* s2 = reinterpret_cast<const __nv_bfloat162*>(&scv[j >> 3]);
-            const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&shv[j >> 3]);
-            const long long e0 = pix * p.Co + (long long)n_tile * p.BN + c0 + j;      // element index of column j in (N,H,W,Co)
-            uint32_t km = 0xFFu;
-            if (p.drop_on) km = xu_keep4(dseed, p.drop_op, (unsigned long long)e0 >> 2, p.drop_rate) |
-                                (xu_keep4(dseed, p.drop_op, ((unsigned long long)e0 >> 2) + 1, p.drop_rate) << 4);
-            const float keep_scale = 1.f / (1.f - p.drop_rate);
-            uint4 dsc, dsh;
-            __nv_bfloat162* dsc2 = reinterpret_cast<__nv_bfloat162*>(&dsc);
-            __nv_bfloat162* dsh2 = reinterpret_cast<__nv_bfloat162*>(&dsh);
-            float tsc[8], tsh[8];
+            if (EPI < 2 && rrow) {
+              const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 pp = __ldg(gprow + c0 + j + q);
-              const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
-              const float sc = (q & 1) ? __high2float(s2[q >> 1]) : __low2float(s2[q >> 1]);
-              const float sh = (q & 1) ? __high2float(h2[q >> 1]) : __low2float(h2[q >> 1]);
-              xh[q] = fmaf(xv, pp.x, pp.y);
-              const float yh = fmaf(xh[q], pp.z, pp.w);
-              const float u = fmaf(yh, 1.f + sc, sh);
-              float gs = f[q];
-              if (p.drop_on) gs = ((km >> q) & 1u) ? gs * keep_scale : 0.f;
-              const float du = gs * swish_gradf_(u);
-              f[q] = du * (1.f + sc);
-              tsc[q] = du * yh;
-              tsh[q] = du;
+              for (int q = 0; q < 4; ++q) { f[2 * q] += __low2float(r2[q]); f[2 * q + 1] += __high2float(r2[q]); }
             }
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              dsc2[q] = __floats2bfloat162_rn(tsc[2 * q], tsc[2 * q + 1]);
-              dsh2[q] = __floats2bfloat162_rn(tsh[2 * q], tsh[2 * q + 1]);
+            for (int q = 0; q < 8; ++q) f[q] *= p.alpha;
+            float xh[8];
+            if constexpr (EPI == 2) {
+              const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
+#pragma unroll
+              for (int q = 0; q < 8; ++q) {
+                const float4 pp = __ldg(gprow + c0 + j + q);
+                const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
+                xh[q] = fmaf(xv, pp.x, pp.y);
+                if (p.gn_swish) f[q] *= swish_gradf_(fmaf(xh[q], pp.z, pp.w));
+              }
             }
-            *reinterpret_cast<uint4*>(gderow + c0 + j) = dsc;
-            *reinterpret_cast<uint4*>(gderow + p.Co + c0 + j) = dsh;
-          }
-          if (p.accumulate && !p.tma_store) {
-            const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&ov[j >> 3]);
+            if constexpr (EPI == 3) {
+              const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
+              const __nv_bfloat162* s2 = reinterpret_cast<const __nv_bfloat162*>(&scv[j >> 3]);
+              const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&shv[j >> 3]);
+              const long long e0 = pix * p.Co + (long long)n_tile * BN + c0 + j;      // element index of column j in (N,H,W,Co)
+              uint32_t km = 0xFFu;
+              if (p.drop_on) km = xu_keep4(dseed, p.drop_op, (unsigned long long)e0 >> 2, p.drop_rate) |
+                                  (xu_keep4(dseed, p.drop_op, ((unsigned long long)e0 >> 2) + 1, p.drop_rate) << 4);
+              const float keep_scale = 1.f / (1.f - p.drop_rate);
+              uint4 dsc, dsh;
+              __nv_bfloat162* dsc2 = reinterpret_cast<__nv_bfloat162*>(&dsc);
+              __nv_bfloat162* dsh2 = reinterpret_cast<__nv_bfloat162*>(&dsh);
+              float tsc[8], tsh[8];
 #pragma unroll
-            for (int q = 0; q < 4; ++q) { f[2 * q] += __low2float(o2[q]); f[2 * q + 1] += __high2float(o2[q]); }
-          }
-          uint4 outv;
-          __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&outv);
+              for (int q = 0; q < 8; ++q) {
+                const float4 pp = __ldg(gprow + c0 + j + q);
+                const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
+                const float sc = (q & 1) ? __high2float(s2[q >> 1]) : __low2float(s2[q >> 1]);
+                const float sh = (q & 1) ? __high2float(h2[q >> 1]) : __low2float(h2[q >> 1]);
+                xh[q] = fmaf(xv, pp.x, pp.y);
+                const float yh = fmaf(xh[q], pp.z, pp.w);
+                const float u = fmaf(yh, 1.f + sc, sh);
+                float gs = f[q];
+                if (p.drop_on) gs = ((km >> q) & 1u) ? gs * keep_scale : 0.f;
+                const float du = gs * swish_gradf_(u);
+                f[q] = du * (1.f + sc);
+                tsc[q] = du * yh;
+                tsh[q] = du;
+              }
 #pragma unroll
-          for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(f[2 * q], f[2 * q + 1]);
-          if (p.tma_store) sts128(yst + ((((ysub << 2) + (j >> 3)) ^ yswz) << 4), outv);
-          else *reinterpret_cast<uint4*>(yrow + c0 + j) = outv;
-          if constexpr (EPI >= 2) {
-            // sums over what is STORED (the second pass reads the rounded dyh back)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float a = __low2float(o2[q]), b = __high2float(o2[q]);
-              sx[(j & 8) + 2 * q] = a * xh[2 * q];   sx[(j & 8) + 2 * q + 1] = b * xh[2 * q + 1];
-              sx[16 + (j & 8) + 2 * q] = a;          sx[16 + (j & 8) + 2 * q + 1] = b;
+              for (int q = 0; q < 4; ++q) {
+                dsc2[q] = __floats2bfloat162_rn(tsc[2 * q], tsc[2 * q + 1]);
+                dsh2[q] = __floats2bfloat162_rn(tsh[2 * q], tsh[2 * q + 1]);
+              }
+              *reinterpret_cast<uint4*>(gderow + c0 + j) = dsc;
+              *reinterpret_cast<uint4*>(gderow + p.Co + c0 + j) = dsh;
             }
-            if (j & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
-          }
-          if constexpr (EPI == 1) {
-            // statistics of what is STORED (rounded), so the consumer's normalisation is exactly zero-mean / unit-variance
+            if (p.accumulate && !p.tma_store) {
+              const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&ov[j >> 3]);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float a = __low2float(o2[q]), b = __high2float(o2[q]);
-              sx[(j & 8) + 2 * q] = a;            sx[(j & 8) + 2 * q + 1] = b;
-              sx[16 + (j & 8) + 2 * q] = a * a;   sx[16 + (j & 8) + 2 * q + 1] = b * b;
+              for (int q = 0; q < 4; ++q) { f[2 * q] += __low2float(o2[q]); f[2 * q + 1] += __high2float(o2[q]); }
             }
-            if (j & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
+            uint4 outv;
+            __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&outv);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(f[2 * q], f[2 * q + 1]);
+            if (p.tma_store) sts128(yst + ((((ysub << 2) + (j >> 3)) ^ yswz) << 4), outv);
+            else *reinterpret_cast<uint4*>(yrow + c0 + j) = outv;
+            if constexpr (EPI >= 2) {
+              // sums over what is STORED (the second pass reads the rounded dyh back)
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float a = __low2float(o2[q]), b = __high2float(o2[q]);
+                sx[(j & 8) + 2 * q] = a * xh[2 * q];   sx[(j & 8) + 2 * q + 1] = b * xh[2 * q + 1];
+                sx[16 + (j & 8) + 2 * q] = a;          sx[16 + (j & 8) + 2 * q + 1] = b;
+              }
+              if (j & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
+            }
+            if constexpr (EPI == 1) {
+              // statistics of what is STORED (rounded), so the consumer's normalisation is exactly zero-mean / unit-variance
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float a = __low2float(o2[q]), b = __high2float(o2[q]);
+                sx[(j & 8) + 2 * q] = a;            sx[(j & 8) + 2 * q + 1] = b;
+                sx[16 + (j & 8) + 2 * q] = a * a;   sx[16 + (j & 8) + 2 * q + 1] = b * b;
+              }
+              if (j & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
+            }
           }
         }
-        if (p.tma_store && (EW == 8 || ysub == sub_per_box - 1)) {
+        if (p.tma_store) {
           fence_async_smem();                 // generic-proxy writes -> visible to the TMA unit
-          named_bar_sync(1, 32 * EW);
+          named_bar_sync(1, 256);
           if (y_issuer) {
             // accumulate: the gradient is ADDED to the destination by the TMA unit (cp.reduce.async.bulk.tensor .add, bf16 at L2)
-            if (p.accumulate) tma_reduce_add_4d(smY + (size_t)(ybox & 1) * Y_BYTES, &tmY, n_tile * p.BN + c0 - (ysub << 5), x0, y0, n0);
-            else tma_store_4d(smY + (size_t)(ybox & 1) * Y_BYTES, &tmY, n_tile * p.BN + c0 - (ysub << 5), x0, y0, n0);
+            if (p.accumulate) tma_reduce_add_4d(smY + (size_t)(ybox & 1) * Y_BYTES, &tmY, n_tile * BN + cc, x0, y0, n0);
+            else tma_store_4d(smY + (size_t)(ybox & 1) * Y_BYTES, &tmY, n_tile * BN + cc, x0, y0, n0);
             bulk_commit_group();
           }
           ++ybox;
         }
+        named_bar_sync(2 + wg, 128);        // transpose buffer read by every warp before the next group overwrites it
       }
-      tcgen05_fence_before();
-      mbar_arrive(&tmem_empty[buf]);     // hand the accumulator back to the MMA lane
     }
   }
-  if (p.tma_store && threadIdx.x == 64) bulk_wait_group<0>();   // all output boxes written before the CTA retires
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
-  }
+  if (p.tma_store && threadIdx.x == 0) bulk_wait_group<0>();   // all output boxes written before the CTA retires
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -515,21 +497,22 @@ bool pick_tile(int N, int H, int W, int& TW, int& TH, int& TN) {
 // together), which beats 16-wide chunks by 3x fewer pipeline stages.
 int pick_bk(int K) { return K % 64 == 0 ? 64 : (K % 32 == 0 ? 32 : (K % 16 == 0 ? (K > 64 ? 64 : 16) : 0)); }
 
-template <int BK, int EPI, int EW>
-void launch_tc_ew(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& y, const TcParams& p, dim3 grid, cudaStream_t s) {
-  const size_t stage = p.halo ? (size_t)(p.TH * (1 + p.m2) + 2) * p.TW * BK * 2 + (size_t)3 * p.BN * BK * 2 : (size_t)128 * BK * 2 + (size_t)p.BN * BK * 2;
-  const size_t smem = stage * p.stages + (p.tma_store ? (size_t)2 * 128 * p.cws * 2 : 0) + 1024 + 8 * (2 * p.stages + 8) + 16;
-  static size_t configured = 0;
-  if (smem > configured) {
-    cudaFuncSetAttribute(conv_tc_kernel<BK, EPI, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(220 * 1024));
-    configured = 220 * 1024;
+template <int BK, int EPI, int BN>
+void launch_tc_bn(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& y, const TcParams& p, size_t smem, dim3 grid, cudaStream_t s) {
+  static bool configured = false;
+  if (!configured) {
+    cudaFuncSetAttribute(conv_tc_kernel<BK, EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    configured = true;
   }
-  xu_launch(conv_tc_kernel<BK, EPI, EW>, grid, 64 + 32 * EW, smem, s, a, b, y, p);
+  xu_launch(conv_tc_kernel<BK, EPI, BN>, grid, kConvThreads, smem, s, a, b, y, p);
 }
 template <int BK, int EPI>
-void launch_tc(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& y, const TcParams& p, dim3 grid, cudaStream_t s) {
-  if (p.ew == 8) launch_tc_ew<BK, EPI, 8>(a, b, y, p, grid, s);
-  else launch_tc_ew<BK, EPI, 4>(a, b, y, p, grid, s);
+void launch_tc(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& y, const TcParams& p, size_t smem, dim3 grid, cudaStream_t s) {
+  switch (p.BN) {
+    case 128: launch_tc_bn<BK, EPI, 128>(a, b, y, p, smem, grid, s); break;
+    case 64: launch_tc_bn<BK, EPI, 64>(a, b, y, p, smem, grid, s); break;
+    default: launch_tc_bn<BK, EPI, 32>(a, b, y, p, smem, grid, s); break;
+  }
 }
 
 }  // namespace
@@ -541,8 +524,7 @@ __global__ void __launch_bounds__(256) weight_prep_kernel(const float* __restric
                                                           const __grid_constant__ WeightPrepTable tab) {
   xu_grid_dep_sync();
   // one block = one 64 (ci) x 64 (co) tile of one (segment, tap) slab: 16-byte reads along co, 8-byte writes of the plain cast,
-  // 16-byte writes of the transposed shadow along ci.  (Round 1 moved 32x32 tiles with 4-byte reads and 2-byte writes: 2.06 TB/s of
-  // DRAM traffic under ncu, 1.7 ms per step at the 3DiM widths -- profiles/r02_membound_ncu.md.)
+  // 16-byte writes of the transposed shadow along ci.
   __shared__ float tile[64][65];
   const long long t = blockIdx.x;
   int lo = 0, hi = tab.n - 1;
@@ -667,17 +649,15 @@ bool conv_tc_stats_supported(int mode, int N, int Ho, int Wo) {
 
 // a: the generic ConvArgs (mode 0 forward: x -> y;  mode 1 dgrad: a.x = dY (N,H,W,wCo), a.y = dX (N,H,W,wCi)).
 // wshadow: forward -> wT [wCo][taps][wCi];  dgrad -> wC [seg|tap][wCi][segw]
-// N-split rule: BN is halved while the tile count stays below a threshold, in quarters of the SM count.  Measured per shape inside
-// the full-128^2 step (profiles/r02_late_ab.md): a 256-wide tile wants a full wave (32^2 512->512: 256 tiles of BN 128 beat 128 tiles
-// of BN 256), but with a long reduction going below 128 columns only pays under 3/4 of a wave (16^2 1024->1024: 128 tiles of BN 128
-// run 88 us, 256 tiles of BN 64 116 us -- the 64-column MMA is bound by fetching A).  Short reductions (the small model: K <= 1152) are
-// latency-bound and keep the full-wave rule at every width (3.82 vs 3.91 ms/step).  XUNET_CONV_BN_QUARTERS=n forces one threshold.
+// N-split rule: BN is halved while the tile count stays below a threshold, in quarters of the SM count: with a long reduction a
+// narrower tile only pays under 3/4 of a wave (the narrow MMA is bound by fetching A), short reductions are latency-bound and take
+// the full-wave rule.  XUNET_CONV_BN_QUARTERS=n forces one threshold.
 static int bn_rule(int bn, int k_total) {
   static const char* env = getenv("XUNET_CONV_BN_QUARTERS");
   return env ? atoi(env) : ((bn > 128 || k_total < 2048) ? 4 : 3);
 }
 
-void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
+static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* cacc, cudaStream_t s) {
   const int taps = a.ks * a.ks;
   const int nseg = a.wCo / a.segw;
   int TW, TH, TN;
@@ -700,36 +680,19 @@ void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
   const int Kdim = a.mode == 0 ? a.wCi : a.segw;      // reduction channels per tap (and segment)
   const int Ndim = a.mode == 0 ? a.wCo : a.wCi;       // GEMM N
   bk = pick_bk(Kdim);
-  p.BN = Ndim <= 256 ? Ndim : 256;
+  // wgmma N of the kernel: 128, 64 or 32 (the largest that divides the GEMM N).  A 256-column tile would need 128 accumulator
+  // registers per thread next to the epilogue's: ptxas caps this 9-warp kernel at 168 and spills ~10 KB per thread.
+  p.BN = Ndim % 128 == 0 ? 128 : (Ndim % 64 == 0 ? 64 : 32);
   // small problems are latency-bound: split N so that at least ~one wave of CTAs exists
   { const long long mt = (long long)p.tiles_x * p.tiles_y * (a.N / TN);
     while (p.BN >= 64 && (p.BN / 2) % 32 == 0 && mt * (a.Co / p.BN) * 4 < xu_num_sms() * bn_rule(p.BN, taps * Kdim)) p.BN /= 2; }
-  // the halo stage (A: 160 pixels, B: 3 taps) must leave room for a >= 3-deep ring.  With BN = 256 a 64-channel stage is 116 KB;
-  // a 32-channel stage (58 KB, 3 stages) keeps the halo trick for the widest tiles: the activation tile is then fetched 3.75x
-  // instead of 9x per output tile (these convolutions are L2->SM bandwidth-bound: 1.73 MB of operands per 128 x 256 tile against
-  // 18.4 k MMA cycles = 94 B/clk/SM).  XUNET_CONV_HALO_BK32=0 restores the 9-tap ring for them.
+  // the halo stage (A: 160 pixels, B: 3 taps) must leave room for a >= 3-deep ring; a 32-channel stage keeps the halo trick for the
+  // widest tiles, so the activation tile is fetched 3.75x instead of 9x per output tile (wide convolutions are bound by the L2->SM
+  // operand stream).  XUNET_CONV_HALO_BK32=0 restores the 9-tap ring for them.
   if (halo && (size_t)(160 * bk * 2 + 3 * p.BN * bk * 2) > (size_t)56 * 1024) {
     static const char* e32 = getenv("XUNET_CONV_HALO_BK32");
     if (bk == 64 && !(e32 && e32[0] == '0') && (size_t)(160 * 32 * 2 + 3 * p.BN * 32 * 2) <= (size_t)72 * 1024) bk = 32;
     else halo = false;
-  }
-  // pair units (m2): wide 3x3 convolutions are bound by the L2->SM operand stream, not by the tensor pipe (256->256 @128^2: 1.73 MB of
-  // A+B per 128 x 256 tile against 18.4 k MMA cycles = 94 B/clk/SM, the chip delivers ~40).  Two vertically adjacent 8 x 16 tiles
-  // share every weight fetch and one 18-row halo box: 1.03 MB per tile-equivalent with BN = 128 (four accumulators: the epilogue
-  // of one unit still overlaps the main loop of the next), 0.81 MB with BN = 256 (XUNET_CONV_M2_BN=256; accumulators single-
-  // buffered).  Only where the reduction is wide and the unit count fills the machine.  XUNET_CONV_M2=1 turns it on (experimental).
-  p.m2 = 0;
-  {
-    const char* em2 = getenv("XUNET_CONV_M2");        // read per launch (tests flip it inside one process)
-    const char* ebn = getenv("XUNET_CONV_M2_BN");
-    const bool halo_shape = !no_halo && a.ks == 3 && a.stride == 1 && nseg == 1 && a.pad_h == 1 && a.pad_w == 1 && a.Wo % 16 == 0 &&
-                            a.Hi == a.Ho && a.Wi == a.Wo;
-    const int bn2 = std::min(Ndim, ebn ? atoi(ebn) : 128);
-    if ((em2 && em2[0] == '1') && halo_shape && a.Ho % 16 == 0 && Kdim >= 256 && Kdim % 32 == 0 && (bn2 == 128 || bn2 == 256) &&
-        Ndim % bn2 == 0) {
-      const long long units = (long long)(a.Wo / 16) * (a.Ho / 16) * a.N * (Ndim / bn2);
-      if (units * 2 >= (long long)xu_num_sms() * 3) { p.m2 = 1; halo = true; bk = 32; p.BN = bn2; }
-    }
   }
   if (a.mode == 0) {
     p.T = taps; p.KC = (a.wCi + bk - 1) / bk; p.flip = 0; p.a_seg_stride = 0; p.b_mode = 0;
@@ -744,8 +707,8 @@ void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
     uint32_t bb[3] = {(uint32_t)bk, (uint32_t)p.BN, 1u};
     if (!encode_bf16(&tmB, wshadow, 3, bd, bs, bb, bk)) return;
   }
-  if (halo) { TW = 16; TH = 8; TN = 1; p.TW = TW; p.TH = TH; p.TN = TN; p.tiles_x = a.Wo / TW; p.tiles_y = a.Ho / (TH * (1 + p.m2)); }
-  const int box_rows = halo ? TH * (1 + p.m2) + 2 : TH;
+  if (halo) { TW = 16; TH = 8; TN = 1; p.TW = TW; p.TH = TH; p.TN = TN; p.tiles_x = a.Wo / TW; p.tiles_y = a.Ho / TH; }
+  const int box_rows = halo ? TH + 2 : TH;
   p.halo = halo ? 1 : 0;
   uint64_t ad[4] = {(uint64_t)Ca, (uint64_t)a.Wi, (uint64_t)a.Hi, (uint64_t)a.N};
   uint64_t as[3] = {(uint64_t)Ca * 2, (uint64_t)a.Wi * Ca * 2, (uint64_t)a.Hi * a.Wi * Ca * 2};
@@ -759,8 +722,8 @@ void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
   CUtensorMap tmY = tmA;
   {
     static const char* env = getenv("XUNET_CONV_TMA_STORE");
-    // measured (profiles/r02_conv_epilogue_tma_store.md): the per-pixel GEMMs gain (1024->512 @128^2: 594 -> 881 TFLOP/s in the same
-    // call), the K-heavy 3x3 convolutions lose the pipeline stage the staging buffer costs -> default on for forward 1x1 only
+    // the per-pixel GEMMs gain from the staged store, the K-heavy 3x3 convolutions lose the pipeline stage the staging buffer
+    // costs -> default on for forward 1x1 only
     p.tma_store = (!a.accumulate && ((env && env[0] == '1') || (!env && a.ks == 1 && a.mode == 0))) ? 1 : 0;
     // accumulating data gradients (the FiLM Dense gradients summing into the embedding gradient): staged tile + TMA reduce-add
     // instead of a 16-byte read-modify-write per thread (XUNET_CONV_TMA_REDUCE=0 restores it)
@@ -776,45 +739,38 @@ void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
   }
   const size_t ystage = p.tma_store ? (size_t)2 * 128 * p.cws * 2 : 0;
   {
-    // optional L2 prefetch of the activation boxes ahead of the ring (XUNET_TMA_PREFETCH=n steps).  Measured and rejected as a
-    // default (profiles/r02_l2_prefetch.md): cp.async.bulk.prefetch.tensor ahead of every load made every large conv SLOWER
-    // (256->256 @128^2 forward 1054 -> 622 TFLOP/s, full-128^2 step 65.8 -> 78.6 ms)
+    // optional L2 prefetch of the activation boxes ahead of the ring (XUNET_TMA_PREFETCH=n steps; off by default)
     static const char* env = getenv("XUNET_TMA_PREFETCH");
     p.prefetch = env ? atoi(env) : 0;
   }
   p.n_tiles = a.Co / p.BN;
   p.m_tiles = p.tiles_x * p.tiles_y * (a.N / TN);
   p.total_tiles = p.m_tiles * p.n_tiles;
-  p.nacc = (2 * p.BN <= 512) ? 2 : 1;
-  if (p.m2) p.nacc = 512 / p.BN;       // 4 (BN = 128) or 2 (BN = 256): always a whole number of pairs
   {
     // with several n-tiles the activation tensor is read once per n-tile: keep those reads adjacent in time (L2 hits) when
     // the activations are the larger operand (XUNET_CONV_TILE_ORDER=m|n forces one order)
     static const char* ord = getenv("XUNET_CONV_TILE_ORDER");
     const double act_bytes = (double)a.N * a.Hi * a.Wi * a.Ci * 2.0, w_bytes = (double)taps * a.wCi * a.wCo * 2.0;
-    // measured (profiles/r02_conv_tile_order.md): m-fastest wins on every full-model shape, 1x1 included (834 vs 754 TFLOP/s at
-    // 1024->512 @128^2): the default stays m-fastest, the switch stays for the record
+    // default m-fastest (the CTAs in flight share one weight slab); the switch selects the other order
     (void)act_bytes; (void)w_bytes;
     p.n_fast = 0;
     if (ord && ord[0] == 'm') p.n_fast = 0;
     if (ord && ord[0] == 'n') p.n_fast = p.n_tiles > 1 ? 1 : 0;
   }
-  uint32_t ncols = 32;
-  while ((int)ncols < p.nacc * p.BN) ncols <<= 1;
-  // CTAs per SM: as many as TMEM (512 columns) and shared memory allow while keeping a >= 3-deep TMA ring; one persistent
-  // CTA per SM with a 4-deep ring otherwise (big tiles)
+  // CTAs per SM: two where the kernel is compiled for it (conv_ctas_per_sm) and shared
+  // memory keeps a >= 3-deep TMA ring for each; one persistent CTA per SM with a 4-deep ring otherwise
+  const size_t fixed = ystage + (size_t)2 * 64 * kXP * 4 + 1024 + 256;
   int per_sm = 1, stages = 2;
-  // (at most two: the kernels are compiled for two resident CTAs per SM; a grid of 3-4 per SM with the extra CTAs queued was measured
-  // 1.3 % slower on the small model than a 2-per-SM persistent grid with deeper rings: 3.600 vs 3.552 ms, same call)
-  for (int cand = 2; cand >= 1; --cand) {
-    if (cand > (int)(512 / ncols)) continue;
-    int st = (int)(((size_t)(220 * 1024) / cand - 2048 - ystage) / stage);
+  for (int cand = conv_ctas_per_sm(a.gn_x != nullptr ? 2 : 0, p.BN); cand >= 1; --cand) {
+    const size_t budget = cand == 1 ? (size_t)227 * 1024 : (size_t)112 * 1024;
+    int st = (int)((budget - fixed) / stage);
     if (st > 6) st = 6;
     if (st >= 3 || cand == 1) { per_sm = cand; stages = st < 1 ? 1 : st; break; }
   }
   if (per_sm == 1 && stages > 4) stages = 4;
   if (stages > total && total >= 2) stages = total;
   p.stages = stages;
+  const size_t smem = stage * stages + fixed + 8 * 2 * stages;
   int ctas = xu_num_sms() * per_sm;
   {
     static int cap = -1;   // experiment knob: XUNET_CONV_CTAS_PER_SM limits the persistent grid (more tiles per CTA)
@@ -824,16 +780,11 @@ void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
   if (ctas > p.total_tiles) ctas = p.total_tiles;
   dim3 grid((unsigned)ctas);
   {
-    // eight epilogue warps where one CTA owns the SM (wide tiles: TMEM / shared memory allow no second CTA); XUNET_CONV_EW8=0: four
-    static const char* e8 = getenv("XUNET_CONV_EW8");
-    p.ew = (per_sm == 1 && p.BN >= 128 && !(p.tma_store && p.cws != 64) && !(e8 && e8[0] == '0')) ? 8 : 4;
-  }
-  {
     static const bool log = getenv("XUNET_CONV_LOG") != nullptr;
-    if (log) fprintf(stderr, "conv_tc mode=%d N=%d %dx%d Ci=%d Co=%d ks=%d st=%d wCi=%d wCo=%d segw=%d bk=%d BN=%d KC=%d T=%d halo=%d m2=%d stages=%d per_sm=%d ctas=%d tiles=%d nacc=%d\n",
-                     a.mode, a.N, a.Ho, a.Wo, a.Ci, a.Co, a.ks, a.stride, a.wCi, a.wCo, a.segw, bk, p.BN, p.KC, p.T, p.halo, p.m2, p.stages, per_sm, ctas, p.total_tiles, p.nacc);
+    if (log) fprintf(stderr, "conv_tc mode=%d N=%d %dx%d Ci=%d Co=%d ks=%d st=%d wCi=%d wCo=%d segw=%d bk=%d BN=%d KC=%d T=%d halo=%d stages=%d per_sm=%d ctas=%d tiles=%d\n",
+                     a.mode, a.N, a.Ho, a.Wo, a.Ci, a.Co, a.ks, a.stride, a.wCi, a.wCo, a.segw, bk, p.BN, p.KC, p.T, p.halo, p.stages, per_sm, ctas, p.total_tiles);
   }
-  p.cstats = a.cstats;
+  p.cstats = cacc;
   p.gx = reinterpret_cast<const bf16*>(a.gn_x); p.gnp = reinterpret_cast<const float4*>(a.gn_params); p.gn_swish = a.gn_swish;
   const bool warp_in_sample = p.TW * p.TH >= 32 || (p.TW * p.TH == 16 && p.TN % 2 == 0);
   if (a.cstats != nullptr && a.gn_x == nullptr) {
@@ -841,9 +792,9 @@ void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
       xu_set_kernel_error("conv_tc: fused GroupNorm statistics requested for an unsupported tile shape");
       return;
     }
-    if (bk == 64) launch_tc<64, 1>(tmA, tmB, tmY, p, grid, s);
-    else if (bk == 32) launch_tc<32, 1>(tmA, tmB, tmY, p, grid, s);
-    else launch_tc<16, 1>(tmA, tmB, tmY, p, grid, s);
+    if (bk == 64) launch_tc<64, 1>(tmA, tmB, tmY, p, smem, grid, s);
+    else if (bk == 32) launch_tc<32, 1>(tmA, tmB, tmY, p, smem, grid, s);
+    else launch_tc<16, 1>(tmA, tmB, tmY, p, smem, grid, s);
     return;
   }
   p.ge = reinterpret_cast<const bf16*>(a.gn_e); p.gde = reinterpret_cast<bf16*>(a.gn_de);
@@ -854,21 +805,30 @@ void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
       xu_set_kernel_error("conv_tc: fused GroupNorm backward requested for an unsupported configuration");
       return;
     }
-    // these epilogues run at 168 registers per thread = two resident CTAs per SM: let the persistent loop take the rest
-    if ((int)grid.x > 2 * xu_num_sms()) grid.x = (unsigned)(2 * xu_num_sms());
+    // persistent grid: at most the CTAs that can be resident at once, the loop takes the rest
+    if ((int)grid.x > per_sm * xu_num_sms()) grid.x = (unsigned)(per_sm * xu_num_sms());
     if (a.gn_e != nullptr) {
       if (a.gn_de == nullptr) { xu_set_kernel_error("conv_tc: fused FiLM backward needs the FiLM gradient buffer"); return; }
-      if (bk == 64) launch_tc<64, 3>(tmA, tmB, tmY, p, grid, s);
-      else if (bk == 32) launch_tc<32, 3>(tmA, tmB, tmY, p, grid, s);
-      else launch_tc<16, 3>(tmA, tmB, tmY, p, grid, s);
+      if (bk == 64) launch_tc<64, 3>(tmA, tmB, tmY, p, smem, grid, s);
+      else if (bk == 32) launch_tc<32, 3>(tmA, tmB, tmY, p, smem, grid, s);
+      else launch_tc<16, 3>(tmA, tmB, tmY, p, smem, grid, s);
       return;
     }
-    if (bk == 64) launch_tc<64, 2>(tmA, tmB, tmY, p, grid, s);
-    else if (bk == 32) launch_tc<32, 2>(tmA, tmB, tmY, p, grid, s);
-    else launch_tc<16, 2>(tmA, tmB, tmY, p, grid, s);
+    if (bk == 64) launch_tc<64, 2>(tmA, tmB, tmY, p, smem, grid, s);
+    else if (bk == 32) launch_tc<32, 2>(tmA, tmB, tmY, p, smem, grid, s);
+    else launch_tc<16, 2>(tmA, tmB, tmY, p, smem, grid, s);
     return;
   }
-  if (bk == 64) launch_tc<64, 0>(tmA, tmB, tmY, p, grid, s);
-  else if (bk == 32) launch_tc<32, 0>(tmA, tmB, tmY, p, grid, s);
-  else launch_tc<16, 0>(tmA, tmB, tmY, p, grid, s);
+  if (bk == 64) launch_tc<64, 0>(tmA, tmB, tmY, p, smem, grid, s);
+  else if (bk == 32) launch_tc<32, 0>(tmA, tmB, tmY, p, smem, grid, s);
+  else launch_tc<16, 0>(tmA, tmB, tmY, p, smem, grid, s);
+}
+
+// the epilogue statistics (a.cstats, (N/2, Co, 2)) are summed in fp64 and folded in once, independent of the tile order
+void launch_conv_tc(const ConvArgs& a, const void* wshadow, cudaStream_t s) {
+  const long long n = a.cstats ? (long long)(a.N / 2) * a.Co * 2 : 0;
+  double* cacc = nullptr;
+  if (n > 0 && (cacc = xu_det_scratch(s, n)) == nullptr) return;
+  launch_conv_tc_impl(a, wshadow, cacc, s);
+  if (cacc != nullptr) xu_det_fold(a.cstats, cacc, n, s);
 }

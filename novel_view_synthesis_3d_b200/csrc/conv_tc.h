@@ -1,4 +1,4 @@
-// conv_tc.h -- tcgen05/TMEM/TMA implicit-GEMM convolution (bf16 in, fp32 accumulate in TMEM) + bf16 weight shadows.
+// conv_tc.h -- wgmma/TMA implicit-GEMM convolution (bf16 in, fp32 accumulate in registers) + bf16 weight shadows.
 #pragma once
 #include "kernels.h"
 
@@ -19,7 +19,7 @@ struct WeightPrepTable {
 };
 void launch_weight_prep(const WeightPrepTable& tab, const float* params, void* ws, cudaStream_t s);
 
-// mode 0: forward conv (N,H,W,Ci)->(N,H,W,Co);  mode 1: its data gradient.  true if the tcgen05 kernel takes it.
+// mode 0: forward conv (N,H,W,Ci)->(N,H,W,Co);  mode 1: its data gradient.  true if the tensor-core kernel takes it.
 bool conv_tc_supported(int dtype, int mode, int N, int H, int W, int Ci, int Co, int ks, int stride, int nseg);
 // true if the forward epilogue can also emit the GroupNorm input statistics of its output (ConvArgs::cstats)
 bool conv_tc_stats_supported(int mode, int N, int Ho, int Wo);

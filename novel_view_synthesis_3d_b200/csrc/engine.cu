@@ -67,7 +67,7 @@ struct Op {
   int x = -1, y = -1, r = -1, e = -1;  // tensors: input, output, second input (residual / concat b), FiLM tensor
   // conv
   int ks = 1, stride = 1, pad_h = 0, pad_w = 0, nseg = 1, impl = 0, impl_d = 0, impl_w = 0;
-  long long wT = -1, wC = -1;         // bf16 weight shadows (workspace byte offsets) for the tcgen05 kernels
+  long long wT = -1, wC = -1;         // bf16 weight shadows (workspace byte offsets) for the tensor-core kernels
   long long w = -1, b = -1;            // param offsets (conv W,bias | gn gamma,beta)
   float alpha = 1.f;
   // gn
@@ -94,6 +94,7 @@ struct Op {
 }  // namespace
 
 struct xunet_handle {
+  XuDetScratch* det = xu_det_create(false);   // fp64 reduction scratch of this engine (kernels.h), freed with it
   xunet_config cfg;
   int B, S, dtype, training, N;
   size_t esize;
@@ -449,7 +450,7 @@ struct Builder {
       H.a_cstats = H.alloc(H.cstats_bytes);
       for (Tensor& t : H.tensors) if (t.cstats >= 0) t.cstats += H.a_cstats;
     }
-    // ---- bf16 weight shadows for the tcgen05 convs: one table-driven cast/transpose kernel per forward
+    // ---- bf16 weight shadows for the tensor-core convs: one table-driven cast/transpose kernel per forward
     {
       WeightPrepTable tab;
       tab.n = 0; tab.total = 0;
@@ -481,7 +482,7 @@ struct Builder {
       }
     }
     // ---- fused GroupNorm backward (XUNET_GN_BWD_FUSED=0 restores the two-kernel backward everywhere): a norm without
-    // resampling, plain or +swish, whose output feeds exactly one tcgen05 conv -> that conv's data-gradient epilogue emits
+    // resampling, plain or +swish, whose output feeds exactly one tensor-core conv -> that conv's data-gradient epilogue emits
     // dyh and the channel sums; the norm's backward is then ONE elementwise kernel
     if (H.training) {
       const char* env = getenv("XUNET_GN_BWD_FUSED");      // read per xunet_create, so one process can build both plans
@@ -946,9 +947,8 @@ extern "C" int xunet_create(const xunet_config* cfg, int batch, int side, int dt
   h->cfg = *cfg;
   h->B = batch; h->S = side; h->dtype = dtype; h->training = training ? 1 : 0; h->N = 2 * batch;
   h->esize = dtype == XUNET_DTYPE_F32 ? 4 : 2;
-  // XUNET_ATTN_BWD_FOLD=1: attention backward (head_dim <= 32) as ONE kernel.  Measured and rejected as the default
-  // (profiles/r02_attention_bwd_fold.md): 24 fewer launches per step but 4.11 vs 3.98 ms -- the per-block barrier for D and
-  // the last-CTA rounding tail cost more than the two small helper kernels they replace
+  // XUNET_ATTN_BWD_FOLD=1: the attention backward keeps its dQ / D scratch buffer all-zero between steps (the dQ store kernel
+  // re-zeroes it), so the buffer needs no clearing of its own
   h->attn_fold = getenv("XUNET_ATTN_BWD_FOLD") != nullptr ? 1 : 0;
   Builder b(*h);
   if (b.build() != 0) { delete h; return 1; }
@@ -958,6 +958,7 @@ extern "C" int xunet_create(const xunet_config* cfg, int batch, int side, int dt
 
 extern "C" void xunet_destroy(xunet_handle* h) {
   if (!h) return;
+  xu_det_destroy(h->det);
   destroy_side(h);
   delete h;
 }
@@ -997,6 +998,7 @@ extern "C" int xunet_forward(xunet_handle* h, const float* params, const xunet_b
   if (train && h->cfg.dropout > 0.f && !seed_dev) return fail("xunet_forward: train=1 with dropout needs seed_dev");
   xu_set_kernel_error("");
   Ctx c{h, params, nullptr, (char*)workspace, batch, seed_dev, train ? 1 : 0, (cudaStream_t)stream};
+  XuDetBind bind(h->det);
   int rc = forward_impl(c, eps_out);
   h->forward_done_train = (rc == 0) ? (train ? 1 : 2) : 0;
   return rc;
@@ -1034,6 +1036,7 @@ extern "C" int xunet_backward(xunet_handle* h, const float* params, const xunet_
   if (!h->forward_done_train) return fail("xunet_backward: call xunet_forward first");
   xu_set_kernel_error("");
   Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
+  XuDetBind bind(h->det);
   return backward_impl(c, noise, loss_out);
 }
 
@@ -1058,6 +1061,7 @@ extern "C" int xunet_count_kernels(xunet_handle* h, const float* params, const x
   if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return fail("count_kernels: stream");
   xu_set_kernel_error("");
   int rc = 0;
+  XuDetBind bind(h->det);
   const xunet_bucket_fn saved_fn = h->bucket_fn;   // nothing executes here: the data-parallel hook must not fire
   h->bucket_fn = nullptr;
   for (int pass = 0; pass < 2 && rc == 0; ++pass) {
@@ -1121,6 +1125,13 @@ extern "C" int xunet_dropout_mask(float* mask_out, long long n, int op_index, un
 }
 
 // ---- operator-level entry points ----------------------------------------------------------------------
+// fp64 reduction scratch of one operator-level call (kernels.h): stream-ordered allocations, released on the call's stream
+struct OpScratch {
+  XuDetScratch* d = xu_det_create(true);
+  XuDetBind bind{d};
+  ~OpScratch() { xu_det_destroy(d); }
+};
+
 static int op_done(const char* what) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("%s: CUDA error: %s", what, cudaGetErrorString(e));
@@ -1167,6 +1178,7 @@ extern "C" int xunet_op_conv(int dtype, int impl, const void* x, const float* w,
                              int N, int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha,
                              void* stream) {
   xu_set_kernel_error("");
+  OpScratch scratch;
   ConvArgs a;
   a.x = x; a.y = y; a.res = res; a.w = w; a.bias = bias;
   a.N = N; a.Hi = Hi; a.Wi = Wi; a.Ci = Ci; a.Co = Co; a.ks = ksize; a.stride = stride; a.mode = 0;
@@ -1175,7 +1187,7 @@ extern "C" int xunet_op_conv(int dtype, int impl, const void* x, const float* w,
   else if (ksize != 1) return fail("xunet_op_conv: ksize must be 1 or 3");
   a.wCi = Ci; a.wCo = Co; a.segw = Co / nseg; a.alpha = alpha; a.accumulate = 0;
   if (impl == 1) {
-    if (!conv_tc_supported(dtype, 0, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv: shape not supported by the tcgen05 kernel");
+    if (!conv_tc_supported(dtype, 0, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv: shape not supported by the tensor-core kernel");
     return op_conv_tc(a, w, ksize * ksize, Ci, Co, nseg, (cudaStream_t)stream, "op_conv");
   }
   if (impl == 2) {
@@ -1192,6 +1204,7 @@ extern "C" int xunet_op_conv_dgrad(int dtype, int impl, const void* dy, const fl
                                    int Ci, int Co, int ksize, int stride, int nseg, float alpha, int accumulate,
                                    void* stream) {
   xu_set_kernel_error("");
+  OpScratch scratch;
   ConvArgs a;
   int pl_h = 0, pl_w = 0, Ho = Hi, Wo = Wi;
   if (ksize == 3) { same_pad(Hi, 3, stride, pl_h, Ho); same_pad(Wi, 3, stride, pl_w, Wo); }
@@ -1200,7 +1213,7 @@ extern "C" int xunet_op_conv_dgrad(int dtype, int impl, const void* dy, const fl
   a.ks = ksize; a.stride = stride; a.pad_h = pl_h; a.pad_w = pl_w; a.mode = 1;
   a.wCi = Ci; a.wCo = Co; a.segw = Co / nseg; a.alpha = alpha; a.accumulate = accumulate;
   if (impl == 1) {
-    if (!conv_tc_supported(dtype, 1, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv_dgrad: shape not supported by the tcgen05 kernel");
+    if (!conv_tc_supported(dtype, 1, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv_dgrad: shape not supported by the tensor-core kernel");
     return op_conv_tc(a, w, ksize * ksize, Ci, Co, nseg, (cudaStream_t)stream, "op_conv_dgrad");
   }
   if (impl == 2) {
@@ -1216,6 +1229,7 @@ extern "C" int xunet_op_conv_wgrad(int dtype, int impl, const void* x, const voi
                                    int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha,
                                    void* stream) {
   xu_set_kernel_error("");
+  OpScratch scratch;
   WgradArgs w;
   int pl_h = 0, pl_w = 0, Ho = Hi, Wo = Wi;
   if (ksize == 3) { same_pad(Hi, 3, stride, pl_h, Ho); same_pad(Wi, 3, stride, pl_w, Wo); }
@@ -1223,7 +1237,7 @@ extern "C" int xunet_op_conv_wgrad(int dtype, int impl, const void* x, const voi
   w.N = N; w.Hi = Hi; w.Wi = Wi; w.Ci = Ci; w.Ho = Ho; w.Wo = Wo; w.Co = Co;
   w.ks = ksize; w.stride = stride; w.pad_h = pl_h; w.pad_w = pl_w; w.segw = Co / nseg; w.alpha = alpha;
   if (impl == 1) {
-    if (!wgrad_tc_supported(dtype, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv_wgrad: shape not supported by the tcgen05 kernel");
+    if (!wgrad_tc_supported(dtype, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv_wgrad: shape not supported by the tensor-core kernel");
     launch_wgrad_tc(w, (cudaStream_t)stream);
   } else if (impl == 2) {
     if (Ci == 3 && ksize == 3 && stride == 1 && Co % 8 == 0) launch_conv_small(dtype, 1, nullptr, &w, (cudaStream_t)stream);
@@ -1236,11 +1250,12 @@ extern "C" int xunet_op_conv_wgrad(int dtype, int impl, const void* x, const voi
 extern "C" int xunet_op_attention(int dtype, int impl, const void* qkv, const void* res, void* out, float* lse, int N,
                                   int L, int C, int heads, int cross, void* stream) {
   xu_set_kernel_error("");
+  OpScratch scratch;
   AttnArgs a;
   memset(&a, 0, sizeof(a));
   a.qkv = qkv; a.res = res; a.out = out; a.lse = lse; a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
   if (impl == 1) {
-    if (!attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention: shape not supported by the tcgen05 kernel");
+    if (!attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention: shape not supported by the tensor-core kernel");
     launch_attn_fwd_tc(a, (cudaStream_t)stream);
   } else launch_attn_fwd_simt(dtype, a, (cudaStream_t)stream);
   return op_done("op_attention");
@@ -1250,15 +1265,16 @@ extern "C" int xunet_op_attention_bwd(int dtype, int impl, const void* qkv, cons
                                       const void* dout, const float* lse, float* dscratch, void* dqkv, int N, int L, int C,
                                       int heads, int cross, void* stream) {
   xu_set_kernel_error("");
+  OpScratch scratch;
   AttnArgs a;
   memset(&a, 0, sizeof(a));
   a.qkv = qkv; a.res = res; a.out = const_cast<void*>(out); a.lse = const_cast<float*>(lse);
   a.dout = dout; a.dscratch = dscratch; a.dqkv = dqkv;
   a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
-  // XUNET_OP_ATTN_FOLD=1: the caller passes an all-zero dscratch (and gets it back all-zero) -> the helper-free path the engine uses
+  // XUNET_OP_ATTN_FOLD=1: the caller passes an all-zero dscratch and gets it back all-zero (the dQ store kernel re-zeroes D)
   a.scratch_zeroed = getenv("XUNET_OP_ATTN_FOLD") != nullptr ? 1 : 0;
   if (impl == 1) {
-    if (!attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention_bwd: shape not supported by the tcgen05 kernel");
+    if (!attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention_bwd: shape not supported by the tensor-core kernel");
     launch_attn_bwd_tc(a, (cudaStream_t)stream);
   } else launch_attn_bwd_simt(dtype, a, (cudaStream_t)stream);
   return op_done("op_attention_bwd");

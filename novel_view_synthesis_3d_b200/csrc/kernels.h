@@ -17,10 +17,10 @@ struct ConvArgs {
   int ks, stride, pad_h, pad_w, mode;
   int wCi, wCo, segw;
   float alpha; int accumulate;
-  // optional (tcgen05 forward only, see conv_tc_stats_supported): per-(sample, channel) [sum, sumsq] of the STORED output,
+  // optional (tensor-core forward only, see conv_tc_stats_supported): per-(sample, channel) [sum, sumsq] of the STORED output,
   // (N/2, Co, 2) fp32, accumulated with atomics into a zeroed buffer -- the GroupNorm statistics of the consumer norm
   float* cstats = nullptr;
-  // optional (tcgen05 data gradient, mode 1): this conv consumes the output of a GroupNorm[+swish] without resampling.  The
+  // optional (tensor-core data gradient, mode 1): this conv consumes the output of a GroupNorm[+swish] without resampling.  The
   // epilogue then stores dyh = dy * swish'(.) instead of dy and accumulates the per-(sample, channel) sums [sum dyh*xhat,
   // sum dyh] into cstats (N/2, Co, 2).  gn_x: the norm's input (N,H,W,Co); gn_params: (N/2, Co) float4 {rstd, -mean*rstd,
   // gamma, beta} written by the forward launch_gn_apply (GnArgs::params_out)
@@ -38,6 +38,8 @@ struct WgradArgs {
   int N, Hi, Wi, Ci, Ho, Wo, Co;
   int ks, stride, pad_h, pad_w, segw;
   float alpha;
+  // set by the launchers: fp64 accumulators laid out like dw / dbias, folded into them after the kernel (xu_det_scratch)
+  double* acc_dw; double* acc_db;
 };
 void launch_wgrad_simt(int dtype, const WgradArgs& a, cudaStream_t s);
 // direct kernels for the 3-channel convs.  which: 0 = Cin3 forward, 1 = Cin3 wgrad, 2 = Cout3 forward, 3 = Cout3 dgrad
@@ -134,14 +136,38 @@ struct AttnArgs {
   int N, L, C, heads, cross;
   int scratch_zeroed;   // backward (head_dim <= 32): dscratch is all-zero on entry -> the fused kernel also forms D and rounds dQ
                         // itself (no prep / store kernels) and leaves dscratch all-zero again
-  float* cstats;   // optional (tcgen05 forward): per-(sample, channel) [sum, sumsq] of the stored output, (N/2, C, 2) fp32, accumulated
+  float* cstats;   // optional (tensor-core forward): per-(sample, channel) [sum, sumsq] of the stored output, (N/2, C, 2) fp32, accumulated
 };
 void launch_attn_fwd_simt(int dtype, const AttnArgs& a, cudaStream_t s);
 void launch_attn_bwd_simt(int dtype, const AttnArgs& a, cudaStream_t s);
-// tcgen05/TMEM/TMA versions (bf16; L % 128 == 0; head_dim 16/32/64/128)
+// wgmma/TMA versions (bf16; L % 128 == 0; head_dim 16/32/64/128)
 bool attn_tc_supported(int dtype, int L, int C, int heads);
 void launch_attn_fwd_tc(const AttnArgs& a, cudaStream_t s);
 void launch_attn_bwd_tc(const AttnArgs& a, cudaStream_t s);
+
+// Order-insensitive accumulation.  Kernels that sum the contributions of many CTAs (or warps) into one value add them in
+// fp64 -- into shared memory, or into a zeroed fp64 scratch obtained from xu_det_scratch -- instead of fp32 atomics on the
+// destination; xu_det_fold then adds each fp64 sum to its fp32 destination once and re-zeroes the scratch.  fp64 keeps 29 more
+// significand bits than the fp32 addends, so reordering the additions changes an fp64 sum only when its addends span about
+// 29 - log2(count) binary orders of magnitude, and the fp32 value folded from it changes only if that fp64 sum then lies at an
+// fp32 rounding boundary: the same inputs give the same bits on every run with overwhelming probability, not by construction.
+//
+// The scratch belongs to an XuDetScratch owner bound to the calling thread (XuDetBind):
+//  * an engine handle owns one for its lifetime: one zeroed region per stream, on the handle's device, grown on demand
+//    (also during stream capture) and freed with the handle;
+//  * operator-level entry points bind a call-scoped owner that takes stream-ordered allocations (cudaMallocAsync) and
+//    releases them on the same stream when the call returns.
+struct XuDetScratch;
+XuDetScratch* xu_det_create(bool stream_ordered);
+void xu_det_destroy(XuDetScratch* d);
+struct XuDetBind {
+  explicit XuDetBind(XuDetScratch* d);
+  ~XuDetBind();
+  XuDetScratch* prev;
+};
+double* xu_det_scratch(cudaStream_t s, long long n);   // n zeroed doubles; nullptr (and a kernel error) if unavailable
+void xu_det_fold(float* dst, double* acc, long long n, cudaStream_t s);   // dst[i] += (float)acc[i]; acc[i] = 0
+__device__ __forceinline__ void xu_det_add(double* acc, float v) { atomicAdd(acc, (double)v); }
 
 const char* xu_kernel_error();  // last launch-configuration error recorded by a launcher ("" if none)
 void xu_set_kernel_error(const char* msg);

@@ -1,6 +1,6 @@
 // kernels_conv.cu -- SIMT implicit-GEMM convolution (forward / data-gradient / weight-gradient).
 //
-// This is the exact-fp32 path ("verify mode", XUNET_DTYPE_F32) and the fallback for shapes the tcgen05
+// This is the exact-fp32 path ("verify mode", XUNET_DTYPE_F32) and the fallback for shapes the tensor-core
 // kernel (conv_tc.cu) does not take (Cin=3 input conv, Cout=3 output conv, strided pose convs).
 // Replaces flax nn.Conv / nn.Dense / nn.DenseGeneral as called from model/xunet.py:59,81,85-89,91,
 // 100-102,199,229,276 and their XLA-autodiff gradients (train.py:70).
@@ -259,12 +259,12 @@ __global__ void __launch_bounds__(256) wgrad_simt_kernel(WgradArgs a) {
     for (int j = 0; j < RN; ++j) {
       const int co = tile_co * TN + txx * RN + j;
       if (co >= a.Co) continue;
-      atomicAdd(a.dw + conv_waddr(tap, ci, co, taps, a.Ci, a.segw), a.alpha * acc[i][j]);
+      xu_det_add(a.acc_dw + conv_waddr(tap, ci, co, taps, a.Ci, a.segw), a.alpha * acc[i][j]);
     }
   }
   if (do_bias && tid < TN) {
     const int co = tile_co * TN + tid;
-    if (co < a.Co) atomicAdd(a.dbias + co, a.alpha * bsum);
+    if (co < a.Co) xu_det_add(a.acc_db + co, a.alpha * bsum);
   }
 }
 
@@ -292,9 +292,26 @@ static void wgrad_dispatch(const WgradArgs& a, cudaStream_t s) {
   }
 }
 
+// Runs `launch` with the weight (and bias) gradient accumulated in fp64 scratch and folded into a.dw / a.dbias afterwards, so
+// that the result does not depend on the order of the split-K contributions.
+template <typename F>
+static void det_wgrad(const WgradArgs& a0, cudaStream_t s, F launch) {
+  WgradArgs a = a0;
+  const long long ndw = (long long)a.ks * a.ks * a.Ci * a.Co, ndb = a.dbias ? a.Co : 0;
+  double* acc = xu_det_scratch(s, ndw + ndb);
+  if (acc == nullptr) return;
+  a.acc_dw = acc;
+  a.acc_db = a.dbias ? acc + ndw : nullptr;
+  launch(a);
+  xu_det_fold(a.dw, acc, ndw, s);
+  if (a.dbias) xu_det_fold(a.dbias, acc + ndw, ndb, s);
+}
+
 void launch_wgrad_simt(int dtype, const WgradArgs& a, cudaStream_t s) {
-  if (dtype == XU_F32) wgrad_dispatch<float>(a, s);
-  else wgrad_dispatch<bf16>(a, s);
+  det_wgrad(a, s, [&](const WgradArgs& aa) {
+    if (dtype == XU_F32) wgrad_dispatch<float>(aa, s);
+    else wgrad_dispatch<bf16>(aa, s);
+  });
 }
 
 // ======================================================================================================
@@ -384,10 +401,10 @@ __global__ void __launch_bounds__(256) conv_cin3_wgrad_kernel(WgradArgs a) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) acc[j] = fmaf(xv, d[j], acc[j]);
     }
-    float* dst = (k == 27) ? (a.dbias ? a.dbias + g * 4 : nullptr) : a.dw + (long long)k * a.Co + g * 4;
+    double* dst = (k == 27) ? (a.dbias ? a.acc_db + g * 4 : nullptr) : a.acc_dw + (long long)k * a.Co + g * 4;
     if (dst)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) atomicAdd(dst + j, a.alpha * acc[j]);
+      for (int j = 0; j < 4; ++j) xu_det_add(dst + j, a.alpha * acc[j]);
   }
 }
 
@@ -504,21 +521,21 @@ __global__ void __launch_bounds__(320) conv_cout3_wgrad_kernel(WgradArgs a) {
       const float xv = ldf(x + (((long long)n * a.Hi + iy) * a.Wi + ix) * a.Ci + ci);
       acc[0] = fmaf(xv, ds[pp][0], acc[0]); acc[1] = fmaf(xv, ds[pp][1], acc[1]); acc[2] = fmaf(xv, ds[pp][2], acc[2]);
     }
-    float* dst = a.dw + (long long)it * 3;
-    atomicAdd(dst, a.alpha * acc[0]); atomicAdd(dst + 1, a.alpha * acc[1]); atomicAdd(dst + 2, a.alpha * acc[2]);
+    double* dst = a.acc_dw + (long long)it * 3;
+    xu_det_add(dst, a.alpha * acc[0]); xu_det_add(dst + 1, a.alpha * acc[1]); xu_det_add(dst + 2, a.alpha * acc[2]);
   }
   if (a.dbias != nullptr && threadIdx.x < 3) {
     float sacc = 0.f;
     for (int pp = 0; pp < PPB; ++pp) sacc += ds[pp][threadIdx.x];
-    atomicAdd(a.dbias + threadIdx.x, a.alpha * sacc);
+    xu_det_add(a.acc_db + threadIdx.x, a.alpha * sacc);
   }
 }
 
 
 // ------------------------------------------------------------------------------------------------------
 // Round-2 versions of the 3-channel kernels.  The round-1 kernels above reloaded the whole weight matrix into shared memory for
-// every 8 pixels, paid one shared-memory load per FMA (8-way bank conflicts on top) and three atomics per (tap, channel, 128 pixels);
-// at the 3DiM widths they were 2.7 ms of a 64 ms step (CUPTI, profiles/r02_kineto_full128.txt) for 5.4 GFLOP.  These are persistent,
+// every 8 pixels, paid one shared-memory load per FMA (8-way bank conflicts on top) and three atomics per (tap, channel, 128 pixels).
+// These are persistent,
 // register-blocked over 4 pixels (one weight fetch serves 4 pixels), read weights with conflict-free 16-byte LDS, and the weight
 // gradients keep their 27 x 2 accumulators in registers over a whole pixel range before one reduction per CTA.
 // ------------------------------------------------------------------------------------------------------
@@ -802,15 +819,15 @@ __global__ void __launch_bounds__(256) wgrad_thin_kernel(WgradArgs a) {
     float v = 0.f;
     for (int s2 = 0; s2 < nstream; ++s2) v += red[(s2 * TS + (ch >> 1)) * 56 + pos_c * 2 + (ch & 1)];
     const int pos = pos_c / 3, k = pos_c - pos * 3;
-    float* dst = FLIP ? a.dw + ((long long)(8 - pos) * Cw + ch) * 3 + k : a.dw + (long long)pos_c * Cw + ch;
-    atomicAdd(dst, a.alpha * v);
+    double* dst = FLIP ? a.acc_dw + ((long long)(8 - pos) * Cw + ch) * 3 + k : a.acc_dw + (long long)pos_c * Cw + ch;
+    xu_det_add(dst, a.alpha * v);
   }
   if (a.dbias != nullptr) {
     if (!FLIP) {
       for (int ch = threadIdx.x; ch < Cw; ch += 256) {
         float v = 0.f;
         for (int s2 = 0; s2 < nstream; ++s2) v += red[(s2 * TS + (ch >> 1)) * 56 + 54 + (ch & 1)];
-        atomicAdd(a.dbias + ch, a.alpha * v);
+        xu_det_add(a.acc_db + ch, a.alpha * v);
       }
     } else {
       // every thread of a stream carries the same three sums: take channel-thread 0 of each stream
@@ -820,7 +837,7 @@ __global__ void __launch_bounds__(256) wgrad_thin_kernel(WgradArgs a) {
       if (threadIdx.x < 3) {
         float v = 0.f;
         for (int s2 = 0; s2 < nstream; ++s2) v += red[(s2 * TS) * 56 + (threadIdx.x == 2 ? 53 : 54 + threadIdx.x)];
-        atomicAdd(a.dbias + threadIdx.x, a.alpha * v);
+        xu_det_add(a.acc_db + threadIdx.x, a.alpha * v);
       }
     }
   }
@@ -906,6 +923,13 @@ static void small_dispatch(int which, const ConvArgs* c, const WgradArgs* w, cud
   }
 }
 void launch_conv_small(int dtype, int which, const ConvArgs* c, const WgradArgs* w, cudaStream_t s) {
+  if (w != nullptr) {
+    det_wgrad(*w, s, [&](const WgradArgs& aa) {
+      if (dtype == XU_F32) small_dispatch<float>(which, c, &aa, s);
+      else small_dispatch<bf16>(which, c, &aa, s);
+    });
+    return;
+  }
   if (dtype == XU_F32) small_dispatch<float>(which, c, w, s);
   else small_dispatch<bf16>(which, c, w, s);
 }

@@ -5,11 +5,105 @@
 #include "kernels.h"
 #include <string.h>
 
+#include <map>
+#include <utility>
+#include <vector>
+
 static thread_local char g_kernel_error[256] = "";
 const char* xu_kernel_error() { return g_kernel_error; }
 void xu_set_kernel_error(const char* msg) {
   strncpy(g_kernel_error, msg, sizeof(g_kernel_error) - 1);
   g_kernel_error[sizeof(g_kernel_error) - 1] = 0;
+}
+
+// ---- order-insensitive accumulation (kernels.h) --------------------------------------------------------------------------
+struct XuDetScratch {
+  struct Region { double* p = nullptr; long long n = 0; };
+  bool stream_ordered = false;
+  int device = -1;                                       // engine owner: the device of its first allocation
+  cudaStream_t zero_stream = nullptr;                    // engine owner: zeroes new regions outside any capture
+  std::map<cudaStream_t, Region> regions;                // engine owner: one region per stream
+  std::vector<double*> retired;                          // engine owner: outgrown regions (a captured graph may still use them)
+  std::vector<std::pair<double*, cudaStream_t>> taken;   // call-scoped owner: stream-ordered allocations to release
+};
+static thread_local XuDetScratch* t_det = nullptr;
+
+XuDetScratch* xu_det_create(bool stream_ordered) {
+  XuDetScratch* d = new XuDetScratch();
+  d->stream_ordered = stream_ordered;
+  return d;
+}
+void xu_det_destroy(XuDetScratch* d) {
+  if (d == nullptr) return;
+  for (auto& t : d->taken) cudaFreeAsync(t.first, t.second);
+  if (d->device >= 0) {
+    int cur = -1;
+    cudaGetDevice(&cur);
+    cudaSetDevice(d->device);
+    for (auto& r : d->regions) cudaFree(r.second.p);    // waits for the work that still uses the region
+    for (double* p : d->retired) cudaFree(p);
+    if (d->zero_stream != nullptr) cudaStreamDestroy(d->zero_stream);
+    cudaSetDevice(cur);
+  }
+  delete d;
+}
+XuDetBind::XuDetBind(XuDetScratch* d) : prev(t_det) { t_det = d; }
+XuDetBind::~XuDetBind() { t_det = prev; }
+
+double* xu_det_scratch(cudaStream_t s, long long n) {
+  XuDetScratch* d = t_det;
+  if (d == nullptr) {
+    xu_set_kernel_error("xu_det_scratch: no reduction scratch is bound to this call");
+    return nullptr;
+  }
+  const size_t bytes = sizeof(double) * (size_t)n;
+  if (d->stream_ordered) {
+    double* p = nullptr;
+    if (cudaMallocAsync(&p, bytes, s) != cudaSuccess || cudaMemsetAsync(p, 0, bytes, s) != cudaSuccess) {
+      xu_set_kernel_error("xu_det_scratch: stream-ordered allocation failed");
+      return nullptr;
+    }
+    d->taken.emplace_back(p, s);
+    return p;
+  }
+  int dev = -1;
+  cudaGetDevice(&dev);
+  if (d->device < 0) d->device = dev;
+  if (dev != d->device) {
+    xu_set_kernel_error("xu_det_scratch: the engine is used on a different device than it was first run on");
+    return nullptr;
+  }
+  XuDetScratch::Region& r = d->regions[s];
+  if (n <= r.n) return r.p;
+  // a larger region replaces the old one, which stays allocated until the owner goes.  cudaMalloc is legal during stream capture in relaxed mode, and the new region is zeroed
+  // on the owner's private stream, outside any graph.
+  const long long want = n < (1LL << 16) ? (1LL << 16) : n;
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  double* p = nullptr;
+  const bool ok = (d->zero_stream != nullptr || cudaStreamCreateWithFlags(&d->zero_stream, cudaStreamNonBlocking) == cudaSuccess) &&
+                  cudaMalloc(&p, sizeof(double) * want) == cudaSuccess &&
+                  cudaMemsetAsync(p, 0, sizeof(double) * want, d->zero_stream) == cudaSuccess &&
+                  cudaStreamSynchronize(d->zero_stream) == cudaSuccess;
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  if (!ok) {
+    xu_set_kernel_error("xu_det_scratch: allocating the reduction scratch failed");
+    return nullptr;
+  }
+  if (r.p != nullptr) d->retired.push_back(r.p);
+  r.p = p; r.n = want;
+  return p;
+}
+
+__global__ void __launch_bounds__(256) det_fold_kernel(float* __restrict__ dst, double* __restrict__ acc, long long n) {
+  xu_grid_dep_sync();
+  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  dst[i] += (float)acc[i];
+  acc[i] = 0.0;
+}
+void xu_det_fold(float* dst, double* acc, long long n, cudaStream_t s) {
+  if (n > 0 && acc != nullptr) xu_launch(det_fold_kernel, cdiv(n, 256), 256, 0, s, dst, acc, n);
 }
 
 // lanes l, l' of a warp hold partial sums of the same channel vector iff (l - l') % TPB == 0 (when TPB divides 32):
@@ -27,12 +121,12 @@ __device__ __forceinline__ bool fold_same_channel_lanes(float (&v)[4], int TPB) 
 // GroupNorm  (model/xunet.py:46-52: nn.GroupNorm(32) on (B,2,H,W,C) -> statistics over F,H,W,C/32 jointly)
 // ======================================================================================================
 template <typename T>
-__global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, float* __restrict__ stats, int P, int C,
+__global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, double* __restrict__ stats, int P, int C,
                                                        int ppb) {
   xu_grid_dep_sync();
-  __shared__ float sg[XU_GROUPS], sq[XU_GROUPS];
+  __shared__ double sg[XU_GROUPS], sq[XU_GROUPS];
   const int tid = threadIdx.x, b = blockIdx.y;
-  if (tid < XU_GROUPS) { sg[tid] = 0.f; sq[tid] = 0.f; }
+  if (tid < XU_GROUPS) { sg[tid] = 0.0; sq[tid] = 0.0; }
   __syncthreads();
   const int C4 = C >> 2, cpg = C / XU_GROUPS;
   const int TPB = C4 < 256 ? C4 : 256;
@@ -58,8 +152,8 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, 
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           int g = (cv * 4 + j) / cpg;
-          atomicAdd(&sg[g], s[j]);
-          atomicAdd(&sq[g], ss[j]);
+          xu_det_add(&sg[g], s[j]);
+          xu_det_add(&sq[g], ss[j]);
         }
       }
     }
@@ -87,19 +181,22 @@ void launch_gn_stats(int dtype, const GnArgs& a, cudaStream_t s) {
   if (!a.skip_zero) cudaMemsetAsync(a.stats, 0, sizeof(float) * B * XU_GROUPS * 2, s);
   dim3 grid; int ppb;
   gn_grid(a.C, P, B, grid, ppb);
-  if (dtype == XU_F32) xu_launch(gn_stats_kernel<float>, grid, 256, 0, s, (const float*)a.x, a.stats, P, a.C, ppb);
-  else xu_launch(gn_stats_kernel<bf16>, grid, 256, 0, s, (const bf16*)a.x, a.stats, P, a.C, ppb);
+  double* acc = xu_det_scratch(s, (long long)B * XU_GROUPS * 2);
+  if (acc == nullptr) return;
+  if (dtype == XU_F32) xu_launch(gn_stats_kernel<float>, grid, 256, 0, s, (const float*)a.x, acc, P, a.C, ppb);
+  else xu_launch(gn_stats_kernel<bf16>, grid, 256, 0, s, (const bf16*)a.x, acc, P, a.C, ppb);
+  xu_det_fold(a.stats, acc, (long long)B * XU_GROUPS * 2, s);
 }
 
 // Per-(sample, channel) statistics for tensors whose producer cannot emit them in its epilogue: same traversal as
 // gn_stats_kernel, channel sums kept in shared memory, one interleaved [sum, sumsq] red per channel and block.
 template <typename T>
-__global__ void __launch_bounds__(256) gn_cstats_kernel(const T* __restrict__ x, float* __restrict__ cstats, int P, int C,
+__global__ void __launch_bounds__(256) gn_cstats_kernel(const T* __restrict__ x, double* __restrict__ cstats, int P, int C,
                                                         int ppb) {
   xu_grid_dep_sync();
-  extern __shared__ float scs[];   // [C][2]
+  extern __shared__ double scsd[];   // [C][2]
   const int tid = threadIdx.x, b = blockIdx.y;
-  for (int i = tid; i < 2 * C; i += 256) scs[i] = 0.f;
+  for (int i = tid; i < 2 * C; i += 256) scsd[i] = 0.0;
   __syncthreads();
   const int C4 = C >> 2;
   const int TPB = C4 < 256 ? C4 : 256;
@@ -123,23 +220,26 @@ __global__ void __launch_bounds__(256) gn_cstats_kernel(const T* __restrict__ x,
     if (owner && pl < PL) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        atomicAdd(&scs[(cv * 4 + j) * 2 + 0], s[j]);
-        atomicAdd(&scs[(cv * 4 + j) * 2 + 1], ss[j]);
+        xu_det_add(&scsd[(cv * 4 + j) * 2 + 0], s[j]);
+        xu_det_add(&scsd[(cv * 4 + j) * 2 + 1], ss[j]);
       }
     }
   }
   __syncthreads();
-  float* dst = cstats + (long long)b * C * 2;
-  for (int i = tid; i < 2 * C; i += 256) atomicAdd(&dst[i], scs[i]);
+  double* dst = cstats + (long long)b * C * 2;
+  for (int i = tid; i < 2 * C; i += 256) atomicAdd(&dst[i], scsd[i]);
 }
 
 void launch_gn_cstats(int dtype, const void* x, float* cstats, int N, int H, int W, int C, cudaStream_t s) {
   const int B = N / 2, P = 2 * H * W;
   dim3 grid; int ppb;
   gn_grid(C, P, B, grid, ppb);
-  const size_t smem = sizeof(float) * 2 * C;
-  if (dtype == XU_F32) xu_launch(gn_cstats_kernel<float>, grid, 256, smem, s, (const float*)x, cstats, P, C, ppb);
-  else xu_launch(gn_cstats_kernel<bf16>, grid, 256, smem, s, (const bf16*)x, cstats, P, C, ppb);
+  const size_t smem = sizeof(double) * 2 * C;
+  double* acc = xu_det_scratch(s, (long long)B * C * 2);
+  if (acc == nullptr) return;
+  if (dtype == XU_F32) xu_launch(gn_cstats_kernel<float>, grid, 256, smem, s, (const float*)x, acc, P, C, ppb);
+  else xu_launch(gn_cstats_kernel<bf16>, grid, 256, smem, s, (const bf16*)x, acc, P, C, ppb);
+  xu_det_fold(cstats, acc, (long long)B * C * 2, s);
 }
 
 struct GnDev {
@@ -152,6 +252,7 @@ struct GnDev {
   const unsigned long long* seed_dev;
   const float* cstatsA; const float* cstatsB; int csA;
   float4* params_out; const float* bcs;
+  double* acc;          // gn_bwd_reduce: fp64 sums [dgamma C][dbeta C][bstats (N/2) x groups x 2] (xu_det_scratch)
 };
 
 static GnDev gn_dev(const GnArgs& a) {
@@ -559,11 +660,11 @@ __device__ __forceinline__ void gn_dyhat_compute(int mode, const float (&g)[4], 
 template <typename T>
 __global__ void __launch_bounds__(256) gn_bwd_reduce_kernel(GnDev d, int ppb) {
   xu_grid_dep_sync();
-  extern __shared__ float sm[];  // sA[C], sB[C]
-  float* sA = sm;
-  float* sB = sm + d.C;
+  extern __shared__ double smd[];  // sA[C], sB[C]
+  double* sA = smd;
+  double* sB = smd + d.C;
   const int tid = threadIdx.x, b = blockIdx.y;
-  for (int i = tid; i < 2 * d.C; i += 256) sm[i] = 0.f;
+  for (int i = tid; i < 2 * d.C; i += 256) smd[i] = 0.0;
   __syncthreads();
   const int C4 = d.C >> 2;
   const int TPB = C4 < 256 ? C4 : 256;
@@ -674,37 +775,30 @@ __global__ void __launch_bounds__(256) gn_bwd_reduce_kernel(GnDev d, int ppb) {
       if (owner && pl < PL) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          atomicAdd(&sA[c0 + j], A[j]);
-          atomicAdd(&sB[c0 + j], Bc[j]);
+          xu_det_add(&sA[c0 + j], A[j]);
+          xu_det_add(&sB[c0 + j], Bc[j]);
         }
       }
     }
   }
   __syncthreads();
   const int cpg = d.C / XU_GROUPS;
-  // L2 atomics on a handful of lines shared by every block are the serial tail of this kernel: 128-bit vector reds
-  // (4 channels per lane-op) when the leaves are 16-byte aligned
-  if (((reinterpret_cast<uintptr_t>(d.dgamma) | reinterpret_cast<uintptr_t>(d.dbeta)) & 15) == 0) {
-    for (int c = tid * 4; c < d.C; c += 1024) {
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d.dgamma + c), "f"(sA[c]), "f"(sA[c + 1]), "f"(sA[c + 2]), "f"(sA[c + 3]) : "memory");
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d.dbeta + c), "f"(sB[c]), "f"(sB[c + 1]), "f"(sB[c + 2]), "f"(sB[c + 3]) : "memory");
-    }
-  } else {
-    for (int c = tid; c < d.C; c += 256) {
-      atomicAdd(&d.dgamma[c], sA[c]);
-      atomicAdd(&d.dbeta[c], sB[c]);
-    }
+  double* gacc = d.acc;
+  double* bacc = d.acc + 2 * d.C;
+  for (int c = tid; c < d.C; c += 256) {
+    atomicAdd(&gacc[c], sA[c]);
+    atomicAdd(&gacc[d.C + c], sB[c]);
   }
   if (tid < XU_GROUPS) {
-    float s1 = 0.f, s2 = 0.f;
+    double s1 = 0.0, s2 = 0.0;
     for (int k = 0; k < cpg; ++k) {
       const int c = tid * cpg + k;
-      const float gmc = d.gamma[c];
-      s1 = fmaf(gmc, sB[c], s1);
-      s2 = fmaf(gmc, sA[c], s2);
+      const double gmc = d.gamma[c];
+      s1 += gmc * sB[c];
+      s2 += gmc * sA[c];
     }
-    atomicAdd(&d.bstats[(b * XU_GROUPS + tid) * 2 + 0], s1);
-    atomicAdd(&d.bstats[(b * XU_GROUPS + tid) * 2 + 1], s2);
+    atomicAdd(&bacc[(b * XU_GROUPS + tid) * 2 + 0], s1);
+    atomicAdd(&bacc[(b * XU_GROUPS + tid) * 2 + 1], s2);
   }
 }
 
@@ -714,9 +808,14 @@ void launch_gn_bwd_reduce(int dtype, const GnArgs& a, cudaStream_t s) {
   if (!a.skip_zero) cudaMemsetAsync(a.bstats, 0, sizeof(float) * B * XU_GROUPS * 2, s);
   dim3 grid; int ppb;
   gn_grid(a.C, P, B, grid, ppb);
-  size_t smem = sizeof(float) * 2 * a.C;
+  size_t smem = sizeof(double) * 2 * a.C;
+  d.acc = xu_det_scratch(s, 2LL * a.C + (long long)B * XU_GROUPS * 2);
+  if (d.acc == nullptr) return;
   if (dtype == XU_F32) xu_launch(gn_bwd_reduce_kernel<float>, grid, 256, smem, s, d, ppb);
   else xu_launch(gn_bwd_reduce_kernel<bf16>, grid, 256, smem, s, d, ppb);
+  xu_det_fold(a.dgamma, d.acc, a.C, s);
+  xu_det_fold(a.dbeta, d.acc + a.C, a.C, s);
+  xu_det_fold(a.bstats, d.acc + 2 * a.C, (long long)B * XU_GROUPS * 2, s);
 }
 
 // pass B: dx = rstd * (gamma*dyh - S1/cnt - xhat*S2/cnt); same thread <-> channel-vector mapping as gn_apply_kernel
@@ -858,11 +957,15 @@ __global__ void __launch_bounds__(256, 2) gn_bwd_apply_pre_kernel(GnDev d, int p
       s_grp[tid][0] = d.stats[(b * XU_GROUPS + tid) * 2 + 0];
       s_grp[tid][1] = d.stats[(b * XU_GROUPS + tid) * 2 + 1];
     }
-    if (blockIdx.x == 0) {     // one block per sample adds its channel sums to the parameter gradients
+    if (blockIdx.x == 0 && b == 0) {     // one block adds the channel sums of every sample, in sample order, to the parameter gradients
       for (int c = tid; c < d.C; c += 256) {
-        const float2 ab = *reinterpret_cast<const float2*>(d.bcs + ((long long)b * d.C + c) * 2);
-        atomicAdd(&d.dgamma[c], ab.x);
-        atomicAdd(&d.dbeta[c], ab.y);
+        float ga = 0.f, gb = 0.f;
+        for (int bb = 0; bb < d.N / 2; ++bb) {
+          const float2 ab = *reinterpret_cast<const float2*>(d.bcs + ((long long)bb * d.C + c) * 2);
+          ga += ab.x; gb += ab.y;
+        }
+        d.dgamma[c] += ga;
+        d.dbeta[c] += gb;
       }
     }
     __syncthreads();
@@ -955,7 +1058,7 @@ void launch_gn_bwd_apply(int dtype, const GnArgs& a, cudaStream_t s) {
 // One Dense layer of the log-SNR MLP for one sample and 32 output columns per CTA: lane <-> column (128-byte coalesced weight rows),
 // the 8 warps split K and are reduced through shared memory in a fixed order (deterministic).  FIRST: the input vector is the
 // DDPM sinusoidal encoding of logsnr[b], built in shared memory (and exported to `pe` for the backward); otherwise swish(h1[b]).
-// grid (E/32, B): E = 1024 -> 32*B CTAs instead of the B CTAs x 2E serial FMAs per thread of round 1 (581 us -> a few us).
+// grid (E/32, B): E = 1024 -> 32*B CTAs instead of the B CTAs x 2E serial FMAs per thread of round 1.
 template <bool FIRST>
 __global__ void __launch_bounds__(256) logsnr_dense_kernel(const float* __restrict__ logsnr, const float* __restrict__ in,
                                                             const float* __restrict__ w, const float* __restrict__ bias,
@@ -1175,7 +1278,7 @@ void launch_pose_emb(int dtype, const float* R1, const float* t1, const float* R
 
 template <typename T>
 __global__ void pose_emb_bwd_kernel(const T* __restrict__ dpose, float* __restrict__ dpos_emb,
-                                    float* __restrict__ dref_first, float* __restrict__ dref_other, int B, int S) {
+                                    double* __restrict__ dref_first, double* __restrict__ dref_other, int B, int S) {
   xu_grid_dep_sync();
   const long long per = (long long)S * S * XU_POSE_DIM;
   const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -1187,14 +1290,21 @@ __global__ void pose_emb_bwd_kernel(const T* __restrict__ dpose, float* __restri
     s1 += ldf(dpose + (long long)(2 * b + 1) * per + idx);
   }
   if (dpos_emb != nullptr) dpos_emb[idx] = s0 + s1;
-  if (dref_first != nullptr) { atomicAdd(&dref_first[j], s0); atomicAdd(&dref_other[j], s1); }
+  if (dref_first != nullptr) { xu_det_add(&dref_first[j], s0); xu_det_add(&dref_other[j], s1); }
 }
 
 void launch_pose_emb_bwd(int dtype, const void* dpose, float* dpos_emb, float* dref_first, float* dref_other, int B, int S,
                          cudaStream_t s) {
   const long long per = (long long)S * S * XU_POSE_DIM;
-  if (dtype == XU_F32) xu_launch(pose_emb_bwd_kernel<float>, cdiv(per, 256), 256, 0, s, (const float*)dpose, dpos_emb, dref_first, dref_other, B, S);
-  else xu_launch(pose_emb_bwd_kernel<bf16>, cdiv(per, 256), 256, 0, s, (const bf16*)dpose, dpos_emb, dref_first, dref_other, B, S);
+  double* acc = nullptr;
+  if (dref_first != nullptr && (acc = xu_det_scratch(s, 2 * XU_POSE_DIM)) == nullptr) return;
+  double* acc2 = acc ? acc + XU_POSE_DIM : nullptr;
+  if (dtype == XU_F32) xu_launch(pose_emb_bwd_kernel<float>, cdiv(per, 256), 256, 0, s, (const float*)dpose, dpos_emb, acc, acc2, B, S);
+  else xu_launch(pose_emb_bwd_kernel<bf16>, cdiv(per, 256), 256, 0, s, (const bf16*)dpose, dpos_emb, acc, acc2, B, S);
+  if (acc != nullptr) {
+    xu_det_fold(dref_first, acc, XU_POSE_DIM, s);
+    xu_det_fold(dref_other, acc2, XU_POSE_DIM, s);
+  }
 }
 
 // ======================================================================================================
@@ -1228,11 +1338,11 @@ void launch_emb_fwd(int dtype, const float* lemb, const void* pe, void* semb, in
 template <typename T>
 __global__ void __launch_bounds__(256) emb_bwd_kernel(const float* __restrict__ lemb, const T* __restrict__ pe,
                                                       const T* __restrict__ dsemb, T* __restrict__ dpe,
-                                                      float* __restrict__ dlemb, int P, int E, int ppb, int write_dpe) {
+                                                      double* __restrict__ dlemb, int P, int E, int ppb, int write_dpe) {
   xu_grid_dep_sync();
-  extern __shared__ float sacc[];  // E
+  extern __shared__ double saccd[];  // E
   const int tid = threadIdx.x, b = blockIdx.y;
-  for (int i = tid; i < E; i += 256) sacc[i] = 0.f;
+  for (int i = tid; i < E; i += 256) saccd[i] = 0.0;
   __syncthreads();
   const int E4 = E >> 2;
   const int TPB = E4 < 256 ? E4 : 256;
@@ -1256,12 +1366,12 @@ __global__ void __launch_bounds__(256) emb_bwd_kernel(const float* __restrict__ 
       }
       if (fold_same_channel_lanes(acc, TPB) && pl < PL) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) atomicAdd(&sacc[cv * 4 + j], acc[j]);
+        for (int j = 0; j < 4; ++j) xu_det_add(&saccd[cv * 4 + j], acc[j]);
       }
     }
   }
   __syncthreads();
-  for (int i = tid; i < E; i += 256) atomicAdd(&dlemb[b * E + i], sacc[i]);
+  for (int i = tid; i < E; i += 256) atomicAdd(&dlemb[b * E + i], saccd[i]);
 }
 
 void launch_emb_bwd(int dtype, const float* lemb, const void* pe, const void* dsemb, void* dpe, float* dlemb, int N, int HW,
@@ -1269,11 +1379,14 @@ void launch_emb_bwd(int dtype, const float* lemb, const void* pe, const void* ds
   const int B = N / 2, P = 2 * HW;
   dim3 grid; int ppb;
   gn_grid(E, P, B, grid, ppb);
-  size_t smem = sizeof(float) * E;
+  size_t smem = sizeof(double) * E;
+  double* acc = xu_det_scratch(s, (long long)B * E);
+  if (acc == nullptr) return;
   if (dtype == XU_F32)
-    xu_launch(emb_bwd_kernel<float>, grid, 256, smem, s, lemb, (const float*)pe, (const float*)dsemb, (float*)dpe, dlemb, P, E, ppb, write_dpe);
+    xu_launch(emb_bwd_kernel<float>, grid, 256, smem, s, lemb, (const float*)pe, (const float*)dsemb, (float*)dpe, acc, P, E, ppb, write_dpe);
   else
-    xu_launch(emb_bwd_kernel<bf16>, grid, 256, smem, s, lemb, (const bf16*)pe, (const bf16*)dsemb, (bf16*)dpe, dlemb, P, E, ppb, write_dpe);
+    xu_launch(emb_bwd_kernel<bf16>, grid, 256, smem, s, lemb, (const bf16*)pe, (const bf16*)dsemb, (bf16*)dpe, acc, P, E, ppb, write_dpe);
+  xu_det_fold(dlemb, acc, (long long)B * E, s);
 }
 
 // ======================================================================================================
@@ -1412,7 +1525,7 @@ void launch_extract_frame1(int dtype, const void* o, float* eps, int B, int S, c
 
 // loss = ||eps - noise||_F  (train.py:67)
 __global__ void __launch_bounds__(256) loss_sumsq_kernel(const float* __restrict__ eps, const float* __restrict__ noise,
-                                                         long long n, float* __restrict__ sumsq) {
+                                                         long long n, double* __restrict__ sumsq) {
   xu_grid_dep_sync();
   __shared__ float sw[8];
   float acc = 0.f;
@@ -1426,7 +1539,7 @@ __global__ void __launch_bounds__(256) loss_sumsq_kernel(const float* __restrict
   if (threadIdx.x < 8) {
     float v = sw[threadIdx.x];
     for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(sumsq, v);
+    if (threadIdx.x == 0) xu_det_add(sumsq, v);
   }
 }
 template <typename T>
@@ -1453,7 +1566,10 @@ void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_s
   cudaMemsetAsync(sumsq_scratch, 0, sizeof(float), s);
   int blocks = cdiv(n, 256 * 4);
   if (blocks > 592) blocks = 592;
-  xu_launch(loss_sumsq_kernel, blocks, 256, 0, s, eps, noise, n, sumsq_scratch);
+  double* acc = xu_det_scratch(s, 1);
+  if (acc == nullptr) return;
+  xu_launch(loss_sumsq_kernel, blocks, 256, 0, s, eps, noise, n, acc);
+  xu_det_fold(sumsq_scratch, acc, 1, s);
   const long long total = 2 * n;
   if (dtype == XU_F32) xu_launch(loss_grad_kernel<float>, cdiv(total, 256), 256, 0, s, eps, noise, sumsq_scratch, loss_out, (float*)dO, B, per);
   else xu_launch(loss_grad_kernel<bf16>, cdiv(total, 256), 256, 0, s, eps, noise, sumsq_scratch, loss_out, (bf16*)dO, B, per);

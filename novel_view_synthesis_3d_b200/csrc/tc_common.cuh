@@ -1,7 +1,8 @@
-// tc_common.cuh -- PTX wrappers shared by the tcgen05 kernels (mbarrier, TMA, tcgen05.mma/ld/commit, UMMA descriptors).
+// tc_common.cuh -- PTX wrappers shared by the tensor-core kernels (mbarrier, TMA, GMMA descriptors; wgmma.cuh has the MMAs).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
+#include "wgmma.cuh"
 
 // ---------------------------------------------------------------------------------------------- PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -59,65 +60,29 @@ __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bul
 template <int N> __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
-      "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-// same load without the trailing tcgen05.wait::ld (issue several, then wait once)
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
-      "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-
-// UMMA shared-memory matrix descriptor, K-major operand whose rows are exactly one swizzle span wide
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout [61,64)).
+// GMMA shared-memory matrix descriptor (sm_90a wgmma): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64)
+// (1 = 128B, 2 = 64B, 3 = 32B swizzle).  K-major operand whose rows are exactly one swizzle span wide (BK * 2 bytes), as a
+// TMA box {BK, rows} lands; SBO = the 8-row core-matrix group stride.  Tiles start on a swizzle-atom boundary, so a K step
+// inside the span is a plain start-address offset (k * 32 bytes per 16 elements).
 template <int BK>
 __device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr) {
   constexpr uint32_t row_bytes = BK * 2;                    // 128 / 64 / 32
-  constexpr uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);  // SWIZZLE_128B / 64B / 32B
-  constexpr uint64_t sbo = (8 * row_bytes) >> 4;            // 8-row core-matrix group stride
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (sbo << 32) | (1ull << 46) | (layout << 61);
+  constexpr uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : 3ull);
+  constexpr uint64_t sbo = (8 * row_bytes) >> 4;
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (sbo << 32) | (layout << 62);
 }
-
 
 // MN-major operand (the M/N index is the contiguous one), tile stored as [K rows][W elements] with row pitch = one swizzle
 // span (W*2 = 128/64/32 bytes) exactly as a TMA box {W, K} lands; wider M/N extents are further [K rows][W] blocks LBO
-// bytes apart.  (cute::UMMA canonical Major-MN layout: SBO = stride between 8-row K groups, LBO = stride between MN blocks.)
+// bytes apart (canonical GMMA Major-MN layout: SBO = stride between 8-row K groups, LBO = stride between MN blocks).
 template <int W>
 __device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
   constexpr uint32_t row_bytes = W * 2;
-  constexpr uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);
+  constexpr uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : 3ull);
   constexpr uint64_t sbo = (8 * row_bytes) >> 4;
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (sbo << 32) | (1ull << 46) |
-         (layout << 61);
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (sbo << 32) | (layout << 62);
 }
 // explicit shared-space accesses: through a generic pointer derived from the dynamic shared-memory base the compiler emits LD.E /
 // ST.E (generic address translation on every access) instead of LDS / STS
@@ -136,19 +101,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(ncols) : "memory");
-}
-// instruction descriptor, kind::f16, bf16 x bf16 -> f32, M = 128
-__device__ __forceinline__ uint32_t make_idesc_bf16(int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((128u >> 4) << 24);
-}
-
 // 2^x on the MUFU pipe, flush-to-zero (one instruction; exp2f() adds denormal-range fix-ups the softmax does not need)
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -181,9 +133,10 @@ __device__ __forceinline__ float warp_transpose_reduce32(float (&x)[32], int lan
 // channels of this lane's pixel (already rounded to the stored dtype), x[16..31] = their squares.  After the transposing
 // reduction lane l < 16 holds sum over the warp's 32 pixels of channel l and lane l >= 16 the sum of squares of channel l-16;
 // one scalar red per lane lands on the interleaved [channel][sum, sumsq] row of the sample: 128 contiguous bytes per warp.
-__device__ __forceinline__ void xu_cstats_emit16(float (&x)[32], int lane, float* cs_row /* &cstats[(b*C + c0) * 2] */) {
+// cs_row is an fp64 accumulator (xu_det_scratch) folded into the fp32 statistics after the kernel.
+__device__ __forceinline__ void xu_cstats_emit16(float (&x)[32], int lane, double* cs_row /* &cstats[(b*C + c0) * 2] */) {
   const float v = warp_transpose_reduce32(x, lane);
-  atomicAdd(cs_row + ((lane & 15) << 1) + (lane >> 4), v);
+  atomicAdd(cs_row + ((lane & 15) << 1) + (lane >> 4), (double)v);
 }
 
 // host: encode a bf16 tiled tensor map (rank <= 5; dims/box innermost first; strides in bytes for dims 1..rank-1;

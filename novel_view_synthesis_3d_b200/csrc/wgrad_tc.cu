@@ -1,12 +1,13 @@
-// wgrad_tc.cu -- tcgen05 weight-gradient of the 3x3 / 1x1 convolutions (XLA autodiff of nn.Conv / nn.Dense, train.py:70).
+// wgrad_tc.cu -- wgmma weight-gradient of the 3x3 / 1x1 convolutions (XLA autodiff of nn.Conv / nn.Dense, train.py:70).
 //
 //   dW[tap][ci][co] += alpha * sum_pixels X[pixel (+) tap][ci] * dY[pixel][co]
 //
 // GEMM view: D[M = (tap, ci)][N = co], K = output pixels.  Both operands are "MN-major" for the tensor core -- the
 // contiguous index of the NHWC tensors (channels) is the GEMM M / N index -- so the TMA boxes {channels, TW, TH, TN}
-// land in shared memory as [128 pixels][channel-chunk] and are consumed through MN-major UMMA descriptors without any
-// transposition.  One CTA accumulates a 128 x BN tile of dW (several (tap, ci-chunk) blocks stacked along M) in TMEM over
-// its share of the pixels (split-K across CTAs), then reduces into the flat fp32 gradient buffer with red.global.add.
+// land in shared memory as [128 pixels][channel-chunk] and are consumed through MN-major GMMA descriptors without any
+// transposition.  One CTA accumulates a 128 x BN tile of dW (several (tap, ci-chunk) blocks stacked along M) in registers over
+// its share of the pixels (split-K across CTAs), then adds it to an fp64 copy of the gradient (xu_det_scratch) that is folded
+// into the flat fp32 gradient buffer afterwards, so the split-K sum does not depend on the order in which the CTAs finish.
 #include "conv_tc.h"
 #include "tc_common.cuh"
 
@@ -20,37 +21,31 @@ struct WgTcParams {
   int Ci, Co, taps, ks, segw, stride, pad_h, pad_w;
   int cpt;          // ci-chunks per tap
   int MB;           // total M-blocks = taps * cpt
-  int BN, NB;       // N tile and its number of CWB-wide blocks
+  int BN;           // N tile (wgmma N)
   int stages;
   float alpha;
-  float* dw;
-  float* dbias;     // if non-null: an all-ones M-block appended after the last (tap, ci) block yields colsum(dY)
-  int two_prod;     // the dY boxes of a stage are issued by a second producer lane (warp 2) in parallel with the x boxes (warp 0)
-  int prefetch;     // pixel tiles by which an L2 prefetch of the x / dY boxes runs ahead of their TMA loads (0: none)
+  double* dw;       // fp64 accumulators laid out like the weight / bias gradients (xu_det_scratch), folded in afterwards
+  double* dbias;    // if non-null: an all-ones M-block appended after the last (tap, ci) block yields colsum(dY)
 };
 
-// MT = 2: the CTA owns TWO 128-row M tiles (256 (tap, ci) rows x BN <= 256 columns = all 512 TMEM columns) and walks 64-pixel
-// K steps: the dY tile is fetched once for 256 rows of dW instead of 128 -- (M + N) / (M * N) operand bytes per MAC drop by a third
-// (the kernel is bound by the L2 -> SM operand stream: 96 KB per 1024 MMA cycles = 94 B/clk/SM at MT = 1), same 64 KB ring stage.
-// PT = pixels (GEMM K) per pipeline step: 128, or 64 for a ring of twice as many, half-sized stages (more loads in flight per byte of
-// shared memory: the K loop streams both operands from L2 / DRAM and a 2-deep ring of 96 KB stages cannot cover the load latency).
-template <int CWA, int CWB, int MT, int PT>
-__global__ void __launch_bounds__(192) wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX,
-                                                       const __grid_constant__ CUtensorMap tmDY, const WgTcParams p) {
-  constexpr int GT = 128 / CWA;                 // M-blocks per 128-row M tile
-  constexpr int G = MT * GT;                    // M-blocks stacked per CTA
+// One CTA accumulates a 128 x BN tile of dW: warps 0-7 are two consumer warpgroups (M rows 64 wg .. 64 wg + 63, fp32
+// accumulators in registers), warp 8 is the TMA producer.  K = pixels, 128 per pipeline step.
+constexpr int kWgThreads = 288;
+template <int CWA, int CWB, int BN>
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX,
+                                                                 const __grid_constant__ CUtensorMap tmDY, const WgTcParams p) {
+  constexpr int PT = 128;
+  constexpr int G = 128 / CWA;                  // M-blocks stacked per CTA
   constexpr int A_BLOCK = PT * CWA * 2;         // bytes of one [PT pixels][CWA] block
   constexpr int B_BLOCK = PT * CWB * 2;
-  constexpr int A_BYTES = G * A_BLOCK;          // 128 * MT * PT * 2 bytes
+  constexpr int A_BYTES = G * A_BLOCK;
+  constexpr int B_BYTES = (BN / CWB) * B_BLOCK;
   extern __shared__ uint8_t smem_raw[];
-  const int B_BYTES = p.NB * B_BLOCK;
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* smA = base;
   uint8_t* smB = base + (size_t)p.stages * A_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(smB + (size_t)p.stages * B_BYTES);
   uint64_t* empty = full + p.stages;
-  uint64_t* tmem_full = empty + p.stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile_m = blockIdx.x, n_tile = blockIdx.y;
@@ -63,15 +58,11 @@ __global__ void __launch_bounds__(192) wgrad_tc_kernel(const __grid_constant__ C
   if (nblk < 0) nblk = 0;
   // bias gradient: the block right after the last weight block is filled with ones (never touched by TMA)
   const int ones_g = (p.dbias != nullptr && n_tile >= 0 && tile_m == p.MB / G && (p.MB % G != 0 || nblk == 0)) ? nblk : -1;
-  uint32_t ncols = 32;
-  while ((int)ncols < MT * p.BN) ncols <<= 1;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, ncols);
   if (ones_g >= 0) {
     const uint32_t ones2 = 0x3F803F80u;          // two bf16 1.0
     for (int st = 0; st < p.stages; ++st) {
@@ -80,139 +71,87 @@ __global__ void __launch_bounds__(192) wgrad_tc_kernel(const __grid_constant__ C
     }
     fence_async_smem();
   }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  xu_grid_dep_sync();     // PDL: everything above (barriers, TMEM) overlaps the previous kernel's tail
-  const uint32_t tmem_base = *tmem_slot;
+  xu_grid_dep_sync();     // PDL: everything above overlaps the previous kernel's tail
+  if (total <= 0) return;
 
-  if (total > 0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        for (int it = 0; it < total; ++it) {
-          const int s = it % p.stages;
-          if (p.prefetch) {
-            // both operands are streamed once from DRAM (K = all pixels): prefetch the boxes of pixel tile it + lead into L2
-            for (int pit = (it == 0 ? 0 : it + p.prefetch); pit <= it + p.prefetch && pit < total; ++pit) {
-              int t = pt_beg + pit;
-              const int tx = t % p.tiles_x; t /= p.tiles_x;
-              const int ty = t % p.tiles_y; t /= p.tiles_y;
-              const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
-              for (int g = 0; g < nblk; ++g) {
-                const int mb = tile_m * G + g;
-                const int tap = mb / p.cpt, chunk = mb - tap * p.cpt;
-                int ox = 0, oy = 0;
-                if (p.ks == 3) { const int dy = tap / 3; oy = dy - p.pad_h; ox = tap - dy * 3 - p.pad_w; }
-                tma_prefetch_4d(&tmX, chunk * CWA, x0 * p.stride + ox, y0 * p.stride + oy, n0);
-              }
-              for (int b = 0; b < p.NB; ++b) tma_prefetch_4d(&tmDY, n_tile * p.BN + b * CWB, x0, y0, n0);
-            }
-          }
-          mbar_wait(&empty[s], ((it / p.stages) & 1) ^ 1);
-          int t = pt_beg + it;
-          const int tx = t % p.tiles_x; t /= p.tiles_x;
-          const int ty = t % p.tiles_y; t /= p.tiles_y;
-          const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
-          mbar_expect_tx(&full[s], nblk * A_BLOCK + B_BYTES);
-          for (int g = 0; g < nblk; ++g) {
-            const int mb = tile_m * G + g;
-            const int tap = mb / p.cpt, chunk = mb - tap * p.cpt;
-            int ox = 0, oy = 0;
-            if (p.ks == 3) { const int dy = tap / 3; oy = dy - p.pad_h; ox = tap - dy * 3 - p.pad_w; }
-            tma_load_4d(smA + (size_t)s * A_BYTES + g * A_BLOCK, &tmX, &full[s], chunk * CWA, x0 * p.stride + ox, y0 * p.stride + oy, n0);
-          }
-          if (!p.two_prod)
-            for (int b = 0; b < p.NB; ++b)
-              tma_load_4d(smB + (size_t)s * B_BYTES + b * B_BLOCK, &tmDY, &full[s], n_tile * p.BN + b * CWB, x0, y0, n0);
+  if (warp == 8) {
+    if (lane == 0) {
+      for (int it = 0; it < total; ++it) {
+        const int s = it % p.stages;
+        mbar_wait(&empty[s], ((it / p.stages) & 1) ^ 1);
+        int t = pt_beg + it;
+        const int tx = t % p.tiles_x; t /= p.tiles_x;
+        const int ty = t % p.tiles_y; t /= p.tiles_y;
+        const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
+        mbar_expect_tx(&full[s], nblk * A_BLOCK + B_BYTES);
+        for (int g = 0; g < nblk; ++g) {
+          const int mb = tile_m * G + g;
+          const int tap = mb / p.cpt, chunk = mb - tap * p.cpt;
+          int ox = 0, oy = 0;
+          if (p.ks == 3) { const int dy = tap / 3; oy = dy - p.pad_h; ox = tap - dy * 3 - p.pad_w; }
+          tma_load_4d(smA + (size_t)s * A_BYTES + g * A_BLOCK, &tmX, &full[s], chunk * CWA, x0 * p.stride + ox, y0 * p.stride + oy, n0);
         }
-      }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        const uint32_t idesc = make_idesc_bf16(p.BN, 1, 1);      // A and B both MN-major
-        for (int it = 0; it < total; ++it) {
-          const int s = it % p.stages;
-          mbar_wait(&full[s], (it / p.stages) & 1);
-          tcgen05_fence_after();
-          const uint32_t a_addr = smem_u32(smA + (size_t)s * A_BYTES);
-          const uint32_t b_addr = smem_u32(smB + (size_t)s * B_BYTES);
-#pragma unroll
-          for (int k = 0; k < PT / 16; ++k) {                     // PT pixels = PT/16 x (K = 16)
-            const uint64_t db = make_mnmajor_desc<CWB>(b_addr + k * 16 * (CWB * 2), B_BLOCK);
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt) {
-              if (mt > 0 && mt * GT >= nblk + (ones_g >= 0 ? 1 : 0)) break;      // no valid block in this M tile
-              const uint64_t da = make_mnmajor_desc<CWA>(a_addr + mt * GT * A_BLOCK + k * 16 * (CWA * 2), A_BLOCK);
-              umma_bf16(tmem_base + (uint32_t)(mt * p.BN), da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty[s]);
-        }
-        umma_commit(tmem_full);
-      }
-    } else {
-      if (p.two_prod && warp == 2) {
-        // second producer (experiment: is one thread issuing all 2 + NB boxes of a stage the limit?  it is not, see the launcher).
-        // This otherwise idle epilogue warp issues the dY boxes; the transaction bytes were announced by the first producer (a
-        // complete_tx that overtakes the expect_tx is legal: the phase cannot complete before that producer's own arrival).
-        if (lane == 0) {
-          for (int it = 0; it < total; ++it) {
-            const int s = it % p.stages;
-            mbar_wait(&empty[s], ((it / p.stages) & 1) ^ 1);
-            int t = pt_beg + it;
-            const int tx = t % p.tiles_x; t /= p.tiles_x;
-            const int ty = t % p.tiles_y; t /= p.tiles_y;
-            const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
-            for (int b = 0; b < p.NB; ++b)
-              tma_load_4d(smB + (size_t)s * B_BYTES + b * B_BLOCK, &tmDY, &full[s], n_tile * p.BN + b * CWB, x0, y0, n0);
-          }
-        }
-        __syncwarp();
-      }
-      mbar_wait(tmem_full, 0);
-      tcgen05_fence_after();
-      const int lane_base = (warp & 3) * 32;
-      const int r = lane_base + lane;
-#pragma unroll 1
-      for (int mt = 0; mt < MT; ++mt) {
-      if (mt > 0 && mt * GT >= nblk + (ones_g >= 0 ? 1 : 0)) break;
-      const int g = mt * GT + r / CWA, c = r % CWA;
-      const int mb = tile_m * G + g;
-      const bool valid = g < nblk;
-      const bool bias_row = (g == ones_g) && c == 0;
-      const int tap = valid ? mb / p.cpt : 0;
-      const int ci = valid ? (mb - tap * p.cpt) * CWA + c : 0;
-      for (int c0 = 0; c0 < p.BN; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)lane_base << 16) + (uint32_t)(mt * p.BN + c0), v);
-        if (valid && ci < p.Ci) {
-          // segw % 32 == 0 -> the 32 columns of this chunk are contiguous in one segment: 8 x red.global.add.v4.f32
-          const int co = n_tile * p.BN + c0;
-          const int seg = co / p.segw;
-          float* dst = p.dw + (long long)seg * p.taps * p.Ci * p.segw + ((long long)tap * p.Ci + ci) * p.segw + (co - seg * p.segw);
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(p.alpha * __uint_as_float(v[j])),
-                         "f"(p.alpha * __uint_as_float(v[j + 1])), "f"(p.alpha * __uint_as_float(v[j + 2])),
-                         "f"(p.alpha * __uint_as_float(v[j + 3]))
-                         : "memory");
-        } else if (bias_row) {
-          float* dst = p.dbias + n_tile * p.BN + c0;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(p.alpha * __uint_as_float(v[j])),
-                         "f"(p.alpha * __uint_as_float(v[j + 1])), "f"(p.alpha * __uint_as_float(v[j + 2])),
-                         "f"(p.alpha * __uint_as_float(v[j + 3]))
-                         : "memory");
-        }
-      }
+        for (int b = 0; b < BN / CWB; ++b)
+          tma_load_4d(smB + (size_t)s * B_BYTES + b * B_BLOCK, &tmDY, &full[s], n_tile * BN + b * CWB, x0, y0, n0);
       }
     }
+    return;
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, ncols);
+  const int wg = warp >> 2, wq = warp & 3;
+  const uint32_t a_off = (uint32_t)((64 * wg / CWA) * A_BLOCK);     // this warpgroup's 64 rows of M
+  float acc[BN / 2];
+  int prev_s = 0;
+  for (int it = 0; it < total; ++it) {
+    const int s = it % p.stages;
+    mbar_wait(&full[s], (it / p.stages) & 1);
+    wgmma_fence();
+    const uint32_t a_addr = smem_u32(smA + (size_t)s * A_BYTES) + a_off;
+    const uint32_t b_addr = smem_u32(smB + (size_t)s * B_BYTES);
+#pragma unroll
+    for (int k = 0; k < PT / 16; ++k)                     // PT pixels = PT/16 x (K = 16); A and B both MN-major
+      Wgmma<BN>::template ss<1, 1>(acc, make_mnmajor_desc<CWA>(a_addr + k * 16 * (CWA * 2), A_BLOCK),
+                                   make_mnmajor_desc<CWB>(b_addr + k * 16 * (CWB * 2), B_BLOCK), (it > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (it > 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+    prev_s = s;
+  }
+  wgmma_wait<0>();
+  if (lane == 0) mbar_arrive(&empty[prev_s]);
+  // accumulator fragment -> fp64 adds (rows R and R + 8, column pairs 8 i + 2 t): the split-K sum does not depend on the order
+  // in which the CTAs of a tile finish
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int R = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+    const int g = R / CWA, c = R % CWA;
+    const int mb = tile_m * G + g;
+    const bool valid = g < nblk;
+    const bool bias_row = (g == ones_g) && c == 0;
+    const int tap = valid ? mb / p.cpt : 0;
+    const int ci = valid ? (mb - tap * p.cpt) * CWA + c : 0;
+    double* dst = nullptr;
+    if (valid && ci < p.Ci) {
+      // segw % 32 == 0 -> both columns of a pair are in one segment
+      dst = p.dw + ((long long)tap * p.Ci + ci) * p.segw;
+    } else if (bias_row) {
+      dst = p.dbias + n_tile * BN;
+    }
+    if (dst == nullptr) continue;
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      const int col = 8 * i + 2 * (lane & 3);
+      double* d = dst;
+      if (!bias_row) {
+        const int co = n_tile * BN + col;
+        const int seg = co / p.segw;
+        d += (long long)seg * p.taps * p.Ci * p.segw + (co - seg * p.segw);
+      } else {
+        d += col;
+      }
+      xu_det_add(d, p.alpha * acc[4 * i + 2 * h]);
+      xu_det_add(d + 1, p.alpha * acc[4 * i + 2 * h + 1]);
+    }
   }
 }
 
@@ -236,22 +175,20 @@ bool pick_tile_w(int N, int H, int W, int& TW, int& TH, int& TN, int PT = 128) {
 }
 int pick_cw(int C) { return C % 64 == 0 ? 64 : (C % 32 == 0 ? 32 : (C % 16 == 0 ? (C > 64 ? 64 : 16) : 0)); }   // 144 -> 64-wide blocks, tail zero-filled
 
-template <int CWA, int CWB, int MT, int PT>
-void launch_wg_mt(const CUtensorMap& x, const CUtensorMap& dy, const WgTcParams& p, dim3 grid, cudaStream_t s) {
-  const size_t stage = (size_t)MT * PT * 128 * 2 + (size_t)p.NB * PT * CWB * 2;
-  const size_t smem = stage * p.stages + 1024 + 8 * (2 * p.stages + 1) + 16;
+template <int CWA, int CWB, int BN>
+void launch_wg_bn(const CUtensorMap& x, const CUtensorMap& dy, const WgTcParams& p, size_t smem, dim3 grid, cudaStream_t s) {
   static bool configured = false;
   if (!configured) {
-    cudaFuncSetAttribute(wgrad_tc_kernel<CWA, CWB, MT, PT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(220 * 1024));
+    cudaFuncSetAttribute(wgrad_tc_kernel<CWA, CWB, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     configured = true;
   }
-  xu_launch(wgrad_tc_kernel<CWA, CWB, MT, PT>, grid, 192, smem, s, x, dy, p);
+  xu_launch(wgrad_tc_kernel<CWA, CWB, BN>, grid, kWgThreads, smem, s, x, dy, p);
 }
 template <int CWA, int CWB>
-void launch_wg(const CUtensorMap& x, const CUtensorMap& dy, const WgTcParams& p, dim3 grid, int mt, int pt, cudaStream_t s) {
-  if (mt == 2) launch_wg_mt<CWA, CWB, 2, 64>(x, dy, p, grid, s);
-  else if (pt == 64) launch_wg_mt<CWA, CWB, 1, 64>(x, dy, p, grid, s);
-  else launch_wg_mt<CWA, CWB, 1, 128>(x, dy, p, grid, s);
+void launch_wg(const CUtensorMap& x, const CUtensorMap& dy, const WgTcParams& p, size_t smem, dim3 grid, cudaStream_t s) {
+  if (p.BN == 128) launch_wg_bn<CWA, CWB, 128>(x, dy, p, smem, grid, s);
+  else if (p.BN == 64) launch_wg_bn<CWA, CWB, 64>(x, dy, p, smem, grid, s);
+  else if constexpr (CWB == 32) launch_wg_bn<CWA, 32, 32>(x, dy, p, smem, grid, s);
 }
 
 }  // namespace
@@ -271,57 +208,32 @@ bool wgrad_tc_supported(int dtype, int N, int H, int W, int Ci, int Co, int ks, 
 
 void launch_wgrad_tc(const WgradArgs& a, cudaStream_t s) {
   WgTcParams p;
-  if ((reinterpret_cast<uintptr_t>(a.dw) & 15) || (a.dbias && (reinterpret_cast<uintptr_t>(a.dbias) & 15))) {
-    xu_set_kernel_error("wgrad_tc: gradient leaves must be 16-byte aligned (vector reds)");
-    return;
-  }
-  // two M tiles per CTA over 64-pixel steps (see the kernel) where there are at least two M tiles to pair, the dY tile is the
-  // larger operand of a stage and the pixel count is large (XUNET_WGRAD_M2=1 turns it on: experimental)
-  int mt = 1;
-  {
-    const char* e = getenv("XUNET_WGRAD_M2");
-    int tw, th, tn;
-    const int cw = pick_cw(a.Ci);
-    if (e && e[0] == '1' && a.stride == 1 && cw >= 32 && a.Co >= 128 && a.ks * a.ks * ((a.Ci + cw - 1) / cw) >= 2 * (128 / cw) &&
-        (long long)a.N * a.Ho * a.Wo >= 16384 && pick_tile_w(a.N, a.Ho, a.Wo, tw, th, tn, 64))
-      mt = 2;
-  }
-  // 64-pixel steps with one M tile: half-sized stages, twice as many (XUNET_WGRAD_PT=64; only where the 128-pixel ring is 2 deep)
-  int pt = mt == 2 ? 64 : 128;
-  {
-    const char* e = getenv("XUNET_WGRAD_PT");
-    int tw, th, tn;
-    const int cwb0 = a.Co % 64 == 0 ? 64 : 32;
-    const int bn0 = a.Co <= 256 ? a.Co : 256;
-    const size_t stage128 = (size_t)32768 + (size_t)(bn0 / cwb0) * 128 * cwb0 * 2;
-    if (mt == 1 && e && atoi(e) == 64 && a.stride == 1 && (200 * 1024) / stage128 < 3 && pick_tile_w(a.N, a.Ho, a.Wo, tw, th, tn, 64)) pt = 64;
-  }
-  if (!pick_tile_w(a.N, a.Ho, a.Wo, p.TW, p.TH, p.TN, pt)) { xu_set_kernel_error("wgrad_tc: unsupported spatial shape"); return; }
+  if (!pick_tile_w(a.N, a.Ho, a.Wo, p.TW, p.TH, p.TN)) { xu_set_kernel_error("wgrad_tc: unsupported spatial shape"); return; }
   p.tiles_x = a.Wo / p.TW; p.tiles_y = a.Ho / p.TH; p.ptiles = p.tiles_x * p.tiles_y * (a.N / p.TN);
   p.Ci = a.Ci; p.Co = a.Co; p.ks = a.ks; p.taps = a.ks * a.ks; p.segw = a.segw;
   p.stride = a.stride; p.pad_h = a.pad_h; p.pad_w = a.pad_w;
   const int cwa = pick_cw(a.Ci);
   const int cwb = a.Co % 64 == 0 ? 64 : 32;
   p.cpt = (a.Ci + cwa - 1) / cwa; p.MB = p.taps * p.cpt;
-  p.BN = a.Co <= 256 ? a.Co : 256; p.NB = p.BN / cwb;
-  p.alpha = a.alpha; p.dw = a.dw;
-  const int G = mt * (128 / cwa);
-  p.dbias = a.dbias;
+  // wgmma N: 128, 64 or 32 (a 256-column tile would spill its 128 accumulator registers per thread)
+  p.BN = a.Co % 128 == 0 ? 128 : (a.Co % 64 == 0 ? 64 : 32);
+  p.alpha = a.alpha;
+  const long long ndw = (long long)a.ks * a.ks * a.Ci * a.Co, ndb = a.dbias ? a.Co : 0;
+  double* acc = xu_det_scratch(s, ndw + ndb);
+  if (acc == nullptr) return;
+  p.dw = acc;
+  const int G = 128 / cwa;
+  p.dbias = a.dbias ? acc + ndw : nullptr;
   const int tiles_m = a.dbias != nullptr ? p.MB / G + 1 : (p.MB + G - 1) / G;   // room for the all-ones bias block
   const int tiles_n = a.Co / p.BN;
-  const size_t stage = (size_t)mt * pt * 128 * 2 + (size_t)p.NB * pt * cwb * 2;
-  int stages = (int)((200 * 1024) / stage);
+  const size_t stage = (size_t)128 * 128 * 2 + (size_t)p.BN * 128 * 2;
+  int stages = (int)((225 * 1024) / stage);
   if (stages > 4) stages = 4;
   if (stages < 1) stages = 1;
   p.stages = stages;
-  {
-    static const char* env = getenv("XUNET_TMA_PREFETCH");      // off by default: measured slower (profiles/r02_l2_prefetch.md)
-    p.prefetch = (env && atoi(env) > 0) ? (atoi(env) + 1) / 2 : 0;     // wgrad steps are twice as long as conv steps
-  }
   // split-K factor: one CTA per SM (the ring takes all of shared memory), so the launch runs in ceil(tiles*k / SMs) waves of
-  // ceil(ptiles / k) pixel tiles each.  Rounding k UP to cover the SMs (round 1: 19 tiles -> k = 8 -> 152 CTAs on 148 SMs) costs a
-  // whole second wave for 4 CTAs: 256->256 @128^2 ran at 0.38 of peak because of it.  Minimise waves x tiles-per-CTA instead
-  // (ties -> fewer splits: every split adds M*N fp32 reds).
+  // ceil(ptiles / k) pixel tiles each.  Rounding k UP to cover the SMs can cost a whole second wave for a handful of CTAs, so
+  // minimise waves x tiles-per-CTA instead (ties -> fewer splits: every split adds M*N fp32 reds).
   int ksplit = 1;
   {
     const long long T = (long long)tiles_m * tiles_n, sms = xu_num_sms();
@@ -329,7 +241,7 @@ void launch_wgrad_tc(const WgradArgs& a, cudaStream_t s) {
     const int kmax = p.ptiles < 64 ? p.ptiles : 64;
     for (int k = 1; k <= kmax; ++k) {
       const long long waves = (T * k + sms - 1) / sms, per = (p.ptiles + k - 1) / k;
-      const long long cost = waves * (per + 8);        // +8: per-CTA pipeline fill + TMEM read-out + reds, in pixel-tile units
+      const long long cost = waves * (per + 8);        // +8: per-CTA pipeline fill + reds, in pixel-tile units
       if (best < 0 || cost < best) { best = cost; ksplit = k; }
     }
     static const char* env = getenv("XUNET_WGRAD_KSPLIT_CEIL");     // A/B switch: the round-1 rule
@@ -345,22 +257,19 @@ void launch_wgrad_tc(const WgradArgs& a, cudaStream_t s) {
   uint64_t ys[3] = {(uint64_t)a.Co * 2, (uint64_t)a.Wo * a.Co * 2, (uint64_t)a.Ho * a.Wo * a.Co * 2};
   uint32_t yb[4] = {(uint32_t)cwb, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TN};
   if (!xu_encode_bf16_map(&tx, a.x, 4, xd, xs, xb, cwa, xe) || !xu_encode_bf16_map(&ty, a.dy, 4, yd, ys, yb, cwb)) return;
-  {
-    // measured and NOT a win (full-128^2 step 55.81 ms with, 56.08 / 55.72 ms without; per-shape 1016 vs 1046 TFLOP/s): the single
-    // producer lane is not what bounds the K loop.  XUNET_WGRAD_TWO_PRODUCERS=1 turns it on.
-    const char* e = getenv("XUNET_WGRAD_TWO_PRODUCERS");
-    p.two_prod = (e && e[0] == '1') ? 1 : 0;
-  }
+  const size_t smem = stage * p.stages + 1024 + 8 * 2 * p.stages + 16;
   dim3 grid((unsigned)tiles_m, (unsigned)tiles_n, (unsigned)ksplit);
   {
     static const bool log = getenv("XUNET_CONV_LOG") != nullptr;      // tools/conv_step_profile.py matches these lines with CUPTI times
-    if (log) fprintf(stderr, "wgrad_tc N=%d %dx%d Ci=%d Co=%d ks=%d st=%d mt=%d pt=%d ksplit=%d tm=%d tn=%d stages=%d ptiles=%d\n", a.N, a.Ho, a.Wo, a.Ci,
-                     a.Co, a.ks, a.stride, mt, pt, ksplit, tiles_m, tiles_n, p.stages, p.ptiles);
+    if (log) fprintf(stderr, "wgrad_tc N=%d %dx%d Ci=%d Co=%d ks=%d st=%d BN=%d ksplit=%d tm=%d tn=%d stages=%d ptiles=%d\n", a.N, a.Ho, a.Wo, a.Ci,
+                     a.Co, a.ks, a.stride, p.BN, ksplit, tiles_m, tiles_n, p.stages, p.ptiles);
   }
-  if (cwa == 64 && cwb == 64) launch_wg<64, 64>(tx, ty, p, grid, mt, pt, s);
-  else if (cwa == 64) launch_wg<64, 32>(tx, ty, p, grid, mt, pt, s);
-  else if (cwa == 32 && cwb == 64) launch_wg<32, 64>(tx, ty, p, grid, mt, pt, s);
-  else if (cwa == 32) launch_wg<32, 32>(tx, ty, p, grid, mt, pt, s);
-  else if (cwb == 64) launch_wg<16, 64>(tx, ty, p, grid, mt, pt, s);
-  else launch_wg<16, 32>(tx, ty, p, grid, mt, pt, s);
+  if (cwa == 64 && cwb == 64) launch_wg<64, 64>(tx, ty, p, smem, grid, s);
+  else if (cwa == 64) launch_wg<64, 32>(tx, ty, p, smem, grid, s);
+  else if (cwa == 32 && cwb == 64) launch_wg<32, 64>(tx, ty, p, smem, grid, s);
+  else if (cwa == 32) launch_wg<32, 32>(tx, ty, p, smem, grid, s);
+  else if (cwb == 64) launch_wg<16, 64>(tx, ty, p, smem, grid, s);
+  else launch_wg<16, 32>(tx, ty, p, smem, grid, s);
+  xu_det_fold(a.dw, acc, ndw, s);
+  if (a.dbias) xu_det_fold(a.dbias, acc + ndw, ndb, s);
 }

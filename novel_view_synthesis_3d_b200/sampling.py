@@ -1,4 +1,4 @@
-"""DDPM ancestral sampler with classifier-free guidance (reference sampling.py:16-53, 73-76, 119-151) on the B200 path.
+"""DDPM ancestral sampler with classifier-free guidance (reference sampling.py:16-53, 73-76, 119-151) on the CUDA path.
 
 Reference behaviour (steps=1000, w=3): per step two model evaluations (cond_mask=1 / 0) -- here ONE forward of a 2B batch
 [cond ; uncond] -- eps=(1+w)eps_c-w eps_u, x0=clip(predict_start_from_noise), posterior mean/variance, z<-mean+sigma*N(0,1)

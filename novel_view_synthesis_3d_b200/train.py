@@ -1,4 +1,4 @@
-"""Training step of the reference (train.py:36-76) on the B200 path.
+"""Training step of the reference (train.py:36-76) on the CUDA path.
 
 Reference call shapes are kept:
     state = create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_sidelength)

@@ -4,7 +4,7 @@
     params = model.init({'params': key, 'dropout': key}, sample, cond_mask=np.zeros(B), train=True)['params']
     eps = model.apply({'params': params}, batch, cond_mask=mask, train=True, rngs={'dropout': key})
 
-All compute runs in libxunet_b200.so (hand-written sm_100a CUDA); PyTorch is used only for device memory,
+All compute runs in libxunet_b200.so (hand-written sm_90a CUDA); PyTorch is used only for device memory,
 streams and torch.distributed.  There is no CPU / eager fallback: without the library or a GPU this raises.
 """
 from __future__ import annotations
@@ -27,7 +27,7 @@ INPUT_ORDER = BATCH_KEYS + ('cond_mask', 'noise')     # segment order of Engine.
 
 @dataclass(frozen=True)
 class XUNetConfig:
-    """The nine XUNet attributes of model/xunet.py:207-215 (+ the two B200-side knobs)."""
+    """The nine XUNet attributes of model/xunet.py:207-215 (+ the two implementation knobs)."""
     ch: int = 32
     ch_mult: Tuple[int, ...] = (1, 2)
     emb_ch: int = 32
@@ -116,7 +116,7 @@ class Engine:
 
     def __init__(self, cfg: XUNetConfig, B: int, S: int, training: bool, device=None):
         if not torch.cuda.is_available():
-            raise RuntimeError('novel_view_synthesis_3d_b200 needs a CUDA device (B200, sm_100a); there is no CPU path')
+            raise RuntimeError('novel_view_synthesis_3d_b200 needs a CUDA device (H100, sm_90a); there is no CPU path')
         self.lib = _lib.load()
         self.cfg, self.B, self.S, self.training = cfg, B, S, training
         self.device = torch.device(device if device is not None else f'cuda:{torch.cuda.current_device()}')

@@ -1,7 +1,7 @@
 """CPU ORACLE for the X-UNet hot path  --  TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
-    PARITY UNPINNED: the reference (JAX/Flax, /root/reference) cannot be imported in this
-    image (jax, flax, optax, visu3d are absent and there is no network) and the reference
+    PARITY UNPINNED: the reference (JAX/Flax) cannot be imported in the
+    project's environment (jax, flax, optax, visu3d are absent and there is no network) and the reference
     ships no tests / golden vectors.  This file is a line-by-line CPU restatement of
     `model/xunet.py`, `train.py:36-76` and `sampling.py:16-53,73-76,119-151` in torch-CPU
     (fp64 = truth, fp32 = what JAX-CPU would produce and the timed CPU baseline).  Its
@@ -12,7 +12,7 @@
     implementation (torch.nn.functional.group_norm / scaled_dot_product_attention / avg_pool2d /
     interpolate / conv2d with explicit padding, tests/test_oracle.py::test_primitive_*), so the
     oracle is no longer "one author's reading, twice"; (ii) `Bf16Emulation` restates WHERE the
-    B200 engine rounds to bf16 (stored activations / gradients, tensor-core weight shadows,
+    CUDA engine rounds to bf16 (stored activations / gradients, tensor-core weight shadows,
     attention probabilities) so the product dtype can be held to a tight tolerance too.
 
 Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline / --impl reference

@@ -1,7 +1,7 @@
 """GPU parity at the widths of the configuration the project is about: full 3DiM X-UNet (ch=256, ch_mult=(1,2,2,4),
 emb_ch=1024, num_res_blocks=3, 8 heads; BASELINE.json configs[2]/[3]; reference model/xunet.py:205-280 with those attributes).
 
-* operator level: tcgen05 conv / dgrad / wgrad at Cin in {768, 1024, 1536, 2048}, Co in {512, 1024, 2048}, the FiLM 1x1
+* operator level: wgmma conv / dgrad / wgrad at Cin in {768, 1024, 1536, 2048}, Co in {512, 1024, 2048}, the FiLM 1x1
   GEMM 1024 -> 2048, the fused q|k|v projection at C = 1024, attention at (L=1024, hd=64) and (L=256, hd=128) forward and
   backward -- against fp64 torch restatements evaluated on the same device (independent library kernels, not ours);
 * model level: the whole full-3DiM network, B=1, 64x64 (0.88 TFLOP forward): eps_hat and EVERY parameter gradient against
@@ -49,7 +49,7 @@ FULL_WIDTH_CONV = [
     (2, 16, 2048, 1024, 1, 1),    # skip Dense on the concat
     (2, 16, 1024, 3072, 1, 3),    # fused q|k|v projection, C = 1024 (hd 128)
     (2, 32, 512, 1536, 1, 3),     # fused q|k|v projection, C = 512 (hd 64)
-    # pair units (two 8 x 16 tiles per pipeline step, conv_tc.cu `m2`): forward and data gradient
+    # wide 3x3 convolutions at the larger sides: forward and data gradient
     (2, 128, 256, 256, 3, 1),     # level-0 Conv_0 / Conv_1 at 128 x 128
     (4, 64, 512, 512, 3, 1),      # level-1 Conv_0 / Conv_1
     (8, 64, 512, 256, 3, 1),      # Ci != Co

@@ -282,7 +282,7 @@ def test_stochastic_conditioning_matches_oracle_loop():
 
 
 def test_flax_checkpoint_roundtrip_drives_the_gpu_path(tmp_path):
-    """sampling.py:106-114: parameters restored from a (device-axis) Flax msgpack checkpoint run on the B200 path."""
+    """sampling.py:106-114: parameters restored from a (device-axis) Flax msgpack checkpoint run on the CUDA path."""
     from novel_view_synthesis_3d_b200 import checkpoint as ck
     model = P.XUNet(**TINY, dtype='fp32')
     S, B = 16, 2

@@ -208,7 +208,7 @@ def test_sampler_update_matches_oracle(lib):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# tcgen05 / TMEM / TMA implicit-GEMM convolution (impl=1) against the fp64 restatement (and therefore the SIMT kernel)
+# wgmma / TMA implicit-GEMM convolution (impl=1) against the fp64 restatement (and therefore the SIMT kernel)
 # ----------------------------------------------------------------------------------------------------------------
 TC_CASES = [
     # N, H, W, Ci, Co, ks, nseg
@@ -404,9 +404,9 @@ def test_conv_tcgen05_strided_forward_and_wgrad(lib, case):
 
 @pytest.mark.parametrize('case', [(2, 128, 32, 2, 0), (4, 1024, 64, 4, 1), (2, 256, 64, 2, 0), (2, 256, 64, 4, 1)])
 def test_attention_tcgen05_bwd_single_kernel_fold(lib, case, monkeypatch):
-    """head_dim <= 32: with a zeroed scratch buffer the fused backward forms D itself and the last key-tile CTA of every
-    (frame, head) rounds dQ and re-zeroes the scratch (no prep / store kernels): same gradients, scratch all-zero afterwards,
-    and a second call on the same scratch is identical."""
+    """XUNET_OP_ATTN_FOLD=1: the caller keeps its scratch buffer all-zero between calls and the backward (prep, dK/dV/dQ,
+    dQ store) hands it back all-zero (the store kernel re-zeroes the D rows): correct gradients, scratch all-zero afterwards,
+    and a second call on the same scratch gives the same gradients."""
     monkeypatch.setenv('XUNET_OP_ATTN_FOLD', '1')
     N, L, Cc, heads, cross = case
     hd = Cc // heads
@@ -435,8 +435,8 @@ def test_attention_tcgen05_bwd_single_kernel_fold(lib, case, monkeypatch):
                                         scratch.data_ptr(), dqkv.data_ptr(), N, L, Cc, heads, cross, _stream())
         assert rc == 0, lib.xunet_last_error()
         torch.cuda.synchronize()
-        assert float(scratch.abs().max()) == 0.0                      # dQ accumulator and tickets left clean
+        assert float(scratch.abs().max()) == 0.0                      # D rows left clean
         gq, gk, gv = [rel_l2(a.float(), b) for a, b in zip(torch.split(dqkv, Cc, dim=-1), torch.split(qr.grad, Cc, dim=-1))]
         assert max(gq, gk, gv) < 4e-2, (gq, gk, gv)
         outs.append(dqkv.float().clone())
-    assert rel_l2(outs[1], outs[0]) < 1e-3                            # (fp32 atomics: last-bit differences only)
+    assert rel_l2(outs[1], outs[0]) < 1e-3                            # same inputs, same gradients

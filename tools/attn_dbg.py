@@ -1,4 +1,4 @@
-"""Time the tcgen05 attention backward at the bench shape (op level, CUDA events), for A/B experiments."""
+"""Time the wgmma attention backward at the bench shape (op level, CUDA events), for A/B experiments."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""Time the tcgen05 attention forward at the bench shape (op level, CUDA events)."""
+"""Time the wgmma attention forward at the bench shape (op level, CUDA events)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""tcgen05 conv kernels at full-3DiM shapes: TFLOP/s of forward, dgrad, wgrad (kernel alone, weights pre-converted)."""
+"""wgmma conv kernels at full-3DiM shapes: TFLOP/s of forward, dgrad, wgrad (kernel alone, weights pre-converted)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ['XUNET_OP_CACHE_SHADOW'] = '1'

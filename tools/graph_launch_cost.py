@@ -1,4 +1,4 @@
-"""Host cost of replaying the captured forward graph, SIMT-only vs tcgen05 kernels."""
+"""Host cost of replaying the captured forward graph, SIMT-only vs wgmma kernels."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

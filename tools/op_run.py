@@ -27,7 +27,7 @@ if which in ('conv', 'all'):
             assert lib.xunet_op_conv(1, 1, x.data_ptr(), w.data_ptr(), b.data_ptr(), None, y.data_ptr(), N, H, H, Ci, Co, 3, 1, 1, 1.0, st) == 0
             assert lib.xunet_op_conv_wgrad(1, 1, x.data_ptr(), y.data_ptr(), dw.data_ptr(), db.data_ptr(), N, H, H, Ci, Co, 3, 1, 1, 1.0, st) == 0
 if which in ('full1x1', 'fullshapes'):
-    # full-3DiM per-pixel GEMMs (FiLM Dense / skip Dense): the shapes profiles/r01_full_model_and_conv_shapes.md lists at 0.36-0.46
+    # full-3DiM per-pixel GEMMs (FiLM Dense / skip Dense)
     for (H, Ci, Co) in ((32, 1024, 2048), (128, 1024, 512)):
         Nn = 8
         x = torch.randn(Nn, H, H, Ci, device='cuda').to(bf); w = torch.randn(Ci * Co, device='cuda') * 0.02

@@ -1,7 +1,7 @@
-"""SASS evidence for the tcgen05 / TMA kernels: per-kernel counts of the Blackwell-only mnemonics in the shipped .so
-(`cuobjdump -sass`), plus a short excerpt around the first UTC*MMA of each kernel.  CPU-only (no GPU needed).
+"""SASS evidence for the wgmma / TMA kernels: per-kernel counts of the Hopper tensor-core, TMA and mbarrier mnemonics in the
+built .so (`cuobjdump -sass`), plus a short excerpt around the first HGMMA of each kernel.  CPU-only (no GPU needed).
 
-    python tools/sass_summary.py > profiles/r02_sass_summary.md
+    python tools/sass_summary.py > sass_summary.md
 """
 import collections
 import os
@@ -11,7 +11,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, 'novel_view_synthesis_3d_b200', 'libxunet_b200.so')
-MNEMONICS = ['UTCHMMA', 'UTCBAR', 'LDTM', 'STTM', 'UTMALDG', 'UTMASTG', 'UTMAREDG', 'UBLKCP', 'UTCCP', 'SYNCS', 'REDG', 'RED.E', 'ATOMG', 'HMMA', 'MUFU.EX2', 'SHFL']
+MNEMONICS = ['HGMMA', 'WARPGROUP', 'UTMALDG', 'UTMASTG', 'UTMAREDG', 'UTMAPF', 'UBLKCP', 'SYNCS', 'REDG', 'RED.E', 'ATOMG', 'DADD', 'HMMA', 'MUFU.EX2', 'SHFL']
 
 
 def main():
@@ -25,9 +25,9 @@ def main():
         elif cur is not None:
             kernels[cur].append(line)
     demangle = lambda n: subprocess.run(['c++filt', n], capture_output=True, text=True).stdout.strip()
-    print('# SASS summary of libxunet_b200.so (cuobjdump -sass, sm_100a)\n')
-    print('Counts of Blackwell-native mnemonics per kernel (tcgen05.mma -> UTCHMMA, tcgen05.ld -> LDTM, TMA -> UTMALDG/UBLKCP, '
-          'tcgen05.commit -> UTCBAR, mbarrier -> SYNCS).  No HMMA (legacy mma.sync) anywhere.\n')
+    print('# SASS summary of libxunet_b200.so (cuobjdump -sass, sm_90a)\n')
+    print('Counts of Hopper-native mnemonics per kernel (wgmma.mma_async -> HGMMA, wgmma fence / commit / wait -> WARPGROUP, '
+          'TMA -> UTMALDG/UTMASTG/UTMAREDG/UBLKCP, mbarrier -> SYNCS, fp64 reductions -> DADD / RED.E).  HMMA = legacy mma.sync.\n')
     print('| kernel | instr | ' + ' | '.join(MNEMONICS) + ' |')
     print('|---|---|' + '---|' * len(MNEMONICS))
     total = collections.Counter()
@@ -35,13 +35,13 @@ def main():
     for name, lines in kernels.items():
         ins = [l for l in lines if re.search(r'/\*[0-9a-f]{4}\*/', l)]
         cnt = {mn: sum(1 for l in ins if re.search(r'(?<![A-Z])' + re.escape(mn), l)) for mn in MNEMONICS}
-        if not any(cnt[mn] for mn in ('UTCHMMA', 'LDTM', 'UTMALDG', 'UBLKCP')):
+        if not any(cnt[mn] for mn in ('HGMMA', 'UTMALDG', 'UBLKCP')):
             continue
         total.update(cnt)
         short = re.sub(r'\(.*', '', demangle(name).replace('(anonymous namespace)::', '')).replace('void ', '')
         print(f'| `{short}` | {len(ins)} | ' + ' | '.join(str(cnt[mn]) for mn in MNEMONICS) + ' |')
         for i, l in enumerate(ins):
-            if 'UTCHMMA' in l:
+            if 'HGMMA' in l:
                 excerpts.append((short, [re.sub(r'\s+', ' ', x.strip()) for x in ins[max(0, i - 3):i + 4]]))
                 break
     print('| **total** | | ' + ' | '.join(str(total[mn]) for mn in MNEMONICS) + ' |\n')
