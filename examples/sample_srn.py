@@ -2,6 +2,7 @@
 ancestral sampler, write PNGs (the reference blocks in cv2.imshow, which cannot run headless).
 
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --steps 256 --out results/
+    python examples/sample_srn.py cars_train_val --ckpt checkpoints --prefix ema --steps 256 --out results_ema/
 """
 import argparse
 import os
@@ -18,6 +19,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('folder')
     ap.add_argument('--ckpt', default='checkpoints')
+    ap.add_argument('--prefix', default='model', help="checkpoint prefix: 'ema' samples the weight EMA of train_srn.py")
     ap.add_argument('--steps', type=int, default=1000)       # the reference runs all 1000 steps, sampling.py:128
     ap.add_argument('--w', type=float, default=3.0)          # sampling.py:133
     ap.add_argument('--views', type=int, default=1)
@@ -27,7 +29,7 @@ def main():
                     help='3DiM stochastic conditioning: generate this many further views autoregressively (the poses of the '
                          'next pairs drawn from the loader), each denoising step conditioned on a random view of the pool')
     a = ap.parse_args()
-    params = P.checkpoint.restore_checkpoint(a.ckpt, prefix='model')
+    params = P.checkpoint.restore_checkpoint(a.ckpt, prefix=a.prefix)
     if params is None:
         raise FileNotFoundError('Checkpoint does not exist')                                          # sampling.py:111-112
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50)

@@ -1,7 +1,10 @@
 """train.py look-alike on the CUDA path (reference: train.py:78-176).  Differences from the reference script: imports,
-a sharded batch under torchrun, device-side forward diffusion, and a Flax-format checkpoint every `save_every` steps.
+a sharded batch under torchrun, device-side forward diffusion, and Flax-format checkpoints every `save_every` steps: the
+params (model<step>), the weight EMA with --ema-decay (ema<step>, a params tree like model<step>), and the whole training
+state (state<step>: params, Adam moments and count, EMA, cond_mask streams) that --resume continues from.
 
-    python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 1000
+    python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 1000 --ema-decay 0.9999
+    python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 2000 --ema-decay 0.9999 --resume
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_srn.py cars_train_val
 """
 import argparse
@@ -26,27 +29,36 @@ def main():
     ap.add_argument('--steps', type=int, default=100000)     # train_num_steps, :86
     ap.add_argument('--save-every', type=int, default=1000)  # :87
     ap.add_argument('--dtype', default='bf16')
+    ap.add_argument('--ema-decay', type=float, default=None,
+                    help='keep an exponential moving average of the weights (e.g. 0.9999) and save it as ema<step>')
+    ap.add_argument('--resume', action='store_true', help='continue from the latest state<step> checkpoint')
+    ap.add_argument('--ckpt', default='checkpoints')
     a = ap.parse_args()
     local = xdist.init_from_env('nccl')
     rank, world = xdist.rank(), xdist.world_size()
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50, seed=rank)      # train.py:99-104
     model = P.XUNet(dtype=a.dtype)
-    state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model)
+    state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model, ema_decay=a.ema_decay)
+    if a.resume and P.checkpoint.restore_train_state(a.ckpt, state) is not None and rank == 0:
+        print(f'resumed from step {state.step}')
     step = P.TrainStep(state)
     fd = P.ForwardDiffusion(step.eng)
     stream = ds.batches(a.batch)
-    for it in range(a.steps):
+    for it in range(state.step, a.steps):
         b = next(stream)
         fd.sample(b['target'], seed=it * world + rank)        # z, noise, logsnr, cond_mask on the GPU
         dev = step.eng.inp
         batch = {k: b[k] for k in ('x', 'R1', 't1', 'R2', 't2', 'K')}
         batch.update(z=dev['z'], logsnr=dev['logsnr'])
         loss = step(batch, dev['noise'], cond_mask=dev['cond_mask'])
-        if rank == 0:
-            if it % 50 == 0:
-                print(f'{it}: {float(loss):.4f}')                                                      # train.py:157
-            if it % a.save_every == 0:
-                P.checkpoint.save_checkpoint('checkpoints/', state.params, step=it, prefix='model', add_device_axis=True)
+        if rank == 0 and it % 50 == 0:
+            print(f'{it}: {float(loss):.4f}')                                                          # train.py:157
+        if it % a.save_every == 0:
+            if rank == 0:
+                P.checkpoint.save_checkpoint(a.ckpt, state.params, step=it, prefix='model', add_device_axis=True)
+                if state.ema_params is not None:
+                    P.checkpoint.save_checkpoint(a.ckpt, state.ema_params, step=it, prefix='ema', add_device_axis=True)
+            P.checkpoint.save_train_state(a.ckpt, state, step=state.step)    # collective: every rank calls it
     if rank == 0:
         print('training completed')
 

@@ -131,6 +131,15 @@ int xunet_adam_step(float* params, const float* grads, float* m, float* v, long 
                     const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
                     void* stream);
 
+/* xunet_adam_step followed by the exponential moving average of the weights DDPM-family models are sampled from:
+ *     ema <- d * ema + (1 - d) * params_new        (d = ema_decay, e.g. 0.9999)
+ * fused into the same pass (params_new never leaves registers).  ema: device, n floats, updated in place.  Each product and
+ * the sum are rounded separately in fp32 (no FMA), so a float32 host restatement reproduces ema bit for bit.  params / m / v
+ * come out bit-identical to xunet_adam_step.  ema == NULL or ema_decay outside [0, 1] is an error.  Graph-capturable. */
+int xunet_adam_ema_step(float* params, const float* grads, float* m, float* v, float* ema, long long n, long long step,
+                        const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
+                        double ema_decay, void* stream);
+
 /* One ancestral update of sampling.py:128-151 given the 2B-batched model output eps2 =
  * [eps_cond (B,S,S,3); eps_uncond (B,S,S,3)]:  eps=(1+w)eps_c-w eps_u; x0=clip(c_recip z - c_recipm1 eps);
  * z' = c1 x0 + c2 z + sigma * noise.  noise==NULL -> device philox-free hash normal from seed.  z_out may alias z. */

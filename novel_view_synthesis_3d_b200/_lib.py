@@ -53,6 +53,8 @@ SYMBOLS = {
                                       C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'xunet_adam_step': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong,
                                   C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_void_p]),
+    'xunet_adam_ema_step': (C.c_int, [C.c_void_p] * 5 + [C.c_longlong, C.c_longlong, C.c_void_p] + [C.c_double] * 6 +
+                            [C.c_void_p]),
     'xunet_sampler_update': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float,
                                        C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_ulonglong,
                                        C.c_void_p]),

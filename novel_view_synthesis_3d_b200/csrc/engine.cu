@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 100; }
+extern "C" int xunet_version(void) { return 101; }
 
 namespace {
 
@@ -1084,9 +1084,20 @@ extern "C" int xunet_adam_step(float* params, const float* grads, float* m, floa
                                const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
                                void* stream) {
   if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_step: bad argument");
-  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, (cudaStream_t)stream);
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, nullptr, 0.0, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("adam: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_adam_ema_step(float* params, const float* grads, float* m, float* v, float* ema, long long n,
+                                   long long step, const long long* step_dev, double lr, double b1, double b2, double eps,
+                                   double grad_scale, double ema_decay, void* stream) {
+  if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_ema_step: bad argument");
+  if (!ema) return fail("xunet_adam_ema_step: ema is NULL (use xunet_adam_step without an EMA)");
+  if (!(ema_decay >= 0.0 && ema_decay <= 1.0)) return fail("xunet_adam_ema_step: ema_decay %g outside [0, 1]", ema_decay);
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema_decay, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("adam_ema: CUDA error: %s", cudaGetErrorString(e));
 }
 
 extern "C" int xunet_sampler_update(const float* eps2, const float* z, const float* noise, float* z_out, long long n,

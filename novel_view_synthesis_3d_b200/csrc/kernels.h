@@ -117,8 +117,9 @@ void launch_extract_frame1(int dtype, const void* o, float* eps, int B, int S, c
 // loss = ||eps - noise||_F ; dO (2B,S,S,3): frame0 = 0, frame1 = (eps-noise)/loss
 void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_scratch, float* loss_out, void* dO, int B,
                  int S, cudaStream_t s);
+// ema == nullptr: plain Adam; otherwise also ema = decay*ema + (1-decay)*p_new in the same pass
 void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                 double lr, double b1, double b2, double eps, double grad_scale, cudaStream_t s);
+                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay, cudaStream_t s);
 void launch_sampler_update(const float* eps2, const float* z, const float* noise, float* z_out, long long n, float w,
                            float c_recip, float c_recipm1, float c1, float c2, float sigma, unsigned long long seed,
                            cudaStream_t s);

@@ -1577,10 +1577,14 @@ void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_s
 
 // optax.adam (train.py:45, 74-76).  (1-b1), (1-b2) and the bias corrections are formed in double (optax forms them
 // from python floats) and only then rounded to fp32.
+// EMA = true also folds the weight EMA into the same pass: ema = d*ema + (1-d)*p_new with p_new still in registers (8 more
+// bytes per parameter instead of 12 for a separate pass).  The _rn intrinsics forbid FMA contraction, so a float32 numpy
+// restatement matches bit for bit.
+template <bool EMA>
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                                   float* __restrict__ v, long long n, long long step,
+                                                   float* __restrict__ v, float* __restrict__ ema, long long n, long long step,
                                                    const long long* __restrict__ step_dev, double lr, double b1d, double b2d,
-                                                   float eps, float gs) {
+                                                   float eps, float gs, double decay) {
   xu_grid_dep_sync();
   __shared__ float sc[2];
   if (threadIdx.x == 0) {
@@ -1591,10 +1595,13 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
   __syncthreads();
   const float c1 = sc[0], c2 = sc[1];
   const float b1 = (float)b1d, b2 = (float)b2d, omb1 = (float)(1.0 - b1d), omb2 = (float)(1.0 - b2d), lrf = (float)lr;
-  // 16-byte accesses (7 streams of n floats: 4 read, 3 written -- the kernel is pure HBM traffic); scalar path for a ragged tail or
-  // unaligned sub-ranges
-  const bool vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
-                     reinterpret_cast<uintptr_t>(v)) & 15) == 0;
+  const float d = (float)decay, omd = (float)(1.0 - decay);
+  // 16-byte accesses (7 streams of n floats: 4 read, 3 written; 9 with the EMA: 5 read, 4 written -- the kernel is pure HBM
+  // traffic); scalar path for a ragged tail or unaligned sub-ranges
+  uintptr_t addr_or = reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+                      reinterpret_cast<uintptr_t>(v);
+  if (EMA) addr_or |= reinterpret_cast<uintptr_t>(ema);
+  const bool vec = (addr_or & 15) == 0;
   const long long n4 = vec ? (n >> 2) : 0;
   auto upd = [&](float gi, float& mi, float& vi, float& pi) {
     gi *= gs;
@@ -1602,6 +1609,7 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
     vi = b2 * vi + omb2 * gi * gi;
     pi -= lrf * (mi * c1) / (sqrtf(vi * c2) + eps);
   };
+  auto avg = [&](float& ei, float pi) { ei = __fadd_rn(__fmul_rn(d, ei), __fmul_rn(omd, pi)); };
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
     const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + i);
     float4 m4 = reinterpret_cast<float4*>(m)[i], v4 = reinterpret_cast<float4*>(v)[i], p4 = reinterpret_cast<float4*>(p)[i];
@@ -1609,19 +1617,34 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
     reinterpret_cast<float4*>(m)[i] = m4;
     reinterpret_cast<float4*>(v)[i] = v4;
     reinterpret_cast<float4*>(p)[i] = p4;
+    if (EMA) {
+      float4 e4 = reinterpret_cast<float4*>(ema)[i];
+      avg(e4.x, p4.x); avg(e4.y, p4.y); avg(e4.z, p4.z); avg(e4.w, p4.w);
+      reinterpret_cast<float4*>(ema)[i] = e4;
+    }
   }
   for (long long i = n4 * 4 + (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
     float mi = m[i], vi = v[i], pi = p[i];
     upd(g[i], mi, vi, pi);
     m[i] = mi; v[i] = vi; p[i] = pi;
+    if (EMA) {
+      float ei = ema[i];
+      avg(ei, pi);
+      ema[i] = ei;
+    }
   }
 }
 void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                 double lr, double b1, double b2, double eps, double grad_scale, cudaStream_t s) {
+                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay, cudaStream_t s) {
   int blocks = cdiv(n, 256 * 4);   // one float4 per thread and pass
   if (blocks > xu_num_sms() * 8) blocks = xu_num_sms() * 8;
   if (blocks < 1) blocks = 1;
-  xu_launch(adam_kernel, blocks, 256, 0, s, p, g, m, v, n, step, step_dev, lr, b1, b2, (float)eps, (float)grad_scale);
+  if (ema == nullptr)
+    xu_launch(adam_kernel<false>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
+              (float)grad_scale, 0.0);
+  else
+    xu_launch(adam_kernel<true>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
+              (float)grad_scale, decay);
 }
 
 // sampling.py:128-151 elementwise update

@@ -109,6 +109,15 @@ def max_over_ranks(value: float) -> float:
     return float(t.item())
 
 
+def all_gather_object(obj) -> list:
+    """Every rank's picklable `obj`, indexed by rank (gloo and NCCL)."""
+    if world_size() == 1:
+        return [obj]
+    out = [None] * world_size()
+    dist.all_gather_object(out, obj)
+    return out
+
+
 def barrier() -> None:
     if world_size() > 1:
         dist.barrier()

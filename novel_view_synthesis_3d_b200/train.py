@@ -53,29 +53,57 @@ class TrainState:
     img_sidelength: int = 0
     grad_scale: float = 1.0
     reference_quirks: bool = False
+    # exponential moving average of the weights (what DDPM-family models are sampled from), updated inside the Adam pass;
+    # None when create_train_state(ema_decay=None)
+    ema_params: Optional[ParamTree] = None
+    ema_decay: Optional[float] = None
     _mask_rng: np.random.RandomState = None
     _frozen_mask: Optional[np.ndarray] = None
 
     def apply_gradients(self, *, grads, copy: bool = False) -> "TrainState":
-        """TrainState.apply_gradients (train.py:76): one fused Adam pass over the flat buffers.
+        """TrainState.apply_gradients (train.py:76): one fused Adam pass over the flat buffers (plus the EMA update when the
+        state carries one).
 
-        Ownership: by default the flat parameter / moment buffers are updated IN PLACE and the returned state shares
+        Ownership: by default the flat parameter / moment / EMA buffers are updated IN PLACE and the returned state shares
         them, i.e. the OLD state's `params` alias the new values (the reference rebinds `state = update_model(state, ..)`
         and never looks at the old one, train.py:153).  copy=True gives the Flax contract literally: the old state keeps
-        its values and the new state owns fresh buffers (3 x 4 bytes per parameter of extra traffic)."""
+        its values and the new state owns fresh buffers (3 x 4 bytes per parameter of extra traffic, 4 x 4 with EMA)."""
         lib = _lib.load()
         flat_g = grads.flat if isinstance(grads, ParamTree) else grads
+        S, B = self.img_sidelength, self.batch_size
         if copy:
-            newp = self.model.tree_from_flat(self.params.flat.clone(), self.img_sidelength, self.batch_size)
-            self = replace(self, params=newp, opt_state=replace(self.opt_state, mu=self.opt_state.mu.clone(),
-                                                                nu=self.opt_state.nu.clone()))
+            newp = self.model.tree_from_flat(self.params.flat.clone(), S, B)
+            newe = None if self.ema_params is None else self.model.tree_from_flat(self.ema_params.flat.clone(), S, B)
+            self = replace(self, params=newp, ema_params=newe,
+                           opt_state=replace(self.opt_state, mu=self.opt_state.mu.clone(), nu=self.opt_state.nu.clone()))
         p = self.params.flat
         count = self.opt_state.count + 1
         st = torch.cuda.current_stream(p.device).cuda_stream
-        _lib.check(lib.xunet_adam_step(p.data_ptr(), flat_g.data_ptr(), self.opt_state.mu.data_ptr(),
-                                       self.opt_state.nu.data_ptr(), p.numel(), count, None, self.tx.learning_rate,
-                                       self.tx.b1, self.tx.b2, self.tx.eps, self.grad_scale, st), 'xunet_adam_step')
+        _adam_launch(lib, self, flat_g, count, None, self.grad_scale, st)
         return replace(self, step=self.step + 1, opt_state=replace(self.opt_state, count=count))
+
+
+def _adam_launch(lib, s: TrainState, flat_g: torch.Tensor, count: int, step_dev, grad_scale: float, stream: int) -> None:
+    """One Adam pass over the flat buffers of `s`; with an EMA buffer the fused Adam + EMA entry point."""
+    p = s.params.flat
+    st_dev = None if step_dev is None else step_dev.data_ptr()
+    if s.ema_params is None:
+        _lib.check(lib.xunet_adam_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(), s.opt_state.nu.data_ptr(),
+                                       p.numel(), count, st_dev, s.tx.learning_rate, s.tx.b1, s.tx.b2, s.tx.eps, grad_scale,
+                                       stream), 'xunet_adam_step')
+    else:
+        _lib.check(lib.xunet_adam_ema_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(),
+                                           s.opt_state.nu.data_ptr(), s.ema_params.flat.data_ptr(), p.numel(), count, st_dev,
+                                           s.tx.learning_rate, s.tx.b1, s.tx.b2, s.tx.eps, grad_scale, s.ema_decay, stream),
+                   'xunet_adam_ema_step')
+
+
+def _opt_buffers(s: TrainState):
+    """Every flat buffer one Adam pass writes."""
+    bufs = [s.params.flat, s.opt_state.mu, s.opt_state.nu]
+    if s.ema_params is not None:
+        bufs.append(s.ema_params.flat)
+    return bufs
 
 
 def create_sample_data(batch_size, img_sidelength):
@@ -87,9 +115,17 @@ def create_sample_data(batch_size, img_sidelength):
 
 
 def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_sidelength, *, model: XUNet = None,
-                       zero_init: bool = True, reference_quirks: bool = False, init_on_device: bool = False) -> TrainState:
+                       zero_init: bool = True, reference_quirks: bool = False, init_on_device: bool = False,
+                       ema_decay: Optional[float] = None) -> TrainState:
     """train.py:36-47.  Under torch.distributed the parameters of rank 0 are broadcast (the reference gives every
-    device a different init, train.py:122-123 -- an ensemble, not data parallelism)."""
+    device a different init, train.py:122-123 -- an ensemble, not data parallelism).
+
+    ema_decay (e.g. 0.9999, Ho et al. 2020): keep `ema_params`, an exponential moving average of the weights updated in
+    the same kernel as Adam, starting as a copy of the initial parameters.  Every rank updates its own copy; the parameters
+    are identical across ranks after the all-reduce and Adam, so the copies stay identical without a collective.  None
+    (default): no EMA buffer, the optimizer step is plain Adam."""
+    if ema_decay is not None and not (0.0 <= ema_decay <= 1.0):
+        raise ValueError(f'ema_decay must lie in [0, 1], got {ema_decay}')
     model = model or XUNet()
     sample = create_sample_data(train_batch_size, img_sidelength)
     params = model.init({'params': rng, 'dropout': rng_dropout}, sample, cond_mask=np.zeros(train_batch_size), train=True,
@@ -102,9 +138,14 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
     # data parallel: every rank draws its OWN cond_mask stream (and dropout seeds, _dropout_seed) for its shard --
     # identical streams would drop sample b of every shard together, which is not a global batch of world*B
     mask_seed ^= (xdist.rank() * 0x9E3779B9) & 0x7FFFFFFF
+    ema = None
+    if ema_decay is not None:
+        ema = model.tree_from_flat(params.flat.clone(), img_sidelength, train_batch_size)
     return TrainState(step=0, apply_fn=model.apply, params=params, tx=opt, opt_state=st, model=model,
                       batch_size=train_batch_size, img_sidelength=img_sidelength, grad_scale=1.0 / world,
-                      reference_quirks=reference_quirks, _mask_rng=np.random.RandomState(mask_seed & 0x7FFFFFFF))
+                      reference_quirks=reference_quirks, ema_params=ema,
+                      ema_decay=None if ema_decay is None else float(ema_decay),
+                      _mask_rng=np.random.RandomState(mask_seed & 0x7FFFFFFF))
 
 
 def _dropout_seed(step_plus_1: int) -> int:
@@ -212,11 +253,8 @@ class TrainStep:
         e.backward(s.params.flat)
 
     def _adam(self):
-        e, s = self.eng, self.state
         st = torch.cuda.current_stream(self.dev).cuda_stream
-        _lib.check(self.lib.xunet_adam_step(s.params.flat.data_ptr(), e.grads.data_ptr(), s.opt_state.mu.data_ptr(),
-                                            s.opt_state.nu.data_ptr(), s.params.flat.numel(), 0, self.step_dev.data_ptr(),
-                                            s.tx.learning_rate, s.tx.b1, s.tx.b2, s.tx.eps, 1.0 / self.world, st), 'adam')
+        _adam_launch(self.lib, self.state, self.eng.grads, 0, self.step_dev, 1.0 / self.world, st)
 
     def _full_step(self):
         self._fwd_bwd()
@@ -236,8 +274,8 @@ class TrainStep:
         backup = None
         one_graph = self.world == 1 or self.capture_collectives
         if one_graph:
-            # warm-up and capture run real Adam updates: snapshot params/moments and restore them afterwards
-            backup = (s.params.flat.clone(), s.opt_state.mu.clone(), s.opt_state.nu.clone())
+            # warm-up and capture run real Adam updates: snapshot params/moments/EMA and restore them afterwards
+            backup = [t.clone() for t in _opt_buffers(s)]
         try:
             with torch.cuda.stream(self.stream):
                 self._set_hook(one_graph)
@@ -265,7 +303,8 @@ class TrainStep:
             self.capture_collectives = False
             self.graph_fb = self.graph_opt = None
             if backup is not None:
-                s.params.flat.copy_(backup[0]); s.opt_state.mu.copy_(backup[1]); s.opt_state.nu.copy_(backup[2])
+                for t, b in zip(_opt_buffers(s), backup):
+                    t.copy_(b)
             self.eng.seed.copy_(seed0)
             self.step_dev.copy_(step0)
             return self._capture()
@@ -273,7 +312,8 @@ class TrainStep:
             self._set_hook(False)
         torch.cuda.synchronize(self.dev)
         if backup is not None:
-            s.params.flat.copy_(backup[0]); s.opt_state.mu.copy_(backup[1]); s.opt_state.nu.copy_(backup[2])
+            for t, b in zip(_opt_buffers(s), backup):
+                t.copy_(b)
         self.eng.seed.copy_(seed0)
         self.step_dev.copy_(step0)
 

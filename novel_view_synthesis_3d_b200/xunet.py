@@ -93,6 +93,23 @@ def _flatten(tree: dict, prefix='') -> Dict[str, object]:
     return out
 
 
+def pack_flat(params: dict, spec, nparams: int) -> torch.Tensor:
+    """Nested dict of arrays in the Flax tree shape -> host fp32 flat buffer laid out by `spec` ({name: (shape, offset)}).
+    Raises KeyError on missing / unexpected leaves and ValueError on a shape mismatch.  Needs no GPU."""
+    leaves = _flatten(params)
+    missing = set(spec) - set(leaves)
+    extra = set(leaves) - set(spec)
+    if missing or extra:
+        raise KeyError(f'parameter tree mismatch: missing {sorted(missing)[:3]}..., unexpected {sorted(extra)[:3]}...')
+    host = torch.empty(nparams, dtype=torch.float32)
+    for name, (shape, off) in spec.items():
+        v = torch.as_tensor(np.asarray(leaves[name]) if not isinstance(leaves[name], torch.Tensor) else leaves[name])
+        if tuple(v.shape) != tuple(shape):
+            raise ValueError(f'{name}: shape {tuple(v.shape)} != {tuple(shape)}')
+        host[off: off + v.numel()] = v.reshape(-1).to(torch.float32).cpu()
+    return host
+
+
 def is_zero_init_kernel(name: str) -> bool:
     """out_init_scale() leaves (model/xunet.py:11-12): every ResnetBlock's Conv_1 (:85-89) and the top-level Conv_1
     (:276-280).  NOT 'ConditioningProcessor_0/Conv_1/kernel' -- the level-1 pose-embedding conv (:197-202) keeps the
@@ -338,18 +355,7 @@ class XUNet:
         if isinstance(params, ParamTree) and params.flat is not None:
             return params.flat
         eng = self.engine(B, S, False)
-        leaves = _flatten(params)
-        missing = set(eng.spec) - set(leaves)
-        extra = set(leaves) - set(eng.spec)
-        if missing or extra:
-            raise KeyError(f'parameter tree mismatch: missing {sorted(missing)[:3]}..., unexpected {sorted(extra)[:3]}...')
-        host = torch.empty(eng.nparams, dtype=torch.float32)
-        for name, (shape, off) in eng.spec.items():
-            v = torch.as_tensor(np.asarray(leaves[name]) if not isinstance(leaves[name], torch.Tensor) else leaves[name])
-            if tuple(v.shape) != tuple(shape):
-                raise ValueError(f'{name}: shape {tuple(v.shape)} != {tuple(shape)}')
-            host[off: off + v.numel()] = v.reshape(-1).to(torch.float32).cpu()
-        return host.to(eng.device)
+        return pack_flat(params, eng.spec, eng.nparams).to(eng.device)
 
     def init(self, rngs, batch, *, cond_mask=None, train=True, zero_init=True, on_device=False) -> Dict[str, ParamTree]:
         """Flax-style initialisation (train.py:41-43): lecun_normal kernels, zero biases, GroupNorm scale 1,
