@@ -5,6 +5,7 @@ state (state<step>: params, Adam moments and count, EMA, cond_mask streams) that
 
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 1000 --ema-decay 0.9999
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 2000 --ema-decay 0.9999 --resume
+    python examples/train_srn.py cars_train_val --batch 8 --side 64 --max-grad-norm 1 --warmup-steps 5000 --ema-decay 0.9999
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_srn.py cars_train_val
 """
 import argparse
@@ -31,6 +32,10 @@ def main():
     ap.add_argument('--dtype', default='bf16')
     ap.add_argument('--ema-decay', type=float, default=None,
                     help='keep an exponential moving average of the weights (e.g. 0.9999) and save it as ema<step>')
+    ap.add_argument('--max-grad-norm', type=float, default=None,
+                    help='clip the gradient to this global L2 norm (e.g. 1) and skip updates whose norm is not finite')
+    ap.add_argument('--warmup-steps', type=int, default=0,
+                    help='warm the learning rate up linearly from 0 over this many steps (e.g. 5000)')
     ap.add_argument('--resume', action='store_true', help='continue from the latest state<step> checkpoint')
     ap.add_argument('--ckpt', default='checkpoints')
     a = ap.parse_args()
@@ -38,7 +43,8 @@ def main():
     rank, world = xdist.rank(), xdist.world_size()
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50, seed=rank)      # train.py:99-104
     model = P.XUNet(dtype=a.dtype)
-    state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model, ema_decay=a.ema_decay)
+    state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model, ema_decay=a.ema_decay,
+                                 max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps)
     if a.resume and P.checkpoint.restore_train_state(a.ckpt, state) is not None and rank == 0:
         print(f'resumed from step {state.step}')
     step = P.TrainStep(state)
@@ -52,7 +58,8 @@ def main():
         batch.update(z=dev['z'], logsnr=dev['logsnr'])
         loss = step(batch, dev['noise'], cond_mask=dev['cond_mask'])
         if rank == 0 and it % 50 == 0:
-            print(f'{it}: {float(loss):.4f}')                                                          # train.py:157
+            norm = '' if step.grad_norm is None else f'  grad norm {float(step.grad_norm):.4f}'
+            print(f'{it}: {float(loss):.4f}{norm}')                                                    # train.py:157
         if it % a.save_every == 0:
             if rank == 0:
                 P.checkpoint.save_checkpoint(a.ckpt, state.params, step=it, prefix='model', add_device_axis=True)
@@ -60,6 +67,8 @@ def main():
                     P.checkpoint.save_checkpoint(a.ckpt, state.ema_params, step=it, prefix='ema', add_device_axis=True)
             P.checkpoint.save_train_state(a.ckpt, state, step=state.step)    # collective: every rank calls it
     if rank == 0:
+        if state.clip is not None:
+            print(f'skipped steps (non-finite gradient norm): {state.skipped_steps}')
         print('training completed')
 
 

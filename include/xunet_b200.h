@@ -140,6 +140,33 @@ int xunet_adam_ema_step(float* params, const float* grads, float* m, float* v, f
                         const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
                         double ema_decay, void* stream);
 
+/* Global L2 norm of the (scaled) flat gradient, the reduction of optax.clip_by_global_norm:
+ *     *norm_out = (float) sqrt( sum_i fp32(grads[i] * grad_scale)^2 )
+ * Every square is accumulated in fp64, in an order fixed by n alone (no atomics, no dependence on the SM count), so the same
+ * buffer gives the same bits on every run and every GPU.  scratch: device, XUNET_GRAD_NORM_SCRATCH doubles, contents
+ * irrelevant on entry; on completion scratch[0] holds the fp64 sum of squares.  norm_out: device, 1 float.  Two kernels,
+ * no host sync, graph-capturable. */
+#define XUNET_GRAD_NORM_SCRATCH 1024
+int xunet_grad_global_norm(const float* grads, long long n, double grad_scale, double* scratch, float* norm_out,
+                           void* stream);
+
+/* xunet_adam_step (ema == NULL) or xunet_adam_ema_step (ema != NULL) with a linear learning-rate warm-up and clipping by a
+ * global gradient norm read from the device: optax.chain(optax.clip_by_global_norm(max_norm),
+ * optax.adam(optax.linear_schedule(0, lr, warmup_steps))).  With the Adam count `step` (after increment, or *step_dev):
+ *   - learning rate: lr_t = lr * min(step - 1, W) / W in double, rounded to fp32 once (W = warmup_steps; the first update
+ *     uses lr_t = 0, as the schedule's own count starts at 0); W == 0: the constant lr;
+ *   - clipping (norm_dev != NULL, *norm_dev = the norm of grads * grad_scale, e.g. from xunet_grad_global_norm): the scaled
+ *     gradient g is used as is if *norm_dev < max_norm, else as fl(fl(g / norm) * max_norm) (each operation rounded once);
+ *   - non-finite *norm_dev: the step is skipped -- params / m / v / ema are not touched -- and *skipped_dev (device int64)
+ *     is incremented.  The caller's step counter still advances, unlike optax.apply_if_finite, which holds the inner count.
+ * norm_dev == NULL: no clipping and no guard (max_norm and skipped_dev are then ignored).  With *norm_dev < max_norm and
+ * W == 0 the result is bit-identical to xunet_adam_step / xunet_adam_ema_step.  Errors: max_norm <= 0 or NaN,
+ * warmup_steps < 0, skipped_dev == NULL with norm_dev given, ema_decay outside [0, 1] with ema given.  Graph-capturable. */
+int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, float* ema, long long n, long long step,
+                         const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
+                         double ema_decay, const float* norm_dev, double max_norm, long long warmup_steps,
+                         long long* skipped_dev, void* stream);
+
 /* One ancestral update of sampling.py:128-151 given the 2B-batched model output eps2 =
  * [eps_cond (B,S,S,3); eps_uncond (B,S,S,3)]:  eps=(1+w)eps_c-w eps_u; x0=clip(c_recip z - c_recipm1 eps);
  * z' = c1 x0 + c2 z + sigma * noise.  noise==NULL -> device philox-free hash normal from seed.  z_out may alias z. */

@@ -9,6 +9,7 @@ from pathlib import Path
 # XUNET_LIB=<path> loads another build of the same library (same-call A/B of a kernel change against the previous build)
 LIB_PATH = Path(os.environ['XUNET_LIB']).resolve() if os.environ.get('XUNET_LIB') else Path(__file__).resolve().parent / 'libxunet_b200.so'
 MAX_LEVELS = 8
+GRAD_NORM_SCRATCH = 1024       # XUNET_GRAD_NORM_SCRATCH: doubles of scratch xunet_grad_global_norm needs
 DTYPE_F32, DTYPE_BF16 = 0, 1
 RAYS = {'v3d130_ij': 0, 'opencv_uv': 1}
 
@@ -55,6 +56,9 @@ SYMBOLS = {
                                   C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_void_p]),
     'xunet_adam_ema_step': (C.c_int, [C.c_void_p] * 5 + [C.c_longlong, C.c_longlong, C.c_void_p] + [C.c_double] * 6 +
                             [C.c_void_p]),
+    'xunet_grad_global_norm': (C.c_int, [C.c_void_p, C.c_longlong, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'xunet_adam_clip_step': (C.c_int, [C.c_void_p] * 5 + [C.c_longlong, C.c_longlong, C.c_void_p] + [C.c_double] * 6 +
+                             [C.c_void_p, C.c_double, C.c_longlong, C.c_void_p, C.c_void_p]),
     'xunet_sampler_update': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float,
                                        C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_ulonglong,
                                        C.c_void_p]),

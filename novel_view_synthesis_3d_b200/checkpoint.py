@@ -191,41 +191,65 @@ def _set_rng_state(rng: np.random.RandomState, d: dict):
 
 
 def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *, ema: Optional[dict] = None,
-                     rng: Optional[list] = None, add_device_axis: bool = False) -> dict:
+                     rng: Optional[list] = None, add_device_axis: bool = False, clip: bool = False,
+                     schedule: bool = False, skipped: Optional[int] = None) -> dict:
     """The nested dict flax.serialization.to_state_dict gives for a flax.training.train_state.TrainState with
     tx=optax.adam(lr), i.e. chain(scale_by_adam, scale(-lr)):
 
         {'step': int32, 'params': {...}, 'opt_state': {'0': {'count': int32, 'mu': {...}, 'nu': {...}}, '1': {}}}
 
-    plus 'ema_params' (a params-shaped tree) when an EMA is kept, and 'rng': {'<rank>': rng_state_dict(..)} for the host
-    cond_mask stream of every rank.  The Flax / optax part is restated from memory of their published sources and has not
-    been checked against files written by the packages themselves.  add_device_axis=True gives every Flax leaf (not 'rng') the leading pmap axis of
-    length 1, as the reference's pmapped state carries it (train.py:161-167).  params / mu / nu / ema: nested dicts of
-    numpy arrays (leaf_tree)."""
+    With gradient clipping (clip=True) and / or a learning-rate schedule (schedule=True) the optimizer is
+    optax.chain(optax.clip_by_global_norm(c), optax.adam(schedule)); clip_by_global_norm keeps an empty state and
+    scale_by_schedule keeps its own count, so 'opt_state' becomes
+
+        clip and schedule: {'0': {}, '1': {'0': {'count', 'mu', 'nu'}, '1': {'count': int32}}}
+        clip only:         {'0': {}, '1': {'0': {'count', 'mu', 'nu'}, '1': {}}}
+        schedule only:     {'0': {'count', 'mu', 'nu'}, '1': {'count': int32}}
+
+    (the schedule's count equals Adam's: both advance once per update).  Plus 'ema_params' (a params-shaped tree) when an
+    EMA is kept, 'rng': {'<rank>': rng_state_dict(..)} for the host cond_mask stream of every rank, and 'skipped_steps'
+    (int64, updates skipped for a non-finite gradient norm) when given.  The Flax / optax layouts are restated from memory
+    of their published sources and have not been checked against files written by the packages themselves.
+    add_device_axis=True gives every Flax leaf (not 'rng' / 'skipped_steps') the leading pmap axis of length 1, as the
+    reference's pmapped state carries it (train.py:161-167).  params / mu / nu / ema: nested dicts of numpy arrays
+    (leaf_tree)."""
     def ax(t):
         if isinstance(t, dict):
             return {k: ax(v) for k, v in t.items()}
         return np.asarray(t)[None] if add_device_axis else np.asarray(t)
-    tree = {'step': np.asarray(step, dtype=np.int32), 'params': params,
-            'opt_state': {'0': {'count': np.asarray(count, dtype=np.int32), 'mu': mu, 'nu': nu}, '1': {}}}
+    adam = {'count': np.asarray(count, dtype=np.int32), 'mu': mu, 'nu': nu}
+    sched = {'count': np.asarray(count, dtype=np.int32)} if schedule else {}
+    opt = {'0': {}, '1': {'0': adam, '1': sched}} if clip else {'0': adam, '1': sched}
+    tree = {'step': np.asarray(step, dtype=np.int32), 'params': params, 'opt_state': opt}
     if ema is not None:
         tree['ema_params'] = ema
     tree = ax(tree)
     if rng is not None:
         tree['rng'] = {str(r): d for r, d in enumerate(rng)}
+    if skipped is not None:
+        tree['skipped_steps'] = np.asarray(skipped, dtype=np.int64)
     return tree
 
 
 def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     """Inverse of train_state_tree onto flat fp32 host buffers laid out by `spec`.  Returns {'step', 'count', 'params',
-    'mu', 'nu', 'ema' (None if the file has none), 'rng' (list indexed by rank, or None)}.  Detects the pmap device axis
-    from the shape of 'step' and takes replica 0.  Missing / unexpected leaves raise KeyError, wrong shapes ValueError."""
+    'mu', 'nu', 'ema' (None if the file has none), 'rng' (list indexed by rank, or None), 'skipped' (0 if the file has
+    none)}.  Accepts all four optimizer layouts (with and without clipping, with and without a schedule), so a run may
+    turn either on or off when it resumes; a schedule count that differs from Adam's raises ValueError.  Detects the pmap
+    device axis from the shape of 'step' and takes replica 0.  Missing / unexpected leaves raise KeyError, wrong shapes
+    ValueError."""
     tree = dict(tree)
     rng = tree.pop('rng', None)
+    skipped = tree.pop('skipped_steps', None)
     if np.ndim(tree['step']) == 1:
         tree = strip_device_axis(tree, 0)
-    adam = tree['opt_state']['0']
-    out = {'step': int(tree['step']), 'count': int(adam['count'])}
+    opt = tree['opt_state']
+    if 'count' not in opt['0']:          # chain(clip_by_global_norm, adam(..)): the clip state is empty
+        opt = opt['1']
+    adam, sched = opt['0'], opt['1']
+    if 'count' in sched and int(sched['count']) != int(adam['count']):
+        raise ValueError(f"schedule count {int(sched['count'])} differs from the Adam count {int(adam['count'])}")
+    out = {'step': int(tree['step']), 'count': int(adam['count']), 'skipped': 0 if skipped is None else int(skipped)}
     for k, sub in (('params', tree['params']), ('mu', adam['mu']), ('nu', adam['nu']), ('ema', tree.get('ema_params'))):
         out[k] = None if sub is None else pack_flat(sub, spec, nparams)
     out['rng'] = None if rng is None else [rng[str(r)] for r in range(len(rng))]
@@ -234,8 +258,8 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
 
 def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', overwrite: bool = True,
                      add_device_axis: bool = False) -> str:
-    """Writes the whole TrainState -- params, Adam mu / nu / count, step, ema_params when the state keeps an EMA, and the
-    host cond_mask stream of every rank -- to f'{prefix}{step}' in ckpt_dir (layout: train_state_tree).  The file stays a
+    """Writes the whole TrainState -- params, Adam mu / nu / count, step, ema_params when the state keeps an EMA, the count
+    of skipped updates when it clips or warms up, and the host cond_mask stream of every rank -- to f'{prefix}{step}' in ckpt_dir (layout: train_state_tree).  The file stays a
     valid params checkpoint: restore_checkpoint(ckpt_dir, prefix=prefix) returns its params tree.
 
     Under torch.distributed this is collective: every rank must call it; the cond_mask streams are gathered and rank 0
@@ -252,7 +276,9 @@ def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', ove
         tree = train_state_tree(host(state.params.flat), host(state.opt_state.mu), host(state.opt_state.nu),
                                 state.opt_state.count, state.step,
                                 ema=None if state.ema_params is None else host(state.ema_params.flat),
-                                rng=rngs, add_device_axis=add_device_axis)
+                                rng=rngs, add_device_axis=add_device_axis, clip=state.tx.max_grad_norm is not None,
+                                schedule=state.tx.warmup_steps > 0,
+                                skipped=state.skipped_steps if state.clip is not None else None)
         path = save_checkpoint(ckpt_dir, tree, step, prefix=prefix, overwrite=overwrite)
     xdist.barrier()
     return path
@@ -266,7 +292,8 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     The flat device buffers are overwritten in place, never rebound, so a TrainStep already built (and CUDA-graph-captured)
     on `state` stays valid; it re-derives its device step counter and dropout seed from the restored count.  A file without
     EMA restored into a state with one starts the EMA from the restored params; a file with an EMA restored into a state
-    without one ignores it.  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
+    without one ignores it.  The clipping / warm-up settings are those of `state`, whatever the file was written with; the
+    skip counter is restored (0 if the file has none).  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
     freshly seeded streams are kept (with a warning), and a resume is then no longer bit-exact."""
     from . import dist as xdist
     path = ckpt_dir if os.path.isfile(ckpt_dir) else latest_checkpoint(ckpt_dir, prefix)
@@ -280,6 +307,8 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     state.opt_state.nu.copy_(r['nu'])
     if state.ema_params is not None:
         state.ema_params.flat.copy_(r['ema'] if r['ema'] is not None else r['params'])
+    if state.clip is not None:
+        state.clip.skipped.fill_(r['skipped'])
     state.step = r['step']
     state.opt_state.count = r['count']
     world = xdist.world_size()

@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 101; }
+extern "C" int xunet_version(void) { return 102; }
 
 namespace {
 
@@ -1098,6 +1098,31 @@ extern "C" int xunet_adam_ema_step(float* params, const float* grads, float* m, 
   launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema_decay, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("adam_ema: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_grad_global_norm(const float* grads, long long n, double grad_scale, double* scratch, float* norm_out,
+                                      void* stream) {
+  if (!grads || !scratch || !norm_out || n < 0) return fail("xunet_grad_global_norm: bad argument");
+  launch_grad_global_norm(grads, n, grad_scale, scratch, norm_out, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("grad_global_norm: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, float* ema, long long n,
+                                    long long step, const long long* step_dev, double lr, double b1, double b2, double eps,
+                                    double grad_scale, double ema_decay, const float* norm_dev, double max_norm,
+                                    long long warmup_steps, long long* skipped_dev, void* stream) {
+  if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_clip_step: bad argument");
+  if (ema && !(ema_decay >= 0.0 && ema_decay <= 1.0)) return fail("xunet_adam_clip_step: ema_decay %g outside [0, 1]", ema_decay);
+  if (warmup_steps < 0) return fail("xunet_adam_clip_step: warmup_steps %lld < 0", warmup_steps);
+  if (norm_dev) {
+    if (!(max_norm > 0.0)) return fail("xunet_adam_clip_step: max_norm %g must be > 0", max_norm);
+    if (!skipped_dev) return fail("xunet_adam_clip_step: skipped_dev is NULL (needed with norm_dev)");
+  }
+  launch_adam_clip(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema ? ema_decay : 0.0, norm_dev,
+                   max_norm, warmup_steps, skipped_dev, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("adam_clip: CUDA error: %s", cudaGetErrorString(e));
 }
 
 extern "C" int xunet_sampler_update(const float* eps2, const float* z, const float* noise, float* z_out, long long n,

@@ -1647,6 +1647,156 @@ void launch_adam(float* p, const float* g, float* m, float* v, long long n, long
               (float)grad_scale, decay);
 }
 
+// ---- global gradient norm (optax.clip_by_global_norm) ----------------------------------------------------------------------
+// Deterministic by construction: the grid depends on n only, each CTA sums a fixed share of the buffer in a fixed order (per
+// thread in index order, then a fixed shuffle / shared-memory tree), and one CTA adds the per-CTA partials the same way.  Each
+// scaled gradient fp32(g_i * gs) is squared and accumulated in fp64 (the square of an fp32 value is exact in fp64).
+__device__ __forceinline__ double block_sum_fixed(double x, double* red) {   // 256 threads; red: 8 doubles of shared memory
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
+  __syncthreads();
+  double t = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < 8; ++w) t += red[w];
+  return t;   // valid in thread 0
+}
+
+__global__ void __launch_bounds__(256) grad_sumsq_partial_kernel(const float* __restrict__ g, long long n, float gs,
+                                                                 double* __restrict__ partials) {
+  xu_grid_dep_sync();
+  __shared__ double red[8];
+  const bool vec = (reinterpret_cast<uintptr_t>(g) & 15) == 0;
+  const long long n4 = vec ? (n >> 2) : 0;
+  double acc = 0.0;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
+    const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + i);
+    const double x = g4.x * gs, y = g4.y * gs, z = g4.z * gs, w = g4.w * gs;
+    acc = fma(x, x, acc); acc = fma(y, y, acc); acc = fma(z, z, acc); acc = fma(w, w, acc);
+  }
+  for (long long i = n4 * 4 + (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    const double x = __ldg(g + i) * gs;
+    acc = fma(x, x, acc);
+  }
+  const double t = block_sum_fixed(acc, red);
+  if (threadIdx.x == 0) partials[blockIdx.x] = t;
+}
+
+__global__ void __launch_bounds__(256) grad_norm_final_kernel(double* __restrict__ partials, int nparts,
+                                                              float* __restrict__ norm_out) {
+  xu_grid_dep_sync();
+  __shared__ double red[8];
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < nparts; i += 256) acc += partials[i];
+  const double t = block_sum_fixed(acc, red);
+  if (threadIdx.x == 0) {
+    partials[0] = t;   // the fp64 sum of squares stays readable in scratch[0]
+    *norm_out = (float)sqrt(t);
+  }
+}
+
+static int grad_norm_partials(long long n) {
+  long long b = (n + 4095) / 4096;   // at least 16 elements per thread
+  if (b > XUNET_GRAD_NORM_SCRATCH) b = XUNET_GRAD_NORM_SCRATCH;
+  return b < 1 ? 1 : (int)b;
+}
+void launch_grad_global_norm(const float* g, long long n, double grad_scale, double* scratch, float* norm_out,
+                             cudaStream_t s) {
+  const int parts = grad_norm_partials(n);
+  xu_launch(grad_sumsq_partial_kernel, parts, 256, 0, s, g, n, (float)grad_scale, scratch);
+  xu_launch(grad_norm_final_kernel, 1, 256, 0, s, scratch, parts, norm_out);
+}
+
+// adam_kernel with a linear learning-rate warm-up and clipping by a global norm read from the device.  Thread 0 of each CTA
+// forms, from the device step counter, the bias corrections (as adam_kernel), lr_t = lr * min(step - 1, W) / W in double
+// rounded once (optax.linear_schedule(0, lr, W) evaluated at the schedule's count, which lags Adam's by one), and the clip
+// decision of optax.clip_by_global_norm: g' = g if norm < max_norm, else fl(fl(g / norm) * max_norm).  A non-finite norm skips
+// the step: every CTA returns before touching p / m / v / ema and CTA 0 counts it in *skipped.  norm == nullptr: no clipping
+// and no guard.  The Adam and EMA arithmetic is written exactly as in adam_kernel, so with g' == g and lr_t == lr the two give
+// the same bits.
+template <bool EMA>
+__global__ void __launch_bounds__(256) adam_clip_kernel(float* __restrict__ p, const float* __restrict__ g,
+                                                        float* __restrict__ m, float* __restrict__ v, float* __restrict__ ema,
+                                                        long long n, long long step, const long long* __restrict__ step_dev,
+                                                        double lr, double b1d, double b2d, float eps, float gs, double decay,
+                                                        const float* __restrict__ norm_dev, float max_norm, long long warmup,
+                                                        long long* __restrict__ skipped) {
+  xu_grid_dep_sync();
+  __shared__ float sc[4];
+  __shared__ int mode;   // 0: plain gradient, 1: clipped, 2: skip the step
+  if (threadIdx.x == 0) {
+    const long long st = step_dev != nullptr ? *step_dev : step;
+    sc[0] = (float)(1.0 / (1.0 - pow(b1d, (double)st)));
+    sc[1] = (float)(1.0 / (1.0 - pow(b2d, (double)st)));
+    const long long c = st - 1;
+    sc[2] = warmup > 0 ? (float)(lr * (double)(c < warmup ? c : warmup) / (double)warmup) : (float)lr;
+    int md = 0;
+    sc[3] = 1.f;
+    if (norm_dev != nullptr) {
+      const float nrm = *norm_dev;
+      sc[3] = nrm;
+      md = !isfinite(nrm) ? 2 : (nrm < max_norm ? 0 : 1);
+      if (md == 2 && blockIdx.x == 0) *skipped += 1;
+    }
+    mode = md;
+  }
+  __syncthreads();
+  const int md = mode;
+  if (md == 2) return;
+  const float c1 = sc[0], c2 = sc[1], lrf = sc[2], nrm = sc[3];
+  const float b1 = (float)b1d, b2 = (float)b2d, omb1 = (float)(1.0 - b1d), omb2 = (float)(1.0 - b2d);
+  const float d = (float)decay, omd = (float)(1.0 - decay);
+  uintptr_t addr_or = reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+                      reinterpret_cast<uintptr_t>(v);
+  if (EMA) addr_or |= reinterpret_cast<uintptr_t>(ema);
+  const bool vec = (addr_or & 15) == 0;
+  const long long n4 = vec ? (n >> 2) : 0;
+  auto upd = [&](float gi, float& mi, float& vi, float& pi) {
+    gi *= gs;
+    if (md == 1) gi = __fmul_rn(__fdiv_rn(gi, nrm), max_norm);
+    mi = b1 * mi + omb1 * gi;
+    vi = b2 * vi + omb2 * gi * gi;
+    pi -= lrf * (mi * c1) / (sqrtf(vi * c2) + eps);
+  };
+  auto avg = [&](float& ei, float pi) { ei = __fadd_rn(__fmul_rn(d, ei), __fmul_rn(omd, pi)); };
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
+    const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + i);
+    float4 m4 = reinterpret_cast<float4*>(m)[i], v4 = reinterpret_cast<float4*>(v)[i], p4 = reinterpret_cast<float4*>(p)[i];
+    upd(g4.x, m4.x, v4.x, p4.x); upd(g4.y, m4.y, v4.y, p4.y); upd(g4.z, m4.z, v4.z, p4.z); upd(g4.w, m4.w, v4.w, p4.w);
+    reinterpret_cast<float4*>(m)[i] = m4;
+    reinterpret_cast<float4*>(v)[i] = v4;
+    reinterpret_cast<float4*>(p)[i] = p4;
+    if (EMA) {
+      float4 e4 = reinterpret_cast<float4*>(ema)[i];
+      avg(e4.x, p4.x); avg(e4.y, p4.y); avg(e4.z, p4.z); avg(e4.w, p4.w);
+      reinterpret_cast<float4*>(ema)[i] = e4;
+    }
+  }
+  for (long long i = n4 * 4 + (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    float mi = m[i], vi = v[i], pi = p[i];
+    upd(g[i], mi, vi, pi);
+    m[i] = mi; v[i] = vi; p[i] = pi;
+    if (EMA) {
+      float ei = ema[i];
+      avg(ei, pi);
+      ema[i] = ei;
+    }
+  }
+}
+void launch_adam_clip(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
+                      double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
+                      const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s) {
+  int blocks = cdiv(n, 256 * 4);   // the grid of launch_adam
+  if (blocks > xu_num_sms() * 8) blocks = xu_num_sms() * 8;
+  if (blocks < 1) blocks = 1;
+  if (ema == nullptr)
+    xu_launch(adam_clip_kernel<false>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
+              (float)grad_scale, 0.0, norm_dev, (float)max_norm, warmup, skipped);
+  else
+    xu_launch(adam_clip_kernel<true>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
+              (float)grad_scale, decay, norm_dev, (float)max_norm, warmup, skipped);
+}
+
 // sampling.py:128-151 elementwise update
 __global__ void sampler_update_kernel(const float* __restrict__ eps2, const float* __restrict__ z,
                                       const float* __restrict__ noise, float* __restrict__ z_out, long long n, float w,

@@ -34,10 +34,34 @@ class AdamState:
 
 @dataclass
 class Adam:
+    """optax.adam hyper-parameters; with max_grad_norm / warmup_steps set, optax.chain(optax.clip_by_global_norm(max_grad_norm),
+    optax.adam(optax.linear_schedule(0, learning_rate, warmup_steps)))."""
     learning_rate: float = 1e-4
     b1: float = 0.9
     b2: float = 0.999
     eps: float = 1e-8
+    max_grad_norm: Optional[float] = None
+    warmup_steps: int = 0
+
+    @property
+    def clip_or_warmup(self) -> bool:
+        """The step goes through the clip / warm-up launches (xunet_adam_clip_step)."""
+        return self.max_grad_norm is not None or self.warmup_steps > 0
+
+
+@dataclass
+class ClipState:
+    """Device block of gradient clipping and warm-up: the pre-clip global gradient norm of the last update, the scratch of
+    its reduction kernel, and the number of updates skipped because that norm was not finite."""
+    norm: torch.Tensor        # (1,) fp32
+    scratch: torch.Tensor     # (GRAD_NORM_SCRATCH,) fp64
+    skipped: torch.Tensor     # (1,) int64
+
+    @staticmethod
+    def zeros(device) -> "ClipState":
+        return ClipState(norm=torch.zeros(1, dtype=torch.float32, device=device),
+                         scratch=torch.zeros(_lib.GRAD_NORM_SCRATCH, dtype=torch.float64, device=device),
+                         skipped=torch.zeros(1, dtype=torch.int64, device=device))
 
 
 @dataclass
@@ -57,6 +81,8 @@ class TrainState:
     # None when create_train_state(ema_decay=None)
     ema_params: Optional[ParamTree] = None
     ema_decay: Optional[float] = None
+    # gradient-norm / skip-counter block; None unless create_train_state(max_grad_norm=..) or (warmup_steps=..)
+    clip: Optional[ClipState] = None
     _mask_rng: np.random.RandomState = None
     _frozen_mask: Optional[np.ndarray] = None
 
@@ -67,14 +93,19 @@ class TrainState:
         Ownership: by default the flat parameter / moment / EMA buffers are updated IN PLACE and the returned state shares
         them, i.e. the OLD state's `params` alias the new values (the reference rebinds `state = update_model(state, ..)`
         and never looks at the old one, train.py:153).  copy=True gives the Flax contract literally: the old state keeps
-        its values and the new state owns fresh buffers (3 x 4 bytes per parameter of extra traffic, 4 x 4 with EMA)."""
+        its values and the new state owns fresh buffers (3 x 4 bytes per parameter of extra traffic, 4 x 4 with EMA).
+
+        With clipping (tx.max_grad_norm) the global gradient norm is reduced first, into `clip.norm`; an update whose norm
+        is not finite changes nothing but the counters and is counted in `skipped_steps`."""
         lib = _lib.load()
         flat_g = grads.flat if isinstance(grads, ParamTree) else grads
         S, B = self.img_sidelength, self.batch_size
         if copy:
             newp = self.model.tree_from_flat(self.params.flat.clone(), S, B)
             newe = None if self.ema_params is None else self.model.tree_from_flat(self.ema_params.flat.clone(), S, B)
-            self = replace(self, params=newp, ema_params=newe,
+            newc = None if self.clip is None else replace(self.clip, norm=self.clip.norm.clone(),
+                                                          skipped=self.clip.skipped.clone())
+            self = replace(self, params=newp, ema_params=newe, clip=newc,
                            opt_state=replace(self.opt_state, mu=self.opt_state.mu.clone(), nu=self.opt_state.nu.clone()))
         p = self.params.flat
         count = self.opt_state.count + 1
@@ -82,12 +113,31 @@ class TrainState:
         _adam_launch(lib, self, flat_g, count, None, self.grad_scale, st)
         return replace(self, step=self.step + 1, opt_state=replace(self.opt_state, count=count))
 
+    @property
+    def skipped_steps(self) -> int:
+        """Updates skipped because the gradient norm was not finite (reads the device counter: synchronises)."""
+        return 0 if self.clip is None else int(self.clip.skipped.item())
+
 
 def _adam_launch(lib, s: TrainState, flat_g: torch.Tensor, count: int, step_dev, grad_scale: float, stream: int) -> None:
-    """One Adam pass over the flat buffers of `s`; with an EMA buffer the fused Adam + EMA entry point."""
+    """One Adam pass over the flat buffers of `s`; with an EMA buffer the fused Adam + EMA entry point.  With clipping or
+    warm-up: the global-norm reduction (clipping only), then the clip / warm-up Adam pass (EMA included)."""
     p = s.params.flat
     st_dev = None if step_dev is None else step_dev.data_ptr()
-    if s.ema_params is None:
+    if s.tx.clip_or_warmup:
+        tx, c = s.tx, s.clip
+        ema = None if s.ema_params is None else s.ema_params.flat.data_ptr()
+        norm = None
+        if tx.max_grad_norm is not None:
+            _lib.check(lib.xunet_grad_global_norm(flat_g.data_ptr(), p.numel(), grad_scale, c.scratch.data_ptr(),
+                                                  c.norm.data_ptr(), stream), 'xunet_grad_global_norm')
+            norm = c.norm.data_ptr()
+        _lib.check(lib.xunet_adam_clip_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(),
+                                            s.opt_state.nu.data_ptr(), ema, p.numel(), count, st_dev, tx.learning_rate,
+                                            tx.b1, tx.b2, tx.eps, grad_scale, s.ema_decay or 0.0, norm,
+                                            tx.max_grad_norm or 0.0, tx.warmup_steps, c.skipped.data_ptr(), stream),
+                   'xunet_adam_clip_step')
+    elif s.ema_params is None:
         _lib.check(lib.xunet_adam_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(), s.opt_state.nu.data_ptr(),
                                        p.numel(), count, st_dev, s.tx.learning_rate, s.tx.b1, s.tx.b2, s.tx.eps, grad_scale,
                                        stream), 'xunet_adam_step')
@@ -99,10 +149,12 @@ def _adam_launch(lib, s: TrainState, flat_g: torch.Tensor, count: int, step_dev,
 
 
 def _opt_buffers(s: TrainState):
-    """Every flat buffer one Adam pass writes."""
+    """Every buffer one Adam pass writes that outlives the step (the flat buffers, and the skip counter)."""
     bufs = [s.params.flat, s.opt_state.mu, s.opt_state.nu]
     if s.ema_params is not None:
         bufs.append(s.ema_params.flat)
+    if s.clip is not None:
+        bufs.append(s.clip.skipped)
     return bufs
 
 
@@ -116,23 +168,37 @@ def create_sample_data(batch_size, img_sidelength):
 
 def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_sidelength, *, model: XUNet = None,
                        zero_init: bool = True, reference_quirks: bool = False, init_on_device: bool = False,
-                       ema_decay: Optional[float] = None) -> TrainState:
+                       ema_decay: Optional[float] = None, max_grad_norm: Optional[float] = None,
+                       warmup_steps: int = 0) -> TrainState:
     """train.py:36-47.  Under torch.distributed the parameters of rank 0 are broadcast (the reference gives every
     device a different init, train.py:122-123 -- an ensemble, not data parallelism).
 
     ema_decay (e.g. 0.9999, Ho et al. 2020): keep `ema_params`, an exponential moving average of the weights updated in
     the same kernel as Adam, starting as a copy of the initial parameters.  Every rank updates its own copy; the parameters
     are identical across ranks after the all-reduce and Adam, so the copies stay identical without a collective.  None
-    (default): no EMA buffer, the optimizer step is plain Adam."""
+    (default): no EMA buffer, the optimizer step is plain Adam.
+
+    max_grad_norm (e.g. 1.0, Ho et al. 2020): clip the averaged gradient to this global L2 norm before Adam
+    (optax.clip_by_global_norm).  The norm is reduced on the device in a fixed order, so runs stay bit-reproducible; an update
+    whose norm is NaN or Inf is skipped entirely (the step count still advances) and counted in `state.skipped_steps`.
+    warmup_steps (e.g. 5000): warm the learning rate up linearly from 0 over this many updates
+    (optax.linear_schedule(0, learning_rate, warmup_steps)); 0 keeps it constant.  With the defaults (None, 0) the
+    optimizer step is exactly the plain one.  Every rank computes the norm of the same all-reduced gradient, so the clip and
+    skip decisions agree across ranks without a collective."""
     if ema_decay is not None and not (0.0 <= ema_decay <= 1.0):
         raise ValueError(f'ema_decay must lie in [0, 1], got {ema_decay}')
+    if max_grad_norm is not None and not (float(max_grad_norm) > 0.0 and np.isfinite(float(max_grad_norm))):
+        raise ValueError(f'max_grad_norm must be a finite number > 0, got {max_grad_norm}')
+    if isinstance(warmup_steps, bool) or int(warmup_steps) != warmup_steps or warmup_steps < 0:
+        raise ValueError(f'warmup_steps must be an integer >= 0, got {warmup_steps}')
     model = model or XUNet()
     sample = create_sample_data(train_batch_size, img_sidelength)
     params = model.init({'params': rng, 'dropout': rng_dropout}, sample, cond_mask=np.zeros(train_batch_size), train=True,
                         zero_init=zero_init, on_device=init_on_device)['params']
     world = xdist.world_size()
     xdist.broadcast_params(params.flat, src=0)
-    opt = Adam(learning_rate)
+    opt = Adam(learning_rate, max_grad_norm=None if max_grad_norm is None else float(max_grad_norm),
+               warmup_steps=int(warmup_steps))
     st = AdamState(mu=torch.zeros_like(params.flat), nu=torch.zeros_like(params.flat), count=0)
     mask_seed = int(np.asarray(rng_dropout).reshape(-1)[-1]) if rng_dropout is not None else 0
     # data parallel: every rank draws its OWN cond_mask stream (and dropout seeds, _dropout_seed) for its shard --
@@ -145,6 +211,7 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
                       batch_size=train_batch_size, img_sidelength=img_sidelength, grad_scale=1.0 / world,
                       reference_quirks=reference_quirks, ema_params=ema,
                       ema_decay=None if ema_decay is None else float(ema_decay),
+                      clip=ClipState.zeros(params.flat.device) if opt.clip_or_warmup else None,
                       _mask_rng=np.random.RandomState(mask_seed & 0x7FFFFFFF))
 
 
@@ -198,6 +265,9 @@ class TrainStep:
                                   XUNET_DP_EAGER_COLLECTIVES=1, or when capturing the collectives fails)
       use_graph=False           : everything eager; the bucket hook still overlaps the all-reduces with the backward
 
+    With gradient clipping the global-norm reduction runs right before Adam in every mode (after the all-reduce), inside
+    the same graph as Adam.
+
     A captured graph holds the NCCL kernels of the process group it was captured with: drop the TrainStep (or call
     `release_graphs()`) before `torch.distributed.destroy_process_group()`.
     """
@@ -229,6 +299,13 @@ class TrainStep:
         self.mode = None
         self._synced_count = None
         self._sync_counters()
+
+    @property
+    def grad_norm(self) -> Optional[torch.Tensor]:
+        """Global L2 norm of the averaged gradient of the step just run, before clipping: a 0-d device view (read or copy
+        it before the next step).  None unless the state clips (create_train_state(max_grad_norm=..))."""
+        s = self.state
+        return None if s.tx.max_grad_norm is None else s.clip.norm[0]
 
     def release_graphs(self):
         self.graph_fb = self.graph_opt = None
