@@ -211,9 +211,10 @@ int xunet_op_conv_wgrad(int dtype, int impl, const void* x, const void* dy, floa
 /* qkv: (N, L, 3C) [q | k | v], heads x hd; res/out: (N, L, C); lse: (N, heads, L) fp32. out=(attn+res)/sqrt2 */
 int xunet_op_attention(int dtype, int impl, const void* qkv, const void* res, void* out, float* lse, int N, int L, int C,
                        int heads, int cross, void* stream);
-/* dscratch: N*L*(heads + C) floats of scratch (row dots D, and the fp32 dQ accumulator of the fused head_dim<=32 path).
- * With XUNET_OP_ATTN_FOLD=1 in the environment the caller promises an all-zero dscratch and gets it back all-zero: the
- * head_dim<=32 path then runs as ONE kernel (D and the dQ rounding inside it), which is how the engine runs it. */
+/* dscratch: at least N*heads*L floats of scratch, the row dots D = rowsum(dO * O) laid out (N, heads, L); nothing past them
+ * is written (a buffer of N*L*(heads + C) floats, the size earlier versions needed, still works).  impl=1 needs lse and
+ * dscratch 16-byte aligned.  With XUNET_OP_ATTN_FOLD=1 in the environment the caller promises an all-zero dscratch and gets
+ * it back all-zero (one extra memset of the D rows). */
 int xunet_op_attention_bwd(int dtype, int impl, const void* qkv, const void* res, const void* out, const void* dout,
                            const float* lse, float* dscratch, void* dqkv, int N, int L, int C, int heads, int cross,
                            void* stream);

@@ -8,10 +8,9 @@
 //   online softmax on the accumulator fragment (a row lives in the 4 lanes of a quad), P_j -> bf16 A-operand registers
 //   O = O * corr + P_j V_j            (wgmma with A from registers, B = V_j MN-major straight from the TMA box)
 // Epilogue: out = (O / l + residual) / sqrt(2), lse = m + log(l) for the backward.
-// Backward (FlashAttention-2 order): one CTA = one (query frame n, head h, 64-key tile); it streams the 64-query blocks of the
-// frame and accumulates dK, dV in registers; the dQ contributions of its keys are summed in an fp64 buffer (xu_det_scratch),
-// so the result does not depend on the order in which the key tiles finish.  attn_bwd_prep_kernel forms D = rowsum(dO * O),
-// attn_bwd_dq_store_kernel rounds dQ to bf16 and re-zeroes the fp64 buffer.
+// Backward: two passes without atomics.  attn_bwd_dq_tc_kernel has the forward's grid (one CTA per 64-query tile): it forms
+// D = rowsum(dO * O) of its rows, streams the key / value blocks and accumulates dQ in registers.  attn_bwd_dkdv_tc_kernel
+// (FlashAttention-2 order: one CTA per 64-key tile) streams the 64-query blocks and accumulates dK, dV in registers.
 #include "kernels.h"
 #include "tc_common.cuh"
 
@@ -192,31 +191,180 @@ __global__ void __launch_bounds__(kAttnThreads) attn_fwd_tc_kernel(const __grid_
 
 // ================================================================================================================
 // backward.  dO = dout / sqrt2 (the AttnBlock residual scale), D = rowsum(dO * O), P = exp(S*scale - lse),
-// dS = P * (dP - D) * scale.
+// dS = P * (dP - D) * scale.  Two passes with the forward's warp layout (one consumer warpgroup + one TMA producer warp):
+//   attn_bwd_dq_tc_kernel   one CTA = one (query frame n, head h, 64-query tile): forms D of its 64 rows (and stores it for
+//                           the second pass), streams the key / value blocks and accumulates dQ = sum_j dS_j K_j in registers
+//                           (each block's product in fp32, their sum in fp64).
+//   attn_bwd_dkdv_tc_kernel one CTA = one (query frame n, head h, 64-key tile): streams the 64-query blocks and accumulates
+//                           dK = sum_j dS_j^T Q_j, dV = sum_j P_j^T dO_j in registers.
+// Every gradient element is owned by one CTA and summed in a fixed order: no atomics, deterministic by construction.
+// S and dP are recomputed by the second pass (a second round of exponentials) in exchange for that.
 // ================================================================================================================
 struct AttnBwdParams {
   const bf16* res; const bf16* out; const bf16* dout;
-  const float* lse; float* Dbuf; double* dq64; bf16* dqkv;
+  const float* lse; float* Dbuf; bf16* dqkv;
   int L, C, heads, cross;
   float scale, scale_log2;
 };
 
+// CTAs per SM the backward kernels are compiled for (__launch_bounds__ minimum): the largest count whose register budget
+// ptxas meets without spilling
+__host__ __device__ constexpr int attn_dq_ctas(int hd) { return hd <= 32 ? 3 : (hd == 64 ? 2 : 1); }
+__host__ __device__ constexpr int attn_dkdv_ctas(int hd) { return hd == 16 ? 3 : (hd <= 64 ? 2 : 1); }
+
 template <int HD>
-__global__ void __launch_bounds__(kAttnThreads) attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQKV,
-                                                                   const __grid_constant__ CUtensorMap tmG, const AttnBwdParams p) {
+__global__ void __launch_bounds__(kAttnThreads, attn_dq_ctas(HD))
+    attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmG, const AttnBwdParams p) {
   constexpr int CW = attn_cw(HD);
   constexpr int NCH = HD / CW;
   constexpr int TILE = kBlk * CW * 2;
   constexpr int ST = attn_stages(HD);
-  constexpr int DQN = HD <= 64 ? HD : 64;     // dQ is formed DQN columns at a time (register budget at head_dim 128)
+  constexpr int DQN = HD <= 64 ? HD : 64;     // dQ_j is formed DQN columns at a time (register budget at head_dim 128)
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* smQ = base;                        // resident query / dout tiles of this CTA
+  uint8_t* smG = smQ + NCH * TILE;
+  uint8_t* smK = smG + NCH * TILE;            // ST x NCH tiles
+  uint8_t* smV = smK + ST * NCH * TILE;
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(smV + ST * NCH * TILE);
+  uint64_t* kv_full = q_full + 1;
+  uint64_t* kv_empty = kv_full + ST;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * kBlk, h = blockIdx.y, n = blockIdx.z;
+  const int nkv = p.cross ? (n ^ 1) : n;
+  const int nkb = p.L / kBlk;
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < ST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 4); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQKV) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
+  }
+  __syncthreads();
+  xu_grid_dep_sync();
+
+  if (warp == 4) {
+    if (lane == 0) {
+      mbar_expect_tx(q_full, 2 * NCH * TILE);
+      for (int c = 0; c < NCH; ++c) {
+        tma_load_3d(smQ + c * TILE, &tmQKV, q_full, h * HD + c * CW, q0, n);
+        tma_load_3d(smG + c * TILE, &tmG, q_full, h * HD + c * CW, q0, n);
+      }
+      for (int j = 0; j < nkb; ++j) {
+        const int s = j % ST;
+        mbar_wait(&kv_empty[s], ((j / ST) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[s], 2 * NCH * TILE);
+        for (int c = 0; c < NCH; ++c) {
+          tma_load_3d(smK + (s * NCH + c) * TILE, &tmQKV, &kv_full[s], p.C + h * HD + c * CW, j * kBlk, nkv);
+          tma_load_3d(smV + (s * NCH + c) * TILE, &tmQKV, &kv_full[s], 2 * p.C + h * HD + c * CW, j * kBlk, nkv);
+        }
+      }
+    }
+    return;
+  }
+  // ===== consumer warpgroup: thread rows 16 warp + g and + 8 (g = lane / 4), columns 8 i + 2 t (+1) =====
+  const int g = lane >> 2, t = lane & 3;
+  const long long row0 = (long long)n * p.L + q0 + 16 * warp + g;
+  const long long srow0 = ((long long)n * p.heads + h) * p.L + q0 + 16 * warp + g;   // (n, h, q) index of lse / D
+  // D = rowsum(dO * O) with O = out * sqrt2 - res, one fma per channel in channel order (every lane of the quad forms its
+  // rows' D the same way).  D and lse are per-row constants of the whole key loop.
+  float Dr[2], lq[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const long long off = (row0 + 8 * hh) * p.C + h * HD;
+    float D = 0.f;
+#pragma unroll
+    for (int c = 0; c < HD; c += 2) {
+      const __nv_bfloat162 g2 = *reinterpret_cast<const __nv_bfloat162*>(p.dout + off + c);
+      const __nv_bfloat162 o2 = *reinterpret_cast<const __nv_bfloat162*>(p.out + off + c);
+      const __nv_bfloat162 r2 = *reinterpret_cast<const __nv_bfloat162*>(p.res + off + c);
+      D = fmaf(__low2float(g2) * XU_RSQRT2, __low2float(o2) * XU_SQRT2 - __low2float(r2), D);
+      D = fmaf(__high2float(g2) * XU_RSQRT2, __high2float(o2) * XU_SQRT2 - __high2float(r2), D);
+    }
+    Dr[hh] = D;
+    lq[hh] = p.lse[srow0 + 8 * hh] * 1.4426950408889634f;
+  }
+  if (t == 0) { p.Dbuf[srow0] = Dr[0]; p.Dbuf[srow0 + 8] = Dr[1]; }
+  double dq[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) dq[i] = 0.0;
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nkb; ++j) {
+    const int s = j % ST;
+    mbar_wait(&kv_full[s], (j / ST) & 1);
+    const uint32_t k_addr = smem_u32(smK + s * NCH * TILE), v_addr = smem_u32(smV + s * NCH * TILE);
+    float sc[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int kk = 0; kk < CW / 16; ++kk) {
+        // S = Q K_j^T  and  dP = dout V_j^T  (every operand K-major: head_dim contiguous)
+        Wgmma<64>::template ss<0, 0>(sc, make_kmajor_desc<CW>(smem_u32(smQ + c * TILE) + kk * 32),
+                                     make_kmajor_desc<CW>(k_addr + c * TILE + kk * 32), (c > 0 || kk > 0) ? 1u : 0u);
+        Wgmma<64>::template ss<0, 0>(dp, make_kmajor_desc<CW>(smem_u32(smG + c * TILE) + kk * 32),
+                                     make_kmajor_desc<CW>(v_addr + c * TILE + kk * 32), (c > 0 || kk > 0) ? 1u : 0u);
+      }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * i + 2 * hh + e;
+          const float pv = ex2_approx(fmaf(sc[x], p.scale_log2, -lq[hh]));
+          dp[x] = pv * (dp[x] * XU_RSQRT2 - Dr[hh]) * p.scale;
+        }
+    uint32_t da[4][4];
+    frag_to_a(dp, da);
+    // dQ_j = dS K_j in fp32 (B = the key tile read MN-major, as the forward reads V), DQN columns at a time, then added to the
+    // fp64 dQ in key-block order: fp64 carries 29 more significand bits than the fp32 addends, so the sum is exact unless they
+    // span about 29 - log2(L / 64) binary orders of magnitude (DESIGN §4); rounded fp64 -> fp32 -> bf16 once at the end
+#pragma unroll
+    for (int c2 = 0; c2 < HD / DQN; ++c2) {
+      float part[DQN / 2];
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        Wgmma<DQN>::template rs<1>(part, da[kk], make_mnmajor_desc<CW>(k_addr + c2 * TILE + kk * 16 * (CW * 2), TILE), kk > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < DQN / 2; ++i) dq[c2 * (DQN / 2) + i] += (double)part[i];
+    }
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
+  }
+#pragma unroll
+  for (int c2 = 0; c2 < HD / DQN; ++c2)
+#pragma unroll
+    for (int i = 0; i < DQN / 8; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const double* v = dq + c2 * (DQN / 2) + 4 * i + 2 * hh;
+        *reinterpret_cast<__nv_bfloat162*>(p.dqkv + (row0 + 8 * hh) * (3LL * p.C) + h * HD + c2 * DQN + 8 * i + 2 * t) =
+            __floats2bfloat162_rn((float)v[0], (float)v[1]);
+      }
+}
+
+// runs after attn_bwd_dq_tc_kernel, whose D (Dbuf) it reads
+template <int HD>
+__global__ void __launch_bounds__(kAttnThreads, attn_dkdv_ctas(HD))
+    attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmG, const AttnBwdParams p) {
+  constexpr int CW = attn_cw(HD);
+  constexpr int NCH = HD / CW;
+  constexpr int TILE = kBlk * CW * 2;
+  constexpr int ST = attn_stages(HD);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* smK = base;                        // resident key / value tiles of this CTA
   uint8_t* smV = smK + NCH * TILE;
-  uint8_t* smDS = smV + NCH * TILE;           // dS^T [64 keys][64 queries] bf16, 128B-swizzled (MN-major A operand of dQ)
-  uint8_t* smQ = smDS + kBlk * kBlk * 2;      // ST x NCH tiles
+  uint8_t* smQ = smV + NCH * TILE;            // ST x NCH tiles
   uint8_t* smG = smQ + ST * NCH * TILE;       // ST x NCH tiles of dout
-  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smG + ST * NCH * TILE);
+  float* smLD = reinterpret_cast<float*>(smG + ST * NCH * TILE);   // ST x [lse | D] of the 64 queries of a block
+  uint64_t* kv_full = reinterpret_cast<uint64_t*>(smLD + ST * 2 * kBlk);
   uint64_t* full = kv_full + 1;
   uint64_t* empty = full + ST;
 
@@ -241,14 +389,17 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_tc_kernel(const __grid_
         tma_load_3d(smK + c * TILE, &tmQKV, kv_full, p.C + h * HD + c * CW, k0, nkv);
         tma_load_3d(smV + c * TILE, &tmQKV, kv_full, 2 * p.C + h * HD + c * CW, k0, nkv);
       }
+      const long long srow = ((long long)n * p.heads + h) * p.L;
       for (int j = 0; j < nqb; ++j) {
         const int s = j % ST;
         mbar_wait(&empty[s], ((j / ST) & 1) ^ 1);
-        mbar_expect_tx(&full[s], 2 * NCH * TILE);
+        mbar_expect_tx(&full[s], 2 * NCH * TILE + 2 * kBlk * 4);
         for (int c = 0; c < NCH; ++c) {
           tma_load_3d(smQ + (s * NCH + c) * TILE, &tmQKV, &full[s], h * HD + c * CW, j * kBlk, n);
           tma_load_3d(smG + (s * NCH + c) * TILE, &tmG, &full[s], h * HD + c * CW, j * kBlk, n);
         }
+        bulk_load(smLD + s * 2 * kBlk, p.lse + srow + j * kBlk, kBlk * 4, &full[s]);
+        bulk_load(smLD + s * 2 * kBlk + kBlk, p.Dbuf + srow + j * kBlk, kBlk * 4, &full[s]);
       }
     }
     return;
@@ -257,22 +408,18 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_tc_kernel(const __grid_
   float dv[HD / 2], dk[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
-  const float* lse_row = p.lse + ((long long)n * p.heads + h) * p.L;
-  const float* D_row = p.Dbuf + ((long long)n * p.heads + h) * p.L;
   mbar_wait(kv_full, 0);
   for (int j = 0; j < nqb; ++j) {
     const int s = j % ST;
-    // per-query operands of the 16 columns this thread holds (L1 / L2 hits: 64 floats per block)
+    mbar_wait(&full[s], (j / ST) & 1);
+    // per-query operands of the 16 columns this thread holds, from the block's stage
     float lq[16], dq_[16];
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int q = j * kBlk + 8 * i + 2 * t + e;
-        lq[2 * i + e] = __ldg(lse_row + q) * 1.4426950408889634f;
-        dq_[2 * i + e] = __ldg(D_row + q);
-      }
-    mbar_wait(&full[s], (j / ST) & 1);
+    for (int i = 0; i < 8; ++i) {
+      const float2 l2 = lds_f32x2(smLD + s * 2 * kBlk + 8 * i + 2 * t), d2 = lds_f32x2(smLD + s * 2 * kBlk + kBlk + 8 * i + 2 * t);
+      lq[2 * i] = l2.x * 1.4426950408889634f; lq[2 * i + 1] = l2.y * 1.4426950408889634f;
+      dq_[2 * i] = d2.x; dq_[2 * i + 1] = d2.y;
+    }
     const uint32_t q_addr = smem_u32(smQ + s * NCH * TILE), g_addr = smem_u32(smG + s * NCH * TILE);
     float st[32], dpt[32];
     wgmma_fence();
@@ -302,18 +449,6 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_tc_kernel(const __grid_
     uint32_t pa[4][4], da[4][4];
     frag_to_a(st, pa);
     frag_to_a(dpt, da);
-    // dS^T -> shared memory (row = key, 128-byte rows of 64 queries, 16-byte chunks XOR-swizzled by row)
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const int R = 16 * warp + g + 8 * hh;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const uint32_t v = pack_bf16(dpt[4 * i + 2 * hh], dpt[4 * i + 2 * hh + 1]);
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(smDS + R * 128 + ((i ^ (R & 7)) << 4) + 4 * t)), "r"(v) : "memory");
-      }
-    }
-    fence_async_smem();
-    named_bar_sync(1, 128);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
@@ -323,29 +458,7 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_tc_kernel(const __grid_
     }
     wgmma_commit();
     wgmma_wait<0>();
-    // dQ[64 q][HD] += dS K: A = dS^T in shared memory read MN-major (M = queries), B = the resident key tile (MN-major)
-    const long long qrow0 = (long long)n * p.L + j * kBlk + 16 * warp + g;
-#pragma unroll
-    for (int c2 = 0; c2 < HD / DQN; ++c2) {
-      float dq[DQN / 2];
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
-        Wgmma<DQN>::template ss<1, 1>(dq, make_mnmajor_desc<64>(smem_u32(smDS) + kk * 16 * 128, 8192),
-                                      make_mnmajor_desc<CW>(smem_u32(smK + c2 * TILE) + kk * 16 * (CW * 2), TILE), kk > 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int i = 0; i < DQN / 8; ++i)
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          double* d = p.dq64 + (qrow0 + 8 * hh) * p.C + h * HD + c2 * DQN + 8 * i + 2 * t;
-          xu_det_add(d, dq[4 * i + 2 * hh]);
-          xu_det_add(d + 1, dq[4 * i + 2 * hh + 1]);
-        }
-    }
     if (lane == 0) mbar_arrive(&empty[s]);
-    named_bar_sync(1, 128);      // every warp's dQ MMAs have read smDS before the next block overwrites it
   }
   // dK, dV of this CTA's 64 keys (dV picks up the 1/sqrt2 of dO here)
   const long long krow0 = (long long)nkv * p.L + k0 + 16 * warp + g;
@@ -360,55 +473,6 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_tc_kernel(const __grid_
     }
 }
 
-// D = rowsum(dO * O) per (row, head) (one thread per row and head)
-template <int HD>
-__global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnBwdParams p, long long total) {
-  xu_grid_dep_sync();
-  const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (idx >= total) return;
-  const int h = (int)(idx % p.heads);
-  const long long row = idx / p.heads;
-  const long long o = row * p.C + h * HD;
-  float D = 0.f;
-#pragma unroll
-  for (int c0 = 0; c0 < HD; c0 += 8) {
-    uint4 gv = *reinterpret_cast<const uint4*>(p.dout + o + c0);
-    uint4 ov = *reinterpret_cast<const uint4*>(p.out + o + c0);
-    uint4 rv = *reinterpret_cast<const uint4*>(p.res + o + c0);
-    const __nv_bfloat162* g2 = reinterpret_cast<const __nv_bfloat162*>(&gv);
-    const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&ov);
-    const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      D = fmaf(__low2float(g2[q]) * XU_RSQRT2, __low2float(o2[q]) * XU_SQRT2 - __low2float(r2[q]), D);
-      D = fmaf(__high2float(g2[q]) * XU_RSQRT2, __high2float(o2[q]) * XU_SQRT2 - __high2float(r2[q]), D);
-    }
-  }
-  const long long n = row / p.L, l = row % p.L;
-  p.Dbuf[(n * p.heads + h) * p.L + l] = D;
-}
-
-// dq64 -> the q third of dqkv (bf16), 4 channels per thread, re-zeroing dq64.  zero: also clear the n_d D values, so that a
-// caller that keeps its scratch buffer all-zero between calls gets it back that way.
-__global__ void __launch_bounds__(256) attn_bwd_dq_store_kernel(double* __restrict__ dq64, bf16* __restrict__ dqkv, long long total4,
-                                                                int C, float* __restrict__ dbuf, long long n_d, int zero) {
-  xu_grid_dep_sync();
-  const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (idx >= total4) return;
-  const int c4 = (int)(idx % (C / 4));
-  const long long row = idx / (C / 4);
-  double2* src = reinterpret_cast<double2*>(dq64 + row * C + c4 * 4);
-  const double2 v01 = src[0], v23 = src[1];
-  src[0] = make_double2(0.0, 0.0);
-  src[1] = make_double2(0.0, 0.0);
-  __nv_bfloat162 a = __floats2bfloat162_rn((float)v01.x, (float)v01.y), b = __floats2bfloat162_rn((float)v23.x, (float)v23.y);
-  uint2 t;
-  t.x = *reinterpret_cast<uint32_t*>(&a);
-  t.y = *reinterpret_cast<uint32_t*>(&b);
-  *reinterpret_cast<uint2*>(dqkv + row * (3LL * C) + c4 * 4) = t;
-  if (zero && idx < n_d) dbuf[idx] = 0.f;
-}
-
 template <int HD>
 void launch_bwd(const AttnArgs& a, cudaStream_t s) {
   constexpr int CW = attn_cw(HD);
@@ -421,25 +485,30 @@ void launch_bwd(const AttnArgs& a, cudaStream_t s) {
   uint64_t gs[2] = {(uint64_t)a.C * 2, (uint64_t)a.L * a.C * 2};
   uint32_t box[3] = {(uint32_t)CW, (uint32_t)kBlk, 1u};
   if (!xu_encode_bf16_map(&tq, a.qkv, 3, qd, qs, box, CW) || !xu_encode_bf16_map(&tg, a.dout, 3, gd, gs, box, CW)) return;
+  if (((uintptr_t)a.lse | (uintptr_t)a.dscratch) & 15) {    // the dK/dV kernel bulk-copies lse / D rows
+    xu_set_kernel_error("attn_tc: lse and dscratch must be 16-byte aligned");
+    return;
+  }
   AttnBwdParams p;
   p.res = (const bf16*)a.res; p.out = (const bf16*)a.out; p.dout = (const bf16*)a.dout;
   p.lse = a.lse; p.Dbuf = a.dscratch; p.dqkv = (bf16*)a.dqkv;
-  const long long rows = (long long)a.N * a.L;
-  p.dq64 = xu_det_scratch(s, rows * a.C);                     // [N*L][C] fp64
-  if (p.dq64 == nullptr) return;
   p.L = a.L; p.C = a.C; p.heads = a.heads; p.cross = a.cross;
   p.scale = 1.f / sqrtf((float)HD);
   p.scale_log2 = 1.4426950408889634f * p.scale;
-  const size_t smem = (size_t)2 * NCH * TILE + kBlk * kBlk * 2 + (size_t)2 * attn_stages(HD) * NCH * TILE + 1024 + 256;
+  // both kernels: two resident tiles per chunk + a ring of tile pairs (dK/dV: + the lse / D rows of each stage)
+  const size_t smem = (size_t)2 * NCH * TILE + (size_t)2 * attn_stages(HD) * NCH * TILE + 1024 + 256;
+  const size_t smem_dkdv = smem + (size_t)attn_stages(HD) * 2 * kBlk * 4;
   static bool configured = false;
   if (!configured) {
-    cudaFuncSetAttribute(attn_bwd_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaFuncSetAttribute(attn_bwd_dq_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaFuncSetAttribute(attn_bwd_dkdv_tc_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     configured = true;
   }
-  xu_launch(attn_bwd_prep_kernel<HD>, cdiv(rows * a.heads, 256), 256, 0, s, p, rows * a.heads);
-  xu_launch(attn_bwd_tc_kernel<HD>, dim3(a.L / kBlk, a.heads, a.N), kAttnThreads, smem, s, tq, tg, p);
-  xu_launch(attn_bwd_dq_store_kernel, cdiv(rows * a.C / 4, 256), 256, 0, s, p.dq64, p.dqkv, rows * a.C / 4, a.C, p.Dbuf,
-            rows * a.heads, a.scratch_zeroed);
+  const dim3 grid(a.L / kBlk, a.heads, a.N);
+  xu_launch(attn_bwd_dq_tc_kernel<HD>, grid, kAttnThreads, smem, s, tq, tg, p);
+  xu_launch(attn_bwd_dkdv_tc_kernel<HD>, grid, kAttnThreads, smem_dkdv, s, tq, tg, p);
+  // a caller that keeps its scratch all-zero between calls gets the D rows back cleared
+  if (a.scratch_zeroed) cudaMemsetAsync(a.dscratch, 0, sizeof(float) * (size_t)a.N * a.heads * a.L, s);
 }
 
 template <int HD>

@@ -124,10 +124,6 @@ struct xunet_handle {
   long long a_stats = 0, stats_bytes = 0, a_bstats = 0, bstats_bytes = 0;   // contiguous GroupNorm statistics regions
   long long a_cstats = 0, cstats_bytes = 0;                                  // contiguous per-channel statistics (one memset)
   long long a_bcs = 0, bcs_bytes = 0;                                        // contiguous backward channel sums (one memset)
-  // attention backward (head_dim <= 32) without helper kernels: its scratch (dQ accumulator + tickets) must be zero on entry and
-  // is left zero on exit; the workspace it was last left clean in (nullptr: unknown / dirty)
-  int attn_fold = 1;
-  const void* scratch_clean_ws = nullptr;
   // top-level blocks in forward order (first op index, first parameter offset): the backward finishes the gradient of
   // every leaf at or above blocks[k].leaf_begin once it has walked down to blocks[k].op_begin -> gradient buckets
   struct Block { int op_begin; long long leaf_begin; };
@@ -304,7 +300,7 @@ struct Builder {
     o.kind = OP_ATTN; o.x = qkv; o.y = y; o.r = h_in; o.cross = cross; o.heads = heads;
     o.impl = (use_tc() && attn_tc_supported(H.dtype, t.h * t.w, C, heads)) ? 1 : 0;
     o.lse = H.alloc(sizeof(float) * t.n * heads * t.h * t.w);
-    o.dscr = H.training ? H.alloc(sizeof(float) * t.n * (heads + C) * t.h * t.w) : -1;   // D [N,heads,L] + fp32 dQ [N,L,C]
+    o.dscr = H.training ? H.alloc(sizeof(float) * t.n * heads * t.h * t.w) : -1;   // D [N,heads,L]
     H.ops.push_back(o);
     H.tensors[y].producer = (int)H.ops.size() - 1;
     return y;
@@ -799,15 +795,6 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
   cudaMemsetAsync(c.aux(h->a_dlemb), 0, sizeof(float) * B * E, c.s);
   if (h->bstats_bytes) cudaMemsetAsync(c.ws + h->a_bstats, 0, (size_t)h->bstats_bytes, c.s);
   if (h->bcs_bytes) cudaMemsetAsync(c.ws + h->a_bcs, 0, (size_t)h->bcs_bytes, c.s);
-  const bool scratch_dirty = h->attn_fold && h->scratch_clean_ws != (const void*)c.ws;
-  if (scratch_dirty) {
-    for (const Op& o : h->ops)
-      if (o.kind == OP_ATTN && o.dscr >= 0) {
-        const Tensor& y = h->tensors[o.y];
-        cudaMemsetAsync(c.ws + o.dscr, 0, sizeof(float) * (size_t)y.n * (o.heads + y.c) * y.h * y.w, c.s);
-      }
-  }
-  h->scratch_clean_ws = nullptr;      // in flight (stays unknown if this backward fails)
   size_t bp = 0;
   long long bucket_end = h->nparams;
   auto emit_bucket = [&](long long off) {
@@ -878,7 +865,6 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
         a.qkv = c.act(o.x); a.res = c.act(o.r); a.out = c.act(o.y); a.lse = c.aux(o.lse);
         a.dout = c.grad(o.y); a.dscratch = c.aux(o.dscr); a.dqkv = c.grad(o.x);
         a.N = y.n; a.L = y.h * y.w; a.C = y.c; a.heads = o.heads; a.cross = o.cross;
-        a.scratch_zeroed = h->attn_fold;
         if (o.impl == 1) launch_attn_bwd_tc(a, c.s);
         else launch_attn_bwd_simt(dt, a, c.s);
         break;
@@ -906,13 +892,6 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("backward: CUDA error: %s", cudaGetErrorString(e));
   if (xu_kernel_error()[0]) return fail("backward: %s", xu_kernel_error());
-  {
-    // the attention scratch is zero again once this backward has run; a capture that had to include the memsets executes
-    // nothing now, so it proves nothing about the buffer
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(c.s, &cap);
-    if (cap == cudaStreamCaptureStatusNone || !scratch_dirty) h->scratch_clean_ws = (const void*)c.ws;
-  }
   return 0;
 }
 
@@ -947,9 +926,6 @@ extern "C" int xunet_create(const xunet_config* cfg, int batch, int side, int dt
   h->cfg = *cfg;
   h->B = batch; h->S = side; h->dtype = dtype; h->training = training ? 1 : 0; h->N = 2 * batch;
   h->esize = dtype == XUNET_DTYPE_F32 ? 4 : 2;
-  // XUNET_ATTN_BWD_FOLD=1: the attention backward keeps its dQ / D scratch buffer all-zero between steps (the dQ store kernel
-  // re-zeroes it), so the buffer needs no clearing of its own
-  h->attn_fold = getenv("XUNET_ATTN_BWD_FOLD") != nullptr ? 1 : 0;
   Builder b(*h);
   if (b.build() != 0) { delete h; return 1; }
   *out = h;
@@ -1307,7 +1283,7 @@ extern "C" int xunet_op_attention_bwd(int dtype, int impl, const void* qkv, cons
   a.qkv = qkv; a.res = res; a.out = const_cast<void*>(out); a.lse = const_cast<float*>(lse);
   a.dout = dout; a.dscratch = dscratch; a.dqkv = dqkv;
   a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
-  // XUNET_OP_ATTN_FOLD=1: the caller passes an all-zero dscratch and gets it back all-zero (the dQ store kernel re-zeroes D)
+  // XUNET_OP_ATTN_FOLD=1: the caller passes an all-zero dscratch and gets it back all-zero (the D rows are cleared after use)
   a.scratch_zeroed = getenv("XUNET_OP_ATTN_FOLD") != nullptr ? 1 : 0;
   if (impl == 1) {
     if (!attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention_bwd: shape not supported by the tensor-core kernel");

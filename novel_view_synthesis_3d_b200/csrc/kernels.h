@@ -146,8 +146,7 @@ struct AttnArgs {
   const void* qkv; const void* res; void* out; float* lse;
   const void* dout; float* dscratch; void* dqkv;   // backward
   int N, L, C, heads, cross;
-  int scratch_zeroed;   // backward (head_dim <= 32): dscratch is all-zero on entry -> the fused kernel also forms D and rounds dQ
-                        // itself (no prep / store kernels) and leaves dscratch all-zero again
+  int scratch_zeroed;   // backward (tensor-core path): dscratch is all-zero on entry and is handed back all-zero
   float* cstats;   // optional (tensor-core forward): per-(sample, channel) [sum, sumsq] of the stored output, (N/2, C, 2) fp32, accumulated
 };
 void launch_attn_fwd_simt(int dtype, const AttnArgs& a, cudaStream_t s);

@@ -56,6 +56,12 @@ __device__ __forceinline__ void tma_reduce_add_4d(const void* src, const CUtenso
                "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+// 1-D bulk copy global -> shared (bytes a multiple of 16, both addresses 16-byte aligned), completing on an mbarrier
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
@@ -92,6 +98,11 @@ __device__ __forceinline__ void sts128(void* smem_ptr, const uint4& v) {
 __device__ __forceinline__ float lds_f32(const void* smem_ptr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(smem_u32(smem_ptr)) : "memory");
+  return v;
+}
+__device__ __forceinline__ float2 lds_f32x2(const void* smem_ptr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_u32(smem_ptr)) : "memory");
   return v;
 }
 __device__ __forceinline__ void sts_f32(void* smem_ptr, float v) {
