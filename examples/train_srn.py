@@ -6,6 +6,7 @@ state (state<step>: params, Adam moments and count, EMA, cond_mask streams) that
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 1000 --ema-decay 0.9999
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 2000 --ema-decay 0.9999 --resume
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --max-grad-norm 1 --warmup-steps 5000 --ema-decay 0.9999
+    python examples/train_srn.py cars_train_val --batch 4 --side 128 --grad-accum-steps 8     # 32 samples per update
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_srn.py cars_train_val
 """
 import argparse
@@ -36,6 +37,8 @@ def main():
                     help='clip the gradient to this global L2 norm (e.g. 1) and skip updates whose norm is not finite')
     ap.add_argument('--warmup-steps', type=int, default=0,
                     help='warm the learning rate up linearly from 0 over this many steps (e.g. 5000)')
+    ap.add_argument('--grad-accum-steps', type=int, default=1,
+                    help='accumulate the gradient over this many micro-batches of --batch samples per update')
     ap.add_argument('--resume', action='store_true', help='continue from the latest state<step> checkpoint')
     ap.add_argument('--ckpt', default='checkpoints')
     a = ap.parse_args()
@@ -47,16 +50,26 @@ def main():
                                  max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps)
     if a.resume and P.checkpoint.restore_train_state(a.ckpt, state) is not None and rank == 0:
         print(f'resumed from step {state.step}')
-    step = P.TrainStep(state)
+    step = P.TrainStep(state, grad_accum_steps=a.grad_accum_steps)
     fd = P.ForwardDiffusion(step.eng)
     stream = ds.batches(a.batch)
+    k = a.grad_accum_steps
     for it in range(state.step, a.steps):
-        b = next(stream)
-        fd.sample(b['target'], seed=it * world + rank)        # z, noise, logsnr, cond_mask on the GPU
-        dev = step.eng.inp
-        batch = {k: b[k] for k in ('x', 'R1', 't1', 'R2', 't2', 'K')}
-        batch.update(z=dev['z'], logsnr=dev['logsnr'])
-        loss = step(batch, dev['noise'], cond_mask=dev['cond_mask'])
+        micro = []
+        for j in range(k):                                     # one update = k micro-batches of --batch samples
+            b = next(stream)
+            fd.sample(b['target'], seed=(it * k + j) * world + rank)     # z, noise, logsnr, cond_mask on the GPU
+            dev = step.eng.inp
+            m = {key: b[key] for key in ('x', 'R1', 't1', 'R2', 't2', 'K')}
+            m.update({key: dev[key] if k == 1 else dev[key].clone() for key in ('z', 'logsnr', 'noise', 'cond_mask')})
+            micro.append(m)
+        if k == 1:
+            batch = micro[0]
+        else:
+            batch = {key: torch.cat([m[key] for m in micro]) if isinstance(micro[0][key], torch.Tensor)
+                     else np.concatenate([m[key] for m in micro]) for key in micro[0]}
+        noise, cond_mask = batch.pop('noise'), batch.pop('cond_mask')
+        loss = step(batch, noise, cond_mask=cond_mask)
         if rank == 0 and it % 50 == 0:
             norm = '' if step.grad_norm is None else f'  grad norm {float(step.grad_norm):.4f}'
             print(f'{it}: {float(loss):.4f}{norm}')                                                    # train.py:157

@@ -105,6 +105,13 @@ int xunet_backward(xunet_handle* h, const float* params, const xunet_batch* batc
                    const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
                    void* stream);
 
+/* xunet_backward that ADDS the parameter gradient into `grads` instead of overwriting it (gradient accumulation over
+ * micro-batches, optax.MultiSteps): each leaf becomes grads + g in fp32, one rounding per element, where g is exactly what
+ * xunet_backward would have written.  Same arguments, ordering guarantees, bucket hook and graph-capture behaviour. */
+int xunet_backward_accumulate(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
+                              const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
+                              void* stream);
+
 /* Data-parallel hook (north_star: "one NCCL allreduce of the gradient bucket"; the reference's pmap step would place
  * lax.pmean between value_and_grad and apply_gradients, train.py:70-76).  With a callback installed, xunet_backward calls
  *     fn(user, elem_offset, n_elems)

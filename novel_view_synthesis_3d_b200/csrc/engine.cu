@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 102; }
+extern "C" int xunet_version(void) { return 103; }
 
 namespace {
 
@@ -568,6 +568,7 @@ struct Ctx {
   int train;
   cudaStream_t s;
   cudaStream_t side = nullptr;   // non-null: weight gradients go here
+  int acc_grads = 0;             // backward: add the parameter gradient into `grads` (xunet_backward_accumulate)
   void* act(int t) const { return ws + h->tensors[t].off; }
   void* grad(int t) const { const Tensor& x = h->tensors[t]; return ws + (x.galias >= 0 ? h->tensors[x.galias].goff : x.goff); }
   float gscale(int t) const { return h->tensors[t].gscale; }
@@ -791,7 +792,9 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
   const int dt = h->dtype, B = h->B, S = h->S, E = h->cfg.emb_ch;
   c.side = ensure_side(h);
   bool emb_joined = false;
-  cudaMemsetAsync(c.grads, 0, sizeof(float) * (size_t)h->nparams, c.s);
+  // every parameter-gradient writer below adds its leaf's gradient exactly once (an fp64 fold or a += per element), except the
+  // log-SNR Dense and pos_emb kernels, which store unless told to add: zeroing the buffer first makes the backward overwrite it
+  if (!c.acc_grads) cudaMemsetAsync(c.grads, 0, sizeof(float) * (size_t)h->nparams, c.s);
   cudaMemsetAsync(c.aux(h->a_dlemb), 0, sizeof(float) * B * E, c.s);
   if (h->bstats_bytes) cudaMemsetAsync(c.ws + h->a_bstats, 0, (size_t)h->bstats_bytes, c.s);
   if (h->bcs_bytes) cudaMemsetAsync(c.ws + h->a_bcs, 0, (size_t)h->bcs_bytes, c.s);
@@ -871,11 +874,11 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
       }
       case OP_POSE:
         if (h->tensors[o.y].need_grad)
-          launch_pose_emb_bwd(dt, c.grad(o.y), c.G(o.p0), c.G(o.p1), c.G(o.p2), B, S, c.s);
+          launch_pose_emb_bwd(dt, c.grad(o.y), c.G(o.p0), c.G(o.p1), c.G(o.p2), B, S, c.acc_grads, c.s);
         break;
       case OP_LOGSNR:
         launch_logsnr_emb_bwd(c.aux(h->a_dlemb), c.P(o.p2), c.aux(h->a_pe), c.aux(h->a_h1), c.aux(h->a_dh1), c.G(o.p0),
-                              c.G(o.p1), c.G(o.p2), c.G(o.p3), B, E, c.s);
+                              c.G(o.p1), c.G(o.p2), c.G(o.p3), B, E, c.acc_grads, c.s);
         break;
       default: break;
     }
@@ -1012,6 +1015,19 @@ extern "C" int xunet_backward(xunet_handle* h, const float* params, const xunet_
   if (!h->forward_done_train) return fail("xunet_backward: call xunet_forward first");
   xu_set_kernel_error("");
   Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
+  XuDetBind bind(h->det);
+  return backward_impl(c, noise, loss_out);
+}
+
+extern "C" int xunet_backward_accumulate(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
+                                         const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
+                                         void* stream) {
+  if (!h || !params || !batch || !noise || !workspace || !grads || !loss_out) return fail("xunet_backward_accumulate: null argument");
+  if (!h->training) return fail("xunet_backward_accumulate: handle was created with training=0");
+  if (!h->forward_done_train) return fail("xunet_backward_accumulate: call xunet_forward first");
+  xu_set_kernel_error("");
+  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
+  c.acc_grads = 1;
   XuDetBind bind(h->det);
   return backward_impl(c, noise, loss_out);
 }

@@ -93,14 +93,16 @@ void launch_gn_bwd_apply_pre(int dtype, const GnArgs& a, cudaStream_t s);
 // logsnr (B) -> posenc_ddpm -> Dense -> swish -> Dense.  pe,h1: saved (B,E) fp32.  lemb (B,E) fp32
 void launch_logsnr_emb(const float* logsnr, const float* w0, const float* b0, const float* w1, const float* b1,
                        float* pe, float* h1, float* lemb, int B, int E, cudaStream_t s);
+// accumulate: dw0/db0/dw1/db1 += instead of =
 void launch_logsnr_emb_bwd(const float* dlemb, const float* w1, const float* pe, const float* h1, float* dh1,
-                           float* dw0, float* db0, float* dw1, float* db1, int B, int E, cudaStream_t s);
+                           float* dw0, float* db0, float* dw1, float* db1, int B, int E, int accumulate, cudaStream_t s);
 // rays + NeRF posenc -> (2B,S,S,144)
 void launch_pose_emb(int dtype, const float* R1, const float* t1, const float* R2, const float* t2, const float* K,
                      const float* cond_mask, const float* pos_emb, const float* ref_first, const float* ref_other,
                      float* kinv_scratch, void* out, int B, int S, int convention, const float* rays, cudaStream_t s);
+// accumulate: dpos_emb += instead of = (dref_first / dref_other are always added to)
 void launch_pose_emb_bwd(int dtype, const void* dpose, float* dpos_emb, float* dref_first, float* dref_other, int B, int S,
-                         cudaStream_t s);
+                         int accumulate, cudaStream_t s);
 // semb = swish(lemb[b] + pe)   /   bwd: dpe (+)= dsemb*swish'(z), dlemb[b] += sum
 void launch_emb_fwd(int dtype, const float* lemb, const void* pe, void* semb, int N, int HW, int E, cudaStream_t s);
 void launch_emb_bwd(int dtype, const float* lemb, const void* pe, const void* dsemb, void* dpe, float* dlemb, int N, int HW,

@@ -1128,7 +1128,8 @@ __global__ void logsnr_bwd_dh1_kernel(const float* __restrict__ dlemb, const flo
   acc = warp_sum(acc);
   if (lane == 0) dh1[b * E + k] = acc * swish_gradf_(h1[b * E + k]);
 }
-// dw1[k][j] = sum_b swish(h1[b,k]) dlemb[b,j];  dw0[k][j] = sum_b pe[b,k] dh1[b,j];  biases
+// dw1[k][j] = sum_b swish(h1[b,k]) dlemb[b,j];  dw0[k][j] = sum_b pe[b,k] dh1[b,j];  biases.  ACC: added to the gradients instead
+template <bool ACC>
 __global__ void logsnr_bwd_w_kernel(const float* __restrict__ dlemb, const float* __restrict__ pe,
                                     const float* __restrict__ h1, const float* __restrict__ dh1, float* __restrict__ dw0,
                                     float* __restrict__ db0, float* __restrict__ dw1, float* __restrict__ db1, int B,
@@ -1144,18 +1145,25 @@ __global__ void logsnr_bwd_w_kernel(const float* __restrict__ dlemb, const float
       s1 += dl;
       s0 += dh;
     }
-    dw1[k * E + j] = a1;
-    dw0[k * E + j] = a0;
-    if (k == 0) { db1[j] = s1; db0[j] = s0; }
+    if (ACC) {
+      dw1[k * E + j] += a1;
+      dw0[k * E + j] += a0;
+      if (k == 0) { db1[j] += s1; db0[j] += s0; }
+    } else {
+      dw1[k * E + j] = a1;
+      dw0[k * E + j] = a0;
+      if (k == 0) { db1[j] = s1; db0[j] = s0; }
+    }
   }
 }
 
 void launch_logsnr_emb_bwd(const float* dlemb, const float* w1, const float* pe, const float* h1, float* dh1, float* dw0,
-                           float* db0, float* dw1, float* db1, int B, int E, cudaStream_t s) {
+                           float* db0, float* dw1, float* db1, int B, int E, int accumulate, cudaStream_t s) {
   dim3 g1(cdiv(E, 8), B);
   xu_launch(logsnr_bwd_dh1_kernel, g1, 256, 0, s, dlemb, w1, h1, dh1, E);
   int threads = E < 256 ? ((E + 31) / 32) * 32 : 256;
-  xu_launch(logsnr_bwd_w_kernel, E, threads, 0, s, dlemb, pe, h1, dh1, dw0, db0, dw1, db1, B, E);
+  if (accumulate) xu_launch(logsnr_bwd_w_kernel<true>, E, threads, 0, s, dlemb, pe, h1, dh1, dw0, db0, dw1, db1, B, E);
+  else xu_launch(logsnr_bwd_w_kernel<false>, E, threads, 0, s, dlemb, pe, h1, dh1, dw0, db0, dw1, db1, B, E);
 }
 
 // ======================================================================================================
@@ -1276,7 +1284,8 @@ void launch_pose_emb(int dtype, const float* R1, const float* t1, const float* R
                                                           ref_other, (bf16*)out, B, S, convention, rays);
 }
 
-template <typename T>
+// ACC: dpos_emb is added to instead of stored (the ref_pose_emb leaves are folded, which always adds)
+template <typename T, bool ACC>
 __global__ void pose_emb_bwd_kernel(const T* __restrict__ dpose, float* __restrict__ dpos_emb,
                                     double* __restrict__ dref_first, double* __restrict__ dref_other, int B, int S) {
   xu_grid_dep_sync();
@@ -1289,18 +1298,27 @@ __global__ void pose_emb_bwd_kernel(const T* __restrict__ dpose, float* __restri
     s0 += ldf(dpose + (long long)(2 * b) * per + idx);
     s1 += ldf(dpose + (long long)(2 * b + 1) * per + idx);
   }
-  if (dpos_emb != nullptr) dpos_emb[idx] = s0 + s1;
+  if (dpos_emb != nullptr) {
+    if (ACC) dpos_emb[idx] += s0 + s1;
+    else dpos_emb[idx] = s0 + s1;
+  }
   if (dref_first != nullptr) { xu_det_add(&dref_first[j], s0); xu_det_add(&dref_other[j], s1); }
 }
 
 void launch_pose_emb_bwd(int dtype, const void* dpose, float* dpos_emb, float* dref_first, float* dref_other, int B, int S,
-                         cudaStream_t s) {
+                         int accumulate, cudaStream_t s) {
   const long long per = (long long)S * S * XU_POSE_DIM;
   double* acc = nullptr;
   if (dref_first != nullptr && (acc = xu_det_scratch(s, 2 * XU_POSE_DIM)) == nullptr) return;
   double* acc2 = acc ? acc + XU_POSE_DIM : nullptr;
-  if (dtype == XU_F32) xu_launch(pose_emb_bwd_kernel<float>, cdiv(per, 256), 256, 0, s, (const float*)dpose, dpos_emb, acc, acc2, B, S);
-  else xu_launch(pose_emb_bwd_kernel<bf16>, cdiv(per, 256), 256, 0, s, (const bf16*)dpose, dpos_emb, acc, acc2, B, S);
+  const int nb = cdiv(per, 256);
+  if (dtype == XU_F32) {
+    if (accumulate) xu_launch(pose_emb_bwd_kernel<float, true>, nb, 256, 0, s, (const float*)dpose, dpos_emb, acc, acc2, B, S);
+    else xu_launch(pose_emb_bwd_kernel<float, false>, nb, 256, 0, s, (const float*)dpose, dpos_emb, acc, acc2, B, S);
+  } else {
+    if (accumulate) xu_launch(pose_emb_bwd_kernel<bf16, true>, nb, 256, 0, s, (const bf16*)dpose, dpos_emb, acc, acc2, B, S);
+    else xu_launch(pose_emb_bwd_kernel<bf16, false>, nb, 256, 0, s, (const bf16*)dpose, dpos_emb, acc, acc2, B, S);
+  }
   if (acc != nullptr) {
     xu_det_fold(dref_first, acc, XU_POSE_DIM, s);
     xu_det_fold(dref_other, acc2, XU_POSE_DIM, s);

@@ -21,7 +21,7 @@ import torch
 
 from . import _lib
 from . import dist as xdist
-from .xunet import XUNet, XUNetConfig, ParamTree, Engine
+from .xunet import XUNet, XUNetConfig, ParamTree, Engine, InputSlots
 
 
 @dataclass
@@ -220,6 +220,36 @@ def _dropout_seed(step_plus_1: int) -> int:
     return (xdist.rank() << 40) + int(step_plus_1)
 
 
+MAX_GRAD_ACCUM_STEPS = 256      # micro-batch indices must fit in bits 32-39 of the dropout seed (_micro_batch_seed)
+
+
+def _micro_batch_seed(step_plus_1: int, j: int) -> int:
+    """Dropout seed of micro-batch j of optimisation step `step_plus_1` under gradient accumulation: micro-batch 0 keeps
+    _dropout_seed, micro-batch j adds j << 32.  j < 256 stays below the rank bits (40 and up), so every (rank, step, j) of a
+    run below 2**32 steps has its own seed."""
+    return _dropout_seed(step_plus_1) + (int(j) << 32)
+
+
+def check_grad_accum_steps(k) -> int:
+    """Validates TrainStep's grad_accum_steps: an int in [1, MAX_GRAD_ACCUM_STEPS]."""
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= MAX_GRAD_ACCUM_STEPS:
+        raise ValueError(f'grad_accum_steps must be an integer in [1, {MAX_GRAD_ACCUM_STEPS}], got {k!r}')
+    return int(k)
+
+
+def check_accum_batch(batch: dict, noise, cond_mask, k: int, B: int) -> None:
+    """Every array of a gradient-accumulation step (the batch dict, noise, and cond_mask when given) must have k*B rows:
+    micro-batch j is rows [j*B, (j+1)*B).  Raises ValueError otherwise."""
+    items = [(key, batch[key]) for key in ('x', 'z', 'logsnr', 'R1', 't1', 'R2', 't2', 'K')] + [('noise', noise)]
+    if cond_mask is not None:
+        items.append(('cond_mask', cond_mask))
+    for key, v in items:
+        shape = tuple(v.shape) if hasattr(v, 'shape') else np.shape(v)
+        rows = int(shape[0]) if shape else 0
+        if rows != k * B:
+            raise ValueError(f"{key} has leading dimension {rows}, expected grad_accum_steps * batch_size = {k} * {B} = {k * B}")
+
+
 def _cond_mask(state: TrainState, B: int) -> np.ndarray:
     # train.py:64  np.where(np.random.random(B) > 0.1, 1, 0)
     if state.reference_quirks:
@@ -268,14 +298,33 @@ class TrainStep:
     With gradient clipping the global-norm reduction runs right before Adam in every mode (after the all-reduce), inside
     the same graph as Adam.
 
+    grad_accum_steps=k (optax.MultiSteps(.., every_k_schedule=k)): each call takes k*B samples per rank (B =
+    state.batch_size) and runs k forward/backward passes of B samples, micro-batch j being rows [j*B, (j+1)*B); the first
+    backward overwrites the flat gradient buffer, the others add into it (xunet_backward_accumulate), and one update (norm,
+    Adam, EMA) follows with grad_scale = 1/(world*k): Adam of the mean micro-batch gradient.  The loss of each micro-batch is
+    its own Frobenius norm, so this is not the gradient of one batch of k*B samples (as data parallelism is not).  Under
+    data parallelism only the last backward carries the bucket hook, so the all-reduce covers the whole sum.  The returned
+    loss is the mean of the k micro-batch losses; `step` and the Adam count advance by one per call.  k = 1 (the default)
+    runs exactly the step without accumulation.
+
     A captured graph holds the NCCL kernels of the process group it was captured with: drop the TrainStep (or call
     `release_graphs()`) before `torch.distributed.destroy_process_group()`.
     """
 
-    def __init__(self, state: TrainState, *, use_graph: bool = True, bucket_mb: float = 128.0, allreduce: bool = True):
+    def __init__(self, state: TrainState, *, use_graph: bool = True, bucket_mb: float = 128.0, allreduce: bool = True,
+                 grad_accum_steps: int = 1):
         import os
+        self.k = check_grad_accum_steps(grad_accum_steps)
         self.state = state
         self.eng: Engine = state.model.engine(state.batch_size, state.img_sidelength, True)
+        if self.k > 1:
+            # the k micro-batches' inputs, dropout seeds and losses, all in device memory: the k forward/backward pairs of
+            # one graph read them in place, and a replay sees the seeds advance
+            self.inputs = InputSlots(self.eng.B, self.eng.S, self.k, self.eng.device)
+            self.seeds = torch.zeros(self.k, dtype=torch.int64, device=self.eng.device)
+            self.losses = torch.zeros(self.k, dtype=torch.float32, device=self.eng.device)
+            self.loss = torch.zeros(1, dtype=torch.float32, device=self.eng.device)
+        self._hook = False
         self.lib = _lib.load()
         self.dev = self.eng.device
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.dev)
@@ -316,22 +365,48 @@ class TrainStep:
         s = self.state
         if self._synced_count != s.opt_state.count:
             self.step_dev.fill_(s.opt_state.count)
-            self.eng.seed.fill_(0 if s.reference_quirks else _dropout_seed(s.opt_state.count))
+            if self.k == 1:
+                self.eng.seed.fill_(0 if s.reference_quirks else _dropout_seed(s.opt_state.count))
+            else:
+                seeds = [0 if s.reference_quirks else _micro_batch_seed(s.opt_state.count, j) for j in range(self.k)]
+                self.seeds.copy_(torch.tensor(seeds, dtype=torch.int64))
             self._synced_count = s.opt_state.count
 
     def _fwd_bwd(self):
         e, s = self.eng, self.state
+        if self.k == 1:
+            if not s.reference_quirks:
+                e.seed.add_(1)
+            self.step_dev.add_(1)
+            e.forward(s.params.flat, train=True)
+            if self.reducer is not None:
+                self.reducer.begin()
+            e.backward(s.params.flat)
+            return
         if not s.reference_quirks:
-            e.seed.add_(1)
+            self.seeds.add_(1)
         self.step_dev.add_(1)
-        e.forward(s.params.flat, train=True)
-        if self.reducer is not None:
-            self.reducer.begin()
-        e.backward(s.params.flat)
+        hook = self._hook
+        try:
+            if hook:
+                self._set_hook(False)        # a bucket is final only in the last backward
+            for j in range(self.k):
+                last = j == self.k - 1
+                sd = self.seeds[j:j + 1]
+                e.forward(s.params.flat, train=True, inputs=(self.inputs, j), seed_dev=sd)
+                if last:
+                    self._set_hook(hook)
+                    if self.reducer is not None:
+                        self.reducer.begin()
+                e.backward(s.params.flat, accumulate=j > 0, inputs=(self.inputs, j), seed_dev=sd,
+                           loss_out=self.losses[j:j + 1])
+        finally:
+            self._set_hook(hook)
+        torch.mean(self.losses, 0, keepdim=True, out=self.loss)
 
     def _adam(self):
         st = torch.cuda.current_stream(self.dev).cuda_stream
-        _adam_launch(self.lib, self.state, self.eng.grads, 0, self.step_dev, 1.0 / self.world, st)
+        _adam_launch(self.lib, self.state, self.eng.grads, 0, self.step_dev, 1.0 / (self.world * self.k), st)
 
     def _full_step(self):
         self._fwd_bwd()
@@ -340,6 +415,7 @@ class TrainStep:
         self._adam()
 
     def _set_hook(self, on: bool):
+        self._hook = on
         if self.reducer is None:
             return
         self.eng.set_bucket_callback(self.reducer.on_bucket if on else None, self.bucket_bytes)
@@ -347,7 +423,8 @@ class TrainStep:
     def _capture(self):
         torch.cuda.synchronize(self.dev)
         s = self.state
-        seed0, step0 = self.eng.seed.clone(), self.step_dev.clone()
+        seeds = self.eng.seed if self.k == 1 else self.seeds
+        seed0, step0 = seeds.clone(), self.step_dev.clone()
         backup = None
         one_graph = self.world == 1 or self.capture_collectives
         if one_graph:
@@ -382,7 +459,7 @@ class TrainStep:
             if backup is not None:
                 for t, b in zip(_opt_buffers(s), backup):
                     t.copy_(b)
-            self.eng.seed.copy_(seed0)
+            seeds.copy_(seed0)
             self.step_dev.copy_(step0)
             return self._capture()
         finally:
@@ -391,16 +468,24 @@ class TrainStep:
         if backup is not None:
             for t, b in zip(_opt_buffers(s), backup):
                 t.copy_(b)
-        self.eng.seed.copy_(seed0)
+        seeds.copy_(seed0)
         self.step_dev.copy_(step0)
 
     def __call__(self, batch: dict, noise, cond_mask=None) -> torch.Tensor:
         """One optimisation step on host (or device) inputs; returns the loss as a 0-d device tensor (a view of the engine's
-        loss slot: read or copy it before the next step)."""
+        loss slot: read or copy it before the next step).  With grad_accum_steps=k every array has k*B rows, and the loss
+        is the mean of the k micro-batch losses."""
         s = self.state
+        if self.k > 1:
+            check_accum_batch(batch, noise, cond_mask, self.k, self.eng.B)
         self._sync_counters()
-        mask = _cond_mask(s, self.eng.B) if cond_mask is None else cond_mask
-        self.h2d_bytes = self.eng.load_inputs(batch, cond_mask=mask, noise=noise)
+        if self.k == 1:
+            mask = _cond_mask(s, self.eng.B) if cond_mask is None else cond_mask
+            self.h2d_bytes = self.eng.load_inputs(batch, cond_mask=mask, noise=noise)
+        else:
+            # micro-batch j draws the j-th B values of the rank's stream: k = 1 consumes it exactly as before
+            mask = np.concatenate([_cond_mask(s, self.eng.B) for _ in range(self.k)]) if cond_mask is None else cond_mask
+            self.h2d_bytes = self.inputs.load(batch, cond_mask=mask, noise=noise)
         if self.use_graph:
             if self.graph_fb is None:
                 self._capture()
@@ -419,4 +504,4 @@ class TrainStep:
         s.step += 1
         s.opt_state.count += 1
         self._synced_count = s.opt_state.count
-        return self.eng.loss[0]
+        return self.eng.loss[0] if self.k == 1 else self.loss[0]

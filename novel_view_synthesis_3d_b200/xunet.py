@@ -127,9 +127,97 @@ def _seed_of(key, default=0) -> int:
     return ((hi << 32) | (int(arr[-1]) & 0xFFFFFFFF)) & 0x7FFFFFFFFFFFFFFF
 
 
+class InputSlots:
+    """Static device inputs of k batches of B samples (k micro-batches of one gradient-accumulation step; k = 1: the engine's
+    own inputs).  Slot j holds rows [j*B, (j+1)*B) of a k*B batch and has its own xunet_batch of device pointers.  All slots
+    live in ONE device buffer (and one pinned mirror), 256-byte aligned segments in INPUT_ORDER, slot after slot: a training
+    step stages every slot with a single H2D copy instead of ten small ones per slot (each costs ~7 us of stream time)."""
+    PIN_SLOTS = int(__import__('os').environ.get('XUNET_PIN_SLOTS', '3'))
+
+    def __init__(self, B: int, S: int, k: int, device):
+        self.B, self.k = B, k
+        f32 = dict(dtype=torch.float32, device=device)
+        self.shapes = {'x': (B, S, S, 3), 'z': (B, S, S, 3), 'logsnr': (B,), 'R1': (B, 3, 3), 't1': (B, 3), 'R2': (B, 3, 3),
+                       't2': (B, 3), 'K': (B, 3, 3), 'cond_mask': (B,), 'noise': (B, S, S, 3)}
+        self._seg, off = {}, 0          # (slot, key) -> (offset, elements)
+        for j in range(k):
+            for key in INPUT_ORDER:
+                n = int(np.prod(self.shapes[key]))
+                self._seg[j, key] = (off, n)
+                off += (n + 63) // 64 * 64
+        self.all = torch.zeros(off, **f32)
+        self.inp = [{key: self.all[o:o + n].view(self.shapes[key]) for key in INPUT_ORDER for o, n in [self._seg[j, key]]}
+                    for j in range(k)]
+        for d in self.inp:
+            d['cond_mask'].fill_(1.0)
+        # pinned staging ring: the host may run several steps ahead of the GPU (a step is a few ms of device time, the host
+        # side far less), so a slot is rewritten only after the H2D copy that last read it has completed (one event per slot)
+        self._pin_ring = [torch.zeros(off, dtype=torch.float32).pin_memory() for _ in range(self.PIN_SLOTS)]
+        self._pin_np = [t.numpy() for t in self._pin_ring]      # numpy views of the same pinned memory
+        self._pin_events = [None] * self.PIN_SLOTS
+        self._pin_next = 0
+        self.cbatch = [_lib.XunetBatch(**{key: d[key].data_ptr() for key in BATCH_KEYS + ('cond_mask',)}, rays=None)
+                       for d in self.inp]
+
+    def load(self, batch: dict, cond_mask=None, noise=None) -> int:
+        """Copies one batch dict of k*B samples (numpy / torch, any float dtype) into the slots, micro-batch j into slot j.
+        Returns the number of host->device bytes moved."""
+        k = self.k
+        nbytes = 0
+        items = [(key, batch[key]) for key in BATCH_KEYS]
+        if cond_mask is not None:
+            items.append(('cond_mask', cond_mask))
+        if noise is not None:
+            items.append(('noise', noise))
+        staged = []
+        slot, pin = None, None
+        for key, v in items:
+            shape = self.shapes[key]
+            if isinstance(v, torch.Tensor) and v.is_cuda:
+                v = v.reshape((k,) + shape)
+                for j in range(k):
+                    self.inp[j][key].copy_(v[j].to(torch.float32), non_blocking=True)
+                continue
+            src = (v.detach().float() if v.dtype == torch.bfloat16 else v.detach()).numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+            full = (k * shape[0],) + shape[1:]
+            if tuple(src.shape) != full and src.size != k * int(np.prod(shape)):
+                raise ValueError(f"batch['{key}'] has shape {tuple(src.shape)}, expected {full}")
+            if pin is None:
+                slot = self._pin_next
+                self._pin_next = (slot + 1) % self.PIN_SLOTS
+                if self._pin_events[slot] is not None:
+                    self._pin_events[slot].synchronize()      # the copy that last read this slot has finished
+                pin = self._pin_ring[slot]
+            # float64 -> float32 down-cast (as JAX does with x64 off) straight into pinned memory.  numpy, not torch: a torch CPU
+            # copy_ of ~1e5 elements fans out over every host core (3.5 ms on 8 threads against 0.1 ms single-threaded)
+            rows = src.reshape(k, -1)
+            for j in range(k):
+                o, n = self._seg[j, key]
+                np.copyto(self._pin_np[slot][o:o + n], rows[j], casting='unsafe')
+                staged.append(j * len(INPUT_ORDER) + INPUT_ORDER.index(key))
+                nbytes += n * 4
+        # one async H2D copy per run of adjacent segments (a full training batch = one copy)
+        idx = sorted(staged)
+        seg = lambda i: self._seg[i // len(INPUT_ORDER), INPUT_ORDER[i % len(INPUT_ORDER)]]
+        i = 0
+        while i < len(idx):
+            j = i
+            while j + 1 < len(idx) and idx[j + 1] == idx[j] + 1:
+                j += 1
+            lo = seg(idx[i])[0]
+            o, n = seg(idx[j])
+            self.all[lo:o + n].copy_(pin[lo:o + n], non_blocking=True)
+            i = j + 1
+        if pin is not None:
+            ev = self._pin_events[slot] or torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(self.all.device))
+            self._pin_events[slot] = ev
+        return nbytes
+
+
 class Engine:
     """One compiled execution plan: (config, B, S, training).  Owns the workspace and static I/O buffers."""
-    PIN_SLOTS = int(__import__('os').environ.get('XUNET_PIN_SLOTS', '3'))
+    PIN_SLOTS = InputSlots.PIN_SLOTS
 
     def __init__(self, cfg: XUNetConfig, B: int, S: int, training: bool, device=None):
         if not torch.cuda.is_available():
@@ -153,30 +241,13 @@ class Engine:
         self.ws_bytes = int(self.lib.xunet_workspace_bytes(h))
         self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=self.device)
         f32 = dict(dtype=torch.float32, device=self.device)
-        # all step inputs live in ONE device buffer (and one pinned mirror), 256-byte aligned segments in INPUT_ORDER: a
-        # training step stages its batch with a single H2D copy instead of ten small ones (each costs ~7 us of stream time)
-        shapes = {'x': (B, S, S, 3), 'z': (B, S, S, 3), 'logsnr': (B,), 'R1': (B, 3, 3), 't1': (B, 3), 'R2': (B, 3, 3), 't2': (B, 3),
-                  'K': (B, 3, 3), 'cond_mask': (B,), 'noise': (B, S, S, 3)}
-        self._seg, off = {}, 0
-        for k in INPUT_ORDER:
-            n = int(np.prod(shapes[k]))
-            self._seg[k] = (off, n)
-            off += (n + 63) // 64 * 64
-        self.inp_all = torch.zeros(off, **f32)
-        self.inp = {k: self.inp_all[o:o + n].view(shapes[k]) for k, (o, n) in self._seg.items()}
-        self.inp['cond_mask'].fill_(1.0)
-        # pinned staging ring: the host may run several steps ahead of the GPU (a step is a few ms of device time, the host
-        # side far less), so a slot is rewritten only after the H2D copy that last read it has completed (one event per slot)
-        self._pin_ring = [torch.zeros(off, dtype=torch.float32).pin_memory() for _ in range(self.PIN_SLOTS)]
-        self._pin_np = [t.numpy() for t in self._pin_ring]      # numpy views of the same pinned memory
-        self._pin_events = [None] * self.PIN_SLOTS
-        self._pin_next = 0
+        self.inputs = InputSlots(B, S, 1, self.device)
+        self.inp_all, self.inp, self.cbatch = self.inputs.all, self.inputs.inp[0], self.inputs.cbatch[0]
         self.rays = None          # optional (B,2,S,S,6) device tensor: explicit-rays entry (set_rays)
         self.eps = torch.zeros(B, S, S, 3, **f32)
         self.loss = torch.zeros(1, **f32)
         self.seed = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.grads = torch.zeros(self.nparams, **f32) if training else None
-        self.cbatch = _lib.XunetBatch(**{k: self.inp[k].data_ptr() for k in BATCH_KEYS + ('cond_mask',)}, rays=None)
         self._taps = None
         self._bucket_cb = None    # keeps the ctypes callback object alive while it is installed
 
@@ -192,50 +263,7 @@ class Engine:
     def load_inputs(self, batch: dict, cond_mask=None, noise=None) -> int:
         """Copies one batch dict (numpy / torch, any float dtype) into the static device buffers.
         Returns the number of host->device bytes moved."""
-        nbytes = 0
-        items = [(k, batch[k]) for k in BATCH_KEYS]
-        if cond_mask is not None:
-            items.append(('cond_mask', cond_mask))
-        if noise is not None:
-            items.append(('noise', noise))
-        staged = []
-        slot, pin = None, None
-        for k, v in items:
-            dst = self.inp[k]
-            if isinstance(v, torch.Tensor) and v.is_cuda:
-                dst.copy_(v.reshape(dst.shape).to(torch.float32), non_blocking=True)
-                continue
-            src = (v.detach().float() if v.dtype == torch.bfloat16 else v.detach()).numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
-            if tuple(src.shape) != tuple(dst.shape) and src.size != dst.numel():
-                raise ValueError(f"batch['{k}'] has shape {tuple(src.shape)}, expected {tuple(dst.shape)}")
-            if pin is None:
-                slot = self._pin_next
-                self._pin_next = (slot + 1) % self.PIN_SLOTS
-                if self._pin_events[slot] is not None:
-                    self._pin_events[slot].synchronize()      # the copy that last read this slot has finished
-                pin = self._pin_ring[slot]
-            o, n = self._seg[k]
-            # float64 -> float32 down-cast (as JAX does with x64 off) straight into pinned memory.  numpy, not torch: a torch CPU
-            # copy_ of ~1e5 elements fans out over every host core (3.5 ms on 8 threads against 0.1 ms single-threaded)
-            np.copyto(self._pin_np[slot][o:o + n], src.reshape(-1), casting='unsafe')
-            staged.append(k)
-            nbytes += dst.numel() * 4
-        # one async H2D copy per run of adjacent segments (a full training batch = one copy)
-        idx = sorted(INPUT_ORDER.index(k) for k in staged)
-        i = 0
-        while i < len(idx):
-            j = i
-            while j + 1 < len(idx) and idx[j + 1] == idx[j] + 1:
-                j += 1
-            lo = self._seg[INPUT_ORDER[idx[i]]][0]
-            o, n = self._seg[INPUT_ORDER[idx[j]]]
-            self.inp_all[lo:o + n].copy_(pin[lo:o + n], non_blocking=True)
-            i = j + 1
-        if pin is not None:
-            ev = self._pin_events[slot] or torch.cuda.Event()
-            ev.record(torch.cuda.current_stream(self.device))
-            self._pin_events[slot] = ev
-        return nbytes
+        return self.inputs.load(batch, cond_mask=cond_mask, noise=noise)
 
     def set_rays(self, rays) -> None:
         """Explicit-rays entry (SURVEY 8(c)): `rays` = (B, 2, S, S, 6) [pos xyz | dir xyz] for camera 1 / camera 2, e.g. the
@@ -263,24 +291,35 @@ class Engine:
         self._bucket_cb = cb
         return int(self.lib.xunet_grad_bucket_count(self.h))
 
-    def forward(self, flat_params: torch.Tensor, *, train: bool, seed: Optional[int] = None) -> torch.Tensor:
+    def forward(self, flat_params: torch.Tensor, *, train: bool, seed: Optional[int] = None,
+                inputs: Optional[Tuple[InputSlots, int]] = None, seed_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """inputs=(slots, j): read slot j of `slots` instead of the engine's own inputs; seed_dev: a device int64 to read the
+        dropout seed from instead of `self.seed` (both default to the engine's own buffers)."""
         assert flat_params.dtype == torch.float32 and flat_params.is_cuda and flat_params.numel() == self.nparams
         if seed is not None:
             self.seed.fill_(int(seed) & 0x7FFFFFFFFFFFFFFF)
+        cb = self.cbatch if inputs is None else inputs[0].cbatch[inputs[1]]
+        sd = self.seed if seed_dev is None else seed_dev
         st = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(self.lib.xunet_forward(self.h, flat_params.data_ptr(), C.byref(self.cbatch), int(train),
-                                          self.seed.data_ptr(), self.ws.data_ptr(), self.eps.data_ptr(), st), 'xunet_forward')
+        _lib.check(self.lib.xunet_forward(self.h, flat_params.data_ptr(), C.byref(cb), int(train),
+                                          sd.data_ptr(), self.ws.data_ptr(), self.eps.data_ptr(), st), 'xunet_forward')
         return self.eps
 
-    def backward(self, flat_params: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-        """loss = ||eps - noise||_F and its parameter gradient (train.py:62-71); follows forward()."""
+    def backward(self, flat_params: torch.Tensor, *, accumulate: bool = False, inputs: Optional[Tuple[InputSlots, int]] = None,
+                 seed_dev: Optional[torch.Tensor] = None, loss_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """loss = ||eps - noise||_F and its parameter gradient (train.py:62-71); follows forward() with the same `inputs` and
+        `seed_dev`.  accumulate=True adds the gradient into `self.grads` (xunet_backward_accumulate) instead of overwriting it.
+        loss_out: a device float to write the loss to instead of `self.loss`."""
         if not self.training:
             raise RuntimeError('engine was built with training=False')
+        cb, noise = (self.cbatch, self.inp['noise']) if inputs is None else (inputs[0].cbatch[inputs[1]], inputs[0].inp[inputs[1]]['noise'])
+        sd = self.seed if seed_dev is None else seed_dev
+        loss = self.loss if loss_out is None else loss_out
+        fn = self.lib.xunet_backward_accumulate if accumulate else self.lib.xunet_backward
         st = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(self.lib.xunet_backward(self.h, flat_params.data_ptr(), C.byref(self.cbatch), self.inp['noise'].data_ptr(),
-                                           self.seed.data_ptr(), self.ws.data_ptr(), self.grads.data_ptr(),
-                                           self.loss.data_ptr(), st), 'xunet_backward')
-        return self.loss, self.grads
+        _lib.check(fn(self.h, flat_params.data_ptr(), C.byref(cb), noise.data_ptr(), sd.data_ptr(), self.ws.data_ptr(),
+                      self.grads.data_ptr(), loss.data_ptr(), st), 'xunet_backward_accumulate' if accumulate else 'xunet_backward')
+        return loss, self.grads
 
     def count_kernels(self, flat_params: torch.Tensor) -> Tuple[int, int]:
         """(forward, backward) kernel launches of this plan, counted from a throw-away graph capture."""
