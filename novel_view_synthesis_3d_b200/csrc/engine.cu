@@ -1076,7 +1076,8 @@ extern "C" int xunet_adam_step(float* params, const float* grads, float* m, floa
                                const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
                                void* stream) {
   if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_step: bad argument");
-  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, nullptr, 0.0, (cudaStream_t)stream);
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, nullptr, 0.0, nullptr, 0.0, 0, nullptr,
+              (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("adam: CUDA error: %s", cudaGetErrorString(e));
 }
@@ -1087,7 +1088,8 @@ extern "C" int xunet_adam_ema_step(float* params, const float* grads, float* m, 
   if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_ema_step: bad argument");
   if (!ema) return fail("xunet_adam_ema_step: ema is NULL (use xunet_adam_step without an EMA)");
   if (!(ema_decay >= 0.0 && ema_decay <= 1.0)) return fail("xunet_adam_ema_step: ema_decay %g outside [0, 1]", ema_decay);
-  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema_decay, (cudaStream_t)stream);
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema_decay, nullptr, 0.0, 0, nullptr,
+              (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("adam_ema: CUDA error: %s", cudaGetErrorString(e));
 }
@@ -1111,8 +1113,8 @@ extern "C" int xunet_adam_clip_step(float* params, const float* grads, float* m,
     if (!(max_norm > 0.0)) return fail("xunet_adam_clip_step: max_norm %g must be > 0", max_norm);
     if (!skipped_dev) return fail("xunet_adam_clip_step: skipped_dev is NULL (needed with norm_dev)");
   }
-  launch_adam_clip(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema ? ema_decay : 0.0, norm_dev,
-                   max_norm, warmup_steps, skipped_dev, (cudaStream_t)stream);
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema ? ema_decay : 0.0, norm_dev,
+              max_norm, warmup_steps, skipped_dev, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("adam_clip: CUDA error: %s", cudaGetErrorString(e));
 }

@@ -121,18 +121,16 @@ void launch_extract_frame1(int dtype, const void* o, float* eps, int B, int S, c
 // loss = ||eps - noise||_F ; dO (2B,S,S,3): frame0 = 0, frame1 = (eps-noise)/loss
 void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_scratch, float* loss_out, void* dO, int B,
                  int S, cudaStream_t s);
-// ema == nullptr: plain Adam; otherwise also ema = decay*ema + (1-decay)*p_new in the same pass
+// Adam; with ema, also ema = decay*ema + (1-decay)*p_new in the same pass.  warmup > 0: lr_t = lr * min(step - 1, warmup) /
+// warmup; norm_dev: optax.clip_by_global_norm by *norm_dev, where a non-finite *norm_dev leaves every buffer untouched and
+// increments *skipped.  Neither (norm_dev == nullptr, warmup == 0): plain Adam, without the clip / warm-up prologue.
 void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay, cudaStream_t s);
+                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
+                 const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s);
 // *norm_out = sqrt(sum_i fp32(g_i * grad_scale)^2), summed in fp64 in a fixed order (grid from n only, no atomics).
 // scratch: XUNET_GRAD_NORM_SCRATCH doubles; on completion scratch[0] holds the fp64 sum of squares.  Two launches.
 void launch_grad_global_norm(const float* g, long long n, double grad_scale, double* scratch, float* norm_out,
                              cudaStream_t s);
-// launch_adam with lr_t = lr * min(step - 1, warmup) / warmup (warmup > 0) and, with norm_dev, optax.clip_by_global_norm by
-// *norm_dev; a non-finite *norm_dev leaves every buffer untouched and increments *skipped
-void launch_adam_clip(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                      double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
-                      const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s);
 void launch_sampler_update(const float* eps2, const float* z, const float* noise, float* z_out, long long n, float w,
                            float c_recip, float c_recipm1, float c1, float c2, float sigma, unsigned long long seed,
                            cudaStream_t s);

@@ -1598,21 +1598,52 @@ void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_s
 // EMA = true also folds the weight EMA into the same pass: ema = d*ema + (1-d)*p_new with p_new still in registers (8 more
 // bytes per parameter instead of 12 for a separate pass).  The _rn intrinsics forbid FMA contraction, so a float32 numpy
 // restatement matches bit for bit.
-template <bool EMA>
+// CLIP = true adds a linear learning-rate warm-up and clipping by a global norm read from the device.  Thread 0 of each CTA
+// also forms lr_t = lr * min(step - 1, W) / W in double rounded once (optax.linear_schedule(0, lr, W) evaluated at the
+// schedule's count, which lags Adam's by one), and the clip decision of optax.clip_by_global_norm: g' = g if norm < max_norm,
+// else fl(fl(g / norm) * max_norm).  A non-finite norm skips the step: every CTA returns before touching p / m / v / ema and
+// CTA 0 counts it in *skipped.  norm == nullptr: no clipping and no guard.  With g' == g and lr_t == lr both instantiations
+// give the same bits; CLIP is a template parameter so that plain Adam keeps its 40 registers (6 CTAs per SM, 46 with CLIP).
+template <bool EMA, bool CLIP>
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, float* __restrict__ ema, long long n, long long step,
                                                    const long long* __restrict__ step_dev, double lr, double b1d, double b2d,
-                                                   float eps, float gs, double decay) {
+                                                   float eps, float gs, double decay, const float* __restrict__ norm_dev,
+                                                   float max_norm, long long warmup, long long* __restrict__ skipped) {
   xu_grid_dep_sync();
-  __shared__ float sc[2];
+  __shared__ float sc[CLIP ? 4 : 2];
+  __shared__ int mode;   // CLIP: 0 plain gradient, 1 clipped, 2 skip the step
   if (threadIdx.x == 0) {
     const long long st = step_dev != nullptr ? *step_dev : step;
     sc[0] = (float)(1.0 / (1.0 - pow(b1d, (double)st)));
     sc[1] = (float)(1.0 / (1.0 - pow(b2d, (double)st)));
+    if constexpr (CLIP) {
+      const long long c = st - 1;
+      sc[2] = warmup > 0 ? (float)(lr * (double)(c < warmup ? c : warmup) / (double)warmup) : (float)lr;
+      int md = 0;
+      sc[3] = 1.f;
+      if (norm_dev != nullptr) {
+        const float nrm = *norm_dev;
+        sc[3] = nrm;
+        md = !isfinite(nrm) ? 2 : (nrm < max_norm ? 0 : 1);
+        if (md == 2 && blockIdx.x == 0) *skipped += 1;
+      }
+      mode = md;
+    }
   }
   __syncthreads();
+  int md = 0;
+  if constexpr (CLIP) {
+    md = mode;
+    if (md == 2) return;
+  }
   const float c1 = sc[0], c2 = sc[1];
-  const float b1 = (float)b1d, b2 = (float)b2d, omb1 = (float)(1.0 - b1d), omb2 = (float)(1.0 - b2d), lrf = (float)lr;
+  const float b1 = (float)b1d, b2 = (float)b2d, omb1 = (float)(1.0 - b1d), omb2 = (float)(1.0 - b2d);
+  float lrf = (float)lr, nrm = 1.f;
+  if constexpr (CLIP) {
+    lrf = sc[2];
+    nrm = sc[3];
+  }
   const float d = (float)decay, omd = (float)(1.0 - decay);
   // 16-byte accesses (7 streams of n floats: 4 read, 3 written; 9 with the EMA: 5 read, 4 written -- the kernel is pure HBM
   // traffic); scalar path for a ragged tail or unaligned sub-ranges
@@ -1623,6 +1654,7 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
   const long long n4 = vec ? (n >> 2) : 0;
   auto upd = [&](float gi, float& mi, float& vi, float& pi) {
     gi *= gs;
+    if (CLIP && md == 1) gi = __fmul_rn(__fdiv_rn(gi, nrm), max_norm);
     mi = b1 * mi + omb1 * gi;
     vi = b2 * vi + omb2 * gi * gi;
     pi -= lrf * (mi * c1) / (sqrtf(vi * c2) + eps);
@@ -1653,16 +1685,16 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
   }
 }
 void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay, cudaStream_t s) {
+                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
+                 const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s) {
   int blocks = cdiv(n, 256 * 4);   // one float4 per thread and pass
   if (blocks > xu_num_sms() * 8) blocks = xu_num_sms() * 8;
   if (blocks < 1) blocks = 1;
-  if (ema == nullptr)
-    xu_launch(adam_kernel<false>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
-              (float)grad_scale, 0.0);
-  else
-    xu_launch(adam_kernel<true>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
-              (float)grad_scale, decay);
+  const bool clip = norm_dev != nullptr || warmup > 0;
+  auto kernel = ema == nullptr ? (clip ? adam_kernel<false, true> : adam_kernel<false, false>)
+                               : (clip ? adam_kernel<true, true> : adam_kernel<true, false>);
+  xu_launch(kernel, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps, (float)grad_scale,
+            decay, norm_dev, (float)max_norm, warmup, skipped);
 }
 
 // ---- global gradient norm (optax.clip_by_global_norm) ----------------------------------------------------------------------
@@ -1723,96 +1755,6 @@ void launch_grad_global_norm(const float* g, long long n, double grad_scale, dou
   const int parts = grad_norm_partials(n);
   xu_launch(grad_sumsq_partial_kernel, parts, 256, 0, s, g, n, (float)grad_scale, scratch);
   xu_launch(grad_norm_final_kernel, 1, 256, 0, s, scratch, parts, norm_out);
-}
-
-// adam_kernel with a linear learning-rate warm-up and clipping by a global norm read from the device.  Thread 0 of each CTA
-// forms, from the device step counter, the bias corrections (as adam_kernel), lr_t = lr * min(step - 1, W) / W in double
-// rounded once (optax.linear_schedule(0, lr, W) evaluated at the schedule's count, which lags Adam's by one), and the clip
-// decision of optax.clip_by_global_norm: g' = g if norm < max_norm, else fl(fl(g / norm) * max_norm).  A non-finite norm skips
-// the step: every CTA returns before touching p / m / v / ema and CTA 0 counts it in *skipped.  norm == nullptr: no clipping
-// and no guard.  The Adam and EMA arithmetic is written exactly as in adam_kernel, so with g' == g and lr_t == lr the two give
-// the same bits.
-template <bool EMA>
-__global__ void __launch_bounds__(256) adam_clip_kernel(float* __restrict__ p, const float* __restrict__ g,
-                                                        float* __restrict__ m, float* __restrict__ v, float* __restrict__ ema,
-                                                        long long n, long long step, const long long* __restrict__ step_dev,
-                                                        double lr, double b1d, double b2d, float eps, float gs, double decay,
-                                                        const float* __restrict__ norm_dev, float max_norm, long long warmup,
-                                                        long long* __restrict__ skipped) {
-  xu_grid_dep_sync();
-  __shared__ float sc[4];
-  __shared__ int mode;   // 0: plain gradient, 1: clipped, 2: skip the step
-  if (threadIdx.x == 0) {
-    const long long st = step_dev != nullptr ? *step_dev : step;
-    sc[0] = (float)(1.0 / (1.0 - pow(b1d, (double)st)));
-    sc[1] = (float)(1.0 / (1.0 - pow(b2d, (double)st)));
-    const long long c = st - 1;
-    sc[2] = warmup > 0 ? (float)(lr * (double)(c < warmup ? c : warmup) / (double)warmup) : (float)lr;
-    int md = 0;
-    sc[3] = 1.f;
-    if (norm_dev != nullptr) {
-      const float nrm = *norm_dev;
-      sc[3] = nrm;
-      md = !isfinite(nrm) ? 2 : (nrm < max_norm ? 0 : 1);
-      if (md == 2 && blockIdx.x == 0) *skipped += 1;
-    }
-    mode = md;
-  }
-  __syncthreads();
-  const int md = mode;
-  if (md == 2) return;
-  const float c1 = sc[0], c2 = sc[1], lrf = sc[2], nrm = sc[3];
-  const float b1 = (float)b1d, b2 = (float)b2d, omb1 = (float)(1.0 - b1d), omb2 = (float)(1.0 - b2d);
-  const float d = (float)decay, omd = (float)(1.0 - decay);
-  uintptr_t addr_or = reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
-                      reinterpret_cast<uintptr_t>(v);
-  if (EMA) addr_or |= reinterpret_cast<uintptr_t>(ema);
-  const bool vec = (addr_or & 15) == 0;
-  const long long n4 = vec ? (n >> 2) : 0;
-  auto upd = [&](float gi, float& mi, float& vi, float& pi) {
-    gi *= gs;
-    if (md == 1) gi = __fmul_rn(__fdiv_rn(gi, nrm), max_norm);
-    mi = b1 * mi + omb1 * gi;
-    vi = b2 * vi + omb2 * gi * gi;
-    pi -= lrf * (mi * c1) / (sqrtf(vi * c2) + eps);
-  };
-  auto avg = [&](float& ei, float pi) { ei = __fadd_rn(__fmul_rn(d, ei), __fmul_rn(omd, pi)); };
-  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
-    const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + i);
-    float4 m4 = reinterpret_cast<float4*>(m)[i], v4 = reinterpret_cast<float4*>(v)[i], p4 = reinterpret_cast<float4*>(p)[i];
-    upd(g4.x, m4.x, v4.x, p4.x); upd(g4.y, m4.y, v4.y, p4.y); upd(g4.z, m4.z, v4.z, p4.z); upd(g4.w, m4.w, v4.w, p4.w);
-    reinterpret_cast<float4*>(m)[i] = m4;
-    reinterpret_cast<float4*>(v)[i] = v4;
-    reinterpret_cast<float4*>(p)[i] = p4;
-    if (EMA) {
-      float4 e4 = reinterpret_cast<float4*>(ema)[i];
-      avg(e4.x, p4.x); avg(e4.y, p4.y); avg(e4.z, p4.z); avg(e4.w, p4.w);
-      reinterpret_cast<float4*>(ema)[i] = e4;
-    }
-  }
-  for (long long i = n4 * 4 + (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
-    float mi = m[i], vi = v[i], pi = p[i];
-    upd(g[i], mi, vi, pi);
-    m[i] = mi; v[i] = vi; p[i] = pi;
-    if (EMA) {
-      float ei = ema[i];
-      avg(ei, pi);
-      ema[i] = ei;
-    }
-  }
-}
-void launch_adam_clip(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                      double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
-                      const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s) {
-  int blocks = cdiv(n, 256 * 4);   // the grid of launch_adam
-  if (blocks > xu_num_sms() * 8) blocks = xu_num_sms() * 8;
-  if (blocks < 1) blocks = 1;
-  if (ema == nullptr)
-    xu_launch(adam_clip_kernel<false>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
-              (float)grad_scale, 0.0, norm_dev, (float)max_norm, warmup, skipped);
-  else
-    xu_launch(adam_clip_kernel<true>, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps,
-              (float)grad_scale, decay, norm_dev, (float)max_norm, warmup, skipped);
 }
 
 // sampling.py:128-151 elementwise update

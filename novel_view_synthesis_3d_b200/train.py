@@ -11,8 +11,6 @@ dropout seed are fresh per step unless reference_quirks=True (the reference free
 from __future__ import annotations
 
 import os
-
-import ctypes as C
 from dataclasses import dataclass, replace
 from typing import Optional
 
@@ -21,7 +19,7 @@ import torch
 
 from . import _lib
 from . import dist as xdist
-from .xunet import XUNet, XUNetConfig, ParamTree, Engine, InputSlots
+from .xunet import XUNet, ParamTree, Engine, InputSlots
 
 
 @dataclass
@@ -45,7 +43,7 @@ class Adam:
 
     @property
     def clip_or_warmup(self) -> bool:
-        """The step goes through the clip / warm-up launches (xunet_adam_clip_step)."""
+        """The step clips the gradient or warms the learning rate up (and the state carries a ClipState)."""
         return self.max_grad_norm is not None or self.warmup_steps > 0
 
 
@@ -120,32 +118,22 @@ class TrainState:
 
 
 def _adam_launch(lib, s: TrainState, flat_g: torch.Tensor, count: int, step_dev, grad_scale: float, stream: int) -> None:
-    """One Adam pass over the flat buffers of `s`; with an EMA buffer the fused Adam + EMA entry point.  With clipping or
-    warm-up: the global-norm reduction (clipping only), then the clip / warm-up Adam pass (EMA included)."""
-    p = s.params.flat
-    st_dev = None if step_dev is None else step_dev.data_ptr()
-    if s.tx.clip_or_warmup:
-        tx, c = s.tx, s.clip
-        ema = None if s.ema_params is None else s.ema_params.flat.data_ptr()
-        norm = None
-        if tx.max_grad_norm is not None:
-            _lib.check(lib.xunet_grad_global_norm(flat_g.data_ptr(), p.numel(), grad_scale, c.scratch.data_ptr(),
-                                                  c.norm.data_ptr(), stream), 'xunet_grad_global_norm')
-            norm = c.norm.data_ptr()
-        _lib.check(lib.xunet_adam_clip_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(),
-                                            s.opt_state.nu.data_ptr(), ema, p.numel(), count, st_dev, tx.learning_rate,
-                                            tx.b1, tx.b2, tx.eps, grad_scale, s.ema_decay or 0.0, norm,
-                                            tx.max_grad_norm or 0.0, tx.warmup_steps, c.skipped.data_ptr(), stream),
-                   'xunet_adam_clip_step')
-    elif s.ema_params is None:
-        _lib.check(lib.xunet_adam_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(), s.opt_state.nu.data_ptr(),
-                                       p.numel(), count, st_dev, s.tx.learning_rate, s.tx.b1, s.tx.b2, s.tx.eps, grad_scale,
-                                       stream), 'xunet_adam_step')
-    else:
-        _lib.check(lib.xunet_adam_ema_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(),
-                                           s.opt_state.nu.data_ptr(), s.ema_params.flat.data_ptr(), p.numel(), count, st_dev,
-                                           s.tx.learning_rate, s.tx.b1, s.tx.b2, s.tx.eps, grad_scale, s.ema_decay, stream),
-                   'xunet_adam_ema_step')
+    """One fused Adam pass over the flat buffers of `s`, with the EMA update, warm-up and clipping the state carries (the
+    library runs plain Adam without the clip / warm-up prologue when there is neither).  With clipping the global-norm
+    reduction runs first."""
+    p, tx, c = s.params.flat, s.tx, s.clip
+    ptr = lambda t: None if t is None else t.data_ptr()
+    norm = None
+    if tx.max_grad_norm is not None:
+        _lib.check(lib.xunet_grad_global_norm(flat_g.data_ptr(), p.numel(), grad_scale, c.scratch.data_ptr(),
+                                              c.norm.data_ptr(), stream), 'xunet_grad_global_norm')
+        norm = c.norm
+    ema = None if s.ema_params is None else s.ema_params.flat
+    skipped = None if c is None else c.skipped
+    _lib.check(lib.xunet_adam_clip_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(), s.opt_state.nu.data_ptr(),
+                                        ptr(ema), p.numel(), count, ptr(step_dev), tx.learning_rate, tx.b1, tx.b2, tx.eps,
+                                        grad_scale, s.ema_decay or 0.0, ptr(norm), tx.max_grad_norm or 0.0, tx.warmup_steps,
+                                        ptr(skipped), stream), 'xunet_adam_clip_step')
 
 
 def _opt_buffers(s: TrainState):
@@ -313,27 +301,29 @@ class TrainStep:
 
     def __init__(self, state: TrainState, *, use_graph: bool = True, bucket_mb: float = 128.0, allreduce: bool = True,
                  grad_accum_steps: int = 1):
-        import os
         self.k = check_grad_accum_steps(grad_accum_steps)
         self.state = state
         self.eng: Engine = state.model.engine(state.batch_size, state.img_sidelength, True)
-        if self.k > 1:
-            # the k micro-batches' inputs, dropout seeds and losses, all in device memory: the k forward/backward pairs of
-            # one graph read them in place, and a replay sees the seeds advance
-            self.inputs = InputSlots(self.eng.B, self.eng.S, self.k, self.eng.device)
-            self.seeds = torch.zeros(self.k, dtype=torch.int64, device=self.eng.device)
-            self.losses = torch.zeros(self.k, dtype=torch.float32, device=self.eng.device)
-            self.loss = torch.zeros(1, dtype=torch.float32, device=self.eng.device)
+        self.dev = self.eng.device
+        # the k micro-batches' inputs, dropout seeds and losses, all in device memory: the k forward/backward pairs of one
+        # graph read them in place, and a replay sees the seeds advance.  k = 1: the engine's own buffers, and `loss` is the
+        # engine's loss slot rather than a mean of one
+        if self.k == 1:
+            self.inputs, self.seeds, self.losses = self.eng.inputs, self.eng.seed, self.eng.loss
+            self.loss = self.eng.loss
+        else:
+            self.inputs = InputSlots(self.eng.B, self.eng.S, self.k, self.dev)
+            self.seeds = torch.zeros(self.k, dtype=torch.int64, device=self.dev)
+            self.losses = torch.zeros(self.k, dtype=torch.float32, device=self.dev)
+            self.loss = torch.zeros(1, dtype=torch.float32, device=self.dev)
         self._hook = False
         self.lib = _lib.load()
-        self.dev = self.eng.device
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.dev)
         self.world = xdist.world_size()
         self.use_graph = use_graph
         self.graph_fb = None      # forward+backward (+ all-reduce + adam when everything is in one graph)
         self.graph_opt = None     # adam (two-graph mode only)
         self.stream = torch.cuda.Stream(device=self.dev) if use_graph else None
-        self.launches_per_step = None
         self.allreduce = allreduce and self.world > 1       # allreduce=False: measurement knob (compute-only step at N>1)
         # XUNET_DP_BUCKET_MB overrides the bucket size (experiments: smaller buckets start the collectives earlier but add launches)
         if os.environ.get('XUNET_DP_BUCKET_MB'):
@@ -365,24 +355,12 @@ class TrainStep:
         s = self.state
         if self._synced_count != s.opt_state.count:
             self.step_dev.fill_(s.opt_state.count)
-            if self.k == 1:
-                self.eng.seed.fill_(0 if s.reference_quirks else _dropout_seed(s.opt_state.count))
-            else:
-                seeds = [0 if s.reference_quirks else _micro_batch_seed(s.opt_state.count, j) for j in range(self.k)]
-                self.seeds.copy_(torch.tensor(seeds, dtype=torch.int64))
+            seeds = [0 if s.reference_quirks else _micro_batch_seed(s.opt_state.count, j) for j in range(self.k)]
+            self.seeds.copy_(torch.tensor(seeds, dtype=torch.int64))
             self._synced_count = s.opt_state.count
 
     def _fwd_bwd(self):
         e, s = self.eng, self.state
-        if self.k == 1:
-            if not s.reference_quirks:
-                e.seed.add_(1)
-            self.step_dev.add_(1)
-            e.forward(s.params.flat, train=True)
-            if self.reducer is not None:
-                self.reducer.begin()
-            e.backward(s.params.flat)
-            return
         if not s.reference_quirks:
             self.seeds.add_(1)
         self.step_dev.add_(1)
@@ -402,7 +380,8 @@ class TrainStep:
                            loss_out=self.losses[j:j + 1])
         finally:
             self._set_hook(hook)
-        torch.mean(self.losses, 0, keepdim=True, out=self.loss)
+        if self.k > 1:
+            torch.mean(self.losses, 0, keepdim=True, out=self.loss)
 
     def _adam(self):
         st = torch.cuda.current_stream(self.dev).cuda_stream
@@ -421,15 +400,13 @@ class TrainStep:
         self.eng.set_bucket_callback(self.reducer.on_bucket if on else None, self.bucket_bytes)
 
     def _capture(self):
-        torch.cuda.synchronize(self.dev)
-        s = self.state
-        seeds = self.eng.seed if self.k == 1 else self.seeds
-        seed0, step0 = seeds.clone(), self.step_dev.clone()
-        backup = None
         one_graph = self.world == 1 or self.capture_collectives
-        if one_graph:
-            # warm-up and capture run real Adam updates: snapshot params/moments/EMA and restore them afterwards
-            backup = [t.clone() for t in _opt_buffers(s)]
+        # warm-up and capture advance the seeds and the step counter and, with Adam in the graph, run real updates: snapshot
+        # what they write and restore it afterwards.  The synchronize orders the snapshot before the warm-up's stream.
+        saved = [self.seeds, self.step_dev] + (_opt_buffers(self.state) if one_graph else [])
+        backup = [t.clone() for t in saved]
+        torch.cuda.synchronize(self.dev)
+        retry = False
         try:
             with torch.cuda.stream(self.stream):
                 self._set_hook(one_graph)
@@ -453,39 +430,28 @@ class TrainStep:
             if not (one_graph and self.world > 1):
                 raise
             # capturing the collectives failed: fall back to eager all-reduces between two graphs
-            torch.cuda.synchronize(self.dev)
             self.capture_collectives = False
             self.graph_fb = self.graph_opt = None
-            if backup is not None:
-                for t, b in zip(_opt_buffers(s), backup):
-                    t.copy_(b)
-            seeds.copy_(seed0)
-            self.step_dev.copy_(step0)
-            return self._capture()
+            retry = True
         finally:
             self._set_hook(False)
         torch.cuda.synchronize(self.dev)
-        if backup is not None:
-            for t, b in zip(_opt_buffers(s), backup):
-                t.copy_(b)
-        seeds.copy_(seed0)
-        self.step_dev.copy_(step0)
+        for t, b in zip(saved, backup):
+            t.copy_(b)
+        if retry:
+            self._capture()
 
     def __call__(self, batch: dict, noise, cond_mask=None) -> torch.Tensor:
-        """One optimisation step on host (or device) inputs; returns the loss as a 0-d device tensor (a view of the engine's
+        """One optimisation step on host (or device) inputs; returns the loss as a 0-d device tensor (a view of the step's
         loss slot: read or copy it before the next step).  With grad_accum_steps=k every array has k*B rows, and the loss
         is the mean of the k micro-batch losses."""
         s = self.state
         if self.k > 1:
             check_accum_batch(batch, noise, cond_mask, self.k, self.eng.B)
         self._sync_counters()
-        if self.k == 1:
-            mask = _cond_mask(s, self.eng.B) if cond_mask is None else cond_mask
-            self.h2d_bytes = self.eng.load_inputs(batch, cond_mask=mask, noise=noise)
-        else:
-            # micro-batch j draws the j-th B values of the rank's stream: k = 1 consumes it exactly as before
-            mask = np.concatenate([_cond_mask(s, self.eng.B) for _ in range(self.k)]) if cond_mask is None else cond_mask
-            self.h2d_bytes = self.inputs.load(batch, cond_mask=mask, noise=noise)
+        # micro-batch j draws the j-th B values of the rank's cond_mask stream
+        mask = np.concatenate([_cond_mask(s, self.eng.B) for _ in range(self.k)]) if cond_mask is None else cond_mask
+        self.h2d_bytes = self.inputs.load(batch, cond_mask=mask, noise=noise)
         if self.use_graph:
             if self.graph_fb is None:
                 self._capture()
@@ -504,4 +470,4 @@ class TrainStep:
         s.step += 1
         s.opt_state.count += 1
         self._synced_count = s.opt_state.count
-        return self.eng.loss[0] if self.k == 1 else self.loss[0]
+        return self.loss[0]

@@ -220,7 +220,9 @@ def test_cond_mask_stream_is_consumed_in_micro_batch_order():
         assert np.array_equal(got, want), i
 
 
-def test_k1_is_the_step_without_accumulation():
+def test_k1_runs_the_loop_on_the_engine_buffers():
+    """grad_accum_steps=1 is the default step, and its micro-batch loop stages, seeds and scores in the engine's own buffers
+    (nothing is allocated twice)."""
     def run(**kw):
         st = _new_state(ema_decay=0.9)
         step = P.TrainStep(st, **kw)
@@ -234,7 +236,8 @@ def test_k1_is_the_step_without_accumulation():
     l0, s0, t0 = run()
     l1, s1, t1 = run(grad_accum_steps=1)
     assert l0 == l1 and _same_state(s0, s1) and torch.equal(s0.ema_params.flat, s1.ema_params.flat)
-    assert torch.equal(t0.eng.grads, t1.eng.grads) and not hasattr(t1, 'inputs')
+    assert torch.equal(t0.eng.grads, t1.eng.grads)
+    assert t1.inputs is t1.eng.inputs and t1.seeds is t1.eng.seed and t1.loss is t1.eng.loss
 
 
 def test_wrong_leading_dimension_raises():
