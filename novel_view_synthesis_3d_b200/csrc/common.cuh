@@ -177,8 +177,6 @@ static inline void xu_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, si
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  static const long long max_blocks = getenv("XUNET_PDL_MAX_BLOCKS") ? atoll(getenv("XUNET_PDL_MAX_BLOCKS")) : 0;   // 0: no limit
-  const long long blocks = (long long)grid.x * grid.y * grid.z;
-  cfg.numAttrs = (xu_pdl_enabled() && (max_blocks == 0 || blocks <= max_blocks)) ? 1 : 0;
+  cfg.numAttrs = xu_pdl_enabled() ? 1 : 0;
   cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }

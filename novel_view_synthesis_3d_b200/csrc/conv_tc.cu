@@ -36,7 +36,6 @@ struct TcParams {
   int BN, stages;
   int n_tiles, m_tiles, total_tiles;
   int halo;      // 3x3 stride-1: one (TH+2) x TW halo box per (channel chunk, dx) serves the three dy taps
-  int n_fast;    // tile order: 1 = the n-tiles of one m-tile are adjacent (A tile re-read from L2, not HBM); 0 = m fastest
   double* cstats; // fp64 accumulators (xu_det_scratch). EPI 1: per-(sample, channel) [sum, sumsq] of the stored output, (N/2, Co, 2) fp32, accumulated
                  // EPI 2: per-(sample, channel) [sum dyh*xhat, sum dyh] of the GroupNorm backward (same layout)
   const bf16* gx;      // EPI 2: input x of the GroupNorm whose OUTPUT gradient this data-gradient produces, (N,H,W,Co)
@@ -49,10 +48,9 @@ struct TcParams {
   // output through shared memory + TMA store: the epilogue writes the rounded tile into a swizzled [128 pixels][cws channels]
   // staging buffer (conflict-free 16-byte st.shared) and one thread issues cp.async.bulk.tensor stores of whole boxes
   int tma_store, cws;
-  int prefetch;  // pipeline steps by which an L2 prefetch of the activation box runs ahead of its TMA load (0: none)
 };
 
-// Persistent: each CTA walks tiles  blockIdx.x, blockIdx.x + gridDim.x, ...  (tile = m_tile * n_tiles + n_tile) with the
+// Persistent: each CTA walks tiles  blockIdx.x, blockIdx.x + gridDim.x, ...  (tile = n_tile * m_tiles + m_tile) with the
 // smem ring running continuously across tiles.  Warps 0-7 are two consumer warpgroups: warpgroup wg issues the wgmma for
 // rows 64 wg .. 64 wg + 63 of the 128-pixel tile (fp32 accumulators in registers) and then runs the epilogue of those rows;
 // warp 8 is the TMA producer (one elected lane), which runs ahead into the next tile while the consumers drain theirs.
@@ -85,7 +83,10 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
   uint8_t* smA = base;
   uint8_t* smB = base + (size_t)p.stages * A_BYTES;
   uint8_t* smY = smB + (size_t)p.stages * B_BYTES;                       // 2 x [128][cws] bf16 staging (tma_store only)
-  const int Y_BYTES = p.tma_store ? 128 * p.cws * 2 : 0;
+  // a data gradient stages its tile only to accumulate, which the fused GroupNorm-backward epilogues (EPI 2/3) never do:
+  // compiling the staging out of them keeps it from costing them registers
+  const bool tma_store = EPI < 2 && p.tma_store;
+  const int Y_BYTES = tma_store ? 128 * p.cws * 2 : 0;
   float* smT = reinterpret_cast<float*>(smY + 2 * (size_t)Y_BYTES);      // 2 x [64][kXP] fp32 transpose buffers
   uint64_t* full = reinterpret_cast<uint64_t*>(smT + 2 * 64 * kXP);
   uint64_t* empty = full + p.stages;
@@ -98,7 +99,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    if (p.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmY) : "memory");
+    if (tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmY) : "memory");
   }
   __syncthreads();
   xu_grid_dep_sync();     // PDL: everything above (barriers) overlaps the previous kernel's tail
@@ -106,51 +107,17 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
   if (warp == 8) {
     if (lane == 0) {
       // ===== TMA producer =====
-      // activation coordinates of pipeline step `it` of tile `tile` (shared by the load and by the L2 prefetch cursor)
-      auto a_coords = [&](int tile, int it, int& c0, int& cx, int& cy, int& cn) {
-        const int n_tile = p.n_fast ? tile % p.n_tiles : tile / p.m_tiles;
-        int t = p.n_fast ? tile / p.n_tiles : tile - n_tile * p.m_tiles;
-        const int tx = t % p.tiles_x; t /= p.tiles_x;
-        const int ty = t % p.tiles_y; t /= p.tiles_y;
-        const int x0 = tx * p.TW, y0 = ty * p.TH;
-        cn = t * p.TN;
-        const int tt = it / p.KC, c = it - tt * p.KC;
-        if (p.halo) {
-          c0 = c * BK; cx = x0 + (p.flip ? 1 - tt : tt - 1); cy = y0 - 1;
-          return;
-        }
-        int ox = 0, oy = 0;
-        if (p.ks == 3) {
-          const int dy = tt / 3, dx = tt - dy * 3;
-          oy = p.flip ? 1 - dy : dy - p.pad_h;
-          ox = p.flip ? 1 - dx : dx - p.pad_w;
-        }
-        c0 = tt * p.a_seg_stride + c * BK; cx = x0 * p.stride + ox; cy = y0 * p.stride + oy;
-      };
-      int pf_tile = blockIdx.x, pf_it = 0, pf_ahead = 0;     // prefetch cursor: runs p.prefetch steps ahead of the load cursor
       int itg = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        // m fastest: the CTAs running at the same time share one weight slab (n_tile) in L2;  n fastest: they share the
-        // activation tile instead (per-pixel GEMMs: the activations are the big operand and would be re-read from HBM)
-        const int n_tile = p.n_fast ? tile % p.n_tiles : tile / p.m_tiles;
-        int t = p.n_fast ? tile / p.n_tiles : tile - n_tile * p.m_tiles;
+        // m fastest: the CTAs running at the same time share one weight slab (n_tile) in L2
+        const int n_tile = tile / p.m_tiles;
+        int t = tile - n_tile * p.m_tiles;
         const int tx = t % p.tiles_x; t /= p.tiles_x;
         const int ty = t % p.tiles_y; t /= p.tiles_y;
         const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
         for (int it = 0; it < total_k; ++it, ++itg) {
           const int s = itg % p.stages;
           const uint32_t ph = (itg / p.stages) & 1;
-          if (p.prefetch) {
-            // keep the cursor p.prefetch steps ahead (the first iteration issues the whole lead)
-            while (pf_ahead <= p.prefetch && pf_tile < p.total_tiles) {
-              int c0, cx, cy, cn;
-              a_coords(pf_tile, pf_it, c0, cx, cy, cn);
-              tma_prefetch_4d(&tmA, c0, cx, cy, cn);
-              ++pf_ahead;
-              if (++pf_it == total_k) { pf_it = 0; pf_tile += gridDim.x; }
-            }
-            --pf_ahead;
-          }
           mbar_wait(&empty[s], ph ^ 1);
           const int tt = it / p.KC, c = it - tt * p.KC;
           if (p.halo) {
@@ -232,8 +199,8 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
       if (lane == 0) mbar_arrive(&empty[prev_s]);
 
       // ===== epilogue =====
-      const int n_tile = p.n_fast ? tile % p.n_tiles : tile / p.m_tiles;
-      int t = p.n_fast ? tile / p.n_tiles : tile - n_tile * p.m_tiles;
+      const int n_tile = tile / p.m_tiles;
+      int t = tile - n_tile * p.m_tiles;
       const int tx = t % p.tiles_x; t /= p.tiles_x;
       const int ty = t % p.tiles_y; t /= p.tiles_y;
       const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
@@ -270,16 +237,12 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
         named_bar_sync(2 + wg, 128);
         const int c0 = cc + ehalf * 32;
         const bool active = c0 < BN;
-        // the residual / accumulate operands of the whole 32-column chunk are requested before anything waits on them:
-        // each is a 16-byte access of a (pixel-pitch strided) row, i.e. a DRAM-latency load per thread when issued one by one
-        uint4 rv[4], ov[4];
+        // the residual operands of the whole 32-column chunk are requested before anything waits on them: each is a 16-byte
+        // access of a (pixel-pitch strided) row, i.e. a DRAM-latency load per thread when issued one by one
+        uint4 rv[4];
         if (active && EPI < 2 && rrow) {
 #pragma unroll
           for (int q = 0; q < 4; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(rrow + c0 + 8 * q));
-        }
-        if (active && p.accumulate && !p.tma_store) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) ov[q] = *reinterpret_cast<const uint4*>(yrow + c0 + 8 * q);
         }
         if constexpr (EPI >= 2) {      // the GroupNorm input of this pixel (rv is free: a data gradient has no residual operand)
           if (active) {
@@ -308,7 +271,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
         }
         const int ysub = p.cws == 64 ? ehalf : 0;
         uint8_t* yst = smY + (size_t)(ybox & 1) * Y_BYTES + (size_t)r * (p.cws * 2);
-        if (p.tma_store) {
+        if (tma_store) {
           // the store that read this staging buffer two boxes ago must have finished reading before it is overwritten
           if (y_issuer) bulk_wait_group_read<1>();
           named_bar_sync(1, 256);
@@ -381,16 +344,11 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
               *reinterpret_cast<uint4*>(gderow + c0 + j) = dsc;
               *reinterpret_cast<uint4*>(gderow + p.Co + c0 + j) = dsh;
             }
-            if (p.accumulate && !p.tma_store) {
-              const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&ov[j >> 3]);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) { f[2 * q] += __low2float(o2[q]); f[2 * q + 1] += __high2float(o2[q]); }
-            }
             uint4 outv;
             __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&outv);
 #pragma unroll
             for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(f[2 * q], f[2 * q + 1]);
-            if (p.tma_store) sts128(yst + ((((ysub << 2) + (j >> 3)) ^ yswz) << 4), outv);
+            if (tma_store) sts128(yst + ((((ysub << 2) + (j >> 3)) ^ yswz) << 4), outv);
             else *reinterpret_cast<uint4*>(yrow + c0 + j) = outv;
             if constexpr (EPI >= 2) {
               // sums over what is STORED (the second pass reads the rounded dyh back)
@@ -414,7 +372,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
             }
           }
         }
-        if (p.tma_store) {
+        if (tma_store) {
           fence_async_smem();                 // generic-proxy writes -> visible to the TMA unit
           named_bar_sync(1, 256);
           if (y_issuer) {
@@ -429,7 +387,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
       }
     }
   }
-  if (p.tma_store && threadIdx.x == 0) bulk_wait_group<0>();   // all output boxes written before the CTA retires
+  if (tma_store && threadIdx.x == 0) bulk_wait_group<0>();   // all output boxes written before the CTA retires
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -651,11 +609,8 @@ bool conv_tc_stats_supported(int mode, int N, int Ho, int Wo) {
 // wshadow: forward -> wT [wCo][taps][wCi];  dgrad -> wC [seg|tap][wCi][segw]
 // N-split rule: BN is halved while the tile count stays below a threshold, in quarters of the SM count: with a long reduction a
 // narrower tile only pays under 3/4 of a wave (the narrow MMA is bound by fetching A), short reductions are latency-bound and take
-// the full-wave rule.  XUNET_CONV_BN_QUARTERS=n forces one threshold.
-static int bn_rule(int bn, int k_total) {
-  static const char* env = getenv("XUNET_CONV_BN_QUARTERS");
-  return env ? atoi(env) : ((bn > 128 || k_total < 2048) ? 4 : 3);
-}
+// the full-wave rule.
+static int bn_rule(int bn, int k_total) { return (bn > 128 || k_total < 2048) ? 4 : 3; }
 
 static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* cacc, cudaStream_t s) {
   const int taps = a.ks * a.ks;
@@ -664,9 +619,8 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
   if (!pick_tile(a.N, a.Ho, a.Wo, TW, TH, TN)) { xu_set_kernel_error("conv_tc: unsupported spatial shape"); return; }
   // halo mode (see the kernel): 3x3, stride 1, SAME, 8 x 16-pixel tiles inside one image; it reads the input 3.75x per
   // output tile instead of 9x (small-channel convolutions are L2-bandwidth-bound on the tap re-reads) and needs a third
-  // of the pipeline steps.  XUNET_CONV_NO_HALO=1 is the A/B switch.
-  static const bool no_halo = getenv("XUNET_CONV_NO_HALO") != nullptr;
-  bool halo = !no_halo && a.ks == 3 && a.stride == 1 && nseg == 1 && a.pad_h == 1 && a.pad_w == 1 && a.Wo % 16 == 0 && a.Ho % 8 == 0 &&
+  // of the pipeline steps.
+  bool halo = a.ks == 3 && a.stride == 1 && nseg == 1 && a.pad_h == 1 && a.pad_w == 1 && a.Wo % 16 == 0 && a.Ho % 8 == 0 &&
               a.Hi == a.Ho && a.Wi == a.Wo;
   TcParams p;
   p.TW = TW; p.TH = TH; p.TN = TN; p.tiles_x = a.Wo / TW; p.tiles_y = a.Ho / TH;
@@ -688,10 +642,9 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
     while (p.BN >= 64 && (p.BN / 2) % 32 == 0 && mt * (a.Co / p.BN) * 4 < xu_num_sms() * bn_rule(p.BN, taps * Kdim)) p.BN /= 2; }
   // the halo stage (A: 160 pixels, B: 3 taps) must leave room for a >= 3-deep ring; a 32-channel stage keeps the halo trick for the
   // widest tiles, so the activation tile is fetched 3.75x instead of 9x per output tile (wide convolutions are bound by the L2->SM
-  // operand stream).  XUNET_CONV_HALO_BK32=0 restores the 9-tap ring for them.
+  // operand stream).
   if (halo && (size_t)(160 * bk * 2 + 3 * p.BN * bk * 2) > (size_t)56 * 1024) {
-    static const char* e32 = getenv("XUNET_CONV_HALO_BK32");
-    if (bk == 64 && !(e32 && e32[0] == '0') && (size_t)(160 * 32 * 2 + 3 * p.BN * 32 * 2) <= (size_t)72 * 1024) bk = 32;
+    if (bk == 64 && (size_t)(160 * 32 * 2 + 3 * p.BN * 32 * 2) <= (size_t)72 * 1024) bk = 32;
     else halo = false;
   }
   if (a.mode == 0) {
@@ -718,17 +671,13 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
   if (!encode_bf16(&tmA, a.x, 4, ad, as, ab, bk, ae)) return;
   const size_t stage = halo ? (size_t)box_rows * TW * bk * 2 + (size_t)3 * p.BN * bk * 2 : (size_t)128 * bk * 2 + (size_t)p.BN * bk * 2;
   const int total = halo ? 3 * p.KC : p.T * p.KC;
-  // output path: shared-memory staging + TMA stores (XUNET_CONV_TMA_STORE=1 everywhere / 0 nowhere) or 16-byte stores from registers
+  // output path: shared-memory staging + TMA stores, or 16-byte stores from registers.  The per-pixel GEMMs gain from the
+  // staged store, the K-heavy 3x3 convolutions lose the pipeline stage the staging buffer costs -> forward 1x1 only.  An
+  // accumulating launch (the FiLM Dense data gradients summing into the embedding gradient) always stages its tile and adds
+  // it with a TMA reduce-add: the epilogue never reads the destination.
   CUtensorMap tmY = tmA;
   {
-    static const char* env = getenv("XUNET_CONV_TMA_STORE");
-    // the per-pixel GEMMs gain from the staged store, the K-heavy 3x3 convolutions lose the pipeline stage the staging buffer
-    // costs -> default on for forward 1x1 only
-    p.tma_store = (!a.accumulate && ((env && env[0] == '1') || (!env && a.ks == 1 && a.mode == 0))) ? 1 : 0;
-    // accumulating data gradients (the FiLM Dense gradients summing into the embedding gradient): staged tile + TMA reduce-add
-    // instead of a 16-byte read-modify-write per thread (XUNET_CONV_TMA_REDUCE=0 restores it)
-    static const char* envr = getenv("XUNET_CONV_TMA_REDUCE");
-    if (a.accumulate && a.mode == 1 && a.gn_x == nullptr && !(envr && envr[0] == '0') && !(env && env[0] == '0')) p.tma_store = 1;
+    p.tma_store = a.accumulate ? 1 : (a.ks == 1 && a.mode == 0);
     p.cws = p.BN % 64 == 0 ? 64 : 32;
     if (p.tma_store) {
       uint64_t yd[4] = {(uint64_t)a.Co, (uint64_t)a.Wo, (uint64_t)a.Ho, (uint64_t)a.N};
@@ -738,25 +687,9 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
     }
   }
   const size_t ystage = p.tma_store ? (size_t)2 * 128 * p.cws * 2 : 0;
-  {
-    // optional L2 prefetch of the activation boxes ahead of the ring (XUNET_TMA_PREFETCH=n steps; off by default)
-    static const char* env = getenv("XUNET_TMA_PREFETCH");
-    p.prefetch = env ? atoi(env) : 0;
-  }
   p.n_tiles = a.Co / p.BN;
   p.m_tiles = p.tiles_x * p.tiles_y * (a.N / TN);
   p.total_tiles = p.m_tiles * p.n_tiles;
-  {
-    // with several n-tiles the activation tensor is read once per n-tile: keep those reads adjacent in time (L2 hits) when
-    // the activations are the larger operand (XUNET_CONV_TILE_ORDER=m|n forces one order)
-    static const char* ord = getenv("XUNET_CONV_TILE_ORDER");
-    const double act_bytes = (double)a.N * a.Hi * a.Wi * a.Ci * 2.0, w_bytes = (double)taps * a.wCi * a.wCo * 2.0;
-    // default m-fastest (the CTAs in flight share one weight slab); the switch selects the other order
-    (void)act_bytes; (void)w_bytes;
-    p.n_fast = 0;
-    if (ord && ord[0] == 'm') p.n_fast = 0;
-    if (ord && ord[0] == 'n') p.n_fast = p.n_tiles > 1 ? 1 : 0;
-  }
   // CTAs per SM: two where the kernel is compiled for it (conv_ctas_per_sm) and shared
   // memory keeps a >= 3-deep TMA ring for each; one persistent CTA per SM with a 4-deep ring otherwise
   const size_t fixed = ystage + (size_t)2 * 64 * kXP * 4 + 1024 + 256;
@@ -772,11 +705,6 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
   p.stages = stages;
   const size_t smem = stage * stages + fixed + 8 * 2 * stages;
   int ctas = xu_num_sms() * per_sm;
-  {
-    static int cap = -1;   // experiment knob: XUNET_CONV_CTAS_PER_SM limits the persistent grid (more tiles per CTA)
-    if (cap < 0) { const char* e = getenv("XUNET_CONV_CTAS_PER_SM"); cap = e ? atoi(e) : 0; }
-    if (cap > 0 && cap < per_sm) ctas = xu_num_sms() * cap;
-  }
   if (ctas > p.total_tiles) ctas = p.total_tiles;
   dim3 grid((unsigned)ctas);
   {

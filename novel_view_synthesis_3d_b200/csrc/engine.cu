@@ -177,10 +177,6 @@ struct Builder {
   xunet_handle& H;
   explicit Builder(xunet_handle& h) : H(h) {}
   int res_counter = 0;
-  static bool use_tc() {
-    const char* e = getenv("XUNET_DISABLE_TC");
-    return !(e && e[0] == '1');
-  }
 
   int conv(int x, int cout, int ks, int stride, long long w, long long b, int res, float alpha, int nseg,
            const std::string& tap = "") {
@@ -191,14 +187,14 @@ struct Builder {
     Op o;
     o.kind = OP_CONV; o.x = x; o.y = y; o.r = res; o.ks = ks; o.stride = stride; o.pad_h = pl_h; o.pad_w = pl_w;
     o.w = w; o.b = b; o.alpha = alpha; o.nseg = nseg;
-    if (use_tc() && conv_tc_supported(H.dtype, 0, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) {
+    if (conv_tc_supported(H.dtype, 0, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) {
       o.impl = 1;
       o.wT = H.alloc((long long)ks * ks * tx.c * cout * 2);
     }
     if (tx.c == 3 && ks == 3 && stride == 1 && cout % 8 == 0 && res < 0 && nseg == 1) o.impl = o.impl_w = 2;      // direct Cin=3 kernels
     if (conv_cout3_supported(tx.c, cout, ks, stride) && res < 0 && nseg == 1) o.impl = o.impl_d = o.impl_w = 3;     // direct Cout=3 kernels
-    if (use_tc() && H.training && wgrad_tc_supported(H.dtype, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) o.impl_w = 1;
-    if (use_tc() && H.training && H.tensors[x].need_grad && conv_tc_supported(H.dtype, 1, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) {
+    if (H.training && wgrad_tc_supported(H.dtype, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) o.impl_w = 1;
+    if (H.training && H.tensors[x].need_grad && conv_tc_supported(H.dtype, 1, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) {
       o.impl_d = 1;
       o.wC = H.alloc((long long)ks * ks * tx.c * cout * 2);
     }
@@ -214,10 +210,10 @@ struct Builder {
     Op o;
     o.kind = OP_GN; o.x = x; o.y = y; o.e = e; o.mode = mode; o.rs = rs; o.w = gamma; o.b = beta; o.op_index = op_index;
     o.stats = -1; o.bstats = -1;   // assigned at the end of build(): one contiguous region -> ONE memset per pass
-    // statistics come from whoever produced x (both halves of a concat): no statistics pass over HBM
-    const bool separate = getenv("XUNET_GN_SEPARATE_STATS") != nullptr;     // A/B switch (read per xunet_create): the gn_stats kernel per norm
+    // statistics come from whoever produced x (both halves of a concat): no statistics pass over HBM.  build() checks that
+    // every norm found its producers.
     const int sa = tx.cat_a >= 0 ? tx.cat_a : x, sb = tx.cat_a >= 0 ? tx.cat_b : -1;
-    if (!separate && H.tensors[sa].producer >= 0 && (sb < 0 || H.tensors[sb].producer >= 0) && H.tensors[sa].cat_a < 0 &&
+    if (H.tensors[sa].producer >= 0 && (sb < 0 || H.tensors[sb].producer >= 0) && H.tensors[sa].cat_a < 0 &&
         (sb < 0 || H.tensors[sb].cat_a < 0)) {
       o.cs_a = sa; o.cs_b = sb;
       H.tensors[sa].cstats = 0;                      // marked; offsets assigned at the end of build()
@@ -298,7 +294,7 @@ struct Builder {
     int y = H.tensor(t.n, t.h, t.w, C, true, tap);
     Op o;
     o.kind = OP_ATTN; o.x = qkv; o.y = y; o.r = h_in; o.cross = cross; o.heads = heads;
-    o.impl = (use_tc() && attn_tc_supported(H.dtype, t.h * t.w, C, heads)) ? 1 : 0;
+    o.impl = attn_tc_supported(H.dtype, t.h * t.w, C, heads) ? 1 : 0;
     o.lse = H.alloc(sizeof(float) * t.n * heads * t.h * t.w);
     o.dscr = H.training ? H.alloc(sizeof(float) * t.n * heads * t.h * t.w) : -1;   // D [N,heads,L]
     H.ops.push_back(o);
@@ -477,14 +473,11 @@ struct Builder {
         }
       }
     }
-    // ---- fused GroupNorm backward (XUNET_GN_BWD_FUSED=0 restores the two-kernel backward everywhere): a norm without
-    // resampling, plain or +swish, whose output feeds exactly one tensor-core conv -> that conv's data-gradient epilogue emits
-    // dyh and the channel sums; the norm's backward is then ONE elementwise kernel
+    // ---- fused GroupNorm backward: a norm without resampling, plain or +swish, whose output feeds exactly one tensor-core conv
+    // -> that conv's data-gradient epilogue emits dyh and the channel sums; the norm's backward is then ONE elementwise kernel
     if (H.training) {
-      const char* env = getenv("XUNET_GN_BWD_FUSED");      // read per xunet_create, so one process can build both plans
-      const bool on = !(env && env[0] == '0');
       H.bcs_bytes = 0;
-      for (size_t g = 0; on && g < H.ops.size(); ++g) {
+      for (size_t g = 0; g < H.ops.size(); ++g) {
         Op& gn = H.ops[g];
         if (gn.kind != OP_GN || gn.rs != RS_NONE) continue;
         int consumer = -1, users = 0;
@@ -496,10 +489,6 @@ struct Builder {
         Op& cv = H.ops[consumer];
         const Tensor& tx = H.tensors[gn.x];
         if (cv.impl_d != 1 || cv.stride != 1 || !conv_tc_stats_supported(1, tx.n, tx.h, tx.w) || !H.tensors[gn.y].need_grad) continue;
-        // the fused epilogue is free only while it hides under the data gradient's main loop (reduction = taps x conv output channels):
-        // XUNET_GN_BWD_FUSED_MIN_K=k keeps the two-kernel backward for narrower reductions
-        { const char* mk = getenv("XUNET_GN_BWD_FUSED_MIN_K");
-          if (mk && cv.ks * cv.ks * H.tensors[cv.y].c < atoi(mk)) continue; }
         gn.gnb = consumer; cv.gnb = (int)g;
         gn.gnp = H.alloc(sizeof(float) * 4 * (long long)H.B * tx.c);
         gn.bcs = H.bcs_bytes;
@@ -508,8 +497,8 @@ struct Builder {
       H.a_bcs = H.alloc(H.bcs_bytes);
       for (Op& o : H.ops) if (o.kind == OP_GN && o.gnb >= 0) o.bcs += H.a_bcs;
     }
-    // ---- residual operands whose gradient is just alpha * grad(y): alias instead of a scale_add pass (XUNET_NO_GRAD_ALIAS=1: off)
-    if (H.training && getenv("XUNET_NO_GRAD_ALIAS") == nullptr) {
+    // ---- residual operands whose gradient is just alpha * grad(y): alias instead of a scale_add pass
+    if (H.training) {
       for (Op& o : H.ops) {
         if (o.kind != OP_CONV || o.r < 0 || o.fuse_res || !H.tensors[o.r].need_grad) continue;
         Tensor& tr = H.tensors[o.r];
@@ -554,6 +543,8 @@ struct Builder {
         if (cv.acc_x != 0 || (gn.mode == GN_FILM && gn.acc_e != 0)) { cv.gnb = -1; gn.gnb = -1; }
       }
     }
+    for (const Op& o : H.ops)
+      if (o.kind == OP_GN && o.cs_a < 0) return fail("internal: a GroupNorm input has no producer-emitted statistics");
     return 0;
   }
 };
@@ -739,11 +730,9 @@ static int forward_impl(Ctx& c, float* eps_out) {
       case OP_GN: {
         if (o.film_idx >= 0 && side != nullptr) cudaStreamWaitEvent(c.s, h->ev_film[o.film_idx], 0);
         GnArgs a = gn_args(c, o);
-        if (o.cs_a >= 0) {
-          a.cstatsA = reinterpret_cast<const float*>(c.ws + h->tensors[o.cs_a].cstats);
-          a.csA = h->tensors[o.cs_a].c;
-          a.cstatsB = o.cs_b >= 0 ? reinterpret_cast<const float*>(c.ws + h->tensors[o.cs_b].cstats) : nullptr;
-        } else launch_gn_stats(dt, a, c.s);
+        a.cstatsA = reinterpret_cast<const float*>(c.ws + h->tensors[o.cs_a].cstats);
+        a.csA = h->tensors[o.cs_a].c;
+        a.cstatsB = o.cs_b >= 0 ? reinterpret_cast<const float*>(c.ws + h->tensors[o.cs_b].cstats) : nullptr;
         if (o.gnb >= 0 && h->training) a.params_out = reinterpret_cast<float*>(c.ws + o.gnp);
         launch_gn_apply(dt, a, c.s);
         break;

@@ -63,8 +63,8 @@ struct GnArgs {
   float* dgamma; float* dbeta;   // backward (atomic accumulate)
   float* stats;       // (B,32,2) sum, sumsq of x         (forward writes, backward reads)
   // producer-emitted statistics (forward apply only): channels [0, csA) of x come with per-channel sums cstatsA (B, csA, 2),
-  // channels [csA, C) with cstatsB (B, C - csA, 2) (a channel concat of two producers); cstatsA == NULL: `stats` was filled
-  // by launch_gn_stats.  With cstats the apply kernel reduces them to group sums itself and stores them to `stats`.
+  // channels [csA, C) with cstatsB (B, C - csA, 2) (a channel concat of two producers).  The apply kernel reduces them to
+  // group sums itself and stores them to `stats`.
   const float* cstatsA; const float* cstatsB; int csA;
   float* params_out;   // forward apply, optional: (B, C) float4 {rstd, -mean*rstd, gamma, beta} for the fused backward epilogue
   const float* bcs;    // launch_gn_bwd_apply_pre: per-(sample, channel) [sum dyh*xhat, sum dyh] emitted by that epilogue
@@ -78,10 +78,10 @@ struct GnArgs {
   float extra_alpha;
   int skip_zero;      // stats / bstats were already zeroed by the caller (one memset for the whole plan)
 };
-void launch_gn_stats(int dtype, const GnArgs& a, cudaStream_t s);        // zeroes + fills a.stats
 // per-(sample, channel) [sum, sumsq] of x (N,H,W,C) accumulated into cstats (N/2, C, 2): the stand-alone producer of the
 // statistics a conv / attention epilogue emits for free (used after kernels that cannot: 3-channel input conv, SIMT paths)
 void launch_gn_cstats(int dtype, const void* x, float* cstats, int N, int H, int W, int C, cudaStream_t s);
+// rs == RS_NONE: any mode; a resampling norm is GN_PLAIN or GN_SWISH, without params_out
 void launch_gn_apply(int dtype, const GnArgs& a, cudaStream_t s);
 void launch_gn_bwd_reduce(int dtype, const GnArgs& a, cudaStream_t s);   // zeroes + fills a.bstats, dgamma/dbeta, de
 void launch_gn_bwd_apply(int dtype, const GnArgs& a, cudaStream_t s);

@@ -843,10 +843,6 @@ __global__ void __launch_bounds__(256) wgrad_thin_kernel(WgradArgs a) {
   }
 }
 
-static bool thin_new_enabled() {
-  static const char* env = getenv("XUNET_CONV3_OLD");
-  return !(env && env[0] == '1');
-}
 static bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
 bool conv_cin3_supported(const ConvArgs& a) { return a.mode == 0 && a.Ci == 3 && a.ks == 3 && a.stride == 1 && a.Co % 8 == 0 && a.segw == a.Co && a.res == nullptr && !a.accumulate && 28 * a.Co * 4 <= 96 * 1024; }
@@ -854,47 +850,45 @@ bool conv_cout3_supported(int Ci, int Co, int ks, int stride) { return Co == 3 &
 
 template <typename T>
 static void small_dispatch(int which, const ConvArgs* c, const WgradArgs* w, cudaStream_t s) {
-  // round-2 kernels where their shape rules hold (XUNET_CONV3_OLD=1 forces the round-1 kernels for A/B)
-  if (thin_new_enabled()) {
-    if ((which == 0 || which == 3) && c->Wo % 4 == 0 && c->Co % 8 == 0 && c->Hi == c->Ho && c->Wi == c->Wo) {
-      const long long total = (long long)c->N * c->Ho * (c->Wo / 4) * (c->Co / 8);
-      const size_t sm = sizeof(float) * 28 * c->Co;
-      const int grid = (int)std::min<long long>(cdiv(total, 256), (long long)xu_num_sms() * 4);
-      if (which == 0) {
-        if (sm > 48 * 1024) cudaFuncSetAttribute(conv_thin_in_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        xu_launch(conv_thin_in_kernel<T, 0>, grid, 256, sm, s, *c);
+  // round-2 kernels where their shape rules hold, the round-1 kernels below for every other shape
+  if ((which == 0 || which == 3) && c->Wo % 4 == 0 && c->Co % 8 == 0 && c->Hi == c->Ho && c->Wi == c->Wo) {
+    const long long total = (long long)c->N * c->Ho * (c->Wo / 4) * (c->Co / 8);
+    const size_t sm = sizeof(float) * 28 * c->Co;
+    const int grid = (int)std::min<long long>(cdiv(total, 256), (long long)xu_num_sms() * 4);
+    if (which == 0) {
+      if (sm > 48 * 1024) cudaFuncSetAttribute(conv_thin_in_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+      xu_launch(conv_thin_in_kernel<T, 0>, grid, 256, sm, s, *c);
+    } else {
+      if (sm > 48 * 1024) cudaFuncSetAttribute(conv_thin_in_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+      xu_launch(conv_thin_in_kernel<T, 1>, grid, 256, sm, s, *c);
+    }
+    return;
+  }
+  if (which == 2 && c->Wo % 4 == 0 && is_pow2(c->Ci / 8) && c->Ci / 8 <= 32 && c->Hi == c->Ho && c->Wi == c->Wo) {
+    const long long quads = (long long)c->N * c->Ho * (c->Wo / 4);
+    const int qpb = 256 / (c->Ci / 8);
+    const size_t sm = sizeof(float) * 27 * c->Ci;
+    const int grid = (int)std::min<long long>(cdiv(quads, qpb), (long long)xu_num_sms() * 4);
+    if (sm > 48 * 1024) cudaFuncSetAttribute(conv_cout3_fwd4_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    xu_launch(conv_cout3_fwd4_kernel<T>, grid, 256, sm, s, *c);
+    return;
+  }
+  if (which == 1 || which == 4) {
+    const int Cw = which == 4 ? w->Ci : w->Co;
+    const int SEG = w->Wo < 32 ? w->Wo : 32;
+    if (is_pow2(Cw) && Cw >= 2 && Cw <= 512 && w->Wo % SEG == 0 && w->Hi == w->Ho && w->Wi == w->Wo) {
+      const int nstream = 256 / (Cw / 2);
+      const long long units = (long long)w->N * w->Ho * (w->Wo / SEG);
+      const int grid = (int)std::min<long long>(cdiv(units, nstream), (long long)xu_num_sms() * 2);
+      const size_t sm = sizeof(float) * 256 * 56;
+      if (which == 1) {
+        cudaFuncSetAttribute(wgrad_thin_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+        xu_launch(wgrad_thin_kernel<T, 0>, grid, 256, sm, s, *w);
       } else {
-        if (sm > 48 * 1024) cudaFuncSetAttribute(conv_thin_in_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        xu_launch(conv_thin_in_kernel<T, 1>, grid, 256, sm, s, *c);
+        cudaFuncSetAttribute(wgrad_thin_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+        xu_launch(wgrad_thin_kernel<T, 1>, grid, 256, sm, s, *w);
       }
       return;
-    }
-    if (which == 2 && c->Wo % 4 == 0 && is_pow2(c->Ci / 8) && c->Ci / 8 <= 32 && c->Hi == c->Ho && c->Wi == c->Wo) {
-      const long long quads = (long long)c->N * c->Ho * (c->Wo / 4);
-      const int qpb = 256 / (c->Ci / 8);
-      const size_t sm = sizeof(float) * 27 * c->Ci;
-      const int grid = (int)std::min<long long>(cdiv(quads, qpb), (long long)xu_num_sms() * 4);
-      if (sm > 48 * 1024) cudaFuncSetAttribute(conv_cout3_fwd4_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-      xu_launch(conv_cout3_fwd4_kernel<T>, grid, 256, sm, s, *c);
-      return;
-    }
-    if (which == 1 || which == 4) {
-      const int Cw = which == 4 ? w->Ci : w->Co;
-      const int SEG = w->Wo < 32 ? w->Wo : 32;
-      if (is_pow2(Cw) && Cw >= 2 && Cw <= 512 && w->Wo % SEG == 0 && w->Hi == w->Ho && w->Wi == w->Wo) {
-        const int nstream = 256 / (Cw / 2);
-        const long long units = (long long)w->N * w->Ho * (w->Wo / SEG);
-        const int grid = (int)std::min<long long>(cdiv(units, nstream), (long long)xu_num_sms() * 2);
-        const size_t sm = sizeof(float) * 256 * 56;
-        if (which == 1) {
-          cudaFuncSetAttribute(wgrad_thin_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-          xu_launch(wgrad_thin_kernel<T, 0>, grid, 256, sm, s, *w);
-        } else {
-          cudaFuncSetAttribute(wgrad_thin_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-          xu_launch(wgrad_thin_kernel<T, 1>, grid, 256, sm, s, *w);
-        }
-        return;
-      }
     }
   }
   if (which == 0) {

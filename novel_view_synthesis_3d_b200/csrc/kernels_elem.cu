@@ -120,76 +120,18 @@ __device__ __forceinline__ bool fold_same_channel_lanes(float (&v)[4], int TPB) 
 // ======================================================================================================
 // GroupNorm  (model/xunet.py:46-52: nn.GroupNorm(32) on (B,2,H,W,C) -> statistics over F,H,W,C/32 jointly)
 // ======================================================================================================
-template <typename T>
-__global__ void __launch_bounds__(256) gn_stats_kernel(const T* __restrict__ x, double* __restrict__ stats, int P, int C,
-                                                       int ppb) {
-  xu_grid_dep_sync();
-  __shared__ double sg[XU_GROUPS], sq[XU_GROUPS];
-  const int tid = threadIdx.x, b = blockIdx.y;
-  if (tid < XU_GROUPS) { sg[tid] = 0.0; sq[tid] = 0.0; }
-  __syncthreads();
-  const int C4 = C >> 2, cpg = C / XU_GROUPS;
-  const int TPB = C4 < 256 ? C4 : 256;
-  const int PL = 256 / TPB;
-  const int cv0 = tid % TPB, pl = tid / TPB;
-  const int pbeg = blockIdx.x * ppb;
-  const int pend = min(pbeg + ppb, P);
-  {
-    for (int cv = cv0; cv < C4; cv += TPB) {
-      float s[4] = {0.f, 0.f, 0.f, 0.f}, ss[4] = {0.f, 0.f, 0.f, 0.f};
-      const T* base = x + ((long long)b * P) * C + cv * 4;
-      if (pl < PL)
-#pragma unroll 4
-        for (int p = pbeg + pl; p < pend; p += PL) {
-          float v[4];
-          Vec4<T>::ldg(base + (long long)p * C, v);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) { s[j] += v[j]; ss[j] = fmaf(v[j], v[j], ss[j]); }
-        }
-      const bool owner = fold_same_channel_lanes(s, TPB);
-      fold_same_channel_lanes(ss, TPB);
-      if (owner && pl < PL) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          int g = (cv * 4 + j) / cpg;
-          xu_det_add(&sg[g], s[j]);
-          xu_det_add(&sq[g], ss[j]);
-        }
-      }
-    }
-  }
-  __syncthreads();
-  if (tid < XU_GROUPS) {
-    atomicAdd(&stats[(b * XU_GROUPS + tid) * 2 + 0], sg[tid]);
-    atomicAdd(&stats[(b * XU_GROUPS + tid) * 2 + 1], sq[tid]);
-  }
-}
-
 static void gn_grid(int C, int P, int B, dim3& grid, int& ppb) {
   int C4 = C / 4;
   int TPB = C4 < 256 ? C4 : 256;
   int PL = 256 / TPB;
-  static const int px = getenv("XUNET_GN_RED_PX") ? atoi(getenv("XUNET_GN_RED_PX")) : 8;
-  ppb = PL * px;
+  ppb = PL * 8;
   // enough blocks to cover the memory latency (reductions are latency-bound), but not absurdly many atomics
   while ((long long)cdiv(P, ppb) * B > xu_num_sms() * 8 && ppb < P) ppb *= 2;
   grid = dim3(cdiv(P, ppb), B);
 }
 
-void launch_gn_stats(int dtype, const GnArgs& a, cudaStream_t s) {
-  const int B = a.N / 2, P = 2 * a.H * a.W;
-  if (!a.skip_zero) cudaMemsetAsync(a.stats, 0, sizeof(float) * B * XU_GROUPS * 2, s);
-  dim3 grid; int ppb;
-  gn_grid(a.C, P, B, grid, ppb);
-  double* acc = xu_det_scratch(s, (long long)B * XU_GROUPS * 2);
-  if (acc == nullptr) return;
-  if (dtype == XU_F32) xu_launch(gn_stats_kernel<float>, grid, 256, 0, s, (const float*)a.x, acc, P, a.C, ppb);
-  else xu_launch(gn_stats_kernel<bf16>, grid, 256, 0, s, (const bf16*)a.x, acc, P, a.C, ppb);
-  xu_det_fold(a.stats, acc, (long long)B * XU_GROUPS * 2, s);
-}
-
-// Per-(sample, channel) statistics for tensors whose producer cannot emit them in its epilogue: same traversal as
-// gn_stats_kernel, channel sums kept in shared memory, one interleaved [sum, sumsq] red per channel and block.
+// Per-(sample, channel) statistics for tensors whose producer cannot emit them in its epilogue: channel sums kept in shared
+// memory, one interleaved [sum, sumsq] red per channel and block.
 template <typename T>
 __global__ void __launch_bounds__(256) gn_cstats_kernel(const T* __restrict__ x, double* __restrict__ cstats, int P, int C,
                                                         int ppb) {
@@ -299,6 +241,37 @@ __device__ __forceinline__ void gn_yhat4(const GnDev& d, int n, int y, int x, in
   }
 }
 
+// group sums of sample b into s_grp: the producers of x emitted per-channel sums, folded here into the 32 group sums (8 lanes
+// per group) -- there is no statistics pass over x.  Block 0 of each sample also stores the group sums where the backward
+// kernels read them.
+template <typename T>
+__device__ __forceinline__ void gn_group_prologue(const GnDev& d, int b, float (*s_grp)[2]) {
+  const int tid = threadIdx.x;
+  const int g = tid >> 3, sub = tid & 7;
+  float s = 0.f, q = 0.f;
+  for (int k = sub; k < d.cpg; k += 8) {
+    const int c = g * d.cpg + k;
+    const float* src = c < d.csA ? d.cstatsA + ((long long)b * d.csA + c) * 2
+                                 : d.cstatsB + ((long long)b * (d.C - d.csA) + (c - d.csA)) * 2;
+    const float2 v = *reinterpret_cast<const float2*>(src);
+    s += v.x; q += v.y;
+  }
+#pragma unroll
+  for (int o = 4; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
+  if (sub == 0) {
+    s_grp[g][0] = s; s_grp[g][1] = q;
+    if (blockIdx.x == 0) { d.stats[(b * XU_GROUPS + g) * 2 + 0] = s; d.stats[(b * XU_GROUPS + g) * 2 + 1] = q; }
+  }
+  __syncthreads();
+}
+__device__ __forceinline__ void gn_group_mean_rstd(const GnDev& d, const float (*s_grp)[2], int c, float& mean, float& rstd) {
+  const int g = gn_group(d, c);
+  mean = s_grp[g][0] * d.inv_cnt;
+  rstd = rsqrtf(fmaxf(s_grp[g][1] * d.inv_cnt - mean * mean, 0.f) + XU_GN_EPS);
+}
+
+// GroupNorm (+ swish) with resampling: RS_DOWN averages 2x2 pixels of the activation, RS_UP repeats each pixel 2x2 (the
+// first norm of a ResnetBlock that resamples).
 // grid (pixel chunks of the OUTPUT, B): every thread owns a fixed 4-channel vector, so the per-channel constants
 // (mean, rstd, gamma, beta) are formed once and the inner loop is load -> fma -> activation -> store.
 template <typename T>
@@ -306,39 +279,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(GnDev d, int ppb) {
   xu_grid_dep_sync();
   const int tid = threadIdx.x, b = blockIdx.y;
   __shared__ float s_grp[XU_GROUPS][2];
-  if (d.cstatsA != nullptr) {
-    // the producers of x emitted per-channel sums: fold them into the 32 group sums here (8 lanes per group) -- there is no
-    // statistics pass over x.  Block 0 of each sample also stores the group sums where the backward kernels read them.
-    const int g = tid >> 3, sub = tid & 7;
-    float s = 0.f, q = 0.f;
-    for (int k = sub; k < d.cpg; k += 8) {
-      const int c = g * d.cpg + k;
-      const float* src = c < d.csA ? d.cstatsA + ((long long)b * d.csA + c) * 2
-                                   : d.cstatsB + ((long long)b * (d.C - d.csA) + (c - d.csA)) * 2;
-      const float2 v = *reinterpret_cast<const float2*>(src);
-      s += v.x; q += v.y;
-    }
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
-    if (sub == 0) {
-      s_grp[g][0] = s; s_grp[g][1] = q;
-      if (blockIdx.x == 0) { d.stats[(b * XU_GROUPS + g) * 2 + 0] = s; d.stats[(b * XU_GROUPS + g) * 2 + 1] = q; }
-    }
-    __syncthreads();
-  }
-  if (d.params_out != nullptr && blockIdx.x == 0) {
-    // per-(sample, channel) {rstd, -mean*rstd, gamma, beta}: what the fused GroupNorm-backward epilogue of the consumer conv's
-    // data gradient needs to rebuild xhat and the pre-activation from x (one 16-byte load per channel there)
-    for (int c = tid; c < d.C; c += 256) {
-      float mean, rstd;
-      if (d.cstatsA != nullptr) {
-        const int g = gn_group(d, c);
-        mean = s_grp[g][0] * d.inv_cnt;
-        rstd = rsqrtf(fmaxf(s_grp[g][1] * d.inv_cnt - mean * mean, 0.f) + XU_GN_EPS);
-      } else gn_mean_rstd(d, b, c, mean, rstd);
-      d.params_out[(long long)b * d.C + c] = make_float4(rstd, -mean * rstd, d.gamma[c], d.beta[c]);
-    }
-  }
+  gn_group_prologue<T>(d, b, s_grp);
   const int C4 = d.C >> 2;
   const int TPB = C4 < 256 ? C4 : 256;
   const int PL = 256 / TPB;
@@ -347,47 +288,22 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(GnDev d, int ppb) {
   const int HWo = d.Ho * d.Wo, P = 2 * HWo;
   const int pbeg = blockIdx.x * ppb;
   const int pend = min(pbeg + ppb, P);
-  const bool drop = d.mode == GN_FILM && d.train && d.drop_rate > 0.f;
-  const unsigned long long seed = drop ? *d.seed_dev : 0ULL;
-  const float keep_scale = 1.f / (1.f - d.drop_rate);
   for (int cv = cv0; cv < C4; cv += TPB) {
     const int c0 = cv * 4;
     float mean[4], rstd[4], gm[4], bt[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      if (d.cstatsA != nullptr) {
-        const int g = gn_group(d, c0 + j);
-        mean[j] = s_grp[g][0] * d.inv_cnt;
-        rstd[j] = rsqrtf(fmaxf(s_grp[g][1] * d.inv_cnt - mean[j] * mean[j], 0.f) + XU_GN_EPS);
-      } else gn_mean_rstd(d, b, c0 + j, mean[j], rstd[j]);
+      gn_group_mean_rstd(d, s_grp, c0 + j, mean[j], rstd[j]);
       gm[j] = d.gamma[c0 + j];
       bt[j] = d.beta[c0 + j];
     }
 #pragma unroll 2
     for (int p = pbeg + pl; p < pend; p += PL) {
-      // without resampling the pixel index alone addresses everything ((2b)*HW + p): no div/mod in the hot loop
-      int n = 2 * b, oy = 0, ox = p;
-      if (d.rs != RS_NONE) {
-        const int f = p / HWo, r = p - f * HWo;
-        oy = r / d.Wo; ox = r - oy * d.Wo; n = b * 2 + f;
-      }
+      const int f = p / HWo, r = p - f * HWo;
+      const int oy = r / d.Wo, ox = r - oy * d.Wo, n = b * 2 + f;
       const long long pix = (long long)(2 * b) * HWo + p;
       float out[4], yh[4], xh[4];
-      if (d.mode == GN_FILM) {
-        gn_yhat4<T>(d, n, oy, ox, c0, mean, rstd, gm, bt, yh, xh);
-        const T* e = reinterpret_cast<const T*>(d.e) + pix * (2LL * d.C);
-        float sc[4], sh[4];
-        Vec4<T>::ldg(e + c0, sc);
-        Vec4<T>::ldg(e + d.C + c0, sh);
-        const uint32_t km = drop ? xu_keep4(seed, d.op_index, (unsigned long long)(pix * d.C + c0) >> 2, d.drop_rate) : 0xFu;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float u = fmaf(yh[j], 1.f + sc[j], sh[j]);
-          float sv = swishf_(u);
-          if (drop) sv = ((km >> j) & 1u) ? sv * keep_scale : 0.f;
-          out[j] = sv;
-        }
-      } else if (d.rs == RS_DOWN) {
+      if (d.rs == RS_DOWN) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) out[j] = 0.f;
         for (int i = 0; i < 2; ++i)
@@ -399,8 +315,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(GnDev d, int ppb) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) out[j] *= 0.25f;
       } else {
-        const int iy = d.rs == RS_UP ? oy >> 1 : oy, ix = d.rs == RS_UP ? ox >> 1 : ox;
-        gn_yhat4<T>(d, n, iy, ix, c0, mean, rstd, gm, bt, yh, xh);
+        gn_yhat4<T>(d, n, oy >> 1, ox >> 1, c0, mean, rstd, gm, bt, yh, xh);
 #pragma unroll
         for (int j = 0; j < 4; ++j) out[j] = (d.mode == GN_SWISH) ? swishf_(yh[j]) : yh[j];
       }
@@ -414,46 +329,14 @@ static void gn_apply_grid(int C, int P, int B, dim3& grid, int& ppb) {
   int C4 = C / 4;
   int TPB = C4 < 256 ? C4 : 256;
   int PL = 256 / TPB;
-  static const int px = getenv("XUNET_GN_APPLY_PX") ? atoi(getenv("XUNET_GN_APPLY_PX")) : 4;   // measured: 4 beats 8 and 2 (latency-bound: more blocks in flight)
   ppb = PL * 16;   // the per-thread prologue (statistics -> scale/shift) is ~200 instructions: amortise it over >= 8 pixels
-  while (ppb > PL * px && (long long)cdiv(P, ppb) * B < xu_num_sms() * 2 * (8 / px)) ppb /= 2;
+  // down to 4 pixels per thread (measured: 4 beats 8 and 2; latency-bound: more blocks in flight)
+  while (ppb > PL * 4 && (long long)cdiv(P, ppb) * B < xu_num_sms() * 4) ppb /= 2;
   grid = dim3(cdiv(P, ppb), B);
 }
 
-
 // ---- no-resample fast paths: 16-byte accesses for both dtypes (8 bf16 / 4 fp32 channels per thread), U pixels of loads in
 // flight per thread before the first use, per-channel affine folded to one fma: yhat = x * a + b -----------------------------
-template <typename T>
-__device__ __forceinline__ void gn_group_prologue(const GnDev& d, int b, float (*s_grp)[2]) {
-  const int tid = threadIdx.x;
-  if (d.cstatsA != nullptr) {
-    const int g = tid >> 3, sub = tid & 7;
-    float s = 0.f, q = 0.f;
-    for (int k = sub; k < d.cpg; k += 8) {
-      const int c = g * d.cpg + k;
-      const float* src = c < d.csA ? d.cstatsA + ((long long)b * d.csA + c) * 2
-                                   : d.cstatsB + ((long long)b * (d.C - d.csA) + (c - d.csA)) * 2;
-      const float2 v = *reinterpret_cast<const float2*>(src);
-      s += v.x; q += v.y;
-    }
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
-    if (sub == 0) {
-      s_grp[g][0] = s; s_grp[g][1] = q;
-      if (blockIdx.x == 0) { d.stats[(b * XU_GROUPS + g) * 2 + 0] = s; d.stats[(b * XU_GROUPS + g) * 2 + 1] = q; }
-    }
-  } else if (tid < XU_GROUPS) {
-    s_grp[tid][0] = d.stats[(b * XU_GROUPS + tid) * 2 + 0];
-    s_grp[tid][1] = d.stats[(b * XU_GROUPS + tid) * 2 + 1];
-  }
-  __syncthreads();
-}
-__device__ __forceinline__ void gn_group_mean_rstd(const GnDev& d, const float (*s_grp)[2], int c, float& mean, float& rstd) {
-  const int g = gn_group(d, c);
-  mean = s_grp[g][0] * d.inv_cnt;
-  rstd = rsqrtf(fmaxf(s_grp[g][1] * d.inv_cnt - mean * mean, 0.f) + XU_GN_EPS);
-}
-
 template <typename T, bool FILM>
 __global__ void __launch_bounds__(256, FILM ? 2 : 3) gn_apply_vec_kernel(GnDev d, int ppb) {
   xu_grid_dep_sync();
@@ -558,8 +441,7 @@ static void gn_vec_grid(int C, int VW, int P, int B, dim3& grid, int& ppb) {
 void launch_gn_apply(int dtype, const GnArgs& a, cudaStream_t s) {
   GnDev d = gn_dev(a);
   dim3 grid; int ppb;
-  static const bool old_path = getenv("XUNET_GN_APPLY_OLD") != nullptr;     // A/B switch: the 8-byte-access kernel
-  if (a.rs == RS_NONE && !old_path && d.C % 8 == 0) {
+  if (a.rs == RS_NONE) {
     const bool film = a.mode == GN_FILM;
     if (dtype == XU_F32) {
       gn_vec_grid(d.C, 4, 2 * d.H * d.W, d.N / 2, grid, ppb);
@@ -570,6 +452,10 @@ void launch_gn_apply(int dtype, const GnArgs& a, cudaStream_t s) {
       if (film) xu_launch(gn_apply_vec_kernel<bf16, true>, grid, 256, 0, s, d, ppb);
       else xu_launch(gn_apply_vec_kernel<bf16, false>, grid, 256, 0, s, d, ppb);
     }
+    return;
+  }
+  if (a.mode == GN_FILM || a.params_out != nullptr) {
+    xu_set_kernel_error("gn_apply: a resampling norm has no FiLM and no fused backward");
     return;
   }
   gn_apply_grid(d.C, 2 * d.Ho * d.Wo, d.N / 2, grid, ppb);

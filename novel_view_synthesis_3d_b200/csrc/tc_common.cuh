@@ -37,12 +37,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// L2 prefetch of a 4-D box (no shared memory, no barrier): issued a few pipeline steps ahead of the real load so that the
-// DRAM latency of streamed activations is paid by the prefetch and the load itself is an L2 hit
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
 // TMA store of a 4-D box from shared memory (bulk async-group completion)
 __device__ __forceinline__ void tma_store_4d(const void* src, const CUtensorMap* map, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map), "r"(smem_u32(src)),

@@ -244,8 +244,6 @@ void launch_wgrad_tc(const WgradArgs& a, cudaStream_t s) {
       const long long cost = waves * (per + 8);        // +8: per-CTA pipeline fill + reds, in pixel-tile units
       if (best < 0 || cost < best) { best = cost; ksplit = k; }
     }
-    static const char* env = getenv("XUNET_WGRAD_KSPLIT_CEIL");     // A/B switch: the round-1 rule
-    if (env) { ksplit = (int)((sms + T - 1) / T); if (ksplit > p.ptiles) ksplit = p.ptiles; if (ksplit < 1) ksplit = 1; }
   }
   CUtensorMap tx, ty;
   uint64_t xd[4] = {(uint64_t)a.Ci, (uint64_t)a.Wi, (uint64_t)a.Hi, (uint64_t)a.N};

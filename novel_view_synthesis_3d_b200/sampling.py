@@ -74,8 +74,6 @@ class Sampler:
         self.z = torch.zeros(batch_size, img_sidelength, img_sidelength, 3, dtype=torch.float32, device=self.dev)
         self.use_graph = use_graph
         self.graph = None
-        import os
-        self.device_schedule = os.environ.get('XUNET_SAMPLER_HOST_SCHEDULE') != '1'     # A/B switch: the host-side loop
         self._tab = None
         self._pos = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self._seed_base = torch.zeros(1, dtype=torch.int64, device=self.dev)
@@ -106,7 +104,7 @@ class Sampler:
     def capture(self, batch: dict) -> None:
         """Builds the static-conditioning state and the per-step CUDA graph without running the loop (benchmarks warm up
         with this instead of a full `steps`-long sample)."""
-        if self.use_graph and self.device_schedule:
+        if self.use_graph:
             self.sample(batch, seed=0, _max_steps=3)
             return
         saved = self.sched
@@ -136,7 +134,7 @@ class Sampler:
         logsnr = -20.0                                                                  # sampling.py:126
         sc = self.sched
         n = B * S * S * 3
-        if noises is None and self.use_graph and self.device_schedule:
+        if noises is None and self.use_graph:
             return self._sample_device_schedule(seed, _max_steps)
         try:
             for i in range(len(sc) - 1, -1, -1):

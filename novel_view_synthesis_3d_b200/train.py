@@ -10,7 +10,6 @@ dropout seed are fresh per step unless reference_quirks=True (the reference free
 """
 from __future__ import annotations
 
-import os
 from dataclasses import dataclass, replace
 from typing import Optional
 
@@ -280,7 +279,7 @@ class TrainStep:
       world > 1, NCCL           : ONE CUDA graph [forward + backward + bucketed all-reduces + Adam]; the collectives are
                                   captured on NCCL's stream as parallel branches of the graph
       world > 1, other backends : graph [forward + backward]; eager bucketed all-reduce; graph [Adam]   (gloo in tests, or
-                                  XUNET_DP_EAGER_COLLECTIVES=1, or when capturing the collectives fails)
+                                  NCCL when capturing the collectives fails)
       use_graph=False           : everything eager; the bucket hook still overlaps the all-reduces with the backward
 
     With gradient clipping the global-norm reduction runs right before Adam in every mode (after the all-reduce), inside
@@ -325,16 +324,12 @@ class TrainStep:
         self.graph_opt = None     # adam (two-graph mode only)
         self.stream = torch.cuda.Stream(device=self.dev) if use_graph else None
         self.allreduce = allreduce and self.world > 1       # allreduce=False: measurement knob (compute-only step at N>1)
-        # XUNET_DP_BUCKET_MB overrides the bucket size (experiments: smaller buckets start the collectives earlier but add launches)
-        if os.environ.get('XUNET_DP_BUCKET_MB'):
-            bucket_mb = float(os.environ['XUNET_DP_BUCKET_MB'])
         self.bucket_bytes = int(bucket_mb * (1 << 20))
         self.reducer = xdist.GradReducer(self.eng.grads) if self.world > 1 else None
         if self.reducer is not None:
             self.reducer.enabled = self.allreduce
         backend = torch.distributed.get_backend() if self.world > 1 else None
-        self.capture_collectives = (self.world > 1 and backend == 'nccl' and use_graph and
-                                    os.environ.get('XUNET_DP_EAGER_COLLECTIVES') != '1')
+        self.capture_collectives = self.world > 1 and backend == 'nccl' and use_graph
         self.mode = None
         self._synced_count = None
         self._sync_counters()

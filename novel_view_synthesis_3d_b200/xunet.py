@@ -132,7 +132,7 @@ class InputSlots:
     own inputs).  Slot j holds rows [j*B, (j+1)*B) of a k*B batch and has its own xunet_batch of device pointers.  All slots
     live in ONE device buffer (and one pinned mirror), 256-byte aligned segments in INPUT_ORDER, slot after slot: a training
     step stages every slot with a single H2D copy instead of ten small ones per slot (each costs ~7 us of stream time)."""
-    PIN_SLOTS = int(__import__('os').environ.get('XUNET_PIN_SLOTS', '3'))
+    PIN_SLOTS = 3
 
     def __init__(self, B: int, S: int, k: int, device):
         self.B, self.k = B, k

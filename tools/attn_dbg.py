@@ -20,4 +20,4 @@ reps = 50
 e0.record()
 for _ in range(reps): f()
 e1.record(); torch.cuda.synchronize()
-print(os.environ.get('XUNET_ATTN_DBG', '0'), os.environ.get('XUNET_ATTN_BWD_SPLIT', '-'), f'{e0.elapsed_time(e1) / reps * 1e3:.1f} us')
+print(f'{e0.elapsed_time(e1) / reps * 1e3:.1f} us')

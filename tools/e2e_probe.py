@@ -1,5 +1,5 @@
 """Where does the host spend its time in an end-to-end step?  (pinned staging ring / event waits / graph launch / loss copy)
-   python tools/e2e_probe.py [steps]      env: XUNET_PIN_SLOTS=k"""
+   python tools/e2e_probe.py [steps]"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
