@@ -7,6 +7,7 @@ state (state<step>: params, Adam moments and count, EMA, cond_mask streams) that
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 2000 --ema-decay 0.9999 --resume
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --max-grad-norm 1 --warmup-steps 5000 --ema-decay 0.9999
     python examples/train_srn.py cars_train_val --batch 4 --side 128 --grad-accum-steps 8     # 32 samples per update
+    python examples/train_srn.py cars_train_val --batch 8 --side 64 --loss mse --min-snr-gamma 5
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_srn.py cars_train_val
 """
 import argparse
@@ -39,19 +40,26 @@ def main():
                     help='warm the learning rate up linearly from 0 over this many steps (e.g. 5000)')
     ap.add_argument('--grad-accum-steps', type=int, default=1,
                     help='accumulate the gradient over this many micro-batches of --batch samples per update')
+    ap.add_argument('--loss', choices=('frobenius', 'mse'), default='frobenius',
+                    help="training loss: the reference's ||eps_hat - noise||_F, or the mean squared error of DDPM / 3DiM")
+    ap.add_argument('--min-snr-gamma', type=float, default=None,
+                    help='with --loss mse: weight each sample by min(SNR_t, G) / SNR_t (min-SNR-gamma, e.g. 5)')
     ap.add_argument('--resume', action='store_true', help='continue from the latest state<step> checkpoint')
     ap.add_argument('--ckpt', default='checkpoints')
     a = ap.parse_args()
+    if a.min_snr_gamma is not None and a.loss != 'mse':
+        ap.error('--min-snr-gamma needs --loss mse')
     local = xdist.init_from_env('nccl')
     rank, world = xdist.rank(), xdist.world_size()
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50, seed=rank)      # train.py:99-104
     model = P.XUNet(dtype=a.dtype)
     state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model, ema_decay=a.ema_decay,
-                                 max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps)
+                                 max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps, loss=a.loss)
     if a.resume and P.checkpoint.restore_train_state(a.ckpt, state) is not None and rank == 0:
         print(f'resumed from step {state.step}')
     step = P.TrainStep(state, grad_accum_steps=a.grad_accum_steps)
-    fd = P.ForwardDiffusion(step.eng)
+    fd = P.ForwardDiffusion(step.eng, min_snr_gamma=a.min_snr_gamma)
+    dev_keys = ('z', 'logsnr', 'noise', 'cond_mask') + (('loss_weight',) if fd.loss_weight is not None else ())
     stream = ds.batches(a.batch)
     k = a.grad_accum_steps
     for it in range(state.step, a.steps):
@@ -61,15 +69,15 @@ def main():
             fd.sample(b['target'], seed=(it * k + j) * world + rank)     # z, noise, logsnr, cond_mask on the GPU
             dev = step.eng.inp
             m = {key: b[key] for key in ('x', 'R1', 't1', 'R2', 't2', 'K')}
-            m.update({key: dev[key] if k == 1 else dev[key].clone() for key in ('z', 'logsnr', 'noise', 'cond_mask')})
+            m.update({key: dev[key] if k == 1 else dev[key].clone() for key in dev_keys})
             micro.append(m)
         if k == 1:
             batch = micro[0]
         else:
             batch = {key: torch.cat([m[key] for m in micro]) if isinstance(micro[0][key], torch.Tensor)
                      else np.concatenate([m[key] for m in micro]) for key in micro[0]}
-        noise, cond_mask = batch.pop('noise'), batch.pop('cond_mask')
-        loss = step(batch, noise, cond_mask=cond_mask)
+        noise, cond_mask, weight = batch.pop('noise'), batch.pop('cond_mask'), batch.pop('loss_weight', None)
+        loss = step(batch, noise, cond_mask=cond_mask, loss_weight=weight)
         if rank == 0 and it % 50 == 0:
             norm = '' if step.grad_norm is None else f'  grad norm {float(step.grad_norm):.4f}'
             print(f'{it}: {float(loss):.4f}{norm}')                                                    # train.py:157

@@ -112,6 +112,17 @@ int xunet_backward_accumulate(xunet_handle* h, const float* params, const xunet_
                               const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
                               void* stream);
 
+/* xunet_backward with the mean-squared epsilon loss (L_simple of DDPM / 3DiM) instead of the Frobenius norm, optionally weighted
+ * per sample (e.g. min-SNR-gamma):
+ *     loss = (1/B) sum_b w_b * (1/P) sum_i (eps_hat - noise)_bi^2        (P = S*S*3; residual in fp32)
+ * The sums of squares are reduced in fp64 in an order fixed by (B, P) alone, without atomics, and rounded to fp32 once
+ * into loss_out.  The output gradient is fl32(2 w_b / (B P)) * (eps_hat - noise), rounded to the activation dtype.
+ * loss_weight: device (B) fp32, or NULL (all 1).  accumulate != 0 adds into grads exactly as xunet_backward_accumulate
+ * does.  Same ordering, bucket hook and graph-capture behaviour as xunet_backward. */
+int xunet_backward_mse(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
+                       const float* loss_weight, const unsigned long long* seed_dev, void* workspace, float* grads,
+                       float* loss_out, int accumulate, void* stream);
+
 /* Data-parallel hook (north_star: "one NCCL allreduce of the gradient bucket"; the reference's pmap step would place
  * lax.pmean between value_and_grad and apply_gradients, train.py:70-76).  With a callback installed, xunet_backward calls
  *     fn(user, elem_offset, n_elems)

@@ -50,6 +50,8 @@ SYMBOLS = {
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     'xunet_backward_accumulate': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'xunet_backward_mse': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 6 +
+                           [C.c_int, C.c_void_p]),
     'xunet_set_grad_bucket_callback': (C.c_int, [C.c_void_p, BUCKET_FN, C.c_void_p, C.c_longlong]),
     'xunet_grad_bucket_count': (C.c_int, [C.c_void_p]),
     'xunet_count_kernels': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_void_p, C.c_void_p, C.c_void_p,

@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 103; }
+extern "C" int xunet_version(void) { return 104; }
 
 namespace {
 
@@ -560,6 +560,8 @@ struct Ctx {
   cudaStream_t s;
   cudaStream_t side = nullptr;   // non-null: weight gradients go here
   int acc_grads = 0;             // backward: add the parameter gradient into `grads` (xunet_backward_accumulate)
+  int mse = 0;                   // backward: seed with the mean-squared loss instead of the Frobenius norm (xunet_backward_mse)
+  const float* loss_weight = nullptr;   // mse: per-sample weights (B), nullptr = all 1
   void* act(int t) const { return ws + h->tensors[t].off; }
   void* grad(int t) const { const Tensor& x = h->tensors[t]; return ws + (x.galias >= 0 ? h->tensors[x.galias].goff : x.goff); }
   float gscale(int t) const { return h->tensors[t].gscale; }
@@ -802,7 +804,8 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
     const Op& o = h->ops[i];
     switch (o.kind) {
       case OP_EXTRACT:
-        launch_loss(dt, c.aux(h->a_eps), noise, c.aux(h->a_sumsq), loss_out, c.grad(o.x), B, S, c.s);
+        if (c.mse) launch_loss_mse(dt, c.aux(h->a_eps), noise, c.loss_weight, loss_out, c.grad(o.x), B, S, c.s);
+        else launch_loss(dt, c.aux(h->a_eps), noise, c.aux(h->a_sumsq), loss_out, c.grad(o.x), B, S, c.s);
         break;
       case OP_CONV: run_conv_bwd(c, o); break;
       case OP_GN: {
@@ -1017,6 +1020,21 @@ extern "C" int xunet_backward_accumulate(xunet_handle* h, const float* params, c
   xu_set_kernel_error("");
   Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
   c.acc_grads = 1;
+  XuDetBind bind(h->det);
+  return backward_impl(c, noise, loss_out);
+}
+
+extern "C" int xunet_backward_mse(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
+                                  const float* loss_weight, const unsigned long long* seed_dev, void* workspace, float* grads,
+                                  float* loss_out, int accumulate, void* stream) {
+  if (!h || !params || !batch || !noise || !workspace || !grads || !loss_out) return fail("xunet_backward_mse: null argument");
+  if (!h->training) return fail("xunet_backward_mse: handle was created with training=0");
+  if (!h->forward_done_train) return fail("xunet_backward_mse: call xunet_forward first");
+  xu_set_kernel_error("");
+  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
+  c.acc_grads = accumulate ? 1 : 0;
+  c.mse = 1;
+  c.loss_weight = loss_weight;
   XuDetBind bind(h->det);
   return backward_impl(c, noise, loss_out);
 }

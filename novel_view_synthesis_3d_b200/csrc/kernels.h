@@ -121,6 +121,10 @@ void launch_extract_frame1(int dtype, const void* o, float* eps, int B, int S, c
 // loss = ||eps - noise||_F ; dO (2B,S,S,3): frame0 = 0, frame1 = (eps-noise)/loss
 void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_scratch, float* loss_out, void* dO, int B,
                  int S, cudaStream_t s);
+// loss = (1/B) sum_b weight_b * mean_i (eps - noise)_bi^2 (weight == nullptr: all 1), reduced in fp64 in a fixed order;
+// dO (2B,S,S,3): frame0 = 0, frame1 = fl32(2 weight_b / (B*S*S*3)) * (eps - noise)
+void launch_loss_mse(int dtype, const float* eps, const float* noise, const float* weight, float* loss_out, void* dO, int B,
+                     int S, cudaStream_t s);
 // Adam; with ema, also ema = decay*ema + (1-decay)*p_new in the same pass.  warmup > 0: lr_t = lr * min(step - 1, warmup) /
 // warmup; norm_dev: optax.clip_by_global_norm by *norm_dev, where a non-finite *norm_dev leaves every buffer untouched and
 // increments *skipped.  Neither (norm_dev == nullptr, warmup == 0): plain Adam, without the clip / warm-up prologue.

@@ -1479,6 +1479,67 @@ void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_s
   else xu_launch(loss_grad_kernel<bf16>, cdiv(total, 256), 256, 0, s, eps, noise, sumsq_scratch, loss_out, (bf16*)dO, B, per);
 }
 
+__device__ __forceinline__ double block_sum_fixed(double x, double* red);
+
+// loss = (1/B) sum_b w_b (1/P) sum_i r_bi^2, r = eps - noise (P = S*S*3 per sample; w == nullptr: all 1).  The gradient does
+// not depend on the loss, so one pass writes the output gradient and the per-sample sums of squares:
+//   dO frame 1 = round_T(fl(c_b * fl(eps - noise))), c_b = fl32(2 w_b / (B P)) formed in double;  dO frame 0 = 0.
+// CTA (j, b) sums elements j, j + parts*256, ... of sample b in fp64 and stores its partial: the grid depends on (B, P) only
+// and nothing is added atomically, so the loss has the same bits on every run by construction.
+template <typename T>
+__global__ void __launch_bounds__(256) mse_grad_sumsq_kernel(const float* __restrict__ eps, const float* __restrict__ noise,
+                                                             const float* __restrict__ w, T* __restrict__ dO, int B,
+                                                             long long per, double* __restrict__ partials) {
+  xu_grid_dep_sync();
+  __shared__ double red[8];
+  const int b = blockIdx.y, parts = gridDim.x;
+  const float c = (float)(2.0 * (w != nullptr ? (double)w[b] : 1.0) / ((double)B * (double)per));
+  const float* e = eps + (long long)b * per;
+  const float* nz = noise + (long long)b * per;
+  T* d0 = dO + 2LL * b * per;
+  T* d1 = d0 + per;
+  double acc = 0.0;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < per; i += (long long)parts * 256) {
+    const float r = __fsub_rn(e[i], nz[i]);
+    acc = fma((double)r, (double)r, acc);
+    stf(d1 + i, __fmul_rn(c, r));
+    stf(d0 + i, 0.f);
+  }
+  const double t = block_sum_fixed(acc, red);
+  if (threadIdx.x == 0) partials[(long long)b * parts + blockIdx.x] = t;
+}
+// *loss_out = fl32( sum_b w_b * S_b / (B P) ), S_b the partials of sample b summed in a fixed order, everything in fp64.
+// The partials are re-zeroed (the reduction scratch is handed back all-zero, kernels.h).
+__global__ void __launch_bounds__(256) mse_loss_final_kernel(double* __restrict__ partials, int parts,
+                                                             const float* __restrict__ w, int B, long long per,
+                                                             float* __restrict__ loss_out) {
+  xu_grid_dep_sync();
+  __shared__ double red[8];
+  double total = 0.0;   // valid in thread 0
+  for (int b = 0; b < B; ++b) {
+    double acc = 0.0;
+    for (int i = threadIdx.x; i < parts; i += 256) {
+      acc += partials[(long long)b * parts + i];
+      partials[(long long)b * parts + i] = 0.0;
+    }
+    const double sb = block_sum_fixed(acc, red);
+    if (threadIdx.x == 0) total += (w != nullptr ? (double)w[b] : 1.0) * sb;
+    __syncthreads();   // red is rewritten by the next sample
+  }
+  if (threadIdx.x == 0) *loss_out = (float)(total / ((double)B * (double)per));
+}
+void launch_loss_mse(int dtype, const float* eps, const float* noise, const float* weight, float* loss_out, void* dO, int B,
+                     int S, cudaStream_t s) {
+  const long long per = (long long)S * S * 3;
+  const int parts = cdiv(per, 256 * 4);
+  double* partials = xu_det_scratch(s, (long long)B * parts);
+  if (partials == nullptr) return;
+  const dim3 grid(parts, B);
+  if (dtype == XU_F32) xu_launch(mse_grad_sumsq_kernel<float>, grid, 256, 0, s, eps, noise, weight, (float*)dO, B, per, partials);
+  else xu_launch(mse_grad_sumsq_kernel<bf16>, grid, 256, 0, s, eps, noise, weight, (bf16*)dO, B, per, partials);
+  xu_launch(mse_loss_final_kernel, 1, 256, 0, s, partials, parts, weight, B, per, loss_out);
+}
+
 // optax.adam (train.py:45, 74-76).  (1-b1), (1-b2) and the bias corrections are formed in double (optax forms them
 // from python floats) and only then rounded to fp32.
 // EMA = true also folds the weight EMA into the same pass: ema = d*ema + (1-d)*p_new with p_new still in registers (8 more

@@ -3,10 +3,14 @@ reference does on the host inside SceneInstanceDataset.__getitem__ (dataset/data
 
     fd = ForwardDiffusion(engine)                 # uploads the cosine-beta tables once
     fd.sample(x0_target, seed)                    # fills engine.inp['z'], ['noise'], ['logsnr'], ['cond_mask'] on the GPU
-Only the clean source / target images and the poses then cross PCIe (no z, no noise)."""
+Only the clean source / target images and the poses then cross PCIe (no z, no noise).
+
+With min_snr_gamma set, sample() also fills engine.inp['loss_weight'] (= fd.loss_weight) with the min-SNR-gamma weights of
+the drawn timesteps (Hang et al. 2023), for a state built with loss='mse'."""
 from __future__ import annotations
 
 import ctypes as C
+from typing import Optional
 
 import numpy as np
 import torch
@@ -15,8 +19,20 @@ from . import _lib
 from .sampling import cosine_beta_schedule
 
 
+def min_snr_weights(gamma: float, timesteps: int = 1000) -> np.ndarray:
+    """min(SNR_t, gamma) / SNR_t for t = 0..timesteps-1 (float64), with SNR_t = alpha_bar_t / (1 - alpha_bar_t) from the
+    cosine-beta table that noises z (data_loader.py:15-25,70-74) -- not from the batch's logsnr, which follows the
+    logsnr-cosine schedule and disagrees with it near both ends."""
+    gamma = float(gamma)
+    if not (gamma > 0.0 and np.isfinite(gamma)):
+        raise ValueError(f'min_snr_gamma must be a finite number > 0, got {gamma}')
+    ac = np.cumprod(1. - cosine_beta_schedule(timesteps), axis=0)
+    snr = ac / (1. - ac)
+    return np.minimum(snr, gamma) / snr
+
+
 class ForwardDiffusion:
-    def __init__(self, engine, p_uncond: float = 0.1):
+    def __init__(self, engine, p_uncond: float = 0.1, min_snr_gamma: Optional[float] = None):
         self.eng, self.lib, self.p_uncond = engine, _lib.load(), float(p_uncond)
         betas = cosine_beta_schedule(1000)
         ac = np.cumprod(1. - betas, axis=0)
@@ -25,6 +41,10 @@ class ForwardDiffusion:
         self.sqrt_1mac = torch.as_tensor(np.sqrt(1. - ac), dtype=torch.float32).to(dev)        # data_loader.py:74
         self.t = torch.zeros(engine.B, dtype=torch.int32, device=dev)
         self.x0 = torch.zeros_like(engine.inp['z'])
+        # per-timestep min-SNR-gamma weights, gathered by the device t of each sample (None: no weighting)
+        self.snr_weight = None if min_snr_gamma is None else \
+            torch.as_tensor(min_snr_weights(min_snr_gamma), dtype=torch.float32).to(dev)
+        self.loss_weight = None if min_snr_gamma is None else engine.inp['loss_weight']
 
     def sample(self, x0, seed: int, *, t=None, noise=None) -> None:
         """x0: clean target images (B,S,S,3), host or device.  t / noise: optional fixed timesteps / noise (parity tests)."""
@@ -45,3 +65,5 @@ class ForwardDiffusion:
                                                     e.inp['z'].data_ptr(), e.inp['noise'].data_ptr(), e.inp['logsnr'].data_ptr(),
                                                     self.t.data_ptr() if t is None else None, e.inp['cond_mask'].data_ptr(),
                                                     e.B, per, st), 'xunet_forward_diffusion')
+        if self.snr_weight is not None:
+            self.loss_weight.copy_(self.snr_weight[self.t.long()])

@@ -18,7 +18,7 @@ import torch
 
 from . import _lib
 from . import dist as xdist
-from .xunet import XUNet, ParamTree, Engine, InputSlots
+from .xunet import XUNet, ParamTree, Engine, InputSlots, check_loss
 
 
 @dataclass
@@ -80,6 +80,9 @@ class TrainState:
     ema_decay: Optional[float] = None
     # gradient-norm / skip-counter block; None unless create_train_state(max_grad_norm=..) or (warmup_steps=..)
     clip: Optional[ClipState] = None
+    # training objective: 'frobenius' (the reference's ||eps_hat - noise||_F, train.py:67) or 'mse' (the mean squared error
+    # of DDPM's L_simple, optionally weighted per sample); not part of the checkpoint
+    loss: str = 'frobenius'
     _mask_rng: np.random.RandomState = None
     _frozen_mask: Optional[np.ndarray] = None
 
@@ -156,7 +159,7 @@ def create_sample_data(batch_size, img_sidelength):
 def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_sidelength, *, model: XUNet = None,
                        zero_init: bool = True, reference_quirks: bool = False, init_on_device: bool = False,
                        ema_decay: Optional[float] = None, max_grad_norm: Optional[float] = None,
-                       warmup_steps: int = 0) -> TrainState:
+                       warmup_steps: int = 0, loss: str = 'frobenius') -> TrainState:
     """train.py:36-47.  Under torch.distributed the parameters of rank 0 are broadcast (the reference gives every
     device a different init, train.py:122-123 -- an ensemble, not data parallelism).
 
@@ -171,7 +174,13 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
     warmup_steps (e.g. 5000): warm the learning rate up linearly from 0 over this many updates
     (optax.linear_schedule(0, learning_rate, warmup_steps)); 0 keeps it constant.  With the defaults (None, 0) the
     optimizer step is exactly the plain one.  Every rank computes the norm of the same all-reduced gradient, so the clip and
-    skip decisions agree across ranks without a collective."""
+    skip decisions agree across ranks without a collective.
+
+    loss: 'frobenius' (default) trains on the reference's ||eps_hat - noise||_F over the whole micro-batch.  'mse' trains on
+    the mean squared error (1/B) sum_b w_b * mean_i (eps_hat - noise)_bi^2 of DDPM and 3DiM, whose per-sample weights w_b
+    (all 1 unless a loss_weight is passed, e.g. from ForwardDiffusion(min_snr_gamma=..)) make per-sample weighting possible.
+    With it, gradient accumulation and data parallelism give the gradient of the mean over the whole global batch."""
+    check_loss(loss)
     if ema_decay is not None and not (0.0 <= ema_decay <= 1.0):
         raise ValueError(f'ema_decay must lie in [0, 1], got {ema_decay}')
     if max_grad_norm is not None and not (float(max_grad_norm) > 0.0 and np.isfinite(float(max_grad_norm))):
@@ -198,7 +207,7 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
                       batch_size=train_batch_size, img_sidelength=img_sidelength, grad_scale=1.0 / world,
                       reference_quirks=reference_quirks, ema_params=ema,
                       ema_decay=None if ema_decay is None else float(ema_decay),
-                      clip=ClipState.zeros(params.flat.device) if opt.clip_or_warmup else None,
+                      clip=ClipState.zeros(params.flat.device) if opt.clip_or_warmup else None, loss=loss,
                       _mask_rng=np.random.RandomState(mask_seed & 0x7FFFFFFF))
 
 
@@ -224,17 +233,36 @@ def check_grad_accum_steps(k) -> int:
     return int(k)
 
 
-def check_accum_batch(batch: dict, noise, cond_mask, k: int, B: int) -> None:
-    """Every array of a gradient-accumulation step (the batch dict, noise, and cond_mask when given) must have k*B rows:
-    micro-batch j is rows [j*B, (j+1)*B).  Raises ValueError otherwise."""
+def check_accum_batch(batch: dict, noise, cond_mask, k: int, B: int, loss_weight=None) -> None:
+    """Every array of a gradient-accumulation step (the batch dict, noise, and cond_mask and loss_weight when given) must
+    have k*B rows: micro-batch j is rows [j*B, (j+1)*B).  Raises ValueError otherwise."""
     items = [(key, batch[key]) for key in ('x', 'z', 'logsnr', 'R1', 't1', 'R2', 't2', 'K')] + [('noise', noise)]
     if cond_mask is not None:
         items.append(('cond_mask', cond_mask))
+    if loss_weight is not None:
+        items.append(('loss_weight', loss_weight))
     for key, v in items:
         shape = tuple(v.shape) if hasattr(v, 'shape') else np.shape(v)
         rows = int(shape[0]) if shape else 0
         if rows != k * B:
             raise ValueError(f"{key} has leading dimension {rows}, expected grad_accum_steps * batch_size = {k} * {B} = {k * B}")
+
+
+def check_loss_weight(loss: str, loss_weight, rows: int) -> None:
+    """Per-sample loss weights: only with loss='mse', shape (rows,), and, when they are on the host, finite and >= 0 (device
+    tensors are not read back).  Raises ValueError otherwise."""
+    if loss_weight is None:
+        return
+    if loss != 'mse':
+        raise ValueError(f"loss_weight needs a state built with loss='mse', this one uses loss={loss!r}")
+    shape = tuple(loss_weight.shape) if hasattr(loss_weight, 'shape') else np.shape(loss_weight)
+    if shape != (rows,):
+        raise ValueError(f'loss_weight has shape {shape}, expected ({rows},)')
+    if isinstance(loss_weight, torch.Tensor) and loss_weight.is_cuda:
+        return
+    w = loss_weight.detach().double().numpy() if isinstance(loss_weight, torch.Tensor) else np.asarray(loss_weight, np.float64)
+    if not (np.isfinite(w).all() and (w >= 0).all()):
+        raise ValueError('loss_weight must be finite and >= 0')
 
 
 def _cond_mask(state: TrainState, B: int) -> np.ndarray:
@@ -247,18 +275,21 @@ def _cond_mask(state: TrainState, B: int) -> np.ndarray:
 
 
 def apply_model(state: TrainState, batch_x, batch_z, batch_logsnr, batch_R1, batch_t1, batch_R2, batch_t2, batch_K,
-                batch_noise, *, cond_mask=None):
-    """train.py:49-72: forward with train=True, loss ||eps_hat - noise||_F, gradients w.r.t. all parameters.
+                batch_noise, *, cond_mask=None, loss_weight=None):
+    """train.py:49-72: forward with train=True, the state's loss (||eps_hat - noise||_F by default), gradients w.r.t. all
+    parameters.  loss_weight: per-sample weights (B,) of loss='mse', host or device (all 1 when None).
     Returns (loss: 0-d device tensor, grads: ParamTree view of the flat gradient bucket).  With
     torch.distributed initialised the gradient bucket is all-reduced (sum) here; update_model applies 1/world."""
     B, S = int(batch_x.shape[0]), int(batch_x.shape[1])
+    check_loss_weight(state.loss, loss_weight, B)
     eng = state.model.engine(B, S, True)
     batch = dict(x=batch_x, z=batch_z, logsnr=batch_logsnr, R1=batch_R1, t1=batch_t1, R2=batch_R2, t2=batch_t2, K=batch_K)
     mask = _cond_mask(state, B) if cond_mask is None else cond_mask
-    eng.load_inputs(batch, cond_mask=mask, noise=batch_noise)
+    eng.load_inputs(batch, cond_mask=mask, noise=batch_noise, loss_weight=loss_weight)
     seed = 0 if state.reference_quirks else _dropout_seed(state.step + 1)   # PRNGKey(0) frozen at trace time, train.py:66
     eng.forward(state.params.flat, train=True, seed=seed)
-    loss, grads = eng.backward(state.params.flat)
+    loss, grads = eng.backward(state.params.flat, loss=state.loss,
+                               loss_weight=None if loss_weight is None else eng.inp['loss_weight'])
     xdist.allreduce_sum_(grads, bucket_elems=64 << 20)
     # the loss is a copy; `grads` are views of the engine's gradient bucket (valid until the next backward of this plan)
     return loss[0].clone(), state.model.tree_from_flat(grads, S, B)
@@ -292,7 +323,9 @@ class TrainStep:
     its own Frobenius norm, so this is not the gradient of one batch of k*B samples (as data parallelism is not).  Under
     data parallelism only the last backward carries the bucket hook, so the all-reduce covers the whole sum.  The returned
     loss is the mean of the k micro-batch losses; `step` and the Adam count advance by one per call.  k = 1 (the default)
-    runs exactly the step without accumulation.
+    runs exactly the step without accumulation.  With a state built with loss='mse' every micro-batch holds B samples of the
+    same mean, so the update is that of the mean squared error over all world*k*B samples, and the returned loss is that
+    mean; per-sample weights, when given, have k*B rows like cond_mask and are staged with the batch.
 
     A captured graph holds the NCCL kernels of the process group it was captured with: drop the TrainStep (or call
     `release_graphs()`) before `torch.distributed.destroy_process_group()`.
@@ -302,6 +335,7 @@ class TrainStep:
                  grad_accum_steps: int = 1):
         self.k = check_grad_accum_steps(grad_accum_steps)
         self.state = state
+        self.mse = state.loss == 'mse'      # the captured graph reads each slot's loss weights in place
         self.eng: Engine = state.model.engine(state.batch_size, state.img_sidelength, True)
         self.dev = self.eng.device
         # the k micro-batches' inputs, dropout seeds and losses, all in device memory: the k forward/backward pairs of one
@@ -372,7 +406,8 @@ class TrainStep:
                     if self.reducer is not None:
                         self.reducer.begin()
                 e.backward(s.params.flat, accumulate=j > 0, inputs=(self.inputs, j), seed_dev=sd,
-                           loss_out=self.losses[j:j + 1])
+                           loss_out=self.losses[j:j + 1], loss=s.loss,
+                           loss_weight=self.inputs.inp[j]['loss_weight'] if self.mse else None)
         finally:
             self._set_hook(hook)
         if self.k > 1:
@@ -436,17 +471,20 @@ class TrainStep:
         if retry:
             self._capture()
 
-    def __call__(self, batch: dict, noise, cond_mask=None) -> torch.Tensor:
+    def __call__(self, batch: dict, noise, cond_mask=None, loss_weight=None) -> torch.Tensor:
         """One optimisation step on host (or device) inputs; returns the loss as a 0-d device tensor (a view of the step's
         loss slot: read or copy it before the next step).  With grad_accum_steps=k every array has k*B rows, and the loss
-        is the mean of the k micro-batch losses."""
+        is the mean of the k micro-batch losses.  loss_weight: per-sample weights of a loss='mse' state (all 1 when None)."""
         s = self.state
         if self.k > 1:
-            check_accum_batch(batch, noise, cond_mask, self.k, self.eng.B)
+            check_accum_batch(batch, noise, cond_mask, self.k, self.eng.B, loss_weight)
+        check_loss_weight(s.loss, loss_weight, self.k * self.eng.B)
+        if self.mse and loss_weight is None:
+            loss_weight = np.ones(self.k * self.eng.B, np.float32)    # the slots may still hold the last call's weights
         self._sync_counters()
         # micro-batch j draws the j-th B values of the rank's cond_mask stream
         mask = np.concatenate([_cond_mask(s, self.eng.B) for _ in range(self.k)]) if cond_mask is None else cond_mask
-        self.h2d_bytes = self.inputs.load(batch, cond_mask=mask, noise=noise)
+        self.h2d_bytes = self.inputs.load(batch, cond_mask=mask, noise=noise, loss_weight=loss_weight)
         if self.use_graph:
             if self.graph_fb is None:
                 self._capture()

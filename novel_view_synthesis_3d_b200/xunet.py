@@ -22,7 +22,15 @@ from . import _lib
 
 POSE_EMB_DIM = 144
 BATCH_KEYS = ('x', 'z', 'logsnr', 'R1', 't1', 'R2', 't2', 'K')
-INPUT_ORDER = BATCH_KEYS + ('cond_mask', 'noise')     # segment order of Engine.inp_all
+INPUT_ORDER = BATCH_KEYS + ('cond_mask', 'noise', 'loss_weight')     # segment order of Engine.inp_all
+LOSSES = ('frobenius', 'mse')
+
+
+def check_loss(loss) -> str:
+    """Validates a training-loss name: 'frobenius' (the reference's ||eps_hat - noise||_F) or 'mse' (mean squared error)."""
+    if loss not in LOSSES:
+        raise ValueError(f'loss must be one of {LOSSES}, got {loss!r}')
+    return loss
 
 
 @dataclass(frozen=True)
@@ -138,7 +146,7 @@ class InputSlots:
         self.B, self.k = B, k
         f32 = dict(dtype=torch.float32, device=device)
         self.shapes = {'x': (B, S, S, 3), 'z': (B, S, S, 3), 'logsnr': (B,), 'R1': (B, 3, 3), 't1': (B, 3), 'R2': (B, 3, 3),
-                       't2': (B, 3), 'K': (B, 3, 3), 'cond_mask': (B,), 'noise': (B, S, S, 3)}
+                       't2': (B, 3), 'K': (B, 3, 3), 'cond_mask': (B,), 'noise': (B, S, S, 3), 'loss_weight': (B,)}
         self._seg, off = {}, 0          # (slot, key) -> (offset, elements)
         for j in range(k):
             for key in INPUT_ORDER:
@@ -150,6 +158,7 @@ class InputSlots:
                     for j in range(k)]
         for d in self.inp:
             d['cond_mask'].fill_(1.0)
+            d['loss_weight'].fill_(1.0)
         # pinned staging ring: the host may run several steps ahead of the GPU (a step is a few ms of device time, the host
         # side far less), so a slot is rewritten only after the H2D copy that last read it has completed (one event per slot)
         self._pin_ring = [torch.zeros(off, dtype=torch.float32).pin_memory() for _ in range(self.PIN_SLOTS)]
@@ -159,9 +168,9 @@ class InputSlots:
         self.cbatch = [_lib.XunetBatch(**{key: d[key].data_ptr() for key in BATCH_KEYS + ('cond_mask',)}, rays=None)
                        for d in self.inp]
 
-    def load(self, batch: dict, cond_mask=None, noise=None) -> int:
-        """Copies one batch dict of k*B samples (numpy / torch, any float dtype) into the slots, micro-batch j into slot j.
-        Returns the number of host->device bytes moved."""
+    def load(self, batch: dict, cond_mask=None, noise=None, loss_weight=None) -> int:
+        """Copies one batch dict of k*B samples (numpy / torch, any float dtype) into the slots, micro-batch j into slot j;
+        cond_mask, noise and the per-sample loss weights too when given.  Returns the number of host->device bytes moved."""
         k = self.k
         nbytes = 0
         items = [(key, batch[key]) for key in BATCH_KEYS]
@@ -169,6 +178,8 @@ class InputSlots:
             items.append(('cond_mask', cond_mask))
         if noise is not None:
             items.append(('noise', noise))
+        if loss_weight is not None:
+            items.append(('loss_weight', loss_weight))
         staged = []
         slot, pin = None, None
         for key, v in items:
@@ -260,10 +271,10 @@ class Engine:
             pass
 
     # ---- host -> device staging (pinned memory, async on the current stream) -------------------------
-    def load_inputs(self, batch: dict, cond_mask=None, noise=None) -> int:
+    def load_inputs(self, batch: dict, cond_mask=None, noise=None, loss_weight=None) -> int:
         """Copies one batch dict (numpy / torch, any float dtype) into the static device buffers.
         Returns the number of host->device bytes moved."""
-        return self.inputs.load(batch, cond_mask=cond_mask, noise=noise)
+        return self.inputs.load(batch, cond_mask=cond_mask, noise=noise, loss_weight=loss_weight)
 
     def set_rays(self, rays) -> None:
         """Explicit-rays entry (SURVEY 8(c)): `rays` = (B, 2, S, S, 6) [pos xyz | dir xyz] for camera 1 / camera 2, e.g. the
@@ -306,20 +317,36 @@ class Engine:
         return self.eps
 
     def backward(self, flat_params: torch.Tensor, *, accumulate: bool = False, inputs: Optional[Tuple[InputSlots, int]] = None,
-                 seed_dev: Optional[torch.Tensor] = None, loss_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-        """loss = ||eps - noise||_F and its parameter gradient (train.py:62-71); follows forward() with the same `inputs` and
-        `seed_dev`.  accumulate=True adds the gradient into `self.grads` (xunet_backward_accumulate) instead of overwriting it.
+                 seed_dev: Optional[torch.Tensor] = None, loss_out: Optional[torch.Tensor] = None, loss: str = 'frobenius',
+                 loss_weight: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The loss and its parameter gradient (train.py:62-71); follows forward() with the same `inputs` and `seed_dev`.
+        loss='frobenius': ||eps - noise||_F (train.py:67); loss='mse': (1/B) sum_b w_b * mean_i (eps - noise)_bi^2
+        (xunet_backward_mse), with w = loss_weight, a device fp32 (B,) tensor, or all 1 when None.
+        accumulate=True adds the gradient into `self.grads` instead of overwriting it.
         loss_out: a device float to write the loss to instead of `self.loss`."""
         if not self.training:
             raise RuntimeError('engine was built with training=False')
+        check_loss(loss)
         cb, noise = (self.cbatch, self.inp['noise']) if inputs is None else (inputs[0].cbatch[inputs[1]], inputs[0].inp[inputs[1]]['noise'])
         sd = self.seed if seed_dev is None else seed_dev
-        loss = self.loss if loss_out is None else loss_out
-        fn = self.lib.xunet_backward_accumulate if accumulate else self.lib.xunet_backward
+        out = self.loss if loss_out is None else loss_out
         st = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(fn(self.h, flat_params.data_ptr(), C.byref(cb), noise.data_ptr(), sd.data_ptr(), self.ws.data_ptr(),
-                      self.grads.data_ptr(), loss.data_ptr(), st), 'xunet_backward_accumulate' if accumulate else 'xunet_backward')
-        return loss, self.grads
+        args = (flat_params.data_ptr(), C.byref(cb), noise.data_ptr())
+        tail = (sd.data_ptr(), self.ws.data_ptr(), self.grads.data_ptr(), out.data_ptr())
+        if loss == 'mse':
+            w = None
+            if loss_weight is not None:
+                if not (loss_weight.is_cuda and loss_weight.dtype == torch.float32 and loss_weight.is_contiguous()
+                        and tuple(loss_weight.shape) == (self.B,)):
+                    raise ValueError(f'loss_weight must be a contiguous fp32 device tensor of shape ({self.B},)')
+                w = loss_weight.data_ptr()
+            _lib.check(self.lib.xunet_backward_mse(self.h, *args, w, *tail, int(accumulate), st), 'xunet_backward_mse')
+            return out, self.grads
+        if loss_weight is not None:
+            raise ValueError("loss_weight needs loss='mse': the Frobenius loss has no per-sample term to weight")
+        fn = self.lib.xunet_backward_accumulate if accumulate else self.lib.xunet_backward
+        _lib.check(fn(self.h, *args, *tail, st), 'xunet_backward_accumulate' if accumulate else 'xunet_backward')
+        return out, self.grads
 
     def count_kernels(self, flat_params: torch.Tensor) -> Tuple[int, int]:
         """(forward, backward) kernel launches of this plan, counted from a throw-away graph capture."""
