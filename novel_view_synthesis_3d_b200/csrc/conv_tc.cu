@@ -66,11 +66,14 @@ struct TcParams {
 // u = yhat*(1+scale)+shift, stores dyh = du*(1+scale) and the FiLM gradient [du*yhat | du], emits the same channel sums.
 constexpr int kConvThreads = 288;      // two consumer warpgroups + one producer warp
 constexpr int kXP = 68;                // fp32 pitch of the transpose buffer (16-byte row reads without bank conflicts)
-// Two CTAs per SM (96 registers per thread) only for narrow tiles with the plain / statistics epilogues; the fused GroupNorm-
-// backward epilogues (EPI 2/3) need more registers and run one CTA per SM.
-__host__ __device__ constexpr int conv_ctas_per_sm(int epi, int bn) { return (bn <= 64 && epi < 2) ? 2 : 1; }
+// Two CTAs per SM (96 registers per thread) for narrow tiles with the plain / statistics epilogues and with the fused
+// GroupNorm-backward one (EPI 2, without spills except at BK = 16, BN = 64); the FiLM-backward epilogue (EPI 3) needs more
+// registers and runs one CTA per SM.
+__host__ __device__ constexpr int conv_ctas_per_sm(int epi, int bn, int bk) {
+  return bn <= 64 && (epi < 2 || (epi == 2 && (bn < 64 || bk > 16))) ? 2 : 1;
+}
 template <int BK, int EPI, int BN>
-__global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+__global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                                const __grid_constant__ CUtensorMap tmB,
                                                                                const __grid_constant__ CUtensorMap tmY, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -90,6 +93,8 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
   float* smT = reinterpret_cast<float*>(smY + 2 * (size_t)Y_BYTES);      // 2 x [64][kXP] fp32 transpose buffers
   uint64_t* full = reinterpret_cast<uint64_t*>(smT + 2 * 64 * kXP);
   uint64_t* empty = full + p.stages;
+  // EPI 2/3: per consumer warp, the {rstd, -mean*rstd, gamma, beta} entries of the BN / 2 columns it handles in a tile
+  float4* smG = reinterpret_cast<float4*>(empty + p.stages) + (threadIdx.x >> 5) * (BN / 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_k = p.halo ? 3 * p.KC : p.T * p.KC;
@@ -157,9 +162,8 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
     const bool bias_vec = (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0;   // leaf offsets are 16-byte aligned in the flat buffer; scalar loads otherwise
     const int lane_base = wg * 64 + (wq & 1) * 32;
     const int r = lane_base + lane;                      // row of the 128-pixel tile
-    const int tw = r % p.TW;
-    const int th = (r / p.TW) % p.TH;
-    const int tn = r / (p.TW * p.TH);
+    // pixel offset of row r from the tile's first pixel (one register across the tile loop instead of three coordinates)
+    const unsigned rofs = (unsigned)((((r / (p.TW * p.TH)) * p.H + (r / p.TW) % p.TH) * p.W + r % p.TW));
     float* tbuf = smT + wg * 64 * kXP;
     const int fr = wq * 16 + (lane >> 2), fc = (lane & 3) * 2;   // accumulator fragment: rows fr, fr + 8; columns 8 i + fc, + 1
     const bool y_issuer = threadIdx.x == 0;               // first consumer thread issues / retires the TMA stores
@@ -204,17 +208,29 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
       const int tx = t % p.tiles_x; t /= p.tiles_x;
       const int ty = t % p.tiles_y; t /= p.tiles_y;
       const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = t * p.TN;
-      const long long pix = ((long long)(n0 + tn) * p.H + (y0 + th)) * p.W + (x0 + tw);
+      const long long pix = ((long long)n0 * p.H + y0) * p.W + x0 + rofs;
       bf16* yrow = p.y + pix * p.Co + (long long)n_tile * BN;
       const bf16* rrow = p.res ? p.res + pix * p.Co + (long long)n_tile * BN : nullptr;
-      const float* brow = p.bias ? p.bias + (long long)n_tile * BN : nullptr;
+      const float* brow = EPI < 2 && p.bias ? p.bias + (long long)n_tile * BN : nullptr;   // a data gradient has no bias
+      // CG accumulator columns per transpose group, CW of them per thread, whose operands are held in registers SW at a time.
+      // The fused GroupNorm-backward epilogues take their CW columns in 16-column sub-chunks (x, the FiLM operands and the
+      // statistics partials of 16 channels live at once), and a 32-column tile in one 32-column group so that all four warps
+      // of a warpgroup have columns: this lets them run two CTAs per SM without spilling.
+      constexpr int CG = EPI >= 2 && BN < 64 ? BN : 64, CW = CG / 2, SW = EPI >= 2 ? 8 : CW;
       // STATS: the 32 pixels of this warp belong to one sample (host-checked): b = image of the warp's first row / 2
       double* cs_row = nullptr;
       const long long srow = (long long)((n0 + lane_base / (p.TW * p.TH)) >> 1) * p.Co + (long long)n_tile * BN;
       if constexpr (EPI != 0) cs_row = p.cstats + srow * 2;
       const bf16* gxrow = nullptr;
       const float4* gprow = nullptr;
-      if constexpr (EPI >= 2) { gxrow = p.gx + pix * p.Co + (long long)n_tile * BN; gprow = p.gnp + srow; }
+      if constexpr (EPI >= 2) {
+        gxrow = p.gx + pix * p.Co + (long long)n_tile * BN; gprow = p.gnp + srow;
+        // stage the norm table of this warp's columns (entry cc / 2 + k <-> column cc + ehalf * CW + k) once per tile: read
+        // from shared memory in the column loop instead of being held in registers
+        __syncwarp();                   // the warp's reads of the previous tile's entries are done
+        for (int k = lane; k < BN / 2; k += 32) smG[k] = __ldg(gprow + (k / CW) * CG + ehalf * CW + k % CW);
+        __syncwarp();
+      }
       const bf16* gerow = nullptr;
       bf16* gderow = nullptr;
       unsigned long long dseed = 0ULL;
@@ -224,62 +240,64 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
         if (p.drop_on) dseed = *p.seed_dev;
       }
 #pragma unroll
-      for (int cc = 0; cc < BN; cc += 64) {
-        // accumulator columns cc .. cc + 63 of this warpgroup's 64 rows -> transpose buffer
+      for (int cc = 0; cc < BN; cc += CG) {
+        // accumulator columns cc .. cc + CG - 1 of this warpgroup's 64 rows -> transpose buffer
 #pragma unroll
         for (int i = 0; i < BN / 2; i += 4) {
           const int col = 8 * (i / 4);
-          if (col >= cc && col < cc + 64) {
+          if (col >= cc && col < cc + CG) {
             *reinterpret_cast<float2*>(tbuf + fr * kXP + col - cc + fc) = make_float2(acc[i], acc[i + 1]);
             *reinterpret_cast<float2*>(tbuf + (fr + 8) * kXP + col - cc + fc) = make_float2(acc[i + 2], acc[i + 3]);
           }
         }
         named_bar_sync(2 + wg, 128);
-        const int c0 = cc + ehalf * 32;
+        float sx[32];     // STATS only (dead otherwise)
+#pragma unroll
+        for (int h = 0; h < CW; h += SW) {
+        const int c0 = cc + ehalf * CW + h;
         const bool active = c0 < BN;
-        // the residual operands of the whole 32-column chunk are requested before anything waits on them: each is a 16-byte
+        // the residual operands of the whole sub-chunk are requested before anything waits on them: each is a 16-byte
         // access of a (pixel-pitch strided) row, i.e. a DRAM-latency load per thread when issued one by one
-        uint4 rv[4];
+        uint4 rv[SW / 8];
         if (active && EPI < 2 && rrow) {
 #pragma unroll
-          for (int q = 0; q < 4; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(rrow + c0 + 8 * q));
+          for (int q = 0; q < SW / 8; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(rrow + c0 + 8 * q));
         }
         if constexpr (EPI >= 2) {      // the GroupNorm input of this pixel (rv is free: a data gradient has no residual operand)
           if (active) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(gxrow + c0 + 8 * q));
+            for (int q = 0; q < SW / 8; ++q) rv[q] = __ldg(reinterpret_cast<const uint4*>(gxrow + c0 + 8 * q));
           }
         }
-        uint4 scv[4], shv[4];
+        uint4 scv[SW / 8], shv[SW / 8];
         if constexpr (EPI == 3) {
           if (active) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
+            for (int q = 0; q < SW / 8; ++q) {
               scv[q] = __ldg(reinterpret_cast<const uint4*>(gerow + c0 + 8 * q));
               shv[q] = __ldg(reinterpret_cast<const uint4*>(gerow + p.Co + c0 + 8 * q));
             }
           }
         }
-        float v[32];
+        float v[SW];
         if (active) {
-          const float* trow = tbuf + (r - wg * 64) * kXP + ehalf * 32;
+          const float* trow = tbuf + (r - wg * 64) * kXP + ehalf * CW + h;
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
+          for (int q = 0; q < SW / 4; ++q) {
             const float4 t4 = *reinterpret_cast<const float4*>(trow + 4 * q);
             v[4 * q] = t4.x; v[4 * q + 1] = t4.y; v[4 * q + 2] = t4.z; v[4 * q + 3] = t4.w;
           }
         }
         const int ysub = p.cws == 64 ? ehalf : 0;
         uint8_t* yst = smY + (size_t)(ybox & 1) * Y_BYTES + (size_t)r * (p.cws * 2);
-        if (tma_store) {
+        if (tma_store) {           // (EPI < 2: a single sub-chunk)
           // the store that read this staging buffer two boxes ago must have finished reading before it is overwritten
           if (y_issuer) bulk_wait_group_read<1>();
           named_bar_sync(1, 256);
         }
         if (active) {
-          float sx[32];     // STATS only (dead otherwise)
 #pragma unroll
-          for (int j = 0; j < 32; j += 8) {
+          for (int j = 0; j < SW; j += 8) {
             float f[8];
             {
               float4 bq0 = make_float4(0.f, 0.f, 0.f, 0.f), bq1 = bq0;
@@ -301,7 +319,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
               const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
 #pragma unroll
               for (int q = 0; q < 8; ++q) {
-                const float4 pp = __ldg(gprow + c0 + j + q);
+                const float4 pp = smG[cc / 2 + h + j + q];
                 const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
                 xh[q] = fmaf(xv, pp.x, pp.y);
                 if (p.gn_swish) f[q] *= swish_gradf_(fmaf(xh[q], pp.z, pp.w));
@@ -322,7 +340,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
               float tsc[8], tsh[8];
 #pragma unroll
               for (int q = 0; q < 8; ++q) {
-                const float4 pp = __ldg(gprow + c0 + j + q);
+                const float4 pp = smG[cc / 2 + h + j + q];
                 const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
                 const float sc = (q & 1) ? __high2float(s2[q >> 1]) : __low2float(s2[q >> 1]);
                 const float sh = (q & 1) ? __high2float(h2[q >> 1]) : __low2float(h2[q >> 1]);
@@ -348,17 +366,17 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
             __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&outv);
 #pragma unroll
             for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(f[2 * q], f[2 * q + 1]);
-            if (tma_store) sts128(yst + ((((ysub << 2) + (j >> 3)) ^ yswz) << 4), outv);
+            if (tma_store) sts128(yst + ((((ysub << 2) + ((h + j) >> 3)) ^ yswz) << 4), outv);
             else *reinterpret_cast<uint4*>(yrow + c0 + j) = outv;
             if constexpr (EPI >= 2) {
               // sums over what is STORED (the second pass reads the rounded dyh back)
 #pragma unroll
               for (int q = 0; q < 4; ++q) {
                 const float a = __low2float(o2[q]), b = __high2float(o2[q]);
-                sx[(j & 8) + 2 * q] = a * xh[2 * q];   sx[(j & 8) + 2 * q + 1] = b * xh[2 * q + 1];
-                sx[16 + (j & 8) + 2 * q] = a;          sx[16 + (j & 8) + 2 * q + 1] = b;
+                sx[((h + j) & 8) + 2 * q] = a * xh[2 * q];   sx[((h + j) & 8) + 2 * q + 1] = b * xh[2 * q + 1];
+                sx[16 + ((h + j) & 8) + 2 * q] = a;          sx[16 + ((h + j) & 8) + 2 * q + 1] = b;
               }
-              if (j & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
+              if ((h + j) & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
             }
             if constexpr (EPI == 1) {
               // statistics of what is STORED (rounded), so the consumer's normalisation is exactly zero-mean / unit-variance
@@ -371,6 +389,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN)) conv_
               if (j & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
             }
           }
+        }
         }
         if (tma_store) {
           fence_async_smem();                 // generic-proxy writes -> visible to the TMA unit
@@ -692,9 +711,11 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
   p.total_tiles = p.m_tiles * p.n_tiles;
   // CTAs per SM: two where the kernel is compiled for it (conv_ctas_per_sm) and shared
   // memory keeps a >= 3-deep TMA ring for each; one persistent CTA per SM with a 4-deep ring otherwise
-  const size_t fixed = ystage + (size_t)2 * 64 * kXP * 4 + 1024 + 256;
+  const int epi = a.gn_x == nullptr ? 0 : (a.gn_e != nullptr ? 3 : 2);
+  const size_t gtab = epi >= 2 ? (size_t)8 * (p.BN / 2) * 16 : 0;      // the EPI 2/3 per-warp norm tables (smG)
+  const size_t fixed = ystage + (size_t)2 * 64 * kXP * 4 + 1024 + 256 + gtab;
   int per_sm = 1, stages = 2;
-  for (int cand = conv_ctas_per_sm(a.gn_x != nullptr ? 2 : 0, p.BN); cand >= 1; --cand) {
+  for (int cand = conv_ctas_per_sm(epi, p.BN, bk); cand >= 1; --cand) {
     const size_t budget = cand == 1 ? (size_t)227 * 1024 : (size_t)112 * 1024;
     int st = (int)((budget - fixed) / stage);
     if (st > 6) st = 6;
@@ -729,7 +750,7 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
   p.drop_rate = a.gn_drop_rate; p.drop_op = a.gn_drop_op; p.seed_dev = a.gn_seed_dev;
   p.drop_on = (a.gn_drop_rate > 0.f && a.gn_train && a.gn_seed_dev != nullptr) ? 1 : 0;
   if (a.gn_x != nullptr) {
-    if (a.mode != 1 || a.accumulate || !warp_in_sample || a.cstats == nullptr || a.gn_params == nullptr) {
+    if (a.mode != 1 || a.accumulate || a.bias != nullptr || !warp_in_sample || a.cstats == nullptr || a.gn_params == nullptr) {
       xu_set_kernel_error("conv_tc: fused GroupNorm backward requested for an unsupported configuration");
       return;
     }

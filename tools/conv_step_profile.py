@@ -1,5 +1,5 @@
 """Per-launch time and TFLOP/s of every wgmma conv launch (forward + data gradient) inside ONE eager training step, matched to
-its shape.  The library logs each launch configuration to stderr with XUNET_CONV_LOG=1 (in launch order); CUPTI (torch.profiler)
+its shape and epilogue variant (EPI, from the kernel's template arguments).  The library logs each launch configuration to stderr with XUNET_CONV_LOG=1 (in launch order); CUPTI (torch.profiler)
 gives the device time of the conv_tc_kernel launches in the same order.
    XU_MODEL=full XU_B=4 XU_S=128 python tools/conv_step_profile.py > conv_step_profile.txt"""
 import os, re, subprocess, sys, collections
@@ -8,6 +8,7 @@ if os.environ.get('XU_CHILD') != '1':
     r = subprocess.run([sys.executable, os.path.abspath(__file__)], env=env, capture_output=True, text=True)
     logs = [l for l in r.stderr.splitlines() if l.startswith('conv_tc mode=')]
     times = [float(l.split()[1]) for l in r.stdout.splitlines() if l.startswith('T ')]
+    epis = [l.split()[2] for l in r.stdout.splitlines() if l.startswith('T ')]
     marks = [i for i, l in enumerate(r.stderr.splitlines()) if l.startswith('conv_tc mode=') or l.startswith('MARK')]
     # keep only the log lines of the profiled step (after the last MARK)
     lines = r.stderr.splitlines()
@@ -40,20 +41,23 @@ if os.environ.get('XU_CHILD') != '1':
         print(r.stderr[-2000:])
         sys.exit(1)
     agg = collections.OrderedDict()
-    for l, t in zip(logs, times):
+    for l, t, epi in zip(logs, times, epis):
         kv = dict(re.findall(r'(\w+)=(-?\d+)', l))
         N, H, W = int(kv['N']), int(l.split()[3].split('x')[0]), int(l.split()[3].split('x')[1])
         Ci, Co, ks = int(kv['Ci']), int(kv['Co']), int(kv['ks'])
         flops = 2.0 * N * H * W * ks * ks * Ci * Co
-        key = (kv['mode'], H, Ci, Co, ks, kv['BN'], kv['tiles'], kv['ctas'], kv['halo'])
+        key = (kv['mode'], epi, H, Ci, Co, ks, kv['BN'], kv['tiles'], kv['ctas'], kv['halo'])
         a = agg.setdefault(key, [0, 0.0, flops])
         a[0] += 1; a[1] += t
     tot = sum(a[1] for a in agg.values())
-    print('mode(0 fwd,1 dgrad) HxH Ci->Co k | BN tiles ctas halo | launches  avg us  TFLOP/s  share')
+    print('mode(0 fwd,1 dgrad) EPI HxH Ci->Co k | BN tiles ctas halo | launches  avg us  TFLOP/s  share')
     for key, (n, t, fl) in sorted(agg.items(), key=lambda kv: -kv[1][1]):
-        mode, H, Ci, Co, ks, BN, tiles, ctas, halo = key
-        print(f'{mode} {H:3d}x{H:<3d} {Ci:4d}->{Co:<4d} k{ks} | BN {BN:>3} tiles {tiles:>5} ctas {ctas:>3} halo {halo} | {n:3d}  {t / n:8.1f}  {fl / (t / n) / 1e6:7.1f}  {t / tot * 100:5.1f}%')
+        mode, epi, H, Ci, Co, ks, BN, tiles, ctas, halo = key
+        print(f'{mode} {epi} {H:3d}x{H:<3d} {Ci:4d}->{Co:<4d} k{ks} | BN {BN:>3} tiles {tiles:>5} ctas {ctas:>3} halo {halo} | {n:3d}  {t / n:8.1f}  {fl / (t / n) / 1e6:7.1f}  {t / tot * 100:5.1f}%')
     print(f'total conv_tc time {tot / 1e3:.2f} ms')
+    for e in sorted(set(epis)):
+        n, t = sum(1 for x in epis if x == e), sum(t for t, x in zip(times, epis) if x == e)
+        print(f'EPI {e}: {n} launches, {t / 1e3:.3f} ms')
     sys.exit(0)
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -79,4 +83,6 @@ kname = 'wgrad_tc_kernel' if os.environ.get('XU_KERNEL') == 'wgrad' else 'conv_t
 evs = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and kname in e.name]
 evs.sort(key=lambda e: e.time_range.start)
 for e in evs:
-    print('T', e.device_time)
+    # conv_tc_kernel<BK, EPI, BN>: the second template argument is the epilogue variant (wgrad: '-')
+    m = re.search(r'conv_tc_kernel<\d+, (\d+), \d+>', e.name)
+    print('T', e.device_time, m.group(1) if m else '-')
