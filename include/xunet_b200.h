@@ -185,24 +185,22 @@ int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, 
                          double ema_decay, const float* norm_dev, double max_norm, long long warmup_steps,
                          long long* skipped_dev, void* stream);
 
-/* One ancestral update of sampling.py:128-151 given the 2B-batched model output eps2 =
- * [eps_cond (B,S,S,3); eps_uncond (B,S,S,3)]:  eps=(1+w)eps_c-w eps_u; x0=clip(c_recip z - c_recipm1 eps);
- * z' = c1 x0 + c2 z + sigma * noise.  noise==NULL -> device philox-free hash normal from seed.  z_out may alias z. */
-int xunet_sampler_update(const float* eps2, const float* z, const float* noise, float* z_out, long long n_per_half,
-                         float w, float c_recip, float c_recipm1, float c1, float c2, float sigma,
-                         unsigned long long seed, void* stream);
-
-/* The same step with the schedule on the device, for a per-step CUDA graph (forward + this call + counter increment) that is
- * replayed with no host arithmetic in between (the reference does the schedule math in numpy between two un-jitted model
- * calls, sampling.py:133-151).  table: device (steps, 8) floats, row k (k = 0: first executed step = highest t) =
- * {sqrt_recip_alphas_cumprod, sqrt_recipm1_alphas_cumprod, posterior_mean_coef1, posterior_mean_coef2, sigma (0 at t=0),
- * log-SNR fed to the NEXT forward (sampling.py:151), 0, 0}; pos_dev: device int32 loop position (the caller increments it
- * after the call, in stream order).  z (n = B*S*S*3) is updated in place; the new z is also written to both halves of the
- * next forward's [cond ; uncond] input next_z2 (2n) and next_logsnr2 (batch2 = 2B entries).  Noise: hash normal of
- * (*seed_dev - k), i.e. the caller stores seed(first step) and the per-step seeds count down like the timestep index;
- * seed_dev is a device uint64 so a captured graph can be re-seeded. */
-int xunet_sampler_step_table(const float* eps2, float* z, long long n, float w, const float* table, const int* pos_dev,
-                             const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2, int batch2, void* stream);
+/* One ancestral update of sampling.py:128-151 with the schedule on the device, for a per-step CUDA graph (forward + this call
+ * + counter increment) that is replayed with no host arithmetic in between (the reference does the schedule math in numpy
+ * between two un-jitted model calls, sampling.py:133-151).  Given the 2B-batched model output eps2 =
+ * [eps_cond (B,S,S,3); eps_uncond (B,S,S,3)] and the coefficients of row k = *pos_dev of the table:
+ *     eps = (1+w) eps_c - w eps_u;  x0 = clip(c_recip z - c_recipm1 eps, -1, 1);  z' = c1 x0 + c2 z + sigma * noise_k.
+ * table: device (steps, 8) floats, row k (k = 0: first executed step = highest t) = {c_recip = sqrt_recip_alphas_cumprod,
+ * c_recipm1 = sqrt_recipm1_alphas_cumprod, c1 = posterior_mean_coef1, c2 = posterior_mean_coef2, sigma (0 at t=0), log-SNR
+ * fed to the NEXT forward (sampling.py:151), 0, 0}; pos_dev: device int32 loop position (the caller increments it after the
+ * call, in stream order).  z (n = B*S*S*3) is updated in place; the new z is also written to both halves of the next
+ * forward's [cond ; uncond] input next_z2 (2n) and next_logsnr2 (batch2 = 2B entries).
+ * Noise: noise != NULL: device (steps, n) floats, step k reads noise[k*n .. k*n+n).  noise == NULL: the device hash normal
+ * of (*seed_dev - k), i.e. the caller stores seed(first step) and the per-step seeds count down like the timestep index;
+ * seed_dev (required either way) is a device uint64 so a captured graph can be re-seeded. */
+int xunet_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* table,
+                             const int* pos_dev, const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2,
+                             int batch2, void* stream);
 
 /* Device-side forward diffusion = the per-item work of SceneInstanceDataset.__getitem__ (dataset/data_loader.py:92-110):
  *   t ~ U{0..999};  noise ~ N(0,1);  z = sqrt_ac[t] * x0 + sqrt_1mac[t] * noise;  logsnr = logsnr_schedule_cosine(t/1000);

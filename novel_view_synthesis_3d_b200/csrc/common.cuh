@@ -115,6 +115,15 @@ __host__ __device__ __forceinline__ uint64_t xu_mix64(uint64_t z) {
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
   return z ^ (z >> 31);
 }
+// Standard normal draw i of `seed`: Box-Muller on two hashed 24-bit uniforms (the device noise of the sampler and of the
+// forward diffusion).
+__device__ __forceinline__ float xu_hash_normal(uint64_t seed, uint64_t i) {
+  const uint64_t h1 = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + 2ULL * i + 1ULL);
+  const uint64_t h2 = xu_mix64(h1 + 0xD1B54A32D192ED03ULL);
+  const float u1 = ((float)(h1 >> 40) + 1.f) * (1.0f / 16777216.0f);
+  const float u2 = (float)(h2 >> 40) * (1.0f / 16777216.0f);
+  return sqrtf(-2.f * logf(u1)) * cosf(6.28318530717958647692f * u2);
+}
 // one 64-bit hash serves the 4 consecutive elements idx4*4 .. idx4*4+3 (16-bit uniforms): bit j of the result = keep
 __host__ __device__ __forceinline__ uint32_t xu_keep4(uint64_t seed, int op_index, uint64_t idx4, float rate) {
   const uint64_t z = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + (uint64_t)(op_index + 1) * 0xD1B54A32D192ED03ULL + idx4);

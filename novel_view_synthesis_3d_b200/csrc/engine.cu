@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 104; }
+extern "C" int xunet_version(void) { return 105; }
 
 namespace {
 
@@ -1126,19 +1126,11 @@ extern "C" int xunet_adam_clip_step(float* params, const float* grads, float* m,
   return e == cudaSuccess ? 0 : fail("adam_clip: CUDA error: %s", cudaGetErrorString(e));
 }
 
-extern "C" int xunet_sampler_update(const float* eps2, const float* z, const float* noise, float* z_out, long long n,
-                                    float w, float c_recip, float c_recipm1, float c1, float c2, float sigma,
-                                    unsigned long long seed, void* stream) {
-  if (!eps2 || !z || !z_out || n <= 0) return fail("xunet_sampler_update: bad argument");
-  launch_sampler_update(eps2, z, noise, z_out, n, w, c_recip, c_recipm1, c1, c2, sigma, seed, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("sampler_update: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_sampler_step_table(const float* eps2, float* z, long long n, float w, const float* table, const int* pos_dev,
-                                        const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2, int batch2, void* stream) {
+extern "C" int xunet_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* table,
+                                        const int* pos_dev, const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2,
+                                        int batch2, void* stream) {
   if (!eps2 || !z || !table || !pos_dev || !seed_dev || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0) return fail("xunet_sampler_step_table: bad argument");
-  launch_sampler_step_table(eps2, z, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, (cudaStream_t)stream);
+  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("sampler_step_table: CUDA error: %s", cudaGetErrorString(e));
 }

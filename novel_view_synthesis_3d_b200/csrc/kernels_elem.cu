@@ -1704,41 +1704,14 @@ void launch_grad_global_norm(const float* g, long long n, double grad_scale, dou
   xu_launch(grad_norm_final_kernel, 1, 256, 0, s, scratch, parts, norm_out);
 }
 
-// sampling.py:128-151 elementwise update
-__global__ void sampler_update_kernel(const float* __restrict__ eps2, const float* __restrict__ z,
-                                      const float* __restrict__ noise, float* __restrict__ z_out, long long n, float w,
-                                      float c_recip, float c_recipm1, float c1, float c2, float sigma,
-                                      unsigned long long seed) {
-  xu_grid_dep_sync();
-  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (i >= n) return;
-  const float e = (1.f + w) * eps2[i] - w * eps2[n + i];
-  const float zi = z[i];
-  float x0 = c_recip * zi - c_recipm1 * e;
-  x0 = fminf(fmaxf(x0, -1.f), 1.f);
-  float nz;
-  if (noise != nullptr) nz = noise[i];
-  else {  // Box-Muller on two hashed uniforms
-    uint64_t h1 = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + 2ULL * (uint64_t)i + 1ULL);
-    uint64_t h2 = xu_mix64(h1 + 0xD1B54A32D192ED03ULL);
-    float u1 = ((float)(h1 >> 40) + 1.f) * (1.0f / 16777216.0f);
-    float u2 = (float)(h2 >> 40) * (1.0f / 16777216.0f);
-    nz = sqrtf(-2.f * logf(u1)) * cosf(6.28318530717958647692f * u2);
-  }
-  z_out[i] = c1 * x0 + c2 * zi + sigma * nz;
-}
-void launch_sampler_update(const float* eps2, const float* z, const float* noise, float* z_out, long long n, float w,
-                           float c_recip, float c_recipm1, float c1, float c2, float sigma, unsigned long long seed,
-                           cudaStream_t s) {
-  xu_launch(sampler_update_kernel, cdiv(n, 256), 256, 0, s, eps2, z, noise, z_out, n, w, c_recip, c_recipm1, c1, c2, sigma, seed);
-}
-
 // One ancestral step with the schedule ON THE DEVICE (sampling.py:128-151): the coefficients of loop position k = *pos_dev come
 // from a table (k = 0 is the first executed step = highest t), and the kernel also writes the NEXT forward's inputs (z into
 // both halves of the [cond ; uncond] batch, the lagging log-SNR), so one CUDA graph = forward + this kernel + counter++ is
 // replayed per step with no host arithmetic or copies in between.  tab row: {c_recip, c_recipm1, c1, c2, sigma, logsnr_next, -, -}
-__global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __restrict__ eps2, float* __restrict__ z, long long n,
-                                                                 float w, const float* __restrict__ tab, const int* __restrict__ pos_dev,
+// The noise of step k is noise[k*n .. k*n+n) if `noise` is set, else the hash normal of (*seed_dev - k).
+__global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __restrict__ eps2, float* __restrict__ z,
+                                                                 const float* __restrict__ noise, long long n, float w,
+                                                                 const float* __restrict__ tab, const int* __restrict__ pos_dev,
                                                                  const unsigned long long* __restrict__ seed_dev, float* __restrict__ inp_z,
                                                                  float* __restrict__ inp_logsnr, int B2) {
   xu_grid_dep_sync();
@@ -1751,20 +1724,17 @@ __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __
   const float zi = z[i];
   float x0 = t[0] * zi - t[1] * e;
   x0 = fminf(fmaxf(x0, -1.f), 1.f);
-  const unsigned long long seed = *seed_dev - (unsigned long long)k;     // = seed0 * 1000003 + timestep index, as the host loop
-  uint64_t h1 = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + 2ULL * (uint64_t)i + 1ULL);
-  uint64_t h2 = xu_mix64(h1 + 0xD1B54A32D192ED03ULL);
-  float u1 = ((float)(h1 >> 40) + 1.f) * (1.0f / 16777216.0f);
-  float u2 = (float)(h2 >> 40) * (1.0f / 16777216.0f);
-  const float nz = sqrtf(-2.f * logf(u1)) * cosf(6.28318530717958647692f * u2);
+  const float nz = noise != nullptr ? noise[k * n + i] : xu_hash_normal(*seed_dev - (unsigned long long)k, (uint64_t)i);
   const float zn = t[2] * x0 + t[3] * zi + t[4] * nz;
   z[i] = zn;
   inp_z[i] = zn;
   inp_z[n + i] = zn;
 }
-void launch_sampler_step_table(const float* eps2, float* z, long long n, float w, const float* tab, const int* pos_dev,
-                               const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2, cudaStream_t s) {
-  xu_launch(sampler_step_table_kernel, cdiv(n > B2 ? n : B2, 256), 256, 0, s, eps2, z, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr, B2);
+void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
+                               const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
+                               cudaStream_t s) {
+  xu_launch(sampler_step_table_kernel, cdiv(n > B2 ? n : B2, 256), 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z,
+            inp_logsnr, B2);
 }
 
 // dataset/data_loader.py:92-110 on the device
@@ -1780,15 +1750,7 @@ __global__ void __launch_bounds__(256) forward_diffusion_kernel(const float* __r
   const int b = (int)(idx / per);
   const uint64_t hb = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + 0xABCDEF0123ULL + (uint64_t)b);
   const int t = t_in != nullptr ? t_in[b] : (int)(hb % 1000ULL);
-  float nz;
-  if (noise_in != nullptr) nz = noise_in[idx];
-  else {
-    const uint64_t h1 = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + 2ULL * (uint64_t)idx + 1ULL);
-    const uint64_t h2 = xu_mix64(h1 + 0xD1B54A32D192ED03ULL);
-    const float u1 = ((float)(h1 >> 40) + 1.f) * (1.0f / 16777216.0f);
-    const float u2 = (float)(h2 >> 40) * (1.0f / 16777216.0f);
-    nz = sqrtf(-2.f * logf(u1)) * cosf(6.28318530717958647692f * u2);
-  }
+  const float nz = noise_in != nullptr ? noise_in[idx] : xu_hash_normal(seed, (uint64_t)idx);
   z[idx] = sqrt_ac[t] * x0[idx] + sqrt_1mac[t] * nz;
   if (noise_out != nullptr) noise_out[idx] = nz;
   if (idx == (long long)b * per) {

@@ -8,7 +8,6 @@ Reference behaviour (steps=1000, w=3): per step two model evaluations (cond_mask
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
 
 import numpy as np
 import torch
@@ -63,6 +62,10 @@ class Schedule:
 
 
 class Sampler:
+    """z, the forward's z / log-SNR inputs, the loop position, the noise seed and the coefficient table all live on the device,
+    so one sampler step is the 2B-batch forward, `xunet_sampler_step_table` and pos += 1, with no host arithmetic in between.
+    use_graph=True replays that step as one CUDA graph; use_graph=False issues the same calls eagerly."""
+
     def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000, w: float = 3.0,
                  use_graph: bool = True):
         self.model, self.B, self.S, self.w = model, batch_size, img_sidelength, float(w)
@@ -73,46 +76,16 @@ class Sampler:
         self.dev = self.eng.device
         self.z = torch.zeros(batch_size, img_sidelength, img_sidelength, 3, dtype=torch.float32, device=self.dev)
         self.use_graph = use_graph
-        self.graph = None
-        self._tab = None
+        self._tab = None            # (steps, 8) coefficient table on the device
+        self._noise = None          # (steps, B*S*S*3) explicit noise on the device
+        self._graphs = {}           # (static conditioning, explicit noise) -> the captured step
         self._pos = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self._seed_base = torch.zeros(1, dtype=torch.int64, device=self.dev)
-        self.graph_step = None
-
-    def _forward(self, first: bool):
-        # poses / params are constant over the loop: only the first step computes rays, posenc, pose convs, weight shadows
-        if first:
-            self.lib.xunet_set_static_conditioning(self.eng.h, 0)
-            self.eng.forward(self.flat, train=False)
-            self.lib.xunet_set_static_conditioning(self.eng.h, 1)
-            return
-        if not self.use_graph:
-            self.eng.forward(self.flat, train=False)
-            return
-        if self.graph is None:
-            torch.cuda.synchronize(self.dev)
-            st = torch.cuda.Stream(device=self.dev)
-            with torch.cuda.stream(st):
-                self.eng.forward(self.flat, train=False)
-                st.synchronize()
-                self.graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(self.graph, stream=st):
-                    self.eng.forward(self.flat, train=False)
-            torch.cuda.synchronize(self.dev)
-        self.graph.replay()
 
     def capture(self, batch: dict) -> None:
-        """Builds the static-conditioning state and the per-step CUDA graph without running the loop (benchmarks warm up
-        with this instead of a full `steps`-long sample)."""
-        if self.use_graph:
-            self.sample(batch, seed=0, _max_steps=3)
-            return
-        saved = self.sched
-        try:
-            self.sched = Schedule(3)
-            self.sample(batch, seed=0)
-        finally:
-            self.sched = saved
+        """Runs the first 3 steps of a sample: builds the static-conditioning state and, with use_graph, the per-step CUDA
+        graph (benchmarks warm up with this instead of a full `steps`-long sample)."""
+        self.sample(batch, seed=0, _max_steps=3)
 
     def sample(self, batch: dict, *, seed: int = 0, z_init=None, noises=None, _max_steps=None) -> torch.Tensor:
         """Generates the target view for each (source image, pose pair) in `batch` (keys as data_loader.py:102-113).
@@ -126,97 +99,86 @@ class Sampler:
         dup = {k: np.concatenate([np.asarray(src[k], dtype=np.float32)] * 2, axis=0) for k in BATCH_KEYS}
         mask = np.concatenate([np.ones(B, np.float32), np.zeros(B, np.float32)])
         e.load_inputs(dup, cond_mask=mask)
+        steps = self._load_schedule()
+        self._start_chain(seed, z_init, noises)
+        self._run(steps if _max_steps is None else min(_max_steps, steps), noises is not None, static=True)
+        return self.z.clone()
+
+    def _load_schedule(self) -> int:
+        """Writes the coefficient table of `self.sched` (callers may have edited it since the last call) to the device and
+        returns its number of steps.  Row k = loop position k = timestep index len-1-k."""
+        sc = self.sched
+        i = np.arange(len(sc) - 1, -1, -1)
+        sigma = np.where(i == 0, 0.0, np.exp(0.5 * sc.posterior_log_variance_clipped[i]))         # sampling.py:142-148
+        zero = np.zeros(len(i))
+        rows = np.stack([sc.sqrt_recip_alphas_cumprod[i], sc.sqrt_recipm1_alphas_cumprod[i], sc.posterior_mean_coef1[i],
+                         sc.posterior_mean_coef2[i], sigma, logsnr_schedule_cosine(sc.timesteps[i] / 1000.0), zero, zero], 1)
+        if self._tab is None or len(self._tab) != len(i):
+            # the captured graphs hold the table and noise pointers: reallocate (and recapture) only when the length changes
+            self._tab = torch.empty(len(i), 8, dtype=torch.float32, device=self.dev)
+            self._noise = None
+            self._graphs = {}
+        self._tab.copy_(torch.as_tensor(rows, dtype=torch.float32))
+        return len(i)
+
+    def _start_chain(self, seed: int, z_init, noises) -> None:
+        """z <- z_init, or N(0, 1) from `seed` (sampling.py:125); the first forward's inputs z and log-SNR = -20
+        (sampling.py:126); the noise of step k: noises[k], or the hash normal of seed * 1000003 + timestep index."""
+        B, steps, e = self.B, len(self._tab), self.eng
         if z_init is None:
             g = torch.Generator(device=self.dev).manual_seed(seed)
-            self.z.copy_(torch.randn(self.z.shape, generator=g, device=self.dev))       # sampling.py:125
+            self.z.copy_(torch.randn(self.z.shape, generator=g, device=self.dev))
         else:
             self.z.copy_(torch.as_tensor(np.asarray(z_init), dtype=torch.float32).to(self.dev))
-        logsnr = -20.0                                                                  # sampling.py:126
-        sc = self.sched
-        n = B * S * S * 3
-        if noises is None and self.use_graph:
-            return self._sample_device_schedule(seed, _max_steps)
-        try:
-            for i in range(len(sc) - 1, -1, -1):
-                first = i == len(sc) - 1
-                e.inp['z'][:B].copy_(self.z)
-                e.inp['z'][B:].copy_(self.z)
-                e.inp['logsnr'].fill_(float(logsnr))
-                self._forward(first)
-                sigma = 0.0 if i == 0 else float(np.exp(0.5 * sc.posterior_log_variance_clipped[i]))   # sampling.py:142-148
-                noise_ptr = None
-                if noises is not None:
-                    nz = torch.as_tensor(np.asarray(noises[len(sc) - 1 - i]), dtype=torch.float32).to(self.dev).contiguous()
-                    noise_ptr = nz.data_ptr()
-                st = torch.cuda.current_stream(self.dev).cuda_stream
-                _lib.check(self.lib.xunet_sampler_update(e.eps.data_ptr(), self.z.data_ptr(), noise_ptr, self.z.data_ptr(), n,
-                                                         self.w, float(sc.sqrt_recip_alphas_cumprod[i]),
-                                                         float(sc.sqrt_recipm1_alphas_cumprod[i]),
-                                                         float(sc.posterior_mean_coef1[i]), float(sc.posterior_mean_coef2[i]),
-                                                         sigma, (seed * 1000003 + i) & 0xFFFFFFFFFFFFFFFF, st), 'sampler_update')
-                logsnr = logsnr_schedule_cosine(sc.timesteps[i] / 1000.0)                   # sampling.py:151
-        finally:
-            # a failure mid-loop must not leave the shared engine reusing stale pose embeddings / weight shadows
-            self.lib.xunet_set_static_conditioning(e.h, 0)
-        return self.z.clone()
-
-
-    # ---- device-side schedule: ONE graph per step (forward + ancestral update + counter), nothing else in the loop ------
-    def _table(self) -> torch.Tensor:
-        sc = self.sched
-        key = (len(sc), int(sc.timesteps[-1]))
-        if self._tab is None or self._tab[0] != key:
-            rows = []
-            for i in range(len(sc) - 1, -1, -1):           # loop position k = len-1-i
-                sigma = 0.0 if i == 0 else float(np.exp(0.5 * sc.posterior_log_variance_clipped[i]))   # sampling.py:142-148
-                rows.append([sc.sqrt_recip_alphas_cumprod[i], sc.sqrt_recipm1_alphas_cumprod[i], sc.posterior_mean_coef1[i],
-                             sc.posterior_mean_coef2[i], sigma, logsnr_schedule_cosine(sc.timesteps[i] / 1000.0), 0.0, 0.0])
-            self._tab = (key, torch.as_tensor(np.asarray(rows, dtype=np.float64), dtype=torch.float32).to(self.dev).contiguous())
-            self.graph_step = None          # the table pointer is baked into the captured graph
-        return self._tab[1]
-
-    def _device_step(self):
-        e = self.eng
-        st = torch.cuda.current_stream(self.dev).cuda_stream
-        _lib.check(self.lib.xunet_sampler_step_table(e.eps.data_ptr(), self.z.data_ptr(), self.B * self.S * self.S * 3, self.w,
-                                                     self._table().data_ptr(), self._pos.data_ptr(), self._seed_base.data_ptr(),
-                                                     e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(), 2 * self.B, st),
-                   'sampler_step_table')
-        self._pos.add_(1)
-
-    def _sample_device_schedule(self, seed: int, max_steps: Optional[int] = None) -> torch.Tensor:
-        """z, the forward's z / log-SNR inputs, the schedule position, the noise seed and the coefficient table all live on
-        the device; step 0 runs eagerly (it builds rays, pose embeddings and weight shadows), steps 1.. replay one graph each."""
-        B, e = self.B, self.eng
-        steps = len(self.sched) if max_steps is None else min(max_steps, len(self.sched))
-        self._seed_base.fill_((seed * 1000003 + len(self.sched) - 1) & 0x7FFFFFFFFFFFFFFF)    # same per-step seeds as the host loop
-        self._table()
-        self._pos.zero_()
         e.inp['z'][:B].copy_(self.z)
         e.inp['z'][B:].copy_(self.z)
-        e.inp['logsnr'].fill_(-20.0)                                                    # sampling.py:126
+        e.inp['logsnr'].fill_(-20.0)
+        self._seed_base.fill_((seed * 1000003 + steps - 1) & 0x7FFFFFFFFFFFFFFF)    # the kernel subtracts the loop position
+        if noises is not None:
+            if self._noise is None:
+                self._noise = torch.empty(steps, self.z.numel(), dtype=torch.float32, device=self.dev)
+            self._noise.copy_(torch.as_tensor(np.asarray(noises[:steps]), dtype=torch.float32).reshape(steps, self.z.numel()))
+
+    def _run(self, steps: int, noise: bool, static: bool, set_view=None) -> None:
+        """The sampling loop from loop position 0: per step set_view(k) (if given), the forward, the table step and pos += 1.
+        Step 0 runs eagerly, so every kernel has run once before a graph is captured.  static: poses, K, cond_mask and
+        params stay fixed, so after step 0 the forwards reuse its rays, pose embeddings and weight shadows."""
+        h = self.eng.h
+        self._pos.zero_()
         try:
-            self.lib.xunet_set_static_conditioning(e.h, 0)
-            e.forward(self.flat, train=False)
-            self.lib.xunet_set_static_conditioning(e.h, 1)
-            self._device_step()
-            if steps > 1 and self.graph_step is None:
-                torch.cuda.synchronize(self.dev)
-                pos0 = self._pos.clone()
-                st = torch.cuda.Stream(device=self.dev)
-                with torch.cuda.stream(st):
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, stream=st):
-                        e.forward(self.flat, train=False)
-                        self._device_step()
-                torch.cuda.synchronize(self.dev)
-                self._pos.copy_(pos0)
-                self.graph_step = g
-            for _ in range(steps - 1):
-                self.graph_step.replay()
+            self.lib.xunet_set_static_conditioning(h, 0)
+            for k in range(steps):
+                if set_view is not None:
+                    set_view(k)
+                if k > 0 and self.use_graph:
+                    self._graph(static, noise).replay()
+                else:
+                    self._step(noise)
+                if static and k == 0:
+                    self.lib.xunet_set_static_conditioning(h, 1)
         finally:
-            self.lib.xunet_set_static_conditioning(e.h, 0)
-        return self.z.clone()
+            # a failure mid-loop must not leave the shared engine reusing stale pose embeddings / weight shadows
+            self.lib.xunet_set_static_conditioning(h, 0)
+
+    def _step(self, noise: bool) -> None:
+        e = self.eng
+        e.forward(self.flat, train=False)
+        st = torch.cuda.current_stream(self.dev).cuda_stream
+        _lib.check(self.lib.xunet_sampler_step_table(e.eps.data_ptr(), self.z.data_ptr(), self._noise.data_ptr() if noise else None,
+                                                     self.z.numel(), self.w, self._tab.data_ptr(), self._pos.data_ptr(),
+                                                     self._seed_base.data_ptr(), e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(),
+                                                     2 * self.B, st), 'sampler_step_table')
+        self._pos.add_(1)
+
+    def _graph(self, static: bool, noise: bool) -> torch.cuda.CUDAGraph:
+        """The captured step; static conditioning and explicit noise both change what it launches."""
+        key = (static, noise)
+        if key not in self._graphs:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=torch.cuda.Stream(device=self.dev)):
+                self._step(noise)
+            self._graphs[key] = g
+        return self._graphs[key]
 
     # ---- stochastic conditioning (3DiM, Watson et al. 2022, section 3.2; the reference implements only k = 1) ---------
     def sample_views(self, views, poses, K, target_poses, *, seed: int = 0, condition_on_generated: bool = True,
@@ -229,11 +191,11 @@ class Sampler:
         one view drawn uniformly from the pool (the k sources plus -- if condition_on_generated -- the targets generated
         so far), exactly as the paper's sampler; one 2B-batch forward per step ([cond ; uncond], guidance weight w) and
         the same posterior update as `sample()`.  The pool lives on the device; a step only copies the chosen view and
-        its pose into the engine's static input buffers, so the per-step CUDA graph is shared with `sample()`'s
-        non-static path.  z_init (m, B,S,S,3) / noises (m, steps, B,S,S,3) make a run reproducible against the oracle;
-        with one source, one target and the same seed the result equals `sample()`.
+        its pose into the engine's input buffers before the step, which runs with the full forward (static conditioning
+        off).  z_init (m, B,S,S,3) / noises (m, steps, B,S,S,3) make a run reproducible against the oracle; with one
+        source, one target and the same seed the result equals `sample()`.
         Returns (B, m, S, S, 3) [and the (m, steps) pool indices that were drawn]."""
-        B, S, e = self.B, self.S, self.eng
+        B, e = self.B, self.eng
         dev = self.dev
         f32 = lambda a: torch.as_tensor(np.asarray(a), dtype=torch.float32).to(dev)
         pool_x = [v for v in f32(views).unbind(1)]                     # each (B,S,S,3)
@@ -243,43 +205,24 @@ class Sampler:
         m = tR.shape[1]
         Kd = f32(K)
         rng = np.random.RandomState(seed)
-        sc = self.sched
-        n = B * S * S * 3
+        steps = self._load_schedule()
         e.inp['K'].copy_(torch.cat([Kd, Kd], 0).reshape(e.inp['K'].shape))
         e.inp['cond_mask'].copy_(torch.cat([torch.ones(B, device=dev), torch.zeros(B, device=dev)]))
-        self.lib.xunet_set_static_conditioning(e.h, 0)                  # the conditioning view changes every step
         outs, choices = [], []
         for j in range(m):
             e.inp['R2'].copy_(torch.cat([tR[:, j], tR[:, j]], 0).reshape(e.inp['R2'].shape))
             e.inp['t2'].copy_(torch.cat([tt[:, j], tt[:, j]], 0).reshape(e.inp['t2'].shape))
-            if z_init is None:
-                g = torch.Generator(device=dev).manual_seed(seed + 7919 * j)
-                self.z.copy_(torch.randn(self.z.shape, generator=g, device=dev))
-            else:
-                self.z.copy_(f32(z_init[j]))
-            logsnr = -20.0
+            self._start_chain(seed + 7919 * j, None if z_init is None else z_init[j], None if noises is None else noises[j])
             row = []
-            for i in range(len(sc) - 1, -1, -1):
+
+            def set_view(k):
                 c = int(rng.randint(len(pool_x)))
                 row.append(c)
                 e.inp['x'].copy_(torch.cat([pool_x[c], pool_x[c]], 0).reshape(e.inp['x'].shape))
                 e.inp['R1'].copy_(torch.cat([pool_R[c], pool_R[c]], 0).reshape(e.inp['R1'].shape))
                 e.inp['t1'].copy_(torch.cat([pool_t[c], pool_t[c]], 0).reshape(e.inp['t1'].shape))
-                e.inp['z'][:B].copy_(self.z)
-                e.inp['z'][B:].copy_(self.z)
-                e.inp['logsnr'].fill_(float(logsnr))
-                self._forward_dynamic()
-                sigma = 0.0 if i == 0 else float(np.exp(0.5 * sc.posterior_log_variance_clipped[i]))
-                st = torch.cuda.current_stream(dev).cuda_stream
-                nz = f32(noises[j][len(sc) - 1 - i]).contiguous() if noises is not None else None
-                _lib.check(self.lib.xunet_sampler_update(e.eps.data_ptr(), self.z.data_ptr(), nz.data_ptr() if nz is not None else None,
-                                                         self.z.data_ptr(), n, self.w,
-                                                         float(sc.sqrt_recip_alphas_cumprod[i]),
-                                                         float(sc.sqrt_recipm1_alphas_cumprod[i]),
-                                                         float(sc.posterior_mean_coef1[i]), float(sc.posterior_mean_coef2[i]),
-                                                         sigma, ((seed + 7919 * j) * 1000003 + i) & 0xFFFFFFFFFFFFFFFF, st),
-                           'sampler_update')
-                logsnr = logsnr_schedule_cosine(sc.timesteps[i] / 1000.0)
+
+            self._run(steps, noises is not None, static=False, set_view=set_view)
             out = self.z.clone()
             outs.append(out)
             choices.append(row)
@@ -287,23 +230,6 @@ class Sampler:
                 pool_x.append(out); pool_R.append(tR[:, j]); pool_t.append(tt[:, j])
         res = torch.stack(outs, 1)
         return (res, np.asarray(choices)) if return_choices else res
-
-    def _forward_dynamic(self):
-        """Full forward (rays, posenc, pose convs recomputed): graph-captured once, replayed per step."""
-        if not self.use_graph:
-            self.eng.forward(self.flat, train=False)
-            return
-        if getattr(self, 'graph_dyn', None) is None:
-            torch.cuda.synchronize(self.dev)
-            st = torch.cuda.Stream(device=self.dev)
-            with torch.cuda.stream(st):
-                self.eng.forward(self.flat, train=False)
-                st.synchronize()
-                self.graph_dyn = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(self.graph_dyn, stream=st):
-                    self.eng.forward(self.flat, train=False)
-            torch.cuda.synchronize(self.dev)
-        self.graph_dyn.replay()
 
 
 def save_view(path: str, img) -> None:

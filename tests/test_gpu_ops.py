@@ -185,25 +185,42 @@ def test_dropout_mask_matches_numpy_replica(lib):
     assert np.array_equal(out.cpu().numpy() > 0.5, keep_mask(123456789, 5, (n,), 0.1))
 
 
-def test_sampler_update_matches_oracle(lib):
+def test_sampler_step_table_matches_oracle(lib):
+    """Loop positions k = 0..3 on table rows t = 999, 500, 1, 0, with explicit noise laid out (steps, n): step k must use row
+    k and noise row k, and hand its z and row k's log-SNR to the next forward."""
     g = torch.Generator().manual_seed(4)
     tab = R.schedule_tables()
-    n = 2 * 8 * 8 * 3
-    for t in (999, 500, 1, 0):
-        ec, eu, z, nz = [torch.randn(n, generator=g, dtype=torch.float64) for _ in range(4)]
-        ref, _ = R.sampler_step(ec, eu, z, t, nz, tab)
+    ts = (999, 500, 1, 0)
+    n, b2 = 2 * 8 * 8 * 3, 4
+    rows = [[tab['sqrt_recip_alphas_cumprod'][t], tab['sqrt_recipm1_alphas_cumprod'][t], tab['posterior_mean_coef1'][t],
+             tab['posterior_mean_coef2'][t], 0.0 if t == 0 else math.exp(0.5 * tab['posterior_log_variance_clipped'][t]),
+             R.logsnr_schedule_cosine(t / 1000.0), 0.0, 0.0] for t in ts]
+    tabd = torch.tensor(rows, dtype=torch.float64).float().cuda()
+    noise = torch.randn(len(ts), n, generator=g, dtype=torch.float64)
+    nd = noise.float().cuda()
+    pos = torch.zeros(1, dtype=torch.int32, device='cuda')
+    seed = torch.zeros(1, dtype=torch.int64, device='cuda')
+    next_z2, next_logsnr2 = torch.zeros(2 * n, device='cuda'), torch.zeros(b2, device='cuda')
+    for k, t in enumerate(ts):
+        ec, eu, z = [torch.randn(n, generator=g, dtype=torch.float64) for _ in range(3)]
+        ref, _ = R.sampler_step(ec, eu, z, t, noise[k], tab)
         eps2 = torch.cat([ec, eu]).float().cuda()
-        zd, nd = z.float().cuda(), nz.float().cuda()
-        sigma = 0.0 if t == 0 else math.exp(0.5 * tab['posterior_log_variance_clipped'][t])
-        assert lib.xunet_sampler_update(eps2.data_ptr(), zd.data_ptr(), nd.data_ptr(), zd.data_ptr(), n, 3.0,
-                                        tab['sqrt_recip_alphas_cumprod'][t], tab['sqrt_recipm1_alphas_cumprod'][t],
-                                        tab['posterior_mean_coef1'][t], tab['posterior_mean_coef2'][t], sigma, 0, _stream()) == 0
+        zd = z.float().cuda()
+        assert lib.xunet_sampler_step_table(eps2.data_ptr(), zd.data_ptr(), nd.data_ptr(), n, 3.0, tabd.data_ptr(), pos.data_ptr(),
+                                            seed.data_ptr(), next_z2.data_ptr(), next_logsnr2.data_ptr(), b2, _stream()) == 0, \
+            lib.xunet_last_error()
+        pos.add_(1)
         # at t=999 sqrt(1/abar) ~ 6e4 amplifies fp32 rounding before the clip; compare on the clipped scale
         assert float((zd.double().cpu() - ref).abs().max()) < 5e-3 if t == 999 else rel_l2(zd, ref) < 1e-5
-    # device-side noise: unit variance, zero mean
+        assert torch.equal(next_z2[:n], zd) and torch.equal(next_z2[n:], zd)
+        assert bool((next_logsnr2 == tabd[k, 5]).all())
+    # device-side noise (noise == NULL): unit variance, zero mean
     big = 1 << 20
-    eps2 = torch.zeros(2 * big, device='cuda'); zz = torch.zeros(big, device='cuda')
-    lib.xunet_sampler_update(eps2.data_ptr(), zz.data_ptr(), None, zz.data_ptr(), big, 3.0, 1.0, 0.0, 0.0, 0.0, 1.0, 77, _stream())
+    eps2 = torch.zeros(2 * big, device='cuda'); zz = torch.zeros(big, device='cuda'); zz2 = torch.zeros(2 * big, device='cuda')
+    unit = torch.tensor([[1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0]], device='cuda')      # z' = 1 * noise
+    pos.zero_(); seed.fill_(77)
+    assert lib.xunet_sampler_step_table(eps2.data_ptr(), zz.data_ptr(), None, big, 3.0, unit.data_ptr(), pos.data_ptr(),
+                                        seed.data_ptr(), zz2.data_ptr(), next_logsnr2.data_ptr(), b2, _stream()) == 0
     assert abs(float(zz.mean())) < 5e-3 and abs(float(zz.std()) - 1.0) < 5e-3
 
 
