@@ -1,0 +1,134 @@
+"""Scores sampled views against held-out ground truth on SRN: PSNR and SSIM per view (novel_view_synthesis_3d_b200.metrics,
+computed on the GPU from the sampler's output), following the single-view protocol of pixelNeRF that 3DiM reports: each
+instance is conditioned on one source view (view 64 by default) and every scored target view is generated from it.
+
+    python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --steps 256 --w 3 \\
+        --source-view 64 --targets 10 --max-instances 20 --views-in-flight 8 --mode independent --out eval/
+
+Modes:
+  independent  each target is sampled from the source alone (Sampler.sample, the reference's k = 1 sampler); the targets
+               of one instance are batched --views-in-flight at a time.
+  stochastic   3DiM's stochastic conditioning (Sampler.sample_views): the source is the pool and the targets are generated
+               in order, each step conditioned on a random view of the pool (the source and the targets generated so far);
+               instances are batched --views-in-flight at a time.
+Writes out/metrics.jsonl (one {instance, view, psnr, ssim} line per scored view) and out/summary.json (mean PSNR, mean SSIM,
+the number of views and the arguments), prints the summary as the last line of stdout, and with --save-views writes each
+generated view as out/views/<instance>_<view>.png.  Seeds derive from --seed, so equal arguments give equal files.
+"""
+import argparse
+import json
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
+
+import novel_view_synthesis_3d_b200 as P
+from novel_view_synthesis_3d_b200.srn_data import SRNScenes
+
+
+def select_targets(n_views: int, source: int, count: int) -> list:
+    """The target views of an instance with n_views views: `count` views spaced evenly over the views other than `source`,
+    in increasing order; all of them when count is 0 or at least their number."""
+    rest = [v for v in range(n_views) if v != source]
+    if count <= 0 or count >= len(rest):
+        return rest
+    return [rest[i] for i in np.linspace(0, len(rest), num=count, endpoint=False, dtype=int)]
+
+
+def _pad(a: np.ndarray, n: int) -> np.ndarray:
+    """Rows of `a` padded to n by repeating the last one (the sampler's batch is fixed; padding rows are not scored)."""
+    return np.concatenate([a, np.repeat(a[-1:], n - len(a), axis=0)]) if len(a) < n else a
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('folder')
+    ap.add_argument('--ckpt', default='checkpoints')
+    ap.add_argument('--prefix', default='model', help="checkpoint prefix: 'ema' scores the weight EMA of train_srn.py")
+    ap.add_argument('--side', type=int, default=64)
+    ap.add_argument('--steps', type=int, default=256)
+    ap.add_argument('--w', type=float, default=3.0)
+    ap.add_argument('--source-view', type=int, default=64, help='conditioning view of every instance (pixelNeRF / 3DiM: 64)')
+    ap.add_argument('--targets', type=int, default=0, help='target views per instance, spaced evenly; 0 = all other views')
+    ap.add_argument('--max-instances', type=int, default=-1, help='score the first N instances of the sorted list')
+    ap.add_argument('--views-in-flight', type=int, default=8, help='sampler batch size')
+    ap.add_argument('--mode', choices=('independent', 'stochastic'), default='independent')
+    ap.add_argument('--seed', type=int, default=0)
+    ap.add_argument('--out', default='eval')
+    ap.add_argument('--save-views', action='store_true')
+    a = ap.parse_args()
+    if a.views_in_flight < 1:
+        ap.error('--views-in-flight must be >= 1')
+    params = P.checkpoint.restore_checkpoint(a.ckpt, prefix=a.prefix)
+    if params is None:
+        raise FileNotFoundError('Checkpoint does not exist')
+    ds = SRNScenes(a.folder, img_sidelength=a.side, max_num_instances=a.max_instances)
+    insts = []
+    for i in range(len(ds.instances)):
+        n = len(ds.instances[i]['imgs'])
+        if a.source_view < 0 or a.source_view >= n:
+            raise SystemExit(f"instance {ds.instances[i]['name']} has {n} views; --source-view {a.source_view} does not exist")
+        insts.append((i, select_targets(n, a.source_view, a.targets)))
+    B = a.views_in_flight
+    sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w)
+    os.makedirs(a.out, exist_ok=True)
+    if a.save_views:
+        os.makedirs(os.path.join(a.out, 'views'), exist_ok=True)
+    records = []
+
+    def score(name, views, gen, truth):
+        m = P.image_metrics(gen, truth)
+        for v, psnr, ssim in zip(views, m['psnr'].tolist(), m['ssim'].tolist()):
+            records.append(dict(instance=name, view=int(v), psnr=psnr, ssim=ssim))
+        if a.save_views:
+            for v, img in zip(views, gen.cpu().numpy()):
+                P.sampling.save_view(os.path.join(a.out, 'views', f'{name}_{v:06d}.png'), img)
+
+    if a.mode == 'independent':
+        for i, targets in insts:
+            d = ds.instance_views(i)
+            s = a.source_view
+            for c, j0 in enumerate(range(0, len(targets), B)):
+                tv = targets[j0:j0 + B]
+                n = len(tv)
+                batch = dict(x=_pad(np.repeat(d['x'][s:s + 1], n, 0), B), R1=_pad(np.repeat(d['R'][s:s + 1], n, 0), B),
+                             t1=_pad(np.repeat(d['t'][s:s + 1], n, 0), B), R2=_pad(d['R'][tv], B), t2=_pad(d['t'][tv], B),
+                             K=np.repeat(d['K'][None], B, 0))
+                gen = sampler.sample(batch, seed=(a.seed * 1000003 + i) * 1009 + c)
+                score(d['name'], tv, gen[:n], d['x'][tv])
+    else:
+        # a batch holds up to B consecutive instances with the same number of targets (one row per instance)
+        groups = []
+        for i, targets in insts:
+            if groups and len(groups[-1]) < B and len(groups[-1][0][1]) == len(targets):
+                groups[-1].append((i, targets))
+            else:
+                groups.append([(i, targets)])
+        for g in groups:
+            if not g[0][1]:
+                continue
+            ds_g =[(ds.instance_views(i), t) for i, t in g]
+            s, n = a.source_view, len(g)
+            src = _pad(np.stack([d['x'][s:s + 1] for d, _ in ds_g]), B)
+            poses = {'R': _pad(np.stack([d['R'][s:s + 1] for d, _ in ds_g]), B),
+                     't': _pad(np.stack([d['t'][s:s + 1] for d, _ in ds_g]), B)}
+            tposes = {'R': _pad(np.stack([d['R'][t] for d, t in ds_g]), B), 't': _pad(np.stack([d['t'][t] for d, t in ds_g]), B)}
+            K = _pad(np.stack([d['K'] for d, _ in ds_g]), B)
+            gen = sampler.sample_views(src, poses, K, tposes, seed=a.seed * 1000003 + g[0][0])
+            for r, (d, t) in enumerate(ds_g):
+                score(d['name'], t, gen[r], d['x'][t])
+
+    with open(os.path.join(a.out, 'metrics.jsonl'), 'w') as fh:
+        for rec in records:
+            fh.write(json.dumps(rec) + '\n')
+    summary = dict(mean_psnr=float(np.mean([r['psnr'] for r in records])) if records else float('nan'),
+                   mean_ssim=float(np.mean([r['ssim'] for r in records])) if records else float('nan'),
+                   n_views=len(records), args=vars(a))
+    with open(os.path.join(a.out, 'summary.json'), 'w') as fh:
+        json.dump(summary, fh, indent=1)
+    print(json.dumps(summary))
+
+
+if __name__ == '__main__':
+    main()

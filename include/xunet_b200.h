@@ -216,6 +216,26 @@ int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t
 int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,
                        void* stream);
 
+/* Image-quality metrics of generated views against ground truth (3DiM reports PSNR and SSIM on SRN).
+ * pred, target: device (B, S, S, 3) fp32 NHWC in [-1, 1] (the sampler's output convention).  Each value is mapped to
+ * u = clamp((v + 1) / 2, 0, 1); then, per image b:
+ *   mse_out[b]  = mean over the S*S*3 values of (u_pred - u_target)^2;
+ *   psnr_out[b] = -10 log10(mse_b)  (data range 1; +inf when mse_b == 0);
+ *   ssim_out[b] = SSIM of Wang et al. 2004 with an 11x11 Gaussian window: 1-D weights exp(-i^2 / (2 * 1.5^2)), i = -5..5,
+ *                 normalised to sum 1, their outer product in 2-D.  Per channel, at each of the (S-10)^2 pixels whose window
+ *                 lies inside the image (no padding), with the window-weighted (population) moments mu_p, mu_t, sp2, st2, spt:
+ *                   s = (2 mu_p mu_t + C1)(2 spt + C2) / ((mu_p^2 + mu_t^2 + C1)(sp2 + st2 + C2)),  C1 = 0.01^2, C2 = 0.03^2;
+ *                 ssim_b is the mean of s over the 3 channels and those pixels.  This equals skimage's
+ *                 structural_similarity(channel_axis=-1, data_range=1, gaussian_weights=True, sigma=1.5,
+ *                 use_sample_covariance=False).
+ * mse_out, psnr_out, ssim_out: device, B floats each.  Moments and sums are fp64, reduced in an order fixed by S alone (one CTA
+ * per image, no atomics), so an image's three values have the same bits alone or at any position of any batch.  One launch; no
+ * allocation, no host sync, graph-capturable.  Errors: a NULL pointer, B < 1, S < 11 or S > XUNET_METRICS_MAX_SIDE (the
+ * shared-memory ring of filtered rows is sized for it). */
+#define XUNET_METRICS_MAX_SIDE 256
+int xunet_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
+                        float* ssim_out, void* stream);
+
 /* ---- operator-level entry points (parity tests / micro-benchmarks of single kernels) ----
  * dtype as above; tensors channels-last (N,H,W,C). */
 int xunet_op_conv(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y,

@@ -3,10 +3,12 @@ shiveshkhaitan/novel_view_synthesis_3d, rebuilt H100-native (hand-written sm_90a
 from .xunet import XUNet, XUNetConfig, SMALL, FULL_3DIM, ParamTree, Engine
 from .train import (TrainState, Adam, AdamState, create_train_state, create_sample_data, apply_model, update_model,
                     TrainStep)
-from . import checkpoint, sampling, srn_data
+from . import checkpoint, metrics, sampling, srn_data
 from .diffusion import ForwardDiffusion
+from .metrics import image_metrics
 from .sampling import Sampler, Schedule, cosine_beta_schedule, logsnr_schedule_cosine
 
 __all__ = ['XUNet', 'XUNetConfig', 'SMALL', 'FULL_3DIM', 'ParamTree', 'Engine', 'TrainState', 'Adam', 'AdamState',
            'create_train_state', 'create_sample_data', 'apply_model', 'update_model', 'TrainStep', 'Sampler',
-           'Schedule', 'cosine_beta_schedule', 'logsnr_schedule_cosine', 'checkpoint', 'ForwardDiffusion']
+           'Schedule', 'cosine_beta_schedule', 'logsnr_schedule_cosine', 'checkpoint', 'ForwardDiffusion', 'metrics',
+           'image_metrics']

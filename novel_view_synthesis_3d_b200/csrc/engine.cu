@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 105; }
+extern "C" int xunet_version(void) { return 106; }
 
 namespace {
 
@@ -1151,6 +1151,17 @@ extern "C" int xunet_dropout_mask(float* mask_out, long long n, int op_index, un
   launch_dropout_mask(mask_out, n, op_index, seed, rate, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("dropout_mask: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
+                                   float* ssim_out, void* stream) {
+  if (!pred || !target || !mse_out || !psnr_out || !ssim_out) return fail("xunet_image_metrics: NULL pointer argument");
+  if (B < 1) return fail("xunet_image_metrics: B = %d, need B >= 1", B);
+  if (S < 11 || S > XUNET_METRICS_MAX_SIDE)
+    return fail("xunet_image_metrics: S = %d outside [11, %d]", S, XUNET_METRICS_MAX_SIDE);
+  launch_image_metrics(pred, target, B, S, mse_out, psnr_out, ssim_out, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("image_metrics: CUDA error: %s", cudaGetErrorString(e));
 }
 
 // ---- operator-level entry points ----------------------------------------------------------------------

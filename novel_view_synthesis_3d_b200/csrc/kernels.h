@@ -142,6 +142,10 @@ void launch_forward_diffusion(const float* x0, const float* noise_in, const int*
                               const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
                               float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, cudaStream_t s);
 void launch_dropout_mask(float* out, long long n, int op_index, unsigned long long seed, float rate, cudaStream_t s);
+// xunet_image_metrics: one CTA per image, fp64 moments and sums in a fixed order (metrics.cu); 11 <= S <= XUNET_METRICS_MAX_SIDE
+struct MetricsWindow { double w[11]; };   // the normalised 1-D Gaussian weights of the SSIM window
+void launch_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
+                          float* ssim_out, cudaStream_t s);
 
 // ---- attention over frames ---------------------------------------------------------------------------------
 struct AttnArgs {

@@ -92,7 +92,7 @@ class SRNScenes:
             if len(imgs) != len(poses) or not imgs:
                 raise ValueError(f'{d}: {len(imgs)} images vs {len(poses)} poses')
             K = parse_intrinsics(os.path.join(d, 'intrinsics.txt'), self.S)
-            self.instances.append(dict(imgs=imgs, poses=poses, K=K))
+            self.instances.append(dict(name=os.path.basename(os.path.normpath(d)), imgs=imgs, poses=poses, K=K))
             self.index += [(len(self.instances) - 1, v) for v in range(len(imgs))]
         if host_diffusion:
             ac = np.cumprod(1. - cosine_beta_schedule(1000), axis=0)
@@ -115,6 +115,15 @@ class SRNScenes:
             item['noise'] = noise
             item['logsnr'] = float(logsnr_schedule_cosine(t / 1000.0))
         return item
+
+    def instance_views(self, i: int) -> Dict:
+        """Every view of instance i, in the reader's sorted file order (index j = the j-th file kept after
+        max_observations_per_instance): dict(name, x (n,S,S,3), R (n,3,3), t (n,3), K (3,3)).  Draws nothing from self.rng,
+        so it leaves the training stream of batches() unchanged (evaluation reads held-out views this way)."""
+        inst = self.instances[i]
+        poses = np.stack([load_pose(p) for p in inst['poses']])
+        return dict(name=inst['name'], x=np.stack([load_rgb(p, self.S) for p in inst['imgs']]),
+                    R=np.ascontiguousarray(poses[:, :3, :3]), t=np.ascontiguousarray(poses[:, :3, 3]), K=inst['K'])
 
     @staticmethod
     def collate(items: List[Dict[str, np.ndarray]]) -> Dict[str, np.ndarray]:
