@@ -4,6 +4,7 @@ instance is conditioned on one source view (view 64 by default) and every scored
 
     python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --steps 256 --w 3 \\
         --source-view 64 --targets 10 --max-instances 20 --views-in-flight 8 --mode independent --out eval/
+    python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --method dpmpp_2m --steps 25 --out eval_dpm/
 
 Modes:
   independent  each target is sampled from the source alone (Sampler.sample, the reference's k = 1 sampler); the targets
@@ -49,6 +50,11 @@ def main():
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--steps', type=int, default=256)
     ap.add_argument('--w', type=float, default=3.0)
+    ap.add_argument('--method', choices=P.sampling.METHODS, default='ddpm',
+                    help="ddpm: the reference's ancestral sampler; ddim and dpmpp_2m (DPM-Solver++(2M)) need tens of steps")
+    ap.add_argument('--eta', type=float, default=0.0, help='DDIM stochasticity in [0, 1] (0: deterministic, 1: DDPM)')
+    ap.add_argument('--spacing', choices=P.sampling.SPACINGS, default=None,
+                    help='timestep spacing (default: logsnr for dpmpp_2m, linear otherwise)')
     ap.add_argument('--source-view', type=int, default=64, help='conditioning view of every instance (pixelNeRF / 3DiM: 64)')
     ap.add_argument('--targets', type=int, default=0, help='target views per instance, spaced evenly; 0 = all other views')
     ap.add_argument('--max-instances', type=int, default=-1, help='score the first N instances of the sorted list')
@@ -71,7 +77,7 @@ def main():
             raise SystemExit(f"instance {ds.instances[i]['name']} has {n} views; --source-view {a.source_view} does not exist")
         insts.append((i, select_targets(n, a.source_view, a.targets)))
     B = a.views_in_flight
-    sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w)
+    sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing)
     os.makedirs(a.out, exist_ok=True)
     if a.save_views:
         os.makedirs(os.path.join(a.out, 'views'), exist_ok=True)

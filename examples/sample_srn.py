@@ -3,6 +3,7 @@ ancestral sampler, write PNGs (the reference blocks in cv2.imshow, which cannot 
 
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --steps 256 --out results/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --prefix ema --steps 256 --out results_ema/
+    python examples/sample_srn.py cars_train_val --ckpt checkpoints --method dpmpp_2m --steps 25 --out results_dpm/
 """
 import argparse
 import os
@@ -22,6 +23,11 @@ def main():
     ap.add_argument('--prefix', default='model', help="checkpoint prefix: 'ema' samples the weight EMA of train_srn.py")
     ap.add_argument('--steps', type=int, default=1000)       # the reference runs all 1000 steps, sampling.py:128
     ap.add_argument('--w', type=float, default=3.0)          # sampling.py:133
+    ap.add_argument('--method', choices=P.sampling.METHODS, default='ddpm',
+                    help="ddpm: the reference's ancestral sampler; ddim and dpmpp_2m (DPM-Solver++(2M)) need tens of steps")
+    ap.add_argument('--eta', type=float, default=0.0, help='DDIM stochasticity in [0, 1] (0: deterministic, 1: DDPM)')
+    ap.add_argument('--spacing', choices=P.sampling.SPACINGS, default=None,
+                    help='timestep spacing (default: logsnr for dpmpp_2m, linear otherwise)')
     ap.add_argument('--views', type=int, default=1)
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--out', default='results')
@@ -35,7 +41,7 @@ def main():
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50)
     batch = next(ds.batches(a.views))
     model = P.XUNet()
-    sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w)
+    sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing)
     os.makedirs(a.out, exist_ok=True)
     if a.orbit > 0:
         it = ds.batches(a.views)

@@ -192,7 +192,7 @@ int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, 
  *     eps = (1+w) eps_c - w eps_u;  x0 = clip(c_recip z - c_recipm1 eps, -1, 1);  z' = c1 x0 + c2 z + sigma * noise_k.
  * table: device (steps, 8) floats, row k (k = 0: first executed step = highest t) = {c_recip = sqrt_recip_alphas_cumprod,
  * c_recipm1 = sqrt_recipm1_alphas_cumprod, c1 = posterior_mean_coef1, c2 = posterior_mean_coef2, sigma (0 at t=0), log-SNR
- * fed to the NEXT forward (sampling.py:151), 0, 0}; pos_dev: device int32 loop position (the caller increments it after the
+ * fed to the NEXT forward (sampling.py:151), 0, 0} (a DDIM table puts its c_x0, c_z, sigma in columns 2-4); pos_dev: device int32 loop position (the caller increments it after the
  * call, in stream order).  z (n = B*S*S*3) is updated in place; the new z is also written to both halves of the next
  * forward's [cond ; uncond] input next_z2 (2n) and next_logsnr2 (batch2 = 2B entries).
  * Noise: noise != NULL: device (steps, n) floats, step k reads noise[k*n .. k*n+n).  noise == NULL: the device hash normal
@@ -201,6 +201,18 @@ int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, 
 int xunet_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* table,
                              const int* pos_dev, const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2,
                              int batch2, void* stream);
+
+/* The multistep form of xunet_sampler_step_table (same arguments, same contract) for second-order solvers such as
+ * DPM-Solver++(2M): row k = *pos_dev of the table is {c_recip, c_recipm1, c_x0, c_z, sigma, log-SNR of the next forward,
+ * c_prev, 0}, and x0_hist (device, n floats, required) carries the previous step's clipped x0 between calls:
+ *     x0 = clip(c_recip z - c_recipm1 eps, -1, 1)  as above;
+ *     z' = fma(sigma, noise_k, fma(c_prev, x0_hist[i], fma(c_x0, x0, c_z * z)))   (fp32, one rounding per fma);
+ *     x0_hist[i] = x0.
+ * A row with c_prev == 0 skips the c_prev term and never reads x0_hist, so the first step of a chain needs no initialised
+ * history.  Graph-capturable. */
+int xunet_sampler_step_multistep(const float* eps2, float* z, const float* noise, long long n, float w, const float* table,
+                                 const int* pos_dev, const unsigned long long* seed_dev, float* x0_hist, float* next_z2,
+                                 float* next_logsnr2, int batch2, void* stream);
 
 /* Device-side forward diffusion = the per-item work of SceneInstanceDataset.__getitem__ (dataset/data_loader.py:92-110):
  *   t ~ U{0..999};  noise ~ N(0,1);  z = sqrt_ac[t] * x0 + sqrt_1mac[t] * noise;  logsnr = logsnr_schedule_cosine(t/1000);

@@ -65,6 +65,8 @@ SYMBOLS = {
                              [C.c_void_p, C.c_double, C.c_longlong, C.c_void_p, C.c_void_p]),
     'xunet_sampler_step_table': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    'xunet_sampler_step_multistep': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float] +
+                                     [C.c_void_p] * 6 + [C.c_int, C.c_void_p]),
     'xunet_forward_diffusion': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p, C.c_void_p, C.c_float,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong,
                                           C.c_void_p]),

@@ -1130,9 +1130,21 @@ extern "C" int xunet_sampler_step_table(const float* eps2, float* z, const float
                                         const int* pos_dev, const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2,
                                         int batch2, void* stream) {
   if (!eps2 || !z || !table || !pos_dev || !seed_dev || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0) return fail("xunet_sampler_step_table: bad argument");
-  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, (cudaStream_t)stream);
+  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, nullptr,
+                            (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("sampler_step_table: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_sampler_step_multistep(const float* eps2, float* z, const float* noise, long long n, float w,
+                                            const float* table, const int* pos_dev, const unsigned long long* seed_dev,
+                                            float* x0_hist, float* next_z2, float* next_logsnr2, int batch2, void* stream) {
+  if (!eps2 || !z || !table || !pos_dev || !seed_dev || !x0_hist || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0)
+    return fail("xunet_sampler_step_multistep: bad argument");
+  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist,
+                            (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("sampler_step_multistep: CUDA error: %s", cudaGetErrorString(e));
 }
 
 extern "C" int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,

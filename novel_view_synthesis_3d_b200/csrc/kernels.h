@@ -135,9 +135,11 @@ void launch_adam(float* p, const float* g, float* m, float* v, long long n, long
 // scratch: XUNET_GRAD_NORM_SCRATCH doubles; on completion scratch[0] holds the fp64 sum of squares.  Two launches.
 void launch_grad_global_norm(const float* g, long long n, double grad_scale, double* scratch, float* norm_out,
                              cudaStream_t s);
+// x0_hist == nullptr: the single-step update (DDPM, DDIM); else the multistep one, which reads column 6 (c_prev) and the
+// previous step's x0 from x0_hist (n floats) and stores this step's x0 there
 void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
-                               cudaStream_t s);
+                               float* x0_hist, cudaStream_t s);
 void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
                               const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
                               float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, cudaStream_t s);

@@ -1707,13 +1707,19 @@ void launch_grad_global_norm(const float* g, long long n, double grad_scale, dou
 // One ancestral step with the schedule ON THE DEVICE (sampling.py:128-151): the coefficients of loop position k = *pos_dev come
 // from a table (k = 0 is the first executed step = highest t), and the kernel also writes the NEXT forward's inputs (z into
 // both halves of the [cond ; uncond] batch, the lagging log-SNR), so one CUDA graph = forward + this kernel + counter++ is
-// replayed per step with no host arithmetic or copies in between.  tab row: {c_recip, c_recipm1, c1, c2, sigma, logsnr_next, -, -}
+// replayed per step with no host arithmetic or copies in between.
+// tab row: {c_recip, c_recipm1, c_x0, c_z, sigma, logsnr_next, c_prev, -}
 // The noise of step k is noise[k*n .. k*n+n) if `noise` is set, else the hash normal of (*seed_dev - k).
+// HIST = false (DDPM, DDIM): z' = c_x0 x0 + c_z z + sigma noise, as the compiler contracts it (the bits of the original
+// single-step kernel).  HIST = true (multistep solvers, DPM-Solver++(2M)) fixes the order, one rounding per fma:
+//   z' = fma(sigma, noise, fma(c_prev, x0_hist[i], fma(c_x0, x0, c_z * z))), the c_prev term skipped when c_prev == 0,
+// then x0_hist[i] = x0.  A row with c_prev == 0 never reads x0_hist (the first step needs no initialised history).
+template <bool HIST>
 __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __restrict__ eps2, float* __restrict__ z,
                                                                  const float* __restrict__ noise, long long n, float w,
                                                                  const float* __restrict__ tab, const int* __restrict__ pos_dev,
                                                                  const unsigned long long* __restrict__ seed_dev, float* __restrict__ inp_z,
-                                                                 float* __restrict__ inp_logsnr, int B2) {
+                                                                 float* __restrict__ inp_logsnr, int B2, float* __restrict__ x0_hist) {
   xu_grid_dep_sync();
   const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
   const int k = *pos_dev;
@@ -1725,16 +1731,30 @@ __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __
   float x0 = t[0] * zi - t[1] * e;
   x0 = fminf(fmaxf(x0, -1.f), 1.f);
   const float nz = noise != nullptr ? noise[k * n + i] : xu_hash_normal(*seed_dev - (unsigned long long)k, (uint64_t)i);
-  const float zn = t[2] * x0 + t[3] * zi + t[4] * nz;
+  float zn;
+  if constexpr (HIST) {
+    const float c_prev = t[6];
+    zn = fmaf(t[2], x0, __fmul_rn(t[3], zi));
+    if (c_prev != 0.f) zn = fmaf(c_prev, x0_hist[i], zn);
+    zn = fmaf(t[4], nz, zn);
+    x0_hist[i] = x0;
+  } else {
+    zn = t[2] * x0 + t[3] * zi + t[4] * nz;
+  }
   z[i] = zn;
   inp_z[i] = zn;
   inp_z[n + i] = zn;
 }
 void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
-                               cudaStream_t s) {
-  xu_launch(sampler_step_table_kernel, cdiv(n > B2 ? n : B2, 256), 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z,
-            inp_logsnr, B2);
+                               float* x0_hist, cudaStream_t s) {
+  const int grid = cdiv(n > B2 ? n : B2, 256);
+  if (x0_hist != nullptr)
+    xu_launch(sampler_step_table_kernel<true>, grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr,
+              B2, x0_hist);
+  else
+    xu_launch(sampler_step_table_kernel<false>, grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr,
+              B2, x0_hist);
 }
 
 // dataset/data_loader.py:92-110 on the device

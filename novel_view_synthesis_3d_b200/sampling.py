@@ -4,6 +4,10 @@ Reference behaviour (steps=1000, w=3): per step two model evaluations (cond_mask
 [cond ; uncond] -- eps=(1+w)eps_c-w eps_u, x0=clip(predict_start_from_noise), posterior mean/variance, z<-mean+sigma*N(0,1)
 (no noise at t=0), and the log-SNR fed to the network lags one step and starts at -20 (sampling.py:126,151).
 `steps<1000` re-spaces the schedule (strided alpha-bar), which is what the 256-step metric uses.
+
+Two samplers that need only tens of steps run through the same device-table step: DDIM (Song et al. 2021; eta = 0
+deterministic, eta = 1 the DDPM posterior) and DPM-Solver++(2M) (Lu et al. 2022), a second-order multistep solver in x0
+that keeps the previous step's clipped x0 on the device.  Both feed the network the log-SNR of the timestep z is at.
 """
 from __future__ import annotations
 
@@ -33,13 +37,30 @@ def logsnr_schedule_cosine(t, *, logsnr_min=-20., logsnr_max=20.):
     return -2. * np.log(np.tan(a * t + b))
 
 
-class Schedule:
-    """The tables of sampling.py:28-41, optionally re-spaced to `steps` < T timesteps."""
+METHODS = ('ddpm', 'ddim', 'dpmpp_2m')
+SPACINGS = ('linear', 'logsnr')
 
-    def __init__(self, steps: int = 1000, T: int = 1000):
+
+class Schedule:
+    """The tables of sampling.py:28-41, optionally re-spaced to `steps` < T timesteps.
+
+    spacing='linear': `steps` timesteps evenly spaced in t (all T when steps >= T).  spacing='logsnr': `steps` points
+    uniform in lambda = log(sqrt(abar) / sqrt(1 - abar)) between lambda(T-1) and lambda(0), each mapped to the timestep
+    with the nearest lambda, duplicates dropped.  The last steps of the cosine schedule hold a large log-SNR jump, so this
+    is the spacing multistep solvers need.  With it, len(self) -- the number of forwards a sample runs -- can be smaller
+    than `steps` (9 for 10, 19 for 25, 36 for 50, 142 for 256)."""
+
+    def __init__(self, steps: int = 1000, T: int = 1000, spacing: str = 'linear'):
+        if spacing not in SPACINGS:
+            raise ValueError(f'unknown spacing {spacing!r}; expected one of {SPACINGS}')
         betas_full = cosine_beta_schedule(T)
         ac_full = np.cumprod(1. - betas_full, axis=0)
-        if steps >= T:
+        if spacing == 'logsnr':
+            lam = 0.5 * np.log(ac_full / (1. - ac_full))
+            target = np.linspace(lam[T - 1], lam[0], steps)
+            self.timesteps = np.unique(np.abs(lam[None, :] - target[:, None]).argmin(1))
+            ac = ac_full[self.timesteps]
+        elif steps >= T:
             self.timesteps = np.arange(T)
             ac = ac_full
         else:
@@ -61,15 +82,93 @@ class Schedule:
         return len(self.timesteps)
 
 
+def _check_method(method: str, eta: float) -> None:
+    if method not in METHODS:
+        raise ValueError(f'unknown sampler method {method!r}; expected one of {METHODS}')
+    if not 0.0 <= eta <= 1.0:
+        raise ValueError(f'eta {eta} outside [0, 1]')
+    if eta != 0.0 and method != 'ddim':
+        raise ValueError(f'eta {eta} is only defined for method ddim, not {method}')
+
+
+def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, logsnr_lag: bool = True):
+    """The device table of `sched` for `method`: (rows, logsnr_first), rows (len(sched), 8) float64 (the sampler rounds
+    them to fp32 once), row k = loop position k = timestep index len-1-k = {c_recip, c_recipm1, c_x0, c_z, sigma,
+    logsnr_next, c_prev, 0}; logsnr_first is the log-SNR of the first forward.  A step is
+        x0 = clip(c_recip z - c_recipm1 eps, -1, 1);  z' = c_x0 x0 + c_z z + c_prev x0_prev + sigma noise.
+    With abar the row's alpha-bar, abar' the next row's (1 after the last step), alpha = sqrt(abar),
+    sigma_t = sqrt(1 - abar) and lambda = log(alpha / sigma_t):
+      ddpm      the posterior of sampling.py:133-151 (reads the schedule's posterior tables), c_prev = 0;
+      ddim      sigma = eta sqrt((1 - abar') / (1 - abar) (1 - abar / abar')), c_z = sqrt(1 - abar' - sigma^2) / sigma_t,
+                c_x0 = sqrt(abar') - c_z alpha: DDIM with eps re-derived from the clipped x0 (eta = 1: the ddpm rows);
+      dpmpp_2m  h = lambda' - lambda, r = h_prev / h, g = alpha' (1 - e^-h), c_z = sigma_t' / sigma_t,
+                c_x0 = g (1 + 1/(2r)), c_prev = -g / (2r), sigma = 0; the first and the last row are first order
+                (c_x0 = g, c_prev = 0), so the last step, to abar' = 1, is z' = x0.
+    ddim and dpmpp_2m read only sched.timesteps and the matching leading entries of sched.alphas_cumprod.
+    logsnr_lag=True: the reference's lag (sampling.py:126,151): the first forward gets -20 and row k hands the next forward
+    the log-SNR of its own timestep t_k.  logsnr_lag=False: each forward gets the log-SNR of the timestep z is at,
+    logsnr_cosine(t_0/1000) first and logsnr_cosine(t_{k+1}/1000) from row k (the last row's value is unused)."""
+    _check_method(method, eta)
+    sc = sched
+    n = len(sc.timesteps)
+    i = np.arange(n - 1, -1, -1)
+    zero = np.zeros(n)
+    c_prev = zero
+    if method == 'ddpm':
+        sigma = np.where(i == 0, 0.0, np.exp(0.5 * sc.posterior_log_variance_clipped[i]))     # sampling.py:142-148
+        c_recip, c_recipm1 = sc.sqrt_recip_alphas_cumprod[i], sc.sqrt_recipm1_alphas_cumprod[i]
+        c_x0, c_z = sc.posterior_mean_coef1[i], sc.posterior_mean_coef2[i]
+    else:
+        ac_all = np.asarray(sc.alphas_cumprod, dtype=np.float64)[:n]
+        a, a_next = ac_all[i], np.concatenate([[1.0], ac_all[:-1]])[i]
+        c_recip, c_recipm1 = np.sqrt(1. / a), np.sqrt(1. / a - 1)
+        if method == 'ddim':
+            sigma = eta * np.sqrt((1. - a_next) / (1. - a) * (1. - a / a_next))
+            # 1 - abar' - sigma^2 = (1 - abar') ((1 - eta^2) + eta^2 abar (1 - abar') / (abar' (1 - abar))), written so that
+            # it does not cancel when sigma^2 is close to 1 - abar' (eta = 1 at high t)
+            keep = (1. - eta ** 2) + eta ** 2 * a * (1. - a_next) / (a_next * (1. - a))
+            c_z = np.sqrt((1. - a_next) * keep) / np.sqrt(1. - a)
+            c_x0 = np.sqrt(a_next) - c_z * np.sqrt(a)
+        else:
+            sigma = zero
+            c_z = np.sqrt((1. - a_next) / (1. - a))
+            with np.errstate(divide='ignore', invalid='ignore'):
+                lam = 0.5 * (np.log(a) - np.log(1. - a))
+                lam_next = 0.5 * (np.log(a_next) - np.log(1. - a_next))        # +inf after the last step
+                h = lam_next - lam
+                g = -np.sqrt(a_next) * np.expm1(-h)
+                r = np.concatenate([[np.nan], h[:-1]]) / h                     # h_prev / h
+                second = (np.arange(n) > 0) & (np.arange(n) < n - 1)
+                c_x0 = np.where(second, g * (1. + 1. / (2. * r)), g)
+                c_prev = np.where(second, -g / (2. * r), 0.0)
+    t = np.asarray(sc.timesteps)[i] / 1000.0
+    if logsnr_lag:
+        logsnr_first, logsnr_next = -20.0, logsnr_schedule_cosine(t)
+    else:
+        logsnr_first, logsnr_next = float(logsnr_schedule_cosine(t[0])), logsnr_schedule_cosine(np.append(t[1:], t[-1]))
+    rows = np.stack([c_recip, c_recipm1, c_x0, c_z, sigma, logsnr_next, c_prev, zero], 1)
+    return rows, logsnr_first
+
+
 class Sampler:
     """z, the forward's z / log-SNR inputs, the loop position, the noise seed and the coefficient table all live on the device,
     so one sampler step is the 2B-batch forward, `xunet_sampler_step_table` and pos += 1, with no host arithmetic in between.
-    use_graph=True replays that step as one CUDA graph; use_graph=False issues the same calls eagerly."""
+    use_graph=True replays that step as one CUDA graph; use_graph=False issues the same calls eagerly.
+
+    method: 'ddpm' (the reference's ancestral sampler), 'ddim' (eta in [0, 1]; 0 = deterministic) or 'dpmpp_2m'
+    (DPM-Solver++(2M); its step is `xunet_sampler_step_multistep`, with the previous step's x0 in a device buffer).
+    spacing: the Schedule's timestep spacing, 'logsnr' for dpmpp_2m and 'linear' otherwise by default; len(self.sched)
+    is the number of forwards a sample runs.  logsnr_lag: the reference's one-step lag of the network's log-SNR input,
+    on by default for ddpm only (see `sampler_table`).  With every default this is the reference sampler."""
 
     def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000, w: float = 3.0,
-                 use_graph: bool = True):
+                 use_graph: bool = True, method: str = 'ddpm', eta: float = 0.0, spacing: str | None = None,
+                 logsnr_lag: bool | None = None):
+        _check_method(method, eta)
+        self.method, self.eta = method, float(eta)
+        self.logsnr_lag = method == 'ddpm' if logsnr_lag is None else bool(logsnr_lag)
         self.model, self.B, self.S, self.w = model, batch_size, img_sidelength, float(w)
-        self.sched = Schedule(steps)
+        self.sched = Schedule(steps, spacing=('logsnr' if method == 'dpmpp_2m' else 'linear') if spacing is None else spacing)
         self.eng = model.engine(2 * batch_size, img_sidelength, False)
         self.flat = model.flat_from_tree(params, img_sidelength, 2 * batch_size)
         self.lib = _lib.load()
@@ -81,6 +180,10 @@ class Sampler:
         self._graphs = {}           # (static conditioning, explicit noise) -> the captured step
         self._pos = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self._seed_base = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self._logsnr_first = -20.0
+        # dpmpp_2m: the previous step's clipped x0.  Allocated once, since the captured graphs hold its pointer; a chain's
+        # first row has c_prev = 0 and overwrites it, so every chain starts with a fresh history.
+        self._x0_hist = torch.empty_like(self.z) if method == 'dpmpp_2m' else None
 
     def capture(self, batch: dict) -> None:
         """Runs the first 3 steps of a sample: builds the static-conditioning state and, with use_graph, the per-step CUDA
@@ -106,24 +209,20 @@ class Sampler:
 
     def _load_schedule(self) -> int:
         """Writes the coefficient table of `self.sched` (callers may have edited it since the last call) to the device and
-        returns its number of steps.  Row k = loop position k = timestep index len-1-k."""
-        sc = self.sched
-        i = np.arange(len(sc) - 1, -1, -1)
-        sigma = np.where(i == 0, 0.0, np.exp(0.5 * sc.posterior_log_variance_clipped[i]))         # sampling.py:142-148
-        zero = np.zeros(len(i))
-        rows = np.stack([sc.sqrt_recip_alphas_cumprod[i], sc.sqrt_recipm1_alphas_cumprod[i], sc.posterior_mean_coef1[i],
-                         sc.posterior_mean_coef2[i], sigma, logsnr_schedule_cosine(sc.timesteps[i] / 1000.0), zero, zero], 1)
-        if self._tab is None or len(self._tab) != len(i):
+        returns its number of steps.  Row k = loop position k = timestep index len-1-k (`sampler_table`)."""
+        rows, self._logsnr_first = sampler_table(self.sched, self.method, eta=self.eta, logsnr_lag=self.logsnr_lag)
+        if self._tab is None or len(self._tab) != len(rows):
             # the captured graphs hold the table and noise pointers: reallocate (and recapture) only when the length changes
-            self._tab = torch.empty(len(i), 8, dtype=torch.float32, device=self.dev)
+            self._tab = torch.empty(len(rows), 8, dtype=torch.float32, device=self.dev)
             self._noise = None
             self._graphs = {}
         self._tab.copy_(torch.as_tensor(rows, dtype=torch.float32))
-        return len(i)
+        return len(rows)
 
     def _start_chain(self, seed: int, z_init, noises) -> None:
-        """z <- z_init, or N(0, 1) from `seed` (sampling.py:125); the first forward's inputs z and log-SNR = -20
-        (sampling.py:126); the noise of step k: noises[k], or the hash normal of seed * 1000003 + timestep index."""
+        """z <- z_init, or N(0, 1) from `seed` (sampling.py:125); the first forward's inputs z and the table's first log-SNR
+        (-20 with the lag, sampling.py:126); the noise of step k: noises[k], or the hash normal of seed * 1000003 + timestep
+        index."""
         B, steps, e = self.B, len(self._tab), self.eng
         if z_init is None:
             g = torch.Generator(device=self.dev).manual_seed(seed)
@@ -132,7 +231,7 @@ class Sampler:
             self.z.copy_(torch.as_tensor(np.asarray(z_init), dtype=torch.float32).to(self.dev))
         e.inp['z'][:B].copy_(self.z)
         e.inp['z'][B:].copy_(self.z)
-        e.inp['logsnr'].fill_(-20.0)
+        e.inp['logsnr'].fill_(self._logsnr_first)
         self._seed_base.fill_((seed * 1000003 + steps - 1) & 0x7FFFFFFFFFFFFFFF)    # the kernel subtracts the loop position
         if noises is not None:
             if self._noise is None:
@@ -164,10 +263,13 @@ class Sampler:
         e = self.eng
         e.forward(self.flat, train=False)
         st = torch.cuda.current_stream(self.dev).cuda_stream
-        _lib.check(self.lib.xunet_sampler_step_table(e.eps.data_ptr(), self.z.data_ptr(), self._noise.data_ptr() if noise else None,
-                                                     self.z.numel(), self.w, self._tab.data_ptr(), self._pos.data_ptr(),
-                                                     self._seed_base.data_ptr(), e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(),
-                                                     2 * self.B, st), 'sampler_step_table')
+        head = (e.eps.data_ptr(), self.z.data_ptr(), self._noise.data_ptr() if noise else None, self.z.numel(), self.w,
+                self._tab.data_ptr(), self._pos.data_ptr(), self._seed_base.data_ptr())
+        tail = (e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(), 2 * self.B, st)
+        if self._x0_hist is None:
+            _lib.check(self.lib.xunet_sampler_step_table(*head, *tail), 'sampler_step_table')
+        else:
+            _lib.check(self.lib.xunet_sampler_step_multistep(*head, self._x0_hist.data_ptr(), *tail), 'sampler_step_multistep')
         self._pos.add_(1)
 
     def _graph(self, static: bool, noise: bool) -> torch.cuda.CUDAGraph:
