@@ -5,6 +5,8 @@ instance is conditioned on one source view (view 64 by default) and every scored
     python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --steps 256 --w 3 \\
         --source-view 64 --targets 10 --max-instances 20 --views-in-flight 8 --mode independent --out eval/
     python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --method dpmpp_2m --steps 25 --out eval_dpm/
+    python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --method dpmpp_2m --steps 25 \\
+        --dynamic-threshold 0.995 --out eval_dpm_dyn/
 
 Modes:
   independent  each target is sampled from the source alone (Sampler.sample, the reference's k = 1 sampler); the targets
@@ -55,6 +57,8 @@ def main():
     ap.add_argument('--eta', type=float, default=0.0, help='DDIM stochasticity in [0, 1] (0: deterministic, 1: DDPM)')
     ap.add_argument('--spacing', choices=P.sampling.SPACINGS, default=None,
                     help='timestep spacing (default: logsnr for dpmpp_2m, linear otherwise)')
+    ap.add_argument('--dynamic-threshold', type=float, default=None, metavar='P',
+                    help='threshold x0 per view at the P-quantile of |x0| (Imagen: 0.995) instead of clipping it to [-1, 1]')
     ap.add_argument('--source-view', type=int, default=64, help='conditioning view of every instance (pixelNeRF / 3DiM: 64)')
     ap.add_argument('--targets', type=int, default=0, help='target views per instance, spaced evenly; 0 = all other views')
     ap.add_argument('--max-instances', type=int, default=-1, help='score the first N instances of the sorted list')
@@ -77,7 +81,8 @@ def main():
             raise SystemExit(f"instance {ds.instances[i]['name']} has {n} views; --source-view {a.source_view} does not exist")
         insts.append((i, select_targets(n, a.source_view, a.targets)))
     B = a.views_in_flight
-    sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing)
+    sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing,
+                        dynamic_threshold=a.dynamic_threshold)
     os.makedirs(a.out, exist_ok=True)
     if a.save_views:
         os.makedirs(os.path.join(a.out, 'views'), exist_ok=True)

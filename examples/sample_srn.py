@@ -28,6 +28,8 @@ def main():
     ap.add_argument('--eta', type=float, default=0.0, help='DDIM stochasticity in [0, 1] (0: deterministic, 1: DDPM)')
     ap.add_argument('--spacing', choices=P.sampling.SPACINGS, default=None,
                     help='timestep spacing (default: logsnr for dpmpp_2m, linear otherwise)')
+    ap.add_argument('--dynamic-threshold', type=float, default=None, metavar='P',
+                    help='threshold x0 per view at the P-quantile of |x0| (Imagen: 0.995) instead of clipping it to [-1, 1]')
     ap.add_argument('--views', type=int, default=1)
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--out', default='results')
@@ -41,7 +43,8 @@ def main():
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50)
     batch = next(ds.batches(a.views))
     model = P.XUNet()
-    sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing)
+    sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing,
+                        dynamic_threshold=a.dynamic_threshold)
     os.makedirs(a.out, exist_ok=True)
     if a.orbit > 0:
         it = ds.batches(a.views)

@@ -214,6 +214,25 @@ int xunet_sampler_step_multistep(const float* eps2, float* z, const float* noise
                                  const int* pos_dev, const unsigned long long* seed_dev, float* x0_hist, float* next_z2,
                                  float* next_logsnr2, int batch2, void* stream);
 
+/* The sampler step with DYNAMIC THRESHOLDING of x0 (Saharia et al. 2022, Imagen section 2.3) in place of the fixed clip:
+ * the same table row, noise, next_z2 / next_logsnr2 writes and (x0_hist != NULL) multistep term as
+ * xunet_sampler_step_table (x0_hist == NULL) and xunet_sampler_step_multistep (x0_hist != NULL), with
+ *     x0 = c_recip z - c_recipm1 eps  (unclipped);  s_b = max(1, quantile_p(|x0|) over the per = n / batch values of view b);
+ *     x0 <- clip(x0, -s_b, s_b) / s_b   (fp32 division, round to nearest),
+ * and this x0 feeds the update and x0_hist.  quantile_p is numpy's np.quantile(a, p) (method 'linear') in fp64 on the fp32
+ * values a = |x0| sorted ascending: idx = (per - 1) p, lo = floor(idx), hi = min(lo + 1, per - 1), g = idx - lo,
+ * d = a[hi] - a[lo], q = g < 0.5 ? a[lo] + d g : a[hi] - d (1 - g), each operation rounded once (no fma); s_b = max(fp32(q), 1).
+ * A view with s_b = 1 gets exactly the bits of the static step.  s_b is found by an integer radix select, so it depends on the
+ * view's values alone (not on batch or on the view's position).  scale_out (device, batch floats) receives s_b when given.
+ * Errors: a NULL required pointer, n <= 0, batch2 <= 0, batch < 1, n % batch != 0, per > XUNET_SAMPLER_DYN_MAX_PER (the
+ * shared-memory slices are sized for it), percentile NaN or outside (0, 1].  One launch; no allocation, no host sync,
+ * graph-capturable. */
+#define XUNET_SAMPLER_DYN_MAX_PER (256 * 256 * 3)
+int xunet_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* table,
+                               const int* pos_dev, const unsigned long long* seed_dev, float* x0_hist, int batch,
+                               double percentile, float* scale_out, float* next_z2, float* next_logsnr2, int batch2,
+                               void* stream);
+
 /* Device-side forward diffusion = the per-item work of SceneInstanceDataset.__getitem__ (dataset/data_loader.py:92-110):
  *   t ~ U{0..999};  noise ~ N(0,1);  z = sqrt_ac[t] * x0 + sqrt_1mac[t] * noise;  logsnr = logsnr_schedule_cosine(t/1000);
  *   cond_mask = (u > p_uncond)  (train.py:64).

@@ -10,6 +10,7 @@ from pathlib import Path
 LIB_PATH = Path(os.environ['XUNET_LIB']).resolve() if os.environ.get('XUNET_LIB') else Path(__file__).resolve().parent / 'libxunet_b200.so'
 MAX_LEVELS = 8
 GRAD_NORM_SCRATCH = 1024       # XUNET_GRAD_NORM_SCRATCH: doubles of scratch xunet_grad_global_norm needs
+SAMPLER_DYN_MAX_PER = 256 * 256 * 3     # XUNET_SAMPLER_DYN_MAX_PER: values per view xunet_sampler_step_dynamic takes
 DTYPE_F32, DTYPE_BF16 = 0, 1
 RAYS = {'v3d130_ij': 0, 'opencv_uv': 1}
 
@@ -67,6 +68,8 @@ SYMBOLS = {
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     'xunet_sampler_step_multistep': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float] +
                                      [C.c_void_p] * 6 + [C.c_int, C.c_void_p]),
+    'xunet_sampler_step_dynamic': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float] + [C.c_void_p] * 4 +
+                                   [C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     'xunet_forward_diffusion': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p, C.c_void_p, C.c_float,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong,
                                           C.c_void_p]),

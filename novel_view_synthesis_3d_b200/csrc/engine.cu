@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 106; }
+extern "C" int xunet_version(void) { return 107; }
 
 namespace {
 
@@ -1145,6 +1145,26 @@ extern "C" int xunet_sampler_step_multistep(const float* eps2, float* z, const f
                             (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("sampler_step_multistep: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w,
+                                          const float* table, const int* pos_dev, const unsigned long long* seed_dev,
+                                          float* x0_hist, int batch, double percentile, float* scale_out, float* next_z2,
+                                          float* next_logsnr2, int batch2, void* stream) {
+  if (!eps2 || !z || !table || !pos_dev || !seed_dev || !next_z2 || !next_logsnr2)
+    return fail("xunet_sampler_step_dynamic: NULL pointer argument");
+  if (n <= 0 || batch2 <= 0) return fail("xunet_sampler_step_dynamic: n = %lld, batch2 = %d, need both >= 1", n, batch2);
+  if (batch < 1) return fail("xunet_sampler_step_dynamic: batch = %d, need batch >= 1", batch);
+  if (n % batch != 0) return fail("xunet_sampler_step_dynamic: n = %lld is not a multiple of batch = %d", n, batch);
+  if (n / batch > XUNET_SAMPLER_DYN_MAX_PER)
+    return fail("xunet_sampler_step_dynamic: %lld values per view, more than XUNET_SAMPLER_DYN_MAX_PER = %d", n / batch,
+                XUNET_SAMPLER_DYN_MAX_PER);
+  if (!(percentile > 0.0 && percentile <= 1.0))
+    return fail("xunet_sampler_step_dynamic: percentile %g outside (0, 1]", percentile);
+  launch_sampler_step_dynamic(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, batch,
+                              percentile, scale_out, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("sampler_step_dynamic: CUDA error: %s", cudaGetErrorString(e));
 }
 
 extern "C" int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,

@@ -140,6 +140,11 @@ void launch_grad_global_norm(const float* g, long long n, double grad_scale, dou
 void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
                                float* x0_hist, cudaStream_t s);
+// xunet_sampler_step_dynamic (sampler_dyn.cu): the step above with x0 thresholded per view at the p-quantile of |x0|; one
+// cluster of 8 CTAs per view, n / B <= XUNET_SAMPLER_DYN_MAX_PER
+void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
+                                 const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
+                                 int B2, float* x0_hist, int B, double p, float* scale_out, cudaStream_t s);
 void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
                               const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
                               float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, cudaStream_t s);

@@ -1,0 +1,194 @@
+// sampler_dyn.cu -- the sampler step with dynamic thresholding of x0 (Saharia et al. 2022, Imagen section 2.3):
+// xunet_sampler_step_dynamic.
+//
+// The step is sampler_step_table_kernel's (kernels_elem.cu) with the fixed clip of x0 to [-1, 1] replaced by a per-view one:
+//   s = max(1, quantile_p(|x0|)) over the per = S*S*3 values of the view;   x0 <- clip(x0, -s, s) / s.
+// quantile_p is numpy's np.quantile(a, p) with the default 'linear' method, evaluated in fp64 on the fp32 values a = |x0|
+// sorted ascending (a[0] <= ... <= a[per-1]):
+//   idx = (per - 1) p,  lo = floor(idx),  hi = min(lo + 1, per - 1),  g = idx - lo,  d = a[hi] - a[lo],
+//   q = g < 0.5 ? a[lo] + d g : a[hi] - d (1 - g),
+// each operation rounded once (__dmul_rn / __dsub_rn / __dadd_rn: no fma contraction, as numpy), then s = fmaxf(fp32(q), 1).
+// With s = 1 the thresholded value is clip(x0, -1, 1) exactly, and e, x0 and z' use the same fp32 operations in the same
+// order as sampler_step_table_kernel (spelled out with intrinsics), so such a view gets the static step's bits.
+//
+// Layout: one thread-block cluster of DYN_CLUSTER CTAs per view (grid B * DYN_CLUSTER).  CTA r of the cluster owns the
+// contiguous slice [r*chunk, min((r+1)*chunk, per)) of its view, chunk = ceil(per / DYN_CLUSTER), and keeps the guided,
+// unclipped x0 of the slice in shared memory.  The order statistic a[lo] is found by a radix select on the bit patterns of
+// |x0| (for non-negative floats the order of the bit patterns is the order of the values): four passes of 8-bit digits,
+// high to low; per pass every CTA counts the digits of its candidates in a shared-memory histogram, the cluster syncs, and
+// every CTA adds the DYN_CLUSTER histograms through distributed shared memory and derives the digit from the merged counts.
+// The counts are integers, so every CTA derives the same digit with no broadcast, and s does not depend on B, on the view's
+// position in the batch or on the order of any addition.  a[hi] is a[lo] when more than lo + 1 values are at or below it,
+// else the cluster minimum of the keys above a[lo].  Each CTA then finishes the step for its slice from shared memory.
+// No atomics outside shared memory, no scratch buffer, one launch.
+#include <cooperative_groups.h>
+
+#include "xunet_b200.h"
+#include "common.cuh"
+#include "kernels.h"
+
+namespace cg = cooperative_groups;
+
+#define DYN_CLUSTER 8
+#define DYN_THREADS 256    // = the number of histogram bins: thread t owns bin t of the merged histogram
+
+static constexpr int kDynMaxChunk = (XUNET_SAMPLER_DYN_MAX_PER + DYN_CLUSTER - 1) / DYN_CLUSTER;
+
+// The fp64 'linear' quantile of the sorted values a[lo] = lo_v, a[hi] = hi_v (see the header of this file)
+__device__ __forceinline__ float dyn_threshold_scale(float lo_v, float hi_v, double g) {
+  const double alo = (double)lo_v, ahi = (double)hi_v;
+  const double d = __dsub_rn(ahi, alo);
+  const double q = g < 0.5 ? __dadd_rn(alo, __dmul_rn(d, g)) : __dsub_rn(ahi, __dmul_rn(d, __dsub_rn(1.0, g)));
+  return fmaxf(__double2float_rn(q), 1.f);
+}
+
+template <bool HIST>
+__global__ void __cluster_dims__(DYN_CLUSTER, 1, 1) __launch_bounds__(DYN_THREADS)
+sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ z, const float* __restrict__ noise, long long n,
+                            float w, const float* __restrict__ tab, const int* __restrict__ pos_dev,
+                            const unsigned long long* __restrict__ seed_dev, float* __restrict__ inp_z,
+                            float* __restrict__ inp_logsnr, int B2, float* __restrict__ x0_hist, int per, double p,
+                            float* __restrict__ scale_out) {
+  extern __shared__ float xs[];                 // the guided, unclipped x0 of this CTA's slice
+  __shared__ unsigned hist[2][DYN_THREADS];     // digit counts of this CTA's candidates, double-buffered across passes
+  __shared__ unsigned wsum[DYN_THREADS / 32];
+  __shared__ unsigned sel[3];                   // the pass's digit, the merged count below it, the merged count of it
+  __shared__ unsigned minkey;                   // the smallest key above a[lo] (this CTA's, then the cluster's)
+  xu_grid_dep_sync();
+  cg::cluster_group cluster = cg::this_cluster();
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned rank = cluster.block_rank();
+  const long long view = blockIdx.x / DYN_CLUSTER;
+  const int chunk = (per + DYN_CLUSTER - 1) / DYN_CLUSTER;
+  const int start = min((int)rank * chunk, per), len = min(chunk, per - start);
+  const long long base = view * per + start;
+  const int k = *pos_dev;
+  const float* t = tab + 8LL * k;
+  for (long long j = (long long)blockIdx.x * DYN_THREADS + tid; j < B2; j += (long long)gridDim.x * DYN_THREADS)
+    inp_logsnr[j] = t[5];
+
+  // guided x0, as sampler_step_table_kernel contracts it: e = fma(1 + w, eps_c, -(w eps_u)), x0 = fma(c_recip, z, -(c_recipm1 e))
+  const float c_recip = t[0], c_recipm1 = t[1], wp1 = __fadd_rn(1.f, w);
+  for (int j = tid; j < len; j += DYN_THREADS) {
+    const long long i = base + j;
+    const float e = fmaf(wp1, eps2[i], -__fmul_rn(w, eps2[n + i]));
+    xs[j] = fmaf(c_recip, z[i], -__fmul_rn(c_recipm1, e));
+  }
+  hist[0][tid] = 0u;
+  __syncthreads();
+
+  // radix select of rank lo: after the pass at `shift`, the candidates are the keys whose bits above shift equal `prefix`
+  const double idx = __dmul_rn((double)(per - 1), p);
+  const int lo = (int)floor(idx), hi = min(lo + 1, per - 1);
+  const double g = __dsub_rn(idx, (double)lo);
+  unsigned prefix = 0u, mask = 0u, r = (unsigned)lo, cnt = 0u;
+#pragma unroll 1
+  for (int pass = 0; pass < 4; ++pass) {
+    const int shift = 24 - 8 * pass, buf = pass & 1;
+    for (int j0 = 0; j0 < len; j0 += DYN_THREADS) {     // uniform trip count: every lane takes part in the match
+      const int j = j0 + tid;
+      unsigned d = DYN_THREADS;
+      if (j < len) {
+        const unsigned key = __float_as_uint(xs[j]) & 0x7FFFFFFFu;
+        if ((key & mask) == prefix) d = (key >> shift) & 0xFFu;
+      }
+      const unsigned peers = __match_any_sync(0xFFFFFFFFu, d);
+      if (d < DYN_THREADS && lane == __ffs(peers) - 1) atomicAdd(&hist[buf][d], (unsigned)__popc(peers));
+    }
+    cluster.sync();
+    unsigned c = 0u;
+#pragma unroll
+    for (int q = 0; q < DYN_CLUSTER; ++q) c += *cluster.map_shared_rank(&hist[buf][tid], q);
+    // every CTA has finished reading the other buffer (the previous pass) before this pass's cluster.sync
+    hist[buf ^ 1][tid] = 0u;
+    unsigned incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    if (lane == 31) wsum[warp] = incl;
+    __syncthreads();
+    unsigned excl = incl - c;
+    for (int q = 0; q < warp; ++q) excl += wsum[q];
+    if (excl <= r && r < excl + c) {
+      sel[0] = (unsigned)tid;
+      sel[1] = excl;
+      sel[2] = c;
+    }
+    __syncthreads();
+    prefix |= sel[0] << shift;
+    mask |= 0xFFu << shift;
+    r -= sel[1];
+    cnt = sel[2];
+  }
+  // prefix = a[lo]'s key; lo - r keys lie below it and cnt are equal to it
+  unsigned key_hi = prefix;
+  if (hi != lo && (unsigned)lo - r + cnt <= (unsigned)hi) {    // a[hi] is the next larger key (the same branch in every CTA)
+    unsigned m = 0xFFFFFFFFu;
+    for (int j = tid; j < len; j += DYN_THREADS) {
+      const unsigned key = __float_as_uint(xs[j]) & 0x7FFFFFFFu;
+      if (key > prefix) m = min(m, key);
+    }
+    m = __reduce_min_sync(0xFFFFFFFFu, m);
+    if (lane == 0) wsum[warp] = m;
+    __syncthreads();
+    if (tid == 0) {
+      unsigned b = wsum[0];
+      for (int q = 1; q < DYN_THREADS / 32; ++q) b = min(b, wsum[q]);
+      minkey = b;
+    }
+    cluster.sync();
+    if (tid == 0) {
+      unsigned b = 0xFFFFFFFFu;
+      for (int q = 0; q < DYN_CLUSTER; ++q) b = min(b, *cluster.map_shared_rank(&minkey, q));
+      wsum[0] = b;
+    }
+    __syncthreads();
+    key_hi = wsum[0];
+  }
+  // no CTA may exit while another still reads its shared memory
+  auto arrived = cluster.barrier_arrive();
+  const float s = dyn_threshold_scale(__uint_as_float(prefix), __uint_as_float(key_hi), g);
+  if (scale_out != nullptr && rank == 0 && tid == 0) scale_out[view] = s;
+
+  for (int j = tid; j < len; j += DYN_THREADS) {
+    const long long i = base + j;
+    const float x0 = __fdiv_rn(fminf(fmaxf(xs[j], -s), s), s);
+    const float zi = z[i];
+    const float nz = noise != nullptr ? noise[k * n + i] : xu_hash_normal(*seed_dev - (unsigned long long)k, (uint64_t)i);
+    float zn = fmaf(t[2], x0, __fmul_rn(t[3], zi));
+    if constexpr (HIST) {
+      const float c_prev = t[6];
+      if (c_prev != 0.f) zn = fmaf(c_prev, x0_hist[i], zn);
+      x0_hist[i] = x0;
+    }
+    zn = fmaf(t[4], nz, zn);
+    z[i] = zn;
+    inp_z[i] = zn;
+    inp_z[n + i] = zn;
+  }
+  cluster.barrier_wait(std::move(arrived));
+}
+
+void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
+                                 const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
+                                 int B2, float* x0_hist, int B, double p, float* scale_out, cudaStream_t s) {
+  static bool configured = false;
+  if (!configured) {
+    cudaFuncSetAttribute(sampler_step_dynamic_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)(sizeof(float) * kDynMaxChunk));
+    cudaFuncSetAttribute(sampler_step_dynamic_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)(sizeof(float) * kDynMaxChunk));
+    configured = true;
+  }
+  const int per = (int)(n / B);
+  const size_t smem = sizeof(float) * (size_t)((per + DYN_CLUSTER - 1) / DYN_CLUSTER);
+  const dim3 grid((unsigned)B * DYN_CLUSTER);
+  if (x0_hist != nullptr)
+    xu_launch(sampler_step_dynamic_kernel<true>, grid, DYN_THREADS, smem, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z,
+              inp_logsnr, B2, x0_hist, per, p, scale_out);
+  else
+    xu_launch(sampler_step_dynamic_kernel<false>, grid, DYN_THREADS, smem, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z,
+              inp_logsnr, B2, x0_hist, per, p, scale_out);
+}

@@ -8,6 +8,7 @@ Reference behaviour (steps=1000, w=3): per step two model evaluations (cond_mask
 Two samplers that need only tens of steps run through the same device-table step: DDIM (Song et al. 2021; eta = 0
 deterministic, eta = 1 the DDPM posterior) and DPM-Solver++(2M) (Lu et al. 2022), a second-order multistep solver in x0
 that keeps the previous step's clipped x0 on the device.  Both feed the network the log-SNR of the timestep z is at.
+Any of the three can replace the fixed clip of x0 with per-view dynamic thresholding (Imagen, Saharia et al. 2022).
 """
 from __future__ import annotations
 
@@ -91,6 +92,16 @@ def _check_method(method: str, eta: float) -> None:
         raise ValueError(f'eta {eta} is only defined for method ddim, not {method}')
 
 
+def _check_dynamic_threshold(p) -> None:
+    """dynamic_threshold is None (the fixed clip of x0 to [-1, 1]) or a percentile p in (0, 1]."""
+    if p is None:
+        return
+    if isinstance(p, bool) or not isinstance(p, (int, float, np.integer, np.floating)):
+        raise ValueError(f'dynamic_threshold {p!r} is not a number')
+    if not 0.0 < float(p) <= 1.0:          # NaN fails the comparison too
+        raise ValueError(f'dynamic_threshold {p} outside (0, 1]')
+
+
 def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, logsnr_lag: bool = True):
     """The device table of `sched` for `method`: (rows, logsnr_first), rows (len(sched), 8) float64 (the sampler rounds
     them to fp32 once), row k = loop position k = timestep index len-1-k = {c_recip, c_recipm1, c_x0, c_z, sigma,
@@ -159,12 +170,19 @@ class Sampler:
     (DPM-Solver++(2M); its step is `xunet_sampler_step_multistep`, with the previous step's x0 in a device buffer).
     spacing: the Schedule's timestep spacing, 'logsnr' for dpmpp_2m and 'linear' otherwise by default; len(self.sched)
     is the number of forwards a sample runs.  logsnr_lag: the reference's one-step lag of the network's log-SNR input,
-    on by default for ddpm only (see `sampler_table`).  With every default this is the reference sampler."""
+    on by default for ddpm only (see `sampler_table`).  With every default this is the reference sampler.
+
+    dynamic_threshold: None clips x0 to [-1, 1] (the reference).  A percentile p in (0, 1] thresholds x0 per view instead
+    (Saharia et al. 2022, Imagen section 2.3): s = max(1, p-quantile of |x0| over the view), x0 <- clip(x0, -s, s) / s, for
+    every method, in `xunet_sampler_step_dynamic` (the paper uses p = 0.995).  It keeps guided x0 far outside [-1, 1] (large
+    w at high noise) from saturating to +-1; a view whose s is 1 gets the fixed clip's bits."""
 
     def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000, w: float = 3.0,
                  use_graph: bool = True, method: str = 'ddpm', eta: float = 0.0, spacing: str | None = None,
-                 logsnr_lag: bool | None = None):
+                 logsnr_lag: bool | None = None, dynamic_threshold: float | None = None):
         _check_method(method, eta)
+        _check_dynamic_threshold(dynamic_threshold)
+        self.dynamic_threshold = None if dynamic_threshold is None else float(dynamic_threshold)
         self.method, self.eta = method, float(eta)
         self.logsnr_lag = method == 'ddpm' if logsnr_lag is None else bool(logsnr_lag)
         self.model, self.B, self.S, self.w = model, batch_size, img_sidelength, float(w)
@@ -266,7 +284,11 @@ class Sampler:
         head = (e.eps.data_ptr(), self.z.data_ptr(), self._noise.data_ptr() if noise else None, self.z.numel(), self.w,
                 self._tab.data_ptr(), self._pos.data_ptr(), self._seed_base.data_ptr())
         tail = (e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(), 2 * self.B, st)
-        if self._x0_hist is None:
+        if self.dynamic_threshold is not None:
+            hist = None if self._x0_hist is None else self._x0_hist.data_ptr()
+            _lib.check(self.lib.xunet_sampler_step_dynamic(*head, hist, self.B, self.dynamic_threshold, None, *tail),
+                       'sampler_step_dynamic')
+        elif self._x0_hist is None:
             _lib.check(self.lib.xunet_sampler_step_table(*head, *tail), 'sampler_step_table')
         else:
             _lib.check(self.lib.xunet_sampler_step_multistep(*head, self._x0_hist.data_ptr(), *tail), 'sampler_step_multistep')
