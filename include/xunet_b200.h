@@ -286,6 +286,57 @@ int xunet_op_attention_bwd(int dtype, int impl, const void* qkv, const void* res
                            const float* lse, float* dscratch, void* dqkv, int N, int L, int C, int heads, int cross,
                            void* stream);
 
+/* ---- operator-level entry points of the GroupNorm path: each runs the launch the engine runs for that stage ----
+ * GroupNorm(32) pools each group over both frames of a sample: samples are frame pairs (2b, 2b+1), so N is even, and the
+ * per-sample tables below have N/2 rows.  C (the normalised channels) is a multiple of 32.  cstats / bcs tables are
+ * (N/2, C, 2) fp32, stats / bstats (N/2, 32, 2) fp32, params (N/2, C) float4.  Every entry checks its arguments and returns
+ * non-zero (xunet_last_error()) before launching anything. */
+#define XUNET_GN_PLAIN 0   /* y = yhat                                   (yhat = (x - mean) * rstd * gamma + beta) */
+#define XUNET_GN_SWISH 1   /* y = swish(yhat)                                                                       */
+#define XUNET_GN_FILM 2    /* y = dropout(swish(yhat * (1 + scale) + shift)), e = [scale | shift] (N,H,W,2C)       */
+#define XUNET_RS_NONE 0
+#define XUNET_RS_DOWN 1    /* the activation averaged over 2x2 pixels: output (N, H/2, W/2, C); H, W even          */
+#define XUNET_RS_UP 2      /* the activation repeated 2x2 (nearest): output (N, 2H, 2W, C)                          */
+/* xunet_op_conv (stride 1, nseg 1) that also ADDS the per-(sample, channel) [sum y, sum y^2] of the stored output y to cstats
+ * (N/2, Co, 2): emitted by the tensor-core epilogue where the engine's plan does (impl 1 and every 32-row epilogue slice
+ * inside one sample), else by a statistics kernel after the conv. */
+int xunet_op_conv_stats(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y,
+                        float* cstats, int N, int H, int W, int Ci, int Co, int ksize, float alpha, void* stream);
+/* xunet_op_attention that also ADDS the statistics of out to cstats (N/2, C, 2): the tensor-core forward (impl 1) emits them,
+ * the SIMT path runs the statistics kernel after it. */
+int xunet_op_attention_stats(int dtype, int impl, const void* qkv, const void* res, void* out, float* lse, float* cstats, int N,
+                             int L, int C, int heads, int cross, void* stream);
+/* GroupNorm forward from producer-emitted channel statistics: channels [0, ca) of x come with cstats_a (N/2, ca, 2), channels
+ * [ca, C) with cstats_b (N/2, C - ca, 2) (a channel concat; cstats_b may be NULL when ca == C).  Writes y, the group sums to
+ * stats, and, if params_out is not NULL, the fused backward's table {rstd, -mean*rstd, gamma, beta} (no resampling only).
+ * FiLM: e (N,H,W,2C); dropout with keep probability 1 - drop_rate and keep scale 1 / (1 - drop_rate) when train and
+ * drop_rate > 0, its mask hashed from (*seed_dev, op_index, element index in (N,H,W,C)) as xunet_dropout_mask does. */
+int xunet_op_groupnorm(int dtype, const void* x, const float* cstats_a, const float* cstats_b, int ca, const float* gamma,
+                       const float* beta, const void* e, void* y, float* stats, float* params_out, int N, int H, int W, int C,
+                       int mode, int resample, float drop_rate, int op_index, const unsigned long long* seed_dev, int train,
+                       void* stream);
+/* bf16 tensor-core data gradient of a conv (stride 1) whose input is the output of a GroupNorm without resampling, fused with
+ * the norm's first backward pass.  dy (N,H,W,Co), w the conv's Flax kernel (ksize^2, C, Co) in nseg segments as in
+ * xunet_op_conv; gn_x (N,H,W,C) the norm's input, gn_params its params_out table.  Stores dyh (N,H,W,C), the gradient w.r.t.
+ * yhat: alpha * (W^T dy) times swish'(yhat) (SWISH), or through FiLM, dropout and swish (FILM: e, and de (N,H,W,2C) receives
+ * [du * yhat | du], du the gradient w.r.t. the swish input), and ADDS [sum dyh * xhat, sum dyh] per (sample, channel) to bcs
+ * (N/2, C, 2).  The shape must be one whose 32-row epilogue slices stay inside one sample. */
+int xunet_op_conv_dgrad_groupnorm(int dtype, const void* dy, const float* w, const void* gn_x, const float* gn_params, int mode,
+                                  const void* e, void* de, float drop_rate, int op_index, const unsigned long long* seed_dev,
+                                  int train, void* dyh, float* bcs, int N, int H, int W, int C, int Co, int ksize, int nseg,
+                                  float alpha, void* stream);
+/* GroupNorm backward.  x, e, gamma, beta, stats as in the forward; dx = rstd (gamma dyh - S1/cnt - xhat S2/cnt) with
+ * S1 = sum_group gamma dyh, S2 = sum_group gamma dyh xhat, cnt = 2 H W C/32, plus extra_alpha * extra (N,H,W,C) when extra is
+ * not NULL; accumulate: dx += instead of =.  dgamma += sum dyh xhat, dbeta += sum dyh.
+ * bcs != NULL (no resampling): the fused second pass after xunet_op_conv_dgrad_groupnorm, dy holds dyh and bcs its sums.
+ * bcs == NULL: the two-kernel backward from dy, the gradient of the norm's output (N,Ho,Wo,C); bstats receives the group sums
+ * [S1, S2], and a FiLM norm writes (de_accumulate: adds) its gradient to de. */
+int xunet_op_groupnorm_bwd(int dtype, const void* x, const void* e, const void* dy, void* dx, void* de, const float* gamma,
+                           const float* beta, float* dgamma, float* dbeta, const float* stats, float* bstats, const float* bcs,
+                           const void* extra, float extra_alpha, int N, int H, int W, int C, int mode, int resample,
+                           float drop_rate, int op_index, const unsigned long long* seed_dev, int train, int accumulate,
+                           int de_accumulate, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

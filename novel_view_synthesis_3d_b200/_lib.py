@@ -85,6 +85,15 @@ SYMBOLS = {
     'xunet_op_attention': (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p] +
                            [C.c_int] * 5 + [C.c_void_p]),
     'xunet_op_attention_bwd': (C.c_int, [C.c_int, C.c_int] + [C.c_void_p] * 7 + [C.c_int] * 5 + [C.c_void_p]),
+    'xunet_op_conv_stats': (C.c_int, [C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_int] * 6 + [C.c_float, C.c_void_p]),
+    'xunet_op_attention_stats': (C.c_int, [C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_int] * 5 + [C.c_void_p]),
+    'xunet_op_groupnorm': (C.c_int, [C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 6 + [C.c_int] * 6 +
+                           [C.c_float, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    'xunet_op_conv_dgrad_groupnorm': (C.c_int, [C.c_int] + [C.c_void_p] * 4 + [C.c_int] + [C.c_void_p] * 2 +
+                                      [C.c_float, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 2 + [C.c_int] * 7 +
+                                      [C.c_float, C.c_void_p]),
+    'xunet_op_groupnorm_bwd': (C.c_int, [C.c_int] + [C.c_void_p] * 13 + [C.c_float] + [C.c_int] * 6 +
+                               [C.c_float, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
 }
 
 _lib = None

@@ -173,6 +173,42 @@ static void same_pad(int in, int k, int s, int& lo, int& out) {
   lo = total / 2;
 }
 
+// The three helpers below fill the launch arguments of the GroupNorm path; the engine and the operator-level entry points
+// (xunet_op_conv_stats, xunet_op_groupnorm, ...) both use them, so the operator tests run the launches the engine runs.
+
+// a convolution's forward epilogue emits the GroupNorm input statistics of its output (EPI 1); else launch_gn_cstats follows it
+static bool conv_emits_stats(int impl, int nseg, int stride, int N, int Ho, int Wo) {
+  return impl == 1 && nseg == 1 && stride == 1 && conv_tc_stats_supported(0, N, Ho, Wo);
+}
+
+// the data gradient `a` of the conv that consumes a GroupNorm output also runs the norm's first backward pass (EPI 2; EPI 3
+// with the FiLM tensor e and its gradient de): it stores dyh and adds the channel sums to bcs
+static void set_gn_bwd_epilogue(ConvArgs& a, const void* gn_x, const void* gn_params, int mode, const void* e, void* de,
+                                float* bcs, float drop_rate, int op_index, const unsigned long long* seed_dev, int train) {
+  a.gn_x = gn_x;
+  a.gn_params = gn_params;
+  a.gn_swish = mode == GN_SWISH ? 1 : 0;
+  a.cstats = bcs;
+  if (mode == GN_FILM) {
+    a.gn_e = e;
+    a.gn_de = de;
+    a.gn_drop_rate = drop_rate; a.gn_drop_op = op_index; a.gn_seed_dev = seed_dev; a.gn_train = train;
+  }
+}
+
+static GnArgs gn_fill(const void* x, void* y, const void* e, const float* gamma, const float* beta, float* stats, int N, int H,
+                      int W, int C, int mode, int rs, float drop_rate, int op_index, const unsigned long long* seed_dev, int train) {
+  GnArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x = x; a.y = y; a.e = e;
+  a.gamma = gamma; a.beta = beta;
+  a.stats = stats;
+  a.N = N; a.H = H; a.W = W; a.C = C; a.mode = mode; a.rs = rs;
+  a.drop_rate = drop_rate; a.op_index = op_index; a.seed_dev = seed_dev; a.train = train;
+  a.skip_zero = 1;
+  return a;
+}
+
 struct Builder {
   xunet_handle& H;
   explicit Builder(xunet_handle& h) : H(h) {}
@@ -436,7 +472,7 @@ struct Builder {
         t.cstats = H.cstats_bytes;
         H.cstats_bytes += bytes;
         const Op& po = H.ops[t.producer];
-        if (po.kind == OP_CONV) t.cs_fused = po.impl == 1 && po.nseg == 1 && po.stride == 1 && conv_tc_stats_supported(0, t.n, t.h, t.w);
+        if (po.kind == OP_CONV) t.cs_fused = conv_emits_stats(po.impl, po.nseg, po.stride, t.n, t.h, t.w);
         else if (po.kind == OP_ATTN) t.cs_fused = po.impl == 1;
       }
       H.a_cstats = H.alloc(H.cstats_bytes);
@@ -658,15 +694,9 @@ static void run_conv_bwd(const Ctx& c, const Op& o) {
     a.alpha = o.alpha * c.gscale(o.y); a.accumulate = o.acc_x;
     if (o.gnb >= 0) {     // the output is d(GroupNorm output): emit dyh + channel sums instead (see build())
       const Op& gn = c.h->ops[o.gnb];
-      a.gn_x = c.act(gn.x);
-      a.gn_params = c.ws + gn.gnp;
-      a.gn_swish = gn.mode == GN_SWISH ? 1 : 0;
-      a.cstats = reinterpret_cast<float*>(c.ws + gn.bcs);
-      if (gn.mode == GN_FILM) {
-        a.gn_e = c.act(gn.e);
-        a.gn_de = c.grad(gn.e);
-        a.gn_drop_rate = c.h->cfg.dropout; a.gn_drop_op = gn.op_index; a.gn_seed_dev = c.seed_dev; a.gn_train = c.train;
-      }
+      const bool film = gn.mode == GN_FILM;
+      set_gn_bwd_epilogue(a, c.act(gn.x), c.ws + gn.gnp, gn.mode, film ? c.act(gn.e) : nullptr, film ? c.grad(gn.e) : nullptr,
+                          reinterpret_cast<float*>(c.ws + gn.bcs), c.h->cfg.dropout, gn.op_index, c.seed_dev, c.train);
     }
     if (o.impl_d == 1) launch_conv_tc(a, c.ws + o.wC, ds);
     else if (o.impl_d == 3) launch_conv_small(dt, 3, &a, nullptr, ds);
@@ -676,15 +706,8 @@ static void run_conv_bwd(const Ctx& c, const Op& o) {
 
 static GnArgs gn_args(const Ctx& c, const Op& o) {
   const Tensor& x = c.h->tensors[o.x];
-  GnArgs a;
-  memset(&a, 0, sizeof(a));
-  a.x = c.act(o.x); a.y = c.act(o.y); a.e = o.e >= 0 ? c.act(o.e) : nullptr;
-  a.gamma = c.P(o.w); a.beta = c.P(o.b);
-  a.stats = c.aux(o.stats);
-  a.N = x.n; a.H = x.h; a.W = x.w; a.C = x.c; a.mode = o.mode; a.rs = o.rs;
-  a.drop_rate = c.h->cfg.dropout; a.op_index = o.op_index; a.seed_dev = c.seed_dev; a.train = c.train;
-  a.skip_zero = 1;
-  return a;
+  return gn_fill(c.act(o.x), c.act(o.y), o.e >= 0 ? c.act(o.e) : nullptr, c.P(o.w), c.P(o.b), c.aux(o.stats), x.n, x.h, x.w, x.c,
+                 o.mode, o.rs, c.h->cfg.dropout, o.op_index, c.seed_dev, c.train);
 }
 
 static int forward_impl(Ctx& c, float* eps_out) {
@@ -1246,30 +1269,39 @@ static int op_conv_tc(const ConvArgs& a, const float* w, int taps, int Ci, int C
   return op_done(what);
 }
 
-extern "C" int xunet_op_conv(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y,
-                             int N, int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha,
-                             void* stream) {
-  xu_set_kernel_error("");
-  OpScratch scratch;
+// forward of xunet_op_conv; cstats != nullptr: also add the GroupNorm input statistics of the stored output to cstats, emitted by
+// the epilogue where the engine's plan lets it (conv_emits_stats), else by launch_gn_cstats after the conv
+static int op_conv_fwd(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y, float* cstats,
+                       int N, int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha, cudaStream_t s,
+                       const char* what) {
   ConvArgs a;
   a.x = x; a.y = y; a.res = res; a.w = w; a.bias = bias;
   a.N = N; a.Hi = Hi; a.Wi = Wi; a.Ci = Ci; a.Co = Co; a.ks = ksize; a.stride = stride; a.mode = 0;
   a.pad_h = a.pad_w = 0; a.Ho = Hi; a.Wo = Wi;
   if (ksize == 3) { same_pad(Hi, 3, stride, a.pad_h, a.Ho); same_pad(Wi, 3, stride, a.pad_w, a.Wo); }
-  else if (ksize != 1) return fail("xunet_op_conv: ksize must be 1 or 3");
+  else if (ksize != 1) return fail("%s: ksize must be 1 or 3", what);
   a.wCi = Ci; a.wCo = Co; a.segw = Co / nseg; a.alpha = alpha; a.accumulate = 0;
+  const bool fused = cstats != nullptr && conv_emits_stats(impl, nseg, stride, N, a.Ho, a.Wo);
+  if (fused) a.cstats = cstats;
   if (impl == 1) {
-    if (!conv_tc_supported(dtype, 0, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv: shape not supported by the tensor-core kernel");
-    return op_conv_tc(a, w, ksize * ksize, Ci, Co, nseg, (cudaStream_t)stream, "op_conv");
-  }
-  if (impl == 2) {
-    if (conv_cin3_supported(a)) launch_conv_small(dtype, 0, &a, nullptr, (cudaStream_t)stream);
-    else if (conv_cout3_supported(Ci, Co, ksize, stride) && res == nullptr) launch_conv_small(dtype, 2, &a, nullptr, (cudaStream_t)stream);
-    else return fail("xunet_op_conv: not a 3-channel conv");
-    return op_done("op_conv");
-  }
-  launch_conv_simt(dtype, a, (cudaStream_t)stream);
-  return op_done("op_conv");
+    if (!conv_tc_supported(dtype, 0, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("%s: shape not supported by the tensor-core kernel", what);
+    if (op_conv_tc(a, w, ksize * ksize, Ci, Co, nseg, s, what) != 0) return 1;
+  } else if (impl == 2) {
+    if (conv_cin3_supported(a)) launch_conv_small(dtype, 0, &a, nullptr, s);
+    else if (conv_cout3_supported(Ci, Co, ksize, stride) && res == nullptr) launch_conv_small(dtype, 2, &a, nullptr, s);
+    else return fail("%s: not a 3-channel conv", what);
+  } else launch_conv_simt(dtype, a, s);
+  if (cstats != nullptr && !fused) launch_gn_cstats(dtype, y, cstats, N, a.Ho, a.Wo, Co, s);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_conv(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y,
+                             int N, int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha,
+                             void* stream) {
+  xu_set_kernel_error("");
+  OpScratch scratch;
+  return op_conv_fwd(dtype, impl, x, w, bias, res, y, nullptr, N, Hi, Wi, Ci, Co, ksize, stride, nseg, alpha, (cudaStream_t)stream,
+                     "xunet_op_conv");
 }
 
 extern "C" int xunet_op_conv_dgrad(int dtype, int impl, const void* dy, const float* w, void* dx, int N, int Hi, int Wi,
@@ -1350,4 +1382,143 @@ extern "C" int xunet_op_attention_bwd(int dtype, int impl, const void* qkv, cons
     launch_attn_bwd_tc(a, (cudaStream_t)stream);
   } else launch_attn_bwd_simt(dtype, a, (cudaStream_t)stream);
   return op_done("op_attention_bwd");
+}
+
+// ---- operator-level entry points of the GroupNorm path ----------------------------------------------------------------
+static_assert(XUNET_GN_PLAIN == GN_PLAIN && XUNET_GN_SWISH == GN_SWISH && XUNET_GN_FILM == GN_FILM, "GroupNorm modes");
+static_assert(XUNET_RS_NONE == RS_NONE && XUNET_RS_DOWN == RS_DOWN && XUNET_RS_UP == RS_UP, "GroupNorm resampling");
+
+// the checks every GroupNorm-path entry shares: GroupNorm(32) over both frames of each sample
+static int gn_check_shape(const char* what, int dtype, int N, int H, int W, int C) {
+  if (dtype != XUNET_DTYPE_F32 && dtype != XUNET_DTYPE_BF16) return fail("%s: bad dtype %d", what, dtype);
+  if (N < 2 || N % 2 != 0) return fail("%s: N = %d, need an even N >= 2 (two frames per sample)", what, N);
+  if (H < 1 || W < 1) return fail("%s: H = %d, W = %d, need both >= 1", what, H, W);
+  if (C < 32 || C % 32 != 0) return fail("%s: C = %d is not a positive multiple of the 32 groups", what, C);
+  return 0;
+}
+
+static int gn_check_mode(const char* what, int mode, int rs, int H, int W, float drop_rate) {
+  if (mode != XUNET_GN_PLAIN && mode != XUNET_GN_SWISH && mode != XUNET_GN_FILM) return fail("%s: bad mode %d", what, mode);
+  if (rs != XUNET_RS_NONE && rs != XUNET_RS_DOWN && rs != XUNET_RS_UP) return fail("%s: bad resample %d", what, rs);
+  if (rs != XUNET_RS_NONE && mode == XUNET_GN_FILM) return fail("%s: a resampling norm has no FiLM", what);
+  if (rs == XUNET_RS_DOWN && (H % 2 != 0 || W % 2 != 0)) return fail("%s: RS_DOWN needs even H, W (got %d x %d)", what, H, W);
+  if (!(drop_rate >= 0.f && drop_rate < 1.f)) return fail("%s: drop_rate %g outside [0, 1)", what, drop_rate);
+  return 0;
+}
+
+extern "C" int xunet_op_conv_stats(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y,
+                                   float* cstats, int N, int H, int W, int Ci, int Co, int ksize, float alpha, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_conv_stats";
+  if (!x || !w || !y || !cstats) return fail("%s: NULL pointer argument", what);
+  if (gn_check_shape(what, dtype, N, H, W, Co)) return 1;
+  OpScratch scratch;
+  return op_conv_fwd(dtype, impl, x, w, bias, res, y, cstats, N, H, W, Ci, Co, ksize, 1, 1, alpha, (cudaStream_t)stream, what);
+}
+
+extern "C" int xunet_op_attention_stats(int dtype, int impl, const void* qkv, const void* res, void* out, float* lse, float* cstats,
+                                        int N, int L, int C, int heads, int cross, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_attention_stats";
+  if (!qkv || !res || !out || !lse || !cstats) return fail("%s: NULL pointer argument", what);
+  if (gn_check_shape(what, dtype, N, L, 1, C)) return 1;
+  if (heads < 1 || C % heads != 0) return fail("%s: C = %d is not a multiple of heads = %d", what, C, heads);
+  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return fail("%s: shape not supported by the tensor-core kernel", what);
+  OpScratch scratch;
+  AttnArgs a;
+  memset(&a, 0, sizeof(a));
+  a.qkv = qkv; a.res = res; a.out = out; a.lse = lse; a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
+  const bool fused = impl == 1;      // the engine's rule: the tensor-core forward emits the statistics, the SIMT one cannot
+  if (fused) {
+    a.cstats = cstats;
+    launch_attn_fwd_tc(a, (cudaStream_t)stream);
+  } else {
+    launch_attn_fwd_simt(dtype, a, (cudaStream_t)stream);
+    launch_gn_cstats(dtype, out, cstats, N, L, 1, C, (cudaStream_t)stream);
+  }
+  return op_done(what);
+}
+
+extern "C" int xunet_op_groupnorm(int dtype, const void* x, const float* cstats_a, const float* cstats_b, int ca, const float* gamma,
+                                  const float* beta, const void* e, void* y, float* stats, float* params_out, int N, int H, int W,
+                                  int C, int mode, int resample, float drop_rate, int op_index,
+                                  const unsigned long long* seed_dev, int train, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_groupnorm";
+  if (!x || !cstats_a || !gamma || !beta || !y || !stats) return fail("%s: NULL pointer argument", what);
+  if (gn_check_shape(what, dtype, N, H, W, C) || gn_check_mode(what, mode, resample, H, W, drop_rate)) return 1;
+  if (ca < 1 || ca > C) return fail("%s: ca = %d outside [1, C = %d]", what, ca, C);
+  if (ca < C && !cstats_b) return fail("%s: ca = %d < C needs cstats_b", what, ca);
+  if (mode == XUNET_GN_FILM && !e) return fail("%s: a FiLM norm needs e", what);
+  if (mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev) return fail("%s: dropout in training needs seed_dev", what);
+  if (resample != XUNET_RS_NONE && params_out) return fail("%s: a resampling norm has no fused backward (params_out)", what);
+  OpScratch scratch;
+  GnArgs a = gn_fill(x, y, mode == XUNET_GN_FILM ? e : nullptr, gamma, beta, stats, N, H, W, C, mode, resample, drop_rate, op_index,
+                     seed_dev, train ? 1 : 0);
+  a.cstatsA = cstats_a; a.csA = ca;
+  a.cstatsB = ca < C ? cstats_b : nullptr;
+  a.params_out = params_out;
+  launch_gn_apply(dtype, a, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_conv_dgrad_groupnorm(int dtype, const void* dy, const float* w, const void* gn_x, const float* gn_params,
+                                             int mode, const void* e, void* de, float drop_rate, int op_index,
+                                             const unsigned long long* seed_dev, int train, void* dyh, float* bcs, int N, int H,
+                                             int W, int C, int Co, int ksize, int nseg, float alpha, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_conv_dgrad_groupnorm";
+  if (!dy || !w || !gn_x || !gn_params || !dyh || !bcs) return fail("%s: NULL pointer argument", what);
+  if (gn_check_shape(what, dtype, N, H, W, C) || gn_check_mode(what, mode, XUNET_RS_NONE, H, W, drop_rate)) return 1;
+  if ((mode == XUNET_GN_FILM) != (e != nullptr)) return fail("%s: e is given exactly for a FiLM norm", what);
+  if (mode == XUNET_GN_FILM && !de) return fail("%s: a FiLM norm needs de", what);
+  if (mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev) return fail("%s: dropout in training needs seed_dev", what);
+  if (ksize != 1 && ksize != 3) return fail("%s: ksize must be 1 or 3", what);
+  if (nseg < 1 || Co % nseg != 0) return fail("%s: Co = %d is not a multiple of nseg = %d", what, Co, nseg);
+  if (!conv_tc_supported(dtype, 1, N, H, W, C, Co, ksize, 1, nseg) || !conv_tc_stats_supported(1, N, H, W))
+    return fail("%s: shape not supported by the fused tensor-core data gradient", what);
+  OpScratch scratch;
+  ConvArgs a;
+  int pl_h = 0, pl_w = 0, Ho = H, Wo = W;
+  if (ksize == 3) { same_pad(H, 3, 1, pl_h, Ho); same_pad(W, 3, 1, pl_w, Wo); }
+  a.x = dy; a.y = dyh; a.res = nullptr; a.w = w; a.bias = nullptr;
+  a.N = N; a.Hi = Ho; a.Wi = Wo; a.Ci = Co; a.Ho = H; a.Wo = W; a.Co = C;
+  a.ks = ksize; a.stride = 1; a.pad_h = pl_h; a.pad_w = pl_w; a.mode = 1;
+  a.wCi = C; a.wCo = Co; a.segw = Co / nseg; a.alpha = alpha; a.accumulate = 0;
+  set_gn_bwd_epilogue(a, gn_x, gn_params, mode, e, de, bcs, drop_rate, op_index, seed_dev, train ? 1 : 0);
+  return op_conv_tc(a, w, ksize * ksize, C, Co, nseg, (cudaStream_t)stream, what);
+}
+
+extern "C" int xunet_op_groupnorm_bwd(int dtype, const void* x, const void* e, const void* dy, void* dx, void* de, const float* gamma,
+                                      const float* beta, float* dgamma, float* dbeta, const float* stats, float* bstats,
+                                      const float* bcs, const void* extra, float extra_alpha, int N, int H, int W, int C, int mode,
+                                      int resample, float drop_rate, int op_index, const unsigned long long* seed_dev, int train,
+                                      int accumulate, int de_accumulate, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_groupnorm_bwd";
+  if (!x || !dy || !dx || !gamma || !beta || !dgamma || !dbeta || !stats) return fail("%s: NULL pointer argument", what);
+  if (gn_check_shape(what, dtype, N, H, W, C) || gn_check_mode(what, mode, resample, H, W, drop_rate)) return 1;
+  if (bcs && resample != XUNET_RS_NONE) return fail("%s: the fused backward (bcs) has no resampling", what);
+  if (!bcs && !bstats) return fail("%s: the two-kernel backward needs bstats", what);
+  if (!bcs && mode == XUNET_GN_FILM && (!e || !de)) return fail("%s: a FiLM norm needs e and de", what);
+  if (!bcs && mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev)
+    return fail("%s: dropout in training needs seed_dev", what);
+  OpScratch scratch;
+  GnArgs a = gn_fill(x, dx, mode == XUNET_GN_FILM ? e : nullptr, gamma, beta, const_cast<float*>(stats), N, H, W, C, mode, resample,
+                     drop_rate, op_index, seed_dev, train ? 1 : 0);
+  a.dy = dy;
+  a.de = mode == XUNET_GN_FILM ? de : nullptr;
+  a.dgamma = dgamma; a.dbeta = dbeta;
+  a.bstats = bstats;
+  a.accumulate = accumulate ? 1 : 0; a.de_accumulate = de_accumulate ? 1 : 0;
+  a.extra = extra; a.extra_alpha = extra_alpha;
+  if (bcs) {
+    a.bcs = bcs;
+    launch_gn_bwd_apply_pre(dtype, a, (cudaStream_t)stream);
+  } else {
+    a.skip_zero = 0;      // bstats is an output here: the reduction zeroes it first (the engine zeroes all of them at once)
+    launch_gn_bwd_reduce(dtype, a, (cudaStream_t)stream);
+    launch_gn_bwd_apply(dtype, a, (cudaStream_t)stream);
+  }
+  return op_done(what);
 }
