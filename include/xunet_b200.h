@@ -123,6 +123,21 @@ int xunet_backward_mse(xunet_handle* h, const float* params, const xunet_batch* 
                        const float* loss_weight, const unsigned long long* seed_dev, void* workspace, float* grads,
                        float* loss_out, int accumulate, void* stream);
 
+/* Vector-Jacobian product of the forward (jax.vjp / jax.grad over XUNet.apply): the backward seeded with the caller's
+ * d_eps = dL/d(eps_hat) instead of a built-in loss, so any loss on eps_hat is host code.  Must follow xunet_forward on the same
+ * handle, workspace, batch, params and seed_dev; that forward's train flag decides the dropout masks, as in xunet_backward.
+ *   d_eps: device (B,S,S,3) fp32, the gradient of the tensor xunet_forward wrote to eps_out.  The output gradient of the
+ *          network is d_eps rounded once to the activation dtype for the target frame, and zero for the conditioning frame.
+ *   grads: device flat fp32 (param layout), overwritten; accumulate != 0 adds into it exactly as xunet_backward_accumulate does.
+ *   dx, dz: device (B,S,S,3) fp32, or NULL (that input's gradient is not computed): dL/dx and dL/dz of the two input views,
+ *          overwritten.  In bf16 mode the rounding of x and z into the bf16 input tensor counts as identity (straight-through),
+ *          and dx / dz come straight from fp32 accumulators, not rounded to bf16.
+ * Fixed reduction order and no atomics: repeated calls give the same bits.  Errors as xunet_backward: a NULL required pointer,
+ * a handle created with training=0, no xunet_forward yet.  Same bucket hook and graph-capture behaviour as xunet_backward. */
+int xunet_backward_vjp(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
+                       const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate, float* dx, float* dz,
+                       void* stream);
+
 /* Data-parallel hook (north_star: "one NCCL allreduce of the gradient bucket"; the reference's pmap step would place
  * lax.pmean between value_and_grad and apply_gradients, train.py:70-76).  With a callback installed, xunet_backward calls
  *     fn(user, elem_offset, n_elems)

@@ -53,6 +53,8 @@ SYMBOLS = {
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'xunet_backward_mse': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 6 +
                            [C.c_int, C.c_void_p]),
+    'xunet_backward_vjp': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 4 +
+                           [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     'xunet_set_grad_bucket_callback': (C.c_int, [C.c_void_p, BUCKET_FN, C.c_void_p, C.c_longlong]),
     'xunet_grad_bucket_count': (C.c_int, [C.c_void_p]),
     'xunet_count_kernels': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_void_p, C.c_void_p, C.c_void_p,

@@ -27,7 +27,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 107; }
+extern "C" int xunet_version(void) { return 108; }
 
 namespace {
 
@@ -598,6 +598,9 @@ struct Ctx {
   int acc_grads = 0;             // backward: add the parameter gradient into `grads` (xunet_backward_accumulate)
   int mse = 0;                   // backward: seed with the mean-squared loss instead of the Frobenius norm (xunet_backward_mse)
   const float* loss_weight = nullptr;   // mse: per-sample weights (B), nullptr = all 1
+  const float* d_eps = nullptr;  // backward: seed with the caller's dL/d(eps_hat) (B,S,S,3) instead of a loss (xunet_backward_vjp)
+  float* dx = nullptr;           // backward: dL/dx and dL/dz (B,S,S,3) fp32 of the two input views, nullptr = not computed
+  float* dz = nullptr;
   void* act(int t) const { return ws + h->tensors[t].off; }
   void* grad(int t) const { const Tensor& x = h->tensors[t]; return ws + (x.galias >= 0 ? h->tensors[x.galias].goff : x.goff); }
   float gscale(int t) const { return h->tensors[t].gscale; }
@@ -827,7 +830,8 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
     const Op& o = h->ops[i];
     switch (o.kind) {
       case OP_EXTRACT:
-        if (c.mse) launch_loss_mse(dt, c.aux(h->a_eps), noise, c.loss_weight, loss_out, c.grad(o.x), B, S, c.s);
+        if (c.d_eps) launch_vjp_seed(dt, c.d_eps, c.grad(o.x), B, S, c.s);
+        else if (c.mse) launch_loss_mse(dt, c.aux(h->a_eps), noise, c.loss_weight, loss_out, c.grad(o.x), B, S, c.s);
         else launch_loss(dt, c.aux(h->a_eps), noise, c.aux(h->a_sumsq), loss_out, c.grad(o.x), B, S, c.s);
         break;
       case OP_CONV: run_conv_bwd(c, o); break;
@@ -887,6 +891,17 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
         else launch_attn_bwd_simt(dt, a, c.s);
         break;
       }
+      case OP_PACK:
+        if (c.dx != nullptr || c.dz != nullptr) {
+          // adjoint of the pack: the data gradient of the conv that reads the packed views, split back into dx / dz.  Every
+          // writer of that conv's output gradient ran on this stream, and its weight gradient only reads it on the side stream.
+          int k = i + 1;
+          while (h->ops[k].kind != OP_CONV || h->ops[k].x != o.y) ++k;
+          const Op& cv = h->ops[k];
+          launch_conv_cin3_dgrad_unpack(dt, c.grad(cv.y), c.P(cv.w), c.dx, c.dz, B, S, h->tensors[cv.y].c,
+                                        cv.alpha * c.gscale(cv.y), c.s);
+        }
+        break;
       case OP_POSE:
         if (h->tensors[o.y].need_grad)
           launch_pose_emb_bwd(dt, c.grad(o.y), c.G(o.p0), c.G(o.p1), c.G(o.p2), B, S, c.acc_grads, c.s);
@@ -1060,6 +1075,22 @@ extern "C" int xunet_backward_mse(xunet_handle* h, const float* params, const xu
   c.loss_weight = loss_weight;
   XuDetBind bind(h->det);
   return backward_impl(c, noise, loss_out);
+}
+
+extern "C" int xunet_backward_vjp(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
+                                  const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate, float* dx,
+                                  float* dz, void* stream) {
+  if (!h || !params || !batch || !d_eps || !workspace || !grads) return fail("xunet_backward_vjp: null argument");
+  if (!h->training) return fail("xunet_backward_vjp: handle was created with training=0");
+  if (!h->forward_done_train) return fail("xunet_backward_vjp: call xunet_forward first");
+  xu_set_kernel_error("");
+  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
+  c.acc_grads = accumulate ? 1 : 0;
+  c.d_eps = d_eps;
+  c.dx = dx;
+  c.dz = dz;
+  XuDetBind bind(h->det);
+  return backward_impl(c, nullptr, nullptr);
 }
 
 static int count_kernel_nodes(cudaGraph_t g) {

@@ -49,6 +49,10 @@ void launch_wgrad_simt(int dtype, const WgradArgs& a, cudaStream_t s);
 bool conv_cin3_supported(const ConvArgs& a);
 bool conv_cout3_supported(int Ci, int Co, int ks, int stride);
 void launch_conv_small(int dtype, int which, const ConvArgs* c, const WgradArgs* w, cudaStream_t s);
+// data gradient of the input conv 3 -> Co, un-packed: dy (2B,S,S,Co) activation dtype, w the fp32 kernel (3,3,3,Co); rows 2b go
+// to dx (B,S,S,3) fp32, rows 2b+1 to dz; a nullptr output is skipped (both nullptr: nothing is launched)
+void launch_conv_cin3_dgrad_unpack(int dtype, const void* dy, const float* w, float* dx, float* dz, int B, int S, int Co,
+                                   float alpha, cudaStream_t s);
 
 // ---- GroupNorm(32) over both frames (+ SiLU / FiLM / dropout / resample) -----------------------------
 enum { GN_PLAIN = 0, GN_SWISH = 1, GN_FILM = 2 };
@@ -125,6 +129,8 @@ void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_s
 // dO (2B,S,S,3): frame0 = 0, frame1 = fl32(2 weight_b / (B*S*S*3)) * (eps - noise)
 void launch_loss_mse(int dtype, const float* eps, const float* noise, const float* weight, float* loss_out, void* dO, int B,
                      int S, cudaStream_t s);
+// dO (2B,S,S,3): frame0 = 0, frame1 = d_eps (B,S,S,3) fp32, rounded once to the activation dtype
+void launch_vjp_seed(int dtype, const float* d_eps, void* dO, int B, int S, cudaStream_t s);
 // Adam; with ema, also ema = decay*ema + (1-decay)*p_new in the same pass.  warmup > 0: lr_t = lr * min(step - 1, warmup) /
 // warmup; norm_dev: optax.clip_by_global_norm by *norm_dev, where a non-finite *norm_dev leaves every buffer untouched and
 // increments *skipped.  Neither (norm_dev == nullptr, warmup == 0): plain Adam, without the clip / warm-up prologue.

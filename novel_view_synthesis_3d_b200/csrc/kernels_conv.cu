@@ -408,6 +408,90 @@ __global__ void __launch_bounds__(256) conv_cin3_wgrad_kernel(WgradArgs a) {
   }
 }
 
+// Data gradient of the input conv, fused with the un-pack of its (2B,S,S,3) input (the adjoint of pack_input_kernel):
+//   dX[n, p, c] = alpha * sum_tap sum_co dY[n, p - tap, co] * W[tap, c, co]     (SAME padding 1)
+// row n = 2b goes to dx[b], row 2b + 1 to dz[b], both fp32 (B,S,S,3); fsel = 0 / 1 computes only the dx / dz rows, -1 both.
+// A group of LP lanes (a power of two <= 32) owns one pixel: lane l reads the 16-byte chunks l, l + LP, ... of dY at each of the
+// 9 neighbours and keeps three fp32 partial sums, tap by tap; the group then adds its lanes with a fixed xor tree.  The order
+// depends on Co alone, so the bits depend neither on the grid nor on where a pixel sits in it.  Whole warps iterate together
+// (the shuffles need every lane); lanes past the end contribute zeros and store nothing.
+template <typename T>
+__global__ void __launch_bounds__(256) conv_cin3_dgrad_unpack_kernel(const T* __restrict__ dy, const float* __restrict__ w,
+                                                                     float* __restrict__ dx, float* __restrict__ dz, int B, int S,
+                                                                     int Co, int LP, float alpha, int fsel) {
+  xu_grid_dep_sync();
+  extern __shared__ float sw[];                 // [27][Co]: the fp32 kernel (1,3,3,3,Co)
+  for (int i = threadIdx.x; i < 27 * Co; i += 256) sw[i] = w[i];
+  __syncthreads();
+  constexpr int V = VecW<T>::W;
+  const int nchunk = Co / V;
+  const int lane = threadIdx.x & (LP - 1);
+  const int gpw = 32 / LP;                      // pixel groups per warp
+  const long long npix = (long long)(fsel < 0 ? 2 * B : B) * S * S;
+  const long long wstep = (long long)gridDim.x * (blockDim.x >> 5) * gpw;
+  for (long long q0 = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * gpw; q0 < npix; q0 += wstep) {
+    const long long q = q0 + ((threadIdx.x & 31) / LP);
+    const bool valid = q < npix;
+    const long long img = valid ? q / ((long long)S * S) : 0;
+    const int pix = valid ? (int)(q - img * S * S) : 0;
+    const int iy = pix / S, ix = pix - iy * S;
+    const long long b = fsel < 0 ? img >> 1 : img;
+    const int f = fsel < 0 ? (int)(img & 1) : fsel;
+    const long long n = 2 * b + f;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+    if (valid) {
+#pragma unroll 1
+      for (int tap = 0; tap < 9; ++tap) {
+        const int oy = iy + 1 - tap / 3, ox = ix + 1 - tap % 3;
+        if (oy < 0 || oy >= S || ox < 0 || ox >= S) continue;
+        const T* src = dy + ((n * S + oy) * S + ox) * Co;
+        const float* wt = sw + tap * 3 * Co;
+        for (int k = lane; k < nchunk; k += LP) {
+          float d[V];
+          VecW<T>::unpack(VecW<T>::ldg(src + k * V), d);
+#pragma unroll
+          for (int j4 = 0; j4 < V; j4 += 4) {
+            const float4 w0 = *reinterpret_cast<const float4*>(wt + k * V + j4);
+            const float4 w1 = *reinterpret_cast<const float4*>(wt + Co + k * V + j4);
+            const float4 w2 = *reinterpret_cast<const float4*>(wt + 2 * Co + k * V + j4);
+            a0 = fmaf(d[j4], w0.x, a0); a0 = fmaf(d[j4 + 1], w0.y, a0); a0 = fmaf(d[j4 + 2], w0.z, a0); a0 = fmaf(d[j4 + 3], w0.w, a0);
+            a1 = fmaf(d[j4], w1.x, a1); a1 = fmaf(d[j4 + 1], w1.y, a1); a1 = fmaf(d[j4 + 2], w1.z, a1); a1 = fmaf(d[j4 + 3], w1.w, a1);
+            a2 = fmaf(d[j4], w2.x, a2); a2 = fmaf(d[j4 + 1], w2.y, a2); a2 = fmaf(d[j4 + 2], w2.z, a2); a2 = fmaf(d[j4 + 3], w2.w, a2);
+          }
+        }
+      }
+    }
+    for (int o = LP >> 1; o > 0; o >>= 1) {     // lanes i and i^o add the same two values: every lane ends with the same bits
+      a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+      a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+      a2 += __shfl_xor_sync(0xffffffffu, a2, o);
+    }
+    if (valid && lane == 0) {
+      float* out = (f ? dz : dx) + ((b * S + iy) * S + ix) * 3;
+      out[0] = alpha * a0; out[1] = alpha * a1; out[2] = alpha * a2;
+    }
+  }
+}
+
+void launch_conv_cin3_dgrad_unpack(int dtype, const void* dy, const float* w, float* dx, float* dz, int B, int S, int Co,
+                                   float alpha, cudaStream_t s) {
+  if (dx == nullptr && dz == nullptr) return;
+  const int fsel = (dx != nullptr && dz != nullptr) ? -1 : (dx != nullptr ? 0 : 1);
+  const int nchunk = Co / (dtype == XU_F32 ? 4 : 8);
+  int LP = 1;
+  while (LP * 2 <= nchunk && LP < 32) LP *= 2;
+  const long long npix = (long long)(fsel < 0 ? 2 * B : B) * S * S;
+  const int grid = (int)std::min<long long>(cdiv(npix, 256 / LP), (long long)xu_num_sms() * 4);
+  const size_t sm = sizeof(float) * 27 * Co;
+  if (dtype == XU_F32) {
+    if (sm > 48 * 1024) cudaFuncSetAttribute(conv_cin3_dgrad_unpack_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    xu_launch(conv_cin3_dgrad_unpack_kernel<float>, grid, 256, sm, s, (const float*)dy, w, dx, dz, B, S, Co, LP, alpha, fsel);
+  } else {
+    if (sm > 48 * 1024) cudaFuncSetAttribute(conv_cin3_dgrad_unpack_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    xu_launch(conv_cin3_dgrad_unpack_kernel<bf16>, grid, 256, sm, s, (const bf16*)dy, w, dx, dz, B, S, Co, LP, alpha, fsel);
+  }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256) conv_cout3_fwd_kernel(ConvArgs a) {
   xu_grid_dep_sync();

@@ -1479,6 +1479,23 @@ void launch_loss(int dtype, const float* eps, const float* noise, float* sumsq_s
   else xu_launch(loss_grad_kernel<bf16>, cdiv(total, 256), 256, 0, s, eps, noise, sumsq_scratch, loss_out, (bf16*)dO, B, per);
 }
 
+// the caller's dL/d(eps_hat) as the output gradient (xunet_backward_vjp), in the layout loss_grad_kernel writes:
+// dO frame 1 = round_T(d_eps[b]), dO frame 0 = 0
+template <typename T>
+__global__ void vjp_seed_kernel(const float* __restrict__ d_eps, T* __restrict__ dO, int B, long long per) {
+  xu_grid_dep_sync();
+  const long long total = (long long)B * 2 * per;
+  const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (idx >= total) return;
+  const long long n = idx / per, r = idx - n * per;
+  stf(dO + idx, (n & 1) ? d_eps[(n >> 1) * per + r] : 0.f);
+}
+void launch_vjp_seed(int dtype, const float* d_eps, void* dO, int B, int S, cudaStream_t s) {
+  const long long per = (long long)S * S * 3, total = 2 * B * per;
+  if (dtype == XU_F32) xu_launch(vjp_seed_kernel<float>, cdiv(total, 256), 256, 0, s, d_eps, (float*)dO, B, per);
+  else xu_launch(vjp_seed_kernel<bf16>, cdiv(total, 256), 256, 0, s, d_eps, (bf16*)dO, B, per);
+}
+
 __device__ __forceinline__ double block_sum_fixed(double x, double* red);
 
 // loss = (1/B) sum_b w_b (1/P) sum_i r_bi^2, r = eps - noise (P = S*S*3 per sample; w == nullptr: all 1).  The gradient does

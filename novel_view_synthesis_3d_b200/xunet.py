@@ -259,6 +259,8 @@ class Engine:
         self.loss = torch.zeros(1, **f32)
         self.seed = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.grads = torch.zeros(self.nparams, **f32) if training else None
+        self.dx = self.dz = None  # backward_vjp's input gradients (B,S,S,3), allocated at the first call that asks for them
+        self.forward_count = 0    # forwards run so far: a VJP taken later checks that its forward is still the last one
         self._taps = None
         self._bucket_cb = None    # keeps the ctypes callback object alive while it is installed
 
@@ -312,6 +314,7 @@ class Engine:
         cb = self.cbatch if inputs is None else inputs[0].cbatch[inputs[1]]
         sd = self.seed if seed_dev is None else seed_dev
         st = torch.cuda.current_stream(self.device).cuda_stream
+        self.forward_count += 1
         _lib.check(self.lib.xunet_forward(self.h, flat_params.data_ptr(), C.byref(cb), int(train),
                                           sd.data_ptr(), self.ws.data_ptr(), self.eps.data_ptr(), st), 'xunet_forward')
         return self.eps
@@ -347,6 +350,32 @@ class Engine:
         fn = self.lib.xunet_backward_accumulate if accumulate else self.lib.xunet_backward
         _lib.check(fn(self.h, *args, *tail, st), 'xunet_backward_accumulate' if accumulate else 'xunet_backward')
         return out, self.grads
+
+    def backward_vjp(self, flat_params: torch.Tensor, d_eps: torch.Tensor, *, accumulate: bool = False, dx: bool = False,
+                     dz: bool = False, inputs: Optional[Tuple[InputSlots, int]] = None,
+                     seed_dev: Optional[torch.Tensor] = None):
+        """Vector-Jacobian product of the last forward (xunet_backward_vjp): d_eps = dL/d(eps_hat), a contiguous fp32 device
+        tensor (B,S,S,3).  Returns (self.grads, dx, dz): the parameter gradient (accumulate=True adds into self.grads) and, when
+        asked for, dL/dx and dL/dz of the input views in the engine's own (B,S,S,3) buffers, which the next call overwrites
+        (None when not asked for).  Follows forward() with the same `inputs` and `seed_dev`, like backward()."""
+        if not self.training:
+            raise RuntimeError('engine was built with training=False')
+        shape = (self.B, self.S, self.S, 3)
+        if not (isinstance(d_eps, torch.Tensor) and d_eps.is_cuda and d_eps.dtype == torch.float32 and d_eps.is_contiguous()
+                and tuple(d_eps.shape) == shape):
+            raise ValueError(f'd_eps must be a contiguous fp32 CUDA tensor of shape {shape}')
+        if dx and self.dx is None:
+            self.dx = torch.zeros(shape, dtype=torch.float32, device=self.device)
+        if dz and self.dz is None:
+            self.dz = torch.zeros(shape, dtype=torch.float32, device=self.device)
+        cb = self.cbatch if inputs is None else inputs[0].cbatch[inputs[1]]
+        sd = self.seed if seed_dev is None else seed_dev
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.xunet_backward_vjp(self.h, flat_params.data_ptr(), C.byref(cb), d_eps.data_ptr(), sd.data_ptr(),
+                                               self.ws.data_ptr(), self.grads.data_ptr(), int(accumulate),
+                                               self.dx.data_ptr() if dx else None, self.dz.data_ptr() if dz else None, st),
+                   'xunet_backward_vjp')
+        return self.grads, (self.dx if dx else None), (self.dz if dz else None)
 
     def count_kernels(self, flat_params: torch.Tensor) -> Tuple[int, int]:
         """(forward, backward) kernel launches of this plan, counted from a throw-away graph capture."""
@@ -409,8 +438,8 @@ class XUNet:
     def param_spec(self, S: int, B: int = 1) -> "OrderedDict[str, Tuple[Tuple[int, ...], int]]":
         return self.engine(B, S, False).spec
 
-    def tree_from_flat(self, flat: torch.Tensor, S: int, B: int = 1) -> ParamTree:
-        spec = self.param_spec(S, B)
+    def tree_from_flat(self, flat: torch.Tensor, S: int, B: int = 1, spec=None) -> ParamTree:
+        spec = self.param_spec(S, B) if spec is None else spec
         leaves = {name: flat[off: off + int(np.prod(shape))].view(shape) for name, (shape, off) in spec.items()}
         tree = ParamTree(_nest(leaves))
         tree.flat, tree.spec = flat, spec
@@ -471,3 +500,70 @@ class XUNet:
             return eng.forward(flat, train=train, seed=seed).clone()
         finally:
             eng.set_rays(None)
+
+    # ---- vector-Jacobian products ------------------------------------------------------------------------
+    def _train_forward(self, flat: torch.Tensor, batch, cond_mask, train: bool, rngs, rays):
+        """The forward a VJP differentiates, on the training engine: (engine, eps_hat copy, the engine's forward count)."""
+        x = batch['x']
+        B, S = int(x.shape[0]), int(x.shape[1])
+        if tuple(np.shape(cond_mask)) != (B,):
+            raise AssertionError(f'cond_mask.shape == (B,) violated: {np.shape(cond_mask)}')   # model/xunet.py:176
+        eng = self.engine(B, S, True)
+        with torch.no_grad():
+            eng.load_inputs({k: batch[k].detach() if isinstance(batch[k], torch.Tensor) else batch[k] for k in BATCH_KEYS},
+                            cond_mask=cond_mask.detach() if isinstance(cond_mask, torch.Tensor) else cond_mask)
+        eng.set_rays(rays if rays is not None else batch.get('rays'))
+        seed = _seed_of(rngs.get('dropout') if isinstance(rngs, dict) else rngs)
+        try:
+            eps = eng.forward(flat.detach(), train=train, seed=seed).clone()
+        finally:
+            eng.set_rays(None)
+        return eng, eps, eng.forward_count
+
+    @staticmethod
+    def _check_current(eng: Engine, count: int):
+        if eng.forward_count != count:
+            raise RuntimeError(f'another forward ran on this engine since the one being differentiated (forward {count}, now '
+                               f'{eng.forward_count}): its activations are gone; run the forward again')
+
+    def vjp(self, variables, batch, *, cond_mask, train: bool, rngs=None, rays=None):
+        """jax.vjp over XUNet.apply: returns (eps_hat, vjp_fn).  vjp_fn(d_eps), d_eps = dL/d(eps_hat) a contiguous fp32 device
+        tensor (B,S,S,3), returns (ParamTree of a copy of dL/dparams, {'x': dL/dx, 'z': dL/dz}); it may be called more than once,
+        as long as no other forward has run on the training engine engine(B, S, True) in between (else RuntimeError)."""
+        x = batch['x']
+        B, S = int(x.shape[0]), int(x.shape[1])
+        flat = self.flat_from_tree(variables['params'], S, B)
+        eng, eps, count = self._train_forward(flat, batch, cond_mask, train, rngs, rays)
+
+        def vjp_fn(d_eps):
+            self._check_current(eng, count)
+            grads, dx, dz = eng.backward_vjp(flat.detach(), d_eps, dx=True, dz=True)
+            return self.tree_from_flat(grads.clone(), S, B, spec=eng.spec), {'x': dx.clone(), 'z': dz.clone()}
+
+        return eps, vjp_fn
+
+    def apply_autograd(self, flat_params: torch.Tensor, batch, *, cond_mask, train: bool, rngs=None, rays=None) -> torch.Tensor:
+        """XUNet.apply as a torch.autograd.Function on the training engine: eps_hat (B,S,S,3) with a grad_fn, so that
+        loss(eps_hat).backward() fills flat_params.grad and, for CUDA tensors batch['x'] / batch['z'] that require grad, their
+        .grad.  Runs the same engine calls as vjp() (forward, then xunet_backward_vjp); the backward is once-differentiable and
+        raises RuntimeError if another forward has run on the engine in between."""
+        return _XUNetVJP.apply(flat_params, batch['x'], batch['z'], self, batch, cond_mask, train, rngs, rays)
+
+
+class _XUNetVJP(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, flat_params, x, z, model, batch, cond_mask, train, rngs, rays):
+        eng, eps, count = model._train_forward(flat_params, dict(batch, x=x, z=z), cond_mask, train, rngs, rays)
+        ctx.eng, ctx.count = eng, count
+        ctx.save_for_backward(flat_params)        # an in-place update of the parameters before backward() then raises
+        return eps
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_eps):
+        XUNet._check_current(ctx.eng, ctx.count)
+        flat, = ctx.saved_tensors
+        need_p, need_x, need_z = ctx.needs_input_grad[:3]
+        grads, dx, dz = ctx.eng.backward_vjp(flat.detach(), d_eps.to(torch.float32).contiguous(), dx=need_x, dz=need_z)
+        return (grads.clone() if need_p else None, dx.clone() if need_x else None, dz.clone() if need_z else None,
+                None, None, None, None, None, None)
