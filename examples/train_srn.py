@@ -8,6 +8,7 @@ state (state<step>: params, Adam moments and count, EMA, cond_mask streams) that
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --max-grad-norm 1 --warmup-steps 5000 --ema-decay 0.9999
     python examples/train_srn.py cars_train_val --batch 4 --side 128 --grad-accum-steps 8     # 32 samples per update
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --loss mse --min-snr-gamma 5
+    python examples/train_srn.py cars_train_val --batch 8 --side 64 --device-data --data-cache cars64.cache
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_srn.py cars_train_val
 """
 import argparse
@@ -44,6 +45,11 @@ def main():
                     help="training loss: the reference's ||eps_hat - noise||_F, or the mean squared error of DDPM / 3DiM")
     ap.add_argument('--min-snr-gamma', type=float, default=None,
                     help='with --loss mse: weight each sample by min(SNR_t, G) / SNR_t (min-SNR-gamma, e.g. 5)')
+    ap.add_argument('--device-data', action='store_true',
+                    help='decode every view once into GPU memory and draw, gather and noise each batch inside the step; '
+                         'the ranks then split one global batch per update instead of each reading its own stream')
+    ap.add_argument('--data-cache', default=None, help='with --device-data: directory of the decoded views, reused by later runs')
+    ap.add_argument('--data-seed', type=int, default=0, help='with --device-data: seed of the data order')
     ap.add_argument('--resume', action='store_true', help='continue from the latest state<step> checkpoint')
     ap.add_argument('--ckpt', default='checkpoints')
     a = ap.parse_args()
@@ -51,12 +57,22 @@ def main():
         ap.error('--min-snr-gamma needs --loss mse')
     local = xdist.init_from_env('nccl')
     rank, world = xdist.rank(), xdist.world_size()
-    ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50, seed=rank)      # train.py:99-104
     model = P.XUNet(dtype=a.dtype)
     state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model, ema_decay=a.ema_decay,
                                  max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps, loss=a.loss)
     if a.resume and P.checkpoint.restore_train_state(a.ckpt, state) is not None and rank == 0:
         print(f'resumed from step {state.step}')
+    if a.device_data:
+        # the data order follows (--data-seed, update count), so --resume continues it exactly
+        store = P.DeviceScenes(a.folder, a.side, max_observations_per_instance=50, cache=a.data_cache)
+        step = P.TrainStep(state, grad_accum_steps=a.grad_accum_steps, data=store, data_seed=a.data_seed,
+                           min_snr_gamma=a.min_snr_gamma)
+        for it in range(state.step, a.steps):
+            loss = step()
+            report(a, state, step, it, loss, rank)
+        finish(state, rank)
+        return
+    ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50, seed=rank)      # train.py:99-104
     step = P.TrainStep(state, grad_accum_steps=a.grad_accum_steps)
     fd = P.ForwardDiffusion(step.eng, min_snr_gamma=a.min_snr_gamma)
     dev_keys = ('z', 'logsnr', 'noise', 'cond_mask') + (('loss_weight',) if fd.loss_weight is not None else ())
@@ -78,15 +94,24 @@ def main():
                      else np.concatenate([m[key] for m in micro]) for key in micro[0]}
         noise, cond_mask, weight = batch.pop('noise'), batch.pop('cond_mask'), batch.pop('loss_weight', None)
         loss = step(batch, noise, cond_mask=cond_mask, loss_weight=weight)
-        if rank == 0 and it % 50 == 0:
-            norm = '' if step.grad_norm is None else f'  grad norm {float(step.grad_norm):.4f}'
-            print(f'{it}: {float(loss):.4f}{norm}')                                                    # train.py:157
-        if it % a.save_every == 0:
-            if rank == 0:
-                P.checkpoint.save_checkpoint(a.ckpt, state.params, step=it, prefix='model', add_device_axis=True)
-                if state.ema_params is not None:
-                    P.checkpoint.save_checkpoint(a.ckpt, state.ema_params, step=it, prefix='ema', add_device_axis=True)
-            P.checkpoint.save_train_state(a.ckpt, state, step=state.step)    # collective: every rank calls it
+        report(a, state, step, it, loss, rank)
+    finish(state, rank)
+
+
+def report(a, state, step, it, loss, rank):
+    """The loss every 50 updates and the checkpoints every --save-every."""
+    if rank == 0 and it % 50 == 0:
+        norm = '' if step.grad_norm is None else f'  grad norm {float(step.grad_norm):.4f}'
+        print(f'{it}: {float(loss):.4f}{norm}')                                                    # train.py:157
+    if it % a.save_every == 0:
+        if rank == 0:
+            P.checkpoint.save_checkpoint(a.ckpt, state.params, step=it, prefix='model', add_device_axis=True)
+            if state.ema_params is not None:
+                P.checkpoint.save_checkpoint(a.ckpt, state.ema_params, step=it, prefix='ema', add_device_axis=True)
+        P.checkpoint.save_train_state(a.ckpt, state, step=state.step)    # collective: every rank calls it
+
+
+def finish(state, rank):
     if rank == 0:
         if state.clip is not None:
             print(f'skipped steps (non-finite gradient norm): {state.skipped_steps}')

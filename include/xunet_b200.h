@@ -257,6 +257,47 @@ int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t
                             const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
                             float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, void* stream);
 
+/* A set of SRN views held in device memory (srn_data.DeviceScenes): item i = view v of instance inst, items of one instance
+ * contiguous, instance after instance.  All pointers are device memory.
+ *   pixels     (n_items, S, S, 3): uint8 (pixel_kind XUNET_PIXELS_U8: the view's 8-bit RGB centre crop, read as
+ *              ((u / 255) - 0.5) * 2 with each fp32 operation rounded once) or fp32 (XUNET_PIXELS_F32: values in [-1, 1]);
+ *   R (n_items, 3, 3), t (n_items, 3): cam->world pose of each item;  K (n_instances, 3, 3): intrinsics rescaled to S;
+ *   first, count (n_instances) int32: first item and number of views of each instance;  item_inst (n_items) int32. */
+#define XUNET_PIXELS_U8 0
+#define XUNET_PIXELS_F32 1
+typedef struct xunet_srn_store {
+  const void* pixels;
+  int pixel_kind;
+  int S;
+  long long n_items;
+  int n_instances;
+  const float* R;
+  const float* t;
+  const float* K;
+  const int* first;
+  const int* count;
+  const int* item_inst;
+} xunet_srn_store;
+
+/* One training micro-batch drawn, gathered and noised on the device: the host loader + xunet_forward_diffusion in one kernel.
+ * step_dev: device int64 holding the 1-based number of the update being run (TrainStep's step counter after its increment);
+ * c = *step_dev - 1 is the Adam count before it.  Sample b of micro-batch j of k, on rank `rank` of `world`, has the draw index
+ *   g = ((c k + j) world + rank) B + b           (the ranks and micro-batches of one update partition [c k world B, (c+1) k world B))
+ * and draws:  epoch = g / N, item = P_{seed,epoch}(g mod N) (a keyed 4-round Feistel bijection of [0, N) with cycle-walking,
+ * so every item is the source once per N draws), (inst, v) = the item's instance and view, v2 = mix(seed, g) mod count[inst]
+ * (uniform over the instance's views, may equal v).  The micro-batch's diffusion seed is s = mix(seed, c k + j, rank).  Then
+ *   out->x[b] = view v, out->R1/t1[b] its pose, out->R2/t2[b] the pose of view v2, out->K[b] = K[inst],
+ *   out->z, noise, out->logsnr, out->cond_mask = exactly xunet_forward_diffusion(view v2 of every sample, seed = s, p_uncond)
+ * and, when given, loss_weight[b] = snr_weight[t_b] (all 1 when snr_weight is NULL), idx_out (B, 3) int32 = (inst, v, v2),
+ * t_out (B) int32 = the drawn timesteps.  The exact mix functions are in csrc/data.cu and restated in numpy by
+ * srn_data.draw_indices / diffusion_seed.  out->rays is ignored; out->x .. K, cond_mask, noise are required.
+ * Errors: a NULL required pointer, B < 1, k < 1, world < 1, rank outside [0, world), j outside [0, k), an empty store, an
+ * unknown pixel_kind.  Deterministic (a function of the store, seed, *step_dev and the integer arguments).  One launch; no
+ * atomics, no allocation, no host sync, graph-capturable. */
+int xunet_srn_batch(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
+                    int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
+                    const xunet_batch* out, float* noise, float* loss_weight, int* idx_out, int* t_out, void* stream);
+
 /* The dropout keep-mask the kernels use for residual-block `op_index` (0/1 floats, device), so tests can
  * hand the identical mask to the oracle (nn.Dropout, model/xunet.py:84). */
 int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,

@@ -5,10 +5,11 @@ from .train import (TrainState, Adam, AdamState, create_train_state, create_samp
                     TrainStep)
 from . import checkpoint, metrics, sampling, srn_data
 from .diffusion import ForwardDiffusion
+from .srn_data import DeviceScenes
 from .metrics import image_metrics
 from .sampling import Sampler, Schedule, cosine_beta_schedule, logsnr_schedule_cosine
 
 __all__ = ['XUNet', 'XUNetConfig', 'SMALL', 'FULL_3DIM', 'ParamTree', 'Engine', 'TrainState', 'Adam', 'AdamState',
            'create_train_state', 'create_sample_data', 'apply_model', 'update_model', 'TrainStep', 'Sampler',
            'Schedule', 'cosine_beta_schedule', 'logsnr_schedule_cosine', 'checkpoint', 'ForwardDiffusion', 'metrics',
-           'image_metrics']
+           'image_metrics', 'DeviceScenes']

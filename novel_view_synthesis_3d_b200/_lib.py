@@ -12,6 +12,7 @@ MAX_LEVELS = 8
 GRAD_NORM_SCRATCH = 1024       # XUNET_GRAD_NORM_SCRATCH: doubles of scratch xunet_grad_global_norm needs
 SAMPLER_DYN_MAX_PER = 256 * 256 * 3     # XUNET_SAMPLER_DYN_MAX_PER: values per view xunet_sampler_step_dynamic takes
 DTYPE_F32, DTYPE_BF16 = 0, 1
+PIXELS_U8, PIXELS_F32 = 0, 1            # XUNET_PIXELS_*: storage of an xunet_srn_store's views
 RAYS = {'v3d130_ij': 0, 'opencv_uv': 1}
 
 
@@ -24,6 +25,12 @@ class XunetConfig(C.Structure):
 
 class XunetBatch(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in ('x', 'z', 'logsnr', 'R1', 't1', 'R2', 't2', 'K', 'cond_mask', 'rays')]
+
+
+class XunetSrnStore(C.Structure):
+    _fields_ = [('pixels', C.c_void_p), ('pixel_kind', C.c_int), ('S', C.c_int), ('n_items', C.c_longlong),
+                ('n_instances', C.c_int), ('R', C.c_void_p), ('t', C.c_void_p), ('K', C.c_void_p), ('first', C.c_void_p),
+                ('count', C.c_void_p), ('item_inst', C.c_void_p)]
 
 
 # void fn(void* user, long long elem_offset, long long n_elems)  -- the data-parallel gradient-bucket hook
@@ -75,6 +82,8 @@ SYMBOLS = {
     'xunet_forward_diffusion': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p, C.c_void_p, C.c_float,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong,
                                           C.c_void_p]),
+    'xunet_srn_batch': (C.c_int, [C.POINTER(XunetSrnStore), C.c_void_p, C.c_ulonglong] + [C.c_int] * 5 +
+                        [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 5),
     'xunet_dropout_mask': (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_ulonglong, C.c_float, C.c_void_p]),
     'xunet_image_metrics': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),

@@ -124,6 +124,24 @@ __device__ __forceinline__ float xu_hash_normal(uint64_t seed, uint64_t i) {
   const float u2 = (float)(h2 >> 40) * (1.0f / 16777216.0f);
   return sqrtf(-2.f * logf(u1)) * cosf(6.28318530717958647692f * u2);
 }
+// ---- forward diffusion (dataset/data_loader.py:92-110), shared by xunet_forward_diffusion and xunet_srn_batch ----------
+// Per-sample hash of sample b under `seed`: it draws the timestep and the cond_mask uniform.
+__device__ __forceinline__ uint64_t xu_fd_sample_hash(uint64_t seed, int b) {
+  return xu_mix64(seed * 0x9E3779B97F4A7C15ULL + 0xABCDEF0123ULL + (uint64_t)b);
+}
+__device__ __forceinline__ int xu_fd_timestep(uint64_t hb) { return (int)(hb % 1000ULL); }
+// logsnr_schedule_cosine(t/1000), logsnr_min=-20, logsnr_max=20 (data_loader.py:94-97), in double like the reference
+__device__ __forceinline__ float xu_fd_logsnr(int t) {
+  const double bb = atan(exp(-10.0)), aa = atan(exp(10.0)) - bb;
+  return (float)(-2.0 * log(tan(aa * ((double)t / 1000.0) + bb)));
+}
+__device__ __forceinline__ float xu_fd_cond_mask(uint64_t hb, float p_uncond) {
+  const float u = (float)(xu_mix64(hb + 0x51ED27ULL) >> 40) * (1.0f / 16777216.0f);
+  return u > p_uncond ? 1.f : 0.f;
+}
+// z of one element: sqrt(abar_t) x0 + sqrt(1 - abar_t) noise
+__device__ __forceinline__ float xu_fd_z(float sa, float x0, float sb, float nz) { return sa * x0 + sb * nz; }
+
 // one 64-bit hash serves the 4 consecutive elements idx4*4 .. idx4*4+3 (16-bit uniforms): bit j of the result = keep
 __host__ __device__ __forceinline__ uint32_t xu_keep4(uint64_t seed, int op_index, uint64_t idx4, float rate) {
   const uint64_t z = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + (uint64_t)(op_index + 1) * 0xD1B54A32D192ED03ULL + idx4);

@@ -1,0 +1,172 @@
+// data.cu -- one training micro-batch drawn from an SRN store in device memory, gathered and forward-diffused (xunet_srn_batch).
+//
+// Grid (chunks, B): CTA (c, b) handles sample b.  Its thread 0 reads the step counter and derives the sample's draw -- source
+// item, target view, diffusion seed and timestep -- into shared memory; the CTA then streams its share of the S*S*3 values:
+// x from the source view, z and noise from the target view (the arithmetic of xunet_forward_diffusion, common.cuh), four
+// values per thread with 16-byte stores (4-byte loads from a uint8 store) when the layout allows.  CTA 0 of each sample also
+// writes the sample's poses, K, logsnr, cond_mask, loss weight and the optional idx / t outputs.  Every output element has one
+// writer and no value is reduced, so the result is deterministic and independent of the grid.
+//
+// The draw functions below are restated in numpy by srn_data.draw_indices / diffusion_seed: change both together.
+#include "xunet_b200.h"
+#include "common.cuh"
+#include "kernels.h"
+
+#define SRN_THREADS 256
+
+// key of round r of the permutation of epoch `epoch`
+__host__ __device__ __forceinline__ uint64_t srn_round_key(uint64_t seed, uint64_t epoch, int r) {
+  return xu_mix64(xu_mix64(seed ^ 0x243F6A8885A308D3ULL) + epoch * 4ULL + (uint64_t)r);
+}
+// P_{seed,epoch}(x) for x in [0, n): a 4-round Feistel network on 2h bits (4^h >= n, h >= 1), cycle-walked back into [0, n)
+__host__ __device__ __forceinline__ uint64_t srn_permute(uint64_t x, uint64_t n, uint64_t seed, uint64_t epoch) {
+  int h = 1;
+  while ((1ULL << (2 * h)) < n) ++h;
+  const uint64_t mask = (1ULL << h) - 1ULL;
+  uint64_t key[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) key[r] = srn_round_key(seed, epoch, r);
+  do {
+    uint64_t L = x >> h, R = x & mask;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const uint64_t F = xu_mix64(R ^ key[r]) & mask;
+      const uint64_t nl = R;
+      R = L ^ F;
+      L = nl;
+    }
+    x = (L << h) | R;
+  } while (x >= n);
+  return x;
+}
+// target-view hash of draw g
+__host__ __device__ __forceinline__ uint64_t srn_view_hash(uint64_t seed, uint64_t g) {
+  return xu_mix64(xu_mix64(seed ^ 0x13198A2E03707344ULL) + g);
+}
+// diffusion seed of micro-batch mb = c k + j on rank r
+__host__ __device__ __forceinline__ uint64_t srn_diffusion_seed(uint64_t seed, uint64_t mb, uint64_t rank) {
+  return xu_mix64(xu_mix64(xu_mix64(seed ^ 0xA4093822299F31D0ULL) + mb) + rank);
+}
+
+__device__ __forceinline__ float srn_u8(unsigned int u) { return __fmul_rn(__fsub_rn(__fdiv_rn((float)u, 255.f), .5f), 2.f); }
+
+template <int PIX> __device__ __forceinline__ float4 srn_load4(const void* px, long long off) {
+  if (PIX == XUNET_PIXELS_U8) {
+    const uchar4 u = *reinterpret_cast<const uchar4*>(static_cast<const uint8_t*>(px) + off);
+    return make_float4(srn_u8(u.x), srn_u8(u.y), srn_u8(u.z), srn_u8(u.w));
+  }
+  return *reinterpret_cast<const float4*>(static_cast<const float*>(px) + off);
+}
+template <int PIX> __device__ __forceinline__ float srn_load1(const void* px, long long off) {
+  if (PIX == XUNET_PIXELS_U8) return srn_u8(static_cast<const uint8_t*>(px)[off]);
+  return static_cast<const float*>(px)[off];
+}
+
+template <int PIX>
+__global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store st, const long long* __restrict__ step_dev,
+                                                                unsigned long long seed, int j, int k, int rank, int world,
+                                                                const float* __restrict__ sqrt_ac,
+                                                                const float* __restrict__ sqrt_1mac, float p_uncond,
+                                                                const float* __restrict__ snr_weight, xunet_batch out,
+                                                                float* __restrict__ noise, float* __restrict__ loss_weight,
+                                                                int* __restrict__ idx_out, int* __restrict__ t_out, int vec) {
+  __shared__ long long s_src, s_tgt;
+  __shared__ unsigned long long s_seed, s_hb;
+  __shared__ int s_inst, s_v, s_v2, s_t;
+  xu_grid_dep_sync();
+  const int b = blockIdx.y, B = gridDim.y;
+  if (threadIdx.x == 0) {
+    const uint64_t c = (uint64_t)(*step_dev - 1);
+    const uint64_t mb = c * (uint64_t)k + (uint64_t)j;
+    const uint64_t g = (mb * (uint64_t)world + (uint64_t)rank) * (uint64_t)B + (uint64_t)b;
+    const uint64_t n = (uint64_t)st.n_items;
+    const long long item = (long long)srn_permute(g % n, n, seed, g / n);
+    const int inst = st.item_inst[item];
+    const int v2 = (int)(srn_view_hash(seed, g) % (uint64_t)st.count[inst]);
+    const uint64_t s = srn_diffusion_seed(seed, mb, (uint64_t)rank);
+    const uint64_t hb = xu_fd_sample_hash(s, b);
+    s_src = item;
+    s_tgt = (long long)st.first[inst] + v2;
+    s_inst = inst;
+    s_v = (int)(item - st.first[inst]);
+    s_v2 = v2;
+    s_seed = s;
+    s_hb = hb;
+    s_t = xu_fd_timestep(hb);
+  }
+  __syncthreads();
+  const long long per = 3LL * st.S * st.S;
+  const long long src = s_src * per, tgt = s_tgt * per, ob = (long long)b * per;
+  const uint64_t s = s_seed;
+  const int t = s_t;
+  const float sa = sqrt_ac[t], sb = sqrt_1mac[t];
+  float* x = const_cast<float*>(out.x);
+  float* z = const_cast<float*>(out.z);
+  const long long stride = (long long)gridDim.x * SRN_THREADS;
+  if (vec) {
+    for (long long q = (long long)blockIdx.x * SRN_THREADS + threadIdx.x; q < per / 4; q += stride) {
+      const long long i = 4 * q;
+      const float4 xs = srn_load4<PIX>(st.pixels, src + i);
+      const float4 xt = srn_load4<PIX>(st.pixels, tgt + i);
+      float4 nz, zz;
+      nz.x = xu_hash_normal(s, (uint64_t)(ob + i));
+      nz.y = xu_hash_normal(s, (uint64_t)(ob + i + 1));
+      nz.z = xu_hash_normal(s, (uint64_t)(ob + i + 2));
+      nz.w = xu_hash_normal(s, (uint64_t)(ob + i + 3));
+      zz.x = xu_fd_z(sa, xt.x, sb, nz.x);
+      zz.y = xu_fd_z(sa, xt.y, sb, nz.y);
+      zz.z = xu_fd_z(sa, xt.z, sb, nz.z);
+      zz.w = xu_fd_z(sa, xt.w, sb, nz.w);
+      *reinterpret_cast<float4*>(x + ob + i) = xs;
+      *reinterpret_cast<float4*>(z + ob + i) = zz;
+      *reinterpret_cast<float4*>(noise + ob + i) = nz;
+    }
+  } else {
+    for (long long i = (long long)blockIdx.x * SRN_THREADS + threadIdx.x; i < per; i += stride) {
+      const float nz = xu_hash_normal(s, (uint64_t)(ob + i));
+      x[ob + i] = srn_load1<PIX>(st.pixels, src + i);
+      z[ob + i] = xu_fd_z(sa, srn_load1<PIX>(st.pixels, tgt + i), sb, nz);
+      noise[ob + i] = nz;
+    }
+  }
+  if (blockIdx.x == 0) {
+    const int tid = threadIdx.x;
+    if (tid < 9) {
+      const_cast<float*>(out.R1)[b * 9 + tid] = st.R[s_src * 9 + tid];
+      const_cast<float*>(out.R2)[b * 9 + tid] = st.R[s_tgt * 9 + tid];
+      const_cast<float*>(out.K)[b * 9 + tid] = st.K[s_inst * 9 + tid];
+    } else if (tid < 12) {
+      const_cast<float*>(out.t1)[b * 3 + tid - 9] = st.t[s_src * 3 + tid - 9];
+      const_cast<float*>(out.t2)[b * 3 + tid - 9] = st.t[s_tgt * 3 + tid - 9];
+    } else if (tid == 12) {
+      const_cast<float*>(out.logsnr)[b] = xu_fd_logsnr(t);
+      const_cast<float*>(out.cond_mask)[b] = xu_fd_cond_mask(s_hb, p_uncond);
+      if (loss_weight != nullptr) loss_weight[b] = snr_weight != nullptr ? snr_weight[t] : 1.f;
+      if (t_out != nullptr) t_out[b] = t;
+      if (idx_out != nullptr) {
+        idx_out[b * 3 + 0] = s_inst;
+        idx_out[b * 3 + 1] = s_v;
+        idx_out[b * 3 + 2] = s_v2;
+      }
+    }
+  }
+}
+
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
+                      int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
+                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, cudaStream_t s) {
+  const long long per = 3LL * st.S * st.S;
+  const size_t px_align = st.pixel_kind == XUNET_PIXELS_U8 ? 4 : 16;
+  const int vec = per % 4 == 0 && ((uintptr_t)st.pixels % px_align) == 0 && aligned16(out.x) && aligned16(out.z) &&
+                  aligned16(noise);
+  const long long work = vec ? per / 4 : per;
+  const dim3 grid((unsigned)cdiv(work, SRN_THREADS), (unsigned)B);
+  if (st.pixel_kind == XUNET_PIXELS_U8)
+    xu_launch(srn_batch_kernel<XUNET_PIXELS_U8>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world, sqrt_ac,
+              sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec);
+  else
+    xu_launch(srn_batch_kernel<XUNET_PIXELS_F32>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world, sqrt_ac,
+              sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec);
+}

@@ -1231,6 +1231,28 @@ extern "C" int xunet_forward_diffusion(const float* x0, const float* noise_in, c
   return e == cudaSuccess ? 0 : fail("forward_diffusion: CUDA error: %s", cudaGetErrorString(e));
 }
 
+extern "C" int xunet_srn_batch(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
+                               int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
+                               const float* snr_weight, const xunet_batch* out, float* noise, float* loss_weight, int* idx_out,
+                               int* t_out, void* stream) {
+  if (!store || !step_dev || !sqrt_ac || !sqrt_1mac || !out || !noise || !store->pixels || !store->R || !store->t || !store->K ||
+      !store->first || !store->count || !store->item_inst || !out->x || !out->z || !out->logsnr || !out->R1 || !out->t1 ||
+      !out->R2 || !out->t2 || !out->K || !out->cond_mask)
+    return fail("xunet_srn_batch: NULL pointer argument");
+  if (B < 1 || k < 1 || world < 1) return fail("xunet_srn_batch: B = %d, k = %d, world = %d, need all >= 1", B, k, world);
+  if (rank < 0 || rank >= world || j < 0 || j >= k)
+    return fail("xunet_srn_batch: rank = %d of world = %d, j = %d of k = %d out of range", rank, world, j, k);
+  if (store->n_items < 1 || store->n_instances < 1 || store->S < 1)
+    return fail("xunet_srn_batch: empty store (n_items = %lld, n_instances = %d, S = %d)", store->n_items, store->n_instances,
+                store->S);
+  if (store->pixel_kind != XUNET_PIXELS_U8 && store->pixel_kind != XUNET_PIXELS_F32)
+    return fail("xunet_srn_batch: unknown pixel_kind %d", store->pixel_kind);
+  launch_srn_batch(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight, *out, noise,
+                   loss_weight, idx_out, t_out, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("srn_batch: CUDA error: %s", cudaGetErrorString(e));
+}
+
 extern "C" int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,
                                   void* stream) {
   if (!mask_out || n <= 0) return fail("xunet_dropout_mask: bad argument");

@@ -154,6 +154,10 @@ void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise
 void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
                               const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
                               float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, cudaStream_t s);
+// xunet_srn_batch (data.cu): one micro-batch drawn from a device SRN store, gathered and forward-diffused; grid (chunks, B)
+void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
+                      int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
+                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, cudaStream_t s);
 void launch_dropout_mask(float* out, long long n, int op_index, unsigned long long seed, float rate, cudaStream_t s);
 // xunet_image_metrics: one CTA per image, fp64 moments and sums in a fixed order (metrics.cu); 11 <= S <= XUNET_METRICS_MAX_SIDE
 struct MetricsWindow { double w[11]; };   // the normalised 1-D Gaussian weights of the SSIM window

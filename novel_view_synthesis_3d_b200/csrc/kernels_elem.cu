@@ -1785,20 +1785,15 @@ __global__ void __launch_bounds__(256) forward_diffusion_kernel(const float* __r
   const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
   if (idx >= (long long)B * per) return;
   const int b = (int)(idx / per);
-  const uint64_t hb = xu_mix64(seed * 0x9E3779B97F4A7C15ULL + 0xABCDEF0123ULL + (uint64_t)b);
-  const int t = t_in != nullptr ? t_in[b] : (int)(hb % 1000ULL);
+  const uint64_t hb = xu_fd_sample_hash(seed, b);
+  const int t = t_in != nullptr ? t_in[b] : xu_fd_timestep(hb);
   const float nz = noise_in != nullptr ? noise_in[idx] : xu_hash_normal(seed, (uint64_t)idx);
-  z[idx] = sqrt_ac[t] * x0[idx] + sqrt_1mac[t] * nz;
+  z[idx] = xu_fd_z(sqrt_ac[t], x0[idx], sqrt_1mac[t], nz);
   if (noise_out != nullptr) noise_out[idx] = nz;
   if (idx == (long long)b * per) {
-    // logsnr_schedule_cosine(t/1000), logsnr_min=-20, logsnr_max=20 (data_loader.py:94-97), in double like the reference
-    const double bb = atan(exp(-10.0)), aa = atan(exp(10.0)) - bb;
-    logsnr_out[b] = (float)(-2.0 * log(tan(aa * ((double)t / 1000.0) + bb)));
+    logsnr_out[b] = xu_fd_logsnr(t);
     if (t_out != nullptr) t_out[b] = t;
-    if (cond_mask_out != nullptr) {
-      const float u = (float)(xu_mix64(hb + 0x51ED27ULL) >> 40) * (1.0f / 16777216.0f);
-      cond_mask_out[b] = u > p_uncond ? 1.f : 0.f;
-    }
+    if (cond_mask_out != nullptr) cond_mask_out[b] = xu_fd_cond_mask(hb, p_uncond);
   }
 }
 void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,

@@ -145,3 +145,238 @@ class SRNScenes:
         threading.Thread(target=work, daemon=True).start()
         while True:
             yield q.get()
+
+
+# ---- device-resident training data --------------------------------------------------------------------------------------
+# DeviceScenes holds every view of an SRN tree in GPU memory; xunet_srn_batch (csrc/data.cu) draws, gathers and noises one
+# micro-batch from it inside the training step.  The draw order is a function of (seed, Adam count, micro-batch, rank), so a
+# resumed run sees the same data as an uninterrupted one.  The functions below restate the kernel's draw in numpy.
+
+_M64 = 0xFFFFFFFFFFFFFFFF
+
+
+def _u64(x) -> np.ndarray:
+    return np.asarray(x, dtype=np.uint64) if not isinstance(x, int) else np.asarray(x & _M64, dtype=np.uint64)
+
+
+def mix64(z) -> np.ndarray:
+    """xu_mix64 (csrc/common.cuh) on uint64 arrays, wrapping like the device."""
+    z = _u64(z)
+    with np.errstate(over='ignore'):
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return z ^ (z >> np.uint64(31))
+
+
+def _add(a, b) -> np.ndarray:
+    with np.errstate(over='ignore'):
+        return _u64(a) + _u64(b)
+
+
+def permute(x, n: int, seed: int, epoch) -> np.ndarray:
+    """P_{seed,epoch}(x) of the kernel (srn_permute): a keyed 4-round Feistel bijection of [0, 4^h) with 4^h >= n, h >= 1,
+    cycle-walked back into [0, n).  x, epoch: integer arrays (broadcast together)."""
+    x, epoch = np.broadcast_arrays(_u64(x), _u64(epoch))
+    h = 1
+    while (1 << (2 * h)) < n:
+        h += 1
+    mask, hh = np.uint64((1 << h) - 1), np.uint64(h)
+    with np.errstate(over='ignore'):
+        base = mix64(_u64(seed) ^ np.uint64(0x243F6A8885A308D3))
+        keys = [mix64(base + epoch * np.uint64(4) + np.uint64(r)) for r in range(4)]
+
+    def rounds(y, ks):
+        L, R = y >> hh, y & mask
+        for k in ks:
+            L, R = R, L ^ (mix64(R ^ k) & mask)
+        return (L << hh) | R
+
+    y = rounds(x.copy(), keys)
+    out = y >= np.uint64(n)
+    while out.any():
+        y[out] = rounds(y[out], [k[out] for k in keys])
+        out = y >= np.uint64(n)
+    return y
+
+
+def diffusion_seed(seed: int, count: int, j: int, k: int, rank: int) -> int:
+    """Forward-diffusion seed of micro-batch j of the update at Adam count `count` on `rank` (srn_diffusion_seed)."""
+    mb = (int(count) * int(k) + int(j)) & _M64
+    s = mix64(_add(mix64(_add(mix64(_u64(seed) ^ np.uint64(0xA4093822299F31D0)), mb)), int(rank)))
+    return int(s)
+
+
+def draw_indices(first: np.ndarray, count: np.ndarray, item_inst: np.ndarray, seed: int, c: int, j: int, k: int, rank: int,
+                 world: int, B: int) -> np.ndarray:
+    """(B, 3) int64 (inst, v, v2) of micro-batch j of the update at Adam count c on `rank` of `world`: draw index
+    g = ((c k + j) world + rank) B + b, source item P_{seed, g // N}(g mod N), target view mix(seed, g) mod count[inst]."""
+    n = len(item_inst)
+    base = ((int(c) * k + j) * world + rank) * B
+    g = np.array([(base + b) & _M64 for b in range(B)], dtype=np.uint64)
+    item = permute(g % np.uint64(n), n, seed, g // np.uint64(n)).astype(np.int64)
+    inst = item_inst[item].astype(np.int64)
+    h = mix64(_add(mix64(_u64(seed) ^ np.uint64(0x13198A2E03707344)), g))
+    v2 = (h % count[inst].astype(np.uint64)).astype(np.int64)
+    return np.stack([inst, item - first[inst], v2], axis=1)
+
+
+def load_rgb_u8(path: str, sidelength: int) -> Optional[np.ndarray]:
+    """load_rgb's 8-bit RGB centre crop (S,S,3) uint8 when the file is an 8-bit PNG whose crop is already S x S (so load_rgb
+    would not resize it); None otherwise.  u8_to_float(load_rgb_u8(p, S)) equals load_rgb(p, S) bit for bit."""
+    import cv2
+    if not path.lower().endswith('.png'):
+        return None
+    img = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    if img is None:
+        raise FileNotFoundError(path)
+    if img.dtype != np.uint8:
+        return None
+    if img.ndim == 2:
+        img = np.repeat(img[:, :, None], 3, axis=2)
+    img = img[:, :, :3][:, :, ::-1]
+    h, w = img.shape[:2]
+    m = min(h, w)
+    cy, cx = h // 2, w // 2
+    img = img[cy - m // 2: cy + m // 2, cx - m // 2: cx + m // 2]
+    if img.shape[:2] != (sidelength, sidelength):
+        return None
+    return np.ascontiguousarray(img)
+
+
+def u8_to_float(u: np.ndarray) -> np.ndarray:
+    """((u / 255) - 0.5) * 2 in float32, one rounding per operation: load_rgb's arithmetic, and the kernel's."""
+    return (u.astype(np.float32) / np.float32(255.0) - np.float32(0.5)) * np.float32(2.0)
+
+
+def scene_files(ds: SRNScenes) -> List[str]:
+    """Every file a decode of `ds` reads, in order (views, poses, intrinsics per instance)."""
+    out = []
+    for inst in ds.instances:
+        out += [os.path.abspath(p) for p in inst['imgs']] + [os.path.abspath(p) for p in inst['poses']]
+        out.append(os.path.abspath(os.path.join(os.path.dirname(os.path.dirname(inst['imgs'][0])), 'intrinsics.txt')))
+    return out
+
+
+def decode_scenes(ds: SRNScenes, workers: int = 8) -> Dict[str, np.ndarray]:
+    """Decodes every view of `ds` once, on a thread pool (cv2 releases the GIL).  Host only.  Returns
+    pixels (N,S,S,3) uint8 when every view is an 8-bit PNG whose centre crop is S x S, else float32 (load_rgb's output);
+    R (N,3,3), t (N,3) float32; K (I,3,3) float32; first, count (I,) int32; item_inst (N,) int32; storage 'uint8' / 'float32'."""
+    from concurrent.futures import ThreadPoolExecutor
+    S = ds.S
+    imgs = [p for inst in ds.instances for p in inst['imgs']]
+    poses = [p for inst in ds.instances for p in inst['poses']]
+
+    def one(path):
+        u = load_rgb_u8(path, S)
+        return u if u is not None else load_rgb(path, S)
+
+    with ThreadPoolExecutor(max_workers=max(1, int(workers))) as ex:
+        views = list(ex.map(one, imgs))
+        pose = np.stack(list(ex.map(load_pose, poses)))
+    if all(v.dtype == np.uint8 for v in views):
+        pixels, storage = np.stack(views), 'uint8'
+    else:
+        pixels = np.stack([u8_to_float(v) if v.dtype == np.uint8 else v for v in views]).astype(np.float32, copy=False)
+        storage = 'float32'
+    counts = np.array([len(inst['imgs']) for inst in ds.instances], dtype=np.int32)
+    first = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int32)
+    return dict(pixels=pixels, storage=storage, R=np.ascontiguousarray(pose[:, :3, :3], dtype=np.float32),
+                t=np.ascontiguousarray(pose[:, :3, 3], dtype=np.float32),
+                K=np.stack([inst['K'] for inst in ds.instances]).astype(np.float32), first=first, count=counts,
+                item_inst=np.repeat(np.arange(len(counts), dtype=np.int32), counts))
+
+
+_CACHE_ARRAYS = ('pixels', 'R', 't', 'K', 'first', 'count', 'item_inst')
+_CACHE_VERSION = 1
+
+
+def load_or_decode(ds: SRNScenes, cache: Optional[str] = None, workers: int = 8,
+                   max_observations_per_instance: int = -1):
+    """decode_scenes(ds), read from / written to the cache directory `cache` when given: one .npy per array plus meta.json
+    (file list, S, storage kind, max_observations_per_instance).  A cache whose meta.json does not match is decoded again and
+    overwritten.  Files are written under temporary names and renamed, meta.json last.  Returns (arrays, read_from_cache)."""
+    import json
+    meta = dict(version=_CACHE_VERSION, files=scene_files(ds), S=int(ds.S),
+                max_observations_per_instance=int(max_observations_per_instance))
+    if cache is not None:
+        mpath = os.path.join(cache, 'meta.json')
+        try:
+            with open(mpath) as fh:
+                saved = json.load(fh)
+            if {k: saved.get(k) for k in meta} == meta:
+                arrays = {k: np.load(os.path.join(cache, k + '.npy')) for k in _CACHE_ARRAYS}
+                arrays['storage'] = saved['storage']
+                if str(arrays['pixels'].dtype) == saved['storage']:
+                    return arrays, True
+        except (OSError, ValueError, KeyError):
+            pass
+    arrays = decode_scenes(ds, workers)
+    if cache is not None:
+        os.makedirs(cache, exist_ok=True)
+        tag = f'.tmp{os.getpid()}'
+        for k in _CACHE_ARRAYS:
+            with open(os.path.join(cache, k + '.npy' + tag), 'wb') as fh:
+                np.save(fh, arrays[k])
+            os.replace(os.path.join(cache, k + '.npy' + tag), os.path.join(cache, k + '.npy'))
+        with open(os.path.join(cache, 'meta.json' + tag), 'w') as fh:
+            json.dump(dict(meta, storage=arrays['storage']), fh)
+        os.replace(os.path.join(cache, 'meta.json' + tag), os.path.join(cache, 'meta.json'))
+    return arrays, False
+
+
+class DeviceScenes:
+    """Every view of an SRN tree decoded once and held in GPU memory, for TrainStep(data=..): each micro-batch is then drawn,
+    gathered and forward-diffused by one kernel inside the step (xunet_srn_batch), with no host work and no PCIe traffic.
+
+        store = DeviceScenes('cars_train', 64, max_observations_per_instance=50, cache='cars64.cache')
+        step = TrainStep(state, data=store, data_seed=0)
+        loss = step()
+
+    root_or_scenes: a directory (read with SRNScenes) or an SRNScenes (its instances and file order are used as they are).
+    Pixels are stored as uint8 (N,S,S,3) when every view is an 8-bit PNG whose centre crop is already S x S -- the kernel then
+    forms load_rgb's float32 values bit for bit -- and as load_rgb's float32 output otherwise (resized, 16-bit or JPEG views).
+    cache: a directory for the decoded arrays (see load_or_decode), so data-parallel ranks and later runs skip the decode.
+    The store is checked against torch.cuda.mem_get_info before anything is allocated: a store that does not fit raises
+    MemoryError with its size instead of failing halfway."""
+
+    def __init__(self, root_or_scenes, img_sidelength: int, max_observations_per_instance: int = -1, device=None,
+                 workers: int = 8, cache: Optional[str] = None):
+        import torch
+        from . import _lib
+        if isinstance(root_or_scenes, SRNScenes):
+            ds = root_or_scenes
+            if ds.S != img_sidelength:
+                raise ValueError(f'the SRNScenes reads views at S = {ds.S}, the store was asked for S = {img_sidelength}')
+        else:
+            ds = SRNScenes(root_or_scenes, img_sidelength=img_sidelength,
+                           max_observations_per_instance=max_observations_per_instance)
+        self.S = int(img_sidelength)
+        self.device = torch.device(device if device is not None else f'cuda:{torch.cuda.current_device()}')
+        if self.device.type == 'cuda' and self.device.index is None:
+            self.device = torch.device(f'cuda:{torch.cuda.current_device()}')
+        arrays, self.from_cache = load_or_decode(ds, cache, workers, max_observations_per_instance)
+        self.storage = arrays['storage']
+        self.nbytes = sum(int(arrays[k].nbytes) for k in _CACHE_ARRAYS)
+        free, total = torch.cuda.mem_get_info(self.device)
+        if self.nbytes > free:
+            raise MemoryError(f'DeviceScenes needs {self.nbytes} bytes of device memory for {len(arrays["item_inst"])} views at '
+                              f'S = {self.S} ({self.storage}); {self.device} has {free} of {total} bytes free')
+        self.first, self.count, self.item_inst = arrays['first'], arrays['count'], arrays['item_inst']
+        self.n_items, self.n_instances = len(self.item_inst), len(self.first)
+        self.names = [inst['name'] for inst in ds.instances]
+        dev = {k: torch.from_numpy(np.ascontiguousarray(arrays[k])).to(self.device) for k in _CACHE_ARRAYS}
+        self.pixels, self.R, self.t, self.K = dev['pixels'], dev['R'], dev['t'], dev['K']
+        self._first, self._count, self._item_inst = dev['first'], dev['count'], dev['item_inst']
+        self.c_store = _lib.XunetSrnStore(
+            pixels=self.pixels.data_ptr(), pixel_kind=_lib.PIXELS_U8 if self.storage == 'uint8' else _lib.PIXELS_F32,
+            S=self.S, n_items=self.n_items, n_instances=self.n_instances, R=self.R.data_ptr(), t=self.t.data_ptr(),
+            K=self.K.data_ptr(), first=self._first.data_ptr(), count=self._count.data_ptr(),
+            item_inst=self._item_inst.data_ptr())
+
+    def __len__(self) -> int:
+        return self.n_items
+
+    def draws(self, count: int, j: int, k: int, rank: int, world: int, B: int, seed: int = 0) -> np.ndarray:
+        """(B, 3) (inst, v, v2) that micro-batch j of the update at Adam count `count` draws on `rank` of `world` with
+        data_seed `seed` (the host restatement of the kernel's draw)."""
+        return draw_indices(self.first, self.count, self.item_inst, seed, count, j, k, rank, world, B)

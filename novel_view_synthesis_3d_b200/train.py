@@ -10,6 +10,7 @@ dropout seed are fresh per step unless reference_quirks=True (the reference free
 """
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass, replace
 from typing import Optional
 
@@ -18,6 +19,8 @@ import torch
 
 from . import _lib
 from . import dist as xdist
+from .diffusion import min_snr_weights
+from .sampling import cosine_beta_schedule
 from .xunet import XUNet, ParamTree, Engine, InputSlots, check_loss
 
 
@@ -329,11 +332,35 @@ class TrainStep:
 
     A captured graph holds the NCCL kernels of the process group it was captured with: drop the TrainStep (or call
     `release_graphs()`) before `torch.distributed.destroy_process_group()`.
+
+    data=DeviceScenes (srn_data): the step draws its own batches from the views held in device memory and is called with no
+    arguments, `loss = step()`.  Each micro-batch's forward is preceded by one kernel (xunet_srn_batch) that draws the B
+    (source, target) pairs, gathers their pixels and poses and runs the forward diffusion with p_uncond (and, with
+    min_snr_gamma, a state built with loss='mse' gets the min-SNR-gamma weights of the drawn timesteps), all in the graph:
+    no host work and no host->device copy per step (`h2d_bytes` is 0; the host cond_mask stream is not used).  The draw is a
+    function of (data_seed, Adam count, micro-batch, rank): sample b of micro-batch j on rank r of the update at Adam count c
+    has the draw index g = ((c k + j) world + r) B + b, so the ranks and micro-batches of one update partition a global batch
+    of world k B draws (the host loader instead gives every rank its own stream), and each run of N consecutive draws visits
+    every view once as the source, in a keyed random order that changes every such epoch.  Epochs are not aligned with
+    updates: an update may take its first draws from one epoch and the rest from the next (nothing is dropped).  Since the
+    order follows the Adam count, restore_train_state + the same store and data_seed continue the data stream exactly.
     """
 
     def __init__(self, state: TrainState, *, use_graph: bool = True, bucket_mb: float = 128.0, allreduce: bool = True,
-                 grad_accum_steps: int = 1):
+                 grad_accum_steps: int = 1, data=None, data_seed: int = 0, p_uncond: float = 0.1,
+                 min_snr_gamma: Optional[float] = None):
         self.k = check_grad_accum_steps(grad_accum_steps)
+        self.data = data
+        if data is None:
+            if min_snr_gamma is not None:
+                raise ValueError('min_snr_gamma weights the batches a data= step draws; without data= pass loss_weight')
+        else:
+            if state.reference_quirks:
+                raise ValueError('data= draws a fresh cond_mask for every sample; reference_quirks=True freezes it')
+            if min_snr_gamma is not None and state.loss != 'mse':
+                raise ValueError(f"min_snr_gamma needs a state built with loss='mse', this one uses loss={state.loss!r}")
+            if data.S != state.img_sidelength:
+                raise ValueError(f'the store holds views at S = {data.S}, the state trains at S = {state.img_sidelength}')
         self.state = state
         self.mse = state.loss == 'mse'      # the captured graph reads each slot's loss weights in place
         self.eng: Engine = state.model.engine(state.batch_size, state.img_sidelength, True)
@@ -367,6 +394,17 @@ class TrainStep:
         self.mode = None
         self._synced_count = None
         self._sync_counters()
+        if data is not None:
+            if data.device != self.dev:
+                raise ValueError(f'the store lives on {data.device}, the state trains on {self.dev}')
+            self.data_seed = int(data_seed) & 0xFFFFFFFFFFFFFFFF
+            self.p_uncond = float(p_uncond)
+            ac = np.cumprod(1. - cosine_beta_schedule(1000), axis=0)
+            self.sqrt_ac = torch.as_tensor(np.sqrt(ac), dtype=torch.float32).to(self.dev)
+            self.sqrt_1mac = torch.as_tensor(np.sqrt(1. - ac), dtype=torch.float32).to(self.dev)
+            self.snr_weight = None if min_snr_gamma is None else \
+                torch.as_tensor(min_snr_weights(min_snr_gamma), dtype=torch.float32).to(self.dev)
+            self.h2d_bytes = 0
 
     @property
     def grad_norm(self) -> Optional[torch.Tensor]:
@@ -388,6 +426,18 @@ class TrainStep:
             self.seeds.copy_(torch.tensor(seeds, dtype=torch.int64))
             self._synced_count = s.opt_state.count
 
+    def _draw(self, j: int):
+        """Micro-batch j of the current update, drawn from the device store into input slot j (xunet_srn_batch)."""
+        d, inp = self.data, self.inputs.inp[j]
+        ptr = lambda t: None if t is None else t.data_ptr()
+        st = torch.cuda.current_stream(self.dev).cuda_stream
+        _lib.check(self.lib.xunet_srn_batch(C.byref(d.c_store), self.step_dev.data_ptr(), self.data_seed, j, self.k,
+                                            xdist.rank(), self.world, self.eng.B, self.sqrt_ac.data_ptr(),
+                                            self.sqrt_1mac.data_ptr(), self.p_uncond, ptr(self.snr_weight),
+                                            C.byref(self.inputs.cbatch[j]), inp['noise'].data_ptr(),
+                                            inp['loss_weight'].data_ptr() if self.mse else None, None, None, st),
+                   'xunet_srn_batch')
+
     def _fwd_bwd(self):
         e, s = self.eng, self.state
         if not s.reference_quirks:
@@ -400,6 +450,8 @@ class TrainStep:
             for j in range(self.k):
                 last = j == self.k - 1
                 sd = self.seeds[j:j + 1]
+                if self.data is not None:
+                    self._draw(j)
                 e.forward(s.params.flat, train=True, inputs=(self.inputs, j), seed_dev=sd)
                 if last:
                     self._set_hook(hook)
@@ -471,20 +523,28 @@ class TrainStep:
         if retry:
             self._capture()
 
-    def __call__(self, batch: dict, noise, cond_mask=None, loss_weight=None) -> torch.Tensor:
+    def __call__(self, batch: Optional[dict] = None, noise=None, cond_mask=None, loss_weight=None) -> torch.Tensor:
         """One optimisation step on host (or device) inputs; returns the loss as a 0-d device tensor (a view of the step's
         loss slot: read or copy it before the next step).  With grad_accum_steps=k every array has k*B rows, and the loss
-        is the mean of the k micro-batch losses.  loss_weight: per-sample weights of a loss='mse' state (all 1 when None)."""
+        is the mean of the k micro-batch losses.  loss_weight: per-sample weights of a loss='mse' state (all 1 when None).
+        A step built with data= draws its own batches and takes no arguments."""
         s = self.state
-        if self.k > 1:
-            check_accum_batch(batch, noise, cond_mask, self.k, self.eng.B, loss_weight)
-        check_loss_weight(s.loss, loss_weight, self.k * self.eng.B)
-        if self.mse and loss_weight is None:
-            loss_weight = np.ones(self.k * self.eng.B, np.float32)    # the slots may still hold the last call's weights
-        self._sync_counters()
-        # micro-batch j draws the j-th B values of the rank's cond_mask stream
-        mask = np.concatenate([_cond_mask(s, self.eng.B) for _ in range(self.k)]) if cond_mask is None else cond_mask
-        self.h2d_bytes = self.inputs.load(batch, cond_mask=mask, noise=noise, loss_weight=loss_weight)
+        if self.data is not None:
+            if batch is not None or noise is not None or cond_mask is not None or loss_weight is not None:
+                raise ValueError('this TrainStep draws its batches from its data= store: call it with no arguments')
+            self._sync_counters()
+        else:
+            if batch is None or noise is None:
+                raise TypeError('TrainStep() without data= needs a batch and its noise')
+            if self.k > 1:
+                check_accum_batch(batch, noise, cond_mask, self.k, self.eng.B, loss_weight)
+            check_loss_weight(s.loss, loss_weight, self.k * self.eng.B)
+            if self.mse and loss_weight is None:
+                loss_weight = np.ones(self.k * self.eng.B, np.float32)    # the slots may still hold the last call's weights
+            self._sync_counters()
+            # micro-batch j draws the j-th B values of the rank's cond_mask stream
+            mask = np.concatenate([_cond_mask(s, self.eng.B) for _ in range(self.k)]) if cond_mask is None else cond_mask
+            self.h2d_bytes = self.inputs.load(batch, cond_mask=mask, noise=noise, loss_weight=loss_weight)
         if self.use_graph:
             if self.graph_fb is None:
                 self._capture()
