@@ -60,13 +60,18 @@ struct Tensor {
   long long numel() const { return (long long)n * h * w * c; }
 };
 
+// a convolution (N,Hi,Wi,Ci) -> (N,Ho,Wo,Co) with SAME padding, its Co outputs in nseg weight segments (conv_shape)
+struct ConvShape { int N, Hi, Wi, Ci, Ho, Wo, Co, ks, stride, pad_h, pad_w, nseg; };
+struct ConvKernels { ConvKernel fwd = CONV_SIMT, dgrad = CONV_SIMT, wgrad = CONV_SIMT; };
+
 enum OpKind { OP_PACK, OP_LOGSNR, OP_POSE, OP_CONV, OP_EMB, OP_GN, OP_RESAMPLE, OP_CONCAT, OP_ATTN, OP_EXTRACT };
 
 struct Op {
   int kind;
   int x = -1, y = -1, r = -1, e = -1;  // tensors: input, output, second input (residual / concat b), FiLM tensor
   // conv
-  int ks = 1, stride = 1, pad_h = 0, pad_w = 0, nseg = 1, impl = 0, impl_d = 0, impl_w = 0;
+  ConvShape cs = {};
+  ConvKernels k;
   long long wT = -1, wC = -1;         // bf16 weight shadows (workspace byte offsets) for the tensor-core kernels
   long long w = -1, b = -1;            // param offsets (conv W,bias | gn gamma,beta)
   float alpha = 1.f;
@@ -74,7 +79,7 @@ struct Op {
   int mode = 0, rs = 0, op_index = 0;
   long long stats = -1, bstats = -1;   // aux byte offsets
   // attn
-  int cross = 0, heads = 1;
+  int cross = 0, heads = 1, impl = 0;   // impl: 1 tensor cores, 0 SIMT
   long long lse = -1, dscr = -1;
   // pose / logsnr params
   long long p0 = -1, p1 = -1, p2 = -1, p3 = -1;
@@ -173,12 +178,99 @@ static void same_pad(int in, int k, int s, int& lo, int& out) {
   lo = total / 2;
 }
 
-// The three helpers below fill the launch arguments of the GroupNorm path; the engine and the operator-level entry points
-// (xunet_op_conv_stats, xunet_op_groupnorm, ...) both use them, so the operator tests run the launches the engine runs.
+// The helpers below choose the kernel of every conv and attention launch, fill its arguments and launch it, and fill the
+// launch arguments of the GroupNorm path; the engine and the operator-level entry points (xunet_op_conv, xunet_op_attention,
+// xunet_op_groupnorm, ...) both use them, so the operator tests run the launches the engine runs.
+
+static ConvShape conv_shape(int N, int Hi, int Wi, int Ci, int Co, int ks, int stride, int nseg) {
+  ConvShape s = {N, Hi, Wi, Ci, Hi, Wi, Co, ks, stride, 0, 0, nseg};
+  if (ks == 3) { same_pad(Hi, 3, stride, s.pad_h, s.Ho); same_pad(Wi, 3, stride, s.pad_w, s.Wo); }
+  return s;
+}
+
+// the kernels the engine runs for a conv of this shape (res: it adds a residual).  The direct 3-channel kernels and the tensor-core
+// ones never take the same shape.
+static ConvKernels conv_kernels(int dtype, const ConvShape& s, bool res) {
+  ConvKernels k;
+  if (conv_cin3_supported(s.Ci, s.Co, s.ks, s.stride, s.nseg, res)) k.fwd = k.wgrad = CONV_CIN3;
+  if (conv_cout3_supported(s.Ci, s.Co, s.ks, s.stride, s.nseg, res)) k.fwd = k.dgrad = k.wgrad = CONV_COUT3;
+  if (conv_tc_supported(dtype, 0, s.N, s.Hi, s.Wi, s.Ci, s.Co, s.ks, s.stride, s.nseg)) k.fwd = CONV_TC;
+  if (conv_tc_supported(dtype, 1, s.N, s.Hi, s.Wi, s.Ci, s.Co, s.ks, s.stride, s.nseg)) k.dgrad = CONV_TC;
+  if (wgrad_tc_supported(dtype, s.N, s.Hi, s.Wi, s.Ci, s.Co, s.ks, s.stride, s.nseg)) k.wgrad = CONV_TC;
+  return k;
+}
+
+static ConvArgs conv_fwd_args(const ConvShape& s, const void* x, const float* w, const float* bias, const void* res, void* y,
+                              float alpha) {
+  ConvArgs a;
+  a.x = x; a.y = y; a.res = res; a.w = w; a.bias = bias;
+  a.N = s.N; a.Hi = s.Hi; a.Wi = s.Wi; a.Ci = s.Ci; a.Ho = s.Ho; a.Wo = s.Wo; a.Co = s.Co;
+  a.ks = s.ks; a.stride = s.stride; a.pad_h = s.pad_h; a.pad_w = s.pad_w; a.mode = 0;
+  a.wCi = s.Ci; a.wCo = s.Co; a.segw = s.Co / s.nseg;
+  a.alpha = alpha; a.accumulate = 0;
+  return a;
+}
+// the data gradient runs the forward's weights and padding backwards (mode 1): from dY (Ho,Wo,Co) to dX (Hi,Wi,Ci)
+static ConvArgs conv_dgrad_args(const ConvShape& s, const void* dy, const float* w, void* dx, float alpha, int accumulate) {
+  ConvArgs a = conv_fwd_args(s, dy, w, nullptr, nullptr, dx, alpha);
+  a.Hi = s.Ho; a.Wi = s.Wo; a.Ci = s.Co; a.Ho = s.Hi; a.Wo = s.Wi; a.Co = s.Ci;
+  a.mode = 1; a.accumulate = accumulate;
+  return a;
+}
+static WgradArgs conv_wgrad_args(const ConvShape& s, const void* x, const void* dy, float* dw, float* dbias, float alpha) {
+  WgradArgs a;
+  a.x = x; a.dy = dy; a.dw = dw; a.dbias = dbias;
+  a.N = s.N; a.Hi = s.Hi; a.Wi = s.Wi; a.Ci = s.Ci; a.Ho = s.Ho; a.Wo = s.Wo; a.Co = s.Co;
+  a.ks = s.ks; a.stride = s.stride; a.pad_h = s.pad_h; a.pad_w = s.pad_w; a.segw = s.Co / s.nseg;
+  a.alpha = alpha;
+  return a;
+}
+static AttnArgs attn_args(const void* qkv, const void* res, void* out, float* lse, int N, int L, int C, int heads, int cross) {
+  AttnArgs a;
+  memset(&a, 0, sizeof(a));
+  a.qkv = qkv; a.res = res; a.out = out; a.lse = lse;
+  a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
+  return a;
+}
+
+// conv forward (a.mode 0) or data gradient (a.mode 1); shadow: the bf16 weight shadow a tensor-core conv reads
+static void dispatch_conv(int dtype, ConvKernel k, const ConvArgs& a, const void* shadow, cudaStream_t s) {
+  if (k == CONV_TC) launch_conv_tc(a, shadow, s);
+  else if (k == CONV_SIMT) launch_conv_simt(dtype, a, s);
+  else launch_conv_direct(dtype, k, a, s);
+}
+static void dispatch_wgrad(int dtype, ConvKernel k, const WgradArgs& a, cudaStream_t s) {
+  if (k == CONV_TC) launch_wgrad_tc(a, s);
+  else if (k == CONV_SIMT) launch_wgrad_simt(dtype, a, s);
+  else launch_wgrad_direct(dtype, k, a, s);
+}
+static void dispatch_attn_fwd(int dtype, int impl, const AttnArgs& a, cudaStream_t s) {
+  if (impl == 1) launch_attn_fwd_tc(a, s);
+  else launch_attn_fwd_simt(dtype, a, s);
+}
+static void dispatch_attn_bwd(int dtype, int impl, const AttnArgs& a, cudaStream_t s) {
+  if (impl == 1) launch_attn_bwd_tc(a, s);
+  else launch_attn_bwd_simt(dtype, a, s);
+}
+
+// appends a conv's weight to a bf16 shadow table: src its element offset in the fp32 parameters, dstT / dstC the byte offsets of
+// the forward / data-gradient shadows (-1: none)
+static void prep_entry(WeightPrepTable& tab, const ConvShape& s, long long src, long long dstT, long long dstC) {
+  WeightPrepEntry& e = tab.e[tab.n++];
+  e.src = src; e.dstT = dstT; e.dstC = dstC; e.prefix = tab.total;
+  e.Ci = s.Ci; e.Co = s.Co; e.taps = s.ks * s.ks; e.nseg = s.nseg;
+  tab.total += (long long)e.taps * e.Ci * e.Co;
+}
 
 // a convolution's forward epilogue emits the GroupNorm input statistics of its output (EPI 1); else launch_gn_cstats follows it
-static bool conv_emits_stats(int impl, int nseg, int stride, int N, int Ho, int Wo) {
-  return impl == 1 && nseg == 1 && stride == 1 && conv_tc_stats_supported(0, N, Ho, Wo);
+static bool conv_emits_stats(ConvKernel k, const ConvShape& s) {
+  return k == CONV_TC && s.nseg == 1 && s.stride == 1 && conv_tc_stats_supported(0, s.N, s.Ho, s.Wo);
+}
+// likewise the tensor-core attention forward; the SIMT one cannot
+static bool attn_emits_stats(int impl) { return impl == 1; }
+// the data gradient of a conv that consumes a GroupNorm output can also run the norm's first backward pass (set_gn_bwd_epilogue)
+static bool dgrad_fuses_gn_bwd(ConvKernel k, const ConvShape& s) {
+  return k == CONV_TC && s.stride == 1 && conv_tc_stats_supported(1, s.N, s.Hi, s.Wi);
 }
 
 // the data gradient `a` of the conv that consumes a GroupNorm output also runs the norm's first backward pass (EPI 2; EPI 3
@@ -217,26 +309,16 @@ struct Builder {
   int conv(int x, int cout, int ks, int stride, long long w, long long b, int res, float alpha, int nseg,
            const std::string& tap = "") {
     const Tensor tx = H.tensors[x];   // by value: H.tensor() below may reallocate the vector
-    int pl_h = 0, pl_w = 0, ho = tx.h, wo = tx.w;
-    if (ks == 3) { same_pad(tx.h, 3, stride, pl_h, ho); same_pad(tx.w, 3, stride, pl_w, wo); }
-    int y = H.tensor(tx.n, ho, wo, cout, true, tap);
     Op o;
-    o.kind = OP_CONV; o.x = x; o.y = y; o.r = res; o.ks = ks; o.stride = stride; o.pad_h = pl_h; o.pad_w = pl_w;
-    o.w = w; o.b = b; o.alpha = alpha; o.nseg = nseg;
-    if (conv_tc_supported(H.dtype, 0, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) {
-      o.impl = 1;
-      o.wT = H.alloc((long long)ks * ks * tx.c * cout * 2);
-    }
-    if (tx.c == 3 && ks == 3 && stride == 1 && cout % 8 == 0 && res < 0 && nseg == 1) o.impl = o.impl_w = 2;      // direct Cin=3 kernels
-    if (conv_cout3_supported(tx.c, cout, ks, stride) && res < 0 && nseg == 1) o.impl = o.impl_d = o.impl_w = 3;     // direct Cout=3 kernels
-    if (H.training && wgrad_tc_supported(H.dtype, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) o.impl_w = 1;
-    if (H.training && H.tensors[x].need_grad && conv_tc_supported(H.dtype, 1, tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg)) {
-      o.impl_d = 1;
-      o.wC = H.alloc((long long)ks * ks * tx.c * cout * 2);
-    }
+    o.kind = OP_CONV; o.x = x; o.r = res; o.w = w; o.b = b; o.alpha = alpha;
+    o.cs = conv_shape(tx.n, tx.h, tx.w, tx.c, cout, ks, stride, nseg);
+    o.k = conv_kernels(H.dtype, o.cs, res >= 0);
+    o.y = H.tensor(tx.n, o.cs.Ho, o.cs.Wo, cout, true, tap);
+    if (o.k.fwd == CONV_TC) o.wT = H.alloc((long long)ks * ks * tx.c * cout * 2);
+    if (o.k.dgrad == CONV_TC && tx.need_grad) o.wC = H.alloc((long long)ks * ks * tx.c * cout * 2);
     H.ops.push_back(o);
-    H.tensors[y].producer = (int)H.ops.size() - 1;
-    return y;
+    H.tensors[o.y].producer = (int)H.ops.size() - 1;
+    return o.y;
   }
   int gn(int x, int mode, int rs, long long gamma, long long beta, int e, int op_index) {
     const Tensor tx = H.tensors[x];
@@ -472,8 +554,8 @@ struct Builder {
         t.cstats = H.cstats_bytes;
         H.cstats_bytes += bytes;
         const Op& po = H.ops[t.producer];
-        if (po.kind == OP_CONV) t.cs_fused = conv_emits_stats(po.impl, po.nseg, po.stride, t.n, t.h, t.w);
-        else if (po.kind == OP_ATTN) t.cs_fused = po.impl == 1;
+        if (po.kind == OP_CONV) t.cs_fused = conv_emits_stats(po.k.fwd, po.cs);
+        else if (po.kind == OP_ATTN) t.cs_fused = attn_emits_stats(po.impl);
       }
       H.a_cstats = H.alloc(H.cstats_bytes);
       for (Tensor& t : H.tensors) if (t.cstats >= 0) t.cstats += H.a_cstats;
@@ -485,10 +567,7 @@ struct Builder {
       for (const Op& o : H.ops) {
         if (o.kind != OP_CONV || (o.wT < 0 && o.wC < 0)) continue;
         if (tab.n == XU_PREP_MAX) { H.prep.push_back(tab); tab.n = 0; tab.total = 0; }
-        WeightPrepEntry& e = tab.e[tab.n++];
-        e.src = o.w; e.dstT = o.wT; e.dstC = o.wC; e.prefix = tab.total;
-        e.Ci = H.tensors[o.x].c; e.Co = H.tensors[o.y].c; e.taps = o.ks * o.ks; e.nseg = o.nseg;
-        tab.total += (long long)e.taps * e.Ci * e.Co;
+        prep_entry(tab, o.cs, o.w, o.wT, o.wC);
       }
       if (tab.n) H.prep.push_back(tab);
     }
@@ -524,7 +603,7 @@ struct Builder {
         if (users != 1 || consumer < 0) continue;
         Op& cv = H.ops[consumer];
         const Tensor& tx = H.tensors[gn.x];
-        if (cv.impl_d != 1 || cv.stride != 1 || !conv_tc_stats_supported(1, tx.n, tx.h, tx.w) || !H.tensors[gn.y].need_grad) continue;
+        if (!dgrad_fuses_gn_bwd(cv.k.dgrad, cv.cs) || !H.tensors[gn.y].need_grad) continue;
         gn.gnb = consumer; cv.gnb = (int)g;
         gn.gnp = H.alloc(sizeof(float) * 4 * (long long)H.B * tx.c);
         gn.bcs = H.bcs_bytes;
@@ -607,6 +686,7 @@ struct Ctx {
   float* aux(long long off) const { return reinterpret_cast<float*>(ws + off); }
   const float* P(long long off) const { return off < 0 ? nullptr : params + off; }
   float* G(long long off) const { return off < 0 ? nullptr : grads + off; }
+  const void* shadow(long long off) const { return off < 0 ? nullptr : ws + off; }
 };
 
 static void destroy_side(xunet_handle* h) {
@@ -646,20 +726,10 @@ static cudaStream_t ensure_side(xunet_handle* h) {
 }
 
 static void run_conv_fwd(const Ctx& c, const Op& o) {
-  const Tensor& x = c.h->tensors[o.x];
   const Tensor& y = c.h->tensors[o.y];
-  ConvArgs a;
-  a.x = c.act(o.x); a.y = c.act(o.y); a.res = o.r >= 0 ? c.act(o.r) : nullptr;
-  a.w = c.P(o.w); a.bias = c.P(o.b);
-  a.N = x.n; a.Hi = x.h; a.Wi = x.w; a.Ci = x.c; a.Ho = y.h; a.Wo = y.w; a.Co = y.c;
-  a.ks = o.ks; a.stride = o.stride; a.pad_h = o.pad_h; a.pad_w = o.pad_w; a.mode = 0;
-  a.wCi = x.c; a.wCo = y.c; a.segw = y.c / o.nseg;
-  a.alpha = o.alpha; a.accumulate = 0;
+  ConvArgs a = conv_fwd_args(o.cs, c.act(o.x), c.P(o.w), c.P(o.b), o.r >= 0 ? c.act(o.r) : nullptr, c.act(o.y), o.alpha);
   a.cstats = (y.cstats >= 0 && y.cs_fused) ? reinterpret_cast<float*>(c.ws + y.cstats) : nullptr;
-  if (o.impl == 1) launch_conv_tc(a, c.ws + o.wT, c.s);
-  else if (o.impl == 2) launch_conv_small(c.h->dtype, 0, &a, nullptr, c.s);
-  else if (o.impl == 3) launch_conv_small(c.h->dtype, 2, &a, nullptr, c.s);
-  else launch_conv_simt(c.h->dtype, a, c.s);
+  dispatch_conv(c.h->dtype, o.k.fwd, a, c.shadow(o.wT), c.s);
   if (y.cstats >= 0 && !y.cs_fused)     // producer without a statistics epilogue (3-channel input conv, SIMT paths)
     launch_gn_cstats(c.h->dtype, c.act(o.y), reinterpret_cast<float*>(c.ws + y.cstats), y.n, y.h, y.w, y.c, c.s);
 }
@@ -670,10 +740,6 @@ static void run_conv_bwd(const Ctx& c, const Op& o) {
   const int dt = c.h->dtype;
   if (o.r >= 0 && c.h->tensors[o.r].need_grad && !o.fuse_res)
     launch_scale_add(dt, c.grad(o.y), c.grad(o.r), y.numel(), o.alpha, o.acc_r, c.s);
-  WgradArgs w;
-  w.x = c.act(o.x); w.dy = c.grad(o.y); w.dw = c.G(o.w); w.dbias = c.G(o.b);
-  w.N = x.n; w.Hi = x.h; w.Wi = x.w; w.Ci = x.c; w.Ho = y.h; w.Wo = y.w; w.Co = y.c;
-  w.ks = o.ks; w.stride = o.stride; w.pad_h = o.pad_h; w.pad_w = o.pad_w; w.segw = y.c / o.nseg; w.alpha = o.alpha * c.gscale(o.y);
   cudaStream_t ws = c.s;
   if (c.side != nullptr) {   // fork: everything grad(y) depends on is already ordered on the main stream
     cudaEvent_t ev = c.h->ev_pool[c.h->ev_next];
@@ -682,28 +748,19 @@ static void run_conv_bwd(const Ctx& c, const Op& o) {
     cudaStreamWaitEvent(c.side, ev, 0);
     ws = c.side;
   }
-  if (o.impl_w == 1) launch_wgrad_tc(w, ws);
-  else if (o.impl_w == 2) launch_conv_small(dt, 1, nullptr, &w, ws);
-  else if (o.impl_w == 3) launch_conv_small(dt, 4, nullptr, &w, ws);
-  else launch_wgrad_simt(dt, w, ws);
+  const float alpha = o.alpha * c.gscale(o.y);
+  dispatch_wgrad(dt, o.k.wgrad, conv_wgrad_args(o.cs, c.act(o.x), c.grad(o.y), c.G(o.w), c.G(o.b), alpha), ws);
   if (x.need_grad) {
     // the FiLM branch's data gradient feeds only the embedding backward at the very end: keep it on the side stream
     cudaStream_t ds = (o.film && c.side != nullptr) ? c.side : c.s;
-    ConvArgs a;
-    a.x = c.grad(o.y); a.y = c.grad(o.x); a.res = nullptr; a.w = c.P(o.w); a.bias = nullptr;
-    a.N = x.n; a.Hi = y.h; a.Wi = y.w; a.Ci = y.c; a.Ho = x.h; a.Wo = x.w; a.Co = x.c;
-    a.ks = o.ks; a.stride = o.stride; a.pad_h = o.pad_h; a.pad_w = o.pad_w; a.mode = 1;
-    a.wCi = x.c; a.wCo = y.c; a.segw = y.c / o.nseg;
-    a.alpha = o.alpha * c.gscale(o.y); a.accumulate = o.acc_x;
+    ConvArgs a = conv_dgrad_args(o.cs, c.grad(o.y), c.P(o.w), c.grad(o.x), alpha, o.acc_x);
     if (o.gnb >= 0) {     // the output is d(GroupNorm output): emit dyh + channel sums instead (see build())
       const Op& gn = c.h->ops[o.gnb];
       const bool film = gn.mode == GN_FILM;
       set_gn_bwd_epilogue(a, c.act(gn.x), c.ws + gn.gnp, gn.mode, film ? c.act(gn.e) : nullptr, film ? c.grad(gn.e) : nullptr,
                           reinterpret_cast<float*>(c.ws + gn.bcs), c.h->cfg.dropout, gn.op_index, c.seed_dev, c.train);
     }
-    if (o.impl_d == 1) launch_conv_tc(a, c.ws + o.wC, ds);
-    else if (o.impl_d == 3) launch_conv_small(dt, 3, &a, nullptr, ds);
-    else launch_conv_simt(dt, a, ds);
+    dispatch_conv(dt, o.k.dgrad, a, c.shadow(o.wC), ds);
   }
 }
 
@@ -780,13 +837,9 @@ static int forward_impl(Ctx& c, float* eps_out) {
       }
       case OP_ATTN: {
         const Tensor& y = h->tensors[o.y];
-        AttnArgs a;
-        memset(&a, 0, sizeof(a));
-        a.qkv = c.act(o.x); a.res = c.act(o.r); a.out = c.act(o.y); a.lse = c.aux(o.lse);
-        a.N = y.n; a.L = y.h * y.w; a.C = y.c; a.heads = o.heads; a.cross = o.cross;
+        AttnArgs a = attn_args(c.act(o.x), c.act(o.r), c.act(o.y), c.aux(o.lse), y.n, y.h * y.w, y.c, o.heads, o.cross);
         a.cstats = (y.cstats >= 0 && y.cs_fused) ? reinterpret_cast<float*>(c.ws + y.cstats) : nullptr;
-        if (o.impl == 1) launch_attn_fwd_tc(a, c.s);
-        else launch_attn_fwd_simt(dt, a, c.s);
+        dispatch_attn_fwd(dt, o.impl, a, c.s);
         if (y.cstats >= 0 && !y.cs_fused)
           launch_gn_cstats(dt, c.act(o.y), reinterpret_cast<float*>(c.ws + y.cstats), y.n, y.h, y.w, y.c, c.s);
         break;
@@ -882,13 +935,9 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
       case OP_ATTN: {
         const Tensor& y = h->tensors[o.y];
         if (!o.fuse_res) launch_scale_add(dt, c.grad(o.y), c.grad(o.r), y.numel(), XU_RSQRT2, o.acc_r, c.s);
-        AttnArgs a;
-        memset(&a, 0, sizeof(a));
-        a.qkv = c.act(o.x); a.res = c.act(o.r); a.out = c.act(o.y); a.lse = c.aux(o.lse);
+        AttnArgs a = attn_args(c.act(o.x), c.act(o.r), c.act(o.y), c.aux(o.lse), y.n, y.h * y.w, y.c, o.heads, o.cross);
         a.dout = c.grad(o.y); a.dscratch = c.aux(o.dscr); a.dqkv = c.grad(o.x);
-        a.N = y.n; a.L = y.h * y.w; a.C = y.c; a.heads = o.heads; a.cross = o.cross;
-        if (o.impl == 1) launch_attn_bwd_tc(a, c.s);
-        else launch_attn_bwd_simt(dt, a, c.s);
+        dispatch_attn_bwd(dt, o.impl, a, c.s);
         break;
       }
       case OP_PACK:
@@ -1287,39 +1336,47 @@ static int op_done(const char* what) {
   return 0;
 }
 
-// operator-level (test / micro-benchmark) path: the bf16 shadow lives in a process-wide scratch buffer (the engine keeps its
-// shadows in the workspace instead).  With XUNET_OP_CACHE_SHADOW=1 the cast/transposition is skipped when the same weight
-// pointer and shape are used again (benchmarks time the conv kernel alone; weights must not change in between).
-static int op_conv_tc(const ConvArgs& a, const float* w, int taps, int Ci, int Co, int nseg, cudaStream_t s, const char* what) {
+// the public impl of the operator-level conv entries (0 SIMT, 1 tensor cores, 2 a direct 3-channel kernel) -> the kernel to run:
+// for 1 and 2, the engine's choice for the shape, which must be of that kind
+static int op_conv_kernel(int impl, ConvKernel engine, const char* what, ConvKernel& k) {
+  if (impl == 1 && engine != CONV_TC) return fail("%s: shape not supported by the tensor-core kernel", what);
+  if (impl == 2 && engine != CONV_CIN3 && engine != CONV_COUT3) return fail("%s: no direct 3-channel kernel takes this shape", what);
+  k = impl == 1 || impl == 2 ? engine : CONV_SIMT;
+  return 0;
+}
+
+// operator-level (test / micro-benchmark) path: the bf16 shadow of a tensor-core conv lives in a process-wide scratch buffer (the
+// engine keeps its shadows in the workspace instead).  With XUNET_OP_CACHE_SHADOW=1 the cast/transposition is skipped when the
+// same weight pointer and shape are used again (benchmarks time the conv kernel alone; weights must not change in between).
+static int op_dispatch_conv(int dtype, ConvKernel k, const ConvShape& cs, const ConvArgs& a, cudaStream_t s, const char* what) {
   static uint8_t* scratch = nullptr;
   static size_t scratch_bytes = 0;
   static const float* last_w = nullptr;
   static long long last_key[4] = {0, 0, 0, 0};
-  const long long n = (long long)taps * Ci * Co;
-  const size_t need = (size_t)n * 2 * 2 + 1024;
-  if (need > scratch_bytes) {
-    cudaDeviceSynchronize();
-    if (scratch) cudaFree(scratch);
-    if (cudaMalloc(&scratch, need) != cudaSuccess) { scratch = nullptr; scratch_bytes = 0; return fail("%s: cudaMalloc", what); }
-    scratch_bytes = need;
-    last_w = nullptr;
-  }
+  const long long n = (long long)cs.ks * cs.ks * cs.Ci * cs.Co;
   const long long offC = (n * 2 + 255) / 256 * 256;
-  const char* e = getenv("XUNET_OP_CACHE_SHADOW");
-  const bool cache = e && e[0] == '1';
-  const long long key[4] = {taps, Ci, Co, nseg};
-  if (!(cache && last_w == w && memcmp(key, last_key, sizeof(key)) == 0)) {
-    WeightPrepTable* tab = new WeightPrepTable();
-    tab->n = 1; tab->total = n;
-    tab->e[0].src = 0; tab->e[0].dstT = 0; tab->e[0].dstC = offC; tab->e[0].prefix = 0;
-    tab->e[0].Ci = Ci; tab->e[0].Co = Co; tab->e[0].taps = taps; tab->e[0].nseg = nseg;
-    launch_weight_prep(*tab, w, scratch, s);
-    delete tab;
-    last_w = w;
-    memcpy(last_key, key, sizeof(key));
+  if (k == CONV_TC) {
+    const size_t need = (size_t)n * 2 * 2 + 1024;
+    if (need > scratch_bytes) {
+      cudaDeviceSynchronize();
+      if (scratch) cudaFree(scratch);
+      if (cudaMalloc(&scratch, need) != cudaSuccess) { scratch = nullptr; scratch_bytes = 0; return fail("%s: cudaMalloc", what); }
+      scratch_bytes = need;
+      last_w = nullptr;
+    }
+    const char* e = getenv("XUNET_OP_CACHE_SHADOW");
+    const bool cache = e && e[0] == '1';
+    const long long key[4] = {cs.ks * cs.ks, cs.Ci, cs.Co, cs.nseg};
+    if (!(cache && last_w == a.w && memcmp(key, last_key, sizeof(key)) == 0)) {
+      WeightPrepTable tab{};
+      prep_entry(tab, cs, 0, 0, offC);
+      launch_weight_prep(tab, a.w, scratch, s);
+      last_w = a.w;
+      memcpy(last_key, key, sizeof(key));
+    }
   }
-  launch_conv_tc(a, scratch + (a.mode == 0 ? 0 : offC), s);
-  return op_done(what);
+  dispatch_conv(dtype, k, a, k == CONV_TC ? scratch + (a.mode == 0 ? 0 : offC) : nullptr, s);
+  return 0;
 }
 
 // forward of xunet_op_conv; cstats != nullptr: also add the GroupNorm input statistics of the stored output to cstats, emitted by
@@ -1327,24 +1384,15 @@ static int op_conv_tc(const ConvArgs& a, const float* w, int taps, int Ci, int C
 static int op_conv_fwd(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y, float* cstats,
                        int N, int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha, cudaStream_t s,
                        const char* what) {
-  ConvArgs a;
-  a.x = x; a.y = y; a.res = res; a.w = w; a.bias = bias;
-  a.N = N; a.Hi = Hi; a.Wi = Wi; a.Ci = Ci; a.Co = Co; a.ks = ksize; a.stride = stride; a.mode = 0;
-  a.pad_h = a.pad_w = 0; a.Ho = Hi; a.Wo = Wi;
-  if (ksize == 3) { same_pad(Hi, 3, stride, a.pad_h, a.Ho); same_pad(Wi, 3, stride, a.pad_w, a.Wo); }
-  else if (ksize != 1) return fail("%s: ksize must be 1 or 3", what);
-  a.wCi = Ci; a.wCo = Co; a.segw = Co / nseg; a.alpha = alpha; a.accumulate = 0;
-  const bool fused = cstats != nullptr && conv_emits_stats(impl, nseg, stride, N, a.Ho, a.Wo);
+  if (ksize != 1 && ksize != 3) return fail("%s: ksize must be 1 or 3", what);
+  const ConvShape cs = conv_shape(N, Hi, Wi, Ci, Co, ksize, stride, nseg);
+  ConvKernel k;
+  if (op_conv_kernel(impl, conv_kernels(dtype, cs, res != nullptr).fwd, what, k)) return 1;
+  ConvArgs a = conv_fwd_args(cs, x, w, bias, res, y, alpha);
+  const bool fused = cstats != nullptr && conv_emits_stats(k, cs);
   if (fused) a.cstats = cstats;
-  if (impl == 1) {
-    if (!conv_tc_supported(dtype, 0, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("%s: shape not supported by the tensor-core kernel", what);
-    if (op_conv_tc(a, w, ksize * ksize, Ci, Co, nseg, s, what) != 0) return 1;
-  } else if (impl == 2) {
-    if (conv_cin3_supported(a)) launch_conv_small(dtype, 0, &a, nullptr, s);
-    else if (conv_cout3_supported(Ci, Co, ksize, stride) && res == nullptr) launch_conv_small(dtype, 2, &a, nullptr, s);
-    else return fail("%s: not a 3-channel conv", what);
-  } else launch_conv_simt(dtype, a, s);
-  if (cstats != nullptr && !fused) launch_gn_cstats(dtype, y, cstats, N, a.Ho, a.Wo, Co, s);
+  if (op_dispatch_conv(dtype, k, cs, a, s, what)) return 1;
+  if (cstats != nullptr && !fused) launch_gn_cstats(dtype, y, cstats, N, cs.Ho, cs.Wo, Co, s);
   return op_done(what);
 }
 
@@ -1361,60 +1409,33 @@ extern "C" int xunet_op_conv_dgrad(int dtype, int impl, const void* dy, const fl
                                    int Ci, int Co, int ksize, int stride, int nseg, float alpha, int accumulate,
                                    void* stream) {
   xu_set_kernel_error("");
+  const char* what = "xunet_op_conv_dgrad";
   OpScratch scratch;
-  ConvArgs a;
-  int pl_h = 0, pl_w = 0, Ho = Hi, Wo = Wi;
-  if (ksize == 3) { same_pad(Hi, 3, stride, pl_h, Ho); same_pad(Wi, 3, stride, pl_w, Wo); }
-  a.x = dy; a.y = dx; a.res = nullptr; a.w = w; a.bias = nullptr;
-  a.N = N; a.Hi = Ho; a.Wi = Wo; a.Ci = Co; a.Ho = Hi; a.Wo = Wi; a.Co = Ci;
-  a.ks = ksize; a.stride = stride; a.pad_h = pl_h; a.pad_w = pl_w; a.mode = 1;
-  a.wCi = Ci; a.wCo = Co; a.segw = Co / nseg; a.alpha = alpha; a.accumulate = accumulate;
-  if (impl == 1) {
-    if (!conv_tc_supported(dtype, 1, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv_dgrad: shape not supported by the tensor-core kernel");
-    return op_conv_tc(a, w, ksize * ksize, Ci, Co, nseg, (cudaStream_t)stream, "op_conv_dgrad");
-  }
-  if (impl == 2) {
-    if (!conv_cout3_supported(Ci, Co, ksize, stride)) return fail("xunet_op_conv_dgrad: not a Cout=3 conv");
-    launch_conv_small(dtype, 3, &a, nullptr, (cudaStream_t)stream);
-    return op_done("op_conv_dgrad");
-  }
-  launch_conv_simt(dtype, a, (cudaStream_t)stream);
-  return op_done("op_conv_dgrad");
+  const ConvShape cs = conv_shape(N, Hi, Wi, Ci, Co, ksize, stride, nseg);
+  ConvKernel k;
+  if (op_conv_kernel(impl, conv_kernels(dtype, cs, false).dgrad, what, k)) return 1;
+  return op_dispatch_conv(dtype, k, cs, conv_dgrad_args(cs, dy, w, dx, alpha, accumulate), (cudaStream_t)stream, what) ? 1 : op_done(what);
 }
 
 extern "C" int xunet_op_conv_wgrad(int dtype, int impl, const void* x, const void* dy, float* dw, float* dbias, int N,
                                    int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha,
                                    void* stream) {
   xu_set_kernel_error("");
+  const char* what = "xunet_op_conv_wgrad";
   OpScratch scratch;
-  WgradArgs w;
-  int pl_h = 0, pl_w = 0, Ho = Hi, Wo = Wi;
-  if (ksize == 3) { same_pad(Hi, 3, stride, pl_h, Ho); same_pad(Wi, 3, stride, pl_w, Wo); }
-  w.x = x; w.dy = dy; w.dw = dw; w.dbias = dbias;
-  w.N = N; w.Hi = Hi; w.Wi = Wi; w.Ci = Ci; w.Ho = Ho; w.Wo = Wo; w.Co = Co;
-  w.ks = ksize; w.stride = stride; w.pad_h = pl_h; w.pad_w = pl_w; w.segw = Co / nseg; w.alpha = alpha;
-  if (impl == 1) {
-    if (!wgrad_tc_supported(dtype, N, Hi, Wi, Ci, Co, ksize, stride, nseg)) return fail("xunet_op_conv_wgrad: shape not supported by the tensor-core kernel");
-    launch_wgrad_tc(w, (cudaStream_t)stream);
-  } else if (impl == 2) {
-    if (Ci == 3 && ksize == 3 && stride == 1 && Co % 8 == 0) launch_conv_small(dtype, 1, nullptr, &w, (cudaStream_t)stream);
-    else if (conv_cout3_supported(Ci, Co, ksize, stride)) launch_conv_small(dtype, 4, nullptr, &w, (cudaStream_t)stream);
-    else return fail("xunet_op_conv_wgrad: not a 3-channel conv");
-  } else launch_wgrad_simt(dtype, w, (cudaStream_t)stream);
-  return op_done("op_conv_wgrad");
+  const ConvShape cs = conv_shape(N, Hi, Wi, Ci, Co, ksize, stride, nseg);
+  ConvKernel k;
+  if (op_conv_kernel(impl, conv_kernels(dtype, cs, false).wgrad, what, k)) return 1;
+  dispatch_wgrad(dtype, k, conv_wgrad_args(cs, x, dy, dw, dbias, alpha), (cudaStream_t)stream);
+  return op_done(what);
 }
 
 extern "C" int xunet_op_attention(int dtype, int impl, const void* qkv, const void* res, void* out, float* lse, int N,
                                   int L, int C, int heads, int cross, void* stream) {
   xu_set_kernel_error("");
   OpScratch scratch;
-  AttnArgs a;
-  memset(&a, 0, sizeof(a));
-  a.qkv = qkv; a.res = res; a.out = out; a.lse = lse; a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
-  if (impl == 1) {
-    if (!attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention: shape not supported by the tensor-core kernel");
-    launch_attn_fwd_tc(a, (cudaStream_t)stream);
-  } else launch_attn_fwd_simt(dtype, a, (cudaStream_t)stream);
+  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention: shape not supported by the tensor-core kernel");
+  dispatch_attn_fwd(dtype, impl, attn_args(qkv, res, out, lse, N, L, C, heads, cross), (cudaStream_t)stream);
   return op_done("op_attention");
 }
 
@@ -1423,17 +1444,12 @@ extern "C" int xunet_op_attention_bwd(int dtype, int impl, const void* qkv, cons
                                       int heads, int cross, void* stream) {
   xu_set_kernel_error("");
   OpScratch scratch;
-  AttnArgs a;
-  memset(&a, 0, sizeof(a));
-  a.qkv = qkv; a.res = res; a.out = const_cast<void*>(out); a.lse = const_cast<float*>(lse);
+  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention_bwd: shape not supported by the tensor-core kernel");
+  AttnArgs a = attn_args(qkv, res, const_cast<void*>(out), const_cast<float*>(lse), N, L, C, heads, cross);
   a.dout = dout; a.dscratch = dscratch; a.dqkv = dqkv;
-  a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
   // XUNET_OP_ATTN_FOLD=1: the caller passes an all-zero dscratch and gets it back all-zero (the D rows are cleared after use)
   a.scratch_zeroed = getenv("XUNET_OP_ATTN_FOLD") != nullptr ? 1 : 0;
-  if (impl == 1) {
-    if (!attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention_bwd: shape not supported by the tensor-core kernel");
-    launch_attn_bwd_tc(a, (cudaStream_t)stream);
-  } else launch_attn_bwd_simt(dtype, a, (cudaStream_t)stream);
+  dispatch_attn_bwd(dtype, impl, a, (cudaStream_t)stream);
   return op_done("op_attention_bwd");
 }
 
@@ -1478,17 +1494,11 @@ extern "C" int xunet_op_attention_stats(int dtype, int impl, const void* qkv, co
   if (heads < 1 || C % heads != 0) return fail("%s: C = %d is not a multiple of heads = %d", what, C, heads);
   if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return fail("%s: shape not supported by the tensor-core kernel", what);
   OpScratch scratch;
-  AttnArgs a;
-  memset(&a, 0, sizeof(a));
-  a.qkv = qkv; a.res = res; a.out = out; a.lse = lse; a.N = N; a.L = L; a.C = C; a.heads = heads; a.cross = cross;
-  const bool fused = impl == 1;      // the engine's rule: the tensor-core forward emits the statistics, the SIMT one cannot
-  if (fused) {
-    a.cstats = cstats;
-    launch_attn_fwd_tc(a, (cudaStream_t)stream);
-  } else {
-    launch_attn_fwd_simt(dtype, a, (cudaStream_t)stream);
-    launch_gn_cstats(dtype, out, cstats, N, L, 1, C, (cudaStream_t)stream);
-  }
+  AttnArgs a = attn_args(qkv, res, out, lse, N, L, C, heads, cross);
+  const bool fused = attn_emits_stats(impl);
+  if (fused) a.cstats = cstats;
+  dispatch_attn_fwd(dtype, impl, a, (cudaStream_t)stream);
+  if (!fused) launch_gn_cstats(dtype, out, cstats, N, L, 1, C, (cudaStream_t)stream);
   return op_done(what);
 }
 
@@ -1528,18 +1538,13 @@ extern "C" int xunet_op_conv_dgrad_groupnorm(int dtype, const void* dy, const fl
   if (mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev) return fail("%s: dropout in training needs seed_dev", what);
   if (ksize != 1 && ksize != 3) return fail("%s: ksize must be 1 or 3", what);
   if (nseg < 1 || Co % nseg != 0) return fail("%s: Co = %d is not a multiple of nseg = %d", what, Co, nseg);
-  if (!conv_tc_supported(dtype, 1, N, H, W, C, Co, ksize, 1, nseg) || !conv_tc_stats_supported(1, N, H, W))
-    return fail("%s: shape not supported by the fused tensor-core data gradient", what);
+  const ConvShape cs = conv_shape(N, H, W, C, Co, ksize, 1, nseg);
+  const ConvKernel k = conv_kernels(dtype, cs, false).dgrad;
+  if (!dgrad_fuses_gn_bwd(k, cs)) return fail("%s: shape not supported by the fused tensor-core data gradient", what);
   OpScratch scratch;
-  ConvArgs a;
-  int pl_h = 0, pl_w = 0, Ho = H, Wo = W;
-  if (ksize == 3) { same_pad(H, 3, 1, pl_h, Ho); same_pad(W, 3, 1, pl_w, Wo); }
-  a.x = dy; a.y = dyh; a.res = nullptr; a.w = w; a.bias = nullptr;
-  a.N = N; a.Hi = Ho; a.Wi = Wo; a.Ci = Co; a.Ho = H; a.Wo = W; a.Co = C;
-  a.ks = ksize; a.stride = 1; a.pad_h = pl_h; a.pad_w = pl_w; a.mode = 1;
-  a.wCi = C; a.wCo = Co; a.segw = Co / nseg; a.alpha = alpha; a.accumulate = 0;
+  ConvArgs a = conv_dgrad_args(cs, dy, w, dyh, alpha, 0);
   set_gn_bwd_epilogue(a, gn_x, gn_params, mode, e, de, bcs, drop_rate, op_index, seed_dev, train ? 1 : 0);
-  return op_conv_tc(a, w, ksize * ksize, C, Co, nseg, (cudaStream_t)stream, what);
+  return op_dispatch_conv(dtype, k, cs, a, (cudaStream_t)stream, what) ? 1 : op_done(what);
 }
 
 extern "C" int xunet_op_groupnorm_bwd(int dtype, const void* x, const void* e, const void* dy, void* dx, void* de, const float* gamma,

@@ -44,11 +44,14 @@ struct WgradArgs {
   double* acc_dw; double* acc_db;
 };
 void launch_wgrad_simt(int dtype, const WgradArgs& a, cudaStream_t s);
-// direct kernels for the 3-channel convs.  which: 0 = Cin3 forward, 1 = Cin3 wgrad, 2 = Cout3 forward, 3 = Cout3 dgrad
-// (ConvArgs in mode-1 convention: x = dO, y = dX), 4 = Cout3 wgrad
-bool conv_cin3_supported(const ConvArgs& a);
-bool conv_cout3_supported(int Ci, int Co, int ks, int stride);
-void launch_conv_small(int dtype, int which, const ConvArgs* c, const WgradArgs* w, cudaStream_t s);
+// the kernel a convolution runs in one direction (forward, data gradient or weight gradient)
+enum ConvKernel { CONV_SIMT, CONV_TC, CONV_CIN3, CONV_COUT3 };
+// direct kernels for the 3-channel convs: CONV_CIN3 (forward, weight gradient) and CONV_COUT3 (forward, data gradient with
+// ConvArgs in the mode-1 convention x = dO, y = dX, weight gradient).  Neither takes a residual (res) or segments (nseg > 1).
+bool conv_cin3_supported(int Ci, int Co, int ks, int stride, int nseg, bool res);
+bool conv_cout3_supported(int Ci, int Co, int ks, int stride, int nseg, bool res);
+void launch_conv_direct(int dtype, ConvKernel k, const ConvArgs& a, cudaStream_t s);
+void launch_wgrad_direct(int dtype, ConvKernel k, const WgradArgs& a, cudaStream_t s);
 // data gradient of the input conv 3 -> Co, un-packed: dy (2B,S,S,Co) activation dtype, w the fp32 kernel (3,3,3,Co); rows 2b go
 // to dx (B,S,S,3) fp32, rows 2b+1 to dz; a nullptr output is skipped (both nullptr: nothing is launched)
 void launch_conv_cin3_dgrad_unpack(int dtype, const void* dy, const float* w, float* dx, float* dz, int B, int S, int Co,

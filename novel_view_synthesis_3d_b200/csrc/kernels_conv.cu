@@ -929,26 +929,24 @@ __global__ void __launch_bounds__(256) wgrad_thin_kernel(WgradArgs a) {
 
 static bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
-bool conv_cin3_supported(const ConvArgs& a) { return a.mode == 0 && a.Ci == 3 && a.ks == 3 && a.stride == 1 && a.Co % 8 == 0 && a.segw == a.Co && a.res == nullptr && !a.accumulate && 28 * a.Co * 4 <= 96 * 1024; }
-bool conv_cout3_supported(int Ci, int Co, int ks, int stride) { return Co == 3 && ks == 3 && stride == 1 && Ci % 8 == 0 && 27 * Ci * 4 <= 96 * 1024; }
+bool conv_cin3_supported(int Ci, int Co, int ks, int stride, int nseg, bool res) { return Ci == 3 && ks == 3 && stride == 1 && Co % 8 == 0 && nseg == 1 && !res; }
+bool conv_cout3_supported(int Ci, int Co, int ks, int stride, int nseg, bool res) { return Co == 3 && ks == 3 && stride == 1 && Ci % 8 == 0 && 27 * Ci * 4 <= 96 * 1024 && nseg == 1 && !res; }
 
+// exactly one of c (forward, or the Cout=3 data gradient in mode 1) and w (weight gradient) is set
 template <typename T>
-static void small_dispatch(int which, const ConvArgs* c, const WgradArgs* w, cudaStream_t s) {
+static void small_dispatch(ConvKernel k, const ConvArgs* c, const WgradArgs* w, cudaStream_t s) {
+  const bool cin3 = k == CONV_CIN3;
   // round-2 kernels where their shape rules hold, the round-1 kernels below for every other shape
-  if ((which == 0 || which == 3) && c->Wo % 4 == 0 && c->Co % 8 == 0 && c->Hi == c->Ho && c->Wi == c->Wo) {
+  if (c && (cin3 || c->mode == 1) && c->Wo % 4 == 0 && c->Co % 8 == 0 && c->Hi == c->Ho && c->Wi == c->Wo) {
     const long long total = (long long)c->N * c->Ho * (c->Wo / 4) * (c->Co / 8);
     const size_t sm = sizeof(float) * 28 * c->Co;
     const int grid = (int)std::min<long long>(cdiv(total, 256), (long long)xu_num_sms() * 4);
-    if (which == 0) {
-      if (sm > 48 * 1024) cudaFuncSetAttribute(conv_thin_in_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-      xu_launch(conv_thin_in_kernel<T, 0>, grid, 256, sm, s, *c);
-    } else {
-      if (sm > 48 * 1024) cudaFuncSetAttribute(conv_thin_in_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-      xu_launch(conv_thin_in_kernel<T, 1>, grid, 256, sm, s, *c);
-    }
+    const auto kernel = cin3 ? conv_thin_in_kernel<T, 0> : conv_thin_in_kernel<T, 1>;
+    if (sm > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    xu_launch(kernel, grid, 256, sm, s, *c);
     return;
   }
-  if (which == 2 && c->Wo % 4 == 0 && is_pow2(c->Ci / 8) && c->Ci / 8 <= 32 && c->Hi == c->Ho && c->Wi == c->Wo) {
+  if (c && !cin3 && c->mode == 0 && c->Wo % 4 == 0 && is_pow2(c->Ci / 8) && c->Ci / 8 <= 32 && c->Hi == c->Ho && c->Wi == c->Wo) {
     const long long quads = (long long)c->N * c->Ho * (c->Wo / 4);
     const int qpb = 256 / (c->Ci / 8);
     const size_t sm = sizeof(float) * 27 * c->Ci;
@@ -957,38 +955,34 @@ static void small_dispatch(int which, const ConvArgs* c, const WgradArgs* w, cud
     xu_launch(conv_cout3_fwd4_kernel<T>, grid, 256, sm, s, *c);
     return;
   }
-  if (which == 1 || which == 4) {
-    const int Cw = which == 4 ? w->Ci : w->Co;
+  if (w) {
+    const int Cw = cin3 ? w->Co : w->Ci;
     const int SEG = w->Wo < 32 ? w->Wo : 32;
     if (is_pow2(Cw) && Cw >= 2 && Cw <= 512 && w->Wo % SEG == 0 && w->Hi == w->Ho && w->Wi == w->Wo) {
       const int nstream = 256 / (Cw / 2);
       const long long units = (long long)w->N * w->Ho * (w->Wo / SEG);
       const int grid = (int)std::min<long long>(cdiv(units, nstream), (long long)xu_num_sms() * 2);
       const size_t sm = sizeof(float) * 256 * 56;
-      if (which == 1) {
-        cudaFuncSetAttribute(wgrad_thin_kernel<T, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        xu_launch(wgrad_thin_kernel<T, 0>, grid, 256, sm, s, *w);
-      } else {
-        cudaFuncSetAttribute(wgrad_thin_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-        xu_launch(wgrad_thin_kernel<T, 1>, grid, 256, sm, s, *w);
-      }
+      const auto kernel = cin3 ? wgrad_thin_kernel<T, 0> : wgrad_thin_kernel<T, 1>;
+      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+      xu_launch(kernel, grid, 256, sm, s, *w);
       return;
     }
   }
-  if (which == 0) {
+  if (c && cin3) {
     const long long total = (long long)c->N * c->Ho * c->Wo * (c->Co / 8);
     const size_t sm = sizeof(float) * 28 * c->Co;
     if (sm > 48 * 1024) cudaFuncSetAttribute(conv_cin3_fwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     xu_launch(conv_cin3_fwd_kernel<T>, cdiv(total, 256), 256, sm, s, *c);
-  } else if (which == 1) {
+  } else if (cin3) {
     const long long M = (long long)w->N * w->Ho * w->Wo;
     xu_launch(conv_cin3_wgrad_kernel<T>, cdiv(M, 128), 256, 0, s, *w);
-  } else if (which == 2) {
+  } else if (c && c->mode == 0) {
     const long long total = (long long)c->N * c->Ho * c->Wo;
     const size_t sm = sizeof(float) * 27 * c->Ci;
     if (sm > 48 * 1024) cudaFuncSetAttribute(conv_cout3_fwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     xu_launch(conv_cout3_fwd_kernel<T>, cdiv(total, 256), 256, sm, s, *c);
-  } else if (which == 3) {
+  } else if (c) {
     const long long total = (long long)c->N * c->Ho * c->Wo * (c->Co / 8);
     const size_t sm = sizeof(float) * 27 * c->Co;
     if (sm > 48 * 1024) cudaFuncSetAttribute(conv_cout3_dgrad_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
@@ -1000,14 +994,13 @@ static void small_dispatch(int which, const ConvArgs* c, const WgradArgs* w, cud
     xu_launch(conv_cout3_wgrad_kernel<T>, cdiv(M, 128), threads, 0, s, *w);
   }
 }
-void launch_conv_small(int dtype, int which, const ConvArgs* c, const WgradArgs* w, cudaStream_t s) {
-  if (w != nullptr) {
-    det_wgrad(*w, s, [&](const WgradArgs& aa) {
-      if (dtype == XU_F32) small_dispatch<float>(which, c, &aa, s);
-      else small_dispatch<bf16>(which, c, &aa, s);
-    });
-    return;
-  }
-  if (dtype == XU_F32) small_dispatch<float>(which, c, w, s);
-  else small_dispatch<bf16>(which, c, w, s);
+void launch_conv_direct(int dtype, ConvKernel k, const ConvArgs& a, cudaStream_t s) {
+  if (dtype == XU_F32) small_dispatch<float>(k, &a, nullptr, s);
+  else small_dispatch<bf16>(k, &a, nullptr, s);
+}
+void launch_wgrad_direct(int dtype, ConvKernel k, const WgradArgs& a, cudaStream_t s) {
+  det_wgrad(a, s, [&](const WgradArgs& aa) {
+    if (dtype == XU_F32) small_dispatch<float>(k, nullptr, &aa, s);
+    else small_dispatch<bf16>(k, nullptr, &aa, s);
+  });
 }

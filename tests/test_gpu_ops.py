@@ -358,7 +358,8 @@ def test_attention_tcgen05_bwd(lib, case):
                                   (2, 64, 64, 3, 256), (2, 64, 64, 256, 3),      # the 3DiM widths: 32 lanes per pixel quad
                                   (2, 8, 48, 3, 32), (2, 8, 48, 32, 3),          # W % 32 != 0: round-1 wgrad kernels, new fwd / dgrad
                                   (2, 12, 20, 3, 32), (2, 12, 20, 32, 3),        # W < 32: one segment per row
-                                  (2, 6, 6, 3, 16), (2, 6, 6, 16, 3)])           # W % 4 != 0: round-1 kernels throughout
+                                  (2, 6, 6, 3, 16), (2, 6, 6, 16, 3),            # W % 4 != 0: round-1 kernels throughout
+                                  (2, 8, 8, 3, 896)])                            # the input conv at ch = 896: > 96 KiB of weights in smem
 def test_three_channel_direct_convs(lib, dtype, case):
     """impl=2: the direct kernels for the input conv (Cin=3) and the output conv (Cout=3)."""
     N, H, W, Ci, Co = case
