@@ -87,6 +87,33 @@ int xunet_tap_count(const xunet_handle* h);
 int xunet_tap(const xunet_handle* h, int i, const char** name, int dims[4], long long* byte_offset, int* is_f32,
               long long* grad_byte_offset);
 
+/* The plan's convolution and attention launches, in op order (read-only; needs no GPU), so that tests can run each one through
+ * the operator-level entry points at exactly the plan's shape and arguments.  kernel: what runs a direction of a conv. */
+#define XUNET_LAUNCH_CONV 0
+#define XUNET_LAUNCH_ATTN 1
+#define XUNET_KERNEL_NONE -1     /* that direction is not run: no backward (training=0), or the input needs no gradient */
+#define XUNET_KERNEL_SIMT 0
+#define XUNET_KERNEL_TC 1        /* tensor cores: xunet_op_conv* impl 1 */
+#define XUNET_KERNEL_CIN3 2      /* direct 3-channel input kernel: impl 2 */
+#define XUNET_KERNEL_COUT3 3     /* direct 3-channel output kernel: impl 2 */
+typedef struct xunet_launch_info {
+  int kind;                /* XUNET_LAUNCH_* */
+  /* conv: y = alpha * (conv(x, W; ksize, stride, SAME) + bias (+ residual)), Co in nseg weight segments */
+  int leaf;                /* index of the kernel leaf (xunet_param_leaf numbering); -1 for attention */
+  int N, Hi, Wi, Ci, Ho, Wo, Co, ksize, stride, nseg;
+  int residual;
+  float alpha;
+  int fwd, dgrad, wgrad;   /* XUNET_KERNEL_* of the forward, data gradient and weight gradient */
+  int emits_stats;         /* conv / attention: the forward emits the GroupNorm statistics of its output */
+  float bwd_alpha;         /* alpha of the data and weight gradients (alpha times the scale of an aliased output gradient) */
+  int accumulate;          /* the data gradient adds into its destination */
+  int gn_mode;             /* the data gradient carries the backward of the GroupNorm before it: XUNET_GN_*; -1 none */
+  /* attention: qkv (N, L, 3C), heads, cross = keys and values of the other frame of the sample; impl 1 tensor cores, 0 SIMT */
+  int L, C, heads, cross, impl;
+} xunet_launch_info;
+int xunet_plan_launch_count(const xunet_handle* h);
+int xunet_plan_launch(const xunet_handle* h, int i, xunet_launch_info* out);
+
 /* XUNet.apply({'params': p}, batch, cond_mask=, train=, rngs=)  (train.py:63-66, sampling.py:131-132).
  * params: device, flat fp32.  seed_dev: device pointer to ONE uint64 dropout seed (read at execution
  * time, so a captured graph sees updates); may be NULL when train==0.  eps_out: device (B,S,S,3) fp32. */

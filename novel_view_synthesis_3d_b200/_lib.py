@@ -27,6 +27,18 @@ class XunetBatch(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in ('x', 'z', 'logsnr', 'R1', 't1', 'R2', 't2', 'K', 'cond_mask', 'rays')]
 
 
+LAUNCH_CONV, LAUNCH_ATTN = 0, 1
+KERNEL_NONE, KERNEL_SIMT, KERNEL_TC, KERNEL_CIN3, KERNEL_COUT3 = -1, 0, 1, 2, 3
+
+
+class XunetLaunchInfo(C.Structure):
+    _fields_ = [('kind', C.c_int), ('leaf', C.c_int)] + \
+        [(k, C.c_int) for k in ('N', 'Hi', 'Wi', 'Ci', 'Ho', 'Wo', 'Co', 'ksize', 'stride', 'nseg', 'residual')] + \
+        [('alpha', C.c_float), ('fwd', C.c_int), ('dgrad', C.c_int), ('wgrad', C.c_int), ('emits_stats', C.c_int),
+         ('bwd_alpha', C.c_float), ('accumulate', C.c_int), ('gn_mode', C.c_int)] + \
+        [(k, C.c_int) for k in ('L', 'C', 'heads', 'cross', 'impl')]
+
+
 class XunetSrnStore(C.Structure):
     _fields_ = [('pixels', C.c_void_p), ('pixel_kind', C.c_int), ('S', C.c_int), ('n_items', C.c_longlong),
                 ('n_instances', C.c_int), ('R', C.c_void_p), ('t', C.c_void_p), ('K', C.c_void_p), ('first', C.c_void_p),
@@ -51,6 +63,8 @@ SYMBOLS = {
     'xunet_tap_count': (C.c_int, [C.c_void_p]),
     'xunet_tap': (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int * 4),
                             C.POINTER(C.c_longlong), C.POINTER(C.c_int), C.POINTER(C.c_longlong)]),
+    'xunet_plan_launch_count': (C.c_int, [C.c_void_p]),
+    'xunet_plan_launch': (C.c_int, [C.c_void_p, C.c_int, C.POINTER(XunetLaunchInfo)]),
     'xunet_forward': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_int, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p]),
     'xunet_set_static_conditioning': (C.c_int, [C.c_void_p, C.c_int]),

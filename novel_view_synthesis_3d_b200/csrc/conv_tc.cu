@@ -731,9 +731,10 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
   {
     static const bool log = getenv("XUNET_CONV_LOG") != nullptr;
     // epi: the epilogue template argument (1: forward with GroupNorm statistics)
-    if (log) fprintf(stderr, "conv_tc mode=%d N=%d %dx%d Ci=%d Co=%d ks=%d st=%d wCi=%d wCo=%d segw=%d bk=%d BN=%d KC=%d T=%d halo=%d stages=%d per_sm=%d ctas=%d tiles=%d epi=%d\n",
+    // acc: the output is added to the destination (TMA reduce-add); tma_store: the tile is staged and stored by TMA
+    if (log) fprintf(stderr, "conv_tc mode=%d N=%d %dx%d Ci=%d Co=%d ks=%d st=%d wCi=%d wCo=%d segw=%d bk=%d BN=%d KC=%d T=%d halo=%d stages=%d per_sm=%d ctas=%d tiles=%d epi=%d acc=%d tma_store=%d\n",
                      a.mode, a.N, a.Ho, a.Wo, a.Ci, a.Co, a.ks, a.stride, a.wCi, a.wCo, a.segw, bk, p.BN, p.KC, p.T, p.halo, p.stages, per_sm, ctas, p.total_tiles,
-                     epi != 0 ? epi : (a.cstats != nullptr ? 1 : 0));
+                     epi != 0 ? epi : (a.cstats != nullptr ? 1 : 0), a.accumulate ? 1 : 0, p.tma_store);
   }
   p.cstats = cacc;
   p.gx = reinterpret_cast<const bf16*>(a.gn_x); p.gnp = reinterpret_cast<const float4*>(a.gn_params); p.gn_swish = a.gn_swish;

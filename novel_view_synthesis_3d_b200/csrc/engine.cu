@@ -1050,6 +1050,61 @@ extern "C" int xunet_tap(const xunet_handle* h, int i, const char** name, int di
   return 0;
 }
 
+static_assert(XUNET_KERNEL_SIMT == CONV_SIMT && XUNET_KERNEL_TC == CONV_TC && XUNET_KERNEL_CIN3 == CONV_CIN3 &&
+              XUNET_KERNEL_COUT3 == CONV_COUT3, "conv kernels");
+
+static bool is_launch(const Op& o) { return o.kind == OP_CONV || o.kind == OP_ATTN; }
+
+extern "C" int xunet_plan_launch_count(const xunet_handle* h) {
+  int n = 0;
+  for (const Op& o : h->ops) n += is_launch(o);
+  return n;
+}
+
+// every field comes from the op and the helpers the launch code uses (run_conv_fwd / run_conv_bwd, forward_impl's OP_ATTN)
+extern "C" int xunet_plan_launch(const xunet_handle* h, int i, xunet_launch_info* out) {
+  if (!h || !out) return fail("xunet_plan_launch: null argument");
+  int k = -1;
+  for (size_t j = 0; j < h->ops.size() && i >= 0; ++j)
+    if (is_launch(h->ops[j]) && i-- == 0) k = (int)j;
+  if (k < 0) return fail("xunet_plan_launch: index out of range");
+  const Op& o = h->ops[k];
+  const Tensor& x = h->tensors[o.x];
+  const Tensor& y = h->tensors[o.y];
+  xunet_launch_info r;
+  memset(&r, 0, sizeof(r));
+  r.leaf = -1;
+  r.fwd = r.dgrad = r.wgrad = XUNET_KERNEL_NONE;
+  r.gn_mode = -1;
+  r.emits_stats = y.cstats >= 0 && y.cs_fused;
+  if (o.kind == OP_ATTN) {
+    r.kind = XUNET_LAUNCH_ATTN;
+    r.N = y.n; r.L = y.h * y.w; r.C = y.c; r.heads = o.heads; r.cross = o.cross; r.impl = o.impl;
+    *out = r;
+    return 0;
+  }
+  r.kind = XUNET_LAUNCH_CONV;
+  for (size_t l = 0; l < h->leaves.size(); ++l)
+    if (h->leaves[l].off == o.w) r.leaf = (int)l;
+  const ConvShape& s = o.cs;
+  r.N = s.N; r.Hi = s.Hi; r.Wi = s.Wi; r.Ci = s.Ci; r.Ho = s.Ho; r.Wo = s.Wo; r.Co = s.Co;
+  r.ksize = s.ks; r.stride = s.stride; r.nseg = s.nseg;
+  r.residual = o.r >= 0;
+  r.alpha = o.alpha;
+  r.fwd = o.k.fwd;
+  r.bwd_alpha = o.alpha * y.gscale;
+  if (h->training) {
+    r.wgrad = o.k.wgrad;
+    if (x.need_grad) {
+      r.dgrad = o.k.dgrad;
+      r.accumulate = o.acc_x;
+      if (o.gnb >= 0) r.gn_mode = h->ops[o.gnb].mode;
+    }
+  }
+  *out = r;
+  return 0;
+}
+
 extern "C" int xunet_forward(xunet_handle* h, const float* params, const xunet_batch* batch, int train,
                              const unsigned long long* seed_dev, void* workspace, float* eps_out, void* stream) {
   if (!h || !params || !batch || !workspace) return fail("xunet_forward: null argument");

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from oracle import xunet_ref as R
+from tests import launch_ref as L
 from novel_view_synthesis_3d_b200 import _lib, XUNetConfig, SMALL, FULL_3DIM
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -101,3 +102,51 @@ def test_library_is_built_from_the_sources_in_the_tree():
     assert lib.exists()
     deps = list(B.CSRC.glob('*.cu')) + list(B.CSRC.glob('*.cuh')) + list(B.CSRC.glob('*.h')) + list(B.INCLUDE.glob('*.h'))
     assert (B.OBJ_DIR / 'stamp').read_text() == B._digest(deps)
+
+
+# ---- the plan's conv and attention launches (xunet_plan_launch), for every plan bench.py measures ----
+@pytest.mark.parametrize('plan', list(L.PLANS))
+def test_plan_launches_cover_every_conv_leaf_and_attention_block(lib, plan):
+    import novel_view_synthesis_3d_b200 as P
+    from tests.util import to_ref_cfg
+    preset, S, B, dtype, training = L.PLANS[plan]
+    cfg = getattr(P, preset)
+    launches, names = L.plan_launches(lib, cfg, B, S, dtype, training)
+    ref = R.param_shapes(to_ref_cfg(cfg), S)
+    convs = [r for r in launches if r['kind'] == _lib.LAUNCH_CONV]
+    attns = [r for r in launches if r['kind'] == _lib.LAUNCH_ATTN]
+    assert len(convs) + len(attns) == len(launches)
+    # one conv per kernel leaf: every conv, 1x1 Dense and FiLM Dense, and the q|k|v projection (its q kernel leads the three
+    # segments); the log-SNR MLP is not a conv
+    conv_leaves = {n for n in ref if n.endswith('/kernel') and not n.startswith('ConditioningProcessor_0/Dense_') and
+                   'DenseGeneral_1' not in n and 'DenseGeneral_2' not in n}
+    got = [names[r['leaf']] for r in convs]
+    assert sorted(got) == sorted(conv_leaves)
+    for r in convs:
+        shp = ref[names[r['leaf']]]
+        if 'DenseGeneral_0' in names[r['leaf']]:
+            ks, ci, co, nseg = 1, shp[0], 3 * shp[1] * shp[2], 3
+        elif len(shp) == 5:
+            ks, ci, co, nseg = shp[1], shp[3], shp[4], 1
+        else:
+            ks, ci, co, nseg = 1, shp[0], shp[1], 1
+        assert (r['ksize'], r['Ci'], r['Co'], r['nseg']) == (ks, ci, co, nseg), names[r['leaf']]
+        assert r['N'] == 2 * B
+        if not training:
+            assert r['dgrad'] == r['wgrad'] == _lib.KERNEL_NONE
+        else:
+            assert r['wgrad'] != _lib.KERNEL_NONE
+        if r['gn_mode'] >= 0:
+            assert r['dgrad'] == _lib.KERNEL_TC and not r['accumulate']
+    # one attention per AttnBlock, in op order, with its C and heads
+    blocks = [n[:-len('/AttnLayer_0/DenseGeneral_0/kernel')] for n in names if n.endswith('AttnLayer_0/DenseGeneral_0/kernel')]
+    assert len(attns) == len(blocks)
+    for r, b in zip(attns, blocks):
+        C_, heads, hd = ref[b + '/AttnLayer_0/DenseGeneral_0/kernel']
+        assert (r['C'], r['heads']) == (C_, heads) and C_ == heads * hd
+        assert r['cross'] == int(b.endswith('AttnBlock_1'))
+        # tensor cores in bf16 exactly for L a multiple of 128 and head_dim 16, 32, 64 or 128; never in fp32
+        assert r['impl'] == int(dtype == 1 and r['L'] % 128 == 0 and hd in (16, 32, 64, 128)), (b, r)
+    if dtype == 0:
+        assert all(_lib.KERNEL_TC not in (r['fwd'], r['dgrad'], r['wgrad']) for r in convs)
+        assert all(r['impl'] == 0 for r in attns)

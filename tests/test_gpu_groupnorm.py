@@ -22,13 +22,14 @@ import torch
 import torch.nn.functional as F
 
 from tests import groupnorm_ref as G
+from tests import launch_ref as L
 from tests.util import keep_mask
 
 pytestmark = pytest.mark.gpu
 
 DT = {0: torch.float32, 1: torch.bfloat16}
 F64 = torch.float64
-BF_REL = 2. ** -8        # a bf16 store: 2^-9 relative, with a factor 2 for the fp32 work before it
+BF_REL = 2. ** -8        # a bf16 store: one rounding, 2^-8 relative (8 significand bits); the fp32 work before it is in the floors
 F32_REL = 1e-5
 SEED = 0x5DEECE66D
 
@@ -109,10 +110,9 @@ def _dgrad_ref(dy, w, ks, C, nseg=1):
     return torch.nn.grad.conv2d_input((N, C, H, W), wt, dy.permute(0, 3, 1, 2), padding=1).permute(0, 2, 3, 1)
 
 
-# tensor-core accumulation floor: wgmma accumulates the K <= 9 * 256 bf16 products of an output in fp32; rounding each partial
-# sum errs by at most 2^-24 of it, a random walk of sqrt(K) 2^-24 sum|terms| <= 2^-18.2 sum|terms|.  2^-16 keeps a 4x margin
-# (and covers truncating accumulation), and is still ~10^-3 of a typical output, so a misplaced element cannot hide in it.
-CONV_FLOOR = 2. ** -16
+# conv accumulation floor of a K-term fp32 sum: L.acc_floor(K) of sum|terms| (tests/launch_ref.py derives it), 2^-16 at
+# K = 9 * 256 and less for the shorter reductions, still ~10^-3 of a typical output, so a misplaced element cannot hide in it.
+CONV_FLOOR = L.acc_floor
 
 
 # ======================================================================================================================
@@ -169,7 +169,7 @@ def test_conv_stats(lib, case):
     if has_res:
         ref, mag = ref + res, mag + res.abs()
     ref, mag = ref * alpha, mag * alpha
-    assert_elems(y, ref, CONV_FLOOR * mag, BF_REL if dtype == 1 else F32_REL, 'y')
+    assert_elems(y, ref, CONV_FLOOR(ks * ks * Ci) * mag, BF_REL if dtype == 1 else F32_REL, 'y')
     assert rel_l2(y, ref) < (6e-3 if dtype == 1 else 1e-5)
 
 
@@ -390,14 +390,14 @@ def _check_epi(r, N, H, W, C, Co, ks, nseg, mode, alpha, rate=0., train=0):
     x, table, e = r['x'], r['table'].to(F64), r['e']
     wb = r['w'].to(torch.bfloat16).to(F64)
     gact = alpha * _dgrad_ref(r['dy'], wb, ks, C, nseg)
-    gmag = alpha * _dgrad_ref(r['dy'].abs(), wb.abs(), ks, C, nseg)
+    gmag = alpha * _dgrad_ref(r['dy'].abs(), wb.abs(), ks, C, nseg) * CONV_FLOOR(ks * ks * Co)   # the floor of the conv's sum
     # stage: dyhat from the kernel's inputs, the norm taken from the stored table (xhat = x rstd + (-mean rstd))
     rstd, nmr = table[..., 0], table[..., 1]
     mean = -nmr / rstd
     keep = torch.from_numpy(keep_mask(SEED, 7, (N, H, W, C), rate)).cuda() if (mode == G.FILM and train and rate > 0) else None
     dyh_ref, de_ref = G.dyhat(gact, x, table[..., 2][0], table[..., 3][0], mode, e=e, keep=keep, drop_rate=rate, mean=mean,
                               rstd=rstd)
-    # floor: the conv's accumulation (CONV_FLOOR of its terms) times the local derivative (<= 1.1 for swish; FiLM: also
+    # floor: the conv's accumulation (gmag: CONV_FLOOR of its terms) times the local derivative (<= 1.1 for swish; FiLM: also
     # |1 + scale| and the keep scale), plus the fp32 evaluation of the derivative's argument (2^-21 of its terms, times
     # |g| max|swish''| <= 0.5)
     xh = G.xhat(x, mean, rstd)
@@ -405,14 +405,14 @@ def _check_epi(r, N, H, W, C, Co, ks, nseg, mode, alpha, rate=0., train=0):
     yh = xh * gm + bt
     yterms = (x * G._per_channel(rstd, N, H, W) * gm).abs() + (G._per_channel(nmr, N, H, W) * gm).abs() + bt.abs()
     if mode == G.PLAIN:
-        fl = CONV_FLOOR * gmag
+        fl = gmag
     elif mode == G.SWISH:
-        fl = 1.1 * CONV_FLOOR * gmag + 0.5 * 2. ** -21 * gact.abs() * yterms
+        fl = 1.1 * gmag + 0.5 * 2. ** -21 * gact.abs() * yterms
     else:
         sc, sh = e[..., :C], e[..., C:]
         ks_ = G.keep_scale(rate) if keep is not None else 1.
         uterms = yterms * (1. + sc).abs() + sh.abs()
-        fl_du = ks_ * (1.1 * CONV_FLOOR * gmag + 0.5 * 2. ** -21 * gact.abs() * uterms)
+        fl_du = ks_ * (1.1 * gmag + 0.5 * 2. ** -21 * gact.abs() * uterms)
         fl = fl_du * (1. + sc).abs()
         du = de_ref[..., C:]
         assert_elems(r['de'], de_ref, torch.cat([fl_du * yh.abs() + du.abs() * 2. ** -21 * yterms, fl_du], -1), BF_REL,
