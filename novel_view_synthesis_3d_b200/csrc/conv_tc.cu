@@ -12,7 +12,7 @@
 // * B comes from a bf16 "shadow" of the fp32 master weights, K-major: forward [Co][tap][Ci] (transposed by
 //   weight_prep_kernel), data-gradient the plain cast [tap][Ci][Co] (there K = Co is already contiguous).
 // * Warp-specialised: warp 8 = TMA producer (one elected lane), warps 0-7 = two consumer warpgroups that issue
-//   wgmma.mma_async (64 rows each), release ring stages through mbarriers and run the epilogue
+//   wgmma.mma_async (64 rows each of every tile, or whole tiles in turn), release ring stages through mbarriers and run the epilogue
 //   (+bias (+residual) * alpha -> bf16 -> 16-byte global stores or a TMA store).
 #include "conv_tc.h"
 #include "tc_common.cuh"
@@ -45,17 +45,28 @@ struct TcParams {
   const bf16* ge;      // (N,H,W,2*Co) [scale | shift]
   bf16* gde;           // gradient of ge (written: [du*yhat | du])
   float drop_rate; int drop_op; int drop_on; const unsigned long long* seed_dev;
-  // output through shared memory + TMA store: the epilogue writes the rounded tile into a swizzled [128 pixels][cws channels]
-  // staging buffer (conflict-free 16-byte st.shared) and one thread issues cp.async.bulk.tensor stores of whole boxes
-  int tma_store, cws;
+  // output through shared memory + TMA store: the epilogue writes the rounded tile into a swizzled [128 pixels][BN or 64
+  // channels] staging buffer (conflict-free 16-byte st.shared) and one thread per buffer issues cp.async.bulk.tensor stores of
+  // whole boxes
+  int tma_store;
 };
 
 // Persistent: each CTA walks tiles  blockIdx.x, blockIdx.x + gridDim.x, ...  (tile = n_tile * m_tiles + m_tile) with the
-// smem ring running continuously across tiles.  Warps 0-7 are two consumer warpgroups: warpgroup wg issues the wgmma for
-// rows 64 wg .. 64 wg + 63 of the 128-pixel tile (fp32 accumulators in registers) and then runs the epilogue of those rows;
-// warp 8 is the TMA producer (one elected lane), which runs ahead into the next tile while the consumers drain theirs.
-// The epilogue moves 64 accumulator columns at a time through a shared-memory transpose ([64 rows][64 columns] fp32 per
-// warpgroup) so that a thread owns ONE pixel row and 32 consecutive channels: 16-byte bf16 stores and per-pixel statistics.
+// smem ring running continuously across tiles; warp 8 is the TMA producer (one elected lane), which fills the ring in tile
+// order and runs ahead into the next tile while the consumers drain theirs.  Warps 0-7 are two consumer warpgroups, scheduled
+// one of two ways (conv_pingpong):
+// * cooperative (BN = 64 and 128): warpgroup wg issues the wgmma for rows 64 wg .. 64 wg + 63 of every tile and then runs
+//   the epilogue of those rows.
+// * ping-pong (BN = 32, where a tile's few hundred cycles of MMA are dwarfed by its epilogue): warpgroup wg takes whole
+//   tiles, the CTA's tiles wg, wg + 2, ..., issuing two m64 wgmmas per k-step (rows 0-63 and 64-127), so that one warpgroup's
+//   epilogue (operand loads at DRAM latency, stores, reductions) runs while the other's main loop waits on TMA and the tensor
+//   cores.  A ring stage belongs to the warpgroup of its tile.  The main loops take turns in tile order (named barriers
+//   4 + wg): a warpgroup starts waiting on the stages of tile j only once the other one has seen every stage of tile j - 1
+//   land, so the stage it waits for was last filled for an earlier use that has completed, and the parity of its mbarrier
+//   phase cannot alias a phase two uses back.
+// The epilogue moves accumulator columns through a shared-memory transpose (fp32, per warpgroup: [64 rows][64 columns]
+// cooperative, [128 rows][32 columns] ping-pong) so that a thread owns ONE pixel row and 32 consecutive channels: 16-byte bf16
+// stores and per-pixel statistics.
 // EPI 1 (forward): the epilogue also emits the GroupNorm input statistics of the tensor it writes (per sample and channel: sum
 // and sum of squares of the bf16-rounded outputs), so the consumer norm needs no statistics pass over HBM.
 // EPI 2 (data gradient of the conv that consumes a GroupNorm[+swish] output): the epilogue turns dy into the gradient w.r.t.
@@ -65,7 +76,18 @@ struct TcParams {
 // EPI 3: the same for the FiLM norm of a ResnetBlock (model/xunet.py:82-84): dy -> dropout mask -> du = . * swish'(u) with
 // u = yhat*(1+scale)+shift, stores dyh = du*(1+scale) and the FiLM gradient [du*yhat | du], emits the same channel sums.
 constexpr int kConvThreads = 288;      // two consumer warpgroups + one producer warp
-constexpr int kXP = 68;                // fp32 pitch of the transpose buffer (16-byte row reads without bank conflicts)
+// The ping-pong schedule parks half of a tile's accumulators in registers through the epilogue of the other half once a
+// tile has more than one 32-column transpose group: at BN = 64 that does not fit the 96 registers of two CTAs per SM.
+__host__ __device__ constexpr bool conv_pingpong(int bn) { return bn < 64; }
+// fp32 transpose buffer of one warpgroup: cooperative [64 rows][64 columns] at a pitch of kXP = 68 (16-byte row reads
+// without bank conflicts); ping-pong [128 rows][32 columns], either with the 16-byte chunks of row r XOR-swizzled by r % 8
+// (the same, in less space than a padded pitch: two CTAs per SM keep their ring depth) or, for the FiLM-backward epilogue
+// (EPI 3, one CTA per SM), at a pitch of 36, whose plainer addressing keeps that epilogue within its registers
+constexpr int kXP = 68;
+__host__ __device__ constexpr int conv_tbuf_floats(int epi, int bn) { return conv_pingpong(bn) ? 128 * (epi == 3 ? 36 : 32) : 64 * kXP; }
+__host__ __device__ constexpr int conv_pp_tbuf_at(int epi, int row, int col) {
+  return epi == 3 ? row * 36 + col : row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
+}
 // Two CTAs per SM (96 registers per thread) for narrow tiles with the plain / statistics epilogues and with the fused
 // GroupNorm-backward one (EPI 2, without spills except at BK = 16, BN = 64); the FiLM-backward epilogue (EPI 3) needs more
 // registers and runs one CTA per SM.
@@ -77,6 +99,12 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
                                                                                const __grid_constant__ CUtensorMap tmB,
                                                                                const __grid_constant__ CUtensorMap tmY, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
+  constexpr bool PP = conv_pingpong(BN);
+  constexpr int NACC = PP ? 2 : 1;                     // m64 accumulator blocks per thread: rows 0-63 and 64-127 (ping-pong)
+  constexpr int TBUF = conv_tbuf_floats(EPI, BN);
+  // CG accumulator columns per transpose group (= channels of one staged output box), 32 of them per thread
+  constexpr int CG = BN < 64 ? BN : 64, CW = 32;
+  constexpr int GT = BN / CG * CW;                     // EPI 2/3: norm-table entries per consumer warp (its columns)
   constexpr int B_TILE = BN * BK * 2;
   // halo mode: the A stage holds (TH+2) x TW pixels -- the dy = 0,1,2 operands are the 128-pixel windows starting
   // dy*TW rows in (dy*TW*BK*2 bytes: a whole number of swizzle atoms since TW % 8 == 0) -- and the B stage the 3 dy taps
@@ -85,22 +113,23 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* smA = base;
   uint8_t* smB = base + (size_t)p.stages * A_BYTES;
-  uint8_t* smY = smB + (size_t)p.stages * B_BYTES;                       // 2 x [128][cws] bf16 staging (tma_store only)
+  uint8_t* smY = smB + (size_t)p.stages * B_BYTES;                       // 2 x [128][CG] bf16 staging (tma_store only)
   // a data gradient stages its tile only to accumulate, which the fused GroupNorm-backward epilogues (EPI 2/3) never do:
   // compiling the staging out of them keeps it from costing them registers
   const bool tma_store = EPI < 2 && p.tma_store;
-  const int Y_BYTES = tma_store ? 128 * p.cws * 2 : 0;
-  float* smT = reinterpret_cast<float*>(smY + 2 * (size_t)Y_BYTES);      // 2 x [64][kXP] fp32 transpose buffers
-  uint64_t* full = reinterpret_cast<uint64_t*>(smT + 2 * 64 * kXP);
+  const int Y_BYTES = tma_store ? 128 * CG * 2 : 0;
+  float* smT = reinterpret_cast<float*>(smY + 2 * (size_t)Y_BYTES);      // 2 x TBUF fp32 transpose buffers
+  uint64_t* full = reinterpret_cast<uint64_t*>(smT + 2 * TBUF);
   uint64_t* empty = full + p.stages;
-  // EPI 2/3: per consumer warp, the {rstd, -mean*rstd, gamma, beta} entries of the BN / 2 columns it handles in a tile
-  float4* smG = reinterpret_cast<float4*>(empty + p.stages) + (threadIdx.x >> 5) * (BN / 2);
+  // EPI 2/3: per consumer warp, the {rstd, -mean*rstd, gamma, beta} entries of the GT columns it handles in a tile
+  float4* smG = reinterpret_cast<float4*>(empty + p.stages) + (threadIdx.x >> 5) * GT;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_k = p.halo ? 3 * p.KC : p.T * p.KC;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // one arrival per consumer warp
+    // one arrival per consumer warp that reads the stage: both warpgroups (cooperative) or the tile's (ping-pong)
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], PP ? 4 : 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
@@ -153,52 +182,60 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
       }
     }
   } else {
-    const int wg = warp >> 2;                            // consumer warpgroup: rows 64 wg .. 64 wg + 63 of the tile
+    const int wg = warp >> 2;                            // consumer warpgroup
     const int wq = warp & 3;
-    const uint32_t a_row_off = (uint32_t)(wg * 64 * BK * 2);
-    // epilogue mapping: warp wq of the warpgroup owns pixel rows lane_base .. +31 and the 32-column half `ehalf` of every
-    // 64-column group
-    const int ehalf = wq >> 1;
+    // epilogue mapping: warp wq of the warpgroup owns pixel rows lane_base .. +31 of the tile; cooperative, it takes the
+    // 32-column half `ehalf` of every 64-column group of the warpgroup's 64 rows, ping-pong every column of its 32 rows
+    const int ehalf = PP ? 0 : wq >> 1;
     const bool bias_vec = (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0;   // leaf offsets are 16-byte aligned in the flat buffer; scalar loads otherwise
-    const int lane_base = wg * 64 + (wq & 1) * 32;
+    const int lane_base = PP ? wq * 32 : wg * 64 + (wq & 1) * 32;
     const int r = lane_base + lane;                      // row of the 128-pixel tile
     // pixel offset of row r from the tile's first pixel (one register across the tile loop instead of three coordinates)
     const unsigned rofs = (unsigned)((((r / (p.TW * p.TH)) * p.H + (r / p.TW) % p.TH) * p.W + r % p.TW));
-    float* tbuf = smT + wg * 64 * kXP;
+    float* tbuf = smT + wg * TBUF;
+    const int tr = PP ? r : r - wg * 64;                 // row of the transpose buffer
     const int fr = wq * 16 + (lane >> 2), fc = (lane & 3) * 2;   // accumulator fragment: rows fr, fr + 8; columns 8 i + fc, + 1
-    const bool y_issuer = threadIdx.x == 0;               // first consumer thread issues / retires the TMA stores
-    const int yswz = p.cws == 64 ? (r & 7) : ((r >> 1) & 3);
-    int ybox = 0;                                         // running count of staging boxes (selects the buffer)
-    int itg = 0;
-    float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    // the thread that issues / retires the TMA stores of a staging buffer: one per warpgroup (ping-pong) or per CTA
+    const bool y_issuer = (threadIdx.x & (PP ? 127 : 255)) == 0;
+    const int yswz = CG == 64 ? (r & 7) : ((r >> 1) & 3);
+    int ybox = 0;                                         // running count of staging boxes (cooperative: selects the buffer)
+    float acc[NACC][BN / 2];
+    // jt: the tile's index in the CTA's sequence, which fixes its ring iterations jt * total_k ..
+    for (int tile = blockIdx.x + (PP ? wg * gridDim.x : 0), jt = PP ? wg : 0; tile < p.total_tiles;
+         tile += (PP ? 2 : 1) * gridDim.x, jt += PP ? 2 : 1) {
       // ===== main loop: wgmma over the ring =====
+      if (PP && jt > 0) named_bar_sync(4 + wg, 256);    // the other warpgroup has seen every stage of tile jt - 1 land
+      int itg = jt * total_k;
       int prev_s = 0;
       for (int it = 0; it < total_k; ++it, ++itg) {
         const int s = itg % p.stages;
         mbar_wait(&full[s], (itg / p.stages) & 1);
         wgmma_fence();
-        const uint32_t a_addr = smem_u32(smA + (size_t)s * A_BYTES) + a_row_off;
         const uint32_t b_addr = smem_u32(smB + (size_t)s * B_BYTES);
-        if (p.halo) {
-          const uint32_t win = (uint32_t)(p.TW * BK * 2);
 #pragma unroll
-          for (int j = 0; j < 3; ++j)
+        for (int m = 0; m < NACC; ++m) {
+          const uint32_t a_addr = smem_u32(smA + (size_t)s * A_BYTES) + (uint32_t)((PP ? m : wg) * 64 * BK * 2);
+          if (p.halo) {
+            const uint32_t win = (uint32_t)(p.TW * BK * 2);
+#pragma unroll
+            for (int j = 0; j < 3; ++j)
+#pragma unroll
+              for (int k = 0; k < BK / 16; ++k)
+                Wgmma<BN>::template ss<0, 0>(acc[m], make_kmajor_desc<BK>(a_addr + j * win + k * 32),
+                                             make_kmajor_desc<BK>(b_addr + j * B_TILE + k * 32), (it > 0 || j > 0 || k > 0) ? 1u : 0u);
+          } else {
 #pragma unroll
             for (int k = 0; k < BK / 16; ++k)
-              Wgmma<BN>::template ss<0, 0>(acc, make_kmajor_desc<BK>(a_addr + j * win + k * 32),
-                                           make_kmajor_desc<BK>(b_addr + j * B_TILE + k * 32), (it > 0 || j > 0 || k > 0) ? 1u : 0u);
-        } else {
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            Wgmma<BN>::template ss<0, 0>(acc, make_kmajor_desc<BK>(a_addr + k * 32), make_kmajor_desc<BK>(b_addr + k * 32),
-                                         (it > 0 || k > 0) ? 1u : 0u);
+              Wgmma<BN>::template ss<0, 0>(acc[m], make_kmajor_desc<BK>(a_addr + k * 32), make_kmajor_desc<BK>(b_addr + k * 32),
+                                           (it > 0 || k > 0) ? 1u : 0u);
+          }
         }
         wgmma_commit();
         wgmma_wait<1>();                                 // the previous step's MMAs are done: release its stage
         if (it > 0 && lane == 0) mbar_arrive(&empty[prev_s]);
         prev_s = s;
       }
+      if (PP && tile + gridDim.x < p.total_tiles) named_bar_arrive(4 + (wg ^ 1), 256);
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(&empty[prev_s]);
 
@@ -212,11 +249,10 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
       bf16* yrow = p.y + pix * p.Co + (long long)n_tile * BN;
       const bf16* rrow = p.res ? p.res + pix * p.Co + (long long)n_tile * BN : nullptr;
       const float* brow = EPI < 2 && p.bias ? p.bias + (long long)n_tile * BN : nullptr;   // a data gradient has no bias
-      // CG accumulator columns per transpose group, CW of them per thread, whose operands are held in registers SW at a time.
-      // The fused GroupNorm-backward epilogues take their CW columns in 16-column sub-chunks (x, the FiLM operands and the
-      // statistics partials of 16 channels live at once), and a 32-column tile in one 32-column group so that all four warps
-      // of a warpgroup have columns: this lets them run two CTAs per SM without spilling.
-      constexpr int CG = EPI >= 2 && BN < 64 ? BN : 64, CW = CG / 2, SW = EPI >= 2 ? 8 : CW;
+      // The thread's CW columns of a group have their operands held in registers SW at a time: the fused GroupNorm-backward
+      // epilogues take 8-column sub-chunks (x, the FiLM operands and the statistics partials of 16 channels live at once),
+      // the ping-pong plain / statistics ones 16 columns: this lets them run two CTAs per SM without spilling.
+      constexpr int SW = EPI >= 2 ? 8 : (PP ? 16 : CW);
       // STATS: the 32 pixels of this warp belong to one sample (host-checked): b = image of the warp's first row / 2
       double* cs_row = nullptr;
       const long long srow = (long long)((n0 + lane_base / (p.TW * p.TH)) >> 1) * p.Co + (long long)n_tile * BN;
@@ -228,7 +264,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
         // stage the norm table of this warp's columns (entry cc / 2 + k <-> column cc + ehalf * CW + k) once per tile: read
         // from shared memory in the column loop instead of being held in registers
         __syncwarp();                   // the warp's reads of the previous tile's entries are done
-        for (int k = lane; k < BN / 2; k += 32) smG[k] = __ldg(gprow + (k / CW) * CG + ehalf * CW + k % CW);
+        for (int k = lane; k < GT; k += 32) smG[k] = __ldg(gprow + (k / CW) * CG + ehalf * CW + k % CW);
         __syncwarp();
       }
       const bf16* gerow = nullptr;
@@ -241,13 +277,18 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
       }
 #pragma unroll
       for (int cc = 0; cc < BN; cc += CG) {
-        // accumulator columns cc .. cc + CG - 1 of this warpgroup's 64 rows -> transpose buffer
+        // accumulator columns cc .. cc + CG - 1 of this warpgroup's rows -> transpose buffer
 #pragma unroll
-        for (int i = 0; i < BN / 2; i += 4) {
-          const int col = 8 * (i / 4);
-          if (col >= cc && col < cc + CG) {
-            *reinterpret_cast<float2*>(tbuf + fr * kXP + col - cc + fc) = make_float2(acc[i], acc[i + 1]);
-            *reinterpret_cast<float2*>(tbuf + (fr + 8) * kXP + col - cc + fc) = make_float2(acc[i + 2], acc[i + 3]);
+        for (int m = 0; m < NACC; ++m) {
+#pragma unroll
+          for (int i = 0; i < BN / 2; i += 4) {
+            const int col = 8 * (i / 4);
+            if (col >= cc && col < cc + CG) {
+              float* t0 = PP ? tbuf + conv_pp_tbuf_at(EPI, m * 64 + fr, col - cc + fc) : tbuf + fr * kXP + col - cc + fc;
+              float* t1 = PP ? tbuf + conv_pp_tbuf_at(EPI, m * 64 + fr + 8, col - cc + fc) : tbuf + (fr + 8) * kXP + col - cc + fc;
+              *reinterpret_cast<float2*>(t0) = make_float2(acc[m][i], acc[m][i + 1]);
+              *reinterpret_cast<float2*>(t1) = make_float2(acc[m][i + 2], acc[m][i + 3]);
+            }
           }
         }
         named_bar_sync(2 + wg, 128);
@@ -281,19 +322,19 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
         }
         float v[SW];
         if (active) {
-          const float* trow = tbuf + (r - wg * 64) * kXP + ehalf * CW + h;
 #pragma unroll
           for (int q = 0; q < SW / 4; ++q) {
-            const float4 t4 = *reinterpret_cast<const float4*>(trow + 4 * q);
+            const float* t = PP ? tbuf + conv_pp_tbuf_at(EPI, tr, h + 4 * q) : tbuf + tr * kXP + ehalf * CW + h + 4 * q;
+            const float4 t4 = *reinterpret_cast<const float4*>(t);
             v[4 * q] = t4.x; v[4 * q + 1] = t4.y; v[4 * q + 2] = t4.z; v[4 * q + 3] = t4.w;
           }
         }
-        const int ysub = p.cws == 64 ? ehalf : 0;
-        uint8_t* yst = smY + (size_t)(ybox & 1) * Y_BYTES + (size_t)r * (p.cws * 2);
-        if (tma_store) {           // (EPI < 2: a single sub-chunk)
-          // the store that read this staging buffer two boxes ago must have finished reading before it is overwritten
-          if (y_issuer) bulk_wait_group_read<1>();
-          named_bar_sync(1, 256);
+        // staging buffer: the warpgroup's own (ping-pong), or the CTA's two in turn
+        uint8_t* yst = smY + (size_t)(PP ? wg : (ybox & 1)) * Y_BYTES + (size_t)r * (CG * 2);
+        if (tma_store && h == 0) {
+          // the store that last read this staging buffer must have finished reading before it is overwritten
+          if (y_issuer) { if constexpr (PP) bulk_wait_group_read<0>(); else bulk_wait_group_read<1>(); }
+          if constexpr (PP) named_bar_sync(2 + wg, 128); else named_bar_sync(1, 256);
         }
         if (active) {
 #pragma unroll
@@ -319,7 +360,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
               const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(&rv[j >> 3]);
 #pragma unroll
               for (int q = 0; q < 8; ++q) {
-                const float4 pp = smG[cc / 2 + h + j + q];
+                const float4 pp = smG[(cc / CG) * CW + h + j + q];
                 const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
                 xh[q] = fmaf(xv, pp.x, pp.y);
                 if (p.gn_swish) f[q] *= swish_gradf_(fmaf(xh[q], pp.z, pp.w));
@@ -340,7 +381,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
               float tsc[8], tsh[8];
 #pragma unroll
               for (int q = 0; q < 8; ++q) {
-                const float4 pp = smG[cc / 2 + h + j + q];
+                const float4 pp = smG[(cc / CG) * CW + h + j + q];
                 const float xv = (q & 1) ? __high2float(x2[q >> 1]) : __low2float(x2[q >> 1]);
                 const float sc = (q & 1) ? __high2float(s2[q >> 1]) : __low2float(s2[q >> 1]);
                 const float sh = (q & 1) ? __high2float(h2[q >> 1]) : __low2float(h2[q >> 1]);
@@ -366,7 +407,7 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
             __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&outv);
 #pragma unroll
             for (int q = 0; q < 4; ++q) o2[q] = __floats2bfloat162_rn(f[2 * q], f[2 * q + 1]);
-            if (tma_store) sts128(yst + ((((ysub << 2) + ((h + j) >> 3)) ^ yswz) << 4), outv);
+            if (tma_store) sts128(yst + ((((ehalf * CW + h + j) >> 3) ^ yswz) << 4), outv);
             else *reinterpret_cast<uint4*>(yrow + c0 + j) = outv;
             if constexpr (EPI >= 2) {
               // sums over what is STORED (the second pass reads the rounded dyh back)
@@ -383,21 +424,22 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
 #pragma unroll
               for (int q = 0; q < 4; ++q) {
                 const float a = __low2float(o2[q]), b = __high2float(o2[q]);
-                sx[(j & 8) + 2 * q] = a;            sx[(j & 8) + 2 * q + 1] = b;
-                sx[16 + (j & 8) + 2 * q] = a * a;   sx[16 + (j & 8) + 2 * q + 1] = b * b;
+                sx[((h + j) & 8) + 2 * q] = a;            sx[((h + j) & 8) + 2 * q + 1] = b;
+                sx[16 + ((h + j) & 8) + 2 * q] = a * a;   sx[16 + ((h + j) & 8) + 2 * q + 1] = b * b;
               }
-              if (j & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
+              if ((h + j) & 8) xu_cstats_emit16(sx, lane, cs_row + (c0 + j - 8) * 2);
             }
           }
         }
         }
         if (tma_store) {
           fence_async_smem();                 // generic-proxy writes -> visible to the TMA unit
-          named_bar_sync(1, 256);
+          if constexpr (PP) named_bar_sync(2 + wg, 128); else named_bar_sync(1, 256);
           if (y_issuer) {
+            uint8_t* ybuf = smY + (size_t)(PP ? wg : (ybox & 1)) * Y_BYTES;
             // accumulate: the gradient is ADDED to the destination by the TMA unit (cp.reduce.async.bulk.tensor .add, bf16 at L2)
-            if (p.accumulate) tma_reduce_add_4d(smY + (size_t)(ybox & 1) * Y_BYTES, &tmY, n_tile * BN + cc, x0, y0, n0);
-            else tma_store_4d(smY + (size_t)(ybox & 1) * Y_BYTES, &tmY, n_tile * BN + cc, x0, y0, n0);
+            if (p.accumulate) tma_reduce_add_4d(ybuf, &tmY, n_tile * BN + cc, x0, y0, n0);
+            else tma_store_4d(ybuf, &tmY, n_tile * BN + cc, x0, y0, n0);
             bulk_commit_group();
           }
           ++ybox;
@@ -405,8 +447,8 @@ __global__ void __launch_bounds__(kConvThreads, conv_ctas_per_sm(EPI, BN, BK)) c
         named_bar_sync(2 + wg, 128);        // transpose buffer read by every warp before the next group overwrites it
       }
     }
+    if (tma_store && y_issuer) bulk_wait_group<0>();   // all output boxes written before the CTA retires
   }
-  if (tma_store && threadIdx.x == 0) bulk_wait_group<0>();   // all output boxes written before the CTA retires
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -695,25 +737,25 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
   // accumulating launch (the FiLM Dense data gradients summing into the embedding gradient) always stages its tile and adds
   // it with a TMA reduce-add: the epilogue never reads the destination.
   CUtensorMap tmY = tmA;
+  const int cws = p.BN % 64 == 0 ? 64 : 32;         // channels of one staged output box (the kernel's CG)
   {
     p.tma_store = a.accumulate ? 1 : (a.ks == 1 && a.mode == 0);
-    p.cws = p.BN % 64 == 0 ? 64 : 32;
     if (p.tma_store) {
       uint64_t yd[4] = {(uint64_t)a.Co, (uint64_t)a.Wo, (uint64_t)a.Ho, (uint64_t)a.N};
       uint64_t ys[3] = {(uint64_t)a.Co * 2, (uint64_t)a.Wo * a.Co * 2, (uint64_t)a.Ho * a.Wo * a.Co * 2};
-      uint32_t yb[4] = {(uint32_t)p.cws, (uint32_t)TW, (uint32_t)TH, (uint32_t)TN};
-      if (!encode_bf16(&tmY, a.y, 4, yd, ys, yb, p.cws)) return;
+      uint32_t yb[4] = {(uint32_t)cws, (uint32_t)TW, (uint32_t)TH, (uint32_t)TN};
+      if (!encode_bf16(&tmY, a.y, 4, yd, ys, yb, cws)) return;
     }
   }
-  const size_t ystage = p.tma_store ? (size_t)2 * 128 * p.cws * 2 : 0;
+  const size_t ystage = p.tma_store ? (size_t)2 * 128 * cws * 2 : 0;
   p.n_tiles = a.Co / p.BN;
   p.m_tiles = p.tiles_x * p.tiles_y * (a.N / TN);
   p.total_tiles = p.m_tiles * p.n_tiles;
   // CTAs per SM: two where the kernel is compiled for it (conv_ctas_per_sm) and shared
   // memory keeps a >= 3-deep TMA ring for each; one persistent CTA per SM with a 4-deep ring otherwise
   const int epi = a.gn_x == nullptr ? 0 : (a.gn_e != nullptr ? 3 : 2);
-  const size_t gtab = epi >= 2 ? (size_t)8 * (p.BN / 2) * 16 : 0;      // the EPI 2/3 per-warp norm tables (smG)
-  const size_t fixed = ystage + (size_t)2 * 64 * kXP * 4 + 1024 + 256 + gtab;
+  const size_t gtab = epi >= 2 ? (size_t)8 * (p.BN < 64 ? 32 : p.BN / 2) * 16 : 0;      // the EPI 2/3 per-warp norm tables (smG)
+  const size_t fixed = ystage + (size_t)2 * conv_tbuf_floats(epi, p.BN) * 4 + 1024 + 256 + gtab;
   int per_sm = 1, stages = 2;
   for (int cand = conv_ctas_per_sm(epi, p.BN, bk); cand >= 1; --cand) {
     const size_t budget = cand == 1 ? (size_t)227 * 1024 : (size_t)112 * 1024;
@@ -732,9 +774,11 @@ static void launch_conv_tc_impl(const ConvArgs& a, const void* wshadow, double* 
     static const bool log = getenv("XUNET_CONV_LOG") != nullptr;
     // epi: the epilogue template argument (1: forward with GroupNorm statistics)
     // acc: the output is added to the destination (TMA reduce-add); tma_store: the tile is staged and stored by TMA
-    if (log) fprintf(stderr, "conv_tc mode=%d N=%d %dx%d Ci=%d Co=%d ks=%d st=%d wCi=%d wCo=%d segw=%d bk=%d BN=%d KC=%d T=%d halo=%d stages=%d per_sm=%d ctas=%d tiles=%d epi=%d acc=%d tma_store=%d\n",
+    // sched: how the two consumer warpgroups share the tiles (cooperative: both on every tile; pingpong: whole tiles in turn)
+    if (log) fprintf(stderr, "conv_tc mode=%d N=%d %dx%d Ci=%d Co=%d ks=%d st=%d wCi=%d wCo=%d segw=%d bk=%d BN=%d KC=%d T=%d halo=%d stages=%d per_sm=%d ctas=%d tiles=%d epi=%d acc=%d tma_store=%d sched=%s\n",
                      a.mode, a.N, a.Ho, a.Wo, a.Ci, a.Co, a.ks, a.stride, a.wCi, a.wCo, a.segw, bk, p.BN, p.KC, p.T, p.halo, p.stages, per_sm, ctas, p.total_tiles,
-                     epi != 0 ? epi : (a.cstats != nullptr ? 1 : 0), a.accumulate ? 1 : 0, p.tma_store);
+                     epi != 0 ? epi : (a.cstats != nullptr ? 1 : 0), a.accumulate ? 1 : 0, p.tma_store,
+                     conv_pingpong(p.BN) ? "pingpong" : "cooperative");
   }
   p.cstats = cacc;
   p.gx = reinterpret_cast<const bf16*>(a.gn_x); p.gnp = reinterpret_cast<const float4*>(a.gn_params); p.gn_swish = a.gn_swish;
