@@ -165,6 +165,35 @@ int xunet_backward_vjp(xunet_handle* h, const float* params, const xunet_batch* 
                        const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate, float* dx, float* dz,
                        void* stream);
 
+/* Input gradients of xunet_backward_vjp_inputs: every pointer is a device fp32 buffer the caller owns, or NULL (not computed).
+ *   dx, dz: (B,S,S,3), as in xunet_backward_vjp.
+ *   d_rays: (B,2,S,S,6), the layout of xunet_batch.rays: dL/d[pos xyz | dir xyz] of every pixel's ray, camera 0 then camera 1,
+ *           whether the rays were given (batch->rays) or generated from R, t, K.  Samples with cond_mask = 0 get exact zeros
+ *           (their pose embedding is zeroed in the forward).  Required when any camera output below is set.
+ *   dR1, dt1, dR2, dt2, dK: (B,3,3) / (B,3) / (B,3,3): dL/dR, dL/dt of the cameras (R a free 3x3 matrix: projecting onto SO(3) is
+ *           the caller's job) and dL/dK of the intrinsics shared by both cameras.  Generated rays only (batch->rays == NULL).
+ * The log-SNR gets no gradient. */
+typedef struct xunet_input_grads {
+  float* dx;
+  float* dz;
+  float* d_rays;
+  float* dR1;
+  float* dt1;
+  float* dR2;
+  float* dt2;
+  float* dK;
+} xunet_input_grads;
+
+/* xunet_backward_vjp that also returns the gradients of the cameras / rays (out may be NULL: parameter gradient only).  The
+ * parameter gradient, dx and dz are bit for bit those of xunet_backward_vjp, with or without camera outputs.  The ray gradient is
+ * the data gradient of the pose-embedding convolutions (tensor cores in bf16 mode, weights as the forward's bf16 shadows) with
+ * the posenc Jacobian applied per pixel; the camera gradients are reduced from it in fp64 in a fixed order.  Fixed bits, no
+ * atomics, no allocation, graph-capturable.  Errors: those of xunet_backward_vjp, a camera output without d_rays, a camera
+ * output with batch->rays set. */
+int xunet_backward_vjp_inputs(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
+                              const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate,
+                              const xunet_input_grads* out, void* stream);
+
 /* Data-parallel hook (north_star: "one NCCL allreduce of the gradient bucket"; the reference's pmap step would place
  * lax.pmean between value_and_grad and apply_gradients, train.py:70-76).  With a callback installed, xunet_backward calls
  *     fn(user, elem_offset, n_elems)

@@ -27,6 +27,10 @@ class XunetBatch(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in ('x', 'z', 'logsnr', 'R1', 't1', 'R2', 't2', 'K', 'cond_mask', 'rays')]
 
 
+class XunetInputGrads(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ('dx', 'dz', 'd_rays', 'dR1', 'dt1', 'dR2', 'dt2', 'dK')]
+
+
 LAUNCH_CONV, LAUNCH_ATTN = 0, 1
 KERNEL_NONE, KERNEL_SIMT, KERNEL_TC, KERNEL_CIN3, KERNEL_COUT3 = -1, 0, 1, 2, 3
 
@@ -76,6 +80,8 @@ SYMBOLS = {
                            [C.c_int, C.c_void_p]),
     'xunet_backward_vjp': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 4 +
                            [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'xunet_backward_vjp_inputs': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 4 +
+                                  [C.c_int, C.POINTER(XunetInputGrads), C.c_void_p]),
     'xunet_set_grad_bucket_callback': (C.c_int, [C.c_void_p, BUCKET_FN, C.c_void_p, C.c_longlong]),
     'xunet_grad_bucket_count': (C.c_int, [C.c_void_p]),
     'xunet_count_kernels': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_void_p, C.c_void_p, C.c_void_p,

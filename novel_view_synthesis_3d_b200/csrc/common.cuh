@@ -161,6 +161,22 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// Ray direction of pixel (row, col) of a camera (model/xunet.py:159-161): normalize(R K^-1 p) with p = (row+.5, col+.5, 1)
+// (convention 0, visu3d 1.3) or (col+.5, row+.5, 1) (convention 1).  ki = K^-1 and R row-major, fp32 throughout; the pose
+// embedding and its gradient share it, so the gradient sees the forward's directions bit for bit.
+__device__ __forceinline__ void xu_ray_dir(const float* ki, const float* R, int row, int col, int convention, float (&d)[3]) {
+  const float p0 = (convention == 0 ? (float)row : (float)col) + 0.5f;
+  const float p1 = (convention == 0 ? (float)col : (float)row) + 0.5f;
+  float cx = ki[0] * p0 + ki[1] * p1 + ki[2];
+  float cy = ki[3] * p0 + ki[4] * p1 + ki[5];
+  float cz = ki[6] * p0 + ki[7] * p1 + ki[8];
+  float wx = R[0] * cx + R[1] * cy + R[2] * cz;
+  float wy = R[3] * cx + R[4] * cy + R[5] * cz;
+  float wz = R[6] * cx + R[7] * cy + R[8] * cz;
+  float inv = 1.f / sqrtf(wx * wx + wy * wy + wz * wz);
+  d[0] = wx * inv; d[1] = wy * inv; d[2] = wz * inv;
+}
+
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // SM count of the current device (132 on an H100 SXM), queried once; grids of persistent / wave-sized kernels derive from it

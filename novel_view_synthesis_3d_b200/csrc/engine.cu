@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "conv_tc.h"
+#include "pose_grad.h"
 
 #include <math.h>
 #include <stdarg.h>
@@ -680,6 +681,7 @@ struct Ctx {
   const float* d_eps = nullptr;  // backward: seed with the caller's dL/d(eps_hat) (B,S,S,3) instead of a loss (xunet_backward_vjp)
   float* dx = nullptr;           // backward: dL/dx and dL/dz (B,S,S,3) fp32 of the two input views, nullptr = not computed
   float* dz = nullptr;
+  const xunet_input_grads* cam = nullptr;   // backward: ray / camera gradients (xunet_backward_vjp_inputs), nullptr = none
   void* act(int t) const { return ws + h->tensors[t].off; }
   void* grad(int t) const { const Tensor& x = h->tensors[t]; return ws + (x.galias >= 0 ? h->tensors[x.galias].goff : x.goff); }
   float gscale(int t) const { return h->tensors[t].gscale; }
@@ -857,6 +859,32 @@ static int forward_impl(Ctx& c, float* eps_out) {
   return 0;
 }
 
+// ray (and camera) gradient of the backward's OP_POSE step: every grad(pose_emb_l) is final, on this stream.  bf16: the
+// levels whose forward runs on the tensor cores (and so has a bf16 weight shadow) run the wgmma kernel one by one, level 0
+// storing d_rays and the rest adding; the others (small images, forward on SIMT cores too) follow in one SIMT launch.  fp32:
+// one SIMT launch over all levels.
+static void run_pose_grad(const Ctx& c) {
+  const xunet_handle* h = c.h;
+  const xunet_batch* bt = c.batch;
+  PoseGradArgs a{bt->R1, bt->t1, bt->R2, bt->t2, bt->K, c.aux(h->a_kinv), bt->rays, bt->cond_mask, c.cam->d_rays,
+                 h->B, h->S, h->cfg.emb_ch, h->cfg.ray_convention};
+  PoseLevels simt{};
+  int stored = 0;
+  for (const Op& o : h->ops) {
+    if (o.kind != OP_CONV || o.x != h->t_pose) continue;
+    const PoseLevel L{c.grad(o.y), c.P(o.w), o.alpha * c.gscale(o.y), o.cs.Ho, o.cs.stride, o.cs.pad_h};
+    if (h->dtype == XU_BF16 && o.k.fwd == CONV_TC && pose_grad_tc_supported(L.So, a.E)) {
+      launch_pose_grad_tc(a, L, c.shadow(o.wT), stored, c.s);
+      stored = 1;
+    } else {
+      simt.l[simt.n++] = L;
+    }
+  }
+  if (simt.n > 0) launch_pose_grad_simt(h->dtype, a, simt, stored, c.s);
+  const xunet_input_grads* g = c.cam;
+  if (g->dR1 || g->dt1 || g->dR2 || g->dt2 || g->dK) launch_camera_grad(a, g->dR1, g->dt1, g->dR2, g->dt2, g->dK, c.s);
+}
+
 static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
   xunet_handle* h = c.h;
   const int dt = h->dtype, B = h->B, S = h->S, E = h->cfg.emb_ch;
@@ -954,6 +982,7 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
       case OP_POSE:
         if (h->tensors[o.y].need_grad)
           launch_pose_emb_bwd(dt, c.grad(o.y), c.G(o.p0), c.G(o.p1), c.G(o.p2), B, S, c.acc_grads, c.s);
+        if (c.cam != nullptr && c.cam->d_rays != nullptr) run_pose_grad(c);
         break;
       case OP_LOGSNR:
         launch_logsnr_emb_bwd(c.aux(h->a_dlemb), c.P(o.p2), c.aux(h->a_pe), c.aux(h->a_h1), c.aux(h->a_dh1), c.G(o.p0),
@@ -1181,20 +1210,41 @@ extern "C" int xunet_backward_mse(xunet_handle* h, const float* params, const xu
   return backward_impl(c, noise, loss_out);
 }
 
-extern "C" int xunet_backward_vjp(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
-                                  const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate, float* dx,
-                                  float* dz, void* stream) {
-  if (!h || !params || !batch || !d_eps || !workspace || !grads) return fail("xunet_backward_vjp: null argument");
-  if (!h->training) return fail("xunet_backward_vjp: handle was created with training=0");
-  if (!h->forward_done_train) return fail("xunet_backward_vjp: call xunet_forward first");
+static int backward_vjp(const char* fn, xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
+                        const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate,
+                        const xunet_input_grads& out, void* stream) {
+  if (!h || !params || !batch || !d_eps || !workspace || !grads) return fail("%s: null argument", fn);
+  if (!h->training) return fail("%s: handle was created with training=0", fn);
+  if (!h->forward_done_train) return fail("%s: call xunet_forward first", fn);
+  const bool cams = out.dR1 || out.dt1 || out.dR2 || out.dt2 || out.dK;
+  if (cams && !out.d_rays) return fail("%s: camera gradients need d_rays", fn);
+  if (cams && batch->rays) return fail("%s: camera gradients need generated rays (batch->rays == NULL)", fn);
   xu_set_kernel_error("");
   Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
   c.acc_grads = accumulate ? 1 : 0;
   c.d_eps = d_eps;
-  c.dx = dx;
-  c.dz = dz;
+  c.dx = out.dx;
+  c.dz = out.dz;
+  c.cam = out.d_rays ? &out : nullptr;
   XuDetBind bind(h->det);
   return backward_impl(c, nullptr, nullptr);
+}
+
+extern "C" int xunet_backward_vjp(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
+                                  const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate, float* dx,
+                                  float* dz, void* stream) {
+  xunet_input_grads out{};
+  out.dx = dx;
+  out.dz = dz;
+  return backward_vjp("xunet_backward_vjp", h, params, batch, d_eps, seed_dev, workspace, grads, accumulate, out, stream);
+}
+
+extern "C" int xunet_backward_vjp_inputs(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
+                                         const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate,
+                                         const xunet_input_grads* out, void* stream) {
+  xunet_input_grads none{};
+  return backward_vjp("xunet_backward_vjp_inputs", h, params, batch, d_eps, seed_dev, workspace, grads, accumulate,
+                      out ? *out : none, stream);
 }
 
 static int count_kernel_nodes(cudaGraph_t g) {

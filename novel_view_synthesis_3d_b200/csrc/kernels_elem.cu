@@ -1119,17 +1119,9 @@ __global__ void __launch_bounds__(256) pose_emb_kernel(const float* __restrict__
     } else if (tid >= 128 && tid < 128 + kPosePix && pix0 + tid - 128 < HW) {
       const int pix = pix0 + tid - 128;
       const int row = pix / S, col = pix - row * S;
-      const float p0 = (convention == 0 ? (float)row : (float)col) + 0.5f;
-      const float p1 = (convention == 0 ? (float)col : (float)row) + 0.5f;
-      const float* ki = kinv + b * 9;
-      float cx = ki[0] * p0 + ki[1] * p1 + ki[2];
-      float cy = ki[3] * p0 + ki[4] * p1 + ki[5];
-      float cz = ki[6] * p0 + ki[7] * p1 + ki[8];
-      float wx = R[0] * cx + R[1] * cy + R[2] * cz;
-      float wy = R[3] * cx + R[4] * cy + R[5] * cz;
-      float wz = R[6] * cx + R[7] * cy + R[8] * cz;
-      float inv = 1.f / sqrtf(wx * wx + wy * wy + wz * wz);
-      s_dir[tid - 128][0] = wx * inv; s_dir[tid - 128][1] = wy * inv; s_dir[tid - 128][2] = wz * inv;
+      float d[3];
+      xu_ray_dir(kinv + b * 9, R, row, col, convention, d);
+      s_dir[tid - 128][0] = d[0]; s_dir[tid - 128][1] = d[1]; s_dir[tid - 128][2] = d[2];
     }
   }
   __syncthreads();

@@ -22,6 +22,7 @@ from . import _lib
 
 POSE_EMB_DIM = 144
 BATCH_KEYS = ('x', 'z', 'logsnr', 'R1', 't1', 'R2', 't2', 'K')
+CAMERA_KEYS = ('R1', 't1', 'R2', 't2', 'K')
 INPUT_ORDER = BATCH_KEYS + ('cond_mask', 'noise', 'loss_weight')     # segment order of Engine.inp_all
 LOSSES = ('frobenius', 'mse')
 
@@ -260,6 +261,8 @@ class Engine:
         self.seed = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.grads = torch.zeros(self.nparams, **f32) if training else None
         self.dx = self.dz = None  # backward_vjp's input gradients (B,S,S,3), allocated at the first call that asks for them
+        self.cam_grads = {}       # backward_vjp_inputs' ray / camera gradients by name, allocated at the first call that asks
+        self._fwd_rays = None     # the explicit rays of the last forward (kept alive for the ray gradient of its VJP)
         self.forward_count = 0    # forwards run so far: a VJP taken later checks that its forward is still the last one
         self._taps = None
         self._bucket_cb = None    # keeps the ctypes callback object alive while it is installed
@@ -315,6 +318,7 @@ class Engine:
         sd = self.seed if seed_dev is None else seed_dev
         st = torch.cuda.current_stream(self.device).cuda_stream
         self.forward_count += 1
+        self._fwd_rays = self.rays if inputs is None else None
         _lib.check(self.lib.xunet_forward(self.h, flat_params.data_ptr(), C.byref(cb), int(train),
                                           sd.data_ptr(), self.ws.data_ptr(), self.eps.data_ptr(), st), 'xunet_forward')
         return self.eps
@@ -358,12 +362,7 @@ class Engine:
         tensor (B,S,S,3).  Returns (self.grads, dx, dz): the parameter gradient (accumulate=True adds into self.grads) and, when
         asked for, dL/dx and dL/dz of the input views in the engine's own (B,S,S,3) buffers, which the next call overwrites
         (None when not asked for).  Follows forward() with the same `inputs` and `seed_dev`, like backward()."""
-        if not self.training:
-            raise RuntimeError('engine was built with training=False')
-        shape = (self.B, self.S, self.S, 3)
-        if not (isinstance(d_eps, torch.Tensor) and d_eps.is_cuda and d_eps.dtype == torch.float32 and d_eps.is_contiguous()
-                and tuple(d_eps.shape) == shape):
-            raise ValueError(f'd_eps must be a contiguous fp32 CUDA tensor of shape {shape}')
+        shape = self._check_d_eps(d_eps)
         if dx and self.dx is None:
             self.dx = torch.zeros(shape, dtype=torch.float32, device=self.device)
         if dz and self.dz is None:
@@ -376,6 +375,49 @@ class Engine:
                                                self.dx.data_ptr() if dx else None, self.dz.data_ptr() if dz else None, st),
                    'xunet_backward_vjp')
         return self.grads, (self.dx if dx else None), (self.dz if dz else None)
+
+    def _check_d_eps(self, d_eps) -> Tuple[int, ...]:
+        if not self.training:
+            raise RuntimeError('engine was built with training=False')
+        shape = (self.B, self.S, self.S, 3)
+        if not (isinstance(d_eps, torch.Tensor) and d_eps.is_cuda and d_eps.dtype == torch.float32 and d_eps.is_contiguous()
+                and tuple(d_eps.shape) == shape):
+            raise ValueError(f'd_eps must be a contiguous fp32 CUDA tensor of shape {shape}')
+        return shape
+
+    def backward_vjp_inputs(self, flat_params: torch.Tensor, d_eps: torch.Tensor, *, accumulate: bool = False, dx: bool = False,
+                            dz: bool = False, rays: bool = False, cameras: bool = False,
+                            inputs: Optional[Tuple[InputSlots, int]] = None, seed_dev: Optional[torch.Tensor] = None):
+        """backward_vjp that also differentiates the cameras (xunet_backward_vjp_inputs).  Returns (self.grads, dict): 'x' / 'z'
+        when dx / dz, 'rays' = dL/d(rays) (B,2,S,S,6) [pos | dir] of camera 1 / camera 2 when rays or cameras, and 'R1', 't1',
+        'R2', 't2', 'K' when cameras (the forward's rays must then have been generated from R, t, K, not given).  The tensors
+        are the engine's own buffers, overwritten by the next call.  The parameter gradient, dx and dz are those backward_vjp
+        gives, bit for bit.  The log-SNR gets no gradient."""
+        shape = self._check_d_eps(d_eps)
+        if cameras and self._fwd_rays is not None:
+            raise ValueError('camera gradients need rays generated from R, t, K: the forward was given explicit rays')
+        sizes = {'x': shape, 'z': shape, 'rays': (self.B, 2, self.S, self.S, 6), 'R1': (self.B, 3, 3), 't1': (self.B, 3),
+                 'R2': (self.B, 3, 3), 't2': (self.B, 3), 'K': (self.B, 3, 3)}
+        want = [k for k, on in (('x', dx), ('z', dz), ('rays', rays or cameras)) if on] + (list(CAMERA_KEYS) if cameras else [])
+        out = {}
+        for k in want:
+            if k in ('x', 'z'):
+                if getattr(self, 'd' + k) is None:
+                    setattr(self, 'd' + k, torch.zeros(shape, dtype=torch.float32, device=self.device))
+                out[k] = getattr(self, 'd' + k)
+            else:
+                if k not in self.cam_grads:
+                    self.cam_grads[k] = torch.zeros(sizes[k], dtype=torch.float32, device=self.device)
+                out[k] = self.cam_grads[k]
+        ig = _lib.XunetInputGrads(**{('d_rays' if k == 'rays' else 'd' + k): v.data_ptr() for k, v in out.items()})
+        cb = _lib.XunetBatch.from_buffer_copy(self.cbatch if inputs is None else inputs[0].cbatch[inputs[1]])
+        cb.rays = self._fwd_rays.data_ptr() if (inputs is None and self._fwd_rays is not None) else None
+        sd = self.seed if seed_dev is None else seed_dev
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.lib.xunet_backward_vjp_inputs(self.h, flat_params.data_ptr(), C.byref(cb), d_eps.data_ptr(), sd.data_ptr(),
+                                                      self.ws.data_ptr(), self.grads.data_ptr(), int(accumulate), C.byref(ig), st),
+                   'xunet_backward_vjp_inputs')
+        return self.grads, out
 
     def count_kernels(self, flat_params: torch.Tensor) -> Tuple[int, int]:
         """(forward, backward) kernel launches of this plan, counted from a throw-away graph capture."""
@@ -512,7 +554,8 @@ class XUNet:
         with torch.no_grad():
             eng.load_inputs({k: batch[k].detach() if isinstance(batch[k], torch.Tensor) else batch[k] for k in BATCH_KEYS},
                             cond_mask=cond_mask.detach() if isinstance(cond_mask, torch.Tensor) else cond_mask)
-        eng.set_rays(rays if rays is not None else batch.get('rays'))
+        rays = rays if rays is not None else batch.get('rays')
+        eng.set_rays(rays.detach() if isinstance(rays, torch.Tensor) else rays)
         seed = _seed_of(rngs.get('dropout') if isinstance(rngs, dict) else rngs)
         try:
             eps = eng.forward(flat.detach(), train=train, seed=seed).clone()
@@ -526,19 +569,25 @@ class XUNet:
             raise RuntimeError(f'another forward ran on this engine since the one being differentiated (forward {count}, now '
                                f'{eng.forward_count}): its activations are gone; run the forward again')
 
-    def vjp(self, variables, batch, *, cond_mask, train: bool, rngs=None, rays=None):
+    def vjp(self, variables, batch, *, cond_mask, train: bool, rngs=None, rays=None, camera_grads: bool = False):
         """jax.vjp over XUNet.apply: returns (eps_hat, vjp_fn).  vjp_fn(d_eps), d_eps = dL/d(eps_hat) a contiguous fp32 device
         tensor (B,S,S,3), returns (ParamTree of a copy of dL/dparams, {'x': dL/dx, 'z': dL/dz}); it may be called more than once,
-        as long as no other forward has run on the training engine engine(B, S, True) in between (else RuntimeError)."""
+        as long as no other forward has run on the training engine engine(B, S, True) in between (else RuntimeError).
+        camera_grads=True adds the camera gradients to that dict: 'R1', 't1', 'R2', 't2', 'K' (R a free 3x3 matrix), or 'rays'
+        (B,2,S,S,6) when explicit rays were given.  The log-SNR gets no gradient."""
         x = batch['x']
         B, S = int(x.shape[0]), int(x.shape[1])
         flat = self.flat_from_tree(variables['params'], S, B)
+        explicit = (rays if rays is not None else batch.get('rays')) is not None
         eng, eps, count = self._train_forward(flat, batch, cond_mask, train, rngs, rays)
 
         def vjp_fn(d_eps):
             self._check_current(eng, count)
-            grads, dx, dz = eng.backward_vjp(flat.detach(), d_eps, dx=True, dz=True)
-            return self.tree_from_flat(grads.clone(), S, B, spec=eng.spec), {'x': dx.clone(), 'z': dz.clone()}
+            if not camera_grads:
+                grads, dx, dz = eng.backward_vjp(flat.detach(), d_eps, dx=True, dz=True)
+                return self.tree_from_flat(grads.clone(), S, B, spec=eng.spec), {'x': dx.clone(), 'z': dz.clone()}
+            grads, out = eng.backward_vjp_inputs(flat.detach(), d_eps, dx=True, dz=True, rays=explicit, cameras=not explicit)
+            return self.tree_from_flat(grads.clone(), S, B, spec=eng.spec), {k: v.clone() for k, v in out.items()}
 
         return eps, vjp_fn
 
@@ -546,15 +595,22 @@ class XUNet:
         """XUNet.apply as a torch.autograd.Function on the training engine: eps_hat (B,S,S,3) with a grad_fn, so that
         loss(eps_hat).backward() fills flat_params.grad and, for CUDA tensors batch['x'] / batch['z'] that require grad, their
         .grad.  Runs the same engine calls as vjp() (forward, then xunet_backward_vjp); the backward is once-differentiable and
-        raises RuntimeError if another forward has run on the engine in between."""
-        return _XUNetVJP.apply(flat_params, batch['x'], batch['z'], self, batch, cond_mask, train, rngs, rays)
+        raises RuntimeError if another forward has run on the engine in between.
+        Camera tensors batch['R1'], 't1', 'R2', 't2', 'K' (generated rays) or the explicit `rays` that are CUDA tensors requiring
+        grad get their .grad too (xunet_backward_vjp_inputs, the same values as vjp(camera_grads=True)); the camera kernels run
+        only when one of them needs a gradient.  The log-SNR gets no gradient."""
+        rays = rays if rays is not None else batch.get('rays')
+        cams = [batch[k] if isinstance(batch[k], torch.Tensor) else None for k in CAMERA_KEYS]
+        ray_t = rays if isinstance(rays, torch.Tensor) else None
+        return _XUNetVJP.apply(flat_params, batch['x'], batch['z'], *cams, ray_t, self, batch, cond_mask, train, rngs, rays)
 
 
 class _XUNetVJP(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, flat_params, x, z, model, batch, cond_mask, train, rngs, rays):
+    def forward(ctx, flat_params, x, z, R1, t1, R2, t2, K, ray_t, model, batch, cond_mask, train, rngs, rays):
         eng, eps, count = model._train_forward(flat_params, dict(batch, x=x, z=z), cond_mask, train, rngs, rays)
-        ctx.eng, ctx.count = eng, count
+        ctx.eng, ctx.count, ctx.explicit = eng, count, rays is not None
+        ctx.cams = [(t.shape, t.dtype) if t is not None else None for t in (R1, t1, R2, t2, K, ray_t)]
         ctx.save_for_backward(flat_params)        # an in-place update of the parameters before backward() then raises
         return eps
 
@@ -564,6 +620,18 @@ class _XUNetVJP(torch.autograd.Function):
         XUNet._check_current(ctx.eng, ctx.count)
         flat, = ctx.saved_tensors
         need_p, need_x, need_z = ctx.needs_input_grad[:3]
-        grads, dx, dz = ctx.eng.backward_vjp(flat.detach(), d_eps.to(torch.float32).contiguous(), dx=need_x, dz=need_z)
-        return (grads.clone() if need_p else None, dx.clone() if need_x else None, dz.clone() if need_z else None,
-                None, None, None, None, None, None)
+        need_cam = ctx.needs_input_grad[3:9]
+        cameras = any(need_cam[:5]) and not ctx.explicit       # with explicit rays the cameras do not reach eps_hat
+        rays = need_cam[5] and ctx.explicit
+        d_eps = d_eps.to(torch.float32).contiguous()
+        if not (cameras or rays):
+            grads, dx, dz = ctx.eng.backward_vjp(flat.detach(), d_eps, dx=need_x, dz=need_z)
+            return (grads.clone() if need_p else None, dx.clone() if need_x else None, dz.clone() if need_z else None,
+                    None, None, None, None, None, None, None, None, None, None, None, None)
+        grads, out = ctx.eng.backward_vjp_inputs(flat.detach(), d_eps, dx=need_x, dz=need_z, rays=rays, cameras=cameras)
+        cam = []
+        for key, need, meta in zip(CAMERA_KEYS + ('rays',), need_cam, ctx.cams):
+            ok = need and key in out and (key == 'rays') == ctx.explicit
+            cam.append(out[key].reshape(meta[0]).to(meta[1]).clone() if ok else None)
+        return (grads.clone() if need_p else None, out['x'].clone() if need_x else None, out['z'].clone() if need_z else None,
+                *cam, None, None, None, None, None, None)
