@@ -114,6 +114,39 @@ typedef struct xunet_launch_info {
 int xunet_plan_launch_count(const xunet_handle* h);
 int xunet_plan_launch(const xunet_handle* h, int i, xunet_launch_info* out);
 
+/* The plan's other launches, in op order (read-only; needs no GPU): what each op's forward and backward launchers receive, so
+ * that tests can run them through the operator-level entry points below at the plan's arguments. */
+#define XUNET_PLAN_OP_LOGSNR 0          /* the log-SNR MLP: xunet_op_logsnr_emb / _bwd at (B, E) */
+#define XUNET_PLAN_OP_POSE 1            /* rays + NeRF posenc: xunet_op_pose_emb / _bwd at (B, S) */
+#define XUNET_PLAN_OP_EMB 2             /* swish(logsnr_emb + pose-embedding level): xunet_op_film_emb / _bwd */
+#define XUNET_PLAN_OP_RESAMPLE 3        /* the residual path of a resampling ResnetBlock: xunet_op_resample */
+#define XUNET_PLAN_OP_CONCAT 4          /* a skip-connection concat: xunet_op_copy_channels, two per direction */
+#define XUNET_PLAN_OP_ATTN_RESIDUAL 5   /* the residual gradient of an attention block: xunet_op_scale_add */
+#define XUNET_PLAN_OP_LOSS 6            /* the frame-1 output and the ||eps_hat - eps|| loss: xunet_op_loss */
+typedef struct xunet_op_info {
+  int kind;                /* XUNET_PLAN_OP_* */
+  int B, S, E;             /* the plan's samples, image side and emb_ch */
+  int N, H, W, C;          /* the op's input (N, H, W, C): EMB the pose-embedding level; RESAMPLE x; CONCAT its first input a;
+                              ATTN_RESIDUAL the block output; else N = 2B, H = W = S and C = E (LOGSNR), 144 (POSE), 3 (LOSS) */
+  int C2;                  /* CONCAT: channels of the second input b */
+  int copies[4][5];        /* CONCAT: (Cs, Cd, src_off, dst_off, Cc) of the forward copies of a and b into y, then of the
+                              backward copies of grad(y) into grad(a) and grad(b) */
+  int rs;                  /* RESAMPLE: XUNET_RS_DOWN or XUNET_RS_UP */
+  int fwd_pool;            /* RESAMPLE: xunet_op_resample's pool and scale in the forward */
+  float fwd_scale;
+  float gscale;            /* RESAMPLE: scale of the output's aliased gradient (1: not aliased) */
+  int bwd_pool;            /* RESAMPLE: pool and scale of the backward (the adjoint, on the output's gradient) */
+  float bwd_scale;
+  float alpha;             /* ATTN_RESIDUAL: grad(residual) = alpha grad(output) (+ the prior when acc_r) */
+  int acc_x, acc_r;        /* the backward adds into grad(x) / grad(second input) instead of storing */
+  int need_grad;           /* the backward runs (POSE: the parameter gradients; CONCAT: grad(a) is written) */
+  int need_grad_r;         /* CONCAT: grad(b) is written */
+  int write_dpe;           /* EMB: the backward writes the gradient of the pose-embedding level */
+  int pos_emb, ref_pose_emb, ray_convention;   /* POSE: the pos_emb / ref_pose_emb leaves exist; XUNET_RAYS_* */
+} xunet_op_info;
+int xunet_plan_op_count(const xunet_handle* h);
+int xunet_plan_op(const xunet_handle* h, int i, xunet_op_info* out);
+
 /* XUNet.apply({'params': p}, batch, cond_mask=, train=, rngs=)  (train.py:63-66, sampling.py:131-132).
  * params: device, flat fp32.  seed_dev: device pointer to ONE uint64 dropout seed (read at execution
  * time, so a captured graph sees updates); may be NULL when train==0.  eps_out: device (B,S,S,3) fp32. */
@@ -448,6 +481,45 @@ int xunet_op_groupnorm_bwd(int dtype, const void* x, const void* e, const void* 
                            const void* extra, float extra_alpha, int N, int H, int W, int C, int mode, int resample,
                            float drop_rate, int op_index, const unsigned long long* seed_dev, int train, int accumulate,
                            int de_accumulate, void* stream);
+
+/* ---- operator-level entry points of the conditioning, resampling, concat and loss launches: each runs the launches the
+ * engine runs for that op and nothing else, and checks its arguments before launching anything.  fp32 unless dtype says. */
+/* log-SNR MLP (B samples, E = emb_ch): pe = posenc_ddpm(1000 * 2 atan(exp(-clip(logsnr, +-20) / 2)) / pi) (B, E),
+ * h1 = pe w0 + b0, lemb = swish(h1) w1 + b1; w (E, E) row-major (Flax Dense kernel), b (E). */
+int xunet_op_logsnr_emb(const float* logsnr, const float* w0, const float* b0, const float* w1, const float* b1, float* pe, float* h1,
+                        float* lemb, int B, int E, void* stream);
+/* its backward from dlemb: dh1 = swish'(h1) (dlemb w1^T); dw1 = swish(h1)^T dlemb, db1 = sum_b dlemb, dw0 = pe^T dh1,
+ * db0 = sum_b dh1, stored (accumulate: added). */
+int xunet_op_logsnr_emb_bwd(const float* dlemb, const float* w1, const float* pe, const float* h1, float* dh1, float* dw0, float* db0,
+                            float* dw1, float* db1, int B, int E, int accumulate, void* stream);
+/* pose embedding out (2B, S, S, 144) of dtype: per frame [posenc_nerf(ray origin, 15) | posenc_nerf(ray direction, 8)],
+ * zero where cond_mask[b] == 0, plus pos_emb (S, S, 144) and ref_first / ref_other (144) when given.  Generated rays
+ * (rays == NULL): kinv (B, 9) receives K^-1 and the directions are normalize(R K^-1 p), p per convention (XUNET_RAYS_*);
+ * else rays (B, 2, S, S, 6) as in xunet_batch. */
+int xunet_op_pose_emb(int dtype, const float* R1, const float* t1, const float* R2, const float* t2, const float* K,
+                      const float* cond_mask, const float* pos_emb, const float* ref_first, const float* ref_other, float* kinv,
+                      void* out, int B, int S, int convention, const float* rays, void* stream);
+/* its parameter gradients from dpose (2B, S, S, 144): dpos_emb = sum over both frames of every sample (stored; accumulate:
+ * added; may be NULL), dref_first / dref_other += the sums over frames 0 / 1 (both NULL or both given). */
+int xunet_op_pose_emb_bwd(int dtype, const void* dpose, float* dpos_emb, float* dref_first, float* dref_other, int B, int S,
+                          int accumulate, void* stream);
+/* semb = swish(lemb[n / 2] + pe) over pe (N, HW, E) of dtype, N = 2B. */
+int xunet_op_film_emb(int dtype, const float* lemb, const void* pe, void* semb, int N, int HW, int E, void* stream);
+/* its backward: dz = dsemb swish'(lemb + pe); dpe = dz when write_dpe; dlemb (B, E) += the sum of dz over both frames. */
+int xunet_op_film_emb_bwd(int dtype, const float* lemb, const void* pe, const void* dsemb, void* dpe, float* dlemb, int N, int HW,
+                          int E, int write_dpe, void* stream);
+/* y = scale * (pool ? the 2x2 sum of x : x repeated 2x2) (+ y when accumulate), x (N, H, W, C) of dtype, C a multiple of 4. */
+int xunet_op_resample(int dtype, const void* x, void* y, int N, int H, int W, int C, int pool, float scale, int accumulate,
+                      void* stream);
+/* dst[p, dst_off + c] = src[p, src_off + c] (+ dst when accumulate) for c < Cc, p < npix; src rows of Cs, dst rows of Cd channels.
+ * Every channel count and offset a multiple of 4. */
+int xunet_op_copy_channels(int dtype, const void* src, void* dst, long long npix, int Cs, int Cd, int src_off, int dst_off, int Cc,
+                           int accumulate, void* stream);
+/* dst = alpha src (+ dst when accumulate) over n elements of dtype, n a multiple of 4. */
+int xunet_op_scale_add(int dtype, const void* src, void* dst, long long n, float alpha, int accumulate, void* stream);
+/* loss = ||eps - noise|| over (B, S, S, 3) fp32; sumsq (1 float) receives the sum of squares, loss (1 float) the loss, and
+ * dO (2B, S, S, 3) of dtype the output gradient: frame 1 of sample b = (eps[b] - noise[b]) / loss (0 when loss == 0), frame 0 = 0. */
+int xunet_op_loss(int dtype, const float* eps, const float* noise, float* sumsq, float* loss, void* dO, int B, int S, void* stream);
 
 #ifdef __cplusplus
 }

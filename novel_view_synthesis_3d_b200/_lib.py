@@ -43,6 +43,18 @@ class XunetLaunchInfo(C.Structure):
         [(k, C.c_int) for k in ('L', 'C', 'heads', 'cross', 'impl')]
 
 
+PLAN_OP_LOGSNR, PLAN_OP_POSE, PLAN_OP_EMB, PLAN_OP_RESAMPLE, PLAN_OP_CONCAT, PLAN_OP_ATTN_RESIDUAL, PLAN_OP_LOSS = range(7)
+RS_NONE, RS_DOWN, RS_UP = 0, 1, 2
+
+
+class XunetOpInfo(C.Structure):
+    _fields_ = [(k, C.c_int) for k in ('kind', 'B', 'S', 'E', 'N', 'H', 'W', 'C', 'C2')] + \
+        [('copies', (C.c_int * 5) * 4), ('rs', C.c_int), ('fwd_pool', C.c_int), ('fwd_scale', C.c_float), ('gscale', C.c_float),
+         ('bwd_pool', C.c_int), ('bwd_scale', C.c_float), ('alpha', C.c_float)] + \
+        [(k, C.c_int) for k in ('acc_x', 'acc_r', 'need_grad', 'need_grad_r', 'write_dpe', 'pos_emb', 'ref_pose_emb',
+                                'ray_convention')]
+
+
 class XunetSrnStore(C.Structure):
     _fields_ = [('pixels', C.c_void_p), ('pixel_kind', C.c_int), ('S', C.c_int), ('n_items', C.c_longlong),
                 ('n_instances', C.c_int), ('R', C.c_void_p), ('t', C.c_void_p), ('K', C.c_void_p), ('first', C.c_void_p),
@@ -69,6 +81,8 @@ SYMBOLS = {
                             C.POINTER(C.c_longlong), C.POINTER(C.c_int), C.POINTER(C.c_longlong)]),
     'xunet_plan_launch_count': (C.c_int, [C.c_void_p]),
     'xunet_plan_launch': (C.c_int, [C.c_void_p, C.c_int, C.POINTER(XunetLaunchInfo)]),
+    'xunet_plan_op_count': (C.c_int, [C.c_void_p]),
+    'xunet_plan_op': (C.c_int, [C.c_void_p, C.c_int, C.POINTER(XunetOpInfo)]),
     'xunet_forward': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_int, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p]),
     'xunet_set_static_conditioning': (C.c_int, [C.c_void_p, C.c_int]),
@@ -125,6 +139,16 @@ SYMBOLS = {
                                       [C.c_float, C.c_void_p]),
     'xunet_op_groupnorm_bwd': (C.c_int, [C.c_int] + [C.c_void_p] * 13 + [C.c_float] + [C.c_int] * 6 +
                                [C.c_float, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'xunet_op_logsnr_emb': (C.c_int, [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_void_p]),
+    'xunet_op_logsnr_emb_bwd': (C.c_int, [C.c_void_p] * 9 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'xunet_op_pose_emb': (C.c_int, [C.c_int] + [C.c_void_p] * 11 + [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    'xunet_op_pose_emb_bwd': (C.c_int, [C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'xunet_op_film_emb': (C.c_int, [C.c_int] + [C.c_void_p] * 3 + [C.c_int] * 3 + [C.c_void_p]),
+    'xunet_op_film_emb_bwd': (C.c_int, [C.c_int] + [C.c_void_p] * 5 + [C.c_int] * 4 + [C.c_void_p]),
+    'xunet_op_resample': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_float, C.c_int, C.c_void_p]),
+    'xunet_op_copy_channels': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_longlong] + [C.c_int] * 6 + [C.c_void_p]),
+    'xunet_op_scale_add': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float, C.c_int, C.c_void_p]),
+    'xunet_op_loss': (C.c_int, [C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p]),
 }
 
 _lib = None

@@ -28,7 +28,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 108; }
+extern "C" int xunet_version(void) { return 109; }
 
 namespace {
 
@@ -300,6 +300,21 @@ static GnArgs gn_fill(const void* x, void* y, const void* e, const float* gamma,
   a.drop_rate = drop_rate; a.op_index = op_index; a.seed_dev = seed_dev; a.train = train;
   a.skip_zero = 1;
   return a;
+}
+
+// the resample launches of an OP_RESAMPLE: the forward averages 2x2 pixels (RS_DOWN) or repeats each pixel 2x2 (RS_UP); the
+// backward runs the adjoint on the output's gradient -- replicate x 0.25, or the 2x2 sum -- times that gradient's alias scale
+struct ResampleArgs { int pool; float scale; };
+static ResampleArgs resample_fwd_args(int rs) { return {rs == RS_DOWN ? 1 : 0, rs == RS_DOWN ? 0.25f : 1.f}; }
+static ResampleArgs resample_bwd_args(int rs, float gscale) { return {rs == RS_UP ? 1 : 0, (rs == RS_DOWN ? 0.25f : 1.f) * gscale}; }
+
+// one channel copy of a concat y = [a | b] (ca + cb channels): the forward copies a (second = 0) or b into y, the backward
+// copies the matching channels of grad(y) out to grad(a) or grad(b)
+struct ChannelCopy { int Cs, Cd, src_off, dst_off, Cc; };
+static ChannelCopy concat_copy(int ca, int cb, bool bwd, bool second) {
+  const int Cd = ca + cb;
+  if (!bwd) return second ? ChannelCopy{cb, Cd, 0, ca, cb} : ChannelCopy{ca, Cd, 0, 0, ca};
+  return second ? ChannelCopy{Cd, cb, ca, 0, cb} : ChannelCopy{Cd, ca, 0, 0, ca};
 }
 
 struct Builder {
@@ -658,6 +673,9 @@ struct Builder {
         Op& cv = H.ops[gn.gnb];
         if (cv.acc_x != 0 || (gn.mode == GN_FILM && gn.acc_e != 0)) { cv.gnb = -1; gn.gnb = -1; }
       }
+      // emb_bwd_kernel stores grad(pose-embedding level): each level must feed nothing but its own OP_EMB
+      for (const Op& o : H.ops)
+        if (o.kind == OP_EMB && o.acc_x) return fail("internal: a pose-embedding level has a gradient writer besides its OP_EMB");
     }
     for (const Op& o : H.ops)
       if (o.kind == OP_GN && o.cs_a < 0) return fail("internal: a GroupNorm input has no producer-emitted statistics");
@@ -826,15 +844,18 @@ static int forward_impl(Ctx& c, float* eps_out) {
       }
       case OP_RESAMPLE: {
         const Tensor& x = h->tensors[o.x];
-        launch_resample(dt, c.act(o.x), c.act(o.y), x.n, x.h, x.w, x.c, o.rs == RS_DOWN, o.rs == RS_DOWN ? 0.25f : 1.f, 0, c.s);
+        const ResampleArgs r = resample_fwd_args(o.rs);
+        launch_resample(dt, c.act(o.x), c.act(o.y), x.n, x.h, x.w, x.c, r.pool, r.scale, 0, c.s);
         break;
       }
       case OP_CONCAT: {
         const Tensor& a = h->tensors[o.x];
         const Tensor& b = h->tensors[o.r];
         const long long npix = (long long)a.n * a.h * a.w;
-        launch_copy_channels(dt, c.act(o.x), c.act(o.y), npix, a.c, a.c + b.c, 0, 0, a.c, 0, c.s);
-        launch_copy_channels(dt, c.act(o.r), c.act(o.y), npix, b.c, a.c + b.c, 0, a.c, b.c, 0, c.s);
+        for (int k = 0; k < 2; ++k) {
+          const ChannelCopy cc = concat_copy(a.c, b.c, false, k == 1);
+          launch_copy_channels(dt, c.act(k ? o.r : o.x), c.act(o.y), npix, cc.Cs, cc.Cd, cc.src_off, cc.dst_off, cc.Cc, 0, c.s);
+        }
         break;
       }
       case OP_ATTN: {
@@ -948,16 +969,20 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
       }
       case OP_RESAMPLE: {
         const Tensor& y = h->tensors[o.y];
-        // adjoint: avg-pool <-> 0.25 * replicate ; replicate <-> 2x2 sum
-        launch_resample(dt, c.grad(o.y), c.grad(o.x), y.n, y.h, y.w, y.c, o.rs == RS_UP, (o.rs == RS_DOWN ? 0.25f : 1.f) * c.gscale(o.y), o.acc_x, c.s);
+        const ResampleArgs r = resample_bwd_args(o.rs, c.gscale(o.y));
+        launch_resample(dt, c.grad(o.y), c.grad(o.x), y.n, y.h, y.w, y.c, r.pool, r.scale, o.acc_x, c.s);
         break;
       }
       case OP_CONCAT: {
         const Tensor& a = h->tensors[o.x];
         const Tensor& b = h->tensors[o.r];
         const long long npix = (long long)a.n * a.h * a.w;
-        if (a.need_grad) launch_copy_channels(dt, c.grad(o.y), c.grad(o.x), npix, a.c + b.c, a.c, 0, 0, a.c, o.acc_x, c.s);
-        if (b.need_grad) launch_copy_channels(dt, c.grad(o.y), c.grad(o.r), npix, a.c + b.c, b.c, a.c, 0, b.c, o.acc_r, c.s);
+        for (int k = 0; k < 2; ++k) {
+          if (!(k ? b : a).need_grad) continue;
+          const ChannelCopy cc = concat_copy(a.c, b.c, true, k == 1);
+          launch_copy_channels(dt, c.grad(o.y), c.grad(k ? o.r : o.x), npix, cc.Cs, cc.Cd, cc.src_off, cc.dst_off, cc.Cc,
+                               k ? o.acc_r : o.acc_x, c.s);
+        }
         break;
       }
       case OP_ATTN: {
@@ -1129,6 +1154,97 @@ extern "C" int xunet_plan_launch(const xunet_handle* h, int i, xunet_launch_info
       r.accumulate = o.acc_x;
       if (o.gnb >= 0) r.gn_mode = h->ops[o.gnb].mode;
     }
+  }
+  *out = r;
+  return 0;
+}
+
+static int plan_op_kind(const Op& o) {
+  switch (o.kind) {
+    case OP_LOGSNR: return XUNET_PLAN_OP_LOGSNR;
+    case OP_POSE: return XUNET_PLAN_OP_POSE;
+    case OP_EMB: return XUNET_PLAN_OP_EMB;
+    case OP_RESAMPLE: return XUNET_PLAN_OP_RESAMPLE;
+    case OP_CONCAT: return XUNET_PLAN_OP_CONCAT;
+    case OP_ATTN: return XUNET_PLAN_OP_ATTN_RESIDUAL;
+    case OP_EXTRACT: return XUNET_PLAN_OP_LOSS;
+    default: return -1;
+  }
+}
+
+extern "C" int xunet_plan_op_count(const xunet_handle* h) {
+  int n = 0;
+  for (const Op& o : h->ops) n += plan_op_kind(o) >= 0;
+  return n;
+}
+
+// every field comes from the op and the helpers forward_impl / backward_impl launch it with
+extern "C" int xunet_plan_op(const xunet_handle* h, int i, xunet_op_info* out) {
+  if (!h || !out) return fail("xunet_plan_op: null argument");
+  int k = -1;
+  for (size_t j = 0; j < h->ops.size() && i >= 0; ++j)
+    if (plan_op_kind(h->ops[j]) >= 0 && i-- == 0) k = (int)j;
+  if (k < 0) return fail("xunet_plan_op: index out of range");
+  const Op& o = h->ops[k];
+  const bool tr = h->training != 0;
+  xunet_op_info r;
+  memset(&r, 0, sizeof(r));
+  r.kind = plan_op_kind(o);
+  r.B = h->B; r.S = h->S; r.E = h->cfg.emb_ch;
+  r.N = h->N; r.H = h->S; r.W = h->S;
+  r.fwd_scale = r.gscale = r.bwd_scale = r.alpha = 1.f;
+  r.need_grad = tr;
+  switch (o.kind) {
+    case OP_LOGSNR: r.C = h->cfg.emb_ch; break;
+    case OP_POSE: {
+      const Tensor& y = h->tensors[o.y];
+      r.C = y.c;
+      r.need_grad = y.need_grad;
+      r.pos_emb = o.p0 >= 0; r.ref_pose_emb = o.p1 >= 0; r.ray_convention = h->cfg.ray_convention;
+      break;
+    }
+    case OP_EMB: {
+      const Tensor& x = h->tensors[o.x];
+      r.N = x.n; r.H = x.h; r.W = x.w; r.C = x.c;
+      r.acc_x = o.acc_x;
+      r.write_dpe = tr && x.need_grad;
+      break;
+    }
+    case OP_RESAMPLE: {
+      const Tensor& x = h->tensors[o.x];
+      const Tensor& y = h->tensors[o.y];
+      r.N = x.n; r.H = x.h; r.W = x.w; r.C = x.c;
+      r.rs = o.rs;
+      const ResampleArgs f = resample_fwd_args(o.rs), b = resample_bwd_args(o.rs, y.gscale);
+      r.fwd_pool = f.pool; r.fwd_scale = f.scale;
+      r.gscale = y.gscale;
+      r.bwd_pool = b.pool; r.bwd_scale = b.scale;
+      r.acc_x = o.acc_x;
+      break;
+    }
+    case OP_CONCAT: {
+      const Tensor& a = h->tensors[o.x];
+      const Tensor& b = h->tensors[o.r];
+      r.N = a.n; r.H = a.h; r.W = a.w; r.C = a.c; r.C2 = b.c;
+      for (int q = 0; q < 4; ++q) {
+        const ChannelCopy cc = concat_copy(a.c, b.c, q >= 2, q & 1);
+        const int v[5] = {cc.Cs, cc.Cd, cc.src_off, cc.dst_off, cc.Cc};
+        memcpy(r.copies[q], v, sizeof(v));
+      }
+      r.acc_x = o.acc_x; r.acc_r = o.acc_r;
+      r.need_grad = tr && a.need_grad;
+      r.need_grad_r = tr && b.need_grad;
+      break;
+    }
+    case OP_ATTN: {
+      const Tensor& y = h->tensors[o.y];
+      r.N = y.n; r.H = y.h; r.W = y.w; r.C = y.c;
+      r.alpha = XU_RSQRT2;
+      r.acc_r = o.acc_r;
+      r.need_grad = tr && !o.fuse_res;   // else the residual gradient is added inside a GroupNorm backward
+      break;
+    }
+    case OP_EXTRACT: r.C = 3; break;
   }
   *out = r;
   return 0;
@@ -1683,5 +1799,156 @@ extern "C" int xunet_op_groupnorm_bwd(int dtype, const void* x, const void* e, c
     launch_gn_bwd_reduce(dtype, a, (cudaStream_t)stream);
     launch_gn_bwd_apply(dtype, a, (cudaStream_t)stream);
   }
+  return op_done(what);
+}
+
+// ---- operator-level entry points of the conditioning, resampling, concat and loss launches -----------------------------
+static int dtype_ok(const char* what, int dtype) {
+  return dtype == XUNET_DTYPE_F32 || dtype == XUNET_DTYPE_BF16 ? 0 : fail("%s: bad dtype %d", what, dtype);
+}
+// 4-wide vector accesses: 16-byte (fp32) / 8-byte (bf16) aligned pointers
+static int vec_aligned(const char* what, int dtype, const void* p) {
+  const size_t a = dtype == XUNET_DTYPE_F32 ? 16 : 8;
+  return (reinterpret_cast<uintptr_t>(p) % a) == 0 ? 0 : fail("%s: pointer %p is not %zu-byte aligned", what, p, a);
+}
+static int emb_check(const char* what, int B, int E) {
+  if (B < 1) return fail("%s: B = %d, need B >= 1", what, B);
+  if (E < 4 || E % 4 != 0) return fail("%s: E = %d, need a positive multiple of 4", what, E);
+  return 0;
+}
+
+extern "C" int xunet_op_logsnr_emb(const float* logsnr, const float* w0, const float* b0, const float* w1, const float* b1, float* pe,
+                                   float* h1, float* lemb, int B, int E, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_logsnr_emb";
+  if (!logsnr || !w0 || !b0 || !w1 || !b1 || !pe || !h1 || !lemb) return fail("%s: NULL pointer argument", what);
+  if (emb_check(what, B, E)) return 1;
+  OpScratch scratch;
+  launch_logsnr_emb(logsnr, w0, b0, w1, b1, pe, h1, lemb, B, E, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_logsnr_emb_bwd(const float* dlemb, const float* w1, const float* pe, const float* h1, float* dh1, float* dw0,
+                                       float* db0, float* dw1, float* db1, int B, int E, int accumulate, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_logsnr_emb_bwd";
+  if (!dlemb || !w1 || !pe || !h1 || !dh1 || !dw0 || !db0 || !dw1 || !db1) return fail("%s: NULL pointer argument", what);
+  if (emb_check(what, B, E)) return 1;
+  OpScratch scratch;
+  launch_logsnr_emb_bwd(dlemb, w1, pe, h1, dh1, dw0, db0, dw1, db1, B, E, accumulate ? 1 : 0, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_pose_emb(int dtype, const float* R1, const float* t1, const float* R2, const float* t2, const float* K,
+                                 const float* cond_mask, const float* pos_emb, const float* ref_first, const float* ref_other,
+                                 float* kinv, void* out, int B, int S, int convention, const float* rays, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_pose_emb";
+  if (dtype_ok(what, dtype)) return 1;
+  if (!cond_mask || !out) return fail("%s: NULL pointer argument", what);
+  if (!rays && (!R1 || !t1 || !R2 || !t2 || !K || !kinv)) return fail("%s: generated rays need R1, t1, R2, t2, K and kinv", what);
+  if (!ref_first != !ref_other) return fail("%s: ref_first and ref_other are given together", what);
+  if (B < 1 || S < 1) return fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
+  if (convention != XUNET_RAYS_V3D130_IJ && convention != XUNET_RAYS_OPENCV_UV) return fail("%s: bad ray convention %d", what, convention);
+  OpScratch scratch;
+  launch_pose_emb(dtype, R1, t1, R2, t2, K, cond_mask, pos_emb, ref_first, ref_other, kinv, out, B, S, convention, rays,
+                  (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_pose_emb_bwd(int dtype, const void* dpose, float* dpos_emb, float* dref_first, float* dref_other, int B, int S,
+                                     int accumulate, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_pose_emb_bwd";
+  if (dtype_ok(what, dtype)) return 1;
+  if (!dpose) return fail("%s: NULL pointer argument", what);
+  if (!dref_first != !dref_other) return fail("%s: dref_first and dref_other are given together", what);
+  if (B < 1 || S < 1) return fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
+  OpScratch scratch;
+  launch_pose_emb_bwd(dtype, dpose, dpos_emb, dref_first, dref_other, B, S, accumulate ? 1 : 0, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+static int film_emb_check(const char* what, int dtype, int N, int HW, int E) {
+  if (dtype_ok(what, dtype)) return 1;
+  if (N < 2 || N % 2 != 0) return fail("%s: N = %d, need an even N >= 2 (two frames per sample)", what, N);
+  if (HW < 1) return fail("%s: HW = %d, need HW >= 1", what, HW);
+  return emb_check(what, N / 2, E);
+}
+
+extern "C" int xunet_op_film_emb(int dtype, const float* lemb, const void* pe, void* semb, int N, int HW, int E, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_film_emb";
+  if (!lemb || !pe || !semb) return fail("%s: NULL pointer argument", what);
+  if (film_emb_check(what, dtype, N, HW, E) || vec_aligned(what, dtype, pe) || vec_aligned(what, dtype, semb)) return 1;
+  OpScratch scratch;
+  launch_emb_fwd(dtype, lemb, pe, semb, N, HW, E, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_film_emb_bwd(int dtype, const float* lemb, const void* pe, const void* dsemb, void* dpe, float* dlemb, int N,
+                                     int HW, int E, int write_dpe, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_film_emb_bwd";
+  if (!lemb || !pe || !dsemb || !dlemb || (write_dpe && !dpe)) return fail("%s: NULL pointer argument", what);
+  if (film_emb_check(what, dtype, N, HW, E) || vec_aligned(what, dtype, pe) || vec_aligned(what, dtype, dsemb) ||
+      (write_dpe && vec_aligned(what, dtype, dpe)))
+    return 1;
+  OpScratch scratch;
+  launch_emb_bwd(dtype, lemb, pe, dsemb, write_dpe ? dpe : nullptr, dlemb, N, HW, E, write_dpe ? 1 : 0, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_resample(int dtype, const void* x, void* y, int N, int H, int W, int C, int pool, float scale, int accumulate,
+                                 void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_resample";
+  if (!x || !y) return fail("%s: NULL pointer argument", what);
+  if (dtype_ok(what, dtype) || vec_aligned(what, dtype, x) || vec_aligned(what, dtype, y)) return 1;
+  if (N < 1 || H < 1 || W < 1) return fail("%s: N = %d, H = %d, W = %d, need all >= 1", what, N, H, W);
+  if (C < 4 || C % 4 != 0) return fail("%s: C = %d, need a positive multiple of 4", what, C);
+  if (pool && (H % 2 != 0 || W % 2 != 0)) return fail("%s: pooling needs even H, W (got %d x %d)", what, H, W);
+  OpScratch scratch;
+  launch_resample(dtype, x, y, N, H, W, C, pool ? 1 : 0, scale, accumulate ? 1 : 0, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_copy_channels(int dtype, const void* src, void* dst, long long npix, int Cs, int Cd, int src_off, int dst_off,
+                                      int Cc, int accumulate, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_copy_channels";
+  if (!src || !dst) return fail("%s: NULL pointer argument", what);
+  if (dtype_ok(what, dtype) || vec_aligned(what, dtype, src) || vec_aligned(what, dtype, dst)) return 1;
+  if (npix < 1) return fail("%s: npix = %lld, need npix >= 1", what, npix);
+  if (Cc < 4 || Cs % 4 || Cd % 4 || src_off % 4 || dst_off % 4 || Cc % 4)
+    return fail("%s: Cs = %d, Cd = %d, src_off = %d, dst_off = %d, Cc = %d, need multiples of 4 and Cc >= 4", what, Cs, Cd, src_off,
+                dst_off, Cc);
+  if (src_off < 0 || dst_off < 0 || src_off + Cc > Cs || dst_off + Cc > Cd)
+    return fail("%s: channels [%d, %d) of %d to [%d, %d) of %d out of range", what, src_off, src_off + Cc, Cs, dst_off, dst_off + Cc, Cd);
+  OpScratch scratch;
+  launch_copy_channels(dtype, src, dst, npix, Cs, Cd, src_off, dst_off, Cc, accumulate ? 1 : 0, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_scale_add(int dtype, const void* src, void* dst, long long n, float alpha, int accumulate, void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_scale_add";
+  if (!src || !dst) return fail("%s: NULL pointer argument", what);
+  if (dtype_ok(what, dtype) || vec_aligned(what, dtype, src) || vec_aligned(what, dtype, dst)) return 1;
+  if (n < 4 || n % 4 != 0) return fail("%s: n = %lld, need a positive multiple of 4", what, n);
+  OpScratch scratch;
+  launch_scale_add(dtype, src, dst, n, alpha, accumulate ? 1 : 0, (cudaStream_t)stream);
+  return op_done(what);
+}
+
+extern "C" int xunet_op_loss(int dtype, const float* eps, const float* noise, float* sumsq, float* loss, void* dO, int B, int S,
+                             void* stream) {
+  xu_set_kernel_error("");
+  const char* what = "xunet_op_loss";
+  if (!eps || !noise || !sumsq || !loss || !dO) return fail("%s: NULL pointer argument", what);
+  if (dtype_ok(what, dtype)) return 1;
+  if (B < 1 || S < 1) return fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
+  OpScratch scratch;
+  launch_loss(dtype, eps, noise, sumsq, loss, dO, B, S, (cudaStream_t)stream);
   return op_done(what);
 }

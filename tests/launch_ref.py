@@ -106,11 +106,12 @@ def store_rel(bf16):
 
 
 def excess(got, ref, bound):
-    """(worst (|got - ref|) / bound, the flat index where it occurs, number of elements over their bound)"""
+    """(worst (|got - ref|) / bound, the flat index where it occurs, number of elements over their bound).  A NaN result is
+    over its bound (and the worst)."""
     err = (got.double() - ref).abs()
     r = err / bound.clamp_min(1e-300)
     i = int(torch.argmax(r.reshape(-1)))
-    return float(r.reshape(-1)[i]), i, int((err > bound).sum())
+    return float(r.reshape(-1)[i]), i, int((~(err <= bound)).sum())
 
 
 def within(got, ref, bound):

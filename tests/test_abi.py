@@ -150,3 +150,47 @@ def test_plan_launches_cover_every_conv_leaf_and_attention_block(lib, plan):
     if dtype == 0:
         assert all(_lib.KERNEL_TC not in (r['fwd'], r['dgrad'], r['wgrad']) for r in convs)
         assert all(r['impl'] == 0 for r in attns)
+
+
+# ---- the plan's other ops (xunet_plan_op): counts against the topology, the resample adjoints and their alias scales ----
+@pytest.mark.parametrize('plan', list(L.PLANS))
+def test_plan_ops_match_the_topology(lib, plan):
+    import novel_view_synthesis_3d_b200 as P
+    from tests import plan_ops_ref as O
+    preset, S, B, dtype, training = L.PLANS[plan]
+    cfg = getattr(P, preset)
+    ops = O.plan_ops(lib, cfg, B, S, dtype, training)
+    launches, _ = L.plan_launches(lib, cfg, B, S, dtype, training)
+    nl = len(cfg.ch_mult)
+    kinds = [o['kind'] for o in ops]
+    assert kinds.count(_lib.PLAN_OP_LOGSNR) == 1 and kinds.count(_lib.PLAN_OP_POSE) == 1 and kinds.count(_lib.PLAN_OP_LOSS) == 1
+    assert kinds.count(_lib.PLAN_OP_EMB) == nl
+    assert kinds.count(_lib.PLAN_OP_RESAMPLE) == 2 * (nl - 1)
+    assert kinds.count(_lib.PLAN_OP_CONCAT) == (cfg.num_res_blocks + 1) * nl
+    assert kinds.count(_lib.PLAN_OP_ATTN_RESIDUAL) == sum(r['kind'] == _lib.LAUNCH_ATTN for r in launches)
+    for o in ops:
+        assert (o['B'], o['S'], o['E']) == (B, S, cfg.emb_ch)
+        if o['kind'] == _lib.PLAN_OP_EMB:
+            # emb_bwd_kernel stores the level's gradient: nothing else may write it
+            assert o['acc_x'] == 0 and o['C'] == cfg.emb_ch and o['write_dpe'] == training
+        if o['kind'] == _lib.PLAN_OP_POSE:
+            assert o['need_grad'] == int(bool(training and (cfg.use_pos_emb or cfg.use_ref_pose_emb)))
+            assert (o['pos_emb'], o['ref_pose_emb'], o['ray_convention']) == (cfg.use_pos_emb, cfg.use_ref_pose_emb,
+                                                                             _lib.RAYS[cfg.ray_convention])
+        if o['kind'] == _lib.PLAN_OP_CONCAT:
+            a, b = o['C'], o['C2']
+            assert o['copies'] == ((a, a + b, 0, 0, a), (b, a + b, 0, a, b), (a + b, a, 0, 0, a), (a + b, b, a, 0, b))
+        if o['kind'] != _lib.PLAN_OP_RESAMPLE:
+            continue
+        # the backward is the forward's adjoint (RS_DOWN: 0.25 x replicate; RS_UP: the 2x2 sum) times the alias scale
+        down = o['rs'] == _lib.RS_DOWN
+        assert o['rs'] in (_lib.RS_DOWN, _lib.RS_UP)
+        assert (o['fwd_pool'], o['fwd_scale']) == ((1, 0.25) if down else (0, 1.))
+        assert o['bwd_pool'] == (0 if down else 1)
+        assert o['bwd_scale'] == np.float32(np.float32(0.25 if down else 1.) * np.float32(o['gscale']))
+        Ho, Wo = (o['H'] // 2, o['W'] // 2) if down else (2 * o['H'], 2 * o['W'])
+        # the alias scale is 1 or the alpha of a residual conv that reads this output at its shape
+        assert o['gscale'] == 1. or any(r['kind'] == _lib.LAUNCH_CONV and r['residual'] and r['alpha'] == o['gscale'] and
+                                         (r['N'], r['Ho'], r['Wo'], r['Co']) == (o['N'], Ho, Wo, o['C']) for r in launches)
+        if not training:
+            assert o['gscale'] == 1.
