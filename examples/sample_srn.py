@@ -4,6 +4,7 @@ ancestral sampler, write PNGs (the reference blocks in cv2.imshow, which cannot 
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --steps 256 --out results/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --prefix ema --steps 256 --out results_ema/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --method dpmpp_2m --steps 25 --out results_dpm/
+    python examples/sample_srn.py cars_train_val --ckpt checkpoints_v --prediction v --method dpmpp_2m --steps 25 --out results_v/
 """
 import argparse
 import os
@@ -30,6 +31,8 @@ def main():
                     help='timestep spacing (default: logsnr for dpmpp_2m, linear otherwise)')
     ap.add_argument('--dynamic-threshold', type=float, default=None, metavar='P',
                     help='threshold x0 per view at the P-quantile of |x0| (Imagen: 0.995) instead of clipping it to [-1, 1]')
+    ap.add_argument('--prediction', choices=P.sampling.PREDICTIONS, default='eps',
+                    help='what the checkpoint predicts: the noise (eps) or v (a model trained with --prediction v)')
     ap.add_argument('--views', type=int, default=1)
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--out', default='results')
@@ -44,7 +47,7 @@ def main():
     batch = next(ds.batches(a.views))
     model = P.XUNet()
     sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing,
-                        dynamic_threshold=a.dynamic_threshold)
+                        dynamic_threshold=a.dynamic_threshold, prediction=a.prediction)
     os.makedirs(a.out, exist_ok=True)
     if a.orbit > 0:
         it = ds.batches(a.views)

@@ -8,6 +8,7 @@ state (state<step>: params, Adam moments and count, EMA, cond_mask streams) that
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --max-grad-norm 1 --warmup-steps 5000 --ema-decay 0.9999
     python examples/train_srn.py cars_train_val --batch 4 --side 128 --grad-accum-steps 8     # 32 samples per update
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --loss mse --min-snr-gamma 5
+    python examples/train_srn.py cars_train_val --batch 8 --side 64 --loss mse --prediction v --device-data
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --device-data --data-cache cars64.cache
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_srn.py cars_train_val
 """
@@ -44,7 +45,11 @@ def main():
     ap.add_argument('--loss', choices=('frobenius', 'mse'), default='frobenius',
                     help="training loss: the reference's ||eps_hat - noise||_F, or the mean squared error of DDPM / 3DiM")
     ap.add_argument('--min-snr-gamma', type=float, default=None,
-                    help='with --loss mse: weight each sample by min(SNR_t, G) / SNR_t (min-SNR-gamma, e.g. 5)')
+                    help='with --loss mse: weight each sample by min(SNR_t, G) / SNR_t, or min(SNR_t, G) / (SNR_t + 1) with '
+                         '--prediction v (min-SNR-gamma, e.g. 5)')
+    ap.add_argument('--prediction', choices=P.sampling.PREDICTIONS, default='eps',
+                    help='what the network learns to predict: the noise (eps) or v = sqrt(abar) eps - sqrt(1 - abar) x0 '
+                         '(needs --loss mse; sample the checkpoints with --prediction v)')
     ap.add_argument('--device-data', action='store_true',
                     help='decode every view once into GPU memory and draw, gather and noise each batch inside the step; '
                          'the ranks then split one global batch per update instead of each reading its own stream')
@@ -55,11 +60,14 @@ def main():
     a = ap.parse_args()
     if a.min_snr_gamma is not None and a.loss != 'mse':
         ap.error('--min-snr-gamma needs --loss mse')
+    if a.prediction == 'v' and a.loss != 'mse':
+        ap.error('--prediction v needs --loss mse')
     local = xdist.init_from_env('nccl')
     rank, world = xdist.rank(), xdist.world_size()
     model = P.XUNet(dtype=a.dtype)
     state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model, ema_decay=a.ema_decay,
-                                 max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps, loss=a.loss)
+                                 max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps, loss=a.loss,
+                                 prediction=a.prediction)
     if a.resume and P.checkpoint.restore_train_state(a.ckpt, state) is not None and rank == 0:
         print(f'resumed from step {state.step}')
     if a.device_data:
@@ -74,7 +82,7 @@ def main():
         return
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50, seed=rank)      # train.py:99-104
     step = P.TrainStep(state, grad_accum_steps=a.grad_accum_steps)
-    fd = P.ForwardDiffusion(step.eng, min_snr_gamma=a.min_snr_gamma)
+    fd = P.ForwardDiffusion(step.eng, min_snr_gamma=a.min_snr_gamma, prediction=a.prediction)   # 'noise' holds v for v
     dev_keys = ('z', 'logsnr', 'noise', 'cond_mask') + (('loss_weight',) if fd.loss_weight is not None else ())
     stream = ds.batches(a.batch)
     k = a.grad_accum_steps

@@ -292,12 +292,16 @@ int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, 
 /* One ancestral update of sampling.py:128-151 with the schedule on the device, for a per-step CUDA graph (forward + this call
  * + counter increment) that is replayed with no host arithmetic in between (the reference does the schedule math in numpy
  * between two un-jitted model calls, sampling.py:133-151).  Given the 2B-batched model output eps2 =
- * [eps_cond (B,S,S,3); eps_uncond (B,S,S,3)] and the coefficients of row k = *pos_dev of the table:
- *     eps = (1+w) eps_c - w eps_u;  x0 = clip(c_recip z - c_recipm1 eps, -1, 1);  z' = c1 x0 + c2 z + sigma * noise_k.
- * table: device (steps, 8) floats, row k (k = 0: first executed step = highest t) = {c_recip = sqrt_recip_alphas_cumprod,
- * c_recipm1 = sqrt_recipm1_alphas_cumprod, c1 = posterior_mean_coef1, c2 = posterior_mean_coef2, sigma (0 at t=0), log-SNR
- * fed to the NEXT forward (sampling.py:151), 0, 0} (a DDIM table puts its c_x0, c_z, sigma in columns 2-4); pos_dev: device int32 loop position (the caller increments it after the
- * call, in stream order).  z (n = B*S*S*3) is updated in place; the new z is also written to both halves of the next
+ * [out_cond (B,S,S,3); out_uncond (B,S,S,3)] and the coefficients of row k = *pos_dev of the table:
+ *     out = (1+w) out_c - w out_u;  x0 = clip(c_recip z - c_recipm1 out, -1, 1);  z' = c1 x0 + c2 z + sigma * noise_k.
+ * The step is linear in the network output, so the table decides what that output is: an eps-prediction table has
+ * c_recip = sqrt_recip_alphas_cumprod = 1/sqrt(abar), c_recipm1 = sqrt_recipm1_alphas_cumprod = sqrt(1/abar - 1); a
+ * v-prediction table (v = sqrt(abar) eps - sqrt(1 - abar) x0, so x0 = sqrt(abar) z - sqrt(1 - abar) v) has c_recip = sqrt(abar),
+ * c_recipm1 = sqrt(1 - abar).  This holds for every step entry below.
+ * table: device (steps, 8) floats, row k (k = 0: first executed step = highest t) = {c_recip, c_recipm1,
+ * c1 = posterior_mean_coef1, c2 = posterior_mean_coef2, sigma (0 at t=0), log-SNR fed to the NEXT forward (sampling.py:151),
+ * 0, 0} (a DDIM table puts its c_x0, c_z, sigma in columns 2-4); pos_dev: device int32 loop position (the caller increments
+ * it after the call, in stream order).  z (n = B*S*S*3) is updated in place; the new z is also written to both halves of the next
  * forward's [cond ; uncond] input next_z2 (2n) and next_logsnr2 (batch2 = 2B entries).
  * Noise: noise != NULL: device (steps, n) floats, step k reads noise[k*n .. k*n+n).  noise == NULL: the device hash normal
  * of (*seed_dev - k), i.e. the caller stores seed(first step) and the per-step seeds count down like the timestep index;
@@ -309,7 +313,7 @@ int xunet_sampler_step_table(const float* eps2, float* z, const float* noise, lo
 /* The multistep form of xunet_sampler_step_table (same arguments, same contract) for second-order solvers such as
  * DPM-Solver++(2M): row k = *pos_dev of the table is {c_recip, c_recipm1, c_x0, c_z, sigma, log-SNR of the next forward,
  * c_prev, 0}, and x0_hist (device, n floats, required) carries the previous step's clipped x0 between calls:
- *     x0 = clip(c_recip z - c_recipm1 eps, -1, 1)  as above;
+ *     x0 = clip(c_recip z - c_recipm1 out, -1, 1)  as above;
  *     z' = fma(sigma, noise_k, fma(c_prev, x0_hist[i], fma(c_x0, x0, c_z * z)))   (fp32, one rounding per fma);
  *     x0_hist[i] = x0.
  * A row with c_prev == 0 skips the c_prev term and never reads x0_hist, so the first step of a chain needs no initialised
@@ -321,7 +325,7 @@ int xunet_sampler_step_multistep(const float* eps2, float* z, const float* noise
 /* The sampler step with DYNAMIC THRESHOLDING of x0 (Saharia et al. 2022, Imagen section 2.3) in place of the fixed clip:
  * the same table row, noise, next_z2 / next_logsnr2 writes and (x0_hist != NULL) multistep term as
  * xunet_sampler_step_table (x0_hist == NULL) and xunet_sampler_step_multistep (x0_hist != NULL), with
- *     x0 = c_recip z - c_recipm1 eps  (unclipped);  s_b = max(1, quantile_p(|x0|) over the per = n / batch values of view b);
+ *     x0 = c_recip z - c_recipm1 out  (unclipped, out the guided network output as above);  s_b = max(1, quantile_p(|x0|) over the per = n / batch values of view b);
  *     x0 <- clip(x0, -s_b, s_b) / s_b   (fp32 division, round to nearest),
  * and this x0 feeds the update and x0_hist.  quantile_p is numpy's np.quantile(a, p) (method 'linear') in fp64 on the fp32
  * values a = |x0| sorted ascending: idx = (per - 1) p, lo = floor(idx), hi = min(lo + 1, per - 1), g = idx - lo,
@@ -345,6 +349,15 @@ int xunet_sampler_step_dynamic(const float* eps2, float* z, const float* noise, 
 int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
                             const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
                             float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, void* stream);
+
+/* xunet_forward_diffusion for v-prediction (Salimans & Ho 2022): the same draws, z, logsnr, t and cond_mask, plus the v target
+ *   v = __fsub_rn(__fmul_rn(sqrt_ac[t], noise), __fmul_rn(sqrt_1mac[t], x0))      (each fp32 operation rounded once)
+ * stored to v_out (device, B * per floats, required) in the same pass.  noise_out may be NULL (the noise is then not stored).
+ * One launch. */
+int xunet_forward_diffusion_v(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
+                              const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
+                              float* v_out, float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per,
+                              void* stream);
 
 /* A set of SRN views held in device memory (srn_data.DeviceScenes): item i = view v of instance inst, items of one instance
  * contiguous, instance after instance.  All pointers are device memory.
@@ -386,6 +399,15 @@ typedef struct xunet_srn_store {
 int xunet_srn_batch(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
                     int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
                     const xunet_batch* out, float* noise, float* loss_weight, int* idx_out, int* t_out, void* stream);
+
+/* xunet_srn_batch for v-prediction: the same draws and outputs, plus v_out (device, B*S*S*3 floats, required) = the v target of
+ * the drawn target views, exactly as xunet_forward_diffusion_v computes it, stored in the same pass.  noise may be NULL (the
+ * noise is then not stored), so a training step passes its regression-target buffer as v_out.  Same errors (a NULL v_out
+ * in place of a NULL noise); one launch, graph-capturable. */
+int xunet_srn_batch_v(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
+                      int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
+                      const xunet_batch* out, float* noise, float* v_out, float* loss_weight, int* idx_out, int* t_out,
+                      void* stream);
 
 /* The dropout keep-mask the kernels use for residual-block `op_index` (0/1 floats, device), so tests can
  * hand the identical mask to the oracle (nn.Dropout, model/xunet.py:84). */

@@ -116,8 +116,12 @@ SYMBOLS = {
     'xunet_forward_diffusion': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p, C.c_void_p, C.c_float,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong,
                                           C.c_void_p]),
+    'xunet_forward_diffusion_v': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p, C.c_void_p,
+                                            C.c_float] + [C.c_void_p] * 6 + [C.c_int, C.c_longlong, C.c_void_p]),
     'xunet_srn_batch': (C.c_int, [C.POINTER(XunetSrnStore), C.c_void_p, C.c_ulonglong] + [C.c_int] * 5 +
                         [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 5),
+    'xunet_srn_batch_v': (C.c_int, [C.POINTER(XunetSrnStore), C.c_void_p, C.c_ulonglong] + [C.c_int] * 5 +
+                          [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 6),
     'xunet_dropout_mask': (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_ulonglong, C.c_float, C.c_void_p]),
     'xunet_image_metrics': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),

@@ -192,7 +192,7 @@ def _set_rng_state(rng: np.random.RandomState, d: dict):
 
 def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *, ema: Optional[dict] = None,
                      rng: Optional[list] = None, add_device_axis: bool = False, clip: bool = False,
-                     schedule: bool = False, skipped: Optional[int] = None) -> dict:
+                     schedule: bool = False, skipped: Optional[int] = None, prediction: Optional[str] = None) -> dict:
     """The nested dict flax.serialization.to_state_dict gives for a flax.training.train_state.TrainState with
     tx=optax.adam(lr), i.e. chain(scale_by_adam, scale(-lr)):
 
@@ -208,7 +208,8 @@ def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *,
 
     (the schedule's count equals Adam's: both advance once per update).  Plus 'ema_params' (a params-shaped tree) when an
     EMA is kept, 'rng': {'<rank>': rng_state_dict(..)} for the host cond_mask stream of every rank, and 'skipped_steps'
-    (int64, updates skipped for a non-finite gradient norm) when given.  The Flax / optax layouts are restated from memory
+    (int64, updates skipped for a non-finite gradient norm) and 'prediction' (the string 'eps' or 'v': what the network was
+    trained to predict) when given.  The Flax / optax layouts are restated from memory
     of their published sources and have not been checked against files written by the packages themselves.
     add_device_axis=True gives every Flax leaf (not 'rng' / 'skipped_steps') the leading pmap axis of length 1, as the
     reference's pmapped state carries it (train.py:161-167).  params / mu / nu / ema: nested dicts of numpy arrays
@@ -228,19 +229,22 @@ def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *,
         tree['rng'] = {str(r): d for r, d in enumerate(rng)}
     if skipped is not None:
         tree['skipped_steps'] = np.asarray(skipped, dtype=np.int64)
+    if prediction is not None:
+        tree['prediction'] = str(prediction)
     return tree
 
 
 def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     """Inverse of train_state_tree onto flat fp32 host buffers laid out by `spec`.  Returns {'step', 'count', 'params',
     'mu', 'nu', 'ema' (None if the file has none), 'rng' (list indexed by rank, or None), 'skipped' (0 if the file has
-    none)}.  Accepts all four optimizer layouts (with and without clipping, with and without a schedule), so a run may
+    none), 'prediction' ('eps' if the file has none: files written before v-prediction existed hold eps models)}.  Accepts all four optimizer layouts (with and without clipping, with and without a schedule), so a run may
     turn either on or off when it resumes; a schedule count that differs from Adam's raises ValueError.  Detects the pmap
     device axis from the shape of 'step' and takes replica 0.  Missing / unexpected leaves raise KeyError, wrong shapes
     ValueError."""
     tree = dict(tree)
     rng = tree.pop('rng', None)
     skipped = tree.pop('skipped_steps', None)
+    prediction = str(tree.pop('prediction', 'eps'))
     if np.ndim(tree['step']) == 1:
         tree = strip_device_axis(tree, 0)
     opt = tree['opt_state']
@@ -249,7 +253,8 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     adam, sched = opt['0'], opt['1']
     if 'count' in sched and int(sched['count']) != int(adam['count']):
         raise ValueError(f"schedule count {int(sched['count'])} differs from the Adam count {int(adam['count'])}")
-    out = {'step': int(tree['step']), 'count': int(adam['count']), 'skipped': 0 if skipped is None else int(skipped)}
+    out = {'step': int(tree['step']), 'count': int(adam['count']), 'skipped': 0 if skipped is None else int(skipped),
+           'prediction': prediction}
     for k, sub in (('params', tree['params']), ('mu', adam['mu']), ('nu', adam['nu']), ('ema', tree.get('ema_params'))):
         out[k] = None if sub is None else pack_flat(sub, spec, nparams)
     out['rng'] = None if rng is None else [rng[str(r)] for r in range(len(rng))]
@@ -259,7 +264,8 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
 def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', overwrite: bool = True,
                      add_device_axis: bool = False) -> str:
     """Writes the whole TrainState -- params, Adam mu / nu / count, step, ema_params when the state keeps an EMA, the count
-    of skipped updates when it clips or warms up, and the host cond_mask stream of every rank -- to f'{prefix}{step}' in ckpt_dir (layout: train_state_tree).  The file stays a
+    of skipped updates when it clips or warms up, the state's prediction ('eps' or 'v') and the host cond_mask stream of
+    every rank -- to f'{prefix}{step}' in ckpt_dir (layout: train_state_tree).  The file stays a
     valid params checkpoint: restore_checkpoint(ckpt_dir, prefix=prefix) returns its params tree.
 
     Under torch.distributed this is collective: every rank must call it; the cond_mask streams are gathered and rank 0
@@ -278,7 +284,8 @@ def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', ove
                                 ema=None if state.ema_params is None else host(state.ema_params.flat),
                                 rng=rngs, add_device_axis=add_device_axis, clip=state.tx.max_grad_norm is not None,
                                 schedule=state.tx.warmup_steps > 0,
-                                skipped=state.skipped_steps if state.clip is not None else None)
+                                skipped=state.skipped_steps if state.clip is not None else None,
+                                prediction=state.prediction)
         path = save_checkpoint(ckpt_dir, tree, step, prefix=prefix, overwrite=overwrite)
     xdist.barrier()
     return path
@@ -293,7 +300,9 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     on `state` stays valid; it re-derives its device step counter and dropout seed from the restored count.  A file without
     EMA restored into a state with one starts the EMA from the restored params; a file with an EMA restored into a state
     without one ignores it.  The clipping / warm-up settings are those of `state`, whatever the file was written with; the
-    skip counter is restored (0 if the file has none).  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
+    skip counter is restored (0 if the file has none).  A file whose prediction ('eps' when it records none) differs from
+    the state's raises ValueError before anything is written: a v model resumed as an eps one (or the reverse) would be
+    trained on the other target.  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
     freshly seeded streams are kept (with a warning), and a resume is then no longer bit-exact."""
     from . import dist as xdist
     path = ckpt_dir if os.path.isfile(ckpt_dir) else latest_checkpoint(ckpt_dir, prefix)
@@ -302,6 +311,9 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     with open(path, 'rb') as fh:
         tree = msgpack_restore(fh.read())
     r = parse_train_state_tree(tree, state.params.spec, state.params.flat.numel())
+    if r['prediction'] != state.prediction:
+        raise ValueError(f"{path}: the checkpoint holds a prediction={r['prediction']!r} model, the state trains "
+                         f"prediction={state.prediction!r}")
     state.params.flat.copy_(r['params'])
     state.opt_state.mu.copy_(r['mu'])
     state.opt_state.nu.copy_(r['nu'])

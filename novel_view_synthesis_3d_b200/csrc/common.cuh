@@ -141,6 +141,20 @@ __device__ __forceinline__ float xu_fd_cond_mask(uint64_t hb, float p_uncond) {
 }
 // z of one element: sqrt(abar_t) x0 + sqrt(1 - abar_t) noise
 __device__ __forceinline__ float xu_fd_z(float sa, float x0, float sb, float nz) { return sa * x0 + sb * nz; }
+// xu_fd_z with its rounding spelled out, for the v-target kernels, whose z must equal the eps kernels' bit for bit: nvcc
+// contracts the plain expression to fma(sa, x0, fl(sb noise)) in forward_diffusion_kernel and in the vector path of
+// srn_batch_kernel (xu_fd_z_rn), and to fma(sb, noise, fl(sa x0)) in its scalar path (xu_fd_z_rn_scalar)
+__device__ __forceinline__ float xu_fd_z_rn(float sa, float x0, float sb, float nz) { return __fmaf_rn(sa, x0, __fmul_rn(sb, nz)); }
+__device__ __forceinline__ float xu_fd_z_rn_scalar(float sa, float x0, float sb, float nz) {
+  return __fmaf_rn(sb, nz, __fmul_rn(sa, x0));
+}
+// v target of one element (Salimans & Ho 2022): sqrt(abar_t) noise - sqrt(1 - abar_t) x0, each product and the difference
+// rounded once (no contraction), so fp32 numpy restates it bit for bit (diffusion.v_target)
+__device__ __forceinline__ float xu_fd_v(float sa, float nz, float sb, float x0) {
+  return __fsub_rn(__fmul_rn(sa, nz), __fmul_rn(sb, x0));
+}
+// what a forward-diffusion producer writes as the regression target: the noise itself, or v in its place / beside it
+enum xu_target { XU_TARGET_EPS = 0, XU_TARGET_V = 1 };
 
 // one 64-bit hash serves the 4 consecutive elements idx4*4 .. idx4*4+3 (16-bit uniforms): bit j of the result = keep
 __host__ __device__ __forceinline__ uint32_t xu_keep4(uint64_t seed, int op_index, uint64_t idx4, float rate) {

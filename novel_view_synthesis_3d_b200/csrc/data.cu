@@ -1,9 +1,11 @@
-// data.cu -- one training micro-batch drawn from an SRN store in device memory, gathered and forward-diffused (xunet_srn_batch).
+// data.cu -- one training micro-batch drawn from an SRN store in device memory, gathered and forward-diffused (xunet_srn_batch,
+// and xunet_srn_batch_v for v-prediction).
 //
 // Grid (chunks, B): CTA (c, b) handles sample b.  Its thread 0 reads the step counter and derives the sample's draw -- source
 // item, target view, diffusion seed and timestep -- into shared memory; the CTA then streams its share of the S*S*3 values:
-// x from the source view, z and noise from the target view (the arithmetic of xunet_forward_diffusion, common.cuh), four
-// values per thread with 16-byte stores (4-byte loads from a uint8 store) when the layout allows.  CTA 0 of each sample also
+// x from the source view, z and noise (and v, xunet_srn_batch_v) from the target view (the arithmetic of
+// xunet_forward_diffusion, common.cuh), four values per thread with 16-byte stores (4-byte loads from a uint8 store) when
+// the layout allows.  CTA 0 of each sample also
 // writes the sample's poses, K, logsnr, cond_mask, loss weight and the optional idx / t outputs.  Every output element has one
 // writer and no value is reduced, so the result is deterministic and independent of the grid.
 //
@@ -62,14 +64,18 @@ template <int PIX> __device__ __forceinline__ float srn_load1(const void* px, lo
   return static_cast<const float*>(px)[off];
 }
 
-template <int PIX>
+// TARGET == XU_TARGET_V also stores v = xu_fd_v(..) to v_out (the last parameter, so the eps instances keep their parameter
+// layout and code), and `noise` may then be NULL.
+template <int PIX, int TARGET>
 __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store st, const long long* __restrict__ step_dev,
                                                                 unsigned long long seed, int j, int k, int rank, int world,
                                                                 const float* __restrict__ sqrt_ac,
                                                                 const float* __restrict__ sqrt_1mac, float p_uncond,
                                                                 const float* __restrict__ snr_weight, xunet_batch out,
                                                                 float* __restrict__ noise, float* __restrict__ loss_weight,
-                                                                int* __restrict__ idx_out, int* __restrict__ t_out, int vec) {
+                                                                int* __restrict__ idx_out, int* __restrict__ t_out, int vec,
+                                                                float* __restrict__ v_out) {
+  constexpr bool V = TARGET == XU_TARGET_V;
   __shared__ long long s_src, s_tgt;
   __shared__ unsigned long long s_seed, s_hb;
   __shared__ int s_inst, s_v, s_v2, s_t;
@@ -113,20 +119,44 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
       nz.y = xu_hash_normal(s, (uint64_t)(ob + i + 1));
       nz.z = xu_hash_normal(s, (uint64_t)(ob + i + 2));
       nz.w = xu_hash_normal(s, (uint64_t)(ob + i + 3));
-      zz.x = xu_fd_z(sa, xt.x, sb, nz.x);
-      zz.y = xu_fd_z(sa, xt.y, sb, nz.y);
-      zz.z = xu_fd_z(sa, xt.z, sb, nz.z);
-      zz.w = xu_fd_z(sa, xt.w, sb, nz.w);
+      if constexpr (V) {
+        zz.x = xu_fd_z_rn(sa, xt.x, sb, nz.x);
+        zz.y = xu_fd_z_rn(sa, xt.y, sb, nz.y);
+        zz.z = xu_fd_z_rn(sa, xt.z, sb, nz.z);
+        zz.w = xu_fd_z_rn(sa, xt.w, sb, nz.w);
+      } else {
+        zz.x = xu_fd_z(sa, xt.x, sb, nz.x);
+        zz.y = xu_fd_z(sa, xt.y, sb, nz.y);
+        zz.z = xu_fd_z(sa, xt.z, sb, nz.z);
+        zz.w = xu_fd_z(sa, xt.w, sb, nz.w);
+      }
       *reinterpret_cast<float4*>(x + ob + i) = xs;
       *reinterpret_cast<float4*>(z + ob + i) = zz;
-      *reinterpret_cast<float4*>(noise + ob + i) = nz;
+      if constexpr (V) {
+        float4 vv;
+        vv.x = xu_fd_v(sa, nz.x, sb, xt.x);
+        vv.y = xu_fd_v(sa, nz.y, sb, xt.y);
+        vv.z = xu_fd_v(sa, nz.z, sb, xt.z);
+        vv.w = xu_fd_v(sa, nz.w, sb, xt.w);
+        *reinterpret_cast<float4*>(v_out + ob + i) = vv;
+        if (noise != nullptr) *reinterpret_cast<float4*>(noise + ob + i) = nz;
+      } else {
+        *reinterpret_cast<float4*>(noise + ob + i) = nz;
+      }
     }
   } else {
     for (long long i = (long long)blockIdx.x * SRN_THREADS + threadIdx.x; i < per; i += stride) {
       const float nz = xu_hash_normal(s, (uint64_t)(ob + i));
       x[ob + i] = srn_load1<PIX>(st.pixels, src + i);
-      z[ob + i] = xu_fd_z(sa, srn_load1<PIX>(st.pixels, tgt + i), sb, nz);
-      noise[ob + i] = nz;
+      if constexpr (V) {
+        const float xt = srn_load1<PIX>(st.pixels, tgt + i);
+        z[ob + i] = xu_fd_z_rn_scalar(sa, xt, sb, nz);
+        v_out[ob + i] = xu_fd_v(sa, nz, sb, xt);
+        if (noise != nullptr) noise[ob + i] = nz;
+      } else {
+        z[ob + i] = xu_fd_z(sa, srn_load1<PIX>(st.pixels, tgt + i), sb, nz);
+        noise[ob + i] = nz;
+      }
     }
   }
   if (blockIdx.x == 0) {
@@ -154,19 +184,33 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
 
 static bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
 
-void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
-                      int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
-                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, cudaStream_t s) {
+template <int TARGET>
+static void launch_srn_batch_target(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k,
+                                    int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
+                                    const float* snr_weight, const xunet_batch& out, float* noise, float* loss_weight,
+                                    int* idx_out, int* t_out, float* v_out, cudaStream_t s) {
   const long long per = 3LL * st.S * st.S;
   const size_t px_align = st.pixel_kind == XUNET_PIXELS_U8 ? 4 : 16;
   const int vec = per % 4 == 0 && ((uintptr_t)st.pixels % px_align) == 0 && aligned16(out.x) && aligned16(out.z) &&
-                  aligned16(noise);
+                  aligned16(noise) && aligned16(v_out);
   const long long work = vec ? per / 4 : per;
   const dim3 grid((unsigned)cdiv(work, SRN_THREADS), (unsigned)B);
   if (st.pixel_kind == XUNET_PIXELS_U8)
-    xu_launch(srn_batch_kernel<XUNET_PIXELS_U8>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world, sqrt_ac,
-              sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec);
+    xu_launch(srn_batch_kernel<XUNET_PIXELS_U8, TARGET>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world,
+              sqrt_ac, sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec, v_out);
   else
-    xu_launch(srn_batch_kernel<XUNET_PIXELS_F32>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world, sqrt_ac,
-              sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec);
+    xu_launch(srn_batch_kernel<XUNET_PIXELS_F32, TARGET>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world,
+              sqrt_ac, sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec, v_out);
+}
+
+void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
+                      int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
+                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, float* v_out,
+                      cudaStream_t s) {
+  if (v_out != nullptr)
+    launch_srn_batch_target<XU_TARGET_V>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight,
+                                         out, noise, loss_weight, idx_out, t_out, v_out, s);
+  else
+    launch_srn_batch_target<XU_TARGET_EPS>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond,
+                                           snr_weight, out, noise, loss_weight, idx_out, t_out, v_out, s);
 }

@@ -28,7 +28,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 109; }
+extern "C" int xunet_version(void) { return 110; }
 
 namespace {
 
@@ -1496,31 +1496,62 @@ extern "C" int xunet_forward_diffusion(const float* x0, const float* noise_in, c
                                        float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, void* stream) {
   if (!x0 || !sqrt_ac || !sqrt_1mac || !z || !logsnr_out || B < 1 || per < 1) return fail("xunet_forward_diffusion: bad argument");
   launch_forward_diffusion(x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac, p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B,
-                           per, (cudaStream_t)stream);
+                           per, nullptr, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("forward_diffusion: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_forward_diffusion_v(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
+                                         const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z,
+                                         float* noise_out, float* v_out, float* logsnr_out, int* t_out, float* cond_mask_out,
+                                         int B, long long per, void* stream) {
+  if (!x0 || !sqrt_ac || !sqrt_1mac || !z || !v_out || !logsnr_out) return fail("xunet_forward_diffusion_v: NULL pointer argument");
+  if (B < 1 || per < 1) return fail("xunet_forward_diffusion_v: B = %d, per = %lld, need both >= 1", B, per);
+  launch_forward_diffusion(x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac, p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B,
+                           per, v_out, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("forward_diffusion_v: CUDA error: %s", cudaGetErrorString(e));
+}
+
+// the argument checks of xunet_srn_batch / _v; the ε buffer `noise` is checked by the caller (optional in the v form)
+static int srn_batch_check(const char* fn, const xunet_srn_store* store, const long long* step_dev, int j, int k, int rank,
+                           int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const xunet_batch* out) {
+  if (!store || !step_dev || !sqrt_ac || !sqrt_1mac || !out || !store->pixels || !store->R || !store->t || !store->K ||
+      !store->first || !store->count || !store->item_inst || !out->x || !out->z || !out->logsnr || !out->R1 || !out->t1 ||
+      !out->R2 || !out->t2 || !out->K || !out->cond_mask)
+    return fail("%s: NULL pointer argument", fn);
+  if (B < 1 || k < 1 || world < 1) return fail("%s: B = %d, k = %d, world = %d, need all >= 1", fn, B, k, world);
+  if (rank < 0 || rank >= world || j < 0 || j >= k)
+    return fail("%s: rank = %d of world = %d, j = %d of k = %d out of range", fn, rank, world, j, k);
+  if (store->n_items < 1 || store->n_instances < 1 || store->S < 1)
+    return fail("%s: empty store (n_items = %lld, n_instances = %d, S = %d)", fn, store->n_items, store->n_instances, store->S);
+  if (store->pixel_kind != XUNET_PIXELS_U8 && store->pixel_kind != XUNET_PIXELS_F32)
+    return fail("%s: unknown pixel_kind %d", fn, store->pixel_kind);
+  return 0;
 }
 
 extern "C" int xunet_srn_batch(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
                                int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
                                const float* snr_weight, const xunet_batch* out, float* noise, float* loss_weight, int* idx_out,
                                int* t_out, void* stream) {
-  if (!store || !step_dev || !sqrt_ac || !sqrt_1mac || !out || !noise || !store->pixels || !store->R || !store->t || !store->K ||
-      !store->first || !store->count || !store->item_inst || !out->x || !out->z || !out->logsnr || !out->R1 || !out->t1 ||
-      !out->R2 || !out->t2 || !out->K || !out->cond_mask)
-    return fail("xunet_srn_batch: NULL pointer argument");
-  if (B < 1 || k < 1 || world < 1) return fail("xunet_srn_batch: B = %d, k = %d, world = %d, need all >= 1", B, k, world);
-  if (rank < 0 || rank >= world || j < 0 || j >= k)
-    return fail("xunet_srn_batch: rank = %d of world = %d, j = %d of k = %d out of range", rank, world, j, k);
-  if (store->n_items < 1 || store->n_instances < 1 || store->S < 1)
-    return fail("xunet_srn_batch: empty store (n_items = %lld, n_instances = %d, S = %d)", store->n_items, store->n_instances,
-                store->S);
-  if (store->pixel_kind != XUNET_PIXELS_U8 && store->pixel_kind != XUNET_PIXELS_F32)
-    return fail("xunet_srn_batch: unknown pixel_kind %d", store->pixel_kind);
+  if (!noise) return fail("xunet_srn_batch: NULL pointer argument");
+  if (const int rc = srn_batch_check("xunet_srn_batch", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out)) return rc;
   launch_srn_batch(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight, *out, noise,
-                   loss_weight, idx_out, t_out, (cudaStream_t)stream);
+                   loss_weight, idx_out, t_out, nullptr, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("srn_batch: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_srn_batch_v(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
+                                 int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
+                                 const float* snr_weight, const xunet_batch* out, float* noise, float* v_out,
+                                 float* loss_weight, int* idx_out, int* t_out, void* stream) {
+  if (!v_out) return fail("xunet_srn_batch_v: NULL pointer argument");
+  if (const int rc = srn_batch_check("xunet_srn_batch_v", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out)) return rc;
+  launch_srn_batch(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight, *out, noise,
+                   loss_weight, idx_out, t_out, v_out, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("srn_batch_v: CUDA error: %s", cudaGetErrorString(e));
 }
 
 extern "C" int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,

@@ -154,13 +154,17 @@ void launch_sampler_step_table(const float* eps2, float* z, const float* noise, 
 void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                  const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
                                  int B2, float* x0_hist, int B, double p, float* scale_out, cudaStream_t s);
+// v_out != nullptr: the v-target instance (xunet_forward_diffusion_v), which also stores v and takes noise_out == nullptr
 void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
                               const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
-                              float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, cudaStream_t s);
-// xunet_srn_batch (data.cu): one micro-batch drawn from a device SRN store, gathered and forward-diffused; grid (chunks, B)
+                              float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, float* v_out,
+                              cudaStream_t s);
+// xunet_srn_batch (data.cu): one micro-batch drawn from a device SRN store, gathered and forward-diffused; grid (chunks, B).
+// v_out != nullptr: the v-target instance (xunet_srn_batch_v), which also stores v and takes noise == nullptr
 void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
                       int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
-                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, cudaStream_t s);
+                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, float* v_out,
+                      cudaStream_t s);
 void launch_dropout_mask(float* out, long long n, int op_index, unsigned long long seed, float rate, cudaStream_t s);
 // xunet_image_metrics: one CTA per image, fp64 moments and sums in a fixed order (metrics.cu); 11 <= S <= XUNET_METRICS_MAX_SIDE
 struct MetricsWindow { double w[11]; };   // the normalised 1-D Gaussian weights of the SSIM window

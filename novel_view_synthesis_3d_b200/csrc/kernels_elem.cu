@@ -1766,13 +1766,16 @@ void launch_sampler_step_table(const float* eps2, float* z, const float* noise, 
               B2, x0_hist);
 }
 
-// dataset/data_loader.py:92-110 on the device
+// dataset/data_loader.py:92-110 on the device.  TARGET == XU_TARGET_V also stores v = xu_fd_v(..) to v_out (the last
+// parameter, so the eps instance keeps its parameter layout and code).
+template <int TARGET>
 __global__ void __launch_bounds__(256) forward_diffusion_kernel(const float* __restrict__ x0, const float* __restrict__ noise_in,
                                                                 const int* __restrict__ t_in, unsigned long long seed,
                                                                 const float* __restrict__ sqrt_ac, const float* __restrict__ sqrt_1mac,
                                                                 float p_uncond, float* __restrict__ z, float* __restrict__ noise_out,
                                                                 float* __restrict__ logsnr_out, int* __restrict__ t_out,
-                                                                float* __restrict__ cond_mask_out, int B, long long per) {
+                                                                float* __restrict__ cond_mask_out, int B, long long per,
+                                                                float* __restrict__ v_out) {
   xu_grid_dep_sync();
   const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
   if (idx >= (long long)B * per) return;
@@ -1780,7 +1783,13 @@ __global__ void __launch_bounds__(256) forward_diffusion_kernel(const float* __r
   const uint64_t hb = xu_fd_sample_hash(seed, b);
   const int t = t_in != nullptr ? t_in[b] : xu_fd_timestep(hb);
   const float nz = noise_in != nullptr ? noise_in[idx] : xu_hash_normal(seed, (uint64_t)idx);
-  z[idx] = xu_fd_z(sqrt_ac[t], x0[idx], sqrt_1mac[t], nz);
+  if constexpr (TARGET == XU_TARGET_V) {
+    const float sa = sqrt_ac[t], sb = sqrt_1mac[t], x = x0[idx];
+    z[idx] = xu_fd_z_rn(sa, x, sb, nz);
+    v_out[idx] = xu_fd_v(sa, nz, sb, x);
+  } else {
+    z[idx] = xu_fd_z(sqrt_ac[t], x0[idx], sqrt_1mac[t], nz);
+  }
   if (noise_out != nullptr) noise_out[idx] = nz;
   if (idx == (long long)b * per) {
     logsnr_out[b] = xu_fd_logsnr(t);
@@ -1790,10 +1799,15 @@ __global__ void __launch_bounds__(256) forward_diffusion_kernel(const float* __r
 }
 void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
                               const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
-                              float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, cudaStream_t s) {
+                              float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, float* v_out,
+                              cudaStream_t s) {
   const long long n = (long long)B * per;
-  xu_launch(forward_diffusion_kernel, cdiv(n, 256), 256, 0, s, x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac, p_uncond, z, noise_out,
-                                                        logsnr_out, t_out, cond_mask_out, B, per);
+  if (v_out != nullptr)
+    xu_launch(forward_diffusion_kernel<XU_TARGET_V>, cdiv(n, 256), 256, 0, s, x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac,
+              p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B, per, v_out);
+  else
+    xu_launch(forward_diffusion_kernel<XU_TARGET_EPS>, cdiv(n, 256), 256, 0, s, x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac,
+              p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B, per, v_out);
 }
 
 __global__ void dropout_mask_kernel(float* __restrict__ out, long long n, int op_index, unsigned long long seed, float rate) {

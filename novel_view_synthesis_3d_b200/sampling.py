@@ -9,6 +9,10 @@ Two samplers that need only tens of steps run through the same device-table step
 deterministic, eta = 1 the DDPM posterior) and DPM-Solver++(2M) (Lu et al. 2022), a second-order multistep solver in x0
 that keeps the previous step's clipped x0 on the device.  Both feed the network the log-SNR of the timestep z is at.
 Any of the three can replace the fixed clip of x0 with per-view dynamic thresholding (Imagen, Saharia et al. 2022).
+
+Every sampler reads the network output as eps by default.  prediction='v' reads it as v = sqrt(abar) eps - sqrt(1 - abar) x0
+(Salimans & Ho 2022): only the first two table columns change, since every step computes x0 = c_recip z - c_recipm1 out and
+the guidance (1 + w) out_c - w out_u is linear in the output.
 """
 from __future__ import annotations
 
@@ -40,6 +44,14 @@ def logsnr_schedule_cosine(t, *, logsnr_min=-20., logsnr_max=20.):
 
 METHODS = ('ddpm', 'ddim', 'dpmpp_2m')
 SPACINGS = ('linear', 'logsnr')
+PREDICTIONS = ('eps', 'v')
+
+
+def check_prediction(prediction) -> str:
+    """Validates what the network predicts: 'eps' (the noise) or 'v' (sqrt(abar) eps - sqrt(1 - abar) x0)."""
+    if prediction not in PREDICTIONS:
+        raise ValueError(f'prediction must be one of {PREDICTIONS}, got {prediction!r}')
+    return prediction
 
 
 class Schedule:
@@ -102,11 +114,15 @@ def _check_dynamic_threshold(p) -> None:
         raise ValueError(f'dynamic_threshold {p} outside (0, 1]')
 
 
-def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, logsnr_lag: bool = True):
+def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, logsnr_lag: bool = True,
+                  prediction: str = 'eps'):
     """The device table of `sched` for `method`: (rows, logsnr_first), rows (len(sched), 8) float64 (the sampler rounds
     them to fp32 once), row k = loop position k = timestep index len-1-k = {c_recip, c_recipm1, c_x0, c_z, sigma,
     logsnr_next, c_prev, 0}; logsnr_first is the log-SNR of the first forward.  A step is
-        x0 = clip(c_recip z - c_recipm1 eps, -1, 1);  z' = c_x0 x0 + c_z z + c_prev x0_prev + sigma noise.
+        x0 = clip(c_recip z - c_recipm1 out, -1, 1);  z' = c_x0 x0 + c_z z + c_prev x0_prev + sigma noise,
+    out the (guided) network output: with prediction='eps' c_recip = sqrt(1/abar), c_recipm1 = sqrt(1/abar - 1); with
+    prediction='v' c_recip = sqrt(abar), c_recipm1 = sqrt(1 - abar) (x0 = alpha z - sigma_t v).  The other columns do not
+    depend on the prediction.
     With abar the row's alpha-bar, abar' the next row's (1 after the last step), alpha = sqrt(abar),
     sigma_t = sqrt(1 - abar) and lambda = log(alpha / sigma_t):
       ddpm      the posterior of sampling.py:133-151 (reads the schedule's posterior tables), c_prev = 0;
@@ -120,6 +136,7 @@ def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, lo
     the log-SNR of its own timestep t_k.  logsnr_lag=False: each forward gets the log-SNR of the timestep z is at,
     logsnr_cosine(t_0/1000) first and logsnr_cosine(t_{k+1}/1000) from row k (the last row's value is unused)."""
     _check_method(method, eta)
+    check_prediction(prediction)
     sc = sched
     n = len(sc.timesteps)
     i = np.arange(n - 1, -1, -1)
@@ -152,6 +169,9 @@ def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, lo
                 second = (np.arange(n) > 0) & (np.arange(n) < n - 1)
                 c_x0 = np.where(second, g * (1. + 1. / (2. * r)), g)
                 c_prev = np.where(second, -g / (2. * r), 0.0)
+    if prediction == 'v':
+        a = np.asarray(sc.alphas_cumprod, dtype=np.float64)[:n][i]
+        c_recip, c_recipm1 = np.sqrt(a), np.sqrt(1. - a)
     t = np.asarray(sc.timesteps)[i] / 1000.0
     if logsnr_lag:
         logsnr_first, logsnr_next = -20.0, logsnr_schedule_cosine(t)
@@ -170,7 +190,13 @@ class Sampler:
     (DPM-Solver++(2M); its step is `xunet_sampler_step_multistep`, with the previous step's x0 in a device buffer).
     spacing: the Schedule's timestep spacing, 'logsnr' for dpmpp_2m and 'linear' otherwise by default; len(self.sched)
     is the number of forwards a sample runs.  logsnr_lag: the reference's one-step lag of the network's log-SNR input,
-    on by default for ddpm only (see `sampler_table`).  With every default this is the reference sampler.
+    on by default for ddpm with prediction='eps' only (see `sampler_table`).  With every default this is the reference
+    sampler.
+
+    prediction: 'eps' (default) reads the network output as the noise; 'v' reads it as v = sqrt(abar) eps - sqrt(1 - abar) x0,
+    for a model trained with create_train_state(prediction='v').  Only the table's x0 columns change (`sampler_table`), so
+    every method, dynamic thresholding and sample_views run the same kernels.  The lag defaults to off for v: it is a quirk
+    of the reference's eps-trained checkpoints.
 
     dynamic_threshold: None clips x0 to [-1, 1] (the reference).  A percentile p in (0, 1] thresholds x0 per view instead
     (Saharia et al. 2022, Imagen section 2.3): s = max(1, p-quantile of |x0| over the view), x0 <- clip(x0, -s, s) / s, for
@@ -179,12 +205,13 @@ class Sampler:
 
     def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000, w: float = 3.0,
                  use_graph: bool = True, method: str = 'ddpm', eta: float = 0.0, spacing: str | None = None,
-                 logsnr_lag: bool | None = None, dynamic_threshold: float | None = None):
+                 logsnr_lag: bool | None = None, dynamic_threshold: float | None = None, prediction: str = 'eps'):
         _check_method(method, eta)
         _check_dynamic_threshold(dynamic_threshold)
+        self.prediction = check_prediction(prediction)
         self.dynamic_threshold = None if dynamic_threshold is None else float(dynamic_threshold)
         self.method, self.eta = method, float(eta)
-        self.logsnr_lag = method == 'ddpm' if logsnr_lag is None else bool(logsnr_lag)
+        self.logsnr_lag = (method == 'ddpm' and prediction == 'eps') if logsnr_lag is None else bool(logsnr_lag)
         self.model, self.B, self.S, self.w = model, batch_size, img_sidelength, float(w)
         self.sched = Schedule(steps, spacing=('logsnr' if method == 'dpmpp_2m' else 'linear') if spacing is None else spacing)
         self.eng = model.engine(2 * batch_size, img_sidelength, False)
@@ -228,7 +255,8 @@ class Sampler:
     def _load_schedule(self) -> int:
         """Writes the coefficient table of `self.sched` (callers may have edited it since the last call) to the device and
         returns its number of steps.  Row k = loop position k = timestep index len-1-k (`sampler_table`)."""
-        rows, self._logsnr_first = sampler_table(self.sched, self.method, eta=self.eta, logsnr_lag=self.logsnr_lag)
+        rows, self._logsnr_first = sampler_table(self.sched, self.method, eta=self.eta, logsnr_lag=self.logsnr_lag,
+                                                 prediction=self.prediction)
         if self._tab is None or len(self._tab) != len(rows):
             # the captured graphs hold the table and noise pointers: reallocate (and recapture) only when the length changes
             self._tab = torch.empty(len(rows), 8, dtype=torch.float32, device=self.dev)

@@ -19,8 +19,8 @@ import torch
 
 from . import _lib
 from . import dist as xdist
-from .diffusion import min_snr_weights
-from .sampling import cosine_beta_schedule
+from .diffusion import diffusion_tables, min_snr_weights
+from .sampling import check_prediction
 from .xunet import XUNet, ParamTree, Engine, InputSlots, check_loss
 
 
@@ -86,6 +86,9 @@ class TrainState:
     # training objective: 'frobenius' (the reference's ||eps_hat - noise||_F, train.py:67) or 'mse' (the mean squared error
     # of DDPM's L_simple, optionally weighted per sample); not part of the checkpoint
     loss: str = 'frobenius'
+    # what the network is trained to predict: 'eps' (the noise) or 'v' (sqrt(abar) eps - sqrt(1 - abar) x0); recorded in
+    # the checkpoint
+    prediction: str = 'eps'
     _mask_rng: np.random.RandomState = None
     _frozen_mask: Optional[np.ndarray] = None
 
@@ -162,7 +165,7 @@ def create_sample_data(batch_size, img_sidelength):
 def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_sidelength, *, model: XUNet = None,
                        zero_init: bool = True, reference_quirks: bool = False, init_on_device: bool = False,
                        ema_decay: Optional[float] = None, max_grad_norm: Optional[float] = None,
-                       warmup_steps: int = 0, loss: str = 'frobenius') -> TrainState:
+                       warmup_steps: int = 0, loss: str = 'frobenius', prediction: str = 'eps') -> TrainState:
     """train.py:36-47.  Under torch.distributed the parameters of rank 0 are broadcast (the reference gives every
     device a different init, train.py:122-123 -- an ensemble, not data parallelism).
 
@@ -182,8 +185,18 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
     loss: 'frobenius' (default) trains on the reference's ||eps_hat - noise||_F over the whole micro-batch.  'mse' trains on
     the mean squared error (1/B) sum_b w_b * mean_i (eps_hat - noise)_bi^2 of DDPM and 3DiM, whose per-sample weights w_b
     (all 1 unless a loss_weight is passed, e.g. from ForwardDiffusion(min_snr_gamma=..)) make per-sample weighting possible.
-    With it, gradient accumulation and data parallelism give the gradient of the mean over the whole global batch."""
+    With it, gradient accumulation and data parallelism give the gradient of the mean over the whole global batch.
+
+    prediction: 'eps' (default) trains the network to predict the noise.  'v' trains it to predict
+    v = sqrt(abar_t) eps - sqrt(1 - abar_t) x0 (Salimans & Ho 2022), from which x0 = sqrt(abar_t) z - sqrt(1 - abar_t) v
+    loses at most the error of v (an eps error reaches x0 multiplied by sqrt(1/abar_t - 1), about 6e4 at t = 999).  It
+    needs loss='mse'.  A TrainStep(data=..) then draws v targets on the device; the host-input calls (apply_model,
+    TrainStep(batch, target)) take the v target (diffusion.v_target) where an eps state takes the noise.  Sample the
+    result with Sampler(prediction='v')."""
     check_loss(loss)
+    check_prediction(prediction)
+    if prediction == 'v' and loss != 'mse':
+        raise ValueError(f"prediction='v' needs loss='mse', got loss={loss!r}")
     if ema_decay is not None and not (0.0 <= ema_decay <= 1.0):
         raise ValueError(f'ema_decay must lie in [0, 1], got {ema_decay}')
     if max_grad_norm is not None and not (float(max_grad_norm) > 0.0 and np.isfinite(float(max_grad_norm))):
@@ -211,6 +224,7 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
                       reference_quirks=reference_quirks, ema_params=ema,
                       ema_decay=None if ema_decay is None else float(ema_decay),
                       clip=ClipState.zeros(params.flat.device) if opt.clip_or_warmup else None, loss=loss,
+                      prediction=prediction,
                       _mask_rng=np.random.RandomState(mask_seed & 0x7FFFFFFF))
 
 
@@ -280,7 +294,9 @@ def _cond_mask(state: TrainState, B: int) -> np.ndarray:
 def apply_model(state: TrainState, batch_x, batch_z, batch_logsnr, batch_R1, batch_t1, batch_R2, batch_t2, batch_K,
                 batch_noise, *, cond_mask=None, loss_weight=None):
     """train.py:49-72: forward with train=True, the state's loss (||eps_hat - noise||_F by default), gradients w.r.t. all
-    parameters.  loss_weight: per-sample weights (B,) of loss='mse', host or device (all 1 when None).
+    parameters.  batch_noise is the regression target: the noise of z for a state built with prediction='eps', the v target
+    (diffusion.v_target of the clean target view, that noise and the timestep) for prediction='v'.  loss_weight: per-sample
+    weights (B,) of loss='mse', host or device (all 1 when None).
     Returns (loss: 0-d device tensor, grads: ParamTree view of the flat gradient bucket).  With
     torch.distributed initialised the gradient bucket is all-reduced (sum) here; update_model applies 1/world."""
     B, S = int(batch_x.shape[0]), int(batch_x.shape[1])
@@ -344,6 +360,8 @@ class TrainStep:
     every view once as the source, in a keyed random order that changes every such epoch.  Epochs are not aligned with
     updates: an update may take its first draws from one epoch and the rest from the next (nothing is dropped).  Since the
     order follows the Adam count, restore_train_state + the same store and data_seed continue the data stream exactly.
+    For a state built with prediction='v' the same kernel (xunet_srn_batch_v) writes the v target of each draw where an
+    eps state gets its noise, and min_snr_gamma gives the v weights; nothing else in the step changes.
     """
 
     def __init__(self, state: TrainState, *, use_graph: bool = True, bucket_mb: float = 128.0, allreduce: bool = True,
@@ -399,11 +417,11 @@ class TrainStep:
                 raise ValueError(f'the store lives on {data.device}, the state trains on {self.dev}')
             self.data_seed = int(data_seed) & 0xFFFFFFFFFFFFFFFF
             self.p_uncond = float(p_uncond)
-            ac = np.cumprod(1. - cosine_beta_schedule(1000), axis=0)
-            self.sqrt_ac = torch.as_tensor(np.sqrt(ac), dtype=torch.float32).to(self.dev)
-            self.sqrt_1mac = torch.as_tensor(np.sqrt(1. - ac), dtype=torch.float32).to(self.dev)
+            sqrt_ac, sqrt_1mac = diffusion_tables()
+            self.sqrt_ac = torch.as_tensor(sqrt_ac).to(self.dev)
+            self.sqrt_1mac = torch.as_tensor(sqrt_1mac).to(self.dev)
             self.snr_weight = None if min_snr_gamma is None else \
-                torch.as_tensor(min_snr_weights(min_snr_gamma), dtype=torch.float32).to(self.dev)
+                torch.as_tensor(min_snr_weights(min_snr_gamma, prediction=state.prediction), dtype=torch.float32).to(self.dev)
             self.h2d_bytes = 0
 
     @property
@@ -427,16 +445,19 @@ class TrainStep:
             self._synced_count = s.opt_state.count
 
     def _draw(self, j: int):
-        """Micro-batch j of the current update, drawn from the device store into input slot j (xunet_srn_batch)."""
+        """Micro-batch j of the current update, drawn from the device store into input slot j (xunet_srn_batch, or
+        xunet_srn_batch_v with the v target in the slot's noise segment)."""
         d, inp = self.data, self.inputs.inp[j]
         ptr = lambda t: None if t is None else t.data_ptr()
         st = torch.cuda.current_stream(self.dev).cuda_stream
-        _lib.check(self.lib.xunet_srn_batch(C.byref(d.c_store), self.step_dev.data_ptr(), self.data_seed, j, self.k,
-                                            xdist.rank(), self.world, self.eng.B, self.sqrt_ac.data_ptr(),
-                                            self.sqrt_1mac.data_ptr(), self.p_uncond, ptr(self.snr_weight),
-                                            C.byref(self.inputs.cbatch[j]), inp['noise'].data_ptr(),
-                                            inp['loss_weight'].data_ptr() if self.mse else None, None, None, st),
-                   'xunet_srn_batch')
+        head = (C.byref(d.c_store), self.step_dev.data_ptr(), self.data_seed, j, self.k, xdist.rank(), self.world, self.eng.B,
+                self.sqrt_ac.data_ptr(), self.sqrt_1mac.data_ptr(), self.p_uncond, ptr(self.snr_weight),
+                C.byref(self.inputs.cbatch[j]))
+        tail = (inp['loss_weight'].data_ptr() if self.mse else None, None, None, st)
+        if self.state.prediction == 'v':
+            _lib.check(self.lib.xunet_srn_batch_v(*head, None, inp['noise'].data_ptr(), *tail), 'xunet_srn_batch_v')
+        else:
+            _lib.check(self.lib.xunet_srn_batch(*head, inp['noise'].data_ptr(), *tail), 'xunet_srn_batch')
 
     def _fwd_bwd(self):
         e, s = self.eng, self.state
@@ -525,7 +546,8 @@ class TrainStep:
 
     def __call__(self, batch: Optional[dict] = None, noise=None, cond_mask=None, loss_weight=None) -> torch.Tensor:
         """One optimisation step on host (or device) inputs; returns the loss as a 0-d device tensor (a view of the step's
-        loss slot: read or copy it before the next step).  With grad_accum_steps=k every array has k*B rows, and the loss
+        loss slot: read or copy it before the next step).  `noise` is the regression target: the noise for a state built
+        with prediction='eps', the v target (diffusion.v_target) for prediction='v'.  With grad_accum_steps=k every array has k*B rows, and the loss
         is the mean of the k micro-batch losses.  loss_weight: per-sample weights of a loss='mse' state (all 1 when None).
         A step built with data= draws its own batches and takes no arguments."""
         s = self.state
