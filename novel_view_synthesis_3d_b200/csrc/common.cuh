@@ -193,15 +193,25 @@ __device__ __forceinline__ void xu_ray_dir(const float* ki, const float* R, int 
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-// SM count of the current device (132 on an H100 SXM), queried once; grids of persistent / wave-sized kernels derive from it
-static inline int xu_num_sms() {
+// SM count of the current device (132 on an H100 SXM), queried once
+static inline int xu_device_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0, v = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) n = v;
     else n = 132;
-    // data parallel: NCCL's reduction CTAs need SMs of their own while the persistent one-CTA-per-SM kernels run; with
-    // XUNET_SM_RESERVE=k the persistent / wave-sized grids leave k SMs free (a persistent grid that does not fit runs a second wave)
+  }
+  return n;
+}
+// SMs the persistent / wave-sized grids may fill.  Data parallel: NCCL's reduction CTAs need SMs of their own while the
+// persistent one-CTA-per-SM kernels run; with XUNET_SM_RESERVE=k those grids leave k SMs free (a persistent grid that does not
+// fit runs a second wave).  How a reduction is split into fp32 partial sums never follows the reserve to longer sums: the
+// split-K and pixels-per-block choices take xu_device_sms(), or at least its split, so each CTA or thread sums no more terms
+// than on the whole device, which the fp64 launch checks bound.
+static inline int xu_num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    n = xu_device_sms();
     const char* e = getenv("XUNET_SM_RESERVE");
     if (e && atoi(e) > 0 && atoi(e) < n) n -= atoi(e);
   }

@@ -275,7 +275,7 @@ static void wgrad_dispatch(const WgradArgs& a, cudaStream_t s) {
   const int taps = a.ks * a.ks;
   if (a.Ci >= 48 && a.Co >= 48) {
     int tiles = cdiv(a.Ci, 64) * cdiv(a.Co, 64);
-    long long ks = (4 * xu_num_sms() + (long long)tiles * taps - 1) / ((long long)tiles * taps);
+    long long ks = (4 * xu_device_sms() + (long long)tiles * taps - 1) / ((long long)tiles * taps);
     if (ks < 1) ks = 1;
     if (ks > chunks) ks = chunks;
     if (ks > 65535) ks = 65535;
@@ -283,7 +283,7 @@ static void wgrad_dispatch(const WgradArgs& a, cudaStream_t s) {
     xu_launch(wgrad_simt_kernel<T, 64, 64, 4, 4>, grid, 256, 0, s, a);
   } else {
     int tiles = cdiv(a.Ci, 32) * cdiv(a.Co, 32);
-    long long ks = (4 * xu_num_sms() + (long long)tiles * taps - 1) / ((long long)tiles * taps);
+    long long ks = (4 * xu_device_sms() + (long long)tiles * taps - 1) / ((long long)tiles * taps);
     if (ks < 1) ks = 1;
     if (ks > chunks) ks = chunks;
     if (ks > 65535) ks = 65535;
@@ -961,7 +961,7 @@ static void small_dispatch(ConvKernel k, const ConvArgs* c, const WgradArgs* w, 
     if (is_pow2(Cw) && Cw >= 2 && Cw <= 512 && w->Wo % SEG == 0 && w->Hi == w->Ho && w->Wi == w->Wo) {
       const int nstream = 256 / (Cw / 2);
       const long long units = (long long)w->N * w->Ho * (w->Wo / SEG);
-      const int grid = (int)std::min<long long>(cdiv(units, nstream), (long long)xu_num_sms() * 2);
+      const int grid = (int)std::min<long long>(cdiv(units, nstream), (long long)xu_device_sms() * 2);   // the split of the sum
       const size_t sm = sizeof(float) * 256 * 56;
       const auto kernel = cin3 ? wgrad_thin_kernel<T, 0> : wgrad_thin_kernel<T, 1>;
       cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);

@@ -126,7 +126,7 @@ static void gn_grid(int C, int P, int B, dim3& grid, int& ppb) {
   int PL = 256 / TPB;
   ppb = PL * 8;
   // enough blocks to cover the memory latency (reductions are latency-bound), but not absurdly many atomics
-  while ((long long)cdiv(P, ppb) * B > xu_num_sms() * 8 && ppb < P) ppb *= 2;
+  while ((long long)cdiv(P, ppb) * B > xu_device_sms() * 8 && ppb < P) ppb *= 2;
   grid = dim3(cdiv(P, ppb), B);
 }
 
@@ -331,7 +331,7 @@ static void gn_apply_grid(int C, int P, int B, dim3& grid, int& ppb) {
   int PL = 256 / TPB;
   ppb = PL * 16;   // the per-thread prologue (statistics -> scale/shift) is ~200 instructions: amortise it over >= 8 pixels
   // down to 4 pixels per thread (measured: 4 beats 8 and 2; latency-bound: more blocks in flight)
-  while (ppb > PL * 4 && (long long)cdiv(P, ppb) * B < xu_num_sms() * 4) ppb /= 2;
+  while (ppb > PL * 4 && (long long)cdiv(P, ppb) * B < xu_device_sms() * 4) ppb /= 2;
   grid = dim3(cdiv(P, ppb), B);
 }
 
@@ -434,7 +434,7 @@ static void gn_vec_grid(int C, int VW, int P, int B, dim3& grid, int& ppb) {
   const int TPB = CV < 256 ? CV : 256;
   const int PL = 256 / TPB;
   ppb = PL * 32;                    // several batches of U pixels per thread when the tensor is large
-  while (ppb > PL * 4 && (long long)cdiv(P, ppb) * B < xu_num_sms() * 4) ppb /= 2;
+  while (ppb > PL * 4 && (long long)cdiv(P, ppb) * B < xu_device_sms() * 4) ppb /= 2;
   grid = dim3(cdiv(P, ppb), B);
 }
 

@@ -233,18 +233,22 @@ void launch_wgrad_tc(const WgradArgs& a, cudaStream_t s) {
   p.stages = stages;
   // split-K factor: one CTA per SM (the ring takes all of shared memory), so the launch runs in ceil(tiles*k / SMs) waves of
   // ceil(ptiles / k) pixel tiles each.  Rounding k UP to cover the SMs can cost a whole second wave for a handful of CTAs, so
-  // minimise waves x tiles-per-CTA instead (ties -> fewer splits: every split adds M*N fp32 reds).
-  int ksplit = 1;
-  {
-    const long long T = (long long)tiles_m * tiles_n, sms = xu_num_sms();
+  // minimise waves x tiles-per-CTA instead (ties -> fewer splits: every split adds M*N fp32 reds).  With SMs reserved
+  // (XUNET_SM_RESERVE) the rule alone would pick fewer, longer splits, up to all the pixels in one CTA, whose fp32 sums in the
+  // tensor cores' truncating accumulator err past what the whole device's splits do; so k is never below the whole device's.
+  const long long T = (long long)tiles_m * tiles_n;
+  auto pick_split = [&](long long sms, int kmin) {
+    int k_best = kmin;
     long long best = -1;
     const int kmax = p.ptiles < 64 ? p.ptiles : 64;
-    for (int k = 1; k <= kmax; ++k) {
+    for (int k = kmin; k <= (kmax > kmin ? kmax : kmin); ++k) {
       const long long waves = (T * k + sms - 1) / sms, per = (p.ptiles + k - 1) / k;
       const long long cost = waves * (per + 8);        // +8: per-CTA pipeline fill + reds, in pixel-tile units
-      if (best < 0 || cost < best) { best = cost; ksplit = k; }
+      if (best < 0 || cost < best) { best = cost; k_best = k; }
     }
-  }
+    return k_best;
+  };
+  const int ksplit = pick_split(xu_num_sms(), pick_split(xu_device_sms(), 1));
   CUtensorMap tx, ty;
   uint64_t xd[4] = {(uint64_t)a.Ci, (uint64_t)a.Wi, (uint64_t)a.Hi, (uint64_t)a.N};
   uint64_t xs[3] = {(uint64_t)a.Ci * 2, (uint64_t)a.Wi * a.Ci * 2, (uint64_t)a.Hi * a.Wi * a.Ci * 2};

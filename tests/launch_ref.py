@@ -95,9 +95,11 @@ def acc_floor(K):
     sqrt(K) 2^-24 sum|terms|.  2^-16 at K = 2304 (9 taps x 256 channels), i.e. 5.3 sqrt(K) 2^-24, keeps a 5x margin over it
     for every K: 2^-14.5 at K = 9 x 2048, the widest reduction of the full model, 2^-19.6 at K = 16, a head_dim-16 score.
     Where the terms share a sign (inputs with offsets) the tensor cores' accumulator, which truncates, errs by up to about
-    (K / 16) 2^-24 sum|terms| (one rounding per 16-product wgmma step) instead: within this floor for sums of up to ~2^15
-    terms per CTA.  The closest call an H100 measured on the benchmarked plans, err / bound 0.93, is such a case: the weight
-    gradient of a strided pose-embedding conv, 32768 pixels summed by few CTAs."""
+    (K / 16) 2^-24 sum|terms| (one rounding per 16-product wgmma step) instead, which reaches this floor near K = 2^13 terms
+    per CTA: same-signed inputs summed 2^14 pixels per CTA measured 1.5 x over it.  The weight-gradient kernels never split a
+    sum into longer runs than on the whole device (wgrad_tc's split-K factor, common.cuh xu_num_sms), whose per-CTA runs stay
+    within it on the benchmarked plans.  The closest call an H100 measured there, err / bound 0.93, is the weight gradient of
+    a strided pose-embedding conv."""
     return 2. ** -16 * math.sqrt(K / 2304.)
 
 

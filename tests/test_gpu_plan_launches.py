@@ -191,10 +191,11 @@ def test_attention_launch(lib, case, peaked):
 # ======================================================================================================================
 # which tensor-core variants the plan-derived launches reach, read from the launchers' log in a child process
 # ======================================================================================================================
-def _launch_all_convs():
-    """every launch test_conv_launch checks, once more on zero-filled buffers and unchecked: what the variants test logs"""
+def _launch_all_convs(cases=None):
+    """every launch test_conv_launch checks (or those of `cases`), once more on zero-filled buffers and unchecked: what the
+    variants tests log"""
     lib = _lib.load()
-    for name, dtype, training, r in CONVS:
+    for name, dtype, training, r in (CONVS if cases is None else cases):
         N, Hi, Wi, Ci, Ho, Wo, Co = (r[k] for k in ('N', 'Hi', 'Wi', 'Ci', 'Ho', 'Wo', 'Co'))
         ks, st, nseg = r['ksize'], r['stride'], r['nseg']
         z = lambda *shape, dt=DT[dtype]: torch.zeros(*shape, dtype=dt, device='cuda')
