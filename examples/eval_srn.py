@@ -9,6 +9,7 @@ instance is conditioned on one source view (view 64 by default) and every scored
         --dynamic-threshold 0.995 --out eval_dpm_dyn/
     python examples/eval_srn.py cars_test --ckpt checkpoints_v --prefix ema --side 128 --prediction v --method dpmpp_2m \\
         --steps 25 --out eval_v/
+    python examples/eval_srn.py cars_test --ckpt checkpoints_d6 --prefix ema --side 128 --steps 256 --distilled 6 --out eval_d6/
 
 Modes:
   independent  each target is sampled from the source alone (Sampler.sample, the reference's k = 1 sampler); the targets
@@ -17,7 +18,8 @@ Modes:
                in order, each step conditioned on a random view of the pool (the source and the targets generated so far);
                instances are batched --views-in-flight at a time.
 Writes out/metrics.jsonl (one {instance, view, psnr, ssim} line per scored view) and out/summary.json (mean PSNR, mean SSIM,
-the number of views, the prediction the checkpoint was read with and the arguments), prints the summary as the last line of stdout, and with --save-views writes each
+the number of views, the prediction the checkpoint was read with, the distillation round --distilled, the forwards per
+view and the arguments), prints the summary as the last line of stdout, and with --save-views writes each
 generated view as out/views/<instance>_<view>.png.  Seeds derive from --seed, so equal arguments give equal files.
 """
 import argparse
@@ -63,6 +65,10 @@ def main():
                     help='threshold x0 per view at the P-quantile of |x0| (Imagen: 0.995) instead of clipping it to [-1, 1]')
     ap.add_argument('--prediction', choices=P.sampling.PREDICTIONS, default='eps',
                     help='what the checkpoint predicts: the noise (eps) or v (a model trained with --prediction v)')
+    ap.add_argument('--distilled', type=int, default=0, metavar='R',
+                    help='sample a student distilled R times (examples/distill_srn.py) from a --steps-step teacher: DDIM '
+                         '(eta 0) on distill_grid(--steps, R) without guidance, reading v; --method, --eta, --spacing, --w '
+                         'and --prediction are then ignored')
     ap.add_argument('--source-view', type=int, default=64, help='conditioning view of every instance (pixelNeRF / 3DiM: 64)')
     ap.add_argument('--targets', type=int, default=0, help='target views per instance, spaced evenly; 0 = all other views')
     ap.add_argument('--max-instances', type=int, default=-1, help='score the first N instances of the sorted list')
@@ -85,8 +91,12 @@ def main():
             raise SystemExit(f"instance {ds.instances[i]['name']} has {n} views; --source-view {a.source_view} does not exist")
         insts.append((i, select_targets(n, a.source_view, a.targets)))
     B = a.views_in_flight
-    sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing,
-                        dynamic_threshold=a.dynamic_threshold, prediction=a.prediction)
+    if a.distilled:
+        sampler = P.Sampler(P.XUNet(), params, B, a.side, w=None, method='ddim', prediction='v',
+                            timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold)
+    else:
+        sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta,
+                            spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction)
     os.makedirs(a.out, exist_ok=True)
     if a.save_views:
         os.makedirs(os.path.join(a.out, 'views'), exist_ok=True)
@@ -139,7 +149,8 @@ def main():
             fh.write(json.dumps(rec) + '\n')
     summary = dict(mean_psnr=float(np.mean([r['psnr'] for r in records])) if records else float('nan'),
                    mean_ssim=float(np.mean([r['ssim'] for r in records])) if records else float('nan'),
-                   n_views=len(records), prediction=a.prediction, args=vars(a))
+                   n_views=len(records), prediction='v' if a.distilled else a.prediction, distilled=a.distilled,
+                   sampler_steps=len(sampler.sched), args=vars(a))
     with open(os.path.join(a.out, 'summary.json'), 'w') as fh:
         json.dump(summary, fh, indent=1)
     print(json.dumps(summary))

@@ -5,6 +5,7 @@ ancestral sampler, write PNGs (the reference blocks in cv2.imshow, which cannot 
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --prefix ema --steps 256 --out results_ema/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --method dpmpp_2m --steps 25 --out results_dpm/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_v --prediction v --method dpmpp_2m --steps 25 --out results_v/
+    python examples/sample_srn.py cars_train_val --ckpt checkpoints_d1 --prefix ema --distilled 1 --steps 256 --out results_d1/
 """
 import argparse
 import os
@@ -33,6 +34,10 @@ def main():
                     help='threshold x0 per view at the P-quantile of |x0| (Imagen: 0.995) instead of clipping it to [-1, 1]')
     ap.add_argument('--prediction', choices=P.sampling.PREDICTIONS, default='eps',
                     help='what the checkpoint predicts: the noise (eps) or v (a model trained with --prediction v)')
+    ap.add_argument('--distilled', type=int, default=0, metavar='R',
+                    help='sample a student distilled R times (examples/distill_srn.py) from a --steps-step teacher: DDIM '
+                         '(eta 0) on distill_grid(--steps, R) without guidance, reading v; --method, --eta, --spacing, --w '
+                         'and --prediction are then ignored')
     ap.add_argument('--views', type=int, default=1)
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--out', default='results')
@@ -46,8 +51,12 @@ def main():
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50)
     batch = next(ds.batches(a.views))
     model = P.XUNet()
-    sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta, spacing=a.spacing,
-                        dynamic_threshold=a.dynamic_threshold, prediction=a.prediction)
+    if a.distilled:
+        sampler = P.Sampler(model, params, a.views, a.side, w=None, method='ddim', prediction='v',
+                            timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold)
+    else:
+        sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta,
+                            spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction)
     os.makedirs(a.out, exist_ok=True)
     if a.orbit > 0:
         it = ds.batches(a.views)

@@ -341,6 +341,20 @@ int xunet_sampler_step_dynamic(const float* eps2, float* z, const float* noise, 
                                double percentile, float* scale_out, float* next_z2, float* next_logsnr2, int batch2,
                                void* stream);
 
+/* The UNGUIDED sampler step, for a model whose guidance is in its weights (a distilled student): one B-batch conditional
+ * forward per step instead of the [cond ; uncond] 2B batch.  out (device, n = B*S*S*3 floats) is that forward's output, used
+ * as is in place of the guided (1+w) out_c - w out_u; everything else is the guided step's:
+ *   percentile == 0, x0_hist == NULL: xunet_sampler_step_table;   percentile == 0, x0_hist != NULL: xunet_sampler_step_multistep;
+ *   percentile in (0, 1]: xunet_sampler_step_dynamic (x0_hist NULL or set as there), scale_out optional as there.
+ * The new z goes to z and to next_z (n floats: the next forward's z input), and the row's log-SNR to next_logsnr (batch
+ * floats).  Each instance is the guided kernel with the guidance expression replaced by out, so the result equals the
+ * guided step run at w = 0 with out in both halves, bit for bit (but for the sign of an exactly zero output).
+ * Errors: a NULL required pointer, n <= 0, batch < 1, n % batch != 0; with percentile != 0 also per > XUNET_SAMPLER_DYN_MAX_PER
+ * or percentile NaN or outside (0, 1].  One launch; graph-capturable. */
+int xunet_sampler_step_cond(const float* out, float* z, const float* noise, long long n, const float* table, const int* pos_dev,
+                            const unsigned long long* seed_dev, float* x0_hist, int batch, double percentile, float* scale_out,
+                            float* next_z, float* next_logsnr, void* stream);
+
 /* Device-side forward diffusion = the per-item work of SceneInstanceDataset.__getitem__ (dataset/data_loader.py:92-110):
  *   t ~ U{0..999};  noise ~ N(0,1);  z = sqrt_ac[t] * x0 + sqrt_1mac[t] * noise;  logsnr = logsnr_schedule_cosine(t/1000);
  *   cond_mask = (u > p_uncond)  (train.py:64).
@@ -408,6 +422,41 @@ int xunet_srn_batch_v(const xunet_srn_store* store, const long long* step_dev, u
                       int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
                       const xunet_batch* out, float* noise, float* v_out, float* loss_weight, int* idx_out, int* t_out,
                       void* stream);
+
+/* xunet_srn_batch for PROGRESSIVE DISTILLATION (Salimans & Ho 2022): the same draws (pairs, poses, K, diffusion seed, noise,
+ * z, logsnr of the drawn timestep; z bit for bit as xunet_srn_batch) except
+ *   m_b = (the sample hash that xunet_srn_batch draws t from) mod n_grid,   t_b = grid_t[m_b]     (grid_t: device int32, n_grid
+ *   entries, the student's timesteps in loop order);   out->cond_mask[b] = 1;   no regression target is stored;
+ * and in the same pass the sample's x, z, logsnr, R1, t1, R2, t2, K go to teacher row c*B + b for c < teacher_copies (2: a
+ * guided teacher's [cond ; uncond] batch, whose cond_mask the caller sets once; 1: an unguided teacher), m_b to m_out (device,
+ * B int32), and idx_out / t_out as in xunet_srn_batch when given.  teacher->cond_mask and ->rays are ignored.  Errors: those of
+ * xunet_srn_batch, a NULL grid_t / teacher / m_out / teacher row pointer, n_grid < 1, teacher_copies not 1 or 2.  One launch;
+ * no atomics, no allocation, graph-capturable. */
+int xunet_srn_batch_distill(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
+                            int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const int* grid_t,
+                            int n_grid, const xunet_batch* out, const xunet_batch* teacher, int teacher_copies, int* m_out,
+                            int* idx_out, int* t_out, void* stream);
+
+/* The teacher's first DDIM step of a distillation sample.  teacher_table: device (2N, 8) floats, the teacher's DDIM (eta = 0)
+ * sampler table on its 2N-step grid with log-SNR lag off (sampling.sampler_table); m_dev: device (B) int32 from
+ * xunet_srn_batch_distill.  Element i of sample b (per = S*S*3 values each, n = B*per) applies row r = 2 m_b exactly as
+ * xunet_sampler_step_table at pos = r does (fp32, as nvcc contracts it, sigma = 0):
+ *   out = (1+w) out_c - w out_u (teacher_copies = 2: out_t = [out_c ; out_u], 2n floats) or out_c (teacher_copies = 1, w unused);
+ *   x0 = clip(c_recip z - c_recipm1 out, -1, 1);   z' = c_x0 x0 + c_z z,
+ * reading z from teacher->z and writing z' to every copy of it, and row r's column 5 (the log-SNR of the next teacher timestep)
+ * to every copy of teacher->logsnr.  Errors: a NULL pointer, B < 1, per < 1, teacher_copies not 1 or 2.  One launch. */
+int xunet_distill_teacher_step(const float* out_t, float w, int teacher_copies, const float* teacher_table, const int* m_dev,
+                               int B, long long per, const xunet_batch* teacher, void* stream);
+
+/* The distillation target: the teacher's second step, row r = 2 m_b + 1, from its second output out_t and teacher_z (z' of
+ * xunet_distill_teacher_step, first copy), to z'' as above; then, with target_table (device (N, 4) floats) row m_b =
+ * {c_a, c_b, alpha_t, sigma_t}, c_a = 1 / (alpha'' - (sigma''/sigma_t) alpha_t), c_b = (sigma''/sigma_t) c_a (fp64, rounded once):
+ *   x~ = __fsub_rn(__fmul_rn(c_a, z''), __fmul_rn(c_b, z_t));   v = __fdiv_rn(__fsub_rn(__fmul_rn(alpha_t, z_t), x~), sigma_t)
+ * stored to v_out (device, n floats: the student slot's regression target).  z_t: the student's z input.  A student DDIM step
+ * from z_t whose v output is v lands on z''.  Errors: a NULL pointer, B < 1, per < 1, teacher_copies not 1 or 2.  One launch. */
+int xunet_distill_target(const float* out_t, float w, int teacher_copies, const float* teacher_table, const float* target_table,
+                         const int* m_dev, const float* z_t, const float* teacher_z, int B, long long per, float* v_out,
+                         void* stream);
 
 /* The dropout keep-mask the kernels use for residual-block `op_index` (0/1 floats, device), so tests can
  * hand the identical mask to the oracle (nn.Dropout, model/xunet.py:84). */

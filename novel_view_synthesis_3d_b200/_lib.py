@@ -122,6 +122,15 @@ SYMBOLS = {
                         [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 5),
     'xunet_srn_batch_v': (C.c_int, [C.POINTER(XunetSrnStore), C.c_void_p, C.c_ulonglong] + [C.c_int] * 5 +
                           [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.POINTER(XunetBatch)] + [C.c_void_p] * 6),
+    'xunet_srn_batch_distill': (C.c_int, [C.POINTER(XunetSrnStore), C.c_void_p, C.c_ulonglong] + [C.c_int] * 5 +
+                                [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(XunetBatch), C.POINTER(XunetBatch),
+                                 C.c_int] + [C.c_void_p] * 4),
+    'xunet_distill_teacher_step': (C.c_int, [C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong,
+                                             C.POINTER(XunetBatch), C.c_void_p]),
+    'xunet_distill_target': (C.c_int, [C.c_void_p, C.c_float, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_longlong,
+                                                                                             C.c_void_p, C.c_void_p]),
+    'xunet_sampler_step_cond': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong] + [C.c_void_p] * 4 +
+                                [C.c_int, C.c_double] + [C.c_void_p] * 4),
     'xunet_dropout_mask': (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_ulonglong, C.c_float, C.c_void_p]),
     'xunet_image_metrics': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),

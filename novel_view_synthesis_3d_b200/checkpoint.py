@@ -192,7 +192,8 @@ def _set_rng_state(rng: np.random.RandomState, d: dict):
 
 def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *, ema: Optional[dict] = None,
                      rng: Optional[list] = None, add_device_axis: bool = False, clip: bool = False,
-                     schedule: bool = False, skipped: Optional[int] = None, prediction: Optional[str] = None) -> dict:
+                     schedule: bool = False, skipped: Optional[int] = None, prediction: Optional[str] = None,
+                     distill: Optional[dict] = None) -> dict:
     """The nested dict flax.serialization.to_state_dict gives for a flax.training.train_state.TrainState with
     tx=optax.adam(lr), i.e. chain(scale_by_adam, scale(-lr)):
 
@@ -209,7 +210,8 @@ def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *,
     (the schedule's count equals Adam's: both advance once per update).  Plus 'ema_params' (a params-shaped tree) when an
     EMA is kept, 'rng': {'<rank>': rng_state_dict(..)} for the host cond_mask stream of every rank, and 'skipped_steps'
     (int64, updates skipped for a non-finite gradient norm) and 'prediction' (the string 'eps' or 'v': what the network was
-    trained to predict) when given.  The Flax / optax layouts are restated from memory
+    trained to predict) when given, and 'distill' ({'teacher_steps', 'rounds'[, 'w']}, a progressively distilled student's
+    record) when given.  The Flax / optax layouts are restated from memory
     of their published sources and have not been checked against files written by the packages themselves.
     add_device_axis=True gives every Flax leaf (not 'rng' / 'skipped_steps') the leading pmap axis of length 1, as the
     reference's pmapped state carries it (train.py:161-167).  params / mu / nu / ema: nested dicts of numpy arrays
@@ -231,13 +233,16 @@ def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *,
         tree['skipped_steps'] = np.asarray(skipped, dtype=np.int64)
     if prediction is not None:
         tree['prediction'] = str(prediction)
+    if distill is not None:
+        tree['distill'] = {k: (float(v) if k == 'w' else int(v)) for k, v in distill.items()}
     return tree
 
 
 def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     """Inverse of train_state_tree onto flat fp32 host buffers laid out by `spec`.  Returns {'step', 'count', 'params',
     'mu', 'nu', 'ema' (None if the file has none), 'rng' (list indexed by rank, or None), 'skipped' (0 if the file has
-    none), 'prediction' ('eps' if the file has none: files written before v-prediction existed hold eps models)}.  Accepts all four optimizer layouts (with and without clipping, with and without a schedule), so a run may
+    none), 'prediction' ('eps' if the file has none: files written before v-prediction existed hold eps models), 'distill'
+    (None if the file has none: a model that is not a distilled student)}.  Accepts all four optimizer layouts (with and without clipping, with and without a schedule), so a run may
     turn either on or off when it resumes; a schedule count that differs from Adam's raises ValueError.  Detects the pmap
     device axis from the shape of 'step' and takes replica 0.  Missing / unexpected leaves raise KeyError, wrong shapes
     ValueError."""
@@ -245,6 +250,9 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     rng = tree.pop('rng', None)
     skipped = tree.pop('skipped_steps', None)
     prediction = str(tree.pop('prediction', 'eps'))
+    distill = tree.pop('distill', None)
+    if distill is not None:
+        distill = {k: (float(v) if k == 'w' else int(v)) for k, v in distill.items()}
     if np.ndim(tree['step']) == 1:
         tree = strip_device_axis(tree, 0)
     opt = tree['opt_state']
@@ -254,7 +262,7 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     if 'count' in sched and int(sched['count']) != int(adam['count']):
         raise ValueError(f"schedule count {int(sched['count'])} differs from the Adam count {int(adam['count'])}")
     out = {'step': int(tree['step']), 'count': int(adam['count']), 'skipped': 0 if skipped is None else int(skipped),
-           'prediction': prediction}
+           'prediction': prediction, 'distill': distill}
     for k, sub in (('params', tree['params']), ('mu', adam['mu']), ('nu', adam['nu']), ('ema', tree.get('ema_params'))):
         out[k] = None if sub is None else pack_flat(sub, spec, nparams)
     out['rng'] = None if rng is None else [rng[str(r)] for r in range(len(rng))]
@@ -264,7 +272,8 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
 def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', overwrite: bool = True,
                      add_device_axis: bool = False) -> str:
     """Writes the whole TrainState -- params, Adam mu / nu / count, step, ema_params when the state keeps an EMA, the count
-    of skipped updates when it clips or warms up, the state's prediction ('eps' or 'v') and the host cond_mask stream of
+    of skipped updates when it clips or warms up, the state's prediction ('eps' or 'v'), a distilled student's record
+    (state.distill) and the host cond_mask stream of
     every rank -- to f'{prefix}{step}' in ckpt_dir (layout: train_state_tree).  The file stays a
     valid params checkpoint: restore_checkpoint(ckpt_dir, prefix=prefix) returns its params tree.
 
@@ -285,7 +294,7 @@ def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', ove
                                 rng=rngs, add_device_axis=add_device_axis, clip=state.tx.max_grad_norm is not None,
                                 schedule=state.tx.warmup_steps > 0,
                                 skipped=state.skipped_steps if state.clip is not None else None,
-                                prediction=state.prediction)
+                                prediction=state.prediction, distill=state.distill)
         path = save_checkpoint(ckpt_dir, tree, step, prefix=prefix, overwrite=overwrite)
     xdist.barrier()
     return path
@@ -302,7 +311,8 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     without one ignores it.  The clipping / warm-up settings are those of `state`, whatever the file was written with; the
     skip counter is restored (0 if the file has none).  A file whose prediction ('eps' when it records none) differs from
     the state's raises ValueError before anything is written: a v model resumed as an eps one (or the reverse) would be
-    trained on the other target.  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
+    trained on the other target.  Likewise a file whose distillation record (None when it has none) differs from the state's:
+    a student resumed for another teacher grid, round or guidance would be trained on other targets.  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
     freshly seeded streams are kept (with a warning), and a resume is then no longer bit-exact."""
     from . import dist as xdist
     path = ckpt_dir if os.path.isfile(ckpt_dir) else latest_checkpoint(ckpt_dir, prefix)
@@ -314,6 +324,9 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     if r['prediction'] != state.prediction:
         raise ValueError(f"{path}: the checkpoint holds a prediction={r['prediction']!r} model, the state trains "
                          f"prediction={state.prediction!r}")
+    if r['distill'] != state.distill:
+        raise ValueError(f"{path}: the checkpoint holds a model with distillation record {r['distill']}, the state trains "
+                         f"one with {state.distill}")
     state.params.flat.copy_(r['params'])
     state.opt_state.mu.copy_(r['mu'])
     state.opt_state.nu.copy_(r['nu'])

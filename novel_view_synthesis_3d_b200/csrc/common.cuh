@@ -153,8 +153,23 @@ __device__ __forceinline__ float xu_fd_z_rn_scalar(float sa, float x0, float sb,
 __device__ __forceinline__ float xu_fd_v(float sa, float nz, float sb, float x0) {
   return __fsub_rn(__fmul_rn(sa, nz), __fmul_rn(sb, x0));
 }
-// what a forward-diffusion producer writes as the regression target: the noise itself, or v in its place / beside it
-enum xu_target { XU_TARGET_EPS = 0, XU_TARGET_V = 1 };
+// what a forward-diffusion producer writes as the regression target: the noise itself, or v in its place / beside it.
+// XU_TARGET_DISTILL writes no target: the timestep comes from a distillation grid and the target is made later from the
+// teacher's two steps (distill.cu)
+enum xu_target { XU_TARGET_EPS = 0, XU_TARGET_V = 1, XU_TARGET_DISTILL = 2 };
+
+// ---- one element of the fixed-clip table step (sampler_step_table_kernel, and the teacher steps of distill.cu) ----------
+// The plain expressions, as nvcc contracts them: out = fma(1 + w, out_c, -(w out_u)) for a guided step (out_c alone for an
+// unguided one), x0 = clip(fma(c_recip, z, -(c_recipm1 out)), -1, 1), and z' = fma(sigma, noise, fma(c_x0, x0, c_z z)).
+// tab is the step's table row {c_recip, c_recipm1, c_x0, c_z, sigma, ...}.
+__device__ __forceinline__ float xu_step_guided(float w, float oc, float ou) { return (1.f + w) * oc - w * ou; }
+__device__ __forceinline__ float xu_step_x0(const float* tab, float zi, float e) {
+  const float x0 = tab[0] * zi - tab[1] * e;
+  return fminf(fmaxf(x0, -1.f), 1.f);
+}
+__device__ __forceinline__ float xu_step_z(const float* tab, float x0, float zi, float nz) {
+  return tab[2] * x0 + tab[3] * zi + tab[4] * nz;
+}
 
 // one 64-bit hash serves the 4 consecutive elements idx4*4 .. idx4*4+3 (16-bit uniforms): bit j of the result = keep
 __host__ __device__ __forceinline__ uint32_t xu_keep4(uint64_t seed, int op_index, uint64_t idx4, float rate) {

@@ -1,5 +1,5 @@
 // data.cu -- one training micro-batch drawn from an SRN store in device memory, gathered and forward-diffused (xunet_srn_batch,
-// and xunet_srn_batch_v for v-prediction).
+// xunet_srn_batch_v for v-prediction, and xunet_srn_batch_distill for progressive distillation).
 //
 // Grid (chunks, B): CTA (c, b) handles sample b.  Its thread 0 reads the step counter and derives the sample's draw -- source
 // item, target view, diffusion seed and timestep -- into shared memory; the CTA then streams its share of the S*S*3 values:
@@ -8,6 +8,10 @@
 // the layout allows.  CTA 0 of each sample also
 // writes the sample's poses, K, logsnr, cond_mask, loss weight and the optional idx / t outputs.  Every output element has one
 // writer and no value is reduced, so the result is deterministic and independent of the grid.
+//
+// The distillation instance (TARGET == XU_TARGET_DISTILL) draws the same pairs, seeds and noise, but the timestep of sample b
+// is grid_t[m_b] with m_b = (sample hash) mod n_grid, cond_mask is 1, no target is stored, and the same x, poses, K, z and
+// logsnr also go to each of the teacher's `copies` row blocks (copy c of sample b = teacher row c B + b), with m_b to m_out.
 //
 // The draw functions below are restated in numpy by srn_data.draw_indices / diffusion_seed: change both together.
 #include "xunet_b200.h"
@@ -65,7 +69,8 @@ template <int PIX> __device__ __forceinline__ float srn_load1(const void* px, lo
 }
 
 // TARGET == XU_TARGET_V also stores v = xu_fd_v(..) to v_out (the last parameter, so the eps instances keep their parameter
-// layout and code), and `noise` may then be NULL.
+// layout and code), and `noise` may then be NULL.  TARGET == XU_TARGET_DISTILL reads `dd` (the last parameter) and takes
+// noise == v_out == NULL.
 template <int PIX, int TARGET>
 __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store st, const long long* __restrict__ step_dev,
                                                                 unsigned long long seed, int j, int k, int rank, int world,
@@ -74,11 +79,11 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
                                                                 const float* __restrict__ snr_weight, xunet_batch out,
                                                                 float* __restrict__ noise, float* __restrict__ loss_weight,
                                                                 int* __restrict__ idx_out, int* __restrict__ t_out, int vec,
-                                                                float* __restrict__ v_out) {
-  constexpr bool V = TARGET == XU_TARGET_V;
+                                                                float* __restrict__ v_out, XuDistillDraw dd) {
+  constexpr bool V = TARGET == XU_TARGET_V, D = TARGET == XU_TARGET_DISTILL;
   __shared__ long long s_src, s_tgt;
   __shared__ unsigned long long s_seed, s_hb;
-  __shared__ int s_inst, s_v, s_v2, s_t;
+  __shared__ int s_inst, s_v, s_v2, s_t, s_m;
   xu_grid_dep_sync();
   const int b = blockIdx.y, B = gridDim.y;
   if (threadIdx.x == 0) {
@@ -98,7 +103,12 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
     s_v2 = v2;
     s_seed = s;
     s_hb = hb;
-    s_t = xu_fd_timestep(hb);
+    if constexpr (D) {
+      s_m = (int)(hb % (uint64_t)dd.n_grid);
+      s_t = dd.grid_t[s_m];
+    } else {
+      s_t = xu_fd_timestep(hb);
+    }
   }
   __syncthreads();
   const long long per = 3LL * st.S * st.S;
@@ -119,7 +129,7 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
       nz.y = xu_hash_normal(s, (uint64_t)(ob + i + 1));
       nz.z = xu_hash_normal(s, (uint64_t)(ob + i + 2));
       nz.w = xu_hash_normal(s, (uint64_t)(ob + i + 3));
-      if constexpr (V) {
+      if constexpr (V || D) {
         zz.x = xu_fd_z_rn(sa, xt.x, sb, nz.x);
         zz.y = xu_fd_z_rn(sa, xt.y, sb, nz.y);
         zz.z = xu_fd_z_rn(sa, xt.z, sb, nz.z);
@@ -140,6 +150,12 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
         vv.w = xu_fd_v(sa, nz.w, sb, xt.w);
         *reinterpret_cast<float4*>(v_out + ob + i) = vv;
         if (noise != nullptr) *reinterpret_cast<float4*>(noise + ob + i) = nz;
+      } else if constexpr (D) {
+        for (int c = 0; c < dd.copies; ++c) {
+          const long long tb = (long long)c * B * per + ob + i;
+          *reinterpret_cast<float4*>(const_cast<float*>(dd.teacher.x) + tb) = xs;
+          *reinterpret_cast<float4*>(const_cast<float*>(dd.teacher.z) + tb) = zz;
+        }
       } else {
         *reinterpret_cast<float4*>(noise + ob + i) = nz;
       }
@@ -153,6 +169,15 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
         z[ob + i] = xu_fd_z_rn_scalar(sa, xt, sb, nz);
         v_out[ob + i] = xu_fd_v(sa, nz, sb, xt);
         if (noise != nullptr) noise[ob + i] = nz;
+      } else if constexpr (D) {
+        const float xt = srn_load1<PIX>(st.pixels, tgt + i), zi = xu_fd_z_rn_scalar(sa, xt, sb, nz);
+        const float xi = srn_load1<PIX>(st.pixels, src + i);
+        z[ob + i] = zi;
+        for (int c = 0; c < dd.copies; ++c) {
+          const long long tb = (long long)c * B * per + ob + i;
+          const_cast<float*>(dd.teacher.x)[tb] = xi;
+          const_cast<float*>(dd.teacher.z)[tb] = zi;
+        }
       } else {
         z[ob + i] = xu_fd_z(sa, srn_load1<PIX>(st.pixels, tgt + i), sb, nz);
         noise[ob + i] = nz;
@@ -170,7 +195,7 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
       const_cast<float*>(out.t2)[b * 3 + tid - 9] = st.t[s_tgt * 3 + tid - 9];
     } else if (tid == 12) {
       const_cast<float*>(out.logsnr)[b] = xu_fd_logsnr(t);
-      const_cast<float*>(out.cond_mask)[b] = xu_fd_cond_mask(s_hb, p_uncond);
+      const_cast<float*>(out.cond_mask)[b] = D ? 1.f : xu_fd_cond_mask(s_hb, p_uncond);
       if (loss_weight != nullptr) loss_weight[b] = snr_weight != nullptr ? snr_weight[t] : 1.f;
       if (t_out != nullptr) t_out[b] = t;
       if (idx_out != nullptr) {
@@ -178,6 +203,22 @@ __global__ void __launch_bounds__(SRN_THREADS) srn_batch_kernel(xunet_srn_store 
         idx_out[b * 3 + 1] = s_v;
         idx_out[b * 3 + 2] = s_v2;
       }
+    }
+    if constexpr (D) {     // the same values into the teacher's rows, and m_b
+      for (int c = 0; c < dd.copies; ++c) {
+        const int tb = c * B + b;
+        if (tid < 9) {
+          const_cast<float*>(dd.teacher.R1)[tb * 9 + tid] = st.R[s_src * 9 + tid];
+          const_cast<float*>(dd.teacher.R2)[tb * 9 + tid] = st.R[s_tgt * 9 + tid];
+          const_cast<float*>(dd.teacher.K)[tb * 9 + tid] = st.K[s_inst * 9 + tid];
+        } else if (tid < 12) {
+          const_cast<float*>(dd.teacher.t1)[tb * 3 + tid - 9] = st.t[s_src * 3 + tid - 9];
+          const_cast<float*>(dd.teacher.t2)[tb * 3 + tid - 9] = st.t[s_tgt * 3 + tid - 9];
+        } else if (tid == 12) {
+          const_cast<float*>(dd.teacher.logsnr)[tb] = xu_fd_logsnr(t);
+        }
+      }
+      if (tid == 12) dd.m_out[b] = s_m;
     }
   }
 }
@@ -188,29 +229,37 @@ template <int TARGET>
 static void launch_srn_batch_target(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k,
                                     int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
                                     const float* snr_weight, const xunet_batch& out, float* noise, float* loss_weight,
-                                    int* idx_out, int* t_out, float* v_out, cudaStream_t s) {
+                                    int* idx_out, int* t_out, float* v_out, const XuDistillDraw& dd, cudaStream_t s) {
   const long long per = 3LL * st.S * st.S;
   const size_t px_align = st.pixel_kind == XUNET_PIXELS_U8 ? 4 : 16;
   const int vec = per % 4 == 0 && ((uintptr_t)st.pixels % px_align) == 0 && aligned16(out.x) && aligned16(out.z) &&
-                  aligned16(noise) && aligned16(v_out);
+                  aligned16(noise) && aligned16(v_out) && aligned16(dd.teacher.x) && aligned16(dd.teacher.z);
   const long long work = vec ? per / 4 : per;
   const dim3 grid((unsigned)cdiv(work, SRN_THREADS), (unsigned)B);
   if (st.pixel_kind == XUNET_PIXELS_U8)
     xu_launch(srn_batch_kernel<XUNET_PIXELS_U8, TARGET>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world,
-              sqrt_ac, sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec, v_out);
+              sqrt_ac, sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec, v_out, dd);
   else
     xu_launch(srn_batch_kernel<XUNET_PIXELS_F32, TARGET>, grid, SRN_THREADS, 0, s, st, step_dev, seed, j, k, rank, world,
-              sqrt_ac, sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec, v_out);
+              sqrt_ac, sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec, v_out, dd);
 }
 
 void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
                       int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
                       const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, float* v_out,
                       cudaStream_t s) {
+  const XuDistillDraw none = {};
   if (v_out != nullptr)
     launch_srn_batch_target<XU_TARGET_V>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight,
-                                         out, noise, loss_weight, idx_out, t_out, v_out, s);
+                                         out, noise, loss_weight, idx_out, t_out, v_out, none, s);
   else
     launch_srn_batch_target<XU_TARGET_EPS>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond,
-                                           snr_weight, out, noise, loss_weight, idx_out, t_out, v_out, s);
+                                           snr_weight, out, noise, loss_weight, idx_out, t_out, v_out, none, s);
+}
+
+void launch_srn_batch_distill(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k,
+                              int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const xunet_batch& out,
+                              const XuDistillDraw& dd, int* idx_out, int* t_out, cudaStream_t s) {
+  launch_srn_batch_target<XU_TARGET_DISTILL>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, 0.f, nullptr, out,
+                                             nullptr, nullptr, idx_out, t_out, nullptr, dd, s);
 }

@@ -28,7 +28,7 @@ static int fail(const char* fmt, ...) {
   return 1;
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 110; }
+extern "C" int xunet_version(void) { return 111; }
 
 namespace {
 
@@ -1454,7 +1454,7 @@ extern "C" int xunet_sampler_step_table(const float* eps2, float* z, const float
                                         const int* pos_dev, const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2,
                                         int batch2, void* stream) {
   if (!eps2 || !z || !table || !pos_dev || !seed_dev || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0) return fail("xunet_sampler_step_table: bad argument");
-  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, nullptr,
+  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, nullptr, true,
                             (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("sampler_step_table: CUDA error: %s", cudaGetErrorString(e));
@@ -1465,7 +1465,7 @@ extern "C" int xunet_sampler_step_multistep(const float* eps2, float* z, const f
                                             float* x0_hist, float* next_z2, float* next_logsnr2, int batch2, void* stream) {
   if (!eps2 || !z || !table || !pos_dev || !seed_dev || !x0_hist || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0)
     return fail("xunet_sampler_step_multistep: bad argument");
-  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist,
+  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, true,
                             (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("sampler_step_multistep: CUDA error: %s", cudaGetErrorString(e));
@@ -1486,9 +1486,32 @@ extern "C" int xunet_sampler_step_dynamic(const float* eps2, float* z, const flo
   if (!(percentile > 0.0 && percentile <= 1.0))
     return fail("xunet_sampler_step_dynamic: percentile %g outside (0, 1]", percentile);
   launch_sampler_step_dynamic(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, batch,
-                              percentile, scale_out, (cudaStream_t)stream);
+                              percentile, scale_out, true, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("sampler_step_dynamic: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_sampler_step_cond(const float* out, float* z, const float* noise, long long n, const float* table,
+                                       const int* pos_dev, const unsigned long long* seed_dev, float* x0_hist, int batch,
+                                       double percentile, float* scale_out, float* next_z, float* next_logsnr, void* stream) {
+  if (!out || !z || !table || !pos_dev || !seed_dev || !next_z || !next_logsnr)
+    return fail("xunet_sampler_step_cond: NULL pointer argument");
+  if (n <= 0 || batch < 1) return fail("xunet_sampler_step_cond: n = %lld, batch = %d, need both >= 1", n, batch);
+  if (n % batch != 0) return fail("xunet_sampler_step_cond: n = %lld is not a multiple of batch = %d", n, batch);
+  if (percentile != 0.0) {
+    if (n / batch > XUNET_SAMPLER_DYN_MAX_PER)
+      return fail("xunet_sampler_step_cond: %lld values per view, more than XUNET_SAMPLER_DYN_MAX_PER = %d", n / batch,
+                  XUNET_SAMPLER_DYN_MAX_PER);
+    if (!(percentile > 0.0 && percentile <= 1.0))
+      return fail("xunet_sampler_step_cond: percentile %g outside (0, 1] (0 selects the fixed clip)", percentile);
+    launch_sampler_step_dynamic(out, z, noise, n, 0.f, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, batch,
+                                percentile, scale_out, false, (cudaStream_t)stream);
+  } else {
+    launch_sampler_step_table(out, z, noise, n, 0.f, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, false,
+                              (cudaStream_t)stream);
+  }
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("sampler_step_cond: CUDA error: %s", cudaGetErrorString(e));
 }
 
 extern "C" int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
@@ -1552,6 +1575,52 @@ extern "C" int xunet_srn_batch_v(const xunet_srn_store* store, const long long* 
                    loss_weight, idx_out, t_out, v_out, (cudaStream_t)stream);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail("srn_batch_v: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_srn_batch_distill(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j,
+                                       int k, int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac,
+                                       const int* grid_t, int n_grid, const xunet_batch* out, const xunet_batch* teacher,
+                                       int teacher_copies, int* m_out, int* idx_out, int* t_out, void* stream) {
+  if (!grid_t || !teacher || !m_out || !teacher->x || !teacher->z || !teacher->logsnr || !teacher->R1 || !teacher->t1 ||
+      !teacher->R2 || !teacher->t2 || !teacher->K)
+    return fail("xunet_srn_batch_distill: NULL pointer argument");
+  if (const int rc = srn_batch_check("xunet_srn_batch_distill", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out))
+    return rc;
+  if (n_grid < 1) return fail("xunet_srn_batch_distill: n_grid = %d, need >= 1", n_grid);
+  if (teacher_copies != 1 && teacher_copies != 2)
+    return fail("xunet_srn_batch_distill: teacher_copies = %d, need 1 or 2", teacher_copies);
+  const XuDistillDraw dd = {*teacher, teacher_copies, grid_t, n_grid, m_out};
+  launch_srn_batch_distill(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, *out, dd, idx_out, t_out,
+                           (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("srn_batch_distill: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_distill_teacher_step(const float* out_t, float w, int teacher_copies, const float* teacher_table,
+                                          const int* m_dev, int B, long long per, const xunet_batch* teacher, void* stream) {
+  if (!out_t || !teacher_table || !m_dev || !teacher || !teacher->z || !teacher->logsnr)
+    return fail("xunet_distill_teacher_step: NULL pointer argument");
+  if (B < 1 || per < 1) return fail("xunet_distill_teacher_step: B = %d, per = %lld, need both >= 1", B, per);
+  if (teacher_copies != 1 && teacher_copies != 2)
+    return fail("xunet_distill_teacher_step: teacher_copies = %d, need 1 or 2", teacher_copies);
+  launch_distill_teacher_step(out_t, w, teacher_copies, teacher_table, m_dev, B, per, const_cast<float*>(teacher->z),
+                              const_cast<float*>(teacher->logsnr), (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("distill_teacher_step: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_distill_target(const float* out_t, float w, int teacher_copies, const float* teacher_table,
+                                    const float* target_table, const int* m_dev, const float* z_t, const float* teacher_z, int B,
+                                    long long per, float* v_out, void* stream) {
+  if (!out_t || !teacher_table || !target_table || !m_dev || !z_t || !teacher_z || !v_out)
+    return fail("xunet_distill_target: NULL pointer argument");
+  if (B < 1 || per < 1) return fail("xunet_distill_target: B = %d, per = %lld, need both >= 1", B, per);
+  if (teacher_copies != 1 && teacher_copies != 2)
+    return fail("xunet_distill_target: teacher_copies = %d, need 1 or 2", teacher_copies);
+  launch_distill_target(out_t, w, teacher_copies, teacher_table, target_table, m_dev, z_t, teacher_z, B, per, v_out,
+                        (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("distill_target: CUDA error: %s", cudaGetErrorString(e));
 }
 
 extern "C" int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,

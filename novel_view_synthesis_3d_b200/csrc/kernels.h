@@ -145,15 +145,16 @@ void launch_adam(float* p, const float* g, float* m, float* v, long long n, long
 void launch_grad_global_norm(const float* g, long long n, double grad_scale, double* scratch, float* norm_out,
                              cudaStream_t s);
 // x0_hist == nullptr: the single-step update (DDPM, DDIM); else the multistep one, which reads column 6 (c_prev) and the
-// previous step's x0 from x0_hist (n floats) and stores this step's x0 there
+// previous step's x0 from x0_hist (n floats) and stores this step's x0 there.  guided: eps2 = [cond ; uncond] (2n) and the new z
+// goes to both halves of inp_z; else eps2 is the conditional output (n), used as is, and inp_z has n values
 void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
-                               float* x0_hist, cudaStream_t s);
+                               float* x0_hist, bool guided, cudaStream_t s);
 // xunet_sampler_step_dynamic (sampler_dyn.cu): the step above with x0 thresholded per view at the p-quantile of |x0|; one
 // cluster of 8 CTAs per view, n / B <= XUNET_SAMPLER_DYN_MAX_PER
 void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                  const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
-                                 int B2, float* x0_hist, int B, double p, float* scale_out, cudaStream_t s);
+                                 int B2, float* x0_hist, int B, double p, float* scale_out, bool guided, cudaStream_t s);
 // v_out != nullptr: the v-target instance (xunet_forward_diffusion_v), which also stores v and takes noise_out == nullptr
 void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
                               const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
@@ -165,6 +166,24 @@ void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsi
                       int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
                       const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, float* v_out,
                       cudaStream_t s);
+// xunet_srn_batch_distill: the draw of xunet_srn_batch with t = grid_t[m], m = (sample hash) mod n_grid, cond_mask 1, no
+// target, and the sample's inputs copied into the teacher's `copies` row blocks
+struct XuDistillDraw {
+  xunet_batch teacher;    // x, z, logsnr, R1, t1, R2, t2, K of the teacher's batch (copies * B rows; cond_mask, rays unused)
+  int copies;             // 2: a guided [cond ; uncond] teacher batch, 1: an unguided one
+  const int* grid_t;      // the student's timesteps, loop order
+  int n_grid;
+  int* m_out;             // (B) the drawn grid positions
+};
+void launch_srn_batch_distill(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k,
+                              int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const xunet_batch& out,
+                              const XuDistillDraw& dd, int* idx_out, int* t_out, cudaStream_t s);
+// distill.cu: the teacher's first DDIM step (row 2 m_b of the teacher table) from the first teacher output, into the teacher's z
+// and logsnr rows; then the target: the second step (row 2 m_b + 1) from the second output, and the student's v target
+void launch_distill_teacher_step(const float* out_t, float w, int copies, const float* ttab, const int* m_dev, int B,
+                                 long long per, float* tz, float* tlogsnr, cudaStream_t s);
+void launch_distill_target(const float* out_t, float w, int copies, const float* ttab, const float* gtab, const int* m_dev,
+                           const float* z_t, const float* tz, int B, long long per, float* v_out, cudaStream_t s);
 void launch_dropout_mask(float* out, long long n, int op_index, unsigned long long seed, float rate, cudaStream_t s);
 // xunet_image_metrics: one CTA per image, fp64 moments and sums in a fixed order (metrics.cu); 11 <= S <= XUNET_METRICS_MAX_SIDE
 struct MetricsWindow { double w[11]; };   // the normalised 1-D Gaussian weights of the SSIM window

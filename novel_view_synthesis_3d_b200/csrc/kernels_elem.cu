@@ -1723,7 +1723,10 @@ void launch_grad_global_norm(const float* g, long long n, double grad_scale, dou
 // single-step kernel).  HIST = true (multistep solvers, DPM-Solver++(2M)) fixes the order, one rounding per fma:
 //   z' = fma(sigma, noise, fma(c_prev, x0_hist[i], fma(c_x0, x0, c_z * z))), the c_prev term skipped when c_prev == 0,
 // then x0_hist[i] = x0.  A row with c_prev == 0 never reads x0_hist (the first step needs no initialised history).
-template <bool HIST>
+// GUIDED = true: eps2 is the [cond ; uncond] output of a 2B batch and the new z goes to both halves of inp_z.  GUIDED = false
+// (a model whose guidance is in its weights, e.g. a distilled student): eps2 is the B-batch conditional output, read as is,
+// and the new z goes to inp_z's n values.
+template <bool HIST, bool GUIDED>
 __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __restrict__ eps2, float* __restrict__ z,
                                                                  const float* __restrict__ noise, long long n, float w,
                                                                  const float* __restrict__ tab, const int* __restrict__ pos_dev,
@@ -1735,10 +1738,9 @@ __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __
   const float* t = tab + 8LL * k;
   if (i < B2) inp_logsnr[i] = t[5];
   if (i >= n) return;
-  const float e = (1.f + w) * eps2[i] - w * eps2[n + i];
+  const float e = GUIDED ? xu_step_guided(w, eps2[i], eps2[n + i]) : eps2[i];
   const float zi = z[i];
-  float x0 = t[0] * zi - t[1] * e;
-  x0 = fminf(fmaxf(x0, -1.f), 1.f);
+  const float x0 = xu_step_x0(t, zi, e);
   const float nz = noise != nullptr ? noise[k * n + i] : xu_hash_normal(*seed_dev - (unsigned long long)k, (uint64_t)i);
   float zn;
   if constexpr (HIST) {
@@ -1748,22 +1750,19 @@ __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __
     zn = fmaf(t[4], nz, zn);
     x0_hist[i] = x0;
   } else {
-    zn = t[2] * x0 + t[3] * zi + t[4] * nz;
+    zn = xu_step_z(t, x0, zi, nz);
   }
   z[i] = zn;
   inp_z[i] = zn;
-  inp_z[n + i] = zn;
+  if constexpr (GUIDED) inp_z[n + i] = zn;
 }
 void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
-                               float* x0_hist, cudaStream_t s) {
+                               float* x0_hist, bool guided, cudaStream_t s) {
   const int grid = cdiv(n > B2 ? n : B2, 256);
-  if (x0_hist != nullptr)
-    xu_launch(sampler_step_table_kernel<true>, grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr,
-              B2, x0_hist);
-  else
-    xu_launch(sampler_step_table_kernel<false>, grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr,
-              B2, x0_hist);
+  auto kernel = x0_hist != nullptr ? (guided ? sampler_step_table_kernel<true, true> : sampler_step_table_kernel<true, false>)
+                                   : (guided ? sampler_step_table_kernel<false, true> : sampler_step_table_kernel<false, false>);
+  xu_launch(kernel, grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr, B2, x0_hist);
 }
 
 // dataset/data_loader.py:92-110 on the device.  TARGET == XU_TARGET_V also stores v = xu_fd_v(..) to v_out (the last

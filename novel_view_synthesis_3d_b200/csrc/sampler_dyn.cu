@@ -42,7 +42,9 @@ __device__ __forceinline__ float dyn_threshold_scale(float lo_v, float hi_v, dou
   return fmaxf(__double2float_rn(q), 1.f);
 }
 
-template <bool HIST>
+// GUIDED = false: the unguided step of sampler_step_table_kernel<.., false> (eps2 the B-batch conditional output, read as is;
+// the new z goes to inp_z's n values only)
+template <bool HIST, bool GUIDED>
 __global__ void __cluster_dims__(DYN_CLUSTER, 1, 1) __launch_bounds__(DYN_THREADS)
 sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ z, const float* __restrict__ noise, long long n,
                             float w, const float* __restrict__ tab, const int* __restrict__ pos_dev,
@@ -71,7 +73,7 @@ sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ 
   const float c_recip = t[0], c_recipm1 = t[1], wp1 = __fadd_rn(1.f, w);
   for (int j = tid; j < len; j += DYN_THREADS) {
     const long long i = base + j;
-    const float e = fmaf(wp1, eps2[i], -__fmul_rn(w, eps2[n + i]));
+    const float e = GUIDED ? fmaf(wp1, eps2[i], -__fmul_rn(w, eps2[n + i])) : eps2[i];
     xs[j] = fmaf(c_recip, z[i], -__fmul_rn(c_recipm1, e));
   }
   hist[0][tid] = 0u;
@@ -166,29 +168,26 @@ sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ 
     zn = fmaf(t[4], nz, zn);
     z[i] = zn;
     inp_z[i] = zn;
-    inp_z[n + i] = zn;
+    if constexpr (GUIDED) inp_z[n + i] = zn;
   }
   cluster.barrier_wait(std::move(arrived));
 }
 
 void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                  const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
-                                 int B2, float* x0_hist, int B, double p, float* scale_out, cudaStream_t s) {
+                                 int B2, float* x0_hist, int B, double p, float* scale_out, bool guided, cudaStream_t s) {
   static bool configured = false;
   if (!configured) {
-    cudaFuncSetAttribute(sampler_step_dynamic_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)(sizeof(float) * kDynMaxChunk));
-    cudaFuncSetAttribute(sampler_step_dynamic_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)(sizeof(float) * kDynMaxChunk));
+    for (auto kernel : {sampler_step_dynamic_kernel<false, true>, sampler_step_dynamic_kernel<true, true>,
+                        sampler_step_dynamic_kernel<false, false>, sampler_step_dynamic_kernel<true, false>})
+      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * kDynMaxChunk));
     configured = true;
   }
   const int per = (int)(n / B);
   const size_t smem = sizeof(float) * (size_t)((per + DYN_CLUSTER - 1) / DYN_CLUSTER);
   const dim3 grid((unsigned)B * DYN_CLUSTER);
-  if (x0_hist != nullptr)
-    xu_launch(sampler_step_dynamic_kernel<true>, grid, DYN_THREADS, smem, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z,
-              inp_logsnr, B2, x0_hist, per, p, scale_out);
-  else
-    xu_launch(sampler_step_dynamic_kernel<false>, grid, DYN_THREADS, smem, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z,
-              inp_logsnr, B2, x0_hist, per, p, scale_out);
+  auto kernel = x0_hist != nullptr ? (guided ? sampler_step_dynamic_kernel<true, true> : sampler_step_dynamic_kernel<true, false>)
+                                   : (guided ? sampler_step_dynamic_kernel<false, true> : sampler_step_dynamic_kernel<false, false>);
+  xu_launch(kernel, grid, DYN_THREADS, smem, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr, B2, x0_hist,
+            per, p, scale_out);
 }

@@ -13,6 +13,10 @@ Any of the three can replace the fixed clip of x0 with per-view dynamic threshol
 Every sampler reads the network output as eps by default.  prediction='v' reads it as v = sqrt(abar) eps - sqrt(1 - abar) x0
 (Salimans & Ho 2022): only the first two table columns change, since every step computes x0 = c_recip z - c_recipm1 out and
 the guidance (1 + w) out_c - w out_u is linear in the output.
+
+w=None samples a model whose guidance is in its weights, such as a progressively distilled student (distill.py): one
+B-batch conditional forward per step, stepped by `xunet_sampler_step_cond`.  `distill_grid` gives the timesteps such a
+student was trained on, and `Schedule(timesteps=...)` the schedule of any such grid.
 """
 from __future__ import annotations
 
@@ -61,14 +65,26 @@ class Schedule:
     uniform in lambda = log(sqrt(abar) / sqrt(1 - abar)) between lambda(T-1) and lambda(0), each mapped to the timestep
     with the nearest lambda, duplicates dropped.  The last steps of the cosine schedule hold a large log-SNR jump, so this
     is the spacing multistep solvers need.  With it, len(self) -- the number of forwards a sample runs -- can be smaller
-    than `steps` (9 for 10, 19 for 25, 36 for 50, 142 for 256)."""
+    than `steps` (9 for 10, 19 for 25, 36 for 50, 142 for 256).
 
-    def __init__(self, steps: int = 1000, T: int = 1000, spacing: str = 'linear'):
+    timesteps: an explicit set of timesteps in [0, T), such as a distilled student's grid (`distill_grid`), in any order
+    and without duplicates; it replaces `steps` and `spacing`.  The tables are built from it exactly as from a spacing's
+    timesteps, so Schedule(timesteps=Schedule(n).timesteps) has the tables of Schedule(n)."""
+
+    def __init__(self, steps: int = 1000, T: int = 1000, spacing: str = 'linear', *, timesteps=None):
         if spacing not in SPACINGS:
             raise ValueError(f'unknown spacing {spacing!r}; expected one of {SPACINGS}')
         betas_full = cosine_beta_schedule(T)
         ac_full = np.cumprod(1. - betas_full, axis=0)
-        if spacing == 'logsnr':
+        if timesteps is not None:
+            ts = np.asarray(timesteps)
+            if ts.ndim != 1 or ts.size == 0 or not np.issubdtype(ts.dtype, np.integer):
+                raise ValueError(f'timesteps must be a non-empty 1-D array of integers, got {timesteps!r}')
+            self.timesteps = np.unique(ts.astype(np.int64))
+            if len(self.timesteps) != ts.size or self.timesteps[0] < 0 or self.timesteps[-1] >= T:
+                raise ValueError(f'timesteps must be distinct integers in [0, {T}), got {timesteps!r}')
+            ac = ac_full[self.timesteps]
+        elif spacing == 'logsnr':
             lam = 0.5 * np.log(ac_full / (1. - ac_full))
             target = np.linspace(lam[T - 1], lam[0], steps)
             self.timesteps = np.unique(np.abs(lam[None, :] - target[:, None]).argmin(1))
@@ -93,6 +109,22 @@ class Schedule:
 
     def __len__(self):
         return len(self.timesteps)
+
+
+def distill_grid(teacher_steps: int, rounds: int) -> np.ndarray:
+    """The timesteps, in loop order (highest t first), of a model progressively distilled `rounds` times (Salimans & Ho
+    2022) from a teacher sampled with DDIM on Schedule(teacher_steps, 'linear'): round 0 is that schedule's timesteps, and
+    each round keeps every other timestep of the last, G_r = G_{r-1}[0::2], so the top timestep stays and the grids nest.
+    Round r halves a grid of even length; an odd one raises ValueError."""
+    if isinstance(rounds, bool) or int(rounds) != rounds or rounds < 0:
+        raise ValueError(f'rounds must be an integer >= 0, got {rounds!r}')
+    g = Schedule(teacher_steps, spacing='linear').timesteps[::-1]
+    for r in range(int(rounds)):
+        if len(g) % 2:
+            raise ValueError(f'round {r + 1} of {rounds} would halve a grid of odd length {len(g)} '
+                             f'(teacher_steps = {teacher_steps}); use a teacher_steps divisible by 2**{rounds}')
+        g = g[0::2]
+    return g.copy()
 
 
 def _check_method(method: str, eta: float) -> None:
@@ -198,24 +230,34 @@ class Sampler:
     every method, dynamic thresholding and sample_views run the same kernels.  The lag defaults to off for v: it is a quirk
     of the reference's eps-trained checkpoints.
 
+    w=None: the model is sampled without classifier-free guidance, for a model whose guidance is in its weights (a
+    distilled student, `distill.py`): the engine holds B rows, all with cond_mask 1, and each step is one B-batch forward
+    and `xunet_sampler_step_cond`, for every method, dynamic thresholding and sample_views.  A float w (0 included) keeps
+    the guided 2B batch.  timesteps: an explicit timestep grid (`Schedule(timesteps=..)`, e.g. `distill_grid`) in place of
+    `steps` and `spacing`.
+
     dynamic_threshold: None clips x0 to [-1, 1] (the reference).  A percentile p in (0, 1] thresholds x0 per view instead
     (Saharia et al. 2022, Imagen section 2.3): s = max(1, p-quantile of |x0| over the view), x0 <- clip(x0, -s, s) / s, for
     every method, in `xunet_sampler_step_dynamic` (the paper uses p = 0.995).  It keeps guided x0 far outside [-1, 1] (large
     w at high noise) from saturating to +-1; a view whose s is 1 gets the fixed clip's bits."""
 
-    def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000, w: float = 3.0,
-                 use_graph: bool = True, method: str = 'ddpm', eta: float = 0.0, spacing: str | None = None,
-                 logsnr_lag: bool | None = None, dynamic_threshold: float | None = None, prediction: str = 'eps'):
+    def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000,
+                 w: float | None = 3.0, use_graph: bool = True, method: str = 'ddpm', eta: float = 0.0,
+                 spacing: str | None = None, logsnr_lag: bool | None = None, dynamic_threshold: float | None = None,
+                 prediction: str = 'eps', timesteps=None):
         _check_method(method, eta)
         _check_dynamic_threshold(dynamic_threshold)
         self.prediction = check_prediction(prediction)
         self.dynamic_threshold = None if dynamic_threshold is None else float(dynamic_threshold)
         self.method, self.eta = method, float(eta)
         self.logsnr_lag = (method == 'ddpm' and prediction == 'eps') if logsnr_lag is None else bool(logsnr_lag)
-        self.model, self.B, self.S, self.w = model, batch_size, img_sidelength, float(w)
-        self.sched = Schedule(steps, spacing=('logsnr' if method == 'dpmpp_2m' else 'linear') if spacing is None else spacing)
-        self.eng = model.engine(2 * batch_size, img_sidelength, False)
-        self.flat = model.flat_from_tree(params, img_sidelength, 2 * batch_size)
+        self.model, self.B, self.S = model, batch_size, img_sidelength
+        self.w = None if w is None else float(w)
+        self.copies = 1 if w is None else 2       # engine rows per view: [cond] or [cond ; uncond]
+        self.sched = Schedule(steps, spacing=('logsnr' if method == 'dpmpp_2m' else 'linear') if spacing is None else spacing,
+                              timesteps=timesteps)
+        self.eng = model.engine(self.copies * batch_size, img_sidelength, False)
+        self.flat = model.flat_from_tree(params, img_sidelength, self.copies * batch_size)
         self.lib = _lib.load()
         self.dev = self.eng.device
         self.z = torch.zeros(batch_size, img_sidelength, img_sidelength, 3, dtype=torch.float32, device=self.dev)
@@ -244,8 +286,8 @@ class Sampler:
         src = dict(batch)
         src.setdefault('z', np.zeros((B, S, S, 3), np.float32))
         src.setdefault('logsnr', np.zeros((B,), np.float32))
-        dup = {k: np.concatenate([np.asarray(src[k], dtype=np.float32)] * 2, axis=0) for k in BATCH_KEYS}
-        mask = np.concatenate([np.ones(B, np.float32), np.zeros(B, np.float32)])
+        dup = {k: np.concatenate([np.asarray(src[k], dtype=np.float32)] * self.copies, axis=0) for k in BATCH_KEYS}
+        mask = np.concatenate([np.ones(B, np.float32), np.zeros((self.copies - 1) * B, np.float32)])
         e.load_inputs(dup, cond_mask=mask)
         steps = self._load_schedule()
         self._start_chain(seed, z_init, noises)
@@ -276,7 +318,8 @@ class Sampler:
         else:
             self.z.copy_(torch.as_tensor(np.asarray(z_init), dtype=torch.float32).to(self.dev))
         e.inp['z'][:B].copy_(self.z)
-        e.inp['z'][B:].copy_(self.z)
+        if self.copies == 2:
+            e.inp['z'][B:].copy_(self.z)
         e.inp['logsnr'].fill_(self._logsnr_first)
         self._seed_base.fill_((seed * 1000003 + steps - 1) & 0x7FFFFFFFFFFFFFFF)    # the kernel subtracts the loop position
         if noises is not None:
@@ -309,11 +352,20 @@ class Sampler:
         e = self.eng
         e.forward(self.flat, train=False)
         st = torch.cuda.current_stream(self.dev).cuda_stream
+        hist = None if self._x0_hist is None else self._x0_hist.data_ptr()
+        if self.w is None:
+            _lib.check(self.lib.xunet_sampler_step_cond(e.eps.data_ptr(), self.z.data_ptr(),
+                                                        self._noise.data_ptr() if noise else None, self.z.numel(),
+                                                        self._tab.data_ptr(), self._pos.data_ptr(), self._seed_base.data_ptr(),
+                                                        hist, self.B, self.dynamic_threshold or 0.0, None,
+                                                        e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(), st),
+                       'sampler_step_cond')
+            self._pos.add_(1)
+            return
         head = (e.eps.data_ptr(), self.z.data_ptr(), self._noise.data_ptr() if noise else None, self.z.numel(), self.w,
                 self._tab.data_ptr(), self._pos.data_ptr(), self._seed_base.data_ptr())
         tail = (e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(), 2 * self.B, st)
         if self.dynamic_threshold is not None:
-            hist = None if self._x0_hist is None else self._x0_hist.data_ptr()
             _lib.check(self.lib.xunet_sampler_step_dynamic(*head, hist, self.B, self.dynamic_threshold, None, *tail),
                        'sampler_step_dynamic')
         elif self._x0_hist is None:
@@ -342,7 +394,7 @@ class Sampler:
         For each of the m target poses in turn the chain starts from noise and, at EVERY denoising step, conditions on
         one view drawn uniformly from the pool (the k sources plus -- if condition_on_generated -- the targets generated
         so far), exactly as the paper's sampler; one 2B-batch forward per step ([cond ; uncond], guidance weight w) and
-        the same posterior update as `sample()`.  The pool lives on the device; a step only copies the chosen view and
+        the same posterior update as `sample()` (w=None: one B-batch conditional forward).  The pool lives on the device; a step only copies the chosen view and
         its pose into the engine's input buffers before the step, which runs with the full forward (static conditioning
         off).  z_init (m, B,S,S,3) / noises (m, steps, B,S,S,3) make a run reproducible against the oracle; with one
         source, one target and the same seed the result equals `sample()`.
@@ -358,21 +410,22 @@ class Sampler:
         Kd = f32(K)
         rng = np.random.RandomState(seed)
         steps = self._load_schedule()
-        e.inp['K'].copy_(torch.cat([Kd, Kd], 0).reshape(e.inp['K'].shape))
-        e.inp['cond_mask'].copy_(torch.cat([torch.ones(B, device=dev), torch.zeros(B, device=dev)]))
+        cp = self.copies
+        e.inp['K'].copy_(torch.cat([Kd] * cp, 0).reshape(e.inp['K'].shape))
+        e.inp['cond_mask'].copy_(torch.cat([torch.ones(B, device=dev), torch.zeros((cp - 1) * B, device=dev)]))
         outs, choices = [], []
         for j in range(m):
-            e.inp['R2'].copy_(torch.cat([tR[:, j], tR[:, j]], 0).reshape(e.inp['R2'].shape))
-            e.inp['t2'].copy_(torch.cat([tt[:, j], tt[:, j]], 0).reshape(e.inp['t2'].shape))
+            e.inp['R2'].copy_(torch.cat([tR[:, j]] * cp, 0).reshape(e.inp['R2'].shape))
+            e.inp['t2'].copy_(torch.cat([tt[:, j]] * cp, 0).reshape(e.inp['t2'].shape))
             self._start_chain(seed + 7919 * j, None if z_init is None else z_init[j], None if noises is None else noises[j])
             row = []
 
             def set_view(k):
                 c = int(rng.randint(len(pool_x)))
                 row.append(c)
-                e.inp['x'].copy_(torch.cat([pool_x[c], pool_x[c]], 0).reshape(e.inp['x'].shape))
-                e.inp['R1'].copy_(torch.cat([pool_R[c], pool_R[c]], 0).reshape(e.inp['R1'].shape))
-                e.inp['t1'].copy_(torch.cat([pool_t[c], pool_t[c]], 0).reshape(e.inp['t1'].shape))
+                e.inp['x'].copy_(torch.cat([pool_x[c]] * cp, 0).reshape(e.inp['x'].shape))
+                e.inp['R1'].copy_(torch.cat([pool_R[c]] * cp, 0).reshape(e.inp['R1'].shape))
+                e.inp['t1'].copy_(torch.cat([pool_t[c]] * cp, 0).reshape(e.inp['t1'].shape))
 
             self._run(steps, noises is not None, static=False, set_view=set_view)
             out = self.z.clone()

@@ -20,6 +20,7 @@ import torch
 from . import _lib
 from . import dist as xdist
 from .diffusion import diffusion_tables, min_snr_weights
+from .distill import check_teacher, run_teacher
 from .sampling import check_prediction
 from .xunet import XUNet, ParamTree, Engine, InputSlots, check_loss
 
@@ -89,6 +90,9 @@ class TrainState:
     # what the network is trained to predict: 'eps' (the noise) or 'v' (sqrt(abar) eps - sqrt(1 - abar) x0); recorded in
     # the checkpoint
     prediction: str = 'eps'
+    # a progressively distilled student's {teacher_steps, rounds[, w]} (distill.Teacher.record); None for any other model.
+    # Recorded in the checkpoint
+    distill: Optional[dict] = None
     _mask_rng: np.random.RandomState = None
     _frozen_mask: Optional[np.ndarray] = None
 
@@ -362,13 +366,27 @@ class TrainStep:
     order follows the Adam count, restore_train_state + the same store and data_seed continue the data stream exactly.
     For a state built with prediction='v' the same kernel (xunet_srn_batch_v) writes the v target of each draw where an
     eps state gets its noise, and min_snr_gamma gives the v weights; nothing else in the step changes.
+
+    teacher=distill.Teacher (with data=): progressive distillation of the teacher into this state, a v / mse student
+    (distill.create_distill_state).  Per micro-batch, before the student's forward and backward, the step draws the batch
+    with t on the student grid (xunet_srn_batch_distill, cond_mask 1), runs the teacher forward, its first DDIM step, the
+    second teacher forward (static conditioning on: the same poses, K, mask and parameters) and the target kernel, which
+    writes the v target of the teacher's two steps into the slot's regression target.  Everything else -- accumulation,
+    clipping, warm-up, EMA, data parallelism and the single-graph capture -- is the data= step's.  Raises ValueError without
+    data=, for a state that is not prediction='v' with loss='mse', with reference_quirks or min_snr_gamma, for an odd teacher
+    grid, and when the teacher's S, B, device or model configuration differ from the state's.
     """
 
     def __init__(self, state: TrainState, *, use_graph: bool = True, bucket_mb: float = 128.0, allreduce: bool = True,
                  grad_accum_steps: int = 1, data=None, data_seed: int = 0, p_uncond: float = 0.1,
-                 min_snr_gamma: Optional[float] = None):
+                 min_snr_gamma: Optional[float] = None, teacher=None):
         self.k = check_grad_accum_steps(grad_accum_steps)
         self.data = data
+        self.teacher = teacher
+        if teacher is not None:
+            check_teacher(state, teacher, data)
+            if min_snr_gamma is not None:
+                raise ValueError('a distilled student is trained with the plain mse (SNR + 1 weighting of v): no min_snr_gamma')
         if data is None:
             if min_snr_gamma is not None:
                 raise ValueError('min_snr_gamma weights the batches a data= step draws; without data= pass loss_weight')
@@ -471,7 +489,9 @@ class TrainStep:
             for j in range(self.k):
                 last = j == self.k - 1
                 sd = self.seeds[j:j + 1]
-                if self.data is not None:
+                if self.teacher is not None:
+                    run_teacher(self, j)
+                elif self.data is not None:
                     self._draw(j)
                 e.forward(s.params.flat, train=True, inputs=(self.inputs, j), seed_dev=sd)
                 if last:
