@@ -483,6 +483,58 @@ int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long
 int xunet_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
                         float* ssim_out, void* stream);
 
+/* Radiance grid of the 3D consistency score (3DiM, Watson et al. 2022, section 5: fit a field to some generated views, render
+ * it at the poses of the others, score the renders).  The field:
+ *   grid  fp32 (G, G, G, 4) channels-last, indexed [ix][iy][iz][c]; c = 0 raw density, c = 1..3 raw colour.  Grid point
+ *         (ix, iy, iz) sits at world position -b + 2b (ix, iy, iz) / (G - 1): the cube [-b, b]^3, b = bound.  Inside it the raw
+ *         vector is the trilinear interpolation of the 8 surrounding grid points; the activations come after:
+ *         sigma = softplus(raw_0 + XUNET_FIELD_DENSITY_SHIFT) (an all-zero grid is nearly transparent), colour =
+ *         sigmoid(raw_1..3) in [0, 1].  No view dependence: colour is a function of position only, so the field cannot explain
+ *         views that disagree as view-dependent appearance.
+ *   rays  pixel (row, col) of view v starts at t_v with direction normalize(R_v K_v^-1 (col + 1/2, row + 1/2, 1)): convention 1
+ *         (XUNET_RAYS_OPENCV_UV), SRN's camera model -- whatever ray convention a checkpoint was trained with.  R (V, 3, 3)
+ *         camera-to-world, t (V, 3), K (V, 3, 3), row-major.
+ *   samples  the ray's segment inside the cube, clipped to t >= near, of length L (empty: the pixel is the background) is cut
+ *         into n = ceil(L / step) pieces of length step, the last one shortened so that the lengths d_k sum to L; piece k is
+ *         sampled at its midpoint.  No early termination.
+ *   compositing  a_k = 1 - exp(-sigma_k d_k), T_0 = 1, T_{k+1} = T_k (1 - a_k); C = sum_k T_k a_k c_k + T_n bg with
+ *         bg = (background + 1) / 2; the pixel is 2C - 1 (the sampler's [-1, 1]).
+ * Limits: XUNET_FIELD_MIN_GRID <= G <= XUNET_FIELD_MAX_GRID, 0 < bound <= XUNET_FIELD_MAX_BOUND, near >= 0, step > 0 with
+ * ceil(2 sqrt(3) bound / step) <= XUNET_FIELD_MAX_SAMPLES samples on the longest chord, V >= 1, S >= 1, V S S < 2^31.
+ * Every entry checks its arguments before it launches anything (message starting with the entry's name); no allocation, no
+ * host sync, graph-capturable.  kinv: device scratch of V * 9 floats (receives K^-1). */
+#define XUNET_FIELD_DENSITY_SHIFT (-6.0f)
+#define XUNET_FIELD_MIN_GRID 2
+#define XUNET_FIELD_MAX_GRID 256
+#define XUNET_FIELD_MAX_BOUND 64.0f
+#define XUNET_FIELD_MAX_SAMPLES 4096
+#define XUNET_FIELD_MAX_RAYS (1 << 20)
+#define XUNET_FIELD_FIXED_ONE 4294967296.0   /* 2^32: one unit of the fixed-point gradient sums */
+/* Renders V views: out (V, S, S, 3) in [-1, 1].  Each pixel is composited by one thread on its own, so a view has the same bits
+ * alone or anywhere in a batch. */
+int xunet_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv, int V,
+                       int S, float near, float step, float background, float* out, void* stream);
+/* One iteration's loss and gradient.  views (V, S, S, 3) in [-1, 1] are the training pixels, u = clamp((view + 1) / 2, 0, 1).
+ * With i = *iter_dev (device int64, the Adam count of the update this gradient feeds, 1-based), ray r < rays is pixel
+ *     xu_mix64(seed * 0x9E3779B97F4A7C15 + i * 0xD1B54A32D192ED03 + r) mod (V S S)      (index v S S + row S + col)
+ * (drawn with replacement), and the loss is (1 / 3N) sum_r sum_ch (C - u)^2 (N = rays) plus the total variation
+ *     tv_density / G^3 sum_axes sum (D raw_0)^2 + tv_color / G^3 sum_axes sum_{c=1..3} (D raw_c)^2   (D: forward difference).
+ * grad (G, G, G, 4) receives the gradient of that loss w.r.t. the raw grid, and loss_out[i - 1] (when 1 <= i <= loss_len) the
+ * data term alone, the mean squared error of the drawn pixels in [0, 1] units.
+ * Determinism: each sample's gradient contribution to each corner word is rounded to a multiple of 1 / XUNET_FIELD_FIXED_ONE
+ * and the contributions, and each ray's squared error, are summed as int64 with integer atomics in acc (4 G^3 + 1 words, all
+ * zero on entry; the call leaves them zero), so grad and loss have the same bits on every run and every GPU.  No overflow:
+ * per ray and word, |dL/dC| <= 2 per channel; the colour words add g_ch T_k a_k c(1 - c) w, at most 2 * 1/4 over the ray
+ * (sum_k T_k a_k <= 1, w <= 1); the density word adds sum_ch g_ch d_k (T_{k+1} c_k - R_{k+1}) sigmoid(.) w, at most
+ * 3 * 2 * L <= 12 sqrt(3) XUNET_FIELD_MAX_BOUND < 1331 (|T_{k+1} c_k - R_{k+1}| <= T_{k+1} <= 1, sum_k d_k = L), plus half a
+ * unit of rounding per sample and corner; a ray's squared error is at most 3.  Over XUNET_FIELD_MAX_RAYS = 2^20 rays every
+ * sum stays below 1331 * 2^20 + 2^20 * 2^12 * 2^-33 < 2^31 in magnitude, i.e. below 2^63 in fixed point.
+ * Three launches: K^-1, the rays, and one finish pass (fixed-point to fp32, the TV stencil, the loss, clearing acc). */
+int xunet_field_loss_grad(const float* grid, int G, float bound, const float* views, const float* R, const float* t,
+                          const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
+                          const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color, long long* acc,
+                          float* grad, float* loss_out, long long loss_len, void* stream);
+
 /* ---- operator-level entry points (parity tests / micro-benchmarks of single kernels) ----
  * dtype as above; tensors channels-last (N,H,W,C). */
 int xunet_op_conv(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y,

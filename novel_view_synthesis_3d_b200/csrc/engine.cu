@@ -1642,6 +1642,50 @@ extern "C" int xunet_image_metrics(const float* pred, const float* target, int B
   return e == cudaSuccess ? 0 : fail("image_metrics: CUDA error: %s", cudaGetErrorString(e));
 }
 
+// The checks both field entries share (include/xunet_b200.h, "Limits"); 0 or the fail() code.
+static int field_check(const char* what, int G, float bound, int V, int S, float near, float step, float background) {
+  if (G < XUNET_FIELD_MIN_GRID || G > XUNET_FIELD_MAX_GRID)
+    return fail("%s: G = %d outside [%d, %d]", what, G, XUNET_FIELD_MIN_GRID, XUNET_FIELD_MAX_GRID);
+  if (V < 1 || S < 1) return fail("%s: V = %d, S = %d, need both >= 1", what, V, S);
+  if ((long long)V * S * S >= (1LL << 31)) return fail("%s: V S S = %lld pixels, need fewer than 2^31", what, (long long)V * S * S);
+  if (!isfinite(bound) || !(bound > 0.f) || bound > XUNET_FIELD_MAX_BOUND)
+    return fail("%s: bound = %g outside (0, %g]", what, bound, XUNET_FIELD_MAX_BOUND);
+  if (!isfinite(near) || near < 0.f) return fail("%s: near = %g, need a finite near >= 0", what, near);
+  if (!isfinite(step) || !(step > 0.f)) return fail("%s: step = %g, need a finite step > 0", what, step);
+  if (ceil(2.0 * sqrt(3.0) * bound / step) > XUNET_FIELD_MAX_SAMPLES)
+    return fail("%s: step = %g gives more than %d samples on a chord of the cube of bound %g", what, step, XUNET_FIELD_MAX_SAMPLES,
+                bound);
+  if (!isfinite(background)) return fail("%s: background = %g is not finite", what, background);
+  return 0;
+}
+
+extern "C" int xunet_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv,
+                                  int V, int S, float near, float step, float background, float* out, void* stream) {
+  if (!grid || !R || !t || !K || !kinv || !out) return fail("xunet_field_render: NULL pointer argument");
+  if (int rc = field_check("xunet_field_render", G, bound, V, S, near, step, background)) return rc;
+  launch_field_render(grid, G, bound, R, t, K, kinv, V, S, near, step, background, out, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("field_render: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_field_loss_grad(const float* grid, int G, float bound, const float* views, const float* R, const float* t,
+                                     const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
+                                     const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color,
+                                     long long* acc, float* grad, float* loss_out, long long loss_len, void* stream) {
+  if (!grid || !views || !R || !t || !K || !kinv || !iter_dev || !acc || !grad || !loss_out)
+    return fail("xunet_field_loss_grad: NULL pointer argument");
+  if (int rc = field_check("xunet_field_loss_grad", G, bound, V, S, near, step, background)) return rc;
+  if (rays < 1 || rays > XUNET_FIELD_MAX_RAYS)
+    return fail("xunet_field_loss_grad: rays = %d outside [1, %d]", rays, XUNET_FIELD_MAX_RAYS);
+  if (!isfinite(tv_density) || !isfinite(tv_color) || tv_density < 0.f || tv_color < 0.f)
+    return fail("xunet_field_loss_grad: tv weights %g, %g, need finite weights >= 0", tv_density, tv_color);
+  if (loss_len < 0) return fail("xunet_field_loss_grad: loss_len = %lld, need loss_len >= 0", loss_len);
+  launch_field_loss_grad(grid, G, bound, views, R, t, K, kinv, V, S, near, step, background, rays, iter_dev, seed, tv_density,
+                         tv_color, acc, grad, loss_out, loss_len, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("field_loss_grad: CUDA error: %s", cudaGetErrorString(e));
+}
+
 // ---- operator-level entry points ----------------------------------------------------------------------
 // fp64 reduction scratch of one operator-level call (kernels.h): stream-ordered allocations, released on the call's stream
 struct OpScratch {

@@ -189,6 +189,15 @@ void launch_dropout_mask(float* out, long long n, int op_index, unsigned long lo
 struct MetricsWindow { double w[11]; };   // the normalised 1-D Gaussian weights of the SSIM window
 void launch_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
                           float* ssim_out, cudaStream_t s);
+// xunet_field_render / xunet_field_loss_grad (field.cu): K^-1 of the V cameras into kinv (V, 9), then the render, or the drawn
+// rays' fixed-point gradient and the finish pass
+__global__ void kinv_kernel(const float* __restrict__ K, float* __restrict__ kinv, int B);
+void launch_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv, int V,
+                         int S, float near, float step, float background, float* out, cudaStream_t s);
+void launch_field_loss_grad(const float* grid, int G, float bound, const float* views, const float* R, const float* t,
+                            const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
+                            const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color, long long* acc,
+                            float* grad, float* loss_out, long long loss_len, cudaStream_t s);
 
 // ---- attention over frames ---------------------------------------------------------------------------------
 struct AttnArgs {
