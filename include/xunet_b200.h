@@ -535,6 +535,55 @@ int xunet_field_loss_grad(const float* grid, int G, float bound, const float* vi
                           const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color, long long* acc,
                           float* grad, float* loss_out, long long loss_len, void* stream);
 
+/* Pose estimation by descent on the denoising loss (ID-Pose / iFusion style): given a conditioning view x at a known camera and a
+ * target view y (S, S, 3), H pose hypotheses for y's camera are fitted side by side, each seeing P noise draws per iteration.
+ * Row b = h P + p of the engine batch (B = H P) is hypothesis h with draw p; n = 3 S^2 values per view.  One iteration is
+ *   xunet_pose_draw -> xunet_forward (train = 0) -> xunet_pose_loss -> xunet_backward_vjp_inputs (dR2, dt2)
+ *   -> xunet_pose_tangent -> xunet_adam_step on the step buffer -> xunet_pose_retract -> the count + 1.
+ * The master poses are fp64 on the device: R (H, 3, 3) cam-to-world, row-major, and t (H, 3).  The tangent coordinates of
+ * hypothesis h are (omega, delta): R' = exp([omega]x) R, t' = exp([omega]x) t + delta, a rotation of the camera about the world
+ * origin (the object's centre in SRN) plus, with translate != 0, a translation; D = 3 (translate = 0) or 6 values per
+ * hypothesis.  i = *iter_dev is the 1-based Adam count (device int64), read at execution time so a replayed graph draws afresh.
+ * Every entry checks its arguments before it launches anything (message starting with the entry's name); no allocation, no
+ * atomics, no host sync, graph-capturable; the results are functions of the inputs alone (fixed bits). */
+#define XUNET_POSE_MAX_T 999                /* timesteps index the 1000-entry cosine-beta tables */
+#define XUNET_POSE_LOSS_CHUNK 4096          /* values per partial sum of xunet_pose_loss */
+#define XUNET_POSE_SMALL_ANGLE2 1e-6        /* |omega|^2 below which xunet_pose_retract uses the Taylor series */
+/* The draws of iteration i: draw p has the hash h_p = xu_mix64(seed * 0x9E3779B97F4A7C15 + i * 0xD1B54A32D192ED03 + p) and
+ *   t_p = t_min + h_p mod (t_max - t_min + 1)                                   (strata == 0: uniform)
+ *   t_p = t_min + floor((2g + 1)(t_max - t_min + 1) / (2 strata)),  g = ((i - 1) P + p) mod strata     (strata > 0: stratified)
+ *   eps_p[k] = the device hash normal of draw k of seed h_p (the sampler's noise, csrc/common.cuh xu_hash_normal).
+ * Every hypothesis shares draw p (common random numbers).  Written: z rows (B, S, S, 3), z_b[k] = fma(sa, y[k], fl(sb eps_p[k]))
+ * with sa = sqrt_ac[t_p], sb = sqrt_1mac[t_p] (xunet_forward_diffusion's rounding); logsnr (B) = logsnr_schedule_cosine(t_p / 1000)
+ * as xunet_forward_diffusion; target (P, S, S, 3) = eps_p (prediction 0) or the v target fl(fl(sa eps) - fl(sb y)) (prediction 1,
+ * xunet_forward_diffusion_v's rounding); t_out (P) int32 when not NULL.  Errors: a NULL required pointer, H < 1, P < 1, S < 1,
+ * H P S^2 >= 2^31 / 3, 0 <= t_min <= t_max <= XUNET_POSE_MAX_T violated, strata < 0, prediction not 0 / 1.  One launch. */
+int xunet_pose_draw(const float* y, int H, int P, int S, int t_min, int t_max, int strata, const long long* iter_dev,
+                    unsigned long long seed, const float* sqrt_ac, const float* sqrt_1mac, int prediction, float* z, float* logsnr,
+                    float* target, int* t_out, void* stream);
+/* The loss of each hypothesis and its seed: with r = fl(out_b - target_p) (out: the forward's output, B rows; target: P rows),
+ *   L_h = (1 / (P n)) sum_p sum_k r^2,  d_out_b = fl(fl32(2 / (P n)) r)   (d_out: B rows, the d_eps of the VJP).
+ * The squares are summed in fp64: per row, chunks of XUNET_POSE_LOSS_CHUNK values (256 thread sums, a fixed shuffle tree, the 8
+ * warp sums in order) into partial (B ceil(n / XUNET_POSE_LOSS_CHUNK) doubles, scratch), then per hypothesis over p and the
+ * chunks in order, divided by P n in fp64 and rounded once to fp32 into loss_out[(i - 1) H + h] when 1 <= i <= loss_len.
+ * Errors: a NULL pointer, H < 1, P < 1, S < 1, H P S^2 >= 2^31 / 3, loss_len < 0.  Two launches. */
+int xunet_pose_loss(const float* out, const float* target, int H, int P, int S, const long long* iter_dev, double* partial,
+                    float* d_out, float* loss_out, long long loss_len, void* stream);
+/* The gradient in tangent coordinates.  dR (B, 3, 3), dt (B, 3): dL/dR2, dL/dt2 of the rows (xunet_backward_vjp_inputs).  In fp64,
+ * G_R = sum_p dR_b and g_t = sum_p dt_b (p ascending), N = G_R R_h^T + g_t t_h^T, and
+ *   g_omega = (N32 - N23, N13 - N31, N21 - N12)   (1-based indices),   g_delta = g_t,
+ * the derivative of L(exp([omega]x) R_h, exp([omega]x) t_h + delta) at 0.  grad (H, D) receives them rounded to fp32, omega first.
+ * Errors: a NULL pointer, H < 1, P < 1, translate not 0 / 1.  One launch. */
+int xunet_pose_tangent(const float* dR, const float* dt, int H, int P, const double* R, const double* t, int translate, float* grad,
+                       void* stream);
+/* The retraction.  step (H, D) fp32 (Adam's update of a zero buffer, i.e. -lr m_hat / (sqrt(v_hat) + eps)) gives omega and delta;
+ * in fp64, theta^2 = |omega|^2, A = sin(theta) / theta and B = 2 sin^2(theta / 2) / theta^2 (theta^2 < XUNET_POSE_SMALL_ANGLE2:
+ * A = 1 - theta^2 / 6 + theta^4 / 120, B = 1/2 - theta^2 / 24 + theta^4 / 720), E = I + A [omega]x + B (omega omega^T - theta^2 I),
+ * R_h <- E R_h, t_h <- E t_h + delta (delta = 0 when translate = 0).  Then R_rows (B, 3, 3) and t_rows (B, 3) of the P rows of
+ * hypothesis h receive fp32(R_h), fp32(t_h), and step is zeroed.  A zero step leaves R and t as they are and only writes the rows.
+ * Errors: a NULL pointer, H < 1, P < 1, translate not 0 / 1.  One launch. */
+int xunet_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows, void* stream);
+
 /* ---- operator-level entry points (parity tests / micro-benchmarks of single kernels) ----
  * dtype as above; tensors channels-last (N,H,W,C). */
 int xunet_op_conv(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y,

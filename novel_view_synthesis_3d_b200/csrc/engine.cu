@@ -1686,6 +1686,58 @@ extern "C" int xunet_field_loss_grad(const float* grid, int G, float bound, cons
   return e == cudaSuccess ? 0 : fail("field_loss_grad: CUDA error: %s", cudaGetErrorString(e));
 }
 
+// The shape checks the pose entries share (include/xunet_b200.h, "Pose estimation"); 0 or the fail() code.
+static int pose_check(const char* what, int H, int P, int S) {
+  if (H < 1 || P < 1 || S < 1) return fail("%s: H = %d, P = %d, S = %d, need all >= 1", what, H, P, S);
+  if ((long long)H * P * S * S >= (1LL << 31) / 3) return fail("%s: H P S^2 = %lld, need H P S^2 < 2^31 / 3", what, (long long)H * P * S * S);
+  return 0;
+}
+
+extern "C" int xunet_pose_draw(const float* y, int H, int P, int S, int t_min, int t_max, int strata, const long long* iter_dev,
+                               unsigned long long seed, const float* sqrt_ac, const float* sqrt_1mac, int prediction, float* z,
+                               float* logsnr, float* target, int* t_out, void* stream) {
+  if (!y || !iter_dev || !sqrt_ac || !sqrt_1mac || !z || !logsnr || !target) return fail("xunet_pose_draw: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_draw", H, P, S)) return rc;
+  if (t_min < 0 || t_min > t_max || t_max > XUNET_POSE_MAX_T)
+    return fail("xunet_pose_draw: t range [%d, %d], need 0 <= t_min <= t_max <= %d", t_min, t_max, XUNET_POSE_MAX_T);
+  if (strata < 0) return fail("xunet_pose_draw: strata = %d, need strata >= 0", strata);
+  if (prediction != 0 && prediction != 1) return fail("xunet_pose_draw: prediction = %d, need 0 (eps) or 1 (v)", prediction);
+  launch_pose_draw(y, H, P, S, t_min, t_max, strata, iter_dev, seed, sqrt_ac, sqrt_1mac, prediction, z, logsnr, target, t_out,
+                   (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("pose_draw: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_pose_loss(const float* out, const float* target, int H, int P, int S, const long long* iter_dev, double* partial,
+                               float* d_out, float* loss_out, long long loss_len, void* stream) {
+  if (!out || !target || !iter_dev || !partial || !d_out || !loss_out) return fail("xunet_pose_loss: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_loss", H, P, S)) return rc;
+  if (loss_len < 0) return fail("xunet_pose_loss: loss_len = %lld, need loss_len >= 0", loss_len);
+  launch_pose_loss(out, target, H, P, S, iter_dev, partial, d_out, loss_out, loss_len, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("pose_loss: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_pose_tangent(const float* dR, const float* dt, int H, int P, const double* R, const double* t, int translate,
+                                  float* grad, void* stream) {
+  if (!dR || !dt || !R || !t || !grad) return fail("xunet_pose_tangent: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_tangent", H, P, 1)) return rc;
+  if (translate != 0 && translate != 1) return fail("xunet_pose_tangent: translate = %d, need 0 or 1", translate);
+  launch_pose_tangent(dR, dt, H, P, R, t, translate, grad, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("pose_tangent: CUDA error: %s", cudaGetErrorString(e));
+}
+
+extern "C" int xunet_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows,
+                                  void* stream) {
+  if (!step || !R || !t || !R_rows || !t_rows) return fail("xunet_pose_retract: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_retract", H, P, 1)) return rc;
+  if (translate != 0 && translate != 1) return fail("xunet_pose_retract: translate = %d, need 0 or 1", translate);
+  launch_pose_retract(step, H, P, translate, R, t, R_rows, t_rows, (cudaStream_t)stream);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : fail("pose_retract: CUDA error: %s", cudaGetErrorString(e));
+}
+
 // ---- operator-level entry points ----------------------------------------------------------------------
 // fp64 reduction scratch of one operator-level call (kernels.h): stream-ordered allocations, released on the call's stream
 struct OpScratch {

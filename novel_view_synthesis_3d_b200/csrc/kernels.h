@@ -198,6 +198,15 @@ void launch_field_loss_grad(const float* grid, int G, float bound, const float* 
                             const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
                             const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color, long long* acc,
                             float* grad, float* loss_out, long long loss_len, cudaStream_t s);
+// xunet_pose_draw / _loss / _tangent / _retract (pose_fit.cu): the loop of pose estimation around the camera gradient
+void launch_pose_draw(const float* y, int H, int P, int S, int t_min, int t_max, int strata, const long long* iter_dev,
+                      unsigned long long seed, const float* sqrt_ac, const float* sqrt_1mac, int prediction, float* z, float* logsnr,
+                      float* target, int* t_out, cudaStream_t s);
+void launch_pose_loss(const float* out, const float* target, int H, int P, int S, const long long* iter_dev, double* partial,
+                      float* d_out, float* loss_out, long long loss_len, cudaStream_t s);
+void launch_pose_tangent(const float* dR, const float* dt, int H, int P, const double* R, const double* t, int translate, float* grad,
+                         cudaStream_t s);
+void launch_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows, cudaStream_t s);
 
 // ---- attention over frames ---------------------------------------------------------------------------------
 struct AttnArgs {
