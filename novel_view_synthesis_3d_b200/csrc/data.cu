@@ -20,6 +20,16 @@
 
 #define SRN_THREADS 256
 
+// xunet_srn_batch_distill: the draw of xunet_srn_batch with t = grid_t[m], m = (sample hash) mod n_grid, cond_mask 1, no
+// target, and the sample's inputs copied into the teacher's `copies` row blocks
+struct XuDistillDraw {
+  xunet_batch teacher;    // x, z, logsnr, R1, t1, R2, t2, K of the teacher's batch (copies * B rows; cond_mask, rays unused)
+  int copies;             // 2: a guided [cond ; uncond] teacher batch, 1: an unguided one
+  const int* grid_t;      // the student's timesteps, loop order
+  int n_grid;
+  int* m_out;             // (B) the drawn grid positions
+};
+
 // key of round r of the permutation of epoch `epoch`
 __host__ __device__ __forceinline__ uint64_t srn_round_key(uint64_t seed, uint64_t epoch, int r) {
   return xu_mix64(xu_mix64(seed ^ 0x243F6A8885A308D3ULL) + epoch * 4ULL + (uint64_t)r);
@@ -244,22 +254,59 @@ static void launch_srn_batch_target(const xunet_srn_store& st, const long long* 
               sqrt_ac, sqrt_1mac, p_uncond, snr_weight, out, noise, loss_weight, idx_out, t_out, vec, v_out, dd);
 }
 
-void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
-                      int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
-                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, float* v_out,
-                      cudaStream_t s) {
-  const XuDistillDraw none = {};
-  if (v_out != nullptr)
-    launch_srn_batch_target<XU_TARGET_V>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight,
-                                         out, noise, loss_weight, idx_out, t_out, v_out, none, s);
-  else
-    launch_srn_batch_target<XU_TARGET_EPS>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond,
-                                           snr_weight, out, noise, loss_weight, idx_out, t_out, v_out, none, s);
+// the argument checks of xunet_srn_batch / _v; the ε buffer `noise` is checked by the caller (optional in the v form)
+static int srn_batch_check(const char* fn, const xunet_srn_store* store, const long long* step_dev, int j, int k, int rank,
+                           int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const xunet_batch* out) {
+  if (!store || !step_dev || !sqrt_ac || !sqrt_1mac || !out || !store->pixels || !store->R || !store->t || !store->K ||
+      !store->first || !store->count || !store->item_inst || !out->x || !out->z || !out->logsnr || !out->R1 || !out->t1 ||
+      !out->R2 || !out->t2 || !out->K || !out->cond_mask)
+    return xu_fail("%s: NULL pointer argument", fn);
+  if (B < 1 || k < 1 || world < 1) return xu_fail("%s: B = %d, k = %d, world = %d, need all >= 1", fn, B, k, world);
+  if (rank < 0 || rank >= world || j < 0 || j >= k)
+    return xu_fail("%s: rank = %d of world = %d, j = %d of k = %d out of range", fn, rank, world, j, k);
+  if (store->n_items < 1 || store->n_instances < 1 || store->S < 1)
+    return xu_fail("%s: empty store (n_items = %lld, n_instances = %d, S = %d)", fn, store->n_items, store->n_instances, store->S);
+  if (store->pixel_kind != XUNET_PIXELS_U8 && store->pixel_kind != XUNET_PIXELS_F32)
+    return xu_fail("%s: unknown pixel_kind %d", fn, store->pixel_kind);
+  return 0;
 }
 
-void launch_srn_batch_distill(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k,
-                              int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const xunet_batch& out,
-                              const XuDistillDraw& dd, int* idx_out, int* t_out, cudaStream_t s) {
-  launch_srn_batch_target<XU_TARGET_DISTILL>(st, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, 0.f, nullptr, out,
-                                             nullptr, nullptr, idx_out, t_out, nullptr, dd, s);
+extern "C" int xunet_srn_batch(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
+                               int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
+                               const float* snr_weight, const xunet_batch* out, float* noise, float* loss_weight, int* idx_out,
+                               int* t_out, void* stream) {
+  if (!noise) return xu_fail("xunet_srn_batch: NULL pointer argument");
+  if (const int rc = srn_batch_check("xunet_srn_batch", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out)) return rc;
+  launch_srn_batch_target<XU_TARGET_EPS>(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight,
+                                         *out, noise, loss_weight, idx_out, t_out, nullptr, XuDistillDraw{}, (cudaStream_t)stream);
+  return xu_launched("srn_batch");
+}
+
+extern "C" int xunet_srn_batch_v(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
+                                 int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
+                                 const float* snr_weight, const xunet_batch* out, float* noise, float* v_out,
+                                 float* loss_weight, int* idx_out, int* t_out, void* stream) {
+  if (!v_out) return xu_fail("xunet_srn_batch_v: NULL pointer argument");
+  if (const int rc = srn_batch_check("xunet_srn_batch_v", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out)) return rc;
+  launch_srn_batch_target<XU_TARGET_V>(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight,
+                                       *out, noise, loss_weight, idx_out, t_out, v_out, XuDistillDraw{}, (cudaStream_t)stream);
+  return xu_launched("srn_batch_v");
+}
+
+extern "C" int xunet_srn_batch_distill(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j,
+                                       int k, int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac,
+                                       const int* grid_t, int n_grid, const xunet_batch* out, const xunet_batch* teacher,
+                                       int teacher_copies, int* m_out, int* idx_out, int* t_out, void* stream) {
+  if (!grid_t || !teacher || !m_out || !teacher->x || !teacher->z || !teacher->logsnr || !teacher->R1 || !teacher->t1 ||
+      !teacher->R2 || !teacher->t2 || !teacher->K)
+    return xu_fail("xunet_srn_batch_distill: NULL pointer argument");
+  if (const int rc = srn_batch_check("xunet_srn_batch_distill", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out))
+    return rc;
+  if (n_grid < 1) return xu_fail("xunet_srn_batch_distill: n_grid = %d, need >= 1", n_grid);
+  if (teacher_copies != 1 && teacher_copies != 2)
+    return xu_fail("xunet_srn_batch_distill: teacher_copies = %d, need 1 or 2", teacher_copies);
+  const XuDistillDraw dd = {*teacher, teacher_copies, grid_t, n_grid, m_out};
+  launch_srn_batch_target<XU_TARGET_DISTILL>(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, 0.f, nullptr,
+                                             *out, nullptr, nullptr, idx_out, t_out, nullptr, dd, (cudaStream_t)stream);
+  return xu_launched("srn_batch_distill");
 }

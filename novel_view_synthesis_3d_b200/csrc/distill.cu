@@ -54,17 +54,31 @@ __global__ void __launch_bounds__(256) distill_target_kernel(const float* __rest
   v_out[i] = __fdiv_rn(__fsub_rn(__fmul_rn(g[2], zt), xt), g[3]);
 }
 
-void launch_distill_teacher_step(const float* out_t, float w, int copies, const float* ttab, const int* m_dev, int B,
-                                 long long per, float* tz, float* tlogsnr, cudaStream_t s) {
+extern "C" int xunet_distill_teacher_step(const float* out_t, float w, int teacher_copies, const float* teacher_table,
+                                          const int* m_dev, int B, long long per, const xunet_batch* teacher, void* stream) {
+  if (!out_t || !teacher_table || !m_dev || !teacher || !teacher->z || !teacher->logsnr)
+    return xu_fail("xunet_distill_teacher_step: NULL pointer argument");
+  if (B < 1 || per < 1) return xu_fail("xunet_distill_teacher_step: B = %d, per = %lld, need both >= 1", B, per);
+  if (teacher_copies != 1 && teacher_copies != 2)
+    return xu_fail("xunet_distill_teacher_step: teacher_copies = %d, need 1 or 2", teacher_copies);
   const long long n = (long long)B * per;
-  const int grid = cdiv(n > (long long)B * copies ? n : (long long)B * copies, 256);
-  xu_launch(copies == 2 ? distill_teacher_step_kernel<true> : distill_teacher_step_kernel<false>, grid, 256, 0, s, out_t, w,
-            ttab, m_dev, per, n, B, copies, tz, tlogsnr);
+  const int grid = cdiv(n > (long long)B * teacher_copies ? n : (long long)B * teacher_copies, 256);
+  xu_launch(teacher_copies == 2 ? distill_teacher_step_kernel<true> : distill_teacher_step_kernel<false>, grid, 256, 0,
+            (cudaStream_t)stream, out_t, w, teacher_table, m_dev, per, n, B, teacher_copies, const_cast<float*>(teacher->z),
+            const_cast<float*>(teacher->logsnr));
+  return xu_launched("distill_teacher_step");
 }
 
-void launch_distill_target(const float* out_t, float w, int copies, const float* ttab, const float* gtab, const int* m_dev,
-                           const float* z_t, const float* tz, int B, long long per, float* v_out, cudaStream_t s) {
+extern "C" int xunet_distill_target(const float* out_t, float w, int teacher_copies, const float* teacher_table,
+                                    const float* target_table, const int* m_dev, const float* z_t, const float* teacher_z, int B,
+                                    long long per, float* v_out, void* stream) {
+  if (!out_t || !teacher_table || !target_table || !m_dev || !z_t || !teacher_z || !v_out)
+    return xu_fail("xunet_distill_target: NULL pointer argument");
+  if (B < 1 || per < 1) return xu_fail("xunet_distill_target: B = %d, per = %lld, need both >= 1", B, per);
+  if (teacher_copies != 1 && teacher_copies != 2)
+    return xu_fail("xunet_distill_target: teacher_copies = %d, need 1 or 2", teacher_copies);
   const long long n = (long long)B * per;
-  xu_launch(copies == 2 ? distill_target_kernel<true> : distill_target_kernel<false>, cdiv(n, 256), 256, 0, s, out_t, w, ttab,
-            gtab, m_dev, z_t, tz, per, n, v_out);
+  xu_launch(teacher_copies == 2 ? distill_target_kernel<true> : distill_target_kernel<false>, cdiv(n, 256), 256, 0,
+            (cudaStream_t)stream, out_t, w, teacher_table, target_table, m_dev, z_t, teacher_z, per, n, v_out);
+  return xu_launched("distill_target");
 }

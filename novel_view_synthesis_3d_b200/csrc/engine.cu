@@ -1,4 +1,7 @@
-// engine.cu -- static execution plan of the X-UNet (model/xunet.py:218-280) and the C-ABI of include/xunet_b200.h.
+// engine.cu -- static execution plan of the X-UNet (model/xunet.py:218-280) and its entries of include/xunet_b200.h:
+// create, introspection, forward, backward, kernel counting and the gradient-bucket hook, plus the operator-level
+// xunet_op_* entries, which share the plan's launch builders.  The C error state (xu_fail, xunet_last_error) lives here
+// too.  Entries that run no plan (Adam, samplers, data, distillation, metrics, field, pose) sit beside their kernels.
 //
 // A config + (B,S,dtype) is compiled ONCE into a flat list of tensor descriptors (arena offsets into the
 // caller-owned workspace) and op descriptors; forward() walks the list, backward() walks it in reverse with
@@ -20,12 +23,16 @@
 #include <vector>
 
 static thread_local char g_err[512] = "";
-static int fail(const char* fmt, ...) {
+int xu_fail(const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
   return 1;
+}
+int xu_launched(const char* what) {
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : xu_fail("%s: CUDA error: %s", what, cudaGetErrorString(e));
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
 extern "C" int xunet_version(void) { return 111; }
@@ -537,7 +544,7 @@ struct Builder {
       }
       if (i != 0) h = rblock(h, semb[i - 1], RS_UP);
     }
-    if (!hs.empty()) return fail("internal: skip stack not empty");
+    if (!hs.empty()) return xu_fail("internal: skip stack not empty");
     // ---- head  :275-280
     mark_block();
     long long g, b;
@@ -675,10 +682,10 @@ struct Builder {
       }
       // emb_bwd_kernel stores grad(pose-embedding level): each level must feed nothing but its own OP_EMB
       for (const Op& o : H.ops)
-        if (o.kind == OP_EMB && o.acc_x) return fail("internal: a pose-embedding level has a gradient writer besides its OP_EMB");
+        if (o.kind == OP_EMB && o.acc_x) return xu_fail("internal: a pose-embedding level has a gradient writer besides its OP_EMB");
     }
     for (const Op& o : H.ops)
-      if (o.kind == OP_GN && o.cs_a < 0) return fail("internal: a GroupNorm input has no producer-emitted statistics");
+      if (o.kind == OP_GN && o.cs_a < 0) return xu_fail("internal: a GroupNorm input has no producer-emitted statistics");
     return 0;
   }
 };
@@ -875,8 +882,8 @@ static int forward_impl(Ctx& c, float* eps_out) {
     }
   }
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("forward: CUDA error: %s", cudaGetErrorString(e));
-  if (xu_kernel_error()[0]) return fail("forward: %s", xu_kernel_error());
+  if (e != cudaSuccess) return xu_fail("forward: CUDA error: %s", cudaGetErrorString(e));
+  if (xu_kernel_error()[0]) return xu_fail("forward: %s", xu_kernel_error());
   return 0;
 }
 
@@ -1026,8 +1033,8 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
     bucket_end = 0;
   }
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("backward: CUDA error: %s", cudaGetErrorString(e));
-  if (xu_kernel_error()[0]) return fail("backward: %s", xu_kernel_error());
+  if (e != cudaSuccess) return xu_fail("backward: CUDA error: %s", cudaGetErrorString(e));
+  if (xu_kernel_error()[0]) return xu_fail("backward: %s", xu_kernel_error());
   return 0;
 }
 
@@ -1037,25 +1044,25 @@ static int backward_impl(Ctx& c, const float* noise, float* loss_out) {
 // C-ABI
 // ======================================================================================================
 extern "C" int xunet_create(const xunet_config* cfg, int batch, int side, int dtype, int training, xunet_handle** out) {
-  if (!cfg || !out) return fail("xunet_create: null argument");
-  if (dtype != XUNET_DTYPE_F32 && dtype != XUNET_DTYPE_BF16) return fail("xunet_create: bad dtype %d", dtype);
-  if (batch < 1 || side < 1) return fail("xunet_create: bad batch/side");
-  if (cfg->n_levels < 1 || cfg->n_levels > XUNET_MAX_LEVELS) return fail("xunet_create: n_levels out of range");
-  if (cfg->n_attn_resolutions < 0 || cfg->n_attn_resolutions > XUNET_MAX_LEVELS) return fail("xunet_create: bad attn_resolutions");
-  if (cfg->ch % 32 != 0) return fail("xunet_create: ch must be a multiple of 32 (GroupNorm(32), model/xunet.py:51)");
-  if (cfg->emb_ch % 4 != 0 || cfg->emb_ch < 4) return fail("xunet_create: emb_ch must be a multiple of 4");
-  if (side % (1 << (cfg->n_levels - 1)) != 0) return fail("xunet_create: side must be divisible by 2^(levels-1)");
-  if (cfg->dropout < 0.f || cfg->dropout >= 1.f) return fail("xunet_create: dropout must be in [0,1)");
+  if (!cfg || !out) return xu_fail("xunet_create: null argument");
+  if (dtype != XUNET_DTYPE_F32 && dtype != XUNET_DTYPE_BF16) return xu_fail("xunet_create: bad dtype %d", dtype);
+  if (batch < 1 || side < 1) return xu_fail("xunet_create: bad batch/side");
+  if (cfg->n_levels < 1 || cfg->n_levels > XUNET_MAX_LEVELS) return xu_fail("xunet_create: n_levels out of range");
+  if (cfg->n_attn_resolutions < 0 || cfg->n_attn_resolutions > XUNET_MAX_LEVELS) return xu_fail("xunet_create: bad attn_resolutions");
+  if (cfg->ch % 32 != 0) return xu_fail("xunet_create: ch must be a multiple of 32 (GroupNorm(32), model/xunet.py:51)");
+  if (cfg->emb_ch % 4 != 0 || cfg->emb_ch < 4) return xu_fail("xunet_create: emb_ch must be a multiple of 4");
+  if (side % (1 << (cfg->n_levels - 1)) != 0) return xu_fail("xunet_create: side must be divisible by 2^(levels-1)");
+  if (cfg->dropout < 0.f || cfg->dropout >= 1.f) return xu_fail("xunet_create: dropout must be in [0,1)");
   for (int i = 0; i < cfg->n_levels; ++i) {
     int C = cfg->ch * cfg->ch_mult[i];
-    if (cfg->ch_mult[i] < 1) return fail("xunet_create: ch_mult must be >= 1");
+    if (cfg->ch_mult[i] < 1) return xu_fail("xunet_create: ch_mult must be >= 1");
     int res = side >> i;
     bool at = false;
     for (int k = 0; k < cfg->n_attn_resolutions; ++k) at |= cfg->attn_resolutions[k] == res;
     if (at) {
-      if (C % cfg->attn_heads != 0) return fail("xunet_create: channels not divisible by attn_heads");
+      if (C % cfg->attn_heads != 0) return xu_fail("xunet_create: channels not divisible by attn_heads");
       int hd = C / cfg->attn_heads;
-      if (hd != 16 && hd != 32 && hd != 64 && hd != 128) return fail("xunet_create: head_dim %d unsupported (16/32/64/128)", hd);
+      if (hd != 16 && hd != 32 && hd != 64 && hd != 128) return xu_fail("xunet_create: head_dim %d unsupported (16/32/64/128)", hd);
     }
   }
   xunet_handle* h = new xunet_handle();
@@ -1078,7 +1085,7 @@ extern "C" long long xunet_param_count(const xunet_handle* h) { return h->nparam
 extern "C" int xunet_param_leaves(const xunet_handle* h) { return (int)h->leaves.size(); }
 extern "C" int xunet_param_leaf(const xunet_handle* h, int i, const char** name, int* ndim, long long shape[5],
                                 long long* offset) {
-  if (i < 0 || i >= (int)h->leaves.size()) return fail("xunet_param_leaf: index out of range");
+  if (i < 0 || i >= (int)h->leaves.size()) return xu_fail("xunet_param_leaf: index out of range");
   const Leaf& l = h->leaves[i];
   *name = l.name.c_str();
   *ndim = l.ndim;
@@ -1090,7 +1097,7 @@ extern "C" long long xunet_workspace_bytes(const xunet_handle* h) { return h->ws
 extern "C" int xunet_tap_count(const xunet_handle* h) { return (int)h->taps.size() + 1; }
 extern "C" int xunet_tap(const xunet_handle* h, int i, const char** name, int dims[4], long long* byte_offset, int* is_f32,
                          long long* grad_byte_offset) {
-  if (i < 0 || i > (int)h->taps.size()) return fail("xunet_tap: index out of range");
+  if (i < 0 || i > (int)h->taps.size()) return xu_fail("xunet_tap: index out of range");
   if (i == (int)h->taps.size()) {  // the fp32 log-SNR embedding lives in aux storage
     *name = "logsnr_emb";
     dims[0] = h->B; dims[1] = 1; dims[2] = 1; dims[3] = h->cfg.emb_ch;
@@ -1117,11 +1124,11 @@ extern "C" int xunet_plan_launch_count(const xunet_handle* h) {
 
 // every field comes from the op and the helpers the launch code uses (run_conv_fwd / run_conv_bwd, forward_impl's OP_ATTN)
 extern "C" int xunet_plan_launch(const xunet_handle* h, int i, xunet_launch_info* out) {
-  if (!h || !out) return fail("xunet_plan_launch: null argument");
+  if (!h || !out) return xu_fail("xunet_plan_launch: null argument");
   int k = -1;
   for (size_t j = 0; j < h->ops.size() && i >= 0; ++j)
     if (is_launch(h->ops[j]) && i-- == 0) k = (int)j;
-  if (k < 0) return fail("xunet_plan_launch: index out of range");
+  if (k < 0) return xu_fail("xunet_plan_launch: index out of range");
   const Op& o = h->ops[k];
   const Tensor& x = h->tensors[o.x];
   const Tensor& y = h->tensors[o.y];
@@ -1180,11 +1187,11 @@ extern "C" int xunet_plan_op_count(const xunet_handle* h) {
 
 // every field comes from the op and the helpers forward_impl / backward_impl launch it with
 extern "C" int xunet_plan_op(const xunet_handle* h, int i, xunet_op_info* out) {
-  if (!h || !out) return fail("xunet_plan_op: null argument");
+  if (!h || !out) return xu_fail("xunet_plan_op: null argument");
   int k = -1;
   for (size_t j = 0; j < h->ops.size() && i >= 0; ++j)
     if (plan_op_kind(h->ops[j]) >= 0 && i-- == 0) k = (int)j;
-  if (k < 0) return fail("xunet_plan_op: index out of range");
+  if (k < 0) return xu_fail("xunet_plan_op: index out of range");
   const Op& o = h->ops[k];
   const bool tr = h->training != 0;
   xunet_op_info r;
@@ -1252,8 +1259,8 @@ extern "C" int xunet_plan_op(const xunet_handle* h, int i, xunet_op_info* out) {
 
 extern "C" int xunet_forward(xunet_handle* h, const float* params, const xunet_batch* batch, int train,
                              const unsigned long long* seed_dev, void* workspace, float* eps_out, void* stream) {
-  if (!h || !params || !batch || !workspace) return fail("xunet_forward: null argument");
-  if (train && h->cfg.dropout > 0.f && !seed_dev) return fail("xunet_forward: train=1 with dropout needs seed_dev");
+  if (!h || !params || !batch || !workspace) return xu_fail("xunet_forward: null argument");
+  if (train && h->cfg.dropout > 0.f && !seed_dev) return xu_fail("xunet_forward: train=1 with dropout needs seed_dev");
   xu_set_kernel_error("");
   Ctx c{h, params, nullptr, (char*)workspace, batch, seed_dev, train ? 1 : 0, (cudaStream_t)stream};
   XuDetBind bind(h->det);
@@ -1263,13 +1270,13 @@ extern "C" int xunet_forward(xunet_handle* h, const float* params, const xunet_b
 }
 
 extern "C" int xunet_set_static_conditioning(xunet_handle* h, int on) {
-  if (!h) return fail("xunet_set_static_conditioning: null handle");
+  if (!h) return xu_fail("xunet_set_static_conditioning: null handle");
   h->static_cond = on ? 1 : 0;
   return 0;
 }
 
 extern "C" int xunet_set_grad_bucket_callback(xunet_handle* h, xunet_bucket_fn fn, void* user, long long min_bucket_bytes) {
-  if (!h) return fail("xunet_set_grad_bucket_callback: null handle");
+  if (!h) return xu_fail("xunet_set_grad_bucket_callback: null handle");
   h->bucket_fn = fn;
   h->bucket_user = user;
   h->bucket_pts.clear();
@@ -1286,81 +1293,72 @@ extern "C" int xunet_set_grad_bucket_callback(xunet_handle* h, xunet_bucket_fn f
 
 extern "C" int xunet_grad_bucket_count(const xunet_handle* h) { return h ? (int)h->bucket_pts.size() + 1 : 0; }
 
+// The preamble of every backward entry (fn: its name in the messages): null arguments, a training handle and a forward to
+// differentiate, then backward_impl in the engine's fp64 scratch.  in == nullptr: the loss backward, seeded from noise and
+// writing loss_out (the mean-squared loss with mse, weighted by loss_weight); else the VJP of d_eps, with the input and
+// camera gradients `in` asks for.
+static int backward_entry(const char* fn, xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
+                          const float* d_eps, const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
+                          int accumulate, int mse, const float* loss_weight, const xunet_input_grads* in, void* stream) {
+  if (!h || !params || !batch || !workspace || !grads || (in ? !d_eps : (!noise || !loss_out)))
+    return xu_fail("%s: null argument", fn);
+  if (!h->training) return xu_fail("%s: handle was created with training=0", fn);
+  if (!h->forward_done_train) return xu_fail("%s: call xunet_forward first", fn);
+  const bool cams = in && (in->dR1 || in->dt1 || in->dR2 || in->dt2 || in->dK);
+  if (cams && !in->d_rays) return xu_fail("%s: camera gradients need d_rays", fn);
+  if (cams && batch->rays) return xu_fail("%s: camera gradients need generated rays (batch->rays == NULL)", fn);
+  xu_set_kernel_error("");
+  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
+  c.acc_grads = accumulate ? 1 : 0;
+  c.mse = mse;
+  c.loss_weight = loss_weight;
+  c.d_eps = d_eps;
+  if (in) {
+    c.dx = in->dx;
+    c.dz = in->dz;
+    c.cam = in->d_rays ? in : nullptr;
+  }
+  XuDetBind bind(h->det);
+  return backward_impl(c, noise, loss_out);
+}
+
 extern "C" int xunet_backward(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
                               const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
                               void* stream) {
-  if (!h || !params || !batch || !noise || !workspace || !grads || !loss_out) return fail("xunet_backward: null argument");
-  if (!h->training) return fail("xunet_backward: handle was created with training=0");
-  if (!h->forward_done_train) return fail("xunet_backward: call xunet_forward first");
-  xu_set_kernel_error("");
-  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
-  XuDetBind bind(h->det);
-  return backward_impl(c, noise, loss_out);
+  return backward_entry("xunet_backward", h, params, batch, noise, nullptr, seed_dev, workspace, grads, loss_out, 0, 0, nullptr,
+                        nullptr, stream);
 }
 
 extern "C" int xunet_backward_accumulate(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
                                          const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
                                          void* stream) {
-  if (!h || !params || !batch || !noise || !workspace || !grads || !loss_out) return fail("xunet_backward_accumulate: null argument");
-  if (!h->training) return fail("xunet_backward_accumulate: handle was created with training=0");
-  if (!h->forward_done_train) return fail("xunet_backward_accumulate: call xunet_forward first");
-  xu_set_kernel_error("");
-  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
-  c.acc_grads = 1;
-  XuDetBind bind(h->det);
-  return backward_impl(c, noise, loss_out);
+  return backward_entry("xunet_backward_accumulate", h, params, batch, noise, nullptr, seed_dev, workspace, grads, loss_out, 1, 0,
+                        nullptr, nullptr, stream);
 }
 
 extern "C" int xunet_backward_mse(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
                                   const float* loss_weight, const unsigned long long* seed_dev, void* workspace, float* grads,
                                   float* loss_out, int accumulate, void* stream) {
-  if (!h || !params || !batch || !noise || !workspace || !grads || !loss_out) return fail("xunet_backward_mse: null argument");
-  if (!h->training) return fail("xunet_backward_mse: handle was created with training=0");
-  if (!h->forward_done_train) return fail("xunet_backward_mse: call xunet_forward first");
-  xu_set_kernel_error("");
-  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
-  c.acc_grads = accumulate ? 1 : 0;
-  c.mse = 1;
-  c.loss_weight = loss_weight;
-  XuDetBind bind(h->det);
-  return backward_impl(c, noise, loss_out);
-}
-
-static int backward_vjp(const char* fn, xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
-                        const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate,
-                        const xunet_input_grads& out, void* stream) {
-  if (!h || !params || !batch || !d_eps || !workspace || !grads) return fail("%s: null argument", fn);
-  if (!h->training) return fail("%s: handle was created with training=0", fn);
-  if (!h->forward_done_train) return fail("%s: call xunet_forward first", fn);
-  const bool cams = out.dR1 || out.dt1 || out.dR2 || out.dt2 || out.dK;
-  if (cams && !out.d_rays) return fail("%s: camera gradients need d_rays", fn);
-  if (cams && batch->rays) return fail("%s: camera gradients need generated rays (batch->rays == NULL)", fn);
-  xu_set_kernel_error("");
-  Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->forward_done_train == 1 ? 1 : 0, (cudaStream_t)stream};
-  c.acc_grads = accumulate ? 1 : 0;
-  c.d_eps = d_eps;
-  c.dx = out.dx;
-  c.dz = out.dz;
-  c.cam = out.d_rays ? &out : nullptr;
-  XuDetBind bind(h->det);
-  return backward_impl(c, nullptr, nullptr);
+  return backward_entry("xunet_backward_mse", h, params, batch, noise, nullptr, seed_dev, workspace, grads, loss_out, accumulate,
+                        1, loss_weight, nullptr, stream);
 }
 
 extern "C" int xunet_backward_vjp(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
                                   const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate, float* dx,
                                   float* dz, void* stream) {
-  xunet_input_grads out{};
-  out.dx = dx;
-  out.dz = dz;
-  return backward_vjp("xunet_backward_vjp", h, params, batch, d_eps, seed_dev, workspace, grads, accumulate, out, stream);
+  xunet_input_grads in{};
+  in.dx = dx;
+  in.dz = dz;
+  return backward_entry("xunet_backward_vjp", h, params, batch, nullptr, d_eps, seed_dev, workspace, grads, nullptr, accumulate,
+                        0, nullptr, &in, stream);
 }
 
 extern "C" int xunet_backward_vjp_inputs(xunet_handle* h, const float* params, const xunet_batch* batch, const float* d_eps,
                                          const unsigned long long* seed_dev, void* workspace, float* grads, int accumulate,
                                          const xunet_input_grads* out, void* stream) {
-  xunet_input_grads none{};
-  return backward_vjp("xunet_backward_vjp_inputs", h, params, batch, d_eps, seed_dev, workspace, grads, accumulate,
-                      out ? *out : none, stream);
+  const xunet_input_grads none{};
+  return backward_entry("xunet_backward_vjp_inputs", h, params, batch, nullptr, d_eps, seed_dev, workspace, grads, nullptr,
+                        accumulate, 0, nullptr, out ? out : &none, stream);
 }
 
 static int count_kernel_nodes(cudaGraph_t g) {
@@ -1379,9 +1377,9 @@ static int count_kernel_nodes(cudaGraph_t g) {
 extern "C" int xunet_count_kernels(xunet_handle* h, const float* params, const xunet_batch* batch, const float* noise,
                                    const unsigned long long* seed_dev, void* workspace, float* grads, float* loss_out,
                                    int* n_forward, int* n_backward) {
-  if (!h || !params || !batch || !workspace || !n_forward) return fail("xunet_count_kernels: null argument");
+  if (!h || !params || !batch || !workspace || !n_forward) return xu_fail("xunet_count_kernels: null argument");
   cudaStream_t s;
-  if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return fail("count_kernels: stream");
+  if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return xu_fail("count_kernels: stream");
   xu_set_kernel_error("");
   int rc = 0;
   XuDetBind bind(h->det);
@@ -1390,352 +1388,17 @@ extern "C" int xunet_count_kernels(xunet_handle* h, const float* params, const x
   for (int pass = 0; pass < 2 && rc == 0; ++pass) {
     if (pass == 1 && (!n_backward || !h->training || !noise || !grads || !loss_out)) break;
     cudaGraph_t g = nullptr;
-    if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { rc = fail("count_kernels: begin capture"); break; }
+    if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { rc = xu_fail("count_kernels: begin capture"); break; }
     Ctx c{h, params, grads, (char*)workspace, batch, seed_dev, h->training ? 1 : 0, s};
     int r = pass == 0 ? forward_impl(c, nullptr) : backward_impl(c, noise, loss_out);
     cudaError_t e = cudaStreamEndCapture(s, &g);
-    if (r != 0 || e != cudaSuccess || !g) { rc = r ? r : fail("count_kernels: end capture: %s", cudaGetErrorString(e)); if (g) cudaGraphDestroy(g); break; }
+    if (r != 0 || e != cudaSuccess || !g) { rc = r ? r : xu_fail("count_kernels: end capture: %s", cudaGetErrorString(e)); if (g) cudaGraphDestroy(g); break; }
     (pass == 0 ? *n_forward : *n_backward) = count_kernel_nodes(g);
     cudaGraphDestroy(g);
   }
   cudaStreamDestroy(s);
   h->bucket_fn = saved_fn;
   return rc;
-}
-
-extern "C" int xunet_adam_step(float* params, const float* grads, float* m, float* v, long long n, long long step,
-                               const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
-                               void* stream) {
-  if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_step: bad argument");
-  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, nullptr, 0.0, nullptr, 0.0, 0, nullptr,
-              (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("adam: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_adam_ema_step(float* params, const float* grads, float* m, float* v, float* ema, long long n,
-                                   long long step, const long long* step_dev, double lr, double b1, double b2, double eps,
-                                   double grad_scale, double ema_decay, void* stream) {
-  if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_ema_step: bad argument");
-  if (!ema) return fail("xunet_adam_ema_step: ema is NULL (use xunet_adam_step without an EMA)");
-  if (!(ema_decay >= 0.0 && ema_decay <= 1.0)) return fail("xunet_adam_ema_step: ema_decay %g outside [0, 1]", ema_decay);
-  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema_decay, nullptr, 0.0, 0, nullptr,
-              (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("adam_ema: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_grad_global_norm(const float* grads, long long n, double grad_scale, double* scratch, float* norm_out,
-                                      void* stream) {
-  if (!grads || !scratch || !norm_out || n < 0) return fail("xunet_grad_global_norm: bad argument");
-  launch_grad_global_norm(grads, n, grad_scale, scratch, norm_out, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("grad_global_norm: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, float* ema, long long n,
-                                    long long step, const long long* step_dev, double lr, double b1, double b2, double eps,
-                                    double grad_scale, double ema_decay, const float* norm_dev, double max_norm,
-                                    long long warmup_steps, long long* skipped_dev, void* stream) {
-  if (!params || !grads || !m || !v || n < 0) return fail("xunet_adam_clip_step: bad argument");
-  if (ema && !(ema_decay >= 0.0 && ema_decay <= 1.0)) return fail("xunet_adam_clip_step: ema_decay %g outside [0, 1]", ema_decay);
-  if (warmup_steps < 0) return fail("xunet_adam_clip_step: warmup_steps %lld < 0", warmup_steps);
-  if (norm_dev) {
-    if (!(max_norm > 0.0)) return fail("xunet_adam_clip_step: max_norm %g must be > 0", max_norm);
-    if (!skipped_dev) return fail("xunet_adam_clip_step: skipped_dev is NULL (needed with norm_dev)");
-  }
-  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema ? ema_decay : 0.0, norm_dev,
-              max_norm, warmup_steps, skipped_dev, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("adam_clip: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* table,
-                                        const int* pos_dev, const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2,
-                                        int batch2, void* stream) {
-  if (!eps2 || !z || !table || !pos_dev || !seed_dev || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0) return fail("xunet_sampler_step_table: bad argument");
-  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, nullptr, true,
-                            (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("sampler_step_table: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_sampler_step_multistep(const float* eps2, float* z, const float* noise, long long n, float w,
-                                            const float* table, const int* pos_dev, const unsigned long long* seed_dev,
-                                            float* x0_hist, float* next_z2, float* next_logsnr2, int batch2, void* stream) {
-  if (!eps2 || !z || !table || !pos_dev || !seed_dev || !x0_hist || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0)
-    return fail("xunet_sampler_step_multistep: bad argument");
-  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, true,
-                            (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("sampler_step_multistep: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w,
-                                          const float* table, const int* pos_dev, const unsigned long long* seed_dev,
-                                          float* x0_hist, int batch, double percentile, float* scale_out, float* next_z2,
-                                          float* next_logsnr2, int batch2, void* stream) {
-  if (!eps2 || !z || !table || !pos_dev || !seed_dev || !next_z2 || !next_logsnr2)
-    return fail("xunet_sampler_step_dynamic: NULL pointer argument");
-  if (n <= 0 || batch2 <= 0) return fail("xunet_sampler_step_dynamic: n = %lld, batch2 = %d, need both >= 1", n, batch2);
-  if (batch < 1) return fail("xunet_sampler_step_dynamic: batch = %d, need batch >= 1", batch);
-  if (n % batch != 0) return fail("xunet_sampler_step_dynamic: n = %lld is not a multiple of batch = %d", n, batch);
-  if (n / batch > XUNET_SAMPLER_DYN_MAX_PER)
-    return fail("xunet_sampler_step_dynamic: %lld values per view, more than XUNET_SAMPLER_DYN_MAX_PER = %d", n / batch,
-                XUNET_SAMPLER_DYN_MAX_PER);
-  if (!(percentile > 0.0 && percentile <= 1.0))
-    return fail("xunet_sampler_step_dynamic: percentile %g outside (0, 1]", percentile);
-  launch_sampler_step_dynamic(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, batch,
-                              percentile, scale_out, true, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("sampler_step_dynamic: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_sampler_step_cond(const float* out, float* z, const float* noise, long long n, const float* table,
-                                       const int* pos_dev, const unsigned long long* seed_dev, float* x0_hist, int batch,
-                                       double percentile, float* scale_out, float* next_z, float* next_logsnr, void* stream) {
-  if (!out || !z || !table || !pos_dev || !seed_dev || !next_z || !next_logsnr)
-    return fail("xunet_sampler_step_cond: NULL pointer argument");
-  if (n <= 0 || batch < 1) return fail("xunet_sampler_step_cond: n = %lld, batch = %d, need both >= 1", n, batch);
-  if (n % batch != 0) return fail("xunet_sampler_step_cond: n = %lld is not a multiple of batch = %d", n, batch);
-  if (percentile != 0.0) {
-    if (n / batch > XUNET_SAMPLER_DYN_MAX_PER)
-      return fail("xunet_sampler_step_cond: %lld values per view, more than XUNET_SAMPLER_DYN_MAX_PER = %d", n / batch,
-                  XUNET_SAMPLER_DYN_MAX_PER);
-    if (!(percentile > 0.0 && percentile <= 1.0))
-      return fail("xunet_sampler_step_cond: percentile %g outside (0, 1] (0 selects the fixed clip)", percentile);
-    launch_sampler_step_dynamic(out, z, noise, n, 0.f, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, batch,
-                                percentile, scale_out, false, (cudaStream_t)stream);
-  } else {
-    launch_sampler_step_table(out, z, noise, n, 0.f, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, false,
-                              (cudaStream_t)stream);
-  }
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("sampler_step_cond: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
-                                       const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
-                                       float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, void* stream) {
-  if (!x0 || !sqrt_ac || !sqrt_1mac || !z || !logsnr_out || B < 1 || per < 1) return fail("xunet_forward_diffusion: bad argument");
-  launch_forward_diffusion(x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac, p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B,
-                           per, nullptr, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("forward_diffusion: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_forward_diffusion_v(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
-                                         const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z,
-                                         float* noise_out, float* v_out, float* logsnr_out, int* t_out, float* cond_mask_out,
-                                         int B, long long per, void* stream) {
-  if (!x0 || !sqrt_ac || !sqrt_1mac || !z || !v_out || !logsnr_out) return fail("xunet_forward_diffusion_v: NULL pointer argument");
-  if (B < 1 || per < 1) return fail("xunet_forward_diffusion_v: B = %d, per = %lld, need both >= 1", B, per);
-  launch_forward_diffusion(x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac, p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B,
-                           per, v_out, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("forward_diffusion_v: CUDA error: %s", cudaGetErrorString(e));
-}
-
-// the argument checks of xunet_srn_batch / _v; the ε buffer `noise` is checked by the caller (optional in the v form)
-static int srn_batch_check(const char* fn, const xunet_srn_store* store, const long long* step_dev, int j, int k, int rank,
-                           int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const xunet_batch* out) {
-  if (!store || !step_dev || !sqrt_ac || !sqrt_1mac || !out || !store->pixels || !store->R || !store->t || !store->K ||
-      !store->first || !store->count || !store->item_inst || !out->x || !out->z || !out->logsnr || !out->R1 || !out->t1 ||
-      !out->R2 || !out->t2 || !out->K || !out->cond_mask)
-    return fail("%s: NULL pointer argument", fn);
-  if (B < 1 || k < 1 || world < 1) return fail("%s: B = %d, k = %d, world = %d, need all >= 1", fn, B, k, world);
-  if (rank < 0 || rank >= world || j < 0 || j >= k)
-    return fail("%s: rank = %d of world = %d, j = %d of k = %d out of range", fn, rank, world, j, k);
-  if (store->n_items < 1 || store->n_instances < 1 || store->S < 1)
-    return fail("%s: empty store (n_items = %lld, n_instances = %d, S = %d)", fn, store->n_items, store->n_instances, store->S);
-  if (store->pixel_kind != XUNET_PIXELS_U8 && store->pixel_kind != XUNET_PIXELS_F32)
-    return fail("%s: unknown pixel_kind %d", fn, store->pixel_kind);
-  return 0;
-}
-
-extern "C" int xunet_srn_batch(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
-                               int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
-                               const float* snr_weight, const xunet_batch* out, float* noise, float* loss_weight, int* idx_out,
-                               int* t_out, void* stream) {
-  if (!noise) return fail("xunet_srn_batch: NULL pointer argument");
-  if (const int rc = srn_batch_check("xunet_srn_batch", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out)) return rc;
-  launch_srn_batch(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight, *out, noise,
-                   loss_weight, idx_out, t_out, nullptr, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("srn_batch: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_srn_batch_v(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j, int k,
-                                 int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond,
-                                 const float* snr_weight, const xunet_batch* out, float* noise, float* v_out,
-                                 float* loss_weight, int* idx_out, int* t_out, void* stream) {
-  if (!v_out) return fail("xunet_srn_batch_v: NULL pointer argument");
-  if (const int rc = srn_batch_check("xunet_srn_batch_v", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out)) return rc;
-  launch_srn_batch(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, p_uncond, snr_weight, *out, noise,
-                   loss_weight, idx_out, t_out, v_out, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("srn_batch_v: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_srn_batch_distill(const xunet_srn_store* store, const long long* step_dev, unsigned long long seed, int j,
-                                       int k, int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac,
-                                       const int* grid_t, int n_grid, const xunet_batch* out, const xunet_batch* teacher,
-                                       int teacher_copies, int* m_out, int* idx_out, int* t_out, void* stream) {
-  if (!grid_t || !teacher || !m_out || !teacher->x || !teacher->z || !teacher->logsnr || !teacher->R1 || !teacher->t1 ||
-      !teacher->R2 || !teacher->t2 || !teacher->K)
-    return fail("xunet_srn_batch_distill: NULL pointer argument");
-  if (const int rc = srn_batch_check("xunet_srn_batch_distill", store, step_dev, j, k, rank, world, B, sqrt_ac, sqrt_1mac, out))
-    return rc;
-  if (n_grid < 1) return fail("xunet_srn_batch_distill: n_grid = %d, need >= 1", n_grid);
-  if (teacher_copies != 1 && teacher_copies != 2)
-    return fail("xunet_srn_batch_distill: teacher_copies = %d, need 1 or 2", teacher_copies);
-  const XuDistillDraw dd = {*teacher, teacher_copies, grid_t, n_grid, m_out};
-  launch_srn_batch_distill(*store, step_dev, seed, j, k, rank, world, B, sqrt_ac, sqrt_1mac, *out, dd, idx_out, t_out,
-                           (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("srn_batch_distill: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_distill_teacher_step(const float* out_t, float w, int teacher_copies, const float* teacher_table,
-                                          const int* m_dev, int B, long long per, const xunet_batch* teacher, void* stream) {
-  if (!out_t || !teacher_table || !m_dev || !teacher || !teacher->z || !teacher->logsnr)
-    return fail("xunet_distill_teacher_step: NULL pointer argument");
-  if (B < 1 || per < 1) return fail("xunet_distill_teacher_step: B = %d, per = %lld, need both >= 1", B, per);
-  if (teacher_copies != 1 && teacher_copies != 2)
-    return fail("xunet_distill_teacher_step: teacher_copies = %d, need 1 or 2", teacher_copies);
-  launch_distill_teacher_step(out_t, w, teacher_copies, teacher_table, m_dev, B, per, const_cast<float*>(teacher->z),
-                              const_cast<float*>(teacher->logsnr), (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("distill_teacher_step: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_distill_target(const float* out_t, float w, int teacher_copies, const float* teacher_table,
-                                    const float* target_table, const int* m_dev, const float* z_t, const float* teacher_z, int B,
-                                    long long per, float* v_out, void* stream) {
-  if (!out_t || !teacher_table || !target_table || !m_dev || !z_t || !teacher_z || !v_out)
-    return fail("xunet_distill_target: NULL pointer argument");
-  if (B < 1 || per < 1) return fail("xunet_distill_target: B = %d, per = %lld, need both >= 1", B, per);
-  if (teacher_copies != 1 && teacher_copies != 2)
-    return fail("xunet_distill_target: teacher_copies = %d, need 1 or 2", teacher_copies);
-  launch_distill_target(out_t, w, teacher_copies, teacher_table, target_table, m_dev, z_t, teacher_z, B, per, v_out,
-                        (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("distill_target: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,
-                                  void* stream) {
-  if (!mask_out || n <= 0) return fail("xunet_dropout_mask: bad argument");
-  launch_dropout_mask(mask_out, n, op_index, seed, rate, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("dropout_mask: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
-                                   float* ssim_out, void* stream) {
-  if (!pred || !target || !mse_out || !psnr_out || !ssim_out) return fail("xunet_image_metrics: NULL pointer argument");
-  if (B < 1) return fail("xunet_image_metrics: B = %d, need B >= 1", B);
-  if (S < 11 || S > XUNET_METRICS_MAX_SIDE)
-    return fail("xunet_image_metrics: S = %d outside [11, %d]", S, XUNET_METRICS_MAX_SIDE);
-  launch_image_metrics(pred, target, B, S, mse_out, psnr_out, ssim_out, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("image_metrics: CUDA error: %s", cudaGetErrorString(e));
-}
-
-// The checks both field entries share (include/xunet_b200.h, "Limits"); 0 or the fail() code.
-static int field_check(const char* what, int G, float bound, int V, int S, float near, float step, float background) {
-  if (G < XUNET_FIELD_MIN_GRID || G > XUNET_FIELD_MAX_GRID)
-    return fail("%s: G = %d outside [%d, %d]", what, G, XUNET_FIELD_MIN_GRID, XUNET_FIELD_MAX_GRID);
-  if (V < 1 || S < 1) return fail("%s: V = %d, S = %d, need both >= 1", what, V, S);
-  if ((long long)V * S * S >= (1LL << 31)) return fail("%s: V S S = %lld pixels, need fewer than 2^31", what, (long long)V * S * S);
-  if (!isfinite(bound) || !(bound > 0.f) || bound > XUNET_FIELD_MAX_BOUND)
-    return fail("%s: bound = %g outside (0, %g]", what, bound, XUNET_FIELD_MAX_BOUND);
-  if (!isfinite(near) || near < 0.f) return fail("%s: near = %g, need a finite near >= 0", what, near);
-  if (!isfinite(step) || !(step > 0.f)) return fail("%s: step = %g, need a finite step > 0", what, step);
-  if (ceil(2.0 * sqrt(3.0) * bound / step) > XUNET_FIELD_MAX_SAMPLES)
-    return fail("%s: step = %g gives more than %d samples on a chord of the cube of bound %g", what, step, XUNET_FIELD_MAX_SAMPLES,
-                bound);
-  if (!isfinite(background)) return fail("%s: background = %g is not finite", what, background);
-  return 0;
-}
-
-extern "C" int xunet_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv,
-                                  int V, int S, float near, float step, float background, float* out, void* stream) {
-  if (!grid || !R || !t || !K || !kinv || !out) return fail("xunet_field_render: NULL pointer argument");
-  if (int rc = field_check("xunet_field_render", G, bound, V, S, near, step, background)) return rc;
-  launch_field_render(grid, G, bound, R, t, K, kinv, V, S, near, step, background, out, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("field_render: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_field_loss_grad(const float* grid, int G, float bound, const float* views, const float* R, const float* t,
-                                     const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
-                                     const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color,
-                                     long long* acc, float* grad, float* loss_out, long long loss_len, void* stream) {
-  if (!grid || !views || !R || !t || !K || !kinv || !iter_dev || !acc || !grad || !loss_out)
-    return fail("xunet_field_loss_grad: NULL pointer argument");
-  if (int rc = field_check("xunet_field_loss_grad", G, bound, V, S, near, step, background)) return rc;
-  if (rays < 1 || rays > XUNET_FIELD_MAX_RAYS)
-    return fail("xunet_field_loss_grad: rays = %d outside [1, %d]", rays, XUNET_FIELD_MAX_RAYS);
-  if (!isfinite(tv_density) || !isfinite(tv_color) || tv_density < 0.f || tv_color < 0.f)
-    return fail("xunet_field_loss_grad: tv weights %g, %g, need finite weights >= 0", tv_density, tv_color);
-  if (loss_len < 0) return fail("xunet_field_loss_grad: loss_len = %lld, need loss_len >= 0", loss_len);
-  launch_field_loss_grad(grid, G, bound, views, R, t, K, kinv, V, S, near, step, background, rays, iter_dev, seed, tv_density,
-                         tv_color, acc, grad, loss_out, loss_len, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("field_loss_grad: CUDA error: %s", cudaGetErrorString(e));
-}
-
-// The shape checks the pose entries share (include/xunet_b200.h, "Pose estimation"); 0 or the fail() code.
-static int pose_check(const char* what, int H, int P, int S) {
-  if (H < 1 || P < 1 || S < 1) return fail("%s: H = %d, P = %d, S = %d, need all >= 1", what, H, P, S);
-  if ((long long)H * P * S * S >= (1LL << 31) / 3) return fail("%s: H P S^2 = %lld, need H P S^2 < 2^31 / 3", what, (long long)H * P * S * S);
-  return 0;
-}
-
-extern "C" int xunet_pose_draw(const float* y, int H, int P, int S, int t_min, int t_max, int strata, const long long* iter_dev,
-                               unsigned long long seed, const float* sqrt_ac, const float* sqrt_1mac, int prediction, float* z,
-                               float* logsnr, float* target, int* t_out, void* stream) {
-  if (!y || !iter_dev || !sqrt_ac || !sqrt_1mac || !z || !logsnr || !target) return fail("xunet_pose_draw: NULL pointer argument");
-  if (int rc = pose_check("xunet_pose_draw", H, P, S)) return rc;
-  if (t_min < 0 || t_min > t_max || t_max > XUNET_POSE_MAX_T)
-    return fail("xunet_pose_draw: t range [%d, %d], need 0 <= t_min <= t_max <= %d", t_min, t_max, XUNET_POSE_MAX_T);
-  if (strata < 0) return fail("xunet_pose_draw: strata = %d, need strata >= 0", strata);
-  if (prediction != 0 && prediction != 1) return fail("xunet_pose_draw: prediction = %d, need 0 (eps) or 1 (v)", prediction);
-  launch_pose_draw(y, H, P, S, t_min, t_max, strata, iter_dev, seed, sqrt_ac, sqrt_1mac, prediction, z, logsnr, target, t_out,
-                   (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("pose_draw: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_pose_loss(const float* out, const float* target, int H, int P, int S, const long long* iter_dev, double* partial,
-                               float* d_out, float* loss_out, long long loss_len, void* stream) {
-  if (!out || !target || !iter_dev || !partial || !d_out || !loss_out) return fail("xunet_pose_loss: NULL pointer argument");
-  if (int rc = pose_check("xunet_pose_loss", H, P, S)) return rc;
-  if (loss_len < 0) return fail("xunet_pose_loss: loss_len = %lld, need loss_len >= 0", loss_len);
-  launch_pose_loss(out, target, H, P, S, iter_dev, partial, d_out, loss_out, loss_len, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("pose_loss: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_pose_tangent(const float* dR, const float* dt, int H, int P, const double* R, const double* t, int translate,
-                                  float* grad, void* stream) {
-  if (!dR || !dt || !R || !t || !grad) return fail("xunet_pose_tangent: NULL pointer argument");
-  if (int rc = pose_check("xunet_pose_tangent", H, P, 1)) return rc;
-  if (translate != 0 && translate != 1) return fail("xunet_pose_tangent: translate = %d, need 0 or 1", translate);
-  launch_pose_tangent(dR, dt, H, P, R, t, translate, grad, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("pose_tangent: CUDA error: %s", cudaGetErrorString(e));
-}
-
-extern "C" int xunet_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows,
-                                  void* stream) {
-  if (!step || !R || !t || !R_rows || !t_rows) return fail("xunet_pose_retract: NULL pointer argument");
-  if (int rc = pose_check("xunet_pose_retract", H, P, 1)) return rc;
-  if (translate != 0 && translate != 1) return fail("xunet_pose_retract: translate = %d, need 0 or 1", translate);
-  launch_pose_retract(step, H, P, translate, R, t, R_rows, t_rows, (cudaStream_t)stream);
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : fail("pose_retract: CUDA error: %s", cudaGetErrorString(e));
 }
 
 // ---- operator-level entry points ----------------------------------------------------------------------
@@ -1747,17 +1410,16 @@ struct OpScratch {
 };
 
 static int op_done(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("%s: CUDA error: %s", what, cudaGetErrorString(e));
-  if (xu_kernel_error()[0]) return fail("%s: %s", what, xu_kernel_error());
+  if (int rc = xu_launched(what)) return rc;
+  if (xu_kernel_error()[0]) return xu_fail("%s: %s", what, xu_kernel_error());
   return 0;
 }
 
 // the public impl of the operator-level conv entries (0 SIMT, 1 tensor cores, 2 a direct 3-channel kernel) -> the kernel to run:
 // for 1 and 2, the engine's choice for the shape, which must be of that kind
 static int op_conv_kernel(int impl, ConvKernel engine, const char* what, ConvKernel& k) {
-  if (impl == 1 && engine != CONV_TC) return fail("%s: shape not supported by the tensor-core kernel", what);
-  if (impl == 2 && engine != CONV_CIN3 && engine != CONV_COUT3) return fail("%s: no direct 3-channel kernel takes this shape", what);
+  if (impl == 1 && engine != CONV_TC) return xu_fail("%s: shape not supported by the tensor-core kernel", what);
+  if (impl == 2 && engine != CONV_CIN3 && engine != CONV_COUT3) return xu_fail("%s: no direct 3-channel kernel takes this shape", what);
   k = impl == 1 || impl == 2 ? engine : CONV_SIMT;
   return 0;
 }
@@ -1777,7 +1439,7 @@ static int op_dispatch_conv(int dtype, ConvKernel k, const ConvShape& cs, const 
     if (need > scratch_bytes) {
       cudaDeviceSynchronize();
       if (scratch) cudaFree(scratch);
-      if (cudaMalloc(&scratch, need) != cudaSuccess) { scratch = nullptr; scratch_bytes = 0; return fail("%s: cudaMalloc", what); }
+      if (cudaMalloc(&scratch, need) != cudaSuccess) { scratch = nullptr; scratch_bytes = 0; return xu_fail("%s: cudaMalloc", what); }
       scratch_bytes = need;
       last_w = nullptr;
     }
@@ -1801,7 +1463,7 @@ static int op_dispatch_conv(int dtype, ConvKernel k, const ConvShape& cs, const 
 static int op_conv_fwd(int dtype, int impl, const void* x, const float* w, const float* bias, const void* res, void* y, float* cstats,
                        int N, int Hi, int Wi, int Ci, int Co, int ksize, int stride, int nseg, float alpha, cudaStream_t s,
                        const char* what) {
-  if (ksize != 1 && ksize != 3) return fail("%s: ksize must be 1 or 3", what);
+  if (ksize != 1 && ksize != 3) return xu_fail("%s: ksize must be 1 or 3", what);
   const ConvShape cs = conv_shape(N, Hi, Wi, Ci, Co, ksize, stride, nseg);
   ConvKernel k;
   if (op_conv_kernel(impl, conv_kernels(dtype, cs, res != nullptr).fwd, what, k)) return 1;
@@ -1851,7 +1513,7 @@ extern "C" int xunet_op_attention(int dtype, int impl, const void* qkv, const vo
                                   int L, int C, int heads, int cross, void* stream) {
   xu_set_kernel_error("");
   OpScratch scratch;
-  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention: shape not supported by the tensor-core kernel");
+  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return xu_fail("xunet_op_attention: shape not supported by the tensor-core kernel");
   dispatch_attn_fwd(dtype, impl, attn_args(qkv, res, out, lse, N, L, C, heads, cross), (cudaStream_t)stream);
   return op_done("op_attention");
 }
@@ -1861,7 +1523,7 @@ extern "C" int xunet_op_attention_bwd(int dtype, int impl, const void* qkv, cons
                                       int heads, int cross, void* stream) {
   xu_set_kernel_error("");
   OpScratch scratch;
-  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return fail("xunet_op_attention_bwd: shape not supported by the tensor-core kernel");
+  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return xu_fail("xunet_op_attention_bwd: shape not supported by the tensor-core kernel");
   AttnArgs a = attn_args(qkv, res, const_cast<void*>(out), const_cast<float*>(lse), N, L, C, heads, cross);
   a.dout = dout; a.dscratch = dscratch; a.dqkv = dqkv;
   // XUNET_OP_ATTN_FOLD=1: the caller passes an all-zero dscratch and gets it back all-zero (the D rows are cleared after use)
@@ -1876,19 +1538,19 @@ static_assert(XUNET_RS_NONE == RS_NONE && XUNET_RS_DOWN == RS_DOWN && XUNET_RS_U
 
 // the checks every GroupNorm-path entry shares: GroupNorm(32) over both frames of each sample
 static int gn_check_shape(const char* what, int dtype, int N, int H, int W, int C) {
-  if (dtype != XUNET_DTYPE_F32 && dtype != XUNET_DTYPE_BF16) return fail("%s: bad dtype %d", what, dtype);
-  if (N < 2 || N % 2 != 0) return fail("%s: N = %d, need an even N >= 2 (two frames per sample)", what, N);
-  if (H < 1 || W < 1) return fail("%s: H = %d, W = %d, need both >= 1", what, H, W);
-  if (C < 32 || C % 32 != 0) return fail("%s: C = %d is not a positive multiple of the 32 groups", what, C);
+  if (dtype != XUNET_DTYPE_F32 && dtype != XUNET_DTYPE_BF16) return xu_fail("%s: bad dtype %d", what, dtype);
+  if (N < 2 || N % 2 != 0) return xu_fail("%s: N = %d, need an even N >= 2 (two frames per sample)", what, N);
+  if (H < 1 || W < 1) return xu_fail("%s: H = %d, W = %d, need both >= 1", what, H, W);
+  if (C < 32 || C % 32 != 0) return xu_fail("%s: C = %d is not a positive multiple of the 32 groups", what, C);
   return 0;
 }
 
 static int gn_check_mode(const char* what, int mode, int rs, int H, int W, float drop_rate) {
-  if (mode != XUNET_GN_PLAIN && mode != XUNET_GN_SWISH && mode != XUNET_GN_FILM) return fail("%s: bad mode %d", what, mode);
-  if (rs != XUNET_RS_NONE && rs != XUNET_RS_DOWN && rs != XUNET_RS_UP) return fail("%s: bad resample %d", what, rs);
-  if (rs != XUNET_RS_NONE && mode == XUNET_GN_FILM) return fail("%s: a resampling norm has no FiLM", what);
-  if (rs == XUNET_RS_DOWN && (H % 2 != 0 || W % 2 != 0)) return fail("%s: RS_DOWN needs even H, W (got %d x %d)", what, H, W);
-  if (!(drop_rate >= 0.f && drop_rate < 1.f)) return fail("%s: drop_rate %g outside [0, 1)", what, drop_rate);
+  if (mode != XUNET_GN_PLAIN && mode != XUNET_GN_SWISH && mode != XUNET_GN_FILM) return xu_fail("%s: bad mode %d", what, mode);
+  if (rs != XUNET_RS_NONE && rs != XUNET_RS_DOWN && rs != XUNET_RS_UP) return xu_fail("%s: bad resample %d", what, rs);
+  if (rs != XUNET_RS_NONE && mode == XUNET_GN_FILM) return xu_fail("%s: a resampling norm has no FiLM", what);
+  if (rs == XUNET_RS_DOWN && (H % 2 != 0 || W % 2 != 0)) return xu_fail("%s: RS_DOWN needs even H, W (got %d x %d)", what, H, W);
+  if (!(drop_rate >= 0.f && drop_rate < 1.f)) return xu_fail("%s: drop_rate %g outside [0, 1)", what, drop_rate);
   return 0;
 }
 
@@ -1896,7 +1558,7 @@ extern "C" int xunet_op_conv_stats(int dtype, int impl, const void* x, const flo
                                    float* cstats, int N, int H, int W, int Ci, int Co, int ksize, float alpha, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_conv_stats";
-  if (!x || !w || !y || !cstats) return fail("%s: NULL pointer argument", what);
+  if (!x || !w || !y || !cstats) return xu_fail("%s: NULL pointer argument", what);
   if (gn_check_shape(what, dtype, N, H, W, Co)) return 1;
   OpScratch scratch;
   return op_conv_fwd(dtype, impl, x, w, bias, res, y, cstats, N, H, W, Ci, Co, ksize, 1, 1, alpha, (cudaStream_t)stream, what);
@@ -1906,10 +1568,10 @@ extern "C" int xunet_op_attention_stats(int dtype, int impl, const void* qkv, co
                                         int N, int L, int C, int heads, int cross, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_attention_stats";
-  if (!qkv || !res || !out || !lse || !cstats) return fail("%s: NULL pointer argument", what);
+  if (!qkv || !res || !out || !lse || !cstats) return xu_fail("%s: NULL pointer argument", what);
   if (gn_check_shape(what, dtype, N, L, 1, C)) return 1;
-  if (heads < 1 || C % heads != 0) return fail("%s: C = %d is not a multiple of heads = %d", what, C, heads);
-  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return fail("%s: shape not supported by the tensor-core kernel", what);
+  if (heads < 1 || C % heads != 0) return xu_fail("%s: C = %d is not a multiple of heads = %d", what, C, heads);
+  if (impl == 1 && !attn_tc_supported(dtype, L, C, heads)) return xu_fail("%s: shape not supported by the tensor-core kernel", what);
   OpScratch scratch;
   AttnArgs a = attn_args(qkv, res, out, lse, N, L, C, heads, cross);
   const bool fused = attn_emits_stats(impl);
@@ -1925,13 +1587,13 @@ extern "C" int xunet_op_groupnorm(int dtype, const void* x, const float* cstats_
                                   const unsigned long long* seed_dev, int train, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_groupnorm";
-  if (!x || !cstats_a || !gamma || !beta || !y || !stats) return fail("%s: NULL pointer argument", what);
+  if (!x || !cstats_a || !gamma || !beta || !y || !stats) return xu_fail("%s: NULL pointer argument", what);
   if (gn_check_shape(what, dtype, N, H, W, C) || gn_check_mode(what, mode, resample, H, W, drop_rate)) return 1;
-  if (ca < 1 || ca > C) return fail("%s: ca = %d outside [1, C = %d]", what, ca, C);
-  if (ca < C && !cstats_b) return fail("%s: ca = %d < C needs cstats_b", what, ca);
-  if (mode == XUNET_GN_FILM && !e) return fail("%s: a FiLM norm needs e", what);
-  if (mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev) return fail("%s: dropout in training needs seed_dev", what);
-  if (resample != XUNET_RS_NONE && params_out) return fail("%s: a resampling norm has no fused backward (params_out)", what);
+  if (ca < 1 || ca > C) return xu_fail("%s: ca = %d outside [1, C = %d]", what, ca, C);
+  if (ca < C && !cstats_b) return xu_fail("%s: ca = %d < C needs cstats_b", what, ca);
+  if (mode == XUNET_GN_FILM && !e) return xu_fail("%s: a FiLM norm needs e", what);
+  if (mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev) return xu_fail("%s: dropout in training needs seed_dev", what);
+  if (resample != XUNET_RS_NONE && params_out) return xu_fail("%s: a resampling norm has no fused backward (params_out)", what);
   OpScratch scratch;
   GnArgs a = gn_fill(x, y, mode == XUNET_GN_FILM ? e : nullptr, gamma, beta, stats, N, H, W, C, mode, resample, drop_rate, op_index,
                      seed_dev, train ? 1 : 0);
@@ -1948,16 +1610,16 @@ extern "C" int xunet_op_conv_dgrad_groupnorm(int dtype, const void* dy, const fl
                                              int W, int C, int Co, int ksize, int nseg, float alpha, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_conv_dgrad_groupnorm";
-  if (!dy || !w || !gn_x || !gn_params || !dyh || !bcs) return fail("%s: NULL pointer argument", what);
+  if (!dy || !w || !gn_x || !gn_params || !dyh || !bcs) return xu_fail("%s: NULL pointer argument", what);
   if (gn_check_shape(what, dtype, N, H, W, C) || gn_check_mode(what, mode, XUNET_RS_NONE, H, W, drop_rate)) return 1;
-  if ((mode == XUNET_GN_FILM) != (e != nullptr)) return fail("%s: e is given exactly for a FiLM norm", what);
-  if (mode == XUNET_GN_FILM && !de) return fail("%s: a FiLM norm needs de", what);
-  if (mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev) return fail("%s: dropout in training needs seed_dev", what);
-  if (ksize != 1 && ksize != 3) return fail("%s: ksize must be 1 or 3", what);
-  if (nseg < 1 || Co % nseg != 0) return fail("%s: Co = %d is not a multiple of nseg = %d", what, Co, nseg);
+  if ((mode == XUNET_GN_FILM) != (e != nullptr)) return xu_fail("%s: e is given exactly for a FiLM norm", what);
+  if (mode == XUNET_GN_FILM && !de) return xu_fail("%s: a FiLM norm needs de", what);
+  if (mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev) return xu_fail("%s: dropout in training needs seed_dev", what);
+  if (ksize != 1 && ksize != 3) return xu_fail("%s: ksize must be 1 or 3", what);
+  if (nseg < 1 || Co % nseg != 0) return xu_fail("%s: Co = %d is not a multiple of nseg = %d", what, Co, nseg);
   const ConvShape cs = conv_shape(N, H, W, C, Co, ksize, 1, nseg);
   const ConvKernel k = conv_kernels(dtype, cs, false).dgrad;
-  if (!dgrad_fuses_gn_bwd(k, cs)) return fail("%s: shape not supported by the fused tensor-core data gradient", what);
+  if (!dgrad_fuses_gn_bwd(k, cs)) return xu_fail("%s: shape not supported by the fused tensor-core data gradient", what);
   OpScratch scratch;
   ConvArgs a = conv_dgrad_args(cs, dy, w, dyh, alpha, 0);
   set_gn_bwd_epilogue(a, gn_x, gn_params, mode, e, de, bcs, drop_rate, op_index, seed_dev, train ? 1 : 0);
@@ -1971,13 +1633,13 @@ extern "C" int xunet_op_groupnorm_bwd(int dtype, const void* x, const void* e, c
                                       int accumulate, int de_accumulate, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_groupnorm_bwd";
-  if (!x || !dy || !dx || !gamma || !beta || !dgamma || !dbeta || !stats) return fail("%s: NULL pointer argument", what);
+  if (!x || !dy || !dx || !gamma || !beta || !dgamma || !dbeta || !stats) return xu_fail("%s: NULL pointer argument", what);
   if (gn_check_shape(what, dtype, N, H, W, C) || gn_check_mode(what, mode, resample, H, W, drop_rate)) return 1;
-  if (bcs && resample != XUNET_RS_NONE) return fail("%s: the fused backward (bcs) has no resampling", what);
-  if (!bcs && !bstats) return fail("%s: the two-kernel backward needs bstats", what);
-  if (!bcs && mode == XUNET_GN_FILM && (!e || !de)) return fail("%s: a FiLM norm needs e and de", what);
+  if (bcs && resample != XUNET_RS_NONE) return xu_fail("%s: the fused backward (bcs) has no resampling", what);
+  if (!bcs && !bstats) return xu_fail("%s: the two-kernel backward needs bstats", what);
+  if (!bcs && mode == XUNET_GN_FILM && (!e || !de)) return xu_fail("%s: a FiLM norm needs e and de", what);
   if (!bcs && mode == XUNET_GN_FILM && train && drop_rate > 0.f && !seed_dev)
-    return fail("%s: dropout in training needs seed_dev", what);
+    return xu_fail("%s: dropout in training needs seed_dev", what);
   OpScratch scratch;
   GnArgs a = gn_fill(x, dx, mode == XUNET_GN_FILM ? e : nullptr, gamma, beta, const_cast<float*>(stats), N, H, W, C, mode, resample,
                      drop_rate, op_index, seed_dev, train ? 1 : 0);
@@ -2000,16 +1662,16 @@ extern "C" int xunet_op_groupnorm_bwd(int dtype, const void* x, const void* e, c
 
 // ---- operator-level entry points of the conditioning, resampling, concat and loss launches -----------------------------
 static int dtype_ok(const char* what, int dtype) {
-  return dtype == XUNET_DTYPE_F32 || dtype == XUNET_DTYPE_BF16 ? 0 : fail("%s: bad dtype %d", what, dtype);
+  return dtype == XUNET_DTYPE_F32 || dtype == XUNET_DTYPE_BF16 ? 0 : xu_fail("%s: bad dtype %d", what, dtype);
 }
 // 4-wide vector accesses: 16-byte (fp32) / 8-byte (bf16) aligned pointers
 static int vec_aligned(const char* what, int dtype, const void* p) {
   const size_t a = dtype == XUNET_DTYPE_F32 ? 16 : 8;
-  return (reinterpret_cast<uintptr_t>(p) % a) == 0 ? 0 : fail("%s: pointer %p is not %zu-byte aligned", what, p, a);
+  return (reinterpret_cast<uintptr_t>(p) % a) == 0 ? 0 : xu_fail("%s: pointer %p is not %zu-byte aligned", what, p, a);
 }
 static int emb_check(const char* what, int B, int E) {
-  if (B < 1) return fail("%s: B = %d, need B >= 1", what, B);
-  if (E < 4 || E % 4 != 0) return fail("%s: E = %d, need a positive multiple of 4", what, E);
+  if (B < 1) return xu_fail("%s: B = %d, need B >= 1", what, B);
+  if (E < 4 || E % 4 != 0) return xu_fail("%s: E = %d, need a positive multiple of 4", what, E);
   return 0;
 }
 
@@ -2017,7 +1679,7 @@ extern "C" int xunet_op_logsnr_emb(const float* logsnr, const float* w0, const f
                                    float* h1, float* lemb, int B, int E, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_logsnr_emb";
-  if (!logsnr || !w0 || !b0 || !w1 || !b1 || !pe || !h1 || !lemb) return fail("%s: NULL pointer argument", what);
+  if (!logsnr || !w0 || !b0 || !w1 || !b1 || !pe || !h1 || !lemb) return xu_fail("%s: NULL pointer argument", what);
   if (emb_check(what, B, E)) return 1;
   OpScratch scratch;
   launch_logsnr_emb(logsnr, w0, b0, w1, b1, pe, h1, lemb, B, E, (cudaStream_t)stream);
@@ -2028,7 +1690,7 @@ extern "C" int xunet_op_logsnr_emb_bwd(const float* dlemb, const float* w1, cons
                                        float* db0, float* dw1, float* db1, int B, int E, int accumulate, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_logsnr_emb_bwd";
-  if (!dlemb || !w1 || !pe || !h1 || !dh1 || !dw0 || !db0 || !dw1 || !db1) return fail("%s: NULL pointer argument", what);
+  if (!dlemb || !w1 || !pe || !h1 || !dh1 || !dw0 || !db0 || !dw1 || !db1) return xu_fail("%s: NULL pointer argument", what);
   if (emb_check(what, B, E)) return 1;
   OpScratch scratch;
   launch_logsnr_emb_bwd(dlemb, w1, pe, h1, dh1, dw0, db0, dw1, db1, B, E, accumulate ? 1 : 0, (cudaStream_t)stream);
@@ -2041,11 +1703,11 @@ extern "C" int xunet_op_pose_emb(int dtype, const float* R1, const float* t1, co
   xu_set_kernel_error("");
   const char* what = "xunet_op_pose_emb";
   if (dtype_ok(what, dtype)) return 1;
-  if (!cond_mask || !out) return fail("%s: NULL pointer argument", what);
-  if (!rays && (!R1 || !t1 || !R2 || !t2 || !K || !kinv)) return fail("%s: generated rays need R1, t1, R2, t2, K and kinv", what);
-  if (!ref_first != !ref_other) return fail("%s: ref_first and ref_other are given together", what);
-  if (B < 1 || S < 1) return fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
-  if (convention != XUNET_RAYS_V3D130_IJ && convention != XUNET_RAYS_OPENCV_UV) return fail("%s: bad ray convention %d", what, convention);
+  if (!cond_mask || !out) return xu_fail("%s: NULL pointer argument", what);
+  if (!rays && (!R1 || !t1 || !R2 || !t2 || !K || !kinv)) return xu_fail("%s: generated rays need R1, t1, R2, t2, K and kinv", what);
+  if (!ref_first != !ref_other) return xu_fail("%s: ref_first and ref_other are given together", what);
+  if (B < 1 || S < 1) return xu_fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
+  if (convention != XUNET_RAYS_V3D130_IJ && convention != XUNET_RAYS_OPENCV_UV) return xu_fail("%s: bad ray convention %d", what, convention);
   OpScratch scratch;
   launch_pose_emb(dtype, R1, t1, R2, t2, K, cond_mask, pos_emb, ref_first, ref_other, kinv, out, B, S, convention, rays,
                   (cudaStream_t)stream);
@@ -2057,9 +1719,9 @@ extern "C" int xunet_op_pose_emb_bwd(int dtype, const void* dpose, float* dpos_e
   xu_set_kernel_error("");
   const char* what = "xunet_op_pose_emb_bwd";
   if (dtype_ok(what, dtype)) return 1;
-  if (!dpose) return fail("%s: NULL pointer argument", what);
-  if (!dref_first != !dref_other) return fail("%s: dref_first and dref_other are given together", what);
-  if (B < 1 || S < 1) return fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
+  if (!dpose) return xu_fail("%s: NULL pointer argument", what);
+  if (!dref_first != !dref_other) return xu_fail("%s: dref_first and dref_other are given together", what);
+  if (B < 1 || S < 1) return xu_fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
   OpScratch scratch;
   launch_pose_emb_bwd(dtype, dpose, dpos_emb, dref_first, dref_other, B, S, accumulate ? 1 : 0, (cudaStream_t)stream);
   return op_done(what);
@@ -2067,15 +1729,15 @@ extern "C" int xunet_op_pose_emb_bwd(int dtype, const void* dpose, float* dpos_e
 
 static int film_emb_check(const char* what, int dtype, int N, int HW, int E) {
   if (dtype_ok(what, dtype)) return 1;
-  if (N < 2 || N % 2 != 0) return fail("%s: N = %d, need an even N >= 2 (two frames per sample)", what, N);
-  if (HW < 1) return fail("%s: HW = %d, need HW >= 1", what, HW);
+  if (N < 2 || N % 2 != 0) return xu_fail("%s: N = %d, need an even N >= 2 (two frames per sample)", what, N);
+  if (HW < 1) return xu_fail("%s: HW = %d, need HW >= 1", what, HW);
   return emb_check(what, N / 2, E);
 }
 
 extern "C" int xunet_op_film_emb(int dtype, const float* lemb, const void* pe, void* semb, int N, int HW, int E, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_film_emb";
-  if (!lemb || !pe || !semb) return fail("%s: NULL pointer argument", what);
+  if (!lemb || !pe || !semb) return xu_fail("%s: NULL pointer argument", what);
   if (film_emb_check(what, dtype, N, HW, E) || vec_aligned(what, dtype, pe) || vec_aligned(what, dtype, semb)) return 1;
   OpScratch scratch;
   launch_emb_fwd(dtype, lemb, pe, semb, N, HW, E, (cudaStream_t)stream);
@@ -2086,7 +1748,7 @@ extern "C" int xunet_op_film_emb_bwd(int dtype, const float* lemb, const void* p
                                      int HW, int E, int write_dpe, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_film_emb_bwd";
-  if (!lemb || !pe || !dsemb || !dlemb || (write_dpe && !dpe)) return fail("%s: NULL pointer argument", what);
+  if (!lemb || !pe || !dsemb || !dlemb || (write_dpe && !dpe)) return xu_fail("%s: NULL pointer argument", what);
   if (film_emb_check(what, dtype, N, HW, E) || vec_aligned(what, dtype, pe) || vec_aligned(what, dtype, dsemb) ||
       (write_dpe && vec_aligned(what, dtype, dpe)))
     return 1;
@@ -2099,11 +1761,11 @@ extern "C" int xunet_op_resample(int dtype, const void* x, void* y, int N, int H
                                  void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_resample";
-  if (!x || !y) return fail("%s: NULL pointer argument", what);
+  if (!x || !y) return xu_fail("%s: NULL pointer argument", what);
   if (dtype_ok(what, dtype) || vec_aligned(what, dtype, x) || vec_aligned(what, dtype, y)) return 1;
-  if (N < 1 || H < 1 || W < 1) return fail("%s: N = %d, H = %d, W = %d, need all >= 1", what, N, H, W);
-  if (C < 4 || C % 4 != 0) return fail("%s: C = %d, need a positive multiple of 4", what, C);
-  if (pool && (H % 2 != 0 || W % 2 != 0)) return fail("%s: pooling needs even H, W (got %d x %d)", what, H, W);
+  if (N < 1 || H < 1 || W < 1) return xu_fail("%s: N = %d, H = %d, W = %d, need all >= 1", what, N, H, W);
+  if (C < 4 || C % 4 != 0) return xu_fail("%s: C = %d, need a positive multiple of 4", what, C);
+  if (pool && (H % 2 != 0 || W % 2 != 0)) return xu_fail("%s: pooling needs even H, W (got %d x %d)", what, H, W);
   OpScratch scratch;
   launch_resample(dtype, x, y, N, H, W, C, pool ? 1 : 0, scale, accumulate ? 1 : 0, (cudaStream_t)stream);
   return op_done(what);
@@ -2113,14 +1775,14 @@ extern "C" int xunet_op_copy_channels(int dtype, const void* src, void* dst, lon
                                       int Cc, int accumulate, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_copy_channels";
-  if (!src || !dst) return fail("%s: NULL pointer argument", what);
+  if (!src || !dst) return xu_fail("%s: NULL pointer argument", what);
   if (dtype_ok(what, dtype) || vec_aligned(what, dtype, src) || vec_aligned(what, dtype, dst)) return 1;
-  if (npix < 1) return fail("%s: npix = %lld, need npix >= 1", what, npix);
+  if (npix < 1) return xu_fail("%s: npix = %lld, need npix >= 1", what, npix);
   if (Cc < 4 || Cs % 4 || Cd % 4 || src_off % 4 || dst_off % 4 || Cc % 4)
-    return fail("%s: Cs = %d, Cd = %d, src_off = %d, dst_off = %d, Cc = %d, need multiples of 4 and Cc >= 4", what, Cs, Cd, src_off,
-                dst_off, Cc);
+    return xu_fail("%s: Cs = %d, Cd = %d, src_off = %d, dst_off = %d, Cc = %d, need multiples of 4 and Cc >= 4", what, Cs, Cd, src_off,
+                   dst_off, Cc);
   if (src_off < 0 || dst_off < 0 || src_off + Cc > Cs || dst_off + Cc > Cd)
-    return fail("%s: channels [%d, %d) of %d to [%d, %d) of %d out of range", what, src_off, src_off + Cc, Cs, dst_off, dst_off + Cc, Cd);
+    return xu_fail("%s: channels [%d, %d) of %d to [%d, %d) of %d out of range", what, src_off, src_off + Cc, Cs, dst_off, dst_off + Cc, Cd);
   OpScratch scratch;
   launch_copy_channels(dtype, src, dst, npix, Cs, Cd, src_off, dst_off, Cc, accumulate ? 1 : 0, (cudaStream_t)stream);
   return op_done(what);
@@ -2129,9 +1791,9 @@ extern "C" int xunet_op_copy_channels(int dtype, const void* src, void* dst, lon
 extern "C" int xunet_op_scale_add(int dtype, const void* src, void* dst, long long n, float alpha, int accumulate, void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_scale_add";
-  if (!src || !dst) return fail("%s: NULL pointer argument", what);
+  if (!src || !dst) return xu_fail("%s: NULL pointer argument", what);
   if (dtype_ok(what, dtype) || vec_aligned(what, dtype, src) || vec_aligned(what, dtype, dst)) return 1;
-  if (n < 4 || n % 4 != 0) return fail("%s: n = %lld, need a positive multiple of 4", what, n);
+  if (n < 4 || n % 4 != 0) return xu_fail("%s: n = %lld, need a positive multiple of 4", what, n);
   OpScratch scratch;
   launch_scale_add(dtype, src, dst, n, alpha, accumulate ? 1 : 0, (cudaStream_t)stream);
   return op_done(what);
@@ -2141,9 +1803,9 @@ extern "C" int xunet_op_loss(int dtype, const float* eps, const float* noise, fl
                              void* stream) {
   xu_set_kernel_error("");
   const char* what = "xunet_op_loss";
-  if (!eps || !noise || !sumsq || !loss || !dO) return fail("%s: NULL pointer argument", what);
+  if (!eps || !noise || !sumsq || !loss || !dO) return xu_fail("%s: NULL pointer argument", what);
   if (dtype_ok(what, dtype)) return 1;
-  if (B < 1 || S < 1) return fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
+  if (B < 1 || S < 1) return xu_fail("%s: B = %d, S = %d, need both >= 1", what, B, S);
   OpScratch scratch;
   launch_loss(dtype, eps, noise, sumsq, loss, dO, B, S, (cudaStream_t)stream);
   return op_done(what);

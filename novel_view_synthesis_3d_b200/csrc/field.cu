@@ -249,21 +249,52 @@ static FieldGeom field_geom(int G, float bound, float near, float step, float ba
   return FieldGeom{G, bound, near, step, 0.5f * (background + 1.f)};
 }
 
-void launch_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv, int V,
-                         int S, float near, float step, float background, float* out, cudaStream_t s) {
+// The checks both field entries share (include/xunet_b200.h, "Limits"); 0 or the xu_fail() code.
+static int field_check(const char* what, int G, float bound, int V, int S, float near, float step, float background) {
+  if (G < XUNET_FIELD_MIN_GRID || G > XUNET_FIELD_MAX_GRID)
+    return xu_fail("%s: G = %d outside [%d, %d]", what, G, XUNET_FIELD_MIN_GRID, XUNET_FIELD_MAX_GRID);
+  if (V < 1 || S < 1) return xu_fail("%s: V = %d, S = %d, need both >= 1", what, V, S);
+  if ((long long)V * S * S >= (1LL << 31)) return xu_fail("%s: V S S = %lld pixels, need fewer than 2^31", what, (long long)V * S * S);
+  if (!isfinite(bound) || !(bound > 0.f) || bound > XUNET_FIELD_MAX_BOUND)
+    return xu_fail("%s: bound = %g outside (0, %g]", what, bound, XUNET_FIELD_MAX_BOUND);
+  if (!isfinite(near) || near < 0.f) return xu_fail("%s: near = %g, need a finite near >= 0", what, near);
+  if (!isfinite(step) || !(step > 0.f)) return xu_fail("%s: step = %g, need a finite step > 0", what, step);
+  if (ceil(2.0 * sqrt(3.0) * bound / step) > XUNET_FIELD_MAX_SAMPLES)
+    return xu_fail("%s: step = %g gives more than %d samples on a chord of the cube of bound %g", what, step, XUNET_FIELD_MAX_SAMPLES,
+                   bound);
+  if (!isfinite(background)) return xu_fail("%s: background = %g is not finite", what, background);
+  return 0;
+}
+
+extern "C" int xunet_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv,
+                                  int V, int S, float near, float step, float background, float* out, void* stream) {
+  if (!grid || !R || !t || !K || !kinv || !out) return xu_fail("xunet_field_render: NULL pointer argument");
+  if (int rc = field_check("xunet_field_render", G, bound, V, S, near, step, background)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   xu_launch(kinv_kernel, cdiv(V, 64), 64, 0, s, K, kinv, V);
   xu_launch(field_render_kernel, cdiv((long long)V * S * S, FIELD_THREADS), FIELD_THREADS, 0, s, grid,
             field_geom(G, bound, near, step, background), (const float*)kinv, R, t, V, S, out);
+  return xu_launched("field_render");
 }
 
-void launch_field_loss_grad(const float* grid, int G, float bound, const float* views, const float* R, const float* t,
-                            const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
-                            const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color, long long* acc,
-                            float* grad, float* loss_out, long long loss_len, cudaStream_t s) {
+extern "C" int xunet_field_loss_grad(const float* grid, int G, float bound, const float* views, const float* R, const float* t,
+                                     const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
+                                     const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color,
+                                     long long* acc, float* grad, float* loss_out, long long loss_len, void* stream) {
+  if (!grid || !views || !R || !t || !K || !kinv || !iter_dev || !acc || !grad || !loss_out)
+    return xu_fail("xunet_field_loss_grad: NULL pointer argument");
+  if (int rc = field_check("xunet_field_loss_grad", G, bound, V, S, near, step, background)) return rc;
+  if (rays < 1 || rays > XUNET_FIELD_MAX_RAYS)
+    return xu_fail("xunet_field_loss_grad: rays = %d outside [1, %d]", rays, XUNET_FIELD_MAX_RAYS);
+  if (!isfinite(tv_density) || !isfinite(tv_color) || tv_density < 0.f || tv_color < 0.f)
+    return xu_fail("xunet_field_loss_grad: tv weights %g, %g, need finite weights >= 0", tv_density, tv_color);
+  if (loss_len < 0) return xu_fail("xunet_field_loss_grad: loss_len = %lld, need loss_len >= 0", loss_len);
+  const cudaStream_t s = (cudaStream_t)stream;
   xu_launch(kinv_kernel, cdiv(V, 64), 64, 0, s, K, kinv, V);
   xu_launch(field_loss_grad_kernel, cdiv(rays, FIELD_THREADS), FIELD_THREADS, 0, s, grid,
             field_geom(G, bound, near, step, background), views, (const float*)kinv, R, t, V, S, rays, iter_dev, seed,
             (unsigned long long*)acc);
   xu_launch(field_finish_kernel, cdiv(4LL * G * G * G, 256), 256, 0, s, grid, G, rays, tv_density, tv_color, iter_dev, acc, grad,
             loss_out, loss_len);
+  return xu_launched("field_loss_grad");
 }

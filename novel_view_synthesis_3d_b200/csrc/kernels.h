@@ -1,4 +1,6 @@
-// kernels.h -- host launchers of the hand-written kernels (all asynchronous on `s`).
+// kernels.h -- what more than one source file needs: the launchers the engine plan runs (all asynchronous on `s`), the
+// shared kinv_kernel, and the determinism and error plumbing.  The C entries that run no plan launch their kernels in the
+// file that holds them.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -134,79 +136,8 @@ void launch_loss_mse(int dtype, const float* eps, const float* noise, const floa
                      int S, cudaStream_t s);
 // dO (2B,S,S,3): frame0 = 0, frame1 = d_eps (B,S,S,3) fp32, rounded once to the activation dtype
 void launch_vjp_seed(int dtype, const float* d_eps, void* dO, int B, int S, cudaStream_t s);
-// Adam; with ema, also ema = decay*ema + (1-decay)*p_new in the same pass.  warmup > 0: lr_t = lr * min(step - 1, warmup) /
-// warmup; norm_dev: optax.clip_by_global_norm by *norm_dev, where a non-finite *norm_dev leaves every buffer untouched and
-// increments *skipped.  Neither (norm_dev == nullptr, warmup == 0): plain Adam, without the clip / warm-up prologue.
-void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
-                 const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s);
-// *norm_out = sqrt(sum_i fp32(g_i * grad_scale)^2), summed in fp64 in a fixed order (grid from n only, no atomics).
-// scratch: XUNET_GRAD_NORM_SCRATCH doubles; on completion scratch[0] holds the fp64 sum of squares.  Two launches.
-void launch_grad_global_norm(const float* g, long long n, double grad_scale, double* scratch, float* norm_out,
-                             cudaStream_t s);
-// x0_hist == nullptr: the single-step update (DDPM, DDIM); else the multistep one, which reads column 6 (c_prev) and the
-// previous step's x0 from x0_hist (n floats) and stores this step's x0 there.  guided: eps2 = [cond ; uncond] (2n) and the new z
-// goes to both halves of inp_z; else eps2 is the conditional output (n), used as is, and inp_z has n values
-void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
-                               const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
-                               float* x0_hist, bool guided, cudaStream_t s);
-// xunet_sampler_step_dynamic (sampler_dyn.cu): the step above with x0 thresholded per view at the p-quantile of |x0|; one
-// cluster of 8 CTAs per view, n / B <= XUNET_SAMPLER_DYN_MAX_PER
-void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
-                                 const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
-                                 int B2, float* x0_hist, int B, double p, float* scale_out, bool guided, cudaStream_t s);
-// v_out != nullptr: the v-target instance (xunet_forward_diffusion_v), which also stores v and takes noise_out == nullptr
-void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
-                              const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
-                              float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, float* v_out,
-                              cudaStream_t s);
-// xunet_srn_batch (data.cu): one micro-batch drawn from a device SRN store, gathered and forward-diffused; grid (chunks, B).
-// v_out != nullptr: the v-target instance (xunet_srn_batch_v), which also stores v and takes noise == nullptr
-void launch_srn_batch(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k, int rank,
-                      int world, int B, const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, const float* snr_weight,
-                      const xunet_batch& out, float* noise, float* loss_weight, int* idx_out, int* t_out, float* v_out,
-                      cudaStream_t s);
-// xunet_srn_batch_distill: the draw of xunet_srn_batch with t = grid_t[m], m = (sample hash) mod n_grid, cond_mask 1, no
-// target, and the sample's inputs copied into the teacher's `copies` row blocks
-struct XuDistillDraw {
-  xunet_batch teacher;    // x, z, logsnr, R1, t1, R2, t2, K of the teacher's batch (copies * B rows; cond_mask, rays unused)
-  int copies;             // 2: a guided [cond ; uncond] teacher batch, 1: an unguided one
-  const int* grid_t;      // the student's timesteps, loop order
-  int n_grid;
-  int* m_out;             // (B) the drawn grid positions
-};
-void launch_srn_batch_distill(const xunet_srn_store& st, const long long* step_dev, unsigned long long seed, int j, int k,
-                              int rank, int world, int B, const float* sqrt_ac, const float* sqrt_1mac, const xunet_batch& out,
-                              const XuDistillDraw& dd, int* idx_out, int* t_out, cudaStream_t s);
-// distill.cu: the teacher's first DDIM step (row 2 m_b of the teacher table) from the first teacher output, into the teacher's z
-// and logsnr rows; then the target: the second step (row 2 m_b + 1) from the second output, and the student's v target
-void launch_distill_teacher_step(const float* out_t, float w, int copies, const float* ttab, const int* m_dev, int B,
-                                 long long per, float* tz, float* tlogsnr, cudaStream_t s);
-void launch_distill_target(const float* out_t, float w, int copies, const float* ttab, const float* gtab, const int* m_dev,
-                           const float* z_t, const float* tz, int B, long long per, float* v_out, cudaStream_t s);
-void launch_dropout_mask(float* out, long long n, int op_index, unsigned long long seed, float rate, cudaStream_t s);
-// xunet_image_metrics: one CTA per image, fp64 moments and sums in a fixed order (metrics.cu); 11 <= S <= XUNET_METRICS_MAX_SIDE
-struct MetricsWindow { double w[11]; };   // the normalised 1-D Gaussian weights of the SSIM window
-void launch_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
-                          float* ssim_out, cudaStream_t s);
-// xunet_field_render / xunet_field_loss_grad (field.cu): K^-1 of the V cameras into kinv (V, 9), then the render, or the drawn
-// rays' fixed-point gradient and the finish pass
+// K^-1 of B cameras into kinv (B, 9): the pose embedding's rays (kernels_elem.cu) and the radiance field's (field.cu)
 __global__ void kinv_kernel(const float* __restrict__ K, float* __restrict__ kinv, int B);
-void launch_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv, int V,
-                         int S, float near, float step, float background, float* out, cudaStream_t s);
-void launch_field_loss_grad(const float* grid, int G, float bound, const float* views, const float* R, const float* t,
-                            const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
-                            const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color, long long* acc,
-                            float* grad, float* loss_out, long long loss_len, cudaStream_t s);
-// xunet_pose_draw / _loss / _tangent / _retract (pose_fit.cu): the loop of pose estimation around the camera gradient
-void launch_pose_draw(const float* y, int H, int P, int S, int t_min, int t_max, int strata, const long long* iter_dev,
-                      unsigned long long seed, const float* sqrt_ac, const float* sqrt_1mac, int prediction, float* z, float* logsnr,
-                      float* target, int* t_out, cudaStream_t s);
-void launch_pose_loss(const float* out, const float* target, int H, int P, int S, const long long* iter_dev, double* partial,
-                      float* d_out, float* loss_out, long long loss_len, cudaStream_t s);
-void launch_pose_tangent(const float* dR, const float* dt, int H, int P, const double* R, const double* t, int translate, float* grad,
-                         cudaStream_t s);
-void launch_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows, cudaStream_t s);
 
 // ---- attention over frames ---------------------------------------------------------------------------------
 struct AttnArgs {
@@ -249,3 +180,7 @@ __device__ __forceinline__ void xu_det_add(double* acc, float v) { atomicAdd(acc
 
 const char* xu_kernel_error();  // last launch-configuration error recorded by a launcher ("" if none)
 void xu_set_kernel_error(const char* msg);
+// xunet_last_error() <- the printf-formatted message; returns 1, the entries' error code
+int xu_fail(const char* fmt, ...);
+// after an entry's launches: 0, or xu_fail("<what>: CUDA error: <cudaGetLastError()>")
+int xu_launched(const char* what);

@@ -1,6 +1,7 @@
 // kernels_elem.cu -- HBM-bound kernels of the X-UNet path: joint-frame GroupNorm (+SiLU/FiLM/dropout/
 // resample) forward and backward, conditioning (log-SNR embedding, camera-ray NeRF posenc), resample,
-// channel copies, loss, Adam, sampler update.  All 128-bit (fp32) / 64-bit (bf16) vectorised along C.
+// channel copies, loss, Adam, forward diffusion.  All 128-bit (fp32) / 64-bit (bf16) vectorised along C.
+// The C entries of Adam, the gradient norm, forward diffusion and the dropout mask launch their kernels here.
 #include "common.cuh"
 #include "kernels.h"
 #include <string.h>
@@ -1640,9 +1641,10 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
     }
   }
 }
-void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
-                 double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
-                 const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s) {
+// ema == nullptr: no EMA.  norm_dev == nullptr and warmup == 0: plain Adam, without the clip / warm-up prologue
+static void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
+                        double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
+                        const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s) {
   int blocks = cdiv(n, 256 * 4);   // one float4 per thread and pass
   if (blocks > xu_num_sms() * 8) blocks = xu_num_sms() * 8;
   if (blocks < 1) blocks = 1;
@@ -1651,6 +1653,42 @@ void launch_adam(float* p, const float* g, float* m, float* v, long long n, long
                                : (clip ? adam_kernel<true, true> : adam_kernel<true, false>);
   xu_launch(kernel, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps, (float)grad_scale,
             decay, norm_dev, (float)max_norm, warmup, skipped);
+}
+
+extern "C" int xunet_adam_step(float* params, const float* grads, float* m, float* v, long long n, long long step,
+                               const long long* step_dev, double lr, double b1, double b2, double eps, double grad_scale,
+                               void* stream) {
+  if (!params || !grads || !m || !v || n < 0) return xu_fail("xunet_adam_step: bad argument");
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, nullptr, 0.0, nullptr, 0.0, 0, nullptr,
+              (cudaStream_t)stream);
+  return xu_launched("adam");
+}
+
+extern "C" int xunet_adam_ema_step(float* params, const float* grads, float* m, float* v, float* ema, long long n,
+                                   long long step, const long long* step_dev, double lr, double b1, double b2, double eps,
+                                   double grad_scale, double ema_decay, void* stream) {
+  if (!params || !grads || !m || !v || n < 0) return xu_fail("xunet_adam_ema_step: bad argument");
+  if (!ema) return xu_fail("xunet_adam_ema_step: ema is NULL (use xunet_adam_step without an EMA)");
+  if (!(ema_decay >= 0.0 && ema_decay <= 1.0)) return xu_fail("xunet_adam_ema_step: ema_decay %g outside [0, 1]", ema_decay);
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema_decay, nullptr, 0.0, 0, nullptr,
+              (cudaStream_t)stream);
+  return xu_launched("adam_ema");
+}
+
+extern "C" int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, float* ema, long long n,
+                                    long long step, const long long* step_dev, double lr, double b1, double b2, double eps,
+                                    double grad_scale, double ema_decay, const float* norm_dev, double max_norm,
+                                    long long warmup_steps, long long* skipped_dev, void* stream) {
+  if (!params || !grads || !m || !v || n < 0) return xu_fail("xunet_adam_clip_step: bad argument");
+  if (ema && !(ema_decay >= 0.0 && ema_decay <= 1.0)) return xu_fail("xunet_adam_clip_step: ema_decay %g outside [0, 1]", ema_decay);
+  if (warmup_steps < 0) return xu_fail("xunet_adam_clip_step: warmup_steps %lld < 0", warmup_steps);
+  if (norm_dev) {
+    if (!(max_norm > 0.0)) return xu_fail("xunet_adam_clip_step: max_norm %g must be > 0", max_norm);
+    if (!skipped_dev) return xu_fail("xunet_adam_clip_step: skipped_dev is NULL (needed with norm_dev)");
+  }
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema ? ema_decay : 0.0, norm_dev,
+              max_norm, warmup_steps, skipped_dev, (cudaStream_t)stream);
+  return xu_launched("adam_clip");
 }
 
 // ---- global gradient norm (optax.clip_by_global_norm) ----------------------------------------------------------------------
@@ -1706,63 +1744,13 @@ static int grad_norm_partials(long long n) {
   if (b > XUNET_GRAD_NORM_SCRATCH) b = XUNET_GRAD_NORM_SCRATCH;
   return b < 1 ? 1 : (int)b;
 }
-void launch_grad_global_norm(const float* g, long long n, double grad_scale, double* scratch, float* norm_out,
-                             cudaStream_t s) {
+extern "C" int xunet_grad_global_norm(const float* grads, long long n, double grad_scale, double* scratch, float* norm_out,
+                                      void* stream) {
+  if (!grads || !scratch || !norm_out || n < 0) return xu_fail("xunet_grad_global_norm: bad argument");
   const int parts = grad_norm_partials(n);
-  xu_launch(grad_sumsq_partial_kernel, parts, 256, 0, s, g, n, (float)grad_scale, scratch);
-  xu_launch(grad_norm_final_kernel, 1, 256, 0, s, scratch, parts, norm_out);
-}
-
-// One ancestral step with the schedule ON THE DEVICE (sampling.py:128-151): the coefficients of loop position k = *pos_dev come
-// from a table (k = 0 is the first executed step = highest t), and the kernel also writes the NEXT forward's inputs (z into
-// both halves of the [cond ; uncond] batch, the lagging log-SNR), so one CUDA graph = forward + this kernel + counter++ is
-// replayed per step with no host arithmetic or copies in between.
-// tab row: {c_recip, c_recipm1, c_x0, c_z, sigma, logsnr_next, c_prev, -}
-// The noise of step k is noise[k*n .. k*n+n) if `noise` is set, else the hash normal of (*seed_dev - k).
-// HIST = false (DDPM, DDIM): z' = c_x0 x0 + c_z z + sigma noise, as the compiler contracts it (the bits of the original
-// single-step kernel).  HIST = true (multistep solvers, DPM-Solver++(2M)) fixes the order, one rounding per fma:
-//   z' = fma(sigma, noise, fma(c_prev, x0_hist[i], fma(c_x0, x0, c_z * z))), the c_prev term skipped when c_prev == 0,
-// then x0_hist[i] = x0.  A row with c_prev == 0 never reads x0_hist (the first step needs no initialised history).
-// GUIDED = true: eps2 is the [cond ; uncond] output of a 2B batch and the new z goes to both halves of inp_z.  GUIDED = false
-// (a model whose guidance is in its weights, e.g. a distilled student): eps2 is the B-batch conditional output, read as is,
-// and the new z goes to inp_z's n values.
-template <bool HIST, bool GUIDED>
-__global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __restrict__ eps2, float* __restrict__ z,
-                                                                 const float* __restrict__ noise, long long n, float w,
-                                                                 const float* __restrict__ tab, const int* __restrict__ pos_dev,
-                                                                 const unsigned long long* __restrict__ seed_dev, float* __restrict__ inp_z,
-                                                                 float* __restrict__ inp_logsnr, int B2, float* __restrict__ x0_hist) {
-  xu_grid_dep_sync();
-  const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-  const int k = *pos_dev;
-  const float* t = tab + 8LL * k;
-  if (i < B2) inp_logsnr[i] = t[5];
-  if (i >= n) return;
-  const float e = GUIDED ? xu_step_guided(w, eps2[i], eps2[n + i]) : eps2[i];
-  const float zi = z[i];
-  const float x0 = xu_step_x0(t, zi, e);
-  const float nz = noise != nullptr ? noise[k * n + i] : xu_hash_normal(*seed_dev - (unsigned long long)k, (uint64_t)i);
-  float zn;
-  if constexpr (HIST) {
-    const float c_prev = t[6];
-    zn = fmaf(t[2], x0, __fmul_rn(t[3], zi));
-    if (c_prev != 0.f) zn = fmaf(c_prev, x0_hist[i], zn);
-    zn = fmaf(t[4], nz, zn);
-    x0_hist[i] = x0;
-  } else {
-    zn = xu_step_z(t, x0, zi, nz);
-  }
-  z[i] = zn;
-  inp_z[i] = zn;
-  if constexpr (GUIDED) inp_z[n + i] = zn;
-}
-void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
-                               const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr, int B2,
-                               float* x0_hist, bool guided, cudaStream_t s) {
-  const int grid = cdiv(n > B2 ? n : B2, 256);
-  auto kernel = x0_hist != nullptr ? (guided ? sampler_step_table_kernel<true, true> : sampler_step_table_kernel<true, false>)
-                                   : (guided ? sampler_step_table_kernel<false, true> : sampler_step_table_kernel<false, false>);
-  xu_launch(kernel, grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr, B2, x0_hist);
+  xu_launch(grad_sumsq_partial_kernel, parts, 256, 0, (cudaStream_t)stream, grads, n, (float)grad_scale, scratch);
+  xu_launch(grad_norm_final_kernel, 1, 256, 0, (cudaStream_t)stream, scratch, parts, norm_out);
+  return xu_launched("grad_global_norm");
 }
 
 // dataset/data_loader.py:92-110 on the device.  TARGET == XU_TARGET_V also stores v = xu_fd_v(..) to v_out (the last
@@ -1796,17 +1784,24 @@ __global__ void __launch_bounds__(256) forward_diffusion_kernel(const float* __r
     if (cond_mask_out != nullptr) cond_mask_out[b] = xu_fd_cond_mask(hb, p_uncond);
   }
 }
-void launch_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
-                              const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
-                              float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, float* v_out,
-                              cudaStream_t s) {
-  const long long n = (long long)B * per;
-  if (v_out != nullptr)
-    xu_launch(forward_diffusion_kernel<XU_TARGET_V>, cdiv(n, 256), 256, 0, s, x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac,
-              p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B, per, v_out);
-  else
-    xu_launch(forward_diffusion_kernel<XU_TARGET_EPS>, cdiv(n, 256), 256, 0, s, x0, noise_in, t_in, seed, sqrt_ac, sqrt_1mac,
-              p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B, per, v_out);
+extern "C" int xunet_forward_diffusion(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
+                                       const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z, float* noise_out,
+                                       float* logsnr_out, int* t_out, float* cond_mask_out, int B, long long per, void* stream) {
+  if (!x0 || !sqrt_ac || !sqrt_1mac || !z || !logsnr_out || B < 1 || per < 1) return xu_fail("xunet_forward_diffusion: bad argument");
+  xu_launch(forward_diffusion_kernel<XU_TARGET_EPS>, cdiv((long long)B * per, 256), 256, 0, (cudaStream_t)stream, x0, noise_in,
+            t_in, seed, sqrt_ac, sqrt_1mac, p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B, per, nullptr);
+  return xu_launched("forward_diffusion");
+}
+
+extern "C" int xunet_forward_diffusion_v(const float* x0, const float* noise_in, const int* t_in, unsigned long long seed,
+                                         const float* sqrt_ac, const float* sqrt_1mac, float p_uncond, float* z,
+                                         float* noise_out, float* v_out, float* logsnr_out, int* t_out, float* cond_mask_out,
+                                         int B, long long per, void* stream) {
+  if (!x0 || !sqrt_ac || !sqrt_1mac || !z || !v_out || !logsnr_out) return xu_fail("xunet_forward_diffusion_v: NULL pointer argument");
+  if (B < 1 || per < 1) return xu_fail("xunet_forward_diffusion_v: B = %d, per = %lld, need both >= 1", B, per);
+  xu_launch(forward_diffusion_kernel<XU_TARGET_V>, cdiv((long long)B * per, 256), 256, 0, (cudaStream_t)stream, x0, noise_in,
+            t_in, seed, sqrt_ac, sqrt_1mac, p_uncond, z, noise_out, logsnr_out, t_out, cond_mask_out, B, per, v_out);
+  return xu_launched("forward_diffusion_v");
 }
 
 __global__ void dropout_mask_kernel(float* __restrict__ out, long long n, int op_index, unsigned long long seed, float rate) {
@@ -1814,6 +1809,9 @@ __global__ void dropout_mask_kernel(float* __restrict__ out, long long n, int op
   const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
   if (i < n) out[i] = xu_keep(seed, op_index, (unsigned long long)i, rate) ? 1.f : 0.f;
 }
-void launch_dropout_mask(float* out, long long n, int op_index, unsigned long long seed, float rate, cudaStream_t s) {
-  xu_launch(dropout_mask_kernel, cdiv(n, 256), 256, 0, s, out, n, op_index, seed, rate);
+extern "C" int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,
+                                  void* stream) {
+  if (!mask_out || n <= 0) return xu_fail("xunet_dropout_mask: bad argument");
+  xu_launch(dropout_mask_kernel, cdiv(n, 256), 256, 0, (cudaStream_t)stream, mask_out, n, op_index, seed, rate);
+  return xu_launched("dropout_mask");
 }

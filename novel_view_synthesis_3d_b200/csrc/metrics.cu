@@ -17,6 +17,8 @@
 #define METRICS_BAND 8                        // output rows per pass
 #define METRICS_RING (METRICS_BAND + 10)      // horizontally filtered rows kept in shared memory
 
+struct MetricsWindow { double w[11]; };   // the normalised 1-D Gaussian weights of the SSIM window
+
 static size_t metrics_smem_bytes(int S) { return sizeof(double) * 5 * METRICS_RING * (size_t)(S - 10); }
 
 __device__ __forceinline__ double metrics_u(float v) { return fmin(fmax(((double)v + 1.0) * 0.5, 0.0), 1.0); }
@@ -113,8 +115,12 @@ static MetricsWindow metrics_window() {
   return win;
 }
 
-void launch_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
-                          float* ssim_out, cudaStream_t s) {
+extern "C" int xunet_image_metrics(const float* pred, const float* target, int B, int S, float* mse_out, float* psnr_out,
+                                   float* ssim_out, void* stream) {
+  if (!pred || !target || !mse_out || !psnr_out || !ssim_out) return xu_fail("xunet_image_metrics: NULL pointer argument");
+  if (B < 1) return xu_fail("xunet_image_metrics: B = %d, need B >= 1", B);
+  if (S < 11 || S > XUNET_METRICS_MAX_SIDE)
+    return xu_fail("xunet_image_metrics: S = %d outside [11, %d]", S, XUNET_METRICS_MAX_SIDE);
   static bool configured = false;
   if (!configured) {
     cudaFuncSetAttribute(image_metrics_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -122,6 +128,7 @@ void launch_image_metrics(const float* pred, const float* target, int B, int S, 
     configured = true;
   }
   static const MetricsWindow win = metrics_window();
-  xu_launch(image_metrics_kernel, B, METRICS_THREADS, metrics_smem_bytes(S), s, pred, target, S, win, mse_out, psnr_out,
-            ssim_out);
+  xu_launch(image_metrics_kernel, B, METRICS_THREADS, metrics_smem_bytes(S), (cudaStream_t)stream, pred, target, S, win, mse_out,
+            psnr_out, ssim_out);
+  return xu_launched("image_metrics");
 }

@@ -172,29 +172,58 @@ __global__ void __launch_bounds__(POSE_THREADS) pose_retract_kernel(float* __res
   for (int j = 0; j < D; ++j) st[j] = 0.f;
 }
 
-void launch_pose_draw(const float* y, int H, int P, int S, int t_min, int t_max, int strata, const long long* iter_dev,
-                      unsigned long long seed, const float* sqrt_ac, const float* sqrt_1mac, int prediction, float* z, float* logsnr,
-                      float* target, int* t_out, cudaStream_t s) {
-  const long long n = 3LL * S * S;
-  auto kernel = prediction == 1 ? pose_draw_kernel<XU_TARGET_V> : pose_draw_kernel<XU_TARGET_EPS>;
-  xu_launch(kernel, cdiv((long long)P * n, POSE_THREADS), POSE_THREADS, 0, s, y, H, P, n, t_min, t_max, strata, iter_dev, seed,
-            sqrt_ac, sqrt_1mac, z, logsnr, target, t_out);
+// The shape checks the pose entries share (include/xunet_b200.h, "Pose estimation"); 0 or the xu_fail() code.
+static int pose_check(const char* what, int H, int P, int S) {
+  if (H < 1 || P < 1 || S < 1) return xu_fail("%s: H = %d, P = %d, S = %d, need all >= 1", what, H, P, S);
+  if ((long long)H * P * S * S >= (1LL << 31) / 3) return xu_fail("%s: H P S^2 = %lld, need H P S^2 < 2^31 / 3", what, (long long)H * P * S * S);
+  return 0;
 }
 
-void launch_pose_loss(const float* out, const float* target, int H, int P, int S, const long long* iter_dev, double* partial,
-                      float* d_out, float* loss_out, long long loss_len, cudaStream_t s) {
+extern "C" int xunet_pose_draw(const float* y, int H, int P, int S, int t_min, int t_max, int strata, const long long* iter_dev,
+                               unsigned long long seed, const float* sqrt_ac, const float* sqrt_1mac, int prediction, float* z,
+                               float* logsnr, float* target, int* t_out, void* stream) {
+  if (!y || !iter_dev || !sqrt_ac || !sqrt_1mac || !z || !logsnr || !target) return xu_fail("xunet_pose_draw: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_draw", H, P, S)) return rc;
+  if (t_min < 0 || t_min > t_max || t_max > XUNET_POSE_MAX_T)
+    return xu_fail("xunet_pose_draw: t range [%d, %d], need 0 <= t_min <= t_max <= %d", t_min, t_max, XUNET_POSE_MAX_T);
+  if (strata < 0) return xu_fail("xunet_pose_draw: strata = %d, need strata >= 0", strata);
+  if (prediction != 0 && prediction != 1) return xu_fail("xunet_pose_draw: prediction = %d, need 0 (eps) or 1 (v)", prediction);
+  const long long n = 3LL * S * S;
+  auto kernel = prediction == 1 ? pose_draw_kernel<XU_TARGET_V> : pose_draw_kernel<XU_TARGET_EPS>;
+  xu_launch(kernel, cdiv((long long)P * n, POSE_THREADS), POSE_THREADS, 0, (cudaStream_t)stream, y, H, P, n, t_min, t_max, strata,
+            iter_dev, seed, sqrt_ac, sqrt_1mac, z, logsnr, target, t_out);
+  return xu_launched("pose_draw");
+}
+
+extern "C" int xunet_pose_loss(const float* out, const float* target, int H, int P, int S, const long long* iter_dev, double* partial,
+                               float* d_out, float* loss_out, long long loss_len, void* stream) {
+  if (!out || !target || !iter_dev || !partial || !d_out || !loss_out) return xu_fail("xunet_pose_loss: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_loss", H, P, S)) return rc;
+  if (loss_len < 0) return xu_fail("xunet_pose_loss: loss_len = %lld, need loss_len >= 0", loss_len);
   const long long n = 3LL * S * S;
   const int chunks = cdiv(n, XUNET_POSE_LOSS_CHUNK);
   const float coef = (float)(2.0 / ((double)P * (double)n));
+  const cudaStream_t s = (cudaStream_t)stream;
   xu_launch(pose_loss_rows_kernel, dim3(chunks, H * P), POSE_THREADS, 0, s, out, target, P, n, coef, partial, d_out);
   xu_launch(pose_loss_finish_kernel, 1, POSE_THREADS, 0, s, (const double*)partial, H, P, chunks, n, iter_dev, loss_out, loss_len);
+  return xu_launched("pose_loss");
 }
 
-void launch_pose_tangent(const float* dR, const float* dt, int H, int P, const double* R, const double* t, int translate, float* grad,
-                         cudaStream_t s) {
-  xu_launch(pose_tangent_kernel, cdiv(H, POSE_THREADS), POSE_THREADS, 0, s, dR, dt, H, P, R, t, translate, grad);
+extern "C" int xunet_pose_tangent(const float* dR, const float* dt, int H, int P, const double* R, const double* t, int translate,
+                                  float* grad, void* stream) {
+  if (!dR || !dt || !R || !t || !grad) return xu_fail("xunet_pose_tangent: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_tangent", H, P, 1)) return rc;
+  if (translate != 0 && translate != 1) return xu_fail("xunet_pose_tangent: translate = %d, need 0 or 1", translate);
+  xu_launch(pose_tangent_kernel, cdiv(H, POSE_THREADS), POSE_THREADS, 0, (cudaStream_t)stream, dR, dt, H, P, R, t, translate, grad);
+  return xu_launched("pose_tangent");
 }
 
-void launch_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows, cudaStream_t s) {
-  xu_launch(pose_retract_kernel, cdiv(H, POSE_THREADS), POSE_THREADS, 0, s, step, H, P, translate, R, t, R_rows, t_rows);
+extern "C" int xunet_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows,
+                                  void* stream) {
+  if (!step || !R || !t || !R_rows || !t_rows) return xu_fail("xunet_pose_retract: NULL pointer argument");
+  if (int rc = pose_check("xunet_pose_retract", H, P, 1)) return rc;
+  if (translate != 0 && translate != 1) return xu_fail("xunet_pose_retract: translate = %d, need 0 or 1", translate);
+  xu_launch(pose_retract_kernel, cdiv(H, POSE_THREADS), POSE_THREADS, 0, (cudaStream_t)stream, step, H, P, translate, R, t, R_rows,
+            t_rows);
+  return xu_launched("pose_retract");
 }
