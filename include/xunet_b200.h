@@ -510,6 +510,7 @@ int xunet_image_metrics(const float* pred, const float* target, int B, int S, fl
 #define XUNET_FIELD_MAX_SAMPLES 4096
 #define XUNET_FIELD_MAX_RAYS (1 << 20)
 #define XUNET_FIELD_FIXED_ONE 4294967296.0   /* 2^32: one unit of the fixed-point gradient sums */
+#define XUNET_FIELD_MAX_GRAD_L1 8388608.0    /* 2^23: the sum of |dC| over the values xunet_field_image_grad scatters */
 /* Renders V views: out (V, S, S, 3) in [-1, 1].  Each pixel is composited by one thread on its own, so a view has the same bits
  * alone or anywhere in a batch. */
 int xunet_field_render(const float* grid, int G, float bound, const float* R, const float* t, const float* K, float* kinv, int V,
@@ -534,6 +535,25 @@ int xunet_field_loss_grad(const float* grid, int G, float bound, const float* vi
                           const float* K, float* kinv, int V, int S, float near, float step, float background, int rays,
                           const long long* iter_dev, unsigned long long seed, float tv_density, float tv_color, long long* acc,
                           float* grad, float* loss_out, long long loss_len, void* stream);
+/* The backward of a given image gradient, over every pixel of V views: with dC (V, S, S, 3) the gradient of some loss w.r.t. the
+ * composited colours C (not the pixels 2C - 1) in units of `unit` (the gradient is unit dC), grad (G, G, G, 4) receives
+ *     unit d/d(raw grid) [ sum_pixels sum_ch dC_ch C_ch ]  +  the total-variation gradient of xunet_field_loss_grad.
+ * A non-finite value of dC is read as 0; a pixel whose three values are 0 is skipped.  The march, the fixed-point scatter, the
+ * per-cell register flush and the finish pass are those of xunet_field_loss_grad (one __device__ backward serves both); the
+ * finish pass multiplies the sums by unit / XUNET_FIELD_FIXED_ONE.  The unit lets a caller whose gradient is a mean over many
+ * values (a few 1e-6 per value) scatter values of order 1, so that a sample's contribution, which can be a few 1e-5 of its
+ * value on a nearly empty grid, stays far above the fixed-point quantum 2^-32.
+ * No overflow, given sum |dC| <= XUNET_FIELD_MAX_GRAD_L1 = 2^23 over all values (the caller's condition; xunet_lift_grad's
+ * output meets it): per ray and word, a colour word adds sum_k dC_ch T_k a_k c(1 - c) w, at most |dC_ch| / 4, and the density
+ * word adds sum_ch dC_ch sum_k d_k (T_{k+1} c_k - R_{k+1}) sigmoid(.) w, at most L sum_ch |dC_ch| with L <= 2 sqrt(3)
+ * XUNET_FIELD_MAX_BOUND < 222.  Summed over the rays that is below 222 * 2^23 < 1.87e9, plus half a unit of rounding per
+ * sample and corner, at most 2^20 rays * 2^12 samples * 2^-33 = 1/2: below 2^31 in magnitude, i.e. below 2^63 in fixed point.
+ * acc: 4 G^3 + 1 int64 words, zero on entry and on return (the last word is unused).  Errors: those of xunet_field_render,
+ * V S S > XUNET_FIELD_MAX_RAYS, unit not finite or not > 0, tv weights negative or not finite.  Three launches: K^-1, the
+ * pixels, and the finish pass. */
+int xunet_field_image_grad(const float* grid, int G, float bound, const float* dC, double unit, const float* R, const float* t,
+                           const float* K, float* kinv, int V, int S, float near, float step, float background, float tv_density,
+                           float tv_color, long long* acc, float* grad, void* stream);
 
 /* Pose estimation by descent on the denoising loss (ID-Pose / iFusion style): given a conditioning view x at a known camera and a
  * target view y (S, S, 3), H pose hypotheses for y's camera are fitted side by side, each seeing P noise draws per iteration.
@@ -583,6 +603,66 @@ int xunet_pose_tangent(const float* dR, const float* dt, int H, int P, const dou
  * hypothesis h receive fp32(R_h), fp32(t_h), and step is zeroed.  A zero step leaves R and t as they are and only writes the rows.
  * Errors: a NULL pointer, H < 1, P < 1, translate not 0 / 1.  One launch. */
 int xunet_pose_retract(float* step, int H, int P, int translate, double* R, double* t, float* R_rows, float* t_rows, void* stream);
+
+/* Lifting one view to a radiance grid by score distillation (DreamFusion's SDS, Poole et al. 2022, on a view-conditioned model as
+ * in Zero-1-to-3 + SJC and Magic123).  A source view x (S, S, 3) at camera (R1, t1, K) conditions the guided X-UNet; each iteration
+ * renders the grid from P drawn cameras around the origin plus the source camera (view P), noises the P renders, runs one forward
+ * of the guided batch of 2P rows [cond ; uncond] (row p and row P + p share draw p) and pushes the weighted residual back through
+ * the renderer.  n = 3 S^2 values per view; i = *iter_dev is the 1-based Adam count (device int64), read at execution time so a
+ * replayed graph draws afresh.  One iteration is
+ *   xunet_lift_draw -> xunet_field_render (P + 1 views) -> xunet_lift_noise -> xunet_forward (train = 0, cond_mask [1]*P + [0]*P)
+ *   -> xunet_lift_grad -> xunet_field_image_grad (P + 1 views) -> xunet_adam_step on the grid -> the count + 1.
+ * Draw p has the hash h_p = xu_mix64((seed ^ XUNET_LIFT_SEED_DOMAIN) 0x9E3779B97F4A7C15 + i 0xD1B54A32D192ED03 + p): the hash of
+ * xunet_pose_draw in a seed domain of its own, so a lift and a pose estimate with the same seed draw independently.
+ * Every entry checks its arguments before it launches anything (message starting with the entry's name); no allocation, no
+ * atomics, no host sync, graph-capturable; the results are functions of the inputs alone (fixed bits). */
+#define XUNET_LIFT_SEED_DOMAIN 0x6C6966745F736473ULL   /* "lift_sds" */
+#define XUNET_LIFT_MAX_RESIDUAL 16.0f                 /* |eps_hat - eps| per value, clamped */
+/* The cameras and timesteps of iteration i, one thread per draw, in fp64 and rounded once to fp32:
+ *   t_p = t_min + h_p mod (t_max - t_min + 1);
+ *   u_1 = (xu_mix64(h_p + 0x5851F42D4C957F2D) >> 11) 2^-53, u_2 = (xu_mix64(h_p + 0x14057B7EF767814F) >> 11) 2^-53 in [0, 1);
+ *   s = sin(elev_lo) + (sin(elev_hi) - sin(elev_lo)) u_1 (the sine of the elevation, uniform: a uniform direction on the band),
+ *   phi = 2 pi u_2, c = radius (s up + sqrt(1 - s^2) (cos(phi) e_1 + sin(phi) e_2)), with up = (up_x, up_y, up_z) / |.|,
+ *   e_1 = normalize(b - (b . up) up), b the first basis vector of least |up_j|, and e_2 = up x e_1;
+ *   the look-at camera at c: f = -c / |c|, right = normalize(f x up), down = f x right, R = [right down f] (columns), and when
+ *   |f x up| < 1e-6 (f parallel or nearly parallel to up) right = normalize(e_1 - (e_1 . f) f).  With up = (0, 0, 1) this is
+ *   synthetic._look_at: e_1 = (1, 0, 0).
+ * Written: R2 (2P, 3, 3) and t2 (2P, 3) rows p and P + p, cam_R (P + 1, 3, 3) and cam_t (P + 1, 3) view p (view P, the source
+ * camera, is the caller's), t_out (P) int32.  Errors: a NULL pointer, P < 1, 0 <= t_min <= t_max <= XUNET_POSE_MAX_T violated,
+ * up zero or not finite, -pi/2 <= elev_lo <= elev_hi <= pi/2 violated, radius not finite and > 0.  One launch. */
+int xunet_lift_draw(int P, int t_min, int t_max, const long long* iter_dev, unsigned long long seed, double up_x, double up_y,
+                    double up_z, double elev_lo, double elev_hi, double radius, float* R2, float* t2, float* cam_R, float* cam_t,
+                    int* t_out, void* stream);
+/* The noise of iteration i, one thread per value of the P drawn views: eps_p[k] = xu_hash_normal(h_p, k), and with
+ * sa = sqrt_ac[t_p], sb = sqrt_1mac[t_p] and render (P + 1, S, S, 3) the renders in [-1, 1] (view P is not read),
+ *   z rows p and P + p (2P, S, S, 3) = fma(sa, render_p[k], fl(sb eps_p[k]))   (xunet_pose_draw's rounding),
+ *   logsnr rows p and P + p = logsnr_schedule_cosine(t_p / 1000), eps (P, S, S, 3) = eps_p.
+ * Errors: a NULL pointer, P < 1, S < 1, (P + 1) S^2 > XUNET_FIELD_MAX_RAYS.  One launch. */
+int xunet_lift_noise(const float* render, const int* t_draw, int P, int S, const long long* iter_dev, unsigned long long seed,
+                     const float* sqrt_ac, const float* sqrt_1mac, float* z, float* logsnr, float* eps, void* stream);
+/* The image gradient and the diagnostics.  out (2P, S, S, 3) is the forward's output, z its noisy input rows, eps the noise of
+ * xunet_lift_noise, render (P + 1, S, S, 3) the renders (pixel = 2C - 1) and x (S, S, 3) the source view.  Per value k of drawn
+ * view p, with sa, sb of t_p:
+ *   o_g = (1 + w) out_p - w out_{P+p};  eps_hat = o_g (prediction 0), = sb z_p + sa o_g (prediction 1, v);
+ *   r = eps_hat - eps_p, 0 if not finite, clamped to +-XUNET_LIFT_MAX_RESIDUAL;
+ *   dC_p[k] = fl32(2 sds_weight omega_t / (3 S^2 P unit)) r,  omega_t = 1 - abar_t = sb^2 in fp64  (the pixel is 2C - 1);
+ * and per value of the source view, with C = (render_P + 1) / 2 and u = clamp((x + 1) / 2, 0, 1):
+ *   dC_P[k] = fl32(2 recon_weight / (3 S^2 unit)) (C - u),
+ * i.e. the gradient w.r.t. C of the loss in units of `unit`, for xunet_field_image_grad with the same unit.  Since |r| <= 16,
+ * omega <= 1 and |C - u| <= 1, sum |dC| <= (32 sds_weight + 2 recon_weight) / unit, and the entry refuses a unit that lets this
+ * exceed XUNET_FIELD_MAX_GRAD_L1.  lift.grad_unit picks the smallest power of two that meets it, so the values are of order 1
+ * (a few 1e-6 before the division at S = 128).  Diagnostics: the squares r^2 and
+ (C - u)^2 are summed in fp64 in chunks of XUNET_POSE_LOSS_CHUNK values (256 thread sums, a fixed shuffle tree, the 8 warp sums in
+ * order) into partial ((P + 1) ceil(n / XUNET_POSE_LOSS_CHUNK) doubles, scratch), then in order, so that when 1 <= i <= loss_len
+ *   sds_out[i - 1] = fp32((1 / (P n)) sum_p sum_k r^2),  loss_out[i - 1] = fp32((1 / n) sum_k (C - u)^2).
+ * Errors: a NULL pointer, P < 1, S < 1, (P + 1) S^2 > XUNET_FIELD_MAX_RAYS, w < 0 or not finite, prediction not 0 / 1, weights
+ * negative or not finite, unit not finite or not > 0, (32 sds_weight + 2 recon_weight) / unit > XUNET_FIELD_MAX_GRAD_L1,
+ * loss_len < 0.  Two launches. */
+int xunet_lift_grad(const float* out, const float* z, const float* eps, const float* render, const float* x, const int* t_draw, int P,
+                    int S, float w, int prediction, float sds_weight, float recon_weight, double unit, const float* sqrt_ac,
+                    const float* sqrt_1mac,
+                    const long long* iter_dev, double* partial, float* dC, float* sds_out, float* loss_out, long long loss_len,
+                    void* stream);
 
 /* ---- operator-level entry points (parity tests / micro-benchmarks of single kernels) ----
  * dtype as above; tensors channels-last (N,H,W,C). */

@@ -139,12 +139,18 @@ SYMBOLS = {
     'xunet_field_loss_grad': (C.c_int, [C.c_void_p, C.c_int, C.c_float] + [C.c_void_p] * 5 + [C.c_int, C.c_int] +
                               [C.c_float] * 3 + [C.c_int, C.c_void_p, C.c_ulonglong, C.c_float, C.c_float] + [C.c_void_p] * 3 +
                               [C.c_longlong, C.c_void_p]),
+    'xunet_field_image_grad': (C.c_int, [C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_double] + [C.c_void_p] * 4 +
+                               [C.c_int, C.c_int] + [C.c_float] * 5 + [C.c_void_p] * 3),
     'xunet_pose_draw': (C.c_int, [C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_ulonglong, C.c_void_p, C.c_void_p, C.c_int] +
                         [C.c_void_p] * 5),
     'xunet_pose_loss': (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 3 + [C.c_void_p] * 4 + [C.c_longlong, C.c_void_p]),
     'xunet_pose_tangent': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                      C.c_void_p]),
     'xunet_pose_retract': (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 5),
+    'xunet_lift_draw': (C.c_int, [C.c_int] * 3 + [C.c_void_p, C.c_ulonglong] + [C.c_double] * 6 + [C.c_void_p] * 6),
+    'xunet_lift_noise': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_ulonglong] + [C.c_void_p] * 6),
+    'xunet_lift_grad': (C.c_int, [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_float, C.c_int, C.c_float, C.c_float, C.c_double] +
+                        [C.c_void_p] * 7 + [C.c_longlong, C.c_void_p]),
     'xunet_op_conv': (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p] +
                       [C.c_int] * 8 + [C.c_float, C.c_void_p]),
     'xunet_op_conv_dgrad': (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 8 +

@@ -1,5 +1,6 @@
-// field.cu -- the radiance grid of the 3D consistency score: volume rendering of a dense (G, G, G, 4) grid
-// (xunet_field_render) and one iteration's loss gradient (xunet_field_loss_grad).  include/xunet_b200.h states the field.
+// field.cu -- the radiance grid of the 3D consistency score and of lifting: volume rendering of a dense (G, G, G, 4) grid
+// (xunet_field_render), one iteration's loss gradient (xunet_field_loss_grad) and the backward of a given image gradient
+// (xunet_field_image_grad).  include/xunet_b200.h states the field.
 //
 // One thread marches one ray; the grid is read with one 16-byte load per corner and stays in L2 (32 MB at G = 128).
 // The gradient pass marches a drawn ray twice -- forward to composite C, then front to back again with the residual
@@ -143,36 +144,11 @@ __device__ __forceinline__ void field_flush(unsigned long long* __restrict__ acc
   }
 }
 
-// One drawn ray per thread: ray r of iteration i = *iter_dev is training pixel
-//   xu_mix64(seed * 0x9E3779B97F4A7C15 + i * 0xD1B54A32D192ED03 + r) mod (V S S)     (consistency.draw_rays restates it).
-// acc receives the gradient of the per-ray sum sum_ch (C - u)^2 w.r.t. the raw grid, and acc[4 G^3] the sum itself.
-__global__ void __launch_bounds__(FIELD_THREADS) field_loss_grad_kernel(const float* __restrict__ grid, FieldGeom g,
-                                                                         const float* __restrict__ views,
-                                                                         const float* __restrict__ kinv, const float* __restrict__ R,
-                                                                         const float* __restrict__ t, int V, int S, int rays,
-                                                                         const long long* __restrict__ iter_dev,
-                                                                         unsigned long long seed,
-                                                                         unsigned long long* __restrict__ acc) {
-  xu_grid_dep_sync();
-  const int r = blockIdx.x * FIELD_THREADS + threadIdx.x;
-  if (r >= rays) return;
-  const unsigned long long i = (unsigned long long)*iter_dev;
-  const long long npix = (long long)V * S * S;
-  const long long p = (long long)(xu_mix64(seed * 0x9E3779B97F4A7C15ULL + i * 0xD1B54A32D192ED03ULL + (unsigned long long)r) %
-                                  (unsigned long long)npix);
-  const int v = (int)(p / ((long long)S * S)), row = (int)(p / S % S), col = (int)(p % S);
-  float o[3], d[3], C[3], gC[3];
-  field_ray(kinv, R, t, v, row, col, o, d);
-  field_composite(grid, g, o, d, C);
-  float lsum = 0.f;
-#pragma unroll
-  for (int ch = 0; ch < 3; ++ch) {
-    const float u = fminf(fmaxf((views[3 * p + ch] + 1.f) * 0.5f, 0.f), 1.f);
-    gC[ch] = 2.f * (C[ch] - u);
-    lsum += (C[ch] - u) * (C[ch] - u);
-  }
-  atomicAdd(acc + 4LL * g.G * g.G * g.G, (unsigned long long)field_fix(lsum));
-
+// The backward of one ray composited to C: front to back again with the residual R_{k+1} = C - sum_{j<=k} T_j a_j c_j,
+// scattering each sample's gradient of sum_ch gC_ch C_ch into its cell's 8 corners of acc (fixed point, flushed per cell).
+__device__ __forceinline__ void field_ray_backward(const float* __restrict__ grid, const FieldGeom& g, const float (&o)[3],
+                                                   const float (&d)[3], const float (&C)[3], const float (&gC)[3],
+                                                   unsigned long long* __restrict__ acc) {
   float t0, L;
   int n;
   if (!field_segment(o, d, g, t0, L, n)) return;
@@ -214,18 +190,78 @@ __global__ void __launch_bounds__(FIELD_THREADS) field_loss_grad_kernel(const fl
   field_flush(acc, cell, g.G, s);
 }
 
-// grad = acc / (XUNET_FIELD_FIXED_ONE 3N) + the total-variation gradient; loss_out[i - 1] = the data loss; acc cleared.
-__global__ void __launch_bounds__(256) field_finish_kernel(const float* __restrict__ grid, int G, int rays, float tv_density,
+// One drawn ray per thread: ray r of iteration i = *iter_dev is training pixel
+//   xu_mix64(seed * 0x9E3779B97F4A7C15 + i * 0xD1B54A32D192ED03 + r) mod (V S S)     (consistency.draw_rays restates it).
+// acc receives the gradient of the per-ray sum sum_ch (C - u)^2 w.r.t. the raw grid, and acc[4 G^3] the sum itself.
+__global__ void __launch_bounds__(FIELD_THREADS) field_loss_grad_kernel(const float* __restrict__ grid, FieldGeom g,
+                                                                         const float* __restrict__ views,
+                                                                         const float* __restrict__ kinv, const float* __restrict__ R,
+                                                                         const float* __restrict__ t, int V, int S, int rays,
+                                                                         const long long* __restrict__ iter_dev,
+                                                                         unsigned long long seed,
+                                                                         unsigned long long* __restrict__ acc) {
+  xu_grid_dep_sync();
+  const int r = blockIdx.x * FIELD_THREADS + threadIdx.x;
+  if (r >= rays) return;
+  const unsigned long long i = (unsigned long long)*iter_dev;
+  const long long npix = (long long)V * S * S;
+  const long long p = (long long)(xu_mix64(seed * 0x9E3779B97F4A7C15ULL + i * 0xD1B54A32D192ED03ULL + (unsigned long long)r) %
+                                  (unsigned long long)npix);
+  const int v = (int)(p / ((long long)S * S)), row = (int)(p / S % S), col = (int)(p % S);
+  float o[3], d[3], C[3], gC[3];
+  field_ray(kinv, R, t, v, row, col, o, d);
+  field_composite(grid, g, o, d, C);
+  float lsum = 0.f;
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    const float u = fminf(fmaxf((views[3 * p + ch] + 1.f) * 0.5f, 0.f), 1.f);
+    gC[ch] = 2.f * (C[ch] - u);
+    lsum += (C[ch] - u) * (C[ch] - u);
+  }
+  atomicAdd(acc + 4LL * g.G * g.G * g.G, (unsigned long long)field_fix(lsum));
+  field_ray_backward(grid, g, o, d, C, gC, acc);
+}
+
+// One pixel of V views per thread: acc receives the gradient of sum_ch dC_ch C_ch w.r.t. the raw grid, dC the given image
+// gradient (V, S, S, 3) in the caller's unit, a non-finite value read as 0.
+__global__ void __launch_bounds__(FIELD_THREADS) field_image_grad_kernel(const float* __restrict__ grid, FieldGeom g,
+                                                                          const float* __restrict__ dC,
+                                                                          const float* __restrict__ kinv, const float* __restrict__ R,
+                                                                          const float* __restrict__ t, int V, int S,
+                                                                          unsigned long long* __restrict__ acc) {
+  xu_grid_dep_sync();
+  const long long p = (long long)blockIdx.x * FIELD_THREADS + threadIdx.x;
+  if (p >= (long long)V * S * S) return;
+  const int v = (int)(p / ((long long)S * S)), row = (int)(p / S % S), col = (int)(p % S);
+  float gC[3];
+  bool any = false;
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    const float x = dC[3 * p + ch];
+    gC[ch] = isfinite(x) ? x : 0.f;
+    any |= gC[ch] != 0.f;
+  }
+  if (!any) return;                                       // every scattered word would be zero
+  float o[3], d[3], C[3];
+  field_ray(kinv, R, t, v, row, col, o, d);
+  field_composite(grid, g, o, d, C);
+  field_ray_backward(grid, g, o, d, C, gC, acc);
+}
+
+// grad = acc inv + the total-variation gradient (inv: 1 / (XUNET_FIELD_FIXED_ONE 3N) for the drawn rays' mean, unit /
+// XUNET_FIELD_FIXED_ONE for an image gradient in units of `unit`); loss_out[i - 1] = acc[4 G^3] inv when iter_dev is given; acc cleared.
+__global__ void __launch_bounds__(256) field_finish_kernel(const float* __restrict__ grid, int G, double inv, float tv_density,
                                                            float tv_color, const long long* __restrict__ iter_dev,
                                                            long long* __restrict__ acc, float* __restrict__ grad,
                                                            float* __restrict__ loss_out, long long loss_len) {
   xu_grid_dep_sync();
   const long long n = 4LL * G * G * G;
   const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
-  const double inv = 1.0 / (XUNET_FIELD_FIXED_ONE * 3.0 * (double)rays);
   if (e == 0) {
-    const long long i = *iter_dev;
-    if (i >= 1 && i <= loss_len) loss_out[i - 1] = (float)((double)acc[n] * inv);
+    if (iter_dev != nullptr) {
+      const long long i = *iter_dev;
+      if (i >= 1 && i <= loss_len) loss_out[i - 1] = (float)((double)acc[n] * inv);
+    }
     acc[n] = 0;
   }
   if (e >= n) return;
@@ -294,7 +330,27 @@ extern "C" int xunet_field_loss_grad(const float* grid, int G, float bound, cons
   xu_launch(field_loss_grad_kernel, cdiv(rays, FIELD_THREADS), FIELD_THREADS, 0, s, grid,
             field_geom(G, bound, near, step, background), views, (const float*)kinv, R, t, V, S, rays, iter_dev, seed,
             (unsigned long long*)acc);
-  xu_launch(field_finish_kernel, cdiv(4LL * G * G * G, 256), 256, 0, s, grid, G, rays, tv_density, tv_color, iter_dev, acc, grad,
-            loss_out, loss_len);
+  xu_launch(field_finish_kernel, cdiv(4LL * G * G * G, 256), 256, 0, s, grid, G, 1.0 / (XUNET_FIELD_FIXED_ONE * 3.0 * (double)rays),
+            tv_density, tv_color, iter_dev, acc, grad, loss_out, loss_len);
   return xu_launched("field_loss_grad");
+}
+
+extern "C" int xunet_field_image_grad(const float* grid, int G, float bound, const float* dC, double unit, const float* R,
+                                      const float* t, const float* K, float* kinv, int V, int S, float near, float step,
+                                      float background, float tv_density, float tv_color, long long* acc, float* grad,
+                                      void* stream) {
+  if (!grid || !dC || !R || !t || !K || !kinv || !acc || !grad) return xu_fail("xunet_field_image_grad: NULL pointer argument");
+  if (int rc = field_check("xunet_field_image_grad", G, bound, V, S, near, step, background)) return rc;
+  if ((long long)V * S * S > XUNET_FIELD_MAX_RAYS)
+    return xu_fail("xunet_field_image_grad: V S S = %lld pixels, need at most %d", (long long)V * S * S, XUNET_FIELD_MAX_RAYS);
+  if (!isfinite(unit) || !(unit > 0.0)) return xu_fail("xunet_field_image_grad: unit = %g, need a finite unit > 0", unit);
+  if (!isfinite(tv_density) || !isfinite(tv_color) || tv_density < 0.f || tv_color < 0.f)
+    return xu_fail("xunet_field_image_grad: tv weights %g, %g, need finite weights >= 0", tv_density, tv_color);
+  const cudaStream_t s = (cudaStream_t)stream;
+  xu_launch(kinv_kernel, cdiv(V, 64), 64, 0, s, K, kinv, V);
+  xu_launch(field_image_grad_kernel, cdiv((long long)V * S * S, FIELD_THREADS), FIELD_THREADS, 0, s, grid,
+            field_geom(G, bound, near, step, background), dC, (const float*)kinv, R, t, V, S, (unsigned long long*)acc);
+  xu_launch(field_finish_kernel, cdiv(4LL * G * G * G, 256), 256, 0, s, grid, G, unit / XUNET_FIELD_FIXED_ONE, tv_density, tv_color,
+            (const long long*)nullptr, acc, grad, (float*)nullptr, 0LL);
+  return xu_launched("field_image_grad");
 }
