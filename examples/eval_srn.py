@@ -10,6 +10,7 @@ instance is conditioned on one source view (view 64 by default) and every scored
     python examples/eval_srn.py cars_test --ckpt checkpoints_v --prefix ema --side 128 --prediction v --method dpmpp_2m \\
         --steps 25 --out eval_v/
     python examples/eval_srn.py cars_test --ckpt checkpoints_d6 --prefix ema --side 128 --steps 256 --distilled 6 --out eval_d6/
+    python examples/eval_srn.py cars_test --ckpt checkpoints_cd --prefix ema --side 128 --consistency 4 --out eval_cd4/
 
 Modes:
   independent  each target is sampled from the source alone (Sampler.sample, the reference's k = 1 sampler); the targets
@@ -18,9 +19,9 @@ Modes:
                in order, each step conditioned on a random view of the pool (the source and the targets generated so far);
                instances are batched --views-in-flight at a time.
 Writes out/metrics.jsonl (one {instance, view, psnr, ssim} line per scored view) and out/summary.json (mean PSNR, mean SSIM,
-the number of views, the prediction the checkpoint was read with, the distillation round --distilled, the forwards per
-view and the arguments), prints the summary as the last line of stdout, and with --save-views writes each
-generated view as out/views/<instance>_<view>.png.  Seeds derive from --seed, so equal arguments give equal files.
+the number of views, the prediction the checkpoint was read with, the distillation round --distilled, the consistency
+sampling steps --consistency and the teacher grid's N of a consistency student, the forwards per view and the arguments),
+prints the summary as the last line of stdout, and with --save-views writes each generated view as out/views/<instance>_<view>.png.  Seeds derive from --seed, so equal arguments give equal files.
 """
 import argparse
 import json
@@ -32,6 +33,9 @@ import numpy as np
 
 import novel_view_synthesis_3d_b200 as P
 from novel_view_synthesis_3d_b200.srn_data import SRNScenes
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from distill_srn import cd_steps  # noqa: E402
 
 
 def select_targets(n_views: int, source: int, count: int) -> list:
@@ -69,6 +73,11 @@ def main():
                     help='sample a student distilled R times (examples/distill_srn.py) from a --steps-step teacher: DDIM '
                          '(eta 0) on distill_grid(--steps, R) without guidance, reading v; --method, --eta, --spacing, --w '
                          'and --prediction are then ignored')
+    ap.add_argument('--consistency', type=int, default=0, metavar='K',
+                    help='sample a consistency-distilled student (examples/distill_srn.py --consistency N) in K steps: '
+                         'multistep consistency sampling on consistency_grid(N, K) without guidance, reading v, with N read '
+                         'from the state<step> checkpoint in --ckpt (a directory); --steps, --method, --eta, --spacing, --w '
+                         'and --prediction are then ignored')
     ap.add_argument('--source-view', type=int, default=64, help='conditioning view of every instance (pixelNeRF / 3DiM: 64)')
     ap.add_argument('--targets', type=int, default=0, help='target views per instance, spaced evenly; 0 = all other views')
     ap.add_argument('--max-instances', type=int, default=-1, help='score the first N instances of the sorted list')
@@ -91,7 +100,11 @@ def main():
             raise SystemExit(f"instance {ds.instances[i]['name']} has {n} views; --source-view {a.source_view} does not exist")
         insts.append((i, select_targets(n, a.source_view, a.targets)))
     B = a.views_in_flight
-    if a.distilled:
+    if a.consistency:
+        sampler = P.Sampler(P.XUNet(), params, B, a.side, w=None, method='consistency', prediction='v',
+                            timesteps=P.consistency_grid(cd_steps(a.ckpt), a.consistency),
+                            dynamic_threshold=a.dynamic_threshold)
+    elif a.distilled:
         sampler = P.Sampler(P.XUNet(), params, B, a.side, w=None, method='ddim', prediction='v',
                             timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold)
     else:
@@ -149,8 +162,9 @@ def main():
             fh.write(json.dumps(rec) + '\n')
     summary = dict(mean_psnr=float(np.mean([r['psnr'] for r in records])) if records else float('nan'),
                    mean_ssim=float(np.mean([r['ssim'] for r in records])) if records else float('nan'),
-                   n_views=len(records), prediction='v' if a.distilled else a.prediction, distilled=a.distilled,
-                   sampler_steps=len(sampler.sched), args=vars(a))
+                   n_views=len(records), prediction='v' if a.distilled or a.consistency else a.prediction,
+                   distilled=a.distilled, consistency=a.consistency,
+                   cd_steps=cd_steps(a.ckpt) if a.consistency else None, sampler_steps=len(sampler.sched), args=vars(a))
     with open(os.path.join(a.out, 'summary.json'), 'w') as fh:
         json.dump(summary, fh, indent=1)
     print(json.dumps(summary))

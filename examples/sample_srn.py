@@ -6,6 +6,7 @@ ancestral sampler, write PNGs (the reference blocks in cv2.imshow, which cannot 
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --method dpmpp_2m --steps 25 --out results_dpm/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_v --prediction v --method dpmpp_2m --steps 25 --out results_v/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_d1 --prefix ema --distilled 1 --steps 256 --out results_d1/
+    python examples/sample_srn.py cars_train_val --ckpt checkpoints_cd --prefix ema --consistency 2 --out results_cd2/
 """
 import argparse
 import os
@@ -16,6 +17,9 @@ import numpy as np
 
 import novel_view_synthesis_3d_b200 as P
 from novel_view_synthesis_3d_b200.srn_data import SRNScenes
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from distill_srn import cd_steps  # noqa: E402
 
 
 def main():
@@ -38,6 +42,11 @@ def main():
                     help='sample a student distilled R times (examples/distill_srn.py) from a --steps-step teacher: DDIM '
                          '(eta 0) on distill_grid(--steps, R) without guidance, reading v; --method, --eta, --spacing, --w '
                          'and --prediction are then ignored')
+    ap.add_argument('--consistency', type=int, default=0, metavar='K',
+                    help='sample a consistency-distilled student (examples/distill_srn.py --consistency N) in K steps: '
+                         'multistep consistency sampling on consistency_grid(N, K) without guidance, reading v, with N read '
+                         'from the state<step> checkpoint in --ckpt (a directory); --steps, --method, --eta, --spacing, --w '
+                         'and --prediction are then ignored')
     ap.add_argument('--views', type=int, default=1)
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--out', default='results')
@@ -51,7 +60,11 @@ def main():
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50)
     batch = next(ds.batches(a.views))
     model = P.XUNet()
-    if a.distilled:
+    if a.consistency:
+        sampler = P.Sampler(model, params, a.views, a.side, w=None, method='consistency', prediction='v',
+                            timesteps=P.consistency_grid(cd_steps(a.ckpt), a.consistency),
+                            dynamic_threshold=a.dynamic_threshold)
+    elif a.distilled:
         sampler = P.Sampler(model, params, a.views, a.side, w=None, method='ddim', prediction='v',
                             timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold)
     else:

@@ -458,6 +458,32 @@ int xunet_distill_target(const float* out_t, float w, int teacher_copies, const 
                          const int* m_dev, const float* z_t, const float* teacher_z, int B, long long per, float* v_out,
                          void* stream);
 
+/* The teacher step of CONSISTENCY DISTILLATION (Song et al. 2023, Consistency Models, Alg. 2; guided as in LCM).  The teacher
+ * grid G holds N timesteps in loop order; sample b sits at position n = m_b (m_dev: device (B) int32 from
+ * xunet_srn_batch_distill with grid_t = G, n_grid = N).  teacher_table: device (N, 8) floats, the teacher's DDIM (eta = 0)
+ * sampler table on G with log-SNR lag off (sampling.sampler_table), its last row going to alpha-bar 1.  Element i of sample b
+ * (per = S*S*3 values each, n = B*per) applies row r = m_b exactly as xunet_sampler_step_table at pos = r does (fp32, as nvcc
+ * contracts it, sigma = 0):
+ *   out = (1+w) out_c - w out_u (teacher_copies = 2: out_t = [out_c ; out_u], 2n floats) or out_c (teacher_copies = 1, w unused);
+ *   x0 = clip(c_recip z_t - c_recipm1 out, -1, 1);   z^ = c_x0 x0 + c_z z_t,
+ * reading z_t (device, n floats: the sample's z) and writing z^ to z_out (device, n floats: the target batch's z, not the
+ * teacher's), and row r's column 5 (the log-SNR of t_{r+1}) to logsnr_out[b] (device, B floats).  On the last row z^ is the
+ * teacher's clipped x0.  Errors: a NULL pointer, B < 1, per < 1, teacher_copies not 1 or 2.  One launch; graph-capturable. */
+int xunet_cd_teacher_step(const float* out_t, float w, int teacher_copies, const float* teacher_table, const int* m_dev, int B,
+                          long long per, const float* z_t, float* z_out, float* logsnr_out, void* stream);
+
+/* The consistency-distillation target.  v_minus: device (n floats), the output of the target network (the student's current
+ * weights, no dropout, cond_mask 1) at (z^, log-SNR(t_{n+1})); target_table: device (N, 4) floats, row n = {a, b, alpha_n,
+ * sigma_n} with a = alpha_{n+1}, b = sigma_{n+1} and (a, b) = (1, 0) on the last row (fp64, rounded once); z_t, z_hat: the
+ * sample's z and xunet_cd_teacher_step's z^.  Element i of sample b, with row m_b:
+ *   x0- = clip(a z^ - b v-, -1, 1)     (the sampler's x0 expression, as nvcc contracts it: clip(fma(a, z^, -(b v-))))
+ *   v*  = __fdiv_rn(__fsub_rn(__fmul_rn(alpha_n, z_t), x0-), sigma_n)
+ * stored to v_out (device, n floats: the student slot's regression target).  A student whose v output is v* has the consistency
+ * function f(z_t, t_n) = alpha_n z_t - sigma_n v* = x0-; on the last row x0- = z^.  Errors: a NULL pointer, B < 1, per < 1.
+ * One launch; graph-capturable. */
+int xunet_cd_target(const float* v_minus, const float* target_table, const int* m_dev, const float* z_t, const float* z_hat,
+                    int B, long long per, float* v_out, void* stream);
+
 /* The dropout keep-mask the kernels use for residual-block `op_index` (0/1 floats, device), so tests can
  * hand the identical mask to the oracle (nn.Dropout, model/xunet.py:84). */
 int xunet_dropout_mask(float* mask_out, long long n, int op_index, unsigned long long seed, float rate,

@@ -18,7 +18,7 @@ OBJ_DIR = ROOT / 'build' / 'obj'
 LIB = PKG / 'libxunet_b200.so'
 SOURCES = ['engine.cu', 'kernels_conv.cu', 'kernels_elem.cu', 'kernels_attn.cu', 'conv_tc.cu', 'attn_tc.cu', 'wgrad_tc.cu', 'metrics.cu',
            'sampler.cu', 'data.cu', 'pose_grad.cu', 'distill.cu', 'field.cu', 'pose_fit.cu',
-           'lift.cu']
+           'lift.cu', 'cd.cu']
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 NVCC_FLAGS = [*ARCH, '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-I', str(INCLUDE), '-I', str(CSRC)]

@@ -17,6 +17,10 @@ the guidance (1 + w) out_c - w out_u is linear in the output.
 w=None samples a model whose guidance is in its weights, such as a progressively distilled student (distill.py): one
 B-batch conditional forward per step, stepped by `xunet_sampler_step_cond`.  `distill_grid` gives the timesteps such a
 student was trained on, and `Schedule(timesteps=...)` the schedule of any such grid.
+
+method='consistency' samples a consistency-distilled student (distill.ConsistencyTeacher) by multistep consistency sampling
+(Song et al. 2023, Alg. 1): x0 = clip(f(z, t_k)), then z' = alpha' x0 + sigma' eps' with fresh noise, landing on x0 after
+the last step.  `consistency_grid` gives its timesteps.
 """
 from __future__ import annotations
 
@@ -47,6 +51,8 @@ def logsnr_schedule_cosine(t, *, logsnr_min=-20., logsnr_max=20.):
 
 
 METHODS = ('ddpm', 'ddim', 'dpmpp_2m')
+# every sampler method: the teacher samplers, and multistep consistency sampling of a consistency-distilled student
+SAMPLER_METHODS = METHODS + ('consistency',)
 SPACINGS = ('linear', 'logsnr')
 PREDICTIONS = ('eps', 'v')
 
@@ -127,9 +133,24 @@ def distill_grid(teacher_steps: int, rounds: int) -> np.ndarray:
     return g.copy()
 
 
+def consistency_grid(teacher_steps: int, k: int) -> np.ndarray:
+    """The K sampling timesteps, in loop order, of a student consistency-distilled (distill.ConsistencyTeacher) on the
+    teacher grid G = distill_grid(teacher_steps, 0) of N timesteps: G[(i N) // K] for i = 0..K-1.  The top timestep is
+    kept and every point is a grid position the student was trained at; K = N gives G.  Raises ValueError for
+    teacher_steps < 1, K < 1 or K > N."""
+    for name, v in (('teacher_steps', teacher_steps), ('k', k)):
+        if isinstance(v, bool) or int(v) != v or v < 1:
+            raise ValueError(f'{name} must be an integer >= 1, got {v!r}')
+    g = distill_grid(int(teacher_steps), 0)
+    n, k = len(g), int(k)
+    if k > n:
+        raise ValueError(f'k = {k} sampling steps, more than the N = {n} timesteps of the teacher grid')
+    return g[(np.arange(k) * n) // k].copy()
+
+
 def _check_method(method: str, eta: float) -> None:
-    if method not in METHODS:
-        raise ValueError(f'unknown sampler method {method!r}; expected one of {METHODS}')
+    if method not in SAMPLER_METHODS:
+        raise ValueError(f'unknown sampler method {method!r}; expected one of {SAMPLER_METHODS}')
     if not 0.0 <= eta <= 1.0:
         raise ValueError(f'eta {eta} outside [0, 1]')
     if eta != 0.0 and method != 'ddim':
@@ -146,7 +167,7 @@ def _check_dynamic_threshold(p) -> None:
         raise ValueError(f'dynamic_threshold {p} outside (0, 1]')
 
 
-def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, logsnr_lag: bool = True,
+def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, logsnr_lag: bool | None = None,
                   prediction: str = 'eps'):
     """The device table of `sched` for `method`: (rows, logsnr_first), rows (len(sched), 8) float64 (the sampler rounds
     them to fp32 once), row k = loop position k = timestep index len-1-k = {c_recip, c_recipm1, c_x0, c_z, sigma,
@@ -162,12 +183,17 @@ def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, lo
                 c_x0 = sqrt(abar') - c_z alpha: DDIM with eps re-derived from the clipped x0 (eta = 1: the ddpm rows);
       dpmpp_2m  h = lambda' - lambda, r = h_prev / h, g = alpha' (1 - e^-h), c_z = sigma_t' / sigma_t,
                 c_x0 = g (1 + 1/(2r)), c_prev = -g / (2r), sigma = 0; the first and the last row are first order
-                (c_x0 = g, c_prev = 0), so the last step, to abar' = 1, is z' = x0.
-    ddim and dpmpp_2m read only sched.timesteps and the matching leading entries of sched.alphas_cumprod.
+                (c_x0 = g, c_prev = 0), so the last step, to abar' = 1, is z' = x0;
+      consistency  multistep consistency sampling (Song et al. 2023, Alg. 1): c_x0 = sqrt(abar'), c_z = 0,
+                sigma = sqrt(1 - abar'), c_prev = 0: z' = alpha' x0 + sigma' noise, and the last step is z' = x0.
+    ddim, dpmpp_2m and consistency read only sched.timesteps and the matching leading entries of sched.alphas_cumprod.
     logsnr_lag=True: the reference's lag (sampling.py:126,151): the first forward gets -20 and row k hands the next forward
     the log-SNR of its own timestep t_k.  logsnr_lag=False: each forward gets the log-SNR of the timestep z is at,
-    logsnr_cosine(t_0/1000) first and logsnr_cosine(t_{k+1}/1000) from row k (the last row's value is unused)."""
+    logsnr_cosine(t_0/1000) first and logsnr_cosine(t_{k+1}/1000) from row k (the last row's value is unused).
+    None (default): True, but False for consistency, whose student was trained without the lag."""
     _check_method(method, eta)
+    if logsnr_lag is None:
+        logsnr_lag = method != 'consistency'
     check_prediction(prediction)
     sc = sched
     n = len(sc.timesteps)
@@ -189,6 +215,8 @@ def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, lo
             keep = (1. - eta ** 2) + eta ** 2 * a * (1. - a_next) / (a_next * (1. - a))
             c_z = np.sqrt((1. - a_next) * keep) / np.sqrt(1. - a)
             c_x0 = np.sqrt(a_next) - c_z * np.sqrt(a)
+        elif method == 'consistency':
+            sigma, c_z, c_x0 = np.sqrt(1. - a_next), zero, np.sqrt(a_next)
         else:
             sigma = zero
             c_z = np.sqrt((1. - a_next) / (1. - a))
@@ -218,8 +246,10 @@ class Sampler:
     so one sampler step is the 2B-batch forward, `xunet_sampler_step_table` and pos += 1, with no host arithmetic in between.
     use_graph=True replays that step as one CUDA graph; use_graph=False issues the same calls eagerly.
 
-    method: 'ddpm' (the reference's ancestral sampler), 'ddim' (eta in [0, 1]; 0 = deterministic) or 'dpmpp_2m'
-    (DPM-Solver++(2M); its step is `xunet_sampler_step_multistep`, with the previous step's x0 in a device buffer).
+    method: 'ddpm' (the reference's ancestral sampler), 'ddim' (eta in [0, 1]; 0 = deterministic), 'dpmpp_2m'
+    (DPM-Solver++(2M); its step is `xunet_sampler_step_multistep`, with the previous step's x0 in a device buffer) or
+    'consistency' (multistep consistency sampling of a consistency-distilled student, usually with w=None,
+    prediction='v' and timesteps=consistency_grid(N, K); the same table step kernels).
     spacing: the Schedule's timestep spacing, 'logsnr' for dpmpp_2m and 'linear' otherwise by default; len(self.sched)
     is the number of forwards a sample runs.  logsnr_lag: the reference's one-step lag of the network's log-SNR input,
     on by default for ddpm with prediction='eps' only (see `sampler_table`).  With every default this is the reference

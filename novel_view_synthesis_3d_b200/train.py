@@ -90,8 +90,8 @@ class TrainState:
     # what the network is trained to predict: 'eps' (the noise) or 'v' (sqrt(abar) eps - sqrt(1 - abar) x0); recorded in
     # the checkpoint
     prediction: str = 'eps'
-    # a progressively distilled student's {teacher_steps, rounds[, w]} (distill.Teacher.record); None for any other model.
-    # Recorded in the checkpoint
+    # a progressively distilled student's {teacher_steps, rounds[, w]} (distill.Teacher.record), a consistency-distilled one's
+    # {cd_steps[, w]} (distill.ConsistencyTeacher.record); None for any other model.  Recorded in the checkpoint
     distill: Optional[dict] = None
     _mask_rng: np.random.RandomState = None
     _frozen_mask: Optional[np.ndarray] = None
@@ -375,6 +375,12 @@ class TrainStep:
     clipping, warm-up, EMA, data parallelism and the single-graph capture -- is the data= step's.  Raises ValueError without
     data=, for a state that is not prediction='v' with loss='mse', with reference_quirks or min_snr_gamma, for an odd teacher
     grid, and when the teacher's S, B, device or model configuration differ from the state's.
+
+    teacher=distill.ConsistencyTeacher (with data=): consistency distillation, with the same checks (but any grid of N >= 2).
+    Per micro-batch the step draws t on the teacher grid, runs the teacher forward and its DDIM step (xunet_cd_teacher_step),
+    then the target forward -- this state's own parameters, train=0, on its training engine, at the stepped z -- and the
+    target kernel (xunet_cd_target), which writes v* into the slot's regression target; the student's forward and backward
+    follow as above.
     """
 
     def __init__(self, state: TrainState, *, use_graph: bool = True, bucket_mb: float = 128.0, allreduce: bool = True,

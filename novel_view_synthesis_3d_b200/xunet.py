@@ -308,20 +308,27 @@ class Engine:
         return int(self.lib.xunet_grad_bucket_count(self.h))
 
     def forward(self, flat_params: torch.Tensor, *, train: bool, seed: Optional[int] = None,
-                inputs: Optional[Tuple[InputSlots, int]] = None, seed_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """inputs=(slots, j): read slot j of `slots` instead of the engine's own inputs; seed_dev: a device int64 to read the
-        dropout seed from instead of `self.seed` (both default to the engine's own buffers)."""
+                inputs: Optional[Tuple[InputSlots, int]] = None, seed_dev: Optional[torch.Tensor] = None,
+                batch: Optional[_lib.XunetBatch] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """inputs=(slots, j): read slot j of `slots` instead of the engine's own inputs; batch: an xunet_batch of device
+        pointers to read instead of either; seed_dev: a device int64 to read the dropout seed from instead of `self.seed`
+        (all default to the engine's own buffers).  out: a contiguous fp32 device tensor of `self.eps`'s shape to write the
+        output to instead of `self.eps`.  Returns the output."""
         assert flat_params.dtype == torch.float32 and flat_params.is_cuda and flat_params.numel() == self.nparams
+        if out is not None and not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous()
+                                    and out.shape == self.eps.shape):
+            raise ValueError(f'out must be a contiguous fp32 device tensor of shape {tuple(self.eps.shape)}')
         if seed is not None:
             self.seed.fill_(int(seed) & 0x7FFFFFFFFFFFFFFF)
-        cb = self.cbatch if inputs is None else inputs[0].cbatch[inputs[1]]
+        cb = batch if batch is not None else self.cbatch if inputs is None else inputs[0].cbatch[inputs[1]]
         sd = self.seed if seed_dev is None else seed_dev
         st = torch.cuda.current_stream(self.device).cuda_stream
+        y = self.eps if out is None else out
         self.forward_count += 1
-        self._fwd_rays = self.rays if inputs is None else None
+        self._fwd_rays = self.rays if inputs is None and batch is None else None
         _lib.check(self.lib.xunet_forward(self.h, flat_params.data_ptr(), C.byref(cb), int(train),
-                                          sd.data_ptr(), self.ws.data_ptr(), self.eps.data_ptr(), st), 'xunet_forward')
-        return self.eps
+                                          sd.data_ptr(), self.ws.data_ptr(), y.data_ptr(), st), 'xunet_forward')
+        return y
 
     def backward(self, flat_params: torch.Tensor, *, accumulate: bool = False, inputs: Optional[Tuple[InputSlots, int]] = None,
                  seed_dev: Optional[torch.Tensor] = None, loss_out: Optional[torch.Tensor] = None, loss: str = 'frobenius',
