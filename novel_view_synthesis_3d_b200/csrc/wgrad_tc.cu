@@ -263,8 +263,9 @@ void launch_wgrad_tc(const WgradArgs& a, cudaStream_t s) {
   dim3 grid((unsigned)tiles_m, (unsigned)tiles_n, (unsigned)ksplit);
   {
     static const bool log = getenv("XUNET_CONV_LOG") != nullptr;      // tools/conv_step_profile.py matches these lines with CUPTI times
-    if (log) fprintf(stderr, "wgrad_tc N=%d %dx%d Ci=%d Co=%d ks=%d st=%d BN=%d ksplit=%d tm=%d tn=%d stages=%d ptiles=%d\n", a.N, a.Ho, a.Wo, a.Ci,
-                     a.Co, a.ks, a.stride, p.BN, ksplit, tiles_m, tiles_n, p.stages, p.ptiles);
+    // cwa / cwb: the kernel's <CWA, CWB> (channels per A / B block); MB: the (tap, ci-chunk) blocks of M, G = 128 / cwa per tile
+    if (log) fprintf(stderr, "wgrad_tc N=%d %dx%d Ci=%d Co=%d ks=%d st=%d BN=%d ksplit=%d tm=%d tn=%d stages=%d ptiles=%d cwa=%d cwb=%d MB=%d\n", a.N,
+                     a.Ho, a.Wo, a.Ci, a.Co, a.ks, a.stride, p.BN, ksplit, tiles_m, tiles_n, p.stages, p.ptiles, cwa, cwb, p.MB);
   }
   if (cwa == 64 && cwb == 64) launch_wg<64, 64>(tx, ty, p, smem, grid, s);
   else if (cwa == 64) launch_wg<64, 32>(tx, ty, p, smem, grid, s);

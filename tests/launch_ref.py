@@ -57,16 +57,30 @@ def plan_launches(lib, cfg, B, S, dtype, training):
         lib.xunet_destroy(h)
 
 
-def unique_launches(lib):
-    """every launch of PLANS once, deduplicated by what changes the launch: [(id, dtype, training, launch)], the id naming the
-    first plan and leaf (conv) or attention index that has it.  An attention's backward runs in training plans only."""
+def plan_config(cfg):
+    """a plan's model configuration: a preset's name (PLANS) or an XUNetConfig"""
     import novel_view_synthesis_3d_b200 as P
+    return getattr(P, cfg) if isinstance(cfg, str) else cfg
+
+
+def launch_key(dtype, training, r):
+    """what changes a launch: two launches with one key run the same kernels on the same shapes and arguments"""
+    return (r['kind'], dtype) + (tuple(r[k] for k in CONV_KEY) if r['kind'] == 0 else (training,) + tuple(r[k] for k in ATTN_KEY))
+
+
+def unique_launches(lib, plans=PLANS, exclude=None):
+    """every launch of `plans` (name -> (preset name or XUNetConfig, side, batch, dtype, training)) once, deduplicated by what
+    changes the launch: [(id, dtype, training, launch)], the id naming the first plan and leaf (conv) or attention index that
+    has it.  Launches that the plans of `exclude` also have are left out.  An attention's backward runs in training plans
+    only."""
     seen, out = set(), []
-    for plan, (preset, S, B, dtype, training) in PLANS.items():
-        launches, names = plan_launches(lib, getattr(P, preset), B, S, dtype, training)
+    if exclude is not None:
+        seen.update(launch_key(dtype, training, r) for _, dtype, training, r in unique_launches(lib, exclude))
+    for plan, (cfg, S, B, dtype, training) in plans.items():
+        launches, names = plan_launches(lib, plan_config(cfg), B, S, dtype, training)
         na = 0
         for r in launches:
-            key = (r['kind'], dtype) + (tuple(r[k] for k in CONV_KEY) if r['kind'] == 0 else (training,) + tuple(r[k] for k in ATTN_KEY))
+            key = launch_key(dtype, training, r)
             if r['kind'] == 1:
                 na += 1
             if key in seen:
@@ -334,9 +348,9 @@ def attn_qkv(N, L, C, heads, peaked, g):
     """attention inputs (N, L, 3C): per-channel offsets on q, k and v, and per-frame offsets on v, so that a routing error
     between frames, heads or channels shows.  peaked: the scores grow from key block to key block (a 64-key ramp along one
     direction u per head), with a step of 6 / sqrt(hd) u before the last block, so that every query's largest score lies in the
-    last 64-key block and the online softmax rescales its state on the way there."""
+    last 64-key block (a partial one when L % 64 != 0) and the online softmax rescales its state on the way there."""
     hd = C // heads
-    nb = L // 64
+    nb = (L + 63) // 64
     ch = torch.arange(3 * C, dtype=torch.float64)
     fr = torch.arange(N, dtype=torch.float64)[:, None, None]
     if not peaked:

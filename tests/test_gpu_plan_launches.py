@@ -20,7 +20,6 @@ import numpy as np
 import pytest
 import torch
 
-import novel_view_synthesis_3d_b200 as P
 from novel_view_synthesis_3d_b200 import _lib
 from tests import groupnorm_ref as G
 from tests import launch_ref as L
@@ -66,8 +65,8 @@ def _check(name, what, got, ref, bound):
                        f'{float(got.reshape(-1)[i]):.6g}, ref {float(ref.reshape(-1)[i]):.6g}, bound {float(bound.reshape(-1)[i]):.3g}')
 
 
-@pytest.mark.parametrize('case', CONVS, ids=[u[0] for u in CONVS])
-def test_conv_launch(lib, case):
+def check_conv(lib, case, plans=L.PLANS):
+    """the forward, data gradient and weight gradient of one conv launch (name, dtype, training, launch) of `plans` against fp64"""
     name, dtype, training, r = case
     N, Hi, Wi, Ci, Ho, Wo, Co = (r[k] for k in ('N', 'Hi', 'Wi', 'Ci', 'Ho', 'Wo', 'Co'))
     ks, st, nseg, alpha, balpha = r['ksize'], r['stride'], r['nseg'], r['alpha'], r['bwd_alpha']
@@ -107,7 +106,7 @@ def test_conv_launch(lib, case):
     dyd = dy.to(DT[dtype])
     if r['gn_mode'] >= 0:
         # the data gradient carries the GroupNorm backward: the fused epilogue at this shape and mode
-        cfg_rate = getattr(P, L.PLANS[name.split(':')[0]][0]).dropout
+        cfg_rate = L.plan_config(plans[name.split(':')[0]][0]).dropout
         rg = torch.Generator().manual_seed(zlib.crc32((name + ':epi').encode()))
         ep = _run_epi(lib, rg, N, Hi, Wi, Ci, Co, ks, nseg, r['gn_mode'], balpha, cfg_rate, 1)
         _check_epi(ep, N, Hi, Wi, Ci, Co, ks, nseg, r['gn_mode'], balpha, cfg_rate, 1)
@@ -137,9 +136,8 @@ def test_conv_launch(lib, case):
         _check(name, 'wgrad dbias', db, rdb, bdb)
 
 
-@pytest.mark.parametrize('peaked', [False, True], ids=['moderate', 'peaked'])
-@pytest.mark.parametrize('case', ATTNS, ids=[u[0] for u in ATTNS])
-def test_attention_launch(lib, case, peaked):
+def check_attention(lib, case, peaked):
+    """the forward and, in a training plan, the backward of one attention launch (name, dtype, training, launch) against fp64"""
     name, dtype, training, r = case
     N, Lk, C, heads, cross, impl = (r[k] for k in ('N', 'L', 'C', 'heads', 'cross', 'impl'))
     bf = dtype == 1
@@ -188,6 +186,17 @@ def test_attention_launch(lib, case, peaked):
     assert rel < (4e-2 if bf else 1e-4), rel
 
 
+@pytest.mark.parametrize('case', CONVS, ids=[u[0] for u in CONVS])
+def test_conv_launch(lib, case):
+    check_conv(lib, case)
+
+
+@pytest.mark.parametrize('peaked', [False, True], ids=['moderate', 'peaked'])
+@pytest.mark.parametrize('case', ATTNS, ids=[u[0] for u in ATTNS])
+def test_attention_launch(lib, case, peaked):
+    check_attention(lib, case, peaked)
+
+
 # ======================================================================================================================
 # which tensor-core variants the plan-derived launches reach, read from the launchers' log in a child process
 # ======================================================================================================================
@@ -230,19 +239,32 @@ def _launch_all_convs(cases=None):
         torch.cuda.synchronize()
 
 
-def test_tensor_core_variants_reached(lib):
+def logged_variants(code):
+    """(conv_tc lines, wgrad_tc lines) the launchers log while a child process runs `code` (python), each line as a dict of its
+    integer fields, its output size (H, W) and the case `code` last named in a 'CASE <id>' line on stderr, in launch order"""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     env = dict(os.environ, XUNET_CONV_LOG='1')
-    r = subprocess.run([sys.executable, '-c', 'from tests.test_gpu_plan_launches import _launch_all_convs; _launch_all_convs()'],
-                       cwd=root, env=env, capture_output=True, text=True, timeout=900)
+    r = subprocess.run([sys.executable, '-c', code], cwd=root, env=env, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    conv, wgrad = [], []
+    conv, wgrad, case = [], [], None
     for line in r.stderr.splitlines():
+        if line.startswith('CASE '):
+            case = line[5:]
+            continue
         kv = {k: int(v) for k, v in re.findall(r'(\w+)=(-?\d+)', line)}
+        hw = re.search(r' (\d+)x(\d+) ', line)
+        if hw:
+            kv['H'], kv['W'] = int(hw.group(1)), int(hw.group(2))
+        kv['case'] = case
         if line.startswith('conv_tc mode='):
             conv.append(kv)
         elif line.startswith('wgrad_tc '):
             wgrad.append(kv)
+    return conv, wgrad
+
+
+def test_tensor_core_variants_reached(lib):
+    conv, wgrad = logged_variants('from tests.test_gpu_plan_launches import _launch_all_convs; _launch_all_convs()')
     reached = {
         'BN 32': any(c['BN'] == 32 for c in conv),
         'BN 64': any(c['BN'] == 64 for c in conv),

@@ -22,6 +22,10 @@ from tests.test_gpu_plan_launches import DT, F64, _check, _gen, _offsets, _q, _r
 
 pytestmark = pytest.mark.gpu
 
+def _op_key(dtype, training, o):
+    return (dtype, training) + tuple(o[k] for k in O.OP_KEY)
+
+
 POSE_PLANS = {
     'small64_posemb': (dataclasses.replace(P.SMALL, use_pos_emb=True, use_ref_pose_emb=True), 64, 8, 1, 1),
     'small64_posemb_f32': (dataclasses.replace(P.SMALL, use_pos_emb=True, use_ref_pose_emb=True), 64, 2, 0, 1),
@@ -29,14 +33,18 @@ POSE_PLANS = {
 }
 
 
-def _unique_ops(lib):
-    """every op of launch_ref.PLANS and POSE_PLANS once, deduplicated by what changes its launches: [(id, dtype, training, op)]"""
-    plans = {k: (getattr(P, v[0]),) + v[1:] for k, v in L.PLANS.items()}
-    plans.update(POSE_PLANS)
+def _unique_ops(lib, plans=None, exclude=None):
+    """every op of `plans` (name -> (preset name or XUNetConfig, side, batch, dtype, training); default launch_ref.PLANS and
+    POSE_PLANS) once, deduplicated by what changes its launches: [(id, dtype, training, op)].  Ops that the plans of `exclude`
+    also have are left out."""
+    if plans is None:
+        plans = dict(L.PLANS, **POSE_PLANS)
     seen, out = set(), []
+    if exclude is not None:
+        seen.update(_op_key(dtype, training, o) for _, dtype, training, o in _unique_ops(lib, exclude))
     for plan, (cfg, S, B, dtype, training) in plans.items():
-        for i, o in enumerate(O.plan_ops(lib, cfg, B, S, dtype, training)):
-            key = (dtype, training) + tuple(o[k] for k in O.OP_KEY)
+        for i, o in enumerate(O.plan_ops(lib, L.plan_config(cfg), B, S, dtype, training)):
+            key = _op_key(dtype, training, o)
             if key in seen:
                 continue
             seen.add(key)
@@ -386,3 +394,9 @@ def test_loss_op(lib, case):
 def test_loss_of_zero(lib, dtype):
     """eps_hat == eps: loss 0 gives dO = 0, not NaN"""
     _run_loss(lib, f'loss zero dtype={dtype}', dtype, 2, 20, zero=True)
+
+
+# the check of each op kind, for op lists built from other plans (tests/test_gpu_plan_sweep.py)
+OP_CHECKS = {_lib.PLAN_OP_LOGSNR: test_logsnr_op, _lib.PLAN_OP_POSE: test_pose_op, _lib.PLAN_OP_EMB: test_film_emb_op,
+             _lib.PLAN_OP_RESAMPLE: test_resample_op, _lib.PLAN_OP_CONCAT: test_concat_op,
+             _lib.PLAN_OP_ATTN_RESIDUAL: test_attn_residual_op, _lib.PLAN_OP_LOSS: test_loss_op}
