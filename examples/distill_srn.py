@@ -68,6 +68,9 @@ def main():
     ap.add_argument('--save-every', type=int, default=1000)
     ap.add_argument('--dtype', default='bf16')
     ap.add_argument('--ema-decay', type=float, default=None)
+    ap.add_argument('--posthoc-ema', type=float, nargs=2, default=None, metavar=('S1', 'S2'),
+                    help="keep two power-function averages of the student's weights (see train_srn.py --posthoc-ema)")
+    ap.add_argument('--snapshot-every', type=int, default=1000)
     ap.add_argument('--max-grad-norm', type=float, default=None)
     ap.add_argument('--warmup-steps', type=int, default=0)
     ap.add_argument('--grad-accum-steps', type=int, default=1)
@@ -80,6 +83,10 @@ def main():
         ap.error('--round must be >= 1')
     if a.consistency < 0 or a.consistency == 1:
         ap.error('--consistency N needs N >= 2')
+    if a.posthoc_ema is not None and a.ema_decay is not None:
+        ap.error('--posthoc-ema and --ema-decay are exclusive')
+    if a.snapshot_every < 1:
+        ap.error('--snapshot-every must be >= 1')
     xdist.init_from_env('nccl')
     rank = xdist.rank()
     params = P.checkpoint.restore_checkpoint(a.teacher_ckpt, prefix=a.teacher_prefix)
@@ -95,7 +102,7 @@ def main():
                             w=a.w if first else None, prediction=a.teacher_prediction if first else 'v', rounds=a.round - 1)
     del params
     state = P.create_distill_state(teacher, a.lr, ema_decay=a.ema_decay, max_grad_norm=a.max_grad_norm,
-                                   warmup_steps=a.warmup_steps)
+                                   warmup_steps=a.warmup_steps, posthoc_ema=a.posthoc_ema)
     if rank == 0 and a.consistency:
         print(f'consistency distillation: teacher DDIM on {len(teacher.grid)} timesteps (w = {a.w:g})')
     elif rank == 0:

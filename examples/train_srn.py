@@ -6,6 +6,7 @@ state (state<step>: params, Adam moments and count, EMA, cond_mask streams) that
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 1000 --ema-decay 0.9999
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --steps 2000 --ema-decay 0.9999 --resume
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --max-grad-norm 1 --warmup-steps 5000 --ema-decay 0.9999
+    python examples/train_srn.py cars_train_val --batch 8 --side 64 --posthoc-ema 0.05 0.10 --snapshot-every 1000
     python examples/train_srn.py cars_train_val --batch 4 --side 128 --grad-accum-steps 8     # 32 samples per update
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --loss mse --min-snr-gamma 5
     python examples/train_srn.py cars_train_val --batch 8 --side 64 --loss mse --prediction v --device-data
@@ -36,6 +37,11 @@ def main():
     ap.add_argument('--dtype', default='bf16')
     ap.add_argument('--ema-decay', type=float, default=None,
                     help='keep an exponential moving average of the weights (e.g. 0.9999) and save it as ema<step>')
+    ap.add_argument('--posthoc-ema', type=float, nargs=2, default=None, metavar=('S1', 'S2'),
+                    help='keep two power-function averages of the weights of these relative widths (e.g. 0.05 0.10) and '
+                         'save snapshots of both, from which posthoc_ema_srn.py rebuilds an EMA of any width after training')
+    ap.add_argument('--snapshot-every', type=int, default=1000,
+                    help='with --posthoc-ema: write a snapshot of both averages every this many updates (posthoc<count>)')
     ap.add_argument('--max-grad-norm', type=float, default=None,
                     help='clip the gradient to this global L2 norm (e.g. 1) and skip updates whose norm is not finite')
     ap.add_argument('--warmup-steps', type=int, default=0,
@@ -62,12 +68,16 @@ def main():
         ap.error('--min-snr-gamma needs --loss mse')
     if a.prediction == 'v' and a.loss != 'mse':
         ap.error('--prediction v needs --loss mse')
+    if a.posthoc_ema is not None and a.ema_decay is not None:
+        ap.error('--posthoc-ema and --ema-decay are exclusive')
+    if a.snapshot_every < 1:
+        ap.error('--snapshot-every must be >= 1')
     local = xdist.init_from_env('nccl')
     rank, world = xdist.rank(), xdist.world_size()
     model = P.XUNet(dtype=a.dtype)
     state = P.create_train_state(0, 1, a.lr, a.batch, a.side, model=model, ema_decay=a.ema_decay,
                                  max_grad_norm=a.max_grad_norm, warmup_steps=a.warmup_steps, loss=a.loss,
-                                 prediction=a.prediction)
+                                 prediction=a.prediction, posthoc_ema=a.posthoc_ema)
     if a.resume and P.checkpoint.restore_train_state(a.ckpt, state) is not None and rank == 0:
         print(f'resumed from step {state.step}')
     if a.device_data:
@@ -107,7 +117,8 @@ def main():
 
 
 def report(a, state, step, it, loss, rank):
-    """The loss every 50 updates and the checkpoints every --save-every."""
+    """The loss every 50 updates, the checkpoints every --save-every and, with --posthoc-ema, a snapshot of both averages
+    every --snapshot-every updates."""
     if rank == 0 and it % 50 == 0:
         norm = '' if step.grad_norm is None else f'  grad norm {float(step.grad_norm):.4f}'
         print(f'{it}: {float(loss):.4f}{norm}')                                                    # train.py:157
@@ -117,6 +128,8 @@ def report(a, state, step, it, loss, rank):
             if state.ema_params is not None:
                 P.checkpoint.save_checkpoint(a.ckpt, state.ema_params, step=it, prefix='ema', add_device_axis=True)
         P.checkpoint.save_train_state(a.ckpt, state, step=state.step)    # collective: every rank calls it
+    if state.posthoc is not None and state.opt_state.count % a.snapshot_every == 0:
+        P.posthoc.save_snapshot(a.ckpt, state)                           # rank 0 writes
 
 
 def finish(state, rank):

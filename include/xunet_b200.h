@@ -289,6 +289,21 @@ int xunet_adam_clip_step(float* params, const float* grads, float* m, float* v, 
                          double ema_decay, const float* norm_dev, double max_norm, long long warmup_steps,
                          long long* skipped_dev, void* stream);
 
+/* xunet_adam_clip_step keeping two power-function averages of the weights instead of an EMA (post-hoc EMA, Karras et al.
+ * 2024, EDM2 §3): with the Adam count t (`step`, or *step_dev) and k in {a, b}
+ *     beta_k = (1 - 1/t)^(gamma_k + 1)            in double, beta_k and 1 - beta_k each rounded to fp32 once
+ *     ema_k <- beta_k * ema_k + (1 - beta_k) * params_new
+ * fused into the same pass, each product and the sum rounded separately in fp32 (no FMA) as in xunet_adam_ema_step.  Weight
+ * of the parameters after update tau in ema_k at count t: (tau^(g+1) - (tau-1)^(g+1)) / t^(g+1), g = gamma_k; beta_1 = 0, so
+ * the first update overwrites both averages.  Warm-up, clipping and the skip of a non-finite norm are xunet_adam_clip_step's;
+ * a skipped update touches neither average.  params / m / v come out bit-identical to xunet_adam_clip_step.  ema_a, ema_b:
+ * device, n floats each, updated in place.  Errors: a NULL average, ema_a == ema_b, a gamma that is not finite or is <= -1,
+ * step < 1 without step_dev, and xunet_adam_clip_step's clip / warm-up argument errors.  Graph-capturable. */
+int xunet_adam_posthoc_step(float* params, const float* grads, float* m, float* v, float* ema_a, float* ema_b, long long n,
+                            long long step, const long long* step_dev, double lr, double b1, double b2, double eps,
+                            double grad_scale, double gamma_a, double gamma_b, const float* norm_dev, double max_norm,
+                            long long warmup_steps, long long* skipped_dev, void* stream);
+
 /* One ancestral update of sampling.py:128-151 with the schedule on the device, for a per-step CUDA graph (forward + this call
  * + counter increment) that is replayed with no host arithmetic in between (the reference does the schedule math in numpy
  * between two un-jitted model calls, sampling.py:133-151).  Given the 2B-batched model output eps2 =

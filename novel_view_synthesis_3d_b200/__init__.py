@@ -3,7 +3,7 @@ shiveshkhaitan/novel_view_synthesis_3d, rebuilt H100-native (hand-written sm_90a
 from .xunet import XUNet, XUNetConfig, SMALL, FULL_3DIM, ParamTree, Engine
 from .train import (TrainState, Adam, AdamState, create_train_state, create_sample_data, apply_model, update_model,
                     TrainStep)
-from . import checkpoint, consistency, distill, lift, metrics, pose, sampling, srn_data
+from . import checkpoint, consistency, distill, lift, metrics, pose, posthoc, sampling, srn_data
 from .consistency import Field, consistency_score, fit_field
 from .distill import ConsistencyTeacher, Teacher, create_distill_state
 from .pose import PoseEstimator, PoseResult, rotation_error_deg
@@ -19,4 +19,4 @@ __all__ = ['XUNet', 'XUNetConfig', 'SMALL', 'FULL_3DIM', 'ParamTree', 'Engine', 
            'image_metrics', 'DeviceScenes', 'distill', 'Teacher', 'create_distill_state', 'distill_grid',
            'consistency', 'Field', 'fit_field', 'consistency_score', 'pose', 'PoseEstimator', 'PoseResult',
            'rotation_error_deg', 'lift', 'FieldLifter', 'LiftResult', 'estimate_up', 'elevation_range',
-           'ConsistencyTeacher', 'consistency_grid']
+           'ConsistencyTeacher', 'consistency_grid', 'posthoc']

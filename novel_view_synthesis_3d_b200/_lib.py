@@ -107,6 +107,8 @@ SYMBOLS = {
     'xunet_grad_global_norm': (C.c_int, [C.c_void_p, C.c_longlong, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     'xunet_adam_clip_step': (C.c_int, [C.c_void_p] * 5 + [C.c_longlong, C.c_longlong, C.c_void_p] + [C.c_double] * 6 +
                              [C.c_void_p, C.c_double, C.c_longlong, C.c_void_p, C.c_void_p]),
+    'xunet_adam_posthoc_step': (C.c_int, [C.c_void_p] * 6 + [C.c_longlong, C.c_longlong, C.c_void_p] + [C.c_double] * 7 +
+                                [C.c_void_p, C.c_double, C.c_longlong, C.c_void_p, C.c_void_p]),
     'xunet_sampler_step_table': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     'xunet_sampler_step_multistep': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_float] +

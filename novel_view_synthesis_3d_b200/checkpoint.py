@@ -9,7 +9,7 @@ arrays larger than 2**30 bytes are stored as a dict of chunks {'__msgpack_chunke
 File name: f'{prefix}{step}' inside ckpt_dir.
 
 save_train_state / restore_train_state extend this to the whole training state (parameters, Adam moments and count, step,
-the weight EMA and the host cond_mask streams), so a run can be resumed where it stopped.
+the weight EMA or the two post-hoc averages, and the host cond_mask streams), so a run can be resumed where it stopped.
 """
 from __future__ import annotations
 
@@ -193,7 +193,8 @@ def _set_rng_state(rng: np.random.RandomState, d: dict):
 def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *, ema: Optional[dict] = None,
                      rng: Optional[list] = None, add_device_axis: bool = False, clip: bool = False,
                      schedule: bool = False, skipped: Optional[int] = None, prediction: Optional[str] = None,
-                     distill: Optional[dict] = None) -> dict:
+                     distill: Optional[dict] = None, posthoc: Optional[tuple] = None,
+                     posthoc_sigma_rel: Optional[tuple] = None) -> dict:
     """The nested dict flax.serialization.to_state_dict gives for a flax.training.train_state.TrainState with
     tx=optax.adam(lr), i.e. chain(scale_by_adam, scale(-lr)):
 
@@ -211,7 +212,8 @@ def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *,
     EMA is kept, 'rng': {'<rank>': rng_state_dict(..)} for the host cond_mask stream of every rank, and 'skipped_steps'
     (int64, updates skipped for a non-finite gradient norm) and 'prediction' (the string 'eps' or 'v': what the network was
     trained to predict) when given, and 'distill' ({'teacher_steps', 'rounds'[, 'w']}, a progressively distilled student's
-    record) when given.  The Flax / optax layouts are restated from memory
+    record) when given, and 'posthoc_ema': {'0': tree, '1': tree} with 'posthoc_sigma_rel' (fp64, both widths) for the two
+    post-hoc averages (posthoc = (a, b), params-shaped trees) when given.  The Flax / optax layouts are restated from memory
     of their published sources and have not been checked against files written by the packages themselves.
     add_device_axis=True gives every Flax leaf (not 'rng' / 'skipped_steps') the leading pmap axis of length 1, as the
     reference's pmapped state carries it (train.py:161-167).  params / mu / nu / ema: nested dicts of numpy arrays
@@ -226,7 +228,11 @@ def train_state_tree(params: dict, mu: dict, nu: dict, count: int, step: int, *,
     tree = {'step': np.asarray(step, dtype=np.int32), 'params': params, 'opt_state': opt}
     if ema is not None:
         tree['ema_params'] = ema
+    if posthoc is not None:
+        tree['posthoc_ema'] = {'0': posthoc[0], '1': posthoc[1]}
     tree = ax(tree)
+    if posthoc is not None:
+        tree['posthoc_sigma_rel'] = np.asarray(posthoc_sigma_rel, dtype=np.float64)
     if rng is not None:
         tree['rng'] = {str(r): d for r, d in enumerate(rng)}
     if skipped is not None:
@@ -242,7 +248,8 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     """Inverse of train_state_tree onto flat fp32 host buffers laid out by `spec`.  Returns {'step', 'count', 'params',
     'mu', 'nu', 'ema' (None if the file has none), 'rng' (list indexed by rank, or None), 'skipped' (0 if the file has
     none), 'prediction' ('eps' if the file has none: files written before v-prediction existed hold eps models), 'distill'
-    (None if the file has none: a model that is not a distilled student)}.  Accepts all four optimizer layouts (with and without clipping, with and without a schedule), so a run may
+    (None if the file has none: a model that is not a distilled student), 'posthoc' ((a, b) flat buffers, None if the file
+    has none) and 'posthoc_sigma_rel' (a tuple, None if the file has none)}.  Accepts all four optimizer layouts (with and without clipping, with and without a schedule), so a run may
     turn either on or off when it resumes; a schedule count that differs from Adam's raises ValueError.  Detects the pmap
     device axis from the shape of 'step' and takes replica 0.  Missing / unexpected leaves raise KeyError, wrong shapes
     ValueError."""
@@ -251,6 +258,7 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
     skipped = tree.pop('skipped_steps', None)
     prediction = str(tree.pop('prediction', 'eps'))
     distill = tree.pop('distill', None)
+    ph_sigma = tree.pop('posthoc_sigma_rel', None)
     if distill is not None:
         distill = {k: (float(v) if k == 'w' else int(v)) for k, v in distill.items()}
     if np.ndim(tree['step']) == 1:
@@ -265,13 +273,17 @@ def parse_train_state_tree(tree: dict, spec, nparams: int) -> dict:
            'prediction': prediction, 'distill': distill}
     for k, sub in (('params', tree['params']), ('mu', adam['mu']), ('nu', adam['nu']), ('ema', tree.get('ema_params'))):
         out[k] = None if sub is None else pack_flat(sub, spec, nparams)
+    ph = tree.get('posthoc_ema')
+    out['posthoc'] = None if ph is None else tuple(pack_flat(ph[k], spec, nparams) for k in ('0', '1'))
+    out['posthoc_sigma_rel'] = None if ph_sigma is None else tuple(float(x) for x in np.asarray(ph_sigma).reshape(-1))
     out['rng'] = None if rng is None else [rng[str(r)] for r in range(len(rng))]
     return out
 
 
 def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', overwrite: bool = True,
                      add_device_axis: bool = False) -> str:
-    """Writes the whole TrainState -- params, Adam mu / nu / count, step, ema_params when the state keeps an EMA, the count
+    """Writes the whole TrainState -- params, Adam mu / nu / count, step, ema_params when the state keeps an EMA, the two
+    post-hoc averages and their sigma_rel when it keeps them, the count
     of skipped updates when it clips or warms up, the state's prediction ('eps' or 'v'), a distilled student's record
     (state.distill) and the host cond_mask stream of
     every rank -- to f'{prefix}{step}' in ckpt_dir (layout: train_state_tree).  The file stays a
@@ -279,7 +291,7 @@ def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', ove
 
     Under torch.distributed this is collective: every rank must call it; the cond_mask streams are gathered and rank 0
     writes.  The tree is built in host memory before it is written (about 7 GB for the full 439 M-parameter model with an
-    EMA).  Returns the file path."""
+    EMA, 8.8 GB with the post-hoc averages).  Returns the file path."""
     from . import dist as xdist
     rngs = xdist.all_gather_object(rng_state_dict(state._mask_rng, state._frozen_mask))
     path = os.path.join(ckpt_dir, f'{prefix}{step}')
@@ -294,7 +306,9 @@ def save_train_state(ckpt_dir: str, state, step: int, prefix: str = 'state', ove
                                 rng=rngs, add_device_axis=add_device_axis, clip=state.tx.max_grad_norm is not None,
                                 schedule=state.tx.warmup_steps > 0,
                                 skipped=state.skipped_steps if state.clip is not None else None,
-                                prediction=state.prediction, distill=state.distill)
+                                prediction=state.prediction, distill=state.distill,
+                                posthoc=None if state.posthoc is None else tuple(host(f) for f in state.posthoc.flats()),
+                                posthoc_sigma_rel=None if state.posthoc is None else state.posthoc.sigma_rel)
         path = save_checkpoint(ckpt_dir, tree, step, prefix=prefix, overwrite=overwrite)
     xdist.barrier()
     return path
@@ -312,7 +326,10 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     skip counter is restored (0 if the file has none).  A file whose prediction ('eps' when it records none) differs from
     the state's raises ValueError before anything is written: a v model resumed as an eps one (or the reverse) would be
     trained on the other target.  Likewise a file whose distillation record (None when it has none) differs from the state's:
-    a student resumed for another teacher grid, round or guidance would be trained on other targets.  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
+    a student resumed for another teacher grid, round or guidance would be trained on other targets.  A state with post-hoc
+    averages takes them from the file, which must hold averages of the same sigma_rel (ValueError otherwise, before anything
+    is written: averages started mid-run would not follow the power profiles reconstruction assumes); a file with averages
+    restored into a state without them ignores them.  Each rank takes its own cond_mask stream; if the world size differs from the saved one the
     freshly seeded streams are kept (with a warning), and a resume is then no longer bit-exact."""
     from . import dist as xdist
     path = ckpt_dir if os.path.isfile(ckpt_dir) else latest_checkpoint(ckpt_dir, prefix)
@@ -327,11 +344,17 @@ def restore_train_state(ckpt_dir: str, state, prefix: str = 'state'):
     if r['distill'] != state.distill:
         raise ValueError(f"{path}: the checkpoint holds a model with distillation record {r['distill']}, the state trains "
                          f"one with {state.distill}")
+    if state.posthoc is not None and r['posthoc_sigma_rel'] != tuple(state.posthoc.sigma_rel):
+        held = 'no post-hoc averages' if r['posthoc'] is None else f"post-hoc averages of sigma_rel {r['posthoc_sigma_rel']}"
+        raise ValueError(f'{path}: the checkpoint holds {held}, the state keeps sigma_rel {state.posthoc.sigma_rel}')
     state.params.flat.copy_(r['params'])
     state.opt_state.mu.copy_(r['mu'])
     state.opt_state.nu.copy_(r['nu'])
     if state.ema_params is not None:
         state.ema_params.flat.copy_(r['ema'] if r['ema'] is not None else r['params'])
+    if state.posthoc is not None:
+        for f, saved in zip(state.posthoc.flats(), r['posthoc']):
+            f.copy_(saved)
     if state.clip is not None:
         state.clip.skipped.fill_(r['skipped'])
     state.step = r['step']

@@ -1552,23 +1552,28 @@ void launch_loss_mse(int dtype, const float* eps, const float* noise, const floa
 
 // optax.adam (train.py:45, 74-76).  (1-b1), (1-b2) and the bias corrections are formed in double (optax forms them
 // from python floats) and only then rounded to fp32.
-// EMA = true also folds the weight EMA into the same pass: ema = d*ema + (1-d)*p_new with p_new still in registers (8 more
+// AVG == 1 also folds the weight EMA into the same pass: ema = d*ema + (1-d)*p_new with p_new still in registers (8 more
 // bytes per parameter instead of 12 for a separate pass).  The _rn intrinsics forbid FMA contraction, so a float32 numpy
 // restatement matches bit for bit.
+// AVG == 2 keeps two power-function averages instead (EDM2's post-hoc EMA): with the Adam count t, thread 0 forms
+// beta_k = (1 - 1/t)^(gamma_k + 1) and 1 - beta_k in double and rounds each to fp32 once; ema_k = beta_k*ema_k +
+// (1-beta_k)*p_new, rounded like the EMA.  beta_1 = 0, so the first update overwrites both averages with p_new.
 // CLIP = true adds a linear learning-rate warm-up and clipping by a global norm read from the device.  Thread 0 of each CTA
 // also forms lr_t = lr * min(step - 1, W) / W in double rounded once (optax.linear_schedule(0, lr, W) evaluated at the
 // schedule's count, which lags Adam's by one), and the clip decision of optax.clip_by_global_norm: g' = g if norm < max_norm,
 // else fl(fl(g / norm) * max_norm).  A non-finite norm skips the step: every CTA returns before touching p / m / v / ema and
 // CTA 0 counts it in *skipped.  norm == nullptr: no clipping and no guard.  With g' == g and lr_t == lr both instantiations
 // give the same bits; CLIP is a template parameter so that plain Adam keeps its 40 registers (6 CTAs per SM, 46 with CLIP).
-template <bool EMA, bool CLIP>
+template <int AVG, bool CLIP>
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, float* __restrict__ ema, long long n, long long step,
                                                    const long long* __restrict__ step_dev, double lr, double b1d, double b2d,
                                                    float eps, float gs, double decay, const float* __restrict__ norm_dev,
-                                                   float max_norm, long long warmup, long long* __restrict__ skipped) {
+                                                   float max_norm, long long warmup, long long* __restrict__ skipped,
+                                                   float* __restrict__ ema_b, double gamma_a, double gamma_b) {
   xu_grid_dep_sync();
-  __shared__ float sc[CLIP ? 4 : 2];
+  constexpr int NSC = CLIP ? 4 : 2;   // sc[NSC..NSC+3]: beta_a, 1-beta_a, beta_b, 1-beta_b of the power averages
+  __shared__ float sc[NSC + (AVG == 2 ? 4 : 0)];
   __shared__ int mode;   // CLIP: 0 plain gradient, 1 clipped, 2 skip the step
   if (threadIdx.x == 0) {
     const long long st = step_dev != nullptr ? *step_dev : step;
@@ -1587,6 +1592,14 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
       }
       mode = md;
     }
+    if constexpr (AVG == 2) {
+      const double keep = 1.0 - 1.0 / (double)st;
+      const double ba = pow(keep, gamma_a + 1.0), bb = pow(keep, gamma_b + 1.0);
+      sc[NSC] = (float)ba;
+      sc[NSC + 1] = (float)(1.0 - ba);
+      sc[NSC + 2] = (float)bb;
+      sc[NSC + 3] = (float)(1.0 - bb);
+    }
   }
   __syncthreads();
   int md = 0;
@@ -1601,12 +1614,19 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
     lrf = sc[2];
     nrm = sc[3];
   }
-  const float d = (float)decay, omd = (float)(1.0 - decay);
-  // 16-byte accesses (7 streams of n floats: 4 read, 3 written; 9 with the EMA: 5 read, 4 written -- the kernel is pure HBM
-  // traffic); scalar path for a ragged tail or unaligned sub-ranges
+  float d = (float)decay, omd = (float)(1.0 - decay), db = 0.f, omdb = 0.f;
+  if constexpr (AVG == 2) {
+    d = sc[NSC];
+    omd = sc[NSC + 1];
+    db = sc[NSC + 2];
+    omdb = sc[NSC + 3];
+  }
+  // 16-byte accesses (7 streams of n floats: 4 read, 3 written; 9 with the EMA: 5 read, 4 written; 11 with the two power
+  // averages: 6 read, 5 written -- the kernel is pure HBM traffic); scalar path for a ragged tail or unaligned sub-ranges
   uintptr_t addr_or = reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                       reinterpret_cast<uintptr_t>(v);
-  if (EMA) addr_or |= reinterpret_cast<uintptr_t>(ema);
+  if (AVG >= 1) addr_or |= reinterpret_cast<uintptr_t>(ema);
+  if (AVG == 2) addr_or |= reinterpret_cast<uintptr_t>(ema_b);
   const bool vec = (addr_or & 15) == 0;
   const long long n4 = vec ? (n >> 2) : 0;
   auto upd = [&](float gi, float& mi, float& vi, float& pi) {
@@ -1616,7 +1636,12 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
     vi = b2 * vi + omb2 * gi * gi;
     pi -= lrf * (mi * c1) / (sqrtf(vi * c2) + eps);
   };
-  auto avg = [&](float& ei, float pi) { ei = __fadd_rn(__fmul_rn(d, ei), __fmul_rn(omd, pi)); };
+  auto avg = [](float& ei, float pi, float dk, float omdk) { ei = __fadd_rn(__fmul_rn(dk, ei), __fmul_rn(omdk, pi)); };
+  auto avg4 = [&](float* buf, long long i, const float4& p4, float dk, float omdk) {
+    float4 e4 = reinterpret_cast<float4*>(buf)[i];
+    avg(e4.x, p4.x, dk, omdk); avg(e4.y, p4.y, dk, omdk); avg(e4.z, p4.z, dk, omdk); avg(e4.w, p4.w, dk, omdk);
+    reinterpret_cast<float4*>(buf)[i] = e4;
+  };
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
     const float4 g4 = __ldg(reinterpret_cast<const float4*>(g) + i);
     float4 m4 = reinterpret_cast<float4*>(m)[i], v4 = reinterpret_cast<float4*>(v)[i], p4 = reinterpret_cast<float4*>(p)[i];
@@ -1624,35 +1649,40 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
     reinterpret_cast<float4*>(m)[i] = m4;
     reinterpret_cast<float4*>(v)[i] = v4;
     reinterpret_cast<float4*>(p)[i] = p4;
-    if (EMA) {
-      float4 e4 = reinterpret_cast<float4*>(ema)[i];
-      avg(e4.x, p4.x); avg(e4.y, p4.y); avg(e4.z, p4.z); avg(e4.w, p4.w);
-      reinterpret_cast<float4*>(ema)[i] = e4;
-    }
+    if (AVG >= 1) avg4(ema, i, p4, d, omd);
+    if (AVG == 2) avg4(ema_b, i, p4, db, omdb);
   }
   for (long long i = n4 * 4 + (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
     float mi = m[i], vi = v[i], pi = p[i];
     upd(g[i], mi, vi, pi);
     m[i] = mi; v[i] = vi; p[i] = pi;
-    if (EMA) {
+    if (AVG >= 1) {
       float ei = ema[i];
-      avg(ei, pi);
+      avg(ei, pi, d, omd);
       ema[i] = ei;
+    }
+    if (AVG == 2) {
+      float ei = ema_b[i];
+      avg(ei, pi, db, omdb);
+      ema_b[i] = ei;
     }
   }
 }
-// ema == nullptr: no EMA.  norm_dev == nullptr and warmup == 0: plain Adam, without the clip / warm-up prologue
+// ema == nullptr: no EMA; ema_b != nullptr: ema and ema_b are the power averages of exponents gamma_a / gamma_b (decay is
+// then unused).  norm_dev == nullptr and warmup == 0: plain Adam, without the clip / warm-up prologue
 static void launch_adam(float* p, const float* g, float* m, float* v, long long n, long long step, const long long* step_dev,
                         double lr, double b1, double b2, double eps, double grad_scale, float* ema, double decay,
-                        const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s) {
+                        const float* norm_dev, double max_norm, long long warmup, long long* skipped, cudaStream_t s,
+                        float* ema_b = nullptr, double gamma_a = 0.0, double gamma_b = 0.0) {
   int blocks = cdiv(n, 256 * 4);   // one float4 per thread and pass
   if (blocks > xu_num_sms() * 8) blocks = xu_num_sms() * 8;
   if (blocks < 1) blocks = 1;
   const bool clip = norm_dev != nullptr || warmup > 0;
-  auto kernel = ema == nullptr ? (clip ? adam_kernel<false, true> : adam_kernel<false, false>)
-                               : (clip ? adam_kernel<true, true> : adam_kernel<true, false>);
+  auto kernel = ema_b != nullptr ? (clip ? adam_kernel<2, true> : adam_kernel<2, false>)
+                : ema == nullptr ? (clip ? adam_kernel<0, true> : adam_kernel<0, false>)
+                                 : (clip ? adam_kernel<1, true> : adam_kernel<1, false>);
   xu_launch(kernel, blocks, 256, 0, s, p, g, m, v, ema, n, step, step_dev, lr, b1, b2, (float)eps, (float)grad_scale,
-            decay, norm_dev, (float)max_norm, warmup, skipped);
+            decay, norm_dev, (float)max_norm, warmup, skipped, ema_b, gamma_a, gamma_b);
 }
 
 extern "C" int xunet_adam_step(float* params, const float* grads, float* m, float* v, long long n, long long step,
@@ -1689,6 +1719,27 @@ extern "C" int xunet_adam_clip_step(float* params, const float* grads, float* m,
   launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema, ema ? ema_decay : 0.0, norm_dev,
               max_norm, warmup_steps, skipped_dev, (cudaStream_t)stream);
   return xu_launched("adam_clip");
+}
+
+extern "C" int xunet_adam_posthoc_step(float* params, const float* grads, float* m, float* v, float* ema_a, float* ema_b,
+                                       long long n, long long step, const long long* step_dev, double lr, double b1,
+                                       double b2, double eps, double grad_scale, double gamma_a, double gamma_b,
+                                       const float* norm_dev, double max_norm, long long warmup_steps,
+                                       long long* skipped_dev, void* stream) {
+  if (!params || !grads || !m || !v || n < 0) return xu_fail("xunet_adam_posthoc_step: bad argument");
+  if (!ema_a || !ema_b) return xu_fail("xunet_adam_posthoc_step: ema_a and ema_b must both be given");
+  if (ema_a == ema_b) return xu_fail("xunet_adam_posthoc_step: ema_a and ema_b are the same buffer");
+  if (!(isfinite(gamma_a) && gamma_a > -1.0) || !(isfinite(gamma_b) && gamma_b > -1.0))
+    return xu_fail("xunet_adam_posthoc_step: gamma_a %g / gamma_b %g must be finite and > -1", gamma_a, gamma_b);
+  if (!step_dev && step < 1) return xu_fail("xunet_adam_posthoc_step: step %lld < 1", step);
+  if (warmup_steps < 0) return xu_fail("xunet_adam_posthoc_step: warmup_steps %lld < 0", warmup_steps);
+  if (norm_dev) {
+    if (!(max_norm > 0.0)) return xu_fail("xunet_adam_posthoc_step: max_norm %g must be > 0", max_norm);
+    if (!skipped_dev) return xu_fail("xunet_adam_posthoc_step: skipped_dev is NULL (needed with norm_dev)");
+  }
+  launch_adam(params, grads, m, v, n, step, step_dev, lr, b1, b2, eps, grad_scale, ema_a, 0.0, norm_dev, max_norm,
+              warmup_steps, skipped_dev, (cudaStream_t)stream, ema_b, gamma_a, gamma_b);
+  return xu_launched("adam_posthoc");
 }
 
 // ---- global gradient norm (optax.clip_by_global_norm) ----------------------------------------------------------------------

@@ -191,17 +191,20 @@ class ConsistencyTeacher(_FrozenTeacher):
 
 
 def create_distill_state(teacher: _FrozenTeacher, learning_rate: float = 1e-4, *, rng_dropout=None, ema_decay: Optional[float] = None,
-                         max_grad_norm: Optional[float] = None, warmup_steps: int = 0):
+                         max_grad_norm: Optional[float] = None, warmup_steps: int = 0, posthoc_ema: Optional[tuple] = None):
     """The TrainState of a student of `teacher` (a Teacher or a ConsistencyTeacher): the teacher's model, batch size and image side, prediction='v' with
-    loss='mse', and parameters (and EMA, when kept) starting from the teacher's.  The state records teacher.record, which
+    loss='mse', and parameters (and EMA or post-hoc averages, when kept) starting from the teacher's.  The state records teacher.record, which
     save_train_state writes and restore_train_state checks.  The optimizer arguments are create_train_state's."""
     from .train import create_train_state
     st = create_train_state(0, rng_dropout, learning_rate, teacher.B, teacher.S, model=teacher.model, init_on_device=True,
                             ema_decay=ema_decay, max_grad_norm=max_grad_norm, warmup_steps=warmup_steps, loss='mse',
-                            prediction='v')
+                            prediction='v', posthoc_ema=posthoc_ema)
     st.params.flat.copy_(teacher.flat)
     if st.ema_params is not None:
         st.ema_params.flat.copy_(teacher.flat)
+    if st.posthoc is not None:
+        for f in st.posthoc.flats():
+            f.copy_(teacher.flat)
     st.distill = teacher.record
     return st
 

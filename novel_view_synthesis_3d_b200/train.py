@@ -21,6 +21,7 @@ from . import _lib
 from . import dist as xdist
 from .diffusion import diffusion_tables, min_snr_weights
 from .distill import check_teacher, run_teacher
+from .posthoc import PosthocEMA, check_posthoc_ema
 from .sampling import check_prediction
 from .xunet import XUNet, ParamTree, Engine, InputSlots, check_loss
 
@@ -82,6 +83,9 @@ class TrainState:
     # None when create_train_state(ema_decay=None)
     ema_params: Optional[ParamTree] = None
     ema_decay: Optional[float] = None
+    # two power-function averages of the weights (post-hoc EMA, posthoc.py), updated inside the Adam pass; None unless
+    # create_train_state(posthoc_ema=..)
+    posthoc: Optional[PosthocEMA] = None
     # gradient-norm / skip-counter block; None unless create_train_state(max_grad_norm=..) or (warmup_steps=..)
     clip: Optional[ClipState] = None
     # training objective: 'frobenius' (the reference's ||eps_hat - noise||_F, train.py:67) or 'mse' (the mean squared error
@@ -103,7 +107,8 @@ class TrainState:
         Ownership: by default the flat parameter / moment / EMA buffers are updated IN PLACE and the returned state shares
         them, i.e. the OLD state's `params` alias the new values (the reference rebinds `state = update_model(state, ..)`
         and never looks at the old one, train.py:153).  copy=True gives the Flax contract literally: the old state keeps
-        its values and the new state owns fresh buffers (3 x 4 bytes per parameter of extra traffic, 4 x 4 with EMA).
+        its values and the new state owns fresh buffers (3 x 4 bytes per parameter of extra traffic, 4 x 4 with EMA, 5 x 4
+        with the two post-hoc averages).
 
         With clipping (tx.max_grad_norm) the global gradient norm is reduced first, into `clip.norm`; an update whose norm
         is not finite changes nothing but the counters and is counted in `skipped_steps`."""
@@ -113,9 +118,12 @@ class TrainState:
         if copy:
             newp = self.model.tree_from_flat(self.params.flat.clone(), S, B)
             newe = None if self.ema_params is None else self.model.tree_from_flat(self.ema_params.flat.clone(), S, B)
+            ph = self.posthoc
+            newh = None if ph is None else replace(ph, a=self.model.tree_from_flat(ph.a.flat.clone(), S, B),
+                                                   b=self.model.tree_from_flat(ph.b.flat.clone(), S, B))
             newc = None if self.clip is None else replace(self.clip, norm=self.clip.norm.clone(),
                                                           skipped=self.clip.skipped.clone())
-            self = replace(self, params=newp, ema_params=newe, clip=newc,
+            self = replace(self, params=newp, ema_params=newe, posthoc=newh, clip=newc,
                            opt_state=replace(self.opt_state, mu=self.opt_state.mu.clone(), nu=self.opt_state.nu.clone()))
         p = self.params.flat
         count = self.opt_state.count + 1
@@ -130,9 +138,9 @@ class TrainState:
 
 
 def _adam_launch(lib, s: TrainState, flat_g: torch.Tensor, count: int, step_dev, grad_scale: float, stream: int) -> None:
-    """One fused Adam pass over the flat buffers of `s`, with the EMA update, warm-up and clipping the state carries (the
-    library runs plain Adam without the clip / warm-up prologue when there is neither).  With clipping the global-norm
-    reduction runs first."""
+    """One fused Adam pass over the flat buffers of `s`, with the EMA (or the two post-hoc averages), warm-up and clipping
+    the state carries (the library runs plain Adam without the clip / warm-up prologue when there is neither).  With
+    clipping the global-norm reduction runs first."""
     p, tx, c = s.params.flat, s.tx, s.clip
     ptr = lambda t: None if t is None else t.data_ptr()
     norm = None
@@ -140,8 +148,16 @@ def _adam_launch(lib, s: TrainState, flat_g: torch.Tensor, count: int, step_dev,
         _lib.check(lib.xunet_grad_global_norm(flat_g.data_ptr(), p.numel(), grad_scale, c.scratch.data_ptr(),
                                               c.norm.data_ptr(), stream), 'xunet_grad_global_norm')
         norm = c.norm
-    ema = None if s.ema_params is None else s.ema_params.flat
     skipped = None if c is None else c.skipped
+    if s.posthoc is not None:
+        ph = s.posthoc
+        _lib.check(lib.xunet_adam_posthoc_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(),
+                                               s.opt_state.nu.data_ptr(), ph.a.flat.data_ptr(), ph.b.flat.data_ptr(),
+                                               p.numel(), count, ptr(step_dev), tx.learning_rate, tx.b1, tx.b2, tx.eps,
+                                               grad_scale, ph.gamma[0], ph.gamma[1], ptr(norm), tx.max_grad_norm or 0.0,
+                                               tx.warmup_steps, ptr(skipped), stream), 'xunet_adam_posthoc_step')
+        return
+    ema = None if s.ema_params is None else s.ema_params.flat
     _lib.check(lib.xunet_adam_clip_step(p.data_ptr(), flat_g.data_ptr(), s.opt_state.mu.data_ptr(), s.opt_state.nu.data_ptr(),
                                         ptr(ema), p.numel(), count, ptr(step_dev), tx.learning_rate, tx.b1, tx.b2, tx.eps,
                                         grad_scale, s.ema_decay or 0.0, ptr(norm), tx.max_grad_norm or 0.0, tx.warmup_steps,
@@ -153,6 +169,8 @@ def _opt_buffers(s: TrainState):
     bufs = [s.params.flat, s.opt_state.mu, s.opt_state.nu]
     if s.ema_params is not None:
         bufs.append(s.ema_params.flat)
+    if s.posthoc is not None:
+        bufs += s.posthoc.flats()
     if s.clip is not None:
         bufs.append(s.clip.skipped)
     return bufs
@@ -169,7 +187,8 @@ def create_sample_data(batch_size, img_sidelength):
 def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_sidelength, *, model: XUNet = None,
                        zero_init: bool = True, reference_quirks: bool = False, init_on_device: bool = False,
                        ema_decay: Optional[float] = None, max_grad_norm: Optional[float] = None,
-                       warmup_steps: int = 0, loss: str = 'frobenius', prediction: str = 'eps') -> TrainState:
+                       warmup_steps: int = 0, loss: str = 'frobenius', prediction: str = 'eps',
+                       posthoc_ema: Optional[tuple] = None) -> TrainState:
     """train.py:36-47.  Under torch.distributed the parameters of rank 0 are broadcast (the reference gives every
     device a different init, train.py:122-123 -- an ensemble, not data parallelism).
 
@@ -177,6 +196,12 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
     the same kernel as Adam, starting as a copy of the initial parameters.  Every rank updates its own copy; the parameters
     are identical across ranks after the all-reduce and Adam, so the copies stay identical without a collective.  None
     (default): no EMA buffer, the optimizer step is plain Adam.
+
+    posthoc_ema (e.g. (0.05, 0.10), Karras et al. 2024): keep `posthoc`, two power-function averages of the weights of
+    these relative widths sigma_rel (two different values in (0, 0.2887)), updated in the same kernel as Adam, from which
+    posthoc.reconstruct rebuilds an EMA of any width after training out of the snapshots posthoc.save_snapshot writes.
+    Both start as copies of the initial parameters, which the first update overwrites.  Every rank updates its own copies,
+    identical across ranks like the EMA's.  Exclusive with ema_decay (ValueError).
 
     max_grad_norm (e.g. 1.0, Ho et al. 2020): clip the averaged gradient to this global L2 norm before Adam
     (optax.clip_by_global_norm).  The norm is reduced on the device in a fixed order, so runs stay bit-reproducible; an update
@@ -203,6 +228,11 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
         raise ValueError(f"prediction='v' needs loss='mse', got loss={loss!r}")
     if ema_decay is not None and not (0.0 <= ema_decay <= 1.0):
         raise ValueError(f'ema_decay must lie in [0, 1], got {ema_decay}')
+    if posthoc_ema is not None:
+        if ema_decay is not None:
+            raise ValueError('ema_decay and posthoc_ema are exclusive: keep either a fixed-decay EMA or the two post-hoc '
+                             'averages')
+        posthoc_ema = check_posthoc_ema(posthoc_ema)
     if max_grad_norm is not None and not (float(max_grad_norm) > 0.0 and np.isfinite(float(max_grad_norm))):
         raise ValueError(f'max_grad_norm must be a finite number > 0, got {max_grad_norm}')
     if isinstance(warmup_steps, bool) or int(warmup_steps) != warmup_steps or warmup_steps < 0:
@@ -227,6 +257,8 @@ def create_train_state(rng, rng_dropout, learning_rate, train_batch_size, img_si
                       batch_size=train_batch_size, img_sidelength=img_sidelength, grad_scale=1.0 / world,
                       reference_quirks=reference_quirks, ema_params=ema,
                       ema_decay=None if ema_decay is None else float(ema_decay),
+                      posthoc=None if posthoc_ema is None else
+                      PosthocEMA.create(model, params, posthoc_ema, img_sidelength, train_batch_size),
                       clip=ClipState.zeros(params.flat.device) if opt.clip_or_warmup else None, loss=loss,
                       prediction=prediction,
                       _mask_rng=np.random.RandomState(mask_seed & 0x7FFFFFFF))
@@ -342,7 +374,7 @@ class TrainStep:
     grad_accum_steps=k (optax.MultiSteps(.., every_k_schedule=k)): each call takes k*B samples per rank (B =
     state.batch_size) and runs k forward/backward passes of B samples, micro-batch j being rows [j*B, (j+1)*B); the first
     backward overwrites the flat gradient buffer, the others add into it (xunet_backward_accumulate), and one update (norm,
-    Adam, EMA) follows with grad_scale = 1/(world*k): Adam of the mean micro-batch gradient.  The loss of each micro-batch is
+    Adam, EMA or post-hoc averages) follows with grad_scale = 1/(world*k): Adam of the mean micro-batch gradient.  The loss of each micro-batch is
     its own Frobenius norm, so this is not the gradient of one batch of k*B samples (as data parallelism is not).  Under
     data parallelism only the last backward carries the bucket hook, so the all-reduce covers the whole sum.  The returned
     loss is the mean of the k micro-batch losses; `step` and the Adam count advance by one per call.  k = 1 (the default)
