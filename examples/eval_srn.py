@@ -11,6 +11,7 @@ instance is conditioned on one source view (view 64 by default) and every scored
         --steps 25 --out eval_v/
     python examples/eval_srn.py cars_test --ckpt checkpoints_d6 --prefix ema --side 128 --steps 256 --distilled 6 --out eval_d6/
     python examples/eval_srn.py cars_test --ckpt checkpoints_cd --prefix ema --side 128 --consistency 4 --out eval_cd4/
+    python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --steps 256 --cache-interval 3 --out eval_dc3/
 
 Modes:
   independent  each target is sampled from the source alone (Sampler.sample, the reference's k = 1 sampler); the targets
@@ -78,6 +79,12 @@ def main():
                          'multistep consistency sampling on consistency_grid(N, K) without guidance, reading v, with N read '
                          'from the state<step> checkpoint in --ckpt (a directory); --steps, --method, --eta, --spacing, --w '
                          'and --prediction are then ignored')
+    ap.add_argument('--cache-interval', type=int, default=1, metavar='N',
+                    help='feature cache (DeepCache): a full forward every N steps, and between them cheap forwards that '
+                         'recompute only the levels below --cache-level and read the deeper feature of the last full one '
+                         '(1: every forward full, the default)')
+    ap.add_argument('--cache-level', type=int, default=1, metavar='L',
+                    help='feature-cache level in [1, levels - 1]: the cheap forwards recompute the levels below L')
     ap.add_argument('--source-view', type=int, default=64, help='conditioning view of every instance (pixelNeRF / 3DiM: 64)')
     ap.add_argument('--targets', type=int, default=0, help='target views per instance, spaced evenly; 0 = all other views')
     ap.add_argument('--max-instances', type=int, default=-1, help='score the first N instances of the sorted list')
@@ -100,16 +107,18 @@ def main():
             raise SystemExit(f"instance {ds.instances[i]['name']} has {n} views; --source-view {a.source_view} does not exist")
         insts.append((i, select_targets(n, a.source_view, a.targets)))
     B = a.views_in_flight
+    cache = dict(cache_interval=a.cache_interval, cache_level=a.cache_level)
     if a.consistency:
         sampler = P.Sampler(P.XUNet(), params, B, a.side, w=None, method='consistency', prediction='v',
                             timesteps=P.consistency_grid(cd_steps(a.ckpt), a.consistency),
-                            dynamic_threshold=a.dynamic_threshold)
+                            dynamic_threshold=a.dynamic_threshold, **cache)
     elif a.distilled:
         sampler = P.Sampler(P.XUNet(), params, B, a.side, w=None, method='ddim', prediction='v',
-                            timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold)
+                            timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold, **cache)
     else:
         sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta,
-                            spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction)
+                            spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction,
+                            **cache)
     os.makedirs(a.out, exist_ok=True)
     if a.save_views:
         os.makedirs(os.path.join(a.out, 'views'), exist_ok=True)

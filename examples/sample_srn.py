@@ -7,6 +7,7 @@ ancestral sampler, write PNGs (the reference blocks in cv2.imshow, which cannot 
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_v --prediction v --method dpmpp_2m --steps 25 --out results_v/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_d1 --prefix ema --distilled 1 --steps 256 --out results_d1/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_cd --prefix ema --consistency 2 --out results_cd2/
+    python examples/sample_srn.py cars_train_val --ckpt checkpoints --method dpmpp_2m --steps 25 --cache-interval 3 --out results_dc3/
 """
 import argparse
 import os
@@ -47,6 +48,12 @@ def main():
                          'multistep consistency sampling on consistency_grid(N, K) without guidance, reading v, with N read '
                          'from the state<step> checkpoint in --ckpt (a directory); --steps, --method, --eta, --spacing, --w '
                          'and --prediction are then ignored')
+    ap.add_argument('--cache-interval', type=int, default=1, metavar='N',
+                    help='feature cache (DeepCache): a full forward every N steps, and between them cheap forwards that '
+                         'recompute only the levels below --cache-level and read the deeper feature of the last full one '
+                         '(1: every forward full, the default)')
+    ap.add_argument('--cache-level', type=int, default=1, metavar='L',
+                    help='feature-cache level in [1, levels - 1]: the cheap forwards recompute the levels below L')
     ap.add_argument('--views', type=int, default=1)
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--out', default='results')
@@ -60,16 +67,18 @@ def main():
     ds = SRNScenes(a.folder, img_sidelength=a.side, max_observations_per_instance=50)
     batch = next(ds.batches(a.views))
     model = P.XUNet()
+    cache = dict(cache_interval=a.cache_interval, cache_level=a.cache_level)
     if a.consistency:
         sampler = P.Sampler(model, params, a.views, a.side, w=None, method='consistency', prediction='v',
                             timesteps=P.consistency_grid(cd_steps(a.ckpt), a.consistency),
-                            dynamic_threshold=a.dynamic_threshold)
+                            dynamic_threshold=a.dynamic_threshold, **cache)
     elif a.distilled:
         sampler = P.Sampler(model, params, a.views, a.side, w=None, method='ddim', prediction='v',
-                            timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold)
+                            timesteps=P.distill_grid(a.steps, a.distilled), dynamic_threshold=a.dynamic_threshold, **cache)
     else:
         sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta,
-                            spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction)
+                            spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction,
+                            **cache)
     os.makedirs(a.out, exist_ok=True)
     if a.orbit > 0:
         it = ds.batches(a.views)

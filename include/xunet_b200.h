@@ -158,6 +158,18 @@ int xunet_forward(xunet_handle* h, const float* params, const xunet_batch* batch
  * 2000 times per view, sampling.py:131-132).  on=0 restores the full forward. */
 int xunet_set_static_conditioning(xunet_handle* h, int on);
 
+/* Sampler feature cache (DeepCache, Ma et al. 2024): level = 0 (the default) restores the full forward; level = L in
+ * [1, n_levels - 1] makes the following xunet_forward calls cheap forwards.  A cheap forward reads the output of the up
+ * ResnetBlock that leaves level L (the input of up-level L - 1) as the last full forward left it in the workspace, and runs
+ * only the ops the output needs given that tensor: the conditioning, the input conv, the down and up blocks of the levels
+ * below L and the head.  The deep blocks, the down ResnetBlock into level L, their FiLM Denses and the pose-embedding convs of
+ * levels >= L are skipped, so the deep feature keeps the log-SNR and inputs of the step that computed it.  Static
+ * conditioning applies to the kept ops as usual, and xunet_count_kernels counts the forward at the current level.
+ * Fails on a training handle (a backward needs every activation) and for a level outside [0, n_levels - 1].  A cheap
+ * forward at L fails unless a full forward has completed on the handle, and no cheap forward at a deeper level (which
+ * recomputes the level-L tensor) has run since. */
+int xunet_set_feature_cache(xunet_handle* h, int level);
+
 /* The value_and_grad half of apply_model (train.py:62-71): must follow xunet_forward on the same
  * workspace.  loss = ||eps_hat - noise||_F (train.py:67).  grads: device flat fp32 (param layout),
  * overwritten.  loss_out: device, 1 float. */

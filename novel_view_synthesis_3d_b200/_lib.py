@@ -86,6 +86,7 @@ SYMBOLS = {
     'xunet_forward': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_int, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p]),
     'xunet_set_static_conditioning': (C.c_int, [C.c_void_p, C.c_int]),
+    'xunet_set_feature_cache': (C.c_int, [C.c_void_p, C.c_int]),
     'xunet_backward': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_void_p]),
     'xunet_backward_accumulate': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(XunetBatch), C.c_void_p, C.c_void_p,

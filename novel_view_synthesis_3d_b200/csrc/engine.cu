@@ -14,6 +14,7 @@
 #include "conv_tc.h"
 #include "pose_grad.h"
 
+#include <algorithm>
 #include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -35,7 +36,7 @@ int xu_launched(const char* what) {
   return e == cudaSuccess ? 0 : xu_fail("%s: CUDA error: %s", what, cudaGetErrorString(e));
 }
 extern "C" const char* xunet_last_error(void) { return g_err; }
-extern "C" int xunet_version(void) { return 111; }
+extern "C" int xunet_version(void) { return 112; }
 
 namespace {
 
@@ -122,6 +123,15 @@ struct xunet_handle {
   int t_in = -1, t_pose = -1, t_out = -1;
   int forward_done_train = 0;
   int static_cond = 0;       // sampler: pose-only ops and weight shadows are reused from the previous forward
+  // feature cache (xunet_set_feature_cache): at cache_level L > 0 a forward runs only the ops keep[] marks, reading the
+  // tensor cache_t[L] the last full forward left in the workspace
+  int cache_level = 0;
+  int cache_from = 0;            // the smallest level whose cached tensor is still the last full forward's (0: none)
+  std::vector<int> cache_t;      // per level L >= 1: the output of the up ResnetBlock that leaves level L; [0] = -1
+  int keep_level = 0;            // the level keep[], keep_fork and keep_clear were derived for
+  std::vector<char> keep;        // per op
+  int keep_fork = -1;            // the last kept OP_EMB: the FiLM side branch forks after it
+  std::vector<std::pair<long long, long long>> keep_clear;   // (offset, bytes): the statistics a cheap forward re-produces
   std::vector<WeightPrepTable> prep;
   // weight-gradient kernels run on a side stream concurrently with the activation-gradient chain (fork/join by events;
   // captured into the same CUDA graph as parallel branches).  Created lazily at the first backward.
@@ -520,6 +530,7 @@ struct Builder {
     int h = conv(H.t_in, c.ch, 3, 1, w_in, b_in, -1, 1.f, 1, "Conv_0");
     std::vector<int> hs;
     hs.push_back(h);
+    H.cache_t.assign(L, -1);
     // ---- down  :231-246
     for (int i = 0; i < L; ++i) {
       for (int k = 0; k < c.num_res_blocks; ++k) {
@@ -542,7 +553,7 @@ struct Builder {
         // use_attn is decided on the skip's resolution (== h's resolution)
         h = xblock(cat, semb[i], c.ch * c.ch_mult[i]);
       }
-      if (i != 0) h = rblock(h, semb[i - 1], RS_UP);
+      if (i != 0) H.cache_t[i] = h = rblock(h, semb[i - 1], RS_UP);
     }
     if (!hs.empty()) return xu_fail("internal: skip stack not empty");
     // ---- head  :275-280
@@ -797,16 +808,56 @@ static GnArgs gn_args(const Ctx& c, const Op& o) {
                  o.mode, o.rs, c.h->cfg.dropout, o.op_index, c.seed_dev, c.train);
 }
 
+// The ops a cheap forward at feature-cache level `level` runs: a walk from the output back through every op's inputs, with
+// the cached tensor as a leaf.  The log-SNR embedding is kept too (the OP_EMBs read it outside the tensor list).  Also derives
+// the statistics ranges the kept ops re-produce: the per-op GroupNorm statistics of the kept norms and the per-channel sums
+// of the tensors a kept op writes.  The cached tensor's sums are not among them, so they survive for the norm that reads it.
+static void plan_feature_cache(xunet_handle* h, int level) {
+  const int nops = (int)h->ops.size(), cached = h->cache_t[level];
+  std::vector<char> need(h->tensors.size(), 0);
+  h->keep.assign(nops, 0);
+  h->keep_fork = -1;
+  for (int i = nops - 1; i >= 0; --i) {
+    const Op& o = h->ops[i];
+    if (!(o.kind == OP_EXTRACT || o.kind == OP_LOGSNR || (o.y >= 0 && need[o.y]))) continue;
+    h->keep[i] = 1;
+    for (int t : {o.x, o.r, o.e, o.cs_a, o.cs_b}) if (t >= 0 && t != cached) need[t] = 1;
+    if (o.kind == OP_EMB && h->keep_fork < 0) h->keep_fork = i;
+  }
+  std::vector<std::pair<long long, long long>> r;
+  const long long per = sizeof(float) * h->B * XU_GROUPS * 2;
+  for (int i = 0; i < nops; ++i)
+    if (h->keep[i] && h->ops[i].kind == OP_GN) r.push_back({h->ops[i].stats, per});
+  for (const Tensor& t : h->tensors)
+    if (t.cstats >= 0 && h->keep[t.producer])
+      r.push_back({t.cstats, (sizeof(float) * 2 * (long long)h->B * t.c + 255) / 256 * 256});
+  std::sort(r.begin(), r.end());
+  h->keep_clear.clear();
+  for (const auto& x : r) {
+    auto& last = h->keep_clear;
+    if (!last.empty() && last.back().first + last.back().second == x.first) last.back().second += x.second;
+    else last.push_back(x);
+  }
+  h->keep_level = level;
+}
+
 static int forward_impl(Ctx& c, float* eps_out) {
   xunet_handle* h = c.h;
   const int dt = h->dtype, B = h->B, S = h->S, E = h->cfg.emb_ch;
   const bool reuse = h->static_cond && h->forward_done_train != 0;
   if (!reuse) for (const WeightPrepTable& t : h->prep) launch_weight_prep(t, c.params, c.ws, c.s);
-  if (h->stats_bytes) cudaMemsetAsync(c.ws + h->a_stats, 0, (size_t)h->stats_bytes, c.s);
-  if (h->cstats_bytes) cudaMemsetAsync(c.ws + h->a_cstats, 0, (size_t)h->cstats_bytes, c.s);
+  const bool cheap = h->cache_level > 0;
+  if (cheap) {
+    for (const auto& r : h->keep_clear) cudaMemsetAsync(c.ws + r.first, 0, (size_t)r.second, c.s);
+  } else {
+    if (h->stats_bytes) cudaMemsetAsync(c.ws + h->a_stats, 0, (size_t)h->stats_bytes, c.s);
+    if (h->cstats_bytes) cudaMemsetAsync(c.ws + h->a_cstats, 0, (size_t)h->cstats_bytes, c.s);
+  }
+  const int fork_op = cheap ? h->keep_fork : h->last_emb_op;
   cudaStream_t side = h->film_ops.empty() ? nullptr : ensure_side(h);
   for (int oi = 0; oi < (int)h->ops.size(); ++oi) {
     const Op& o = h->ops[oi];
+    if (cheap && !h->keep[oi]) continue;
     switch (o.kind) {
       case OP_LOGSNR:
         launch_logsnr_emb(c.batch->logsnr, c.P(o.p0), c.P(o.p1), c.P(o.p2), c.P(o.p3), c.aux(h->a_pe), c.aux(h->a_h1),
@@ -826,13 +877,14 @@ static int forward_impl(Ctx& c, float* eps_out) {
       case OP_EMB: {
         const Tensor& x = h->tensors[o.x];
         launch_emb_fwd(dt, c.aux(h->a_lemb), c.act(o.x), c.act(o.y), x.n, x.h * x.w, x.c, c.s);
-        if (oi == h->last_emb_op && side != nullptr) {
+        if (oi == fork_op && side != nullptr) {
           // every FiLM Dense depends only on the embeddings: run the whole branch concurrently with the trunk
           cudaEventRecord(h->ev_fork, c.s);
           cudaStreamWaitEvent(side, h->ev_fork, 0);
           Ctx cs = c;
           cs.s = side;
           for (size_t k = 0; k < h->film_ops.size(); ++k) {
+            if (cheap && !h->keep[h->film_ops[k]]) continue;   // its norm is skipped too, so nothing waits on its event
             run_conv_fwd(cs, h->ops[h->film_ops[k]]);
             cudaEventRecord(h->ev_film[k], side);
           }
@@ -1261,12 +1313,31 @@ extern "C" int xunet_forward(xunet_handle* h, const float* params, const xunet_b
                              const unsigned long long* seed_dev, void* workspace, float* eps_out, void* stream) {
   if (!h || !params || !batch || !workspace) return xu_fail("xunet_forward: null argument");
   if (train && h->cfg.dropout > 0.f && !seed_dev) return xu_fail("xunet_forward: train=1 with dropout needs seed_dev");
+  if (h->cache_level > 0 && (h->cache_from == 0 || h->cache_level < h->cache_from))
+    return xu_fail("xunet_forward: a cheap forward at feature-cache level %d needs a full forward first (none has completed since "
+                   "the handle was created, or a cheap forward at a deeper level has recomputed the cached tensor since)",
+                   h->cache_level);
   xu_set_kernel_error("");
   Ctx c{h, params, nullptr, (char*)workspace, batch, seed_dev, train ? 1 : 0, (cudaStream_t)stream};
   XuDetBind bind(h->det);
   int rc = forward_impl(c, eps_out);
   h->forward_done_train = (rc == 0) ? (train ? 1 : 2) : 0;
+  // a cheap forward at L recomputes the cached tensors of every level below L
+  h->cache_from = rc != 0 ? 0 : h->cache_level == 0 ? 1 : std::max(h->cache_from, h->cache_level);
   return rc;
+}
+
+extern "C" int xunet_set_feature_cache(xunet_handle* h, int level) {
+  if (!h) return xu_fail("xunet_set_feature_cache: null handle");
+  if (h->training)
+    return xu_fail("xunet_set_feature_cache: the handle was created with training=1, and a backward needs every activation of a "
+                   "full forward");
+  if (level < 0 || level > h->cfg.n_levels - 1)
+    return xu_fail("xunet_set_feature_cache: level %d outside [0, %d] for a %d-level config", level, h->cfg.n_levels - 1,
+                   h->cfg.n_levels);
+  if (level > 0 && level != h->keep_level) plan_feature_cache(h, level);
+  h->cache_level = level;
+  return 0;
 }
 
 extern "C" int xunet_set_static_conditioning(xunet_handle* h, int on) {

@@ -167,6 +167,22 @@ def _check_dynamic_threshold(p) -> None:
         raise ValueError(f'dynamic_threshold {p} outside (0, 1]')
 
 
+def _check_feature_cache(cache_interval, cache_level, n_levels: int) -> None:
+    """cache_interval N is an integer >= 1; cache_level L an integer >= 1, and at most n_levels - 1 when N > 1 (with N = 1
+    every forward is full and L is not used)."""
+    for name, v in (('cache_interval', cache_interval), ('cache_level', cache_level)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+            raise ValueError(f'{name} must be an integer >= 1, got {v!r}')
+    if cache_interval > 1 and cache_level > n_levels - 1:
+        raise ValueError(f'cache_level {cache_level} outside [1, {n_levels - 1}] for a {n_levels}-level model')
+
+
+def feature_cache_full_steps(steps: int, cache_interval: int) -> np.ndarray:
+    """The uniform feature-cache schedule: (steps,) bool, True where loop position k runs a full forward (k % N == 0, so step
+    0 always does) and False where it runs a cheap one."""
+    return np.arange(steps) % cache_interval == 0
+
+
 def sampler_table(sched: Schedule, method: str = 'ddpm', *, eta: float = 0.0, logsnr_lag: bool | None = None,
                   prediction: str = 'eps'):
     """The device table of `sched` for `method`: (rows, logsnr_first), rows (len(sched), 8) float64 (the sampler rounds
@@ -269,14 +285,23 @@ class Sampler:
     dynamic_threshold: None clips x0 to [-1, 1] (the reference).  A percentile p in (0, 1] thresholds x0 per view instead
     (Saharia et al. 2022, Imagen section 2.3): s = max(1, p-quantile of |x0| over the view), x0 <- clip(x0, -s, s) / s, for
     every method, in `xunet_sampler_step_dynamic` (the paper uses p = 0.995).  It keeps guided x0 far outside [-1, 1] (large
-    w at high noise) from saturating to +-1; a view whose s is 1 gets the fixed clip's bits."""
+    w at high noise) from saturating to +-1; a view whose s is 1 gets the fixed clip's bits.
+
+    cache_interval N, cache_level L: the feature cache (DeepCache, Ma et al. 2024; `xunet_set_feature_cache`).  Loop
+    position k runs a full forward when k % N == 0 and a cheap one otherwise: the cheap forward recomputes only the
+    conditioning, the input conv, the blocks of the levels below L and the head, and reads the deep feature (the output of
+    the up-resampler leaving level L) from the last full forward, with that step's log-SNR and inputs.  It works with every
+    method, guidance and sample_views; its effect on sample quality (PSNR / SSIM on SRN) at N > 1 has not been measured.
+    N = 1 (the default) runs every forward in full and gives the bits of a sampler built without these arguments."""
 
     def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000,
                  w: float | None = 3.0, use_graph: bool = True, method: str = 'ddpm', eta: float = 0.0,
                  spacing: str | None = None, logsnr_lag: bool | None = None, dynamic_threshold: float | None = None,
-                 prediction: str = 'eps', timesteps=None):
+                 prediction: str = 'eps', timesteps=None, cache_interval: int = 1, cache_level: int = 1):
         _check_method(method, eta)
         _check_dynamic_threshold(dynamic_threshold)
+        _check_feature_cache(cache_interval, cache_level, len(model.config.ch_mult))
+        self.cache_interval, self.cache_level = int(cache_interval), int(cache_level)
         self.prediction = check_prediction(prediction)
         self.dynamic_threshold = None if dynamic_threshold is None else float(dynamic_threshold)
         self.method, self.eta = method, float(eta)
@@ -294,7 +319,7 @@ class Sampler:
         self.use_graph = use_graph
         self._tab = None            # (steps, 8) coefficient table on the device
         self._noise = None          # (steps, B*S*S*3) explicit noise on the device
-        self._graphs = {}           # (static conditioning, explicit noise) -> the captured step
+        self._graphs = {}           # (static conditioning, explicit noise, cheap forward) -> the captured step
         self._pos = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self._seed_base = torch.zeros(1, dtype=torch.int64, device=self.dev)
         self._logsnr_first = -20.0
@@ -360,23 +385,31 @@ class Sampler:
     def _run(self, steps: int, noise: bool, static: bool, set_view=None) -> None:
         """The sampling loop from loop position 0: per step set_view(k) (if given), the forward, the table step and pos += 1.
         Step 0 runs eagerly, so every kernel has run once before a graph is captured.  static: poses, K, cond_mask and
-        params stay fixed, so after step 0 the forwards reuse its rays, pose embeddings and weight shadows."""
+        params stay fixed, so after step 0 the forwards reuse its rays, pose embeddings and weight shadows.  Steps the
+        feature-cache schedule marks cheap run at cache_level (`feature_cache_full_steps`)."""
         h = self.eng.h
         self._pos.zero_()
+        full = feature_cache_full_steps(steps, self.cache_interval)
+        level = 0
         try:
             self.lib.xunet_set_static_conditioning(h, 0)
             for k in range(steps):
                 if set_view is not None:
                     set_view(k)
+                want = 0 if full[k] else self.cache_level
+                if want != level:
+                    level = want
+                    _lib.check(self.lib.xunet_set_feature_cache(h, level), 'set_feature_cache')
                 if k > 0 and self.use_graph:
-                    self._graph(static, noise).replay()
+                    self._graph(static, noise, level > 0).replay()
                 else:
                     self._step(noise)
                 if static and k == 0:
                     self.lib.xunet_set_static_conditioning(h, 1)
         finally:
-            # a failure mid-loop must not leave the shared engine reusing stale pose embeddings / weight shadows
+            # a failure mid-loop must not leave the shared engine reusing stale pose embeddings / weight shadows, or cheap
             self.lib.xunet_set_static_conditioning(h, 0)
+            self.lib.xunet_set_feature_cache(h, 0)
 
     def _step(self, noise: bool) -> None:
         e = self.eng
@@ -404,9 +437,9 @@ class Sampler:
             _lib.check(self.lib.xunet_sampler_step_multistep(*head, self._x0_hist.data_ptr(), *tail), 'sampler_step_multistep')
         self._pos.add_(1)
 
-    def _graph(self, static: bool, noise: bool) -> torch.cuda.CUDAGraph:
-        """The captured step; static conditioning and explicit noise both change what it launches."""
-        key = (static, noise)
+    def _graph(self, static: bool, noise: bool, cheap: bool) -> torch.cuda.CUDAGraph:
+        """The captured step; static conditioning, explicit noise and a cheap forward each change what it launches."""
+        key = (static, noise, cheap)
         if key not in self._graphs:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, stream=torch.cuda.Stream(device=self.dev)):
@@ -427,8 +460,9 @@ class Sampler:
         the same posterior update as `sample()` (w=None: one B-batch conditional forward).  The pool lives on the device; a step only copies the chosen view and
         its pose into the engine's input buffers before the step, which runs with the full forward (static conditioning
         off).  z_init (m, B,S,S,3) / noises (m, steps, B,S,S,3) make a run reproducible against the oracle; with one
-        source, one target and the same seed the result equals `sample()`.
-        Returns (B, m, S, S, 3) [and the (m, steps) pool indices that were drawn]."""
+        source, one target and the same seed the result equals `sample()`.  With a feature cache (cache_interval > 1) a view
+        is drawn on full steps only: a cheap step keeps the view of the last full step, which its cached deep feature saw.
+        Returns (B, m, S, S, 3) [and the (m, steps) pool indices in use at each step]."""
         B, e = self.B, self.eng
         dev = self.dev
         f32 = lambda a: torch.as_tensor(np.asarray(a), dtype=torch.float32).to(dev)
@@ -440,6 +474,7 @@ class Sampler:
         Kd = f32(K)
         rng = np.random.RandomState(seed)
         steps = self._load_schedule()
+        full = feature_cache_full_steps(steps, self.cache_interval)
         cp = self.copies
         e.inp['K'].copy_(torch.cat([Kd] * cp, 0).reshape(e.inp['K'].shape))
         e.inp['cond_mask'].copy_(torch.cat([torch.ones(B, device=dev), torch.zeros((cp - 1) * B, device=dev)]))
@@ -451,6 +486,9 @@ class Sampler:
             row = []
 
             def set_view(k):
+                if not full[k]:
+                    row.append(row[-1])
+                    return
                 c = int(rng.randint(len(pool_x)))
                 row.append(c)
                 e.inp['x'].copy_(torch.cat([pool_x[c]] * cp, 0).reshape(e.inp['x'].shape))
