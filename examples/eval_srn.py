@@ -12,6 +12,8 @@ instance is conditioned on one source view (view 64 by default) and every scored
     python examples/eval_srn.py cars_test --ckpt checkpoints_d6 --prefix ema --side 128 --steps 256 --distilled 6 --out eval_d6/
     python examples/eval_srn.py cars_test --ckpt checkpoints_cd --prefix ema --side 128 --consistency 4 --out eval_cd4/
     python examples/eval_srn.py cars_test --ckpt checkpoints --prefix ema --side 128 --steps 256 --cache-interval 3 --out eval_dc3/
+    python examples/eval_srn.py cars_test --ckpt checkpoints --prefix phema010 --guide-prefix guide005 --w 1 --side 128 \
+        --method dpmpp_2m --steps 25 --out eval_ag/
 
 Modes:
   independent  each target is sampled from the source alone (Sampler.sample, the reference's k = 1 sampler); the targets
@@ -37,6 +39,7 @@ from novel_view_synthesis_3d_b200.srn_data import SRNScenes
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from distill_srn import cd_steps  # noqa: E402
+from sample_srn import add_guide_args, load_guide  # noqa: E402
 
 
 def select_targets(n_views: int, source: int, count: int) -> list:
@@ -85,6 +88,7 @@ def main():
                          '(1: every forward full, the default)')
     ap.add_argument('--cache-level', type=int, default=1, metavar='L',
                     help='feature-cache level in [1, levels - 1]: the cheap forwards recompute the levels below L')
+    add_guide_args(ap)
     ap.add_argument('--source-view', type=int, default=64, help='conditioning view of every instance (pixelNeRF / 3DiM: 64)')
     ap.add_argument('--targets', type=int, default=0, help='target views per instance, spaced evenly; 0 = all other views')
     ap.add_argument('--max-instances', type=int, default=-1, help='score the first N instances of the sorted list')
@@ -96,6 +100,7 @@ def main():
     a = ap.parse_args()
     if a.views_in_flight < 1:
         ap.error('--views-in-flight must be >= 1')
+    guide = load_guide(ap, a)
     params = P.checkpoint.restore_checkpoint(a.ckpt, prefix=a.prefix)
     if params is None:
         raise FileNotFoundError('Checkpoint does not exist')
@@ -118,7 +123,7 @@ def main():
     else:
         sampler = P.Sampler(P.XUNet(), params, B, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta,
                             spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction,
-                            **cache)
+                            guide_params=guide, **cache)
     os.makedirs(a.out, exist_ok=True)
     if a.save_views:
         os.makedirs(os.path.join(a.out, 'views'), exist_ok=True)

@@ -8,6 +8,9 @@ ancestral sampler, write PNGs (the reference blocks in cv2.imshow, which cannot 
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_d1 --prefix ema --distilled 1 --steps 256 --out results_d1/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints_cd --prefix ema --consistency 2 --out results_cd2/
     python examples/sample_srn.py cars_train_val --ckpt checkpoints --method dpmpp_2m --steps 25 --cache-interval 3 --out results_dc3/
+    python examples/posthoc_ema_srn.py --ckpt checkpoints --sigma-rel 0.05 --step 100000 --prefix guide005
+    python examples/sample_srn.py cars_train_val --ckpt checkpoints --prefix phema010 --guide-prefix guide005 --w 1 \
+        --method dpmpp_2m --steps 25 --out results_ag/
 """
 import argparse
 import os
@@ -21,6 +24,30 @@ from novel_view_synthesis_3d_b200.srn_data import SRNScenes
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from distill_srn import cd_steps  # noqa: E402
+
+
+def add_guide_args(ap) -> None:
+    ap.add_argument('--guide-ckpt', default=None, metavar='DIR',
+                    help='directory of the autoguidance checkpoint (default: --ckpt)')
+    ap.add_argument('--guide-prefix', default=None, metavar='P',
+                    help='autoguidance (Karras et al. 2024): guide with this weaker checkpoint of the same model, for '
+                         'example a post-hoc EMA at a short sigma_rel and an early step (examples/posthoc_ema_srn.py), in '
+                         'place of the pose-dropped branch; --w then weights (1 + w) out - w out_guide')
+
+
+def load_guide(ap, a):
+    """The guide's parameter tree (None without --guide-prefix); argparse errors for a combination that has no guidance."""
+    if a.guide_prefix is None:
+        if a.guide_ckpt is not None:
+            ap.error('--guide-ckpt needs --guide-prefix')
+        return None
+    if a.distilled or a.consistency:
+        ap.error('--guide-prefix guides the classifier-free-guided sampler; --distilled and --consistency sample without '
+                 'guidance')
+    guide = P.checkpoint.restore_checkpoint(a.guide_ckpt or a.ckpt, prefix=a.guide_prefix)
+    if guide is None:
+        raise FileNotFoundError(f'Guide checkpoint {a.guide_prefix} does not exist in {a.guide_ckpt or a.ckpt}')
+    return guide
 
 
 def main():
@@ -54,6 +81,7 @@ def main():
                          '(1: every forward full, the default)')
     ap.add_argument('--cache-level', type=int, default=1, metavar='L',
                     help='feature-cache level in [1, levels - 1]: the cheap forwards recompute the levels below L')
+    add_guide_args(ap)
     ap.add_argument('--views', type=int, default=1)
     ap.add_argument('--side', type=int, default=64)
     ap.add_argument('--out', default='results')
@@ -61,6 +89,7 @@ def main():
                     help='3DiM stochastic conditioning: generate this many further views autoregressively (the poses of the '
                          'next pairs drawn from the loader), each denoising step conditioned on a random view of the pool')
     a = ap.parse_args()
+    guide = load_guide(ap, a)
     params = P.checkpoint.restore_checkpoint(a.ckpt, prefix=a.prefix)
     if params is None:
         raise FileNotFoundError('Checkpoint does not exist')                                          # sampling.py:111-112
@@ -78,7 +107,7 @@ def main():
     else:
         sampler = P.Sampler(model, params, a.views, a.side, steps=a.steps, w=a.w, method=a.method, eta=a.eta,
                             spacing=a.spacing, dynamic_threshold=a.dynamic_threshold, prediction=a.prediction,
-                            **cache)
+                            guide_params=guide, **cache)
     os.makedirs(a.out, exist_ok=True)
     if a.orbit > 0:
         it = ds.batches(a.views)

@@ -382,6 +382,24 @@ int xunet_sampler_step_cond(const float* out, float* z, const float* noise, long
                             const unsigned long long* seed_dev, float* x0_hist, int batch, double percentile, float* scale_out,
                             float* next_z, float* next_logsnr, void* stream);
 
+/* The AUTOGUIDED sampler step (Karras et al. 2024, "Guiding a diffusion model with a bad version of itself"): the negative
+ * of the guidance is the output of a weaker guide model on the same inputs, not the pose-dropped branch of a 2B batch.
+ * out_main and out_guide (device, n = B*S*S*3 floats each) are the B-batch outputs of the main and the guide forward, both
+ * with cond_mask 1; the step uses
+ *     out = (1+w) out_main - w out_guide
+ * with the same fp32 operations, in the same order, as the guided steps' (1+w) out_c - w out_u, and is otherwise
+ * xunet_sampler_step_cond's:
+ *   percentile == 0, x0_hist == NULL: xunet_sampler_step_table;   percentile == 0, x0_hist != NULL: xunet_sampler_step_multistep;
+ *   percentile in (0, 1]: xunet_sampler_step_dynamic (x0_hist NULL or set as there), scale_out optional as there.
+ * The new z goes to z and to next_z (n floats: the main forward's z input, which the guide forward reads too), and the row's
+ * log-SNR to next_logsnr (batch floats).  With w = 0, or with out_guide equal to out_main and w = 1, the result is the bits
+ * of xunet_sampler_step_cond on out_main.
+ * Errors: a NULL required pointer, n <= 0, batch < 1, n % batch != 0; with percentile != 0 also per > XUNET_SAMPLER_DYN_MAX_PER
+ * or percentile NaN or outside (0, 1].  One launch; graph-capturable. */
+int xunet_sampler_step_guide(const float* out_main, const float* out_guide, float* z, const float* noise, long long n, float w,
+                             const float* table, const int* pos_dev, const unsigned long long* seed_dev, float* x0_hist,
+                             int batch, double percentile, float* scale_out, float* next_z, float* next_logsnr, void* stream);
+
 /* Device-side forward diffusion = the per-item work of SceneInstanceDataset.__getitem__ (dataset/data_loader.py:92-110):
  *   t ~ U{0..999};  noise ~ N(0,1);  z = sqrt_ac[t] * x0 + sqrt_1mac[t] * noise;  logsnr = logsnr_schedule_cosine(t/1000);
  *   cond_mask = (u > p_uncond)  (train.py:64).

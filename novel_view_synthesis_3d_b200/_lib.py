@@ -137,6 +137,8 @@ SYMBOLS = {
     'xunet_cd_target': (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
     'xunet_sampler_step_cond': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong] + [C.c_void_p] * 4 +
                                 [C.c_int, C.c_double] + [C.c_void_p] * 4),
+    'xunet_sampler_step_guide': (C.c_int, [C.c_void_p] * 4 + [C.c_longlong, C.c_float] + [C.c_void_p] * 4 +
+                                 [C.c_int, C.c_double] + [C.c_void_p] * 4),
     'xunet_dropout_mask': (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_ulonglong, C.c_float, C.c_void_p]),
     'xunet_image_metrics': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),

@@ -1,5 +1,5 @@
 // sampler.cu -- one sampler step with the schedule on the device, and the C entries that launch it
-// (xunet_sampler_step_table, _multistep, _dynamic and _cond): sampler_step_table_kernel clips x0 to [-1, 1],
+// (xunet_sampler_step_table, _multistep, _dynamic, _cond and _guide): sampler_step_table_kernel clips x0 to [-1, 1],
 // sampler_step_dynamic_kernel thresholds it per view (dynamic thresholding, Saharia et al. 2022, Imagen section 2.3).
 //
 // The dynamic step is sampler_step_table_kernel's with the fixed clip of x0 to [-1, 1] replaced by a per-view one:
@@ -40,22 +40,30 @@ namespace cg = cooperative_groups;
 // single-step kernel).  HIST = true (multistep solvers, DPM-Solver++(2M)) fixes the order, one rounding per fma:
 //   z' = fma(sigma, noise, fma(c_prev, x0_hist[i], fma(c_x0, x0, c_z * z))), the c_prev term skipped when c_prev == 0,
 // then x0_hist[i] = x0.  A row with c_prev == 0 never reads x0_hist (the first step needs no initialised history).
-// GUIDED = true: eps2 is the [cond ; uncond] output of a 2B batch and the new z goes to both halves of inp_z.  GUIDED = false
-// (a model whose guidance is in its weights, e.g. a distilled student): eps2 is the B-batch conditional output, read as is,
-// and the new z goes to inp_z's n values.
-template <bool HIST, bool GUIDED>
+// NEG selects where the guidance's negative output comes from:
+//   NEG_HALF (classifier-free guidance): eps2 is the [cond ; uncond] output of a 2B batch, the negative is eps2[n + i], and the
+//            new z goes to both halves of inp_z;
+//   NEG_NONE (a model whose guidance is in its weights, e.g. a distilled student): eps2 is the B-batch conditional output, read
+//            as is, and the new z goes to inp_z's n values;
+//   NEG_PTR  (autoguidance): eps2 is the B-batch output of the main model, the negative is neg[i], the B-batch output of a
+//            second (guide) model on the same inputs, and the new z goes to inp_z's n values.
+// NEG_HALF and NEG_PTR combine the two outputs with the same fp32 operations (xu_step_guided); neg is read only by NEG_PTR.
+enum SamplerNeg { NEG_NONE = 0, NEG_HALF = 1, NEG_PTR = 2 };
+
+template <bool HIST, int NEG>
 __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __restrict__ eps2, float* __restrict__ z,
                                                                  const float* __restrict__ noise, long long n, float w,
                                                                  const float* __restrict__ tab, const int* __restrict__ pos_dev,
                                                                  const unsigned long long* __restrict__ seed_dev, float* __restrict__ inp_z,
-                                                                 float* __restrict__ inp_logsnr, int B2, float* __restrict__ x0_hist) {
+                                                                 float* __restrict__ inp_logsnr, int B2, float* __restrict__ x0_hist,
+                                                                 const float* __restrict__ neg) {
   xu_grid_dep_sync();
   const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
   const int k = *pos_dev;
   const float* t = tab + 8LL * k;
   if (i < B2) inp_logsnr[i] = t[5];
   if (i >= n) return;
-  const float e = GUIDED ? xu_step_guided(w, eps2[i], eps2[n + i]) : eps2[i];
+  const float e = NEG == NEG_NONE ? eps2[i] : xu_step_guided(w, eps2[i], NEG == NEG_HALF ? eps2[n + i] : neg[i]);
   const float zi = z[i];
   const float x0 = xu_step_x0(t, zi, e);
   const float nz = noise != nullptr ? noise[k * n + i] : xu_hash_normal(*seed_dev - (unsigned long long)k, (uint64_t)i);
@@ -71,15 +79,20 @@ __global__ void __launch_bounds__(256) sampler_step_table_kernel(const float* __
   }
   z[i] = zn;
   inp_z[i] = zn;
-  if constexpr (GUIDED) inp_z[n + i] = zn;
+  if constexpr (NEG == NEG_HALF) inp_z[n + i] = zn;
 }
 static void launch_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                       const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
-                                      int B2, float* x0_hist, bool guided, cudaStream_t s) {
+                                      int B2, float* x0_hist, int neg_mode, const float* neg, cudaStream_t s) {
   const int grid = cdiv(n > B2 ? n : B2, 256);
-  auto kernel = x0_hist != nullptr ? (guided ? sampler_step_table_kernel<true, true> : sampler_step_table_kernel<true, false>)
-                                   : (guided ? sampler_step_table_kernel<false, true> : sampler_step_table_kernel<false, false>);
-  xu_launch(kernel, grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr, B2, x0_hist);
+  static void (*const kernels[2][3])(const float*, float*, const float*, long long, float, const float*, const int*,
+                                     const unsigned long long*, float*, float*, int, float*, const float*) = {
+      {sampler_step_table_kernel<false, NEG_NONE>, sampler_step_table_kernel<false, NEG_HALF>,
+       sampler_step_table_kernel<false, NEG_PTR>},
+      {sampler_step_table_kernel<true, NEG_NONE>, sampler_step_table_kernel<true, NEG_HALF>,
+       sampler_step_table_kernel<true, NEG_PTR>}};
+  xu_launch(kernels[x0_hist != nullptr][neg_mode], grid, 256, 0, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z,
+            inp_logsnr, B2, x0_hist, neg);
 }
 
 #define DYN_CLUSTER 8
@@ -95,15 +108,15 @@ __device__ __forceinline__ float dyn_threshold_scale(float lo_v, float hi_v, dou
   return fmaxf(__double2float_rn(q), 1.f);
 }
 
-// GUIDED = false: the unguided step of sampler_step_table_kernel<.., false> (eps2 the B-batch conditional output, read as is;
-// the new z goes to inp_z's n values only)
-template <bool HIST, bool GUIDED>
+// NEG as in sampler_step_table_kernel: NEG_HALF reads the negative from eps2[n + i] and writes both halves of inp_z, NEG_NONE
+// reads eps2 as is, NEG_PTR reads the negative from neg[i]; the last two write inp_z's n values only
+template <bool HIST, int NEG>
 __global__ void __cluster_dims__(DYN_CLUSTER, 1, 1) __launch_bounds__(DYN_THREADS)
 sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ z, const float* __restrict__ noise, long long n,
                             float w, const float* __restrict__ tab, const int* __restrict__ pos_dev,
                             const unsigned long long* __restrict__ seed_dev, float* __restrict__ inp_z,
                             float* __restrict__ inp_logsnr, int B2, float* __restrict__ x0_hist, int per, double p,
-                            float* __restrict__ scale_out) {
+                            float* __restrict__ scale_out, const float* __restrict__ neg) {
   extern __shared__ float xs[];                 // the guided, unclipped x0 of this CTA's slice
   __shared__ unsigned hist[2][DYN_THREADS];     // digit counts of this CTA's candidates, double-buffered across passes
   __shared__ unsigned wsum[DYN_THREADS / 32];
@@ -126,7 +139,7 @@ sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ 
   const float c_recip = t[0], c_recipm1 = t[1], wp1 = __fadd_rn(1.f, w);
   for (int j = tid; j < len; j += DYN_THREADS) {
     const long long i = base + j;
-    const float e = GUIDED ? fmaf(wp1, eps2[i], -__fmul_rn(w, eps2[n + i])) : eps2[i];
+    const float e = NEG == NEG_NONE ? eps2[i] : fmaf(wp1, eps2[i], -__fmul_rn(w, NEG == NEG_HALF ? eps2[n + i] : neg[i]));
     xs[j] = fmaf(c_recip, z[i], -__fmul_rn(c_recipm1, e));
   }
   hist[0][tid] = 0u;
@@ -221,7 +234,7 @@ sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ 
     zn = fmaf(t[4], nz, zn);
     z[i] = zn;
     inp_z[i] = zn;
-    if constexpr (GUIDED) inp_z[n + i] = zn;
+    if constexpr (NEG == NEG_HALF) inp_z[n + i] = zn;
   }
   cluster.barrier_wait(std::move(arrived));
 }
@@ -229,29 +242,35 @@ sampler_step_dynamic_kernel(const float* __restrict__ eps2, float* __restrict__ 
 // n / B <= XUNET_SAMPLER_DYN_MAX_PER values per view (the entries check it)
 static void launch_sampler_step_dynamic(const float* eps2, float* z, const float* noise, long long n, float w, const float* tab,
                                         const int* pos_dev, const unsigned long long* seed_dev, float* inp_z, float* inp_logsnr,
-                                        int B2, float* x0_hist, int B, double p, float* scale_out, bool guided, cudaStream_t s) {
+                                        int B2, float* x0_hist, int B, double p, float* scale_out, int neg_mode,
+                                        const float* neg, cudaStream_t s) {
+  static void (*const kernels[2][3])(const float*, float*, const float*, long long, float, const float*, const int*,
+                                     const unsigned long long*, float*, float*, int, float*, int, double, float*,
+                                     const float*) = {
+      {sampler_step_dynamic_kernel<false, NEG_NONE>, sampler_step_dynamic_kernel<false, NEG_HALF>,
+       sampler_step_dynamic_kernel<false, NEG_PTR>},
+      {sampler_step_dynamic_kernel<true, NEG_NONE>, sampler_step_dynamic_kernel<true, NEG_HALF>,
+       sampler_step_dynamic_kernel<true, NEG_PTR>}};
   static bool configured = false;
   if (!configured) {
-    for (auto kernel : {sampler_step_dynamic_kernel<false, true>, sampler_step_dynamic_kernel<true, true>,
-                        sampler_step_dynamic_kernel<false, false>, sampler_step_dynamic_kernel<true, false>})
-      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * kDynMaxChunk));
+    for (auto& row : kernels)
+      for (auto kernel : row)
+        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * kDynMaxChunk));
     configured = true;
   }
   const int per = (int)(n / B);
   const size_t smem = sizeof(float) * (size_t)((per + DYN_CLUSTER - 1) / DYN_CLUSTER);
   const dim3 grid((unsigned)B * DYN_CLUSTER);
-  auto kernel = x0_hist != nullptr ? (guided ? sampler_step_dynamic_kernel<true, true> : sampler_step_dynamic_kernel<true, false>)
-                                   : (guided ? sampler_step_dynamic_kernel<false, true> : sampler_step_dynamic_kernel<false, false>);
-  xu_launch(kernel, grid, DYN_THREADS, smem, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev, inp_z, inp_logsnr, B2, x0_hist,
-            per, p, scale_out);
+  xu_launch(kernels[x0_hist != nullptr][neg_mode], grid, DYN_THREADS, smem, s, eps2, z, noise, n, w, tab, pos_dev, seed_dev,
+            inp_z, inp_logsnr, B2, x0_hist, per, p, scale_out, neg);
 }
 
 extern "C" int xunet_sampler_step_table(const float* eps2, float* z, const float* noise, long long n, float w, const float* table,
                                         const int* pos_dev, const unsigned long long* seed_dev, float* next_z2, float* next_logsnr2,
                                         int batch2, void* stream) {
   if (!eps2 || !z || !table || !pos_dev || !seed_dev || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0) return xu_fail("xunet_sampler_step_table: bad argument");
-  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, nullptr, true,
-                            (cudaStream_t)stream);
+  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, nullptr, NEG_HALF,
+                            nullptr, (cudaStream_t)stream);
   return xu_launched("sampler_step_table");
 }
 
@@ -260,8 +279,8 @@ extern "C" int xunet_sampler_step_multistep(const float* eps2, float* z, const f
                                             float* x0_hist, float* next_z2, float* next_logsnr2, int batch2, void* stream) {
   if (!eps2 || !z || !table || !pos_dev || !seed_dev || !x0_hist || !next_z2 || !next_logsnr2 || n <= 0 || batch2 <= 0)
     return xu_fail("xunet_sampler_step_multistep: bad argument");
-  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, true,
-                            (cudaStream_t)stream);
+  launch_sampler_step_table(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, NEG_HALF,
+                            nullptr, (cudaStream_t)stream);
   return xu_launched("sampler_step_multistep");
 }
 
@@ -280,7 +299,7 @@ extern "C" int xunet_sampler_step_dynamic(const float* eps2, float* z, const flo
   if (!(percentile > 0.0 && percentile <= 1.0))
     return xu_fail("xunet_sampler_step_dynamic: percentile %g outside (0, 1]", percentile);
   launch_sampler_step_dynamic(eps2, z, noise, n, w, table, pos_dev, seed_dev, next_z2, next_logsnr2, batch2, x0_hist, batch,
-                              percentile, scale_out, true, (cudaStream_t)stream);
+                              percentile, scale_out, NEG_HALF, nullptr, (cudaStream_t)stream);
   return xu_launched("sampler_step_dynamic");
 }
 
@@ -298,10 +317,33 @@ extern "C" int xunet_sampler_step_cond(const float* out, float* z, const float* 
     if (!(percentile > 0.0 && percentile <= 1.0))
       return xu_fail("xunet_sampler_step_cond: percentile %g outside (0, 1] (0 selects the fixed clip)", percentile);
     launch_sampler_step_dynamic(out, z, noise, n, 0.f, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, batch,
-                                percentile, scale_out, false, (cudaStream_t)stream);
+                                percentile, scale_out, NEG_NONE, nullptr, (cudaStream_t)stream);
   } else {
-    launch_sampler_step_table(out, z, noise, n, 0.f, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, false,
-                              (cudaStream_t)stream);
+    launch_sampler_step_table(out, z, noise, n, 0.f, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, NEG_NONE,
+                              nullptr, (cudaStream_t)stream);
   }
   return xu_launched("sampler_step_cond");
+}
+
+extern "C" int xunet_sampler_step_guide(const float* out_main, const float* out_guide, float* z, const float* noise, long long n,
+                                        float w, const float* table, const int* pos_dev, const unsigned long long* seed_dev,
+                                        float* x0_hist, int batch, double percentile, float* scale_out, float* next_z,
+                                        float* next_logsnr, void* stream) {
+  if (!out_main || !out_guide || !z || !table || !pos_dev || !seed_dev || !next_z || !next_logsnr)
+    return xu_fail("xunet_sampler_step_guide: NULL pointer argument");
+  if (n <= 0 || batch < 1) return xu_fail("xunet_sampler_step_guide: n = %lld, batch = %d, need both >= 1", n, batch);
+  if (n % batch != 0) return xu_fail("xunet_sampler_step_guide: n = %lld is not a multiple of batch = %d", n, batch);
+  if (percentile != 0.0) {
+    if (n / batch > XUNET_SAMPLER_DYN_MAX_PER)
+      return xu_fail("xunet_sampler_step_guide: %lld values per view, more than XUNET_SAMPLER_DYN_MAX_PER = %d", n / batch,
+                     XUNET_SAMPLER_DYN_MAX_PER);
+    if (!(percentile > 0.0 && percentile <= 1.0))
+      return xu_fail("xunet_sampler_step_guide: percentile %g outside (0, 1] (0 selects the fixed clip)", percentile);
+    launch_sampler_step_dynamic(out_main, z, noise, n, w, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, batch,
+                                percentile, scale_out, NEG_PTR, out_guide, (cudaStream_t)stream);
+  } else {
+    launch_sampler_step_table(out_main, z, noise, n, w, table, pos_dev, seed_dev, next_z, next_logsnr, batch, x0_hist, NEG_PTR,
+                              out_guide, (cudaStream_t)stream);
+  }
+  return xu_launched("sampler_step_guide");
 }

@@ -18,6 +18,11 @@ w=None samples a model whose guidance is in its weights, such as a progressively
 B-batch conditional forward per step, stepped by `xunet_sampler_step_cond`.  `distill_grid` gives the timesteps such a
 student was trained on, and `Schedule(timesteps=...)` the schedule of any such grid.
 
+guide_params samples with autoguidance (Karras et al. 2024): the negative of the guidance is a weaker version of the same
+model (fewer training steps, a shorter EMA, a narrower config) under the same conditioning, instead of the pose-dropped
+branch.  Each step is a B-batch forward of the main model, a B-batch forward of the guide on the same device inputs, and
+`xunet_sampler_step_guide`: (1 + w) out_main - w out_guide.
+
 method='consistency' samples a consistency-distilled student (distill.ConsistencyTeacher) by multistep consistency sampling
 (Song et al. 2023, Alg. 1): x0 = clip(f(z, t_k)), then z' = alpha' x0 + sigma' eps' with fresh noise, landing on x0 after
 the last step.  `consistency_grid` gives its timesteps.
@@ -30,7 +35,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .xunet import XUNet, BATCH_KEYS
+from .xunet import XUNet, BATCH_KEYS, Engine, ParamTree, pack_flat
 
 
 def cosine_beta_schedule(timesteps, s=0.008):
@@ -292,15 +297,39 @@ class Sampler:
     conditioning, the input conv, the blocks of the levels below L and the head, and reads the deep feature (the output of
     the up-resampler leaving level L) from the last full forward, with that step's log-SNR and inputs.  It works with every
     method, guidance and sample_views; its effect on sample quality (PSNR / SSIM on SRN) at N > 1 has not been measured.
-    N = 1 (the default) runs every forward in full and gives the bits of a sampler built without these arguments."""
+    N = 1 (the default) runs every forward in full and gives the bits of a sampler built without these arguments.
+
+    guide_params, guide_model: autoguidance (Karras et al. 2024, "Guiding a diffusion model with a bad version of itself").
+    guide_params is the parameter tree of a weaker guide: for example the same run's post-hoc EMA reconstructed at a short
+    sigma_rel and an early snapshot (`posthoc.reconstruct`, examples/posthoc_ema_srn.py).  guide_model (an XUNet or an
+    XUNetConfig; default: `model`'s config) is its architecture: any config at the same image side, a narrower `ch` for
+    instance.  The guide must have been trained with the same `prediction` as the model.  It needs a float w: the main
+    engine then holds B rows, all with cond_mask 1 (the w=None layout, the same `model.engine(B, S, False)`), and a second
+    engine of the guide config, owned by this sampler, runs the guide's B-batch forward on the main engine's device inputs
+    (z, log-SNR, view, poses, cond_mask), so sample_views and the feature cache work unchanged.  A step is the two forwards
+    and `xunet_sampler_step_guide`, which forms (1 + w) out_main - w out_guide with the fp32 operations of the guided step:
+    w means what it means for classifier-free guidance (Karras' guidance weight is 1 + w).  Every method,
+    prediction, dynamic thresholding, explicit timesteps, sample_views and the feature cache (cache_level must exist in
+    both configs) work with a guide.  w = 0 gives the bits of w=None on the main params, and so does a guide equal to the
+    model at w = 1.  Two B-row forwards replace the one 2B-row forward of guidance (tools/autoguide_cost.py measures
+    both)."""
 
     def __init__(self, model: XUNet, params, batch_size: int, img_sidelength: int, *, steps: int = 1000,
                  w: float | None = 3.0, use_graph: bool = True, method: str = 'ddpm', eta: float = 0.0,
                  spacing: str | None = None, logsnr_lag: bool | None = None, dynamic_threshold: float | None = None,
-                 prediction: str = 'eps', timesteps=None, cache_interval: int = 1, cache_level: int = 1):
+                 prediction: str = 'eps', timesteps=None, cache_interval: int = 1, cache_level: int = 1,
+                 guide_params=None, guide_model=None):
         _check_method(method, eta)
         _check_dynamic_threshold(dynamic_threshold)
         _check_feature_cache(cache_interval, cache_level, len(model.config.ch_mult))
+        if guide_params is None and guide_model is not None:
+            raise ValueError('guide_model is given without guide_params')
+        if guide_params is not None and w is None:
+            raise ValueError('guide_params needs a float guidance weight w; w=None samples without guidance')
+        guide_cfg = None
+        if guide_params is not None:
+            guide_cfg = model.config if guide_model is None else getattr(guide_model, 'config', guide_model)
+            _check_feature_cache(cache_interval, cache_level, len(guide_cfg.ch_mult))
         self.cache_interval, self.cache_level = int(cache_interval), int(cache_level)
         self.prediction = check_prediction(prediction)
         self.dynamic_threshold = None if dynamic_threshold is None else float(dynamic_threshold)
@@ -308,13 +337,17 @@ class Sampler:
         self.logsnr_lag = (method == 'ddpm' and prediction == 'eps') if logsnr_lag is None else bool(logsnr_lag)
         self.model, self.B, self.S = model, batch_size, img_sidelength
         self.w = None if w is None else float(w)
-        self.copies = 1 if w is None else 2       # engine rows per view: [cond] or [cond ; uncond]
+        self.copies = 1 if w is None or guide_params is not None else 2    # engine rows per view: [cond] or [cond ; uncond]
         self.sched = Schedule(steps, spacing=('logsnr' if method == 'dpmpp_2m' else 'linear') if spacing is None else spacing,
                               timesteps=timesteps)
         self.eng = model.engine(self.copies * batch_size, img_sidelength, False)
         self.flat = model.flat_from_tree(params, img_sidelength, self.copies * batch_size)
         self.lib = _lib.load()
         self.dev = self.eng.device
+        # the guide's own engine: model.engine() would hand back the main engine for a same-config guide, and the two
+        # forwards would share one workspace and one output
+        self.guide_eng = None if guide_cfg is None else Engine(guide_cfg, batch_size, img_sidelength, False, self.dev)
+        self.guide_flat = None if guide_cfg is None else self._guide_flat(guide_params)
         self.z = torch.zeros(batch_size, img_sidelength, img_sidelength, 3, dtype=torch.float32, device=self.dev)
         self.use_graph = use_graph
         self._tab = None            # (steps, 8) coefficient table on the device
@@ -326,6 +359,18 @@ class Sampler:
         # dpmpp_2m: the previous step's clipped x0.  Allocated once, since the captured graphs hold its pointer; a chain's
         # first row has c_prev = 0 and overwrites it, so every chain starts with a fresh history.
         self._x0_hist = torch.empty_like(self.z) if method == 'dpmpp_2m' else None
+
+    def _guide_flat(self, params) -> torch.Tensor:
+        """The guide's flat parameter buffer, laid out by the guide engine's spec; ValueError when the tree does not match."""
+        g = self.guide_eng
+        if isinstance(params, ParamTree) and params.flat is not None:
+            if params.spec is not None and dict(params.spec) != dict(g.spec) or params.flat.numel() != g.nparams:
+                raise ValueError(f'guide_params does not match the guide config {g.cfg}')
+            return params.flat
+        try:
+            return pack_flat(params, g.spec, g.nparams).to(self.dev)
+        except KeyError as err:
+            raise ValueError(f'guide_params does not match the guide config {g.cfg}: {err}') from err
 
     def capture(self, batch: dict) -> None:
         """Runs the first 3 steps of a sample: builds the static-conditioning state and, with use_graph, the per-step CUDA
@@ -386,36 +431,52 @@ class Sampler:
         """The sampling loop from loop position 0: per step set_view(k) (if given), the forward, the table step and pos += 1.
         Step 0 runs eagerly, so every kernel has run once before a graph is captured.  static: poses, K, cond_mask and
         params stay fixed, so after step 0 the forwards reuse its rays, pose embeddings and weight shadows.  Steps the
-        feature-cache schedule marks cheap run at cache_level (`feature_cache_full_steps`)."""
-        h = self.eng.h
+        feature-cache schedule marks cheap run at cache_level (`feature_cache_full_steps`).  Both settings apply to the
+        guide engine too."""
+        hs = [self.eng.h] + ([] if self.guide_eng is None else [self.guide_eng.h])
         self._pos.zero_()
         full = feature_cache_full_steps(steps, self.cache_interval)
         level = 0
         try:
-            self.lib.xunet_set_static_conditioning(h, 0)
+            for h in hs:
+                self.lib.xunet_set_static_conditioning(h, 0)
             for k in range(steps):
                 if set_view is not None:
                     set_view(k)
                 want = 0 if full[k] else self.cache_level
                 if want != level:
                     level = want
-                    _lib.check(self.lib.xunet_set_feature_cache(h, level), 'set_feature_cache')
+                    for h in hs:
+                        _lib.check(self.lib.xunet_set_feature_cache(h, level), 'set_feature_cache')
                 if k > 0 and self.use_graph:
                     self._graph(static, noise, level > 0).replay()
                 else:
                     self._step(noise)
                 if static and k == 0:
-                    self.lib.xunet_set_static_conditioning(h, 1)
+                    for h in hs:
+                        self.lib.xunet_set_static_conditioning(h, 1)
         finally:
             # a failure mid-loop must not leave the shared engine reusing stale pose embeddings / weight shadows, or cheap
-            self.lib.xunet_set_static_conditioning(h, 0)
-            self.lib.xunet_set_feature_cache(h, 0)
+            for h in hs:
+                self.lib.xunet_set_static_conditioning(h, 0)
+                self.lib.xunet_set_feature_cache(h, 0)
 
     def _step(self, noise: bool) -> None:
         e = self.eng
         e.forward(self.flat, train=False)
         st = torch.cuda.current_stream(self.dev).cuda_stream
         hist = None if self._x0_hist is None else self._x0_hist.data_ptr()
+        if self.guide_eng is not None:
+            g = self.guide_eng
+            g.forward(self.guide_flat, train=False, batch=e.cbatch)        # the main engine's z, log-SNR, view and poses
+            _lib.check(self.lib.xunet_sampler_step_guide(e.eps.data_ptr(), g.eps.data_ptr(), self.z.data_ptr(),
+                                                         self._noise.data_ptr() if noise else None, self.z.numel(), self.w,
+                                                         self._tab.data_ptr(), self._pos.data_ptr(), self._seed_base.data_ptr(),
+                                                         hist, self.B, self.dynamic_threshold or 0.0, None,
+                                                         e.inp['z'].data_ptr(), e.inp['logsnr'].data_ptr(), st),
+                       'sampler_step_guide')
+            self._pos.add_(1)
+            return
         if self.w is None:
             _lib.check(self.lib.xunet_sampler_step_cond(e.eps.data_ptr(), self.z.data_ptr(),
                                                         self._noise.data_ptr() if noise else None, self.z.numel(),
@@ -457,7 +518,8 @@ class Sampler:
         For each of the m target poses in turn the chain starts from noise and, at EVERY denoising step, conditions on
         one view drawn uniformly from the pool (the k sources plus -- if condition_on_generated -- the targets generated
         so far), exactly as the paper's sampler; one 2B-batch forward per step ([cond ; uncond], guidance weight w) and
-        the same posterior update as `sample()` (w=None: one B-batch conditional forward).  The pool lives on the device; a step only copies the chosen view and
+        the same posterior update as `sample()` (w=None: one B-batch conditional forward; with a guide: the main and the
+        guide B-batch forwards, the guide reading the main engine's inputs).  The pool lives on the device; a step only copies the chosen view and
         its pose into the engine's input buffers before the step, which runs with the full forward (static conditioning
         off).  z_init (m, B,S,S,3) / noises (m, steps, B,S,S,3) make a run reproducible against the oracle; with one
         source, one target and the same seed the result equals `sample()`.  With a feature cache (cache_interval > 1) a view
